@@ -1,7 +1,8 @@
 #!/usr/bin/env python
-"""bench.py - openWakeWord's streaming hot path on B200, measured on BASELINE.json's configs.
+"""bench.py - openWakeWord's streaming hot path on H100, measured on BASELINE.json's configs.
 
   python bench.py [--gpus N] [--steps K] [--warmup W]        # own arm (CUDA, libowwb200)
+  python bench.py ... --dump-outputs DIR                     # + the scores of the last timed step as DIR/<workload>_scores.npy
   python bench.py --impl reference [...]                    # reference arm (CPU, host cores)
   torchrun --nproc-per-node N ... bench.py --gpus N ...      # one rank per GPU, weak scaling
 
@@ -19,8 +20,8 @@ heads (+ one score gather when N > 1).  Prints ONE JSON line (rank 0).
   parity     after the timed regions the SAME engine (same kernels, group size, mode) is reset and driven for 12 steps;
              16 sampled streams (first / last ragged group included) are compared with the NumPy oracle: max |delta|,
              asserted <= 1e-3
-  roofline   the step's dominant kernel (tc_inc_kernel): executed and reference-algorithmic FLOP/s against both
-             measured bf16 peaks (MEASURED_PEAKS.json)
+  roofline   the step's dominant kernel (tc_inc_kernel): executed and reference-algorithmic FLOP/s against the dense
+             bf16 peak (MEASURED_PEAKS.json when present, else the H100 SXM data-sheet figure)
   cpu_baseline / --impl reference : the NumPy oracle (a port - onnxruntime and the .onnx files do not exist in this
              image) driven as the reference is: one single-stream model per process, one process per usable host core,
              predict() per 80 ms frame, same head set.
@@ -177,7 +178,7 @@ def _cpu_worker(conn, stream_id, seed, workload):
         # in this image - SURVEY.md F2 - but the arm upgrades itself when the assets exist)
         try:
             import glob
-            for extra in (os.path.join(ROOT, "baseline", "_ref"), "/root/reference"):
+            for extra in (os.path.join(ROOT, "baseline", "_ref"),):
                 if os.path.isdir(extra) and extra not in sys.path:
                     sys.path.insert(0, extra)
             import openwakeword
@@ -343,7 +344,7 @@ def measure(args, wl, rank, world, local, dev, sampler_windows, do_model=True):
     n_total = B * world
     K, Wm = args.steps, max(args.warmup, 3)
     heads = bench_heads(wl)
-    pool_bytes = 168e6                                           # distinct PCM cycled through: larger than the 126 MB L2
+    pool_bytes = 168e6                                           # distinct PCM cycled through: larger than the 50 MB L2
     POOL = max(4, int(np.ceil(pool_bytes / (B * CHUNK * 2))))
 
     def factory(n_local, lo, hi):
@@ -373,13 +374,18 @@ def measure(args, wl, rank, world, local, dev, sampler_windows, do_model=True):
     barrier()
     t_a = time.perf_counter()
     e0.record()
+    last = None
     for k in range(K):
-        sh.step(dev_steps[(Wm + k) % POOL], 1)
+        last = sh.step(dev_steps[(Wm + k) % POOL], 1)
     sh.flush()
     e1.record()
     barrier()
     sampler_windows.append((t_a, time.perf_counter()))
     ms_dev = e0.elapsed_time(e1)
+    # scores of the last timed step (what a caller of sh.step receives), kept for --dump-outputs
+    last_scores = None
+    if last is not None:
+        last_scores = (last.wait() if hasattr(last, "wait") else last).float().cpu().numpy()
     stage = eng.ctx.stage_ms()
     eng.ctx.enable_stage_timing(0)
     launches = eng.ctx.launch_count - l0
@@ -402,7 +408,7 @@ def measure(args, wl, rank, world, local, dev, sampler_windows, do_model=True):
     ms_e2e = 1e3 * (t1 - t0)
     out = {"B": B, "ms_dev": ms_dev, "ms_e2e": ms_e2e, "cnn_ms": stage["cnn"], "heads_ms": stage["heads"], "mel_ms": stage["mel"],
            "launches": int(launches), "n_cols": eng.n_cols, "heads": len(heads), "G": None, "gather": sh.gather_kind,
-           "h2d": B * CHUNK * 2, "d2h": B * eng.n_cols * 4}
+           "h2d": B * CHUNK * 2, "d2h": B * eng.n_cols * 4, "last_scores": last_scores}
     # ---- parity of the configuration that was just timed (rank 0, checker only) ----
     if rank == 0:
         out["parity"] = parity_check(eng, heads, B)
@@ -466,8 +472,8 @@ def run_own_arm(args):
     import torch
     import torch.distributed as dist
     from openwakeword_b200 import distributed as owd
-    import __graft_entry__ as g
-    g.build()
+    from openwakeword_b200 import _native
+    _native.load_library()                      # built by __graft_entry__.build(); nothing is compiled or written here
     from oracle.probe import parity_label      # labelling only (which oracle the 1e-3 gate was checked against)
 
     rank, world, local = owd.init_process_group("nccl" if int(os.environ.get("WORLD_SIZE", "1")) > 1 else None)
@@ -494,6 +500,11 @@ def run_own_arm(args):
             v = measure_variant(args, args.workload, local, dev, sf, windows)
             variants.append(v)
     clocks = sampler.stop(windows) if rank == 0 else None
+    if args.dump_outputs and rank == 0:
+        os.makedirs(args.dump_outputs, exist_ok=True)
+        for wl in order:
+            if res[wl]["last_scores"] is not None:
+                np.save(os.path.join(args.dump_outputs, f"{wl}_scores.npy"), np.ascontiguousarray(res[wl]["last_scores"], np.float32))
 
     keys = ["ms_dev", "ms_e2e", "cnn_ms", "heads_ms", "mel_ms"]
     flat = [res[wl][k] for wl in order for k in keys]
@@ -515,10 +526,10 @@ def run_own_arm(args):
         peaks = json.load(open(os.path.join(ROOT, "MEASURED_PEAKS.json")))
     except Exception:
         pass
-    pk_sus = peaks.get("bf16_tflops_sustained", 1400.0)
-    pk_burst = peaks.get("bf16_tflops", 1590.0)
+    pk_sus = peaks.get("bf16_tflops_sustained", 989.0)
+    pk_burst = peaks.get("bf16_tflops", 989.0)
     peak_src = ("MEASURED_PEAKS.json bf16_tflops_sustained / bf16_tflops (of measured)" if peaks
-                else "fallback 1.4 / 1.59 PFLOP/s (of fallback)")
+                else "NVIDIA H100 SXM data sheet, dense BF16 at 700 W: 989 TFLOP/s (not a measured peak)")
     main = res[args.workload]
     B = main["B"]
     n_total = B * world
@@ -530,7 +541,7 @@ def run_own_arm(args):
     peak_used = pk_burst if timed_s < 1.0 else pk_sus         # burst figure for a short region at full clocks, sustained for a long one
     fused = args.cnn_mode == 3 and not args.no_fuse
     sf = args.split_from or 11
-    kernel_name = ((f"tc_inc_kernel<{sf}> (cnn_tc_inc.cu): log-mel frontend + conv layers 0..{sf - 1} of every stream on tcgen05 in ONE persistent launch"
+    kernel_name = ((f"tc_inc_kernel<{sf}> (cnn_tc_inc.cu): log-mel frontend + conv layers 0..{sf - 1} of every stream on wgmma in ONE persistent launch"
                     + (f"; layers {sf}..19 follow as tc_conv_blk_kernel launches on fp16 hi/lo split operands (3 MMA terms), then heads_grp_kernel"
                        if sf < 20 else " + ring append" + (" + heads" if main["heads_ms"] == 0.0 else "; heads_grp_kernel follows")))
                    if fused else "embedding CNN stage (separate launches)")
@@ -588,9 +599,8 @@ def run_own_arm(args):
                              "per frame: 11.2 MFLOP with one MMA term per K step, 16.4 MFLOP with the default three-term split operands "
                              "from layer 11 on; SURVEY.md F10/8d); achieved/frac = reference-algorithmic 83.9 MFLOP per frame delivered per "
                              "second.  kernel_ms is the CNN stage (frontend + conv layers + ring append), CUDA events inside the timed region. "
-                             "Why the fraction is low by construction: N = Cout is 24..96 and an M128 x N x K16 tcgen05.mma costs ~60-75 cycles "
-                             "for every N <= 128 (scripts/micro/mma_layout.cu, profiles/r2_mma_layout.txt) - at N = 96 the pipe's ceiling is "
-                             "~40 % of its N = 256 rate, and layers 0-2 (N = 24) ~10 %; ncu summaries of the same command: profiles/"},
+                             "The fraction is low by construction: N = Cout is only 24..96 per layer and the fused kernel issues 64 x 32 "
+                             "wgmma tiles."},
         "cpu_baseline": cpu,
     }
     if "ms_model" in main:
@@ -621,7 +631,7 @@ def main():
     ap.add_argument("--impl", default="own", choices=["own", "reference"])
     ap.add_argument("--workload", default="c3", choices=sorted(WORKLOADS), help="c3 = configs[2] (headline), c2 = configs[1]")
     ap.add_argument("--no-secondary", dest="secondary", action="store_false", help="skip the configs[1] measurement")
-    ap.add_argument("--cnn-mode", type=int, default=3, help="0 fp32 window, 2 tcgen05 window, 3 tcgen05 fused incremental")
+    ap.add_argument("--cnn-mode", type=int, default=3, help="0 fp32 window, 2 tensor-core window, 3 tensor-core fused incremental")
     ap.add_argument("--no-cpu-baseline", action="store_true")
     ap.add_argument("--gather", default="nccl-overlap", choices=["nccl", "nccl-overlap", "peer"],
                     help="N>1: per-step score gather: NCCL all-gather on the compute stream, NCCL all-gather on a side stream "
@@ -634,6 +644,9 @@ def main():
     ap.add_argument("--split-from", type=int, default=0,
                     help="first conv layer on fp16 hi/lo split operands (11 = default, scores within ~2e-4 of the fp32 graph; "
                          "20 = plain fp16 everywhere and the whole step as one fused launch, ~9e-4)")
+    ap.add_argument("--dump-outputs", default=None, metavar="DIR",
+                    help="after the timed steps, write the scores of the last timed step of every measured workload as "
+                         "DIR/<workload>_scores.npy (float32 [streams, score columns]; seeded inputs, identical from run to run)")
     args = ap.parse_args()
     if args.impl == "reference":
         return run_reference_arm(args)

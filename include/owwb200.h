@@ -1,9 +1,9 @@
 /*
- * owwb200.h - C ABI of libowwb200.so: the B200 (sm_100a) replacement for the three
+ * owwb200.h - C ABI of libowwb200.so: the H100 (sm_90a) replacement for the three
  * inference sessions on openWakeWord's streaming hot path, plus the device-resident
  * stream state that sits between them.
  *
- * What each entry point replaces in the reference (paths under /root/reference/):
+ * What each entry point replaces in the reference (paths in the original openWakeWord project):
  *   oww_melspectrogram   -> AudioFeatures.melspec_model_predict   openwakeword/utils.py:84-87,202
  *                           (melspectrogram.onnx; graph spec notebooks/converting_google_speech_embedding_model.ipynb:426-477)
  *   oww_embed_windows    -> AudioFeatures.embedding_model_predict openwakeword/utils.py:90-93,235,443
@@ -53,10 +53,10 @@ extern "C" {
 
 /* embedding-CNN execution modes */
 #define OWW_CNN_FP32_WINDOW       0  /* CUDA-core fp32, full 76-row window per frame (reference-shaped)  */
-#define OWW_CNN_TC_WINDOW         2  /* tcgen05 fp16-operand/fp32-accumulate implicit GEMM, full window  */
-#define OWW_CNN_TC_INCREMENTAL    3  /* tcgen05, fused 20-layer kernel on the 8 new mel rows per stream
+#define OWW_CNN_TC_WINDOW         2  /* wgmma fp16-operand/fp32-accumulate implicit GEMM, full window    */
+#define OWW_CNN_TC_INCREMENTAL    3  /* wgmma, fused 20-layer kernel on the 8 new mel rows per stream
                                         (per-stream activation tails in HBM); first step after a reset and
-                                        the stateless/batch calls use the full-window tcgen05 kernels      */
+                                        the stateless/batch calls use the full-window wgmma kernels        */
 
 typedef struct oww_ctx oww_ctx;
 
@@ -194,14 +194,14 @@ int oww_debug_inc_plan(oww_ctx* ctx, int group, int n_streams, int32_t* out, int
 
 /* cnn_mode 3 only, instrumentation: oww_debug_inc_clocks arms a clock buffer; the next step then records clock64()
  * stamps taken by CTA 0 on its first group; oww_debug_inc_clocks_read synchronises and returns 104 values:
- * [0..19] start of each layer phase, [20] end of layer 19, per layer l [21+l] cycles the MMA warp waited for weights,
- * [41+l] its MMA issue time, [61+l] phase start -> first accumulator ready, [81+l] phase start -> last tile stored,
- * [101] group start (before the fused frontend), [102] end of the fused heads phase (0 when the step was not fused). */
+ * [0..19] start of each layer phase, [20] end of layer 19, per layer l [61+l] phase start -> first accumulator ready,
+ * [81+l] phase start -> last tile stored, [92..97] frontend phases of warp 0, [101] group start (before the fused
+ * frontend), [102] end of the fused heads phase (0 when the step was not fused); other entries stay 0. */
 int oww_debug_inc_clocks(oww_ctx* ctx, int64_t* h_unused);
 int oww_debug_inc_clocks_read(oww_ctx* ctx, int64_t* h_out104);
-/* Instrumentation of the grouped heads kernel (heads_grp.cu): the first call arms the stamps, later calls synchronise and
- * return 8 clock64() values per head group (tile 0's CTA): start, producer done, last first-layer MMA issued,
- * first-layer accumulators complete, team 0 done, CTA end, 0, 0. */
+/* Instrumentation of the mirror-path heads kernel (heads_grp.cu): the first call arms the stamps, later calls synchronise
+ * and return 8 clock64() values per head (CTA 0 of its launch): [0] start, [1] producer done, [2] first-layer
+ * accumulators complete, [4] scores stored; the other entries stay 0. */
 int oww_debug_heads_clocks(oww_ctx* ctx, int64_t* h_out64);
 
 /* ---- multi-GPU gather over peer memory (one process per GPU) ---------------------------------
@@ -211,7 +211,7 @@ int oww_debug_heads_clocks(oww_ctx* ctx, int64_t* h_out64);
  * with oww_peer_copy - one DMA over NVLink; d_scores of oww_step may also point into the mapping directly, at the
  * price of scattered 4-byte remote stores - then publishes a step counter with oww_peer_signal; the gathering rank
  * orders its consumer behind oww_peer_wait.  openwakeword_b200.distributed.PeerGather drives the protocol
- * (double-buffered slots, acknowledgement counters); validated on 2 x B200 by tests/test_gpu_multi.py.
+ * (double-buffered slots, acknowledgement counters); checked by tests/test_gpu_multi.py on two GPUs.
  *   oww_peer_alloc  - cudaMalloc'd, zero-filled buffer on this handle's device + its 64-byte CUDA IPC handle
  *   oww_peer_open   - map another process's buffer (peer access is enabled lazily); oww_peer_close unmaps it
  *   oww_peer_signal - stream-ordered: after all earlier work of `stream`, *d_flag = value (system-scope release;

@@ -1,6 +1,6 @@
-"""openwakeword_b200 - B200-native drop-in for openWakeWord's streaming inference hot path.
+"""openwakeword_b200 - CUDA-native (H100, sm_90a) drop-in for openWakeWord's streaming inference hot path.
 
-Mirrors the public names of /root/reference/openwakeword/__init__.py for the path in scope
+Mirrors the public names of openwakeword/__init__.py for the path in scope
 (SURVEY.md section 8): ``Model``, ``MODELS``, ``FEATURE_MODELS``, ``model_class_mappings``,
 ``get_pretrained_model_paths``; ``utils.AudioFeatures`` and ``utils.bulk_predict``.
 Importing the package needs neither a GPU nor the built library; constructing a ``Model`` /

@@ -1,7 +1,7 @@
 """ctypes binding of libowwb200.so (the C ABI in include/owwb200.h).
 
-The library is built in-tree by ``__graft_entry__.build()`` (nvcc, sm_100a).  There is no CPU
-fallback: if the shared object is missing, or no B200-class GPU is present, constructing a
+The library is built in-tree by ``__graft_entry__.build()`` (nvcc, sm_90a).  There is no CPU
+fallback: if the shared object is missing, or no H100-class (sm_90) GPU is present, constructing a
 ``Context`` raises - the product path never routes through the NumPy oracle.
 """
 import ctypes as C
@@ -90,7 +90,7 @@ def load_library():
     if not os.path.exists(LIB_PATH):
         raise ImportError(
             f"{LIB_PATH} is missing: the CUDA extension has not been built. Run "
-            "`python -c 'import __graft_entry__ as g; g.build()'` at the repo root (nvcc, sm_100a). "
+            "`python -c 'import __graft_entry__ as g; g.build()'` at the repo root (nvcc, sm_90a). "
             "There is no CPU fallback for the b200 backend.")
     lib = C.CDLL(LIB_PATH)
     for name, (res, args) in _SIGNATURES.items():

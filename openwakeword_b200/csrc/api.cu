@@ -104,7 +104,7 @@ __global__ void gather_chunk_kernel(const int16_t* pcm, int n_clips, int n_sampl
 
 }  // namespace
 // Tails of the all-ones window per tails-bearing tensor, in the compact G = 1 layout, computed once per weight set by
-// the full-window tcgen05 kernels (cnn_tc.cu) - the state every freshly reset stream starts from (its mel history IS
+// the full-window tensor-core kernels (cnn_tc.cu) - the state every freshly reset stream starts from (its mel history IS
 // ones(76,32), utils.py:165, and a constant history is shift invariant, so no per-stream re-priming pass is needed).
 int oww_inc_build_template(oww_ctx* ctx);
 namespace {
@@ -299,7 +299,7 @@ int reset_enqueue(oww_ctx* ctx, const int32_t* h_stream_ids, int n, const float*
 
 extern "C" {
 
-const char* oww_version(void) { return "owwb200 0.1 (sm_100a)"; }
+const char* oww_version(void) { return "owwb200 0.1 (sm_90a)"; }
 
 const char* oww_last_error(const oww_ctx* ctx) { return ctx ? ctx->err.c_str() : g_create_error.c_str(); }
 
@@ -327,8 +327,8 @@ int oww_create(const oww_config* cfg, oww_ctx** out) {
     cudaDeviceProp prop;
     cudaGetDeviceProperties(&prop, ctx->device);
     ctx->sm_count = prop.multiProcessorCount;
-    if (prop.major != 10) {
-        oww_fail(nullptr, OWW_EUNSUPPORTED, "device is sm_%d%d; this library is built for sm_100a only", prop.major, prop.minor);
+    if (prop.major != 9 || prop.minor != 0) {
+        oww_fail(nullptr, OWW_EUNSUPPORTED, "device is sm_%d%d; this library is built for sm_90a only", prop.major, prop.minor);
         delete ctx; return OWW_EUNSUPPORTED;
     }
     ctx->tc_heads = (cfg->reserved[0] & 2) == 0;
@@ -686,7 +686,7 @@ int oww_embed_clips(oww_ctx* ctx, const int16_t* d_pcm, int n_clips, int n_sampl
     cudaStream_t s = (cudaStream_t)stream;
     if (ctx->cfg.cnn_mode != OWW_CNN_FP32_WINDOW) {
         // tensor-core modes: per-clip mel (one call per clip, as the reference's CPU path runs the graph), then ONE fully
-        // convolutional tcgen05 pass over the clip's [T x 32] mel (SURVEY.md F10) - slabs bounded by a ~1 GB plane scratch
+        // convolutional tensor-core pass over the clip's [T x 32] mel (SURVEY.md F10) - slabs bounded by a ~1 GB plane scratch
         const int t_use = OWW_WINDOW_ROWS + 8 * (W - 1);
         const size_t per1 = oww_tc_act_units_T(ctx, 1, t_use);
         int slab = (int)std::max<size_t>(1, ((size_t)1 << 26) / per1);          // 2^26 units = 1 GiB per buffer
@@ -735,7 +735,7 @@ int oww_predict_clips(oww_ctx* ctx, const int16_t* d_pcm, int n_clips, int n_sam
     {
         // ---- bulk path (SURVEY.md F10): per slab of clips ONE mel launch over the padded clips (frames grouped and
         //      clamped per streaming call, behind the 71 rows of ones a fresh stream's window starts with), ONE fully
-        //      convolutional tcgen05 pass per conv layer over [76 + 8 (steps-1)] x 32, then the heads over all sliding
+        //      convolutional tensor-core pass per conv layer over [76 + 8 (steps-1)] x 32, then the heads over all sliding
         //      windows of [feature_init rows | embeddings] in one launch.  Bit-identical to streaming the clips.
         bool tc_all = ctx->cfg.cnn_mode != OWW_CNN_FP32_WINDOW && steps <= 8192 && !ctx->heads.empty();
         for (size_t i = 0; i < ctx->heads.size(); ++i) tc_all = tc_all && oww_heads_tc_supported(ctx, (int)i);

@@ -1,7 +1,7 @@
 // K2 (fp32 CUDA-core path): the speech-embedding CNN as 20 implicit-GEMM convolutions.
 //
 // Replaces the embedding_model.onnx session of the reference
-// (/root/reference/openwakeword/utils.py:90-93,235,443; graph spec
+// (openwakeword/utils.py:90-93,235,443; graph spec
 // notebooks/converting_google_speech_embedding_model.ipynb:871-951, shapes :521-859; SURVEY.md
 // Appendix B): 3x3 conv on the 76x32 mel window, then alternating (1,3) "same" / (3,1) "valid"
 // dense convs, folded BatchNorm + max(0.2x,x) + max(x,-0.4) after every conv but the last,

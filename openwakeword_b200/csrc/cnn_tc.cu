@@ -1,23 +1,23 @@
-// K2 (tensor-core path): the speech-embedding CNN as tcgen05 implicit GEMMs for sm_100a.
+// K2 (tensor-core path): the speech-embedding CNN as warpgroup-MMA (wgmma) implicit GEMMs for sm_90a.
 //
-// Same graph as cnn_fp32.cu (reference: embedding_model.onnx, /root/reference/openwakeword/utils.py:90-93;
+// Same graph as cnn_fp32.cu (reference: embedding_model.onnx, openwakeword/utils.py:90-93 of the original project;
 // spec notebooks/converting_google_speech_embedding_model.ipynb:871-951).  Layers 1..19 are dense
 // (1,3)/(3,1) convolutions: M = output positions, N = Cout, K = 3 taps x Cin.
 //
 // Layout.  Activations live in HBM/L2 as fp16 "channel-group planes": plane g holds channels
 // 8g..8g+7 of every position as one 16-byte unit, positions ordered (window, t, f) with ONE zero pad
-// column per row (f = W), i.e. exactly the canonical no-swizzle K-major UMMA core-matrix order
-// (8 consecutive positions x 16 B = one 8x8 core matrix, SBO = 128 B, LBO = plane pitch).  Hence
+// column per row (f = W), i.e. exactly the canonical no-swizzle K-major core-matrix order of a wgmma
+// operand (8 consecutive positions x 16 B = one 8x8 core matrix, SBO = 128 B, LBO = plane pitch).  Hence
 //   * an A tile (128 positions + halo, all planes) is CG contiguous runs -> CG 1-D bulk copies
 //     (cp.async.bulk, mbarrier complete_tx), no im2col, no tensor map;
 //   * a conv tap is just a 16-byte-granular shift of the A descriptor's start address:
 //     (1,3) taps shift by -1/0/+1 positions (the pad column supplies the "same" zeros),
 //     (3,1) taps shift by 0/Wp/2Wp positions; one smem tile feeds all three taps.
 // Weights are pre-packed per layer as fp16 [tap][plane][n][8] (same core-matrix order, K-major B).
-// D accumulates in TMEM (fp32, 128 lanes x N columns, two stages); the epilogue warps read their
-// lane quarter with tcgen05.ld, apply folded BN + leaky + clamp in fp32 and write the next layer's
-// fp16 planes directly (16-byte coalesced stores).  Warp roles: 0 = bulk-copy producer,
-// 1 = TMEM allocator + single-thread MMA issuer, 2..5 = epilogue.  Persistent CTAs, grid = #SMs.
+// Two MMA warpgroups each own 64 of a tile's 128 positions: D accumulates in their registers (fp32), and the same
+// threads apply folded BN + leaky + clamp in fp32 and write the next layer's fp16 planes (each thread holds two
+// adjacent channels of two positions: 4-byte stores, 128 contiguous bytes per warp and plane).  Warp 0 = bulk-copy
+// producer.  Persistent CTAs, grid = #SMs.
 #include "oww_internal.h"
 #include "tc_common.cuh"
 #include <cmath>
@@ -98,7 +98,7 @@ __global__ void __launch_bounds__(256) tc_conv0_kernel(Tc0Args a) {
     }
 }
 
-// ---------------------------------------------------------------- tcgen05 conv layer
+// ---------------------------------------------------------------- tensor-core conv layer
 struct TcConvArgs {
     const __half* in; int64_t in_plane;     // units (16 B) per input plane, guard included
     __half* out; int64_t out_plane;
@@ -128,6 +128,9 @@ struct TcConvArgs {
 // [cg_in, 2 cg_in), the weights hi and lo blocks of W * 2^s (2^-s folded into `scale`), and every K step issues
 // hi*hi + lo*hi + hi*lo into the same fp32 accumulator: the product is fp32-grade (~2^-21), at 3x the MMAs, 2x the
 // operand bytes and half the pipeline stages.
+// Warp roles: warp 0 lane 0 = bulk-copy producer (warps 1-3 only take part in the set-up); warpgroups 1 and 2 each own
+// 64 of the tile's 128 positions: they issue the tile's MMAs (wgmma, accumulators in registers), release the stage and
+// run the epilogue from the register fragment.
 template <int CGP, int NP, int TERMS>
 __global__ void __launch_bounds__(kTcThreads, 1) tc_conv_kernel(TcConvArgs a) {
     extern __shared__ __align__(128) uint8_t smem[];
@@ -140,22 +143,18 @@ __global__ void __launch_bounds__(kTcThreads, 1) tc_conv_kernel(TcConvArgs a) {
     const int stage_bytes = kSplit * term_bytes;
     uint8_t* a_smem = smem + W_BYTES;
     uint64_t* bars = reinterpret_cast<uint64_t*>(a_smem + kStages * stage_bytes);
-    // bars: [0..S) full, [S..2S) empty, [2S..2S+A) tmem_full, [..+A) tmem_empty, then w_full
-    uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(bars + 2 * kStages + 2 * kAccStages + 1);
-    float* s_sb = reinterpret_cast<float*>(tmem_slot + 4);                 // folded BN scale[NP] | bias[NP], read by every epilogue thread
+    // bars: [0..S) full, [S..2S) empty, then w_full
+    float* s_sb = reinterpret_cast<float*>(bars + 2 * kStages + 2);          // folded BN scale[NP] | bias[NP]
     for (int i = threadIdx.x; i < NP; i += kTcThreads) { s_sb[i] = a.scale[i]; s_sb[NP + i] = a.bias[i]; }
 
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
     const uint32_t bar0 = smem_u32(bars);
     auto full_bar = [&](int s) { return bar0 + 8u * s; };
     auto empty_bar = [&](int s) { return bar0 + 8u * (kStages + s); };
-    auto tfull_bar = [&](int s) { return bar0 + 8u * (2 * kStages + s); };
-    auto tempty_bar = [&](int s) { return bar0 + 8u * (2 * kStages + kAccStages + s); };
-    const uint32_t wfull_bar = bar0 + 8u * (2 * kStages + 2 * kAccStages);
+    const uint32_t wfull_bar = bar0 + 8u * (2 * kStages);
 
     if (threadIdx.x == 0) {
-        for (int s = 0; s < kStages; ++s) { mbar_init(full_bar(s), 1); mbar_init(empty_bar(s), 1); }
-        for (int s = 0; s < kAccStages; ++s) { mbar_init(tfull_bar(s), 1); mbar_init(tempty_bar(s), 8); }   // 8 epilogue warps
+        for (int s = 0; s < kStages; ++s) { mbar_init(full_bar(s), 1); mbar_init(empty_bar(s), 8); }   // one arrival per MMA warp
         mbar_init(wfull_bar, 1);
         asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
     }
@@ -167,14 +166,7 @@ __global__ void __launch_bounds__(kTcThreads, 1) tc_conv_kernel(TcConvArgs a) {
         }
     }
     asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
-    if (warp == 1) {
-        asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(tmem_slot)), "r"(256));
-        asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;");
-    }
-    tc_fence_before();
     __syncthreads();
-    tc_fence_after();
-    const uint32_t tmem_base = *tmem_slot;
 
     if (warp == 0) {
         // ===================== producer: weights once, then one A tile per stage =====================
@@ -194,45 +186,47 @@ __global__ void __launch_bounds__(kTcThreads, 1) tc_conv_kernel(TcConvArgs a) {
                 if (++stage == kStages) { stage = 0; phase ^= 1; }
             }
         }
-    } else if (warp == 1) {
-        // ===================== MMA issuer (one elected lane; the warp stays converged) =====================
-        {
-            const uint32_t idesc = (1u << 4) | ((uint32_t)(NP >> 3) << 17) | ((uint32_t)(128 >> 4) << 24);
-            tc_warp_wait(wfull_bar, 0, lane);
-            int stage = 0; uint32_t phase = 0; int acc = 0; uint32_t acc_phase = 0;
-            const uint32_t w_addr = smem_u32(w_smem);
-            const uint32_t lbo_a = (uint32_t)a.rows * 16u;
-            const uint32_t rows16 = (uint32_t)a.rows * 16u;
-            const uint32_t tap16[3] = {(uint32_t)a.tap_off[0] * 16u, (uint32_t)a.tap_off[1] * 16u, (uint32_t)a.tap_off[2] * 16u};
-            for (int tile = blockIdx.x; tile < a.n_tiles; tile += gridDim.x) {
-                tc_warp_wait(tempty_bar(acc), acc_phase ^ 1, lane);
-                tc_warp_wait(full_bar(stage), phase, lane);
-                tc_fence_after();
-                const uint32_t a_addr = smem_u32(a_smem + stage * stage_bytes);
-                const uint32_t d_tmem = tmem_base + (uint32_t)acc * 128u;
-                if (tc_elect_one()) {
-                    uint32_t accumulate = 0;
-                    if (TERMS == 1 && (a.cg_in & 1)) {
-                        // odd plane count, plain operands: the K octets of the three taps are chained exactly as in the fused
-                        // step kernel (cnn_tc_inc.cu: the last plane of tap 0 shares an MMA with the first plane of tap 1),
-                        // with the weights packed in that order - one MMA per tile less, and the same accumulation order
-                        // as the streaming path (bulk == streaming, bit for bit)
-                        constexpr int CG = CGP - 1, NPAIR = CG / 2;
-                        uint32_t b = w_addr;
-                        constexpr uint32_t np2 = 2u * NP * 16u;
-                        auto mma = [&](uint32_t a_at, uint32_t lbo) {
-                            tc_mma_f16(d_tmem, make_desc(a_at, lbo, 128u), make_desc(b, NP * 16u, 128u), idesc, accumulate);
-                            accumulate = 1; b += np2;
-                        };
+    } else if (warp >= 4) {
+        // ===================== MMA + epilogue: warpgroup wg owns accumulator rows [64 wg, 64 wg + 64) =====================
+        const int wg = (warp >> 2) - 1, wq = warp & 3, q = lane & 3;
+        const uint32_t row_off = (uint32_t)wg * 64u * 16u;                 // 8 core-matrix rows of 128 B per 8 positions
+        tc_warp_wait(wfull_bar, 0, lane);
+        int stage = 0; uint32_t phase = 0;
+        const uint32_t w_addr = smem_u32(w_smem);
+        const uint32_t lbo_a = (uint32_t)a.rows * 16u;
+        const uint32_t rows16 = (uint32_t)a.rows * 16u;
+        const uint32_t tap16[3] = {(uint32_t)a.tap_off[0] * 16u, (uint32_t)a.tap_off[1] * 16u, (uint32_t)a.tap_off[2] * 16u};
+        const int Wp = a.W + 1;
+        const int per_in = a.T * Wp;
+        const int per_out = a.T_out * Wp;
+        for (int tile = blockIdx.x; tile < a.n_tiles; tile += gridDim.x) {
+            tc_warp_wait(full_bar(stage), phase, lane);
+            float acc[NP / 2];
+            const uint32_t a_addr = smem_u32(a_smem + stage * stage_bytes) + row_off;
+            wg_fence();
+            {
+                uint32_t accumulate = 0;
+                if (TERMS == 1 && (a.cg_in & 1)) {
+                    // odd plane count, plain operands: the K octets of the three taps are chained exactly as in the fused
+                    // step kernel (cnn_tc_inc.cu: the last plane of tap 0 shares an MMA with the first plane of tap 1),
+                    // with the weights packed in that order - one MMA per tile less, and the same accumulation order
+                    // as the streaming path (bulk == streaming, bit for bit)
+                    constexpr int CG = CGP - 1, NPAIR = CG / 2;
+                    uint32_t b = w_addr;
+                    constexpr uint32_t np2 = 2u * NP * 16u;
+                    auto mma = [&](uint32_t a_at, uint32_t lbo) {
+                        wg_mma<NP>(acc, make_desc(a_at, lbo, 128u), make_desc(b, NP * 16u, 128u), accumulate);
+                        accumulate = 1; b += np2;
+                    };
 #pragma unroll
-                        for (int k = 0; k < NPAIR; ++k) mma(a_addr + tap16[0] + (uint32_t)(2 * k) * rows16, lbo_a);
-                        mma(a_addr + tap16[1], (uint32_t)CG * rows16 - rows16 + tap16[0] - tap16[1]);
+                    for (int k = 0; k < NPAIR; ++k) mma(a_addr + tap16[0] + (uint32_t)(2 * k) * rows16, lbo_a);
+                    mma(a_addr + tap16[1], (uint32_t)CG * rows16 - rows16 + tap16[0] - tap16[1]);
 #pragma unroll
-                        for (int k = 0; k < NPAIR; ++k) mma(a_addr + tap16[1] + (uint32_t)(2 * k + 1) * rows16, lbo_a);
+                    for (int k = 0; k < NPAIR; ++k) mma(a_addr + tap16[1] + (uint32_t)(2 * k + 1) * rows16, lbo_a);
 #pragma unroll
-                        for (int k = 0; k < NPAIR; ++k) mma(a_addr + tap16[2] + (uint32_t)(2 * k) * rows16, lbo_a);
-                        mma(a_addr + tap16[2] + (uint32_t)(CG - 1) * rows16, 0u);
-                    } else {
+                    for (int k = 0; k < NPAIR; ++k) mma(a_addr + tap16[2] + (uint32_t)(2 * k) * rows16, lbo_a);
+                    mma(a_addr + tap16[2] + (uint32_t)(CG - 1) * rows16, 0u);
+                } else {
                     // term order: every K step with the hi activations ((hi,hi), (hi,lo)), then every K step with the lo
                     // activations ((lo,hi)) - the order tc_conv_blk_kernel is bound to (it holds one half at a time), so the
                     // window / clip passes and the incremental late layers accumulate identically (bulk == streaming, bit for bit)
@@ -241,121 +235,84 @@ __global__ void __launch_bounds__(kTcThreads, 1) tc_conv_kernel(TcConvArgs a) {
 #pragma unroll
                         for (int j = 0; j < 3; ++j) {
 #pragma unroll
-                            for (int q = 0; q < CGP / 2; ++q) {
+                            for (int qq = 0; qq < CGP / 2; ++qq) {
 #pragma unroll
                                 for (int wt = 0; wt < (TERMS == 3 && ph == 0 ? 2 : 1); ++wt) {
                                     const uint32_t a_t = a_addr + (ph == 1 ? (uint32_t)term_bytes : 0u);
                                     const uint32_t w_t = w_addr + (wt == 1 ? (uint32_t)W_TERM : 0u);
-                                    const uint64_t ad = make_desc(a_t + (uint32_t)(2 * q) * rows16 + tap16[j], lbo_a, 128u);
-                                    const uint64_t bd = make_desc(w_t + (uint32_t)((j * CGP + 2 * q) * NP) * 16u, NP * 16u, 128u);
-                                    tc_mma_f16(d_tmem, ad, bd, idesc, accumulate);
+                                    const uint64_t ad = make_desc(a_t + (uint32_t)(2 * qq) * rows16 + tap16[j], lbo_a, 128u);
+                                    const uint64_t bd = make_desc(w_t + (uint32_t)((j * CGP + 2 * qq) * NP) * 16u, NP * 16u, 128u);
+                                    wg_mma<NP>(acc, ad, bd, accumulate);
                                     accumulate = 1;
                                 }
                             }
                         }
                     }
-                    }
-                    tc_commit(empty_bar(stage));
-                    tc_commit(tfull_bar(acc));
                 }
-                __syncwarp();
-                if (++stage == kStages) { stage = 0; phase ^= 1; }
-                if (++acc == kAccStages) { acc = 0; acc_phase ^= 1; }
             }
-        }
-    } else {
-        // ===================== epilogue: 8 warps = 4 TMEM lane quarters x 2 halves of the channel-group planes ============
-        const int quarter = warp & 3, half = (warp - 2) >> 2;
-        constexpr int NP8 = NP / 8, PH = NP8 / 2;              // planes per half (NP8 is even for every instance)
-        const int pl0 = half * PH;
-        const int row = quarter * 32 + lane;
-        const int Wp = a.W + 1;
-        const int per_in = a.T * Wp;
-        const int per_out = a.T_out * Wp;
-        int acc = 0; uint32_t acc_phase = 0;
-        for (int tile = blockIdx.x; tile < a.n_tiles; tile += gridDim.x) {
-            mbar_wait(tfull_bar(acc), acc_phase);
-            tc_fence_after();
-            uint32_t v[PH * 8];
-            const uint32_t taddr = tmem_base + ((uint32_t)(quarter * 32) << 16) + (uint32_t)acc * 128u + (uint32_t)pl0 * 8u;
-#pragma unroll
-            for (int k = 0; k < PH; ++k) tc_tmem_ld8(taddr + k * 8, v + k * 8);
-            tmem_wait_ld();
-            tc_fence_before();
+            wg_commit();
+            wg_wait_all();
             __syncwarp();
-            if (lane == 0) mbar_arrive(tempty_bar(acc));
-            if (++acc == kAccStages) { acc = 0; acc_phase ^= 1; }
+            if (lane == 0) mbar_arrive(empty_bar(stage));                  // this warp's share of the stage has been read
+            if (++stage == kStages) { stage = 0; phase ^= 1; }
 
-            const int64_t m = (int64_t)tile * 128 + row;
-            if (m >= a.p_in) continue;
-            const int n = (int)(m / per_in);
-            const int rem = (int)(m - (int64_t)n * per_in);
-            const int t = rem / Wp, f = rem - t * Wp;
-            if (t >= a.T_out) continue;
-            if (a.out_f32) {
-                if (f != 0) continue;
-                float* o = a.out_f32 + ((int64_t)n * a.rows_out + t) * 96;
 #pragma unroll
-                for (int k = 0; k < PH; ++k) {
-                    const int c = (pl0 + k) * 8;
-                    if (c >= 96) continue;
-                    float4 r0, r1;
-                    r0.x = fmaf(__uint_as_float(v[k * 8 + 0]), s_sb[c + 0], s_sb[NP + c + 0]);
-                    r0.y = fmaf(__uint_as_float(v[k * 8 + 1]), s_sb[c + 1], s_sb[NP + c + 1]);
-                    r0.z = fmaf(__uint_as_float(v[k * 8 + 2]), s_sb[c + 2], s_sb[NP + c + 2]);
-                    r0.w = fmaf(__uint_as_float(v[k * 8 + 3]), s_sb[c + 3], s_sb[NP + c + 3]);
-                    r1.x = fmaf(__uint_as_float(v[k * 8 + 4]), s_sb[c + 4], s_sb[NP + c + 4]);
-                    r1.y = fmaf(__uint_as_float(v[k * 8 + 5]), s_sb[c + 5], s_sb[NP + c + 5]);
-                    r1.z = fmaf(__uint_as_float(v[k * 8 + 6]), s_sb[c + 6], s_sb[NP + c + 6]);
-                    r1.w = fmaf(__uint_as_float(v[k * 8 + 7]), s_sb[c + 7], s_sb[NP + c + 7]);
-                    reinterpret_cast<float4*>(o + c)[0] = r0;
-                    reinterpret_cast<float4*>(o + c)[1] = r1;
+            for (int i = 0; i < 2; ++i) {
+                const int row = wg * 64 + wq * 16 + (lane >> 2) + 8 * i;
+                const int64_t m = (int64_t)tile * 128 + row;
+                if (m >= a.p_in) continue;
+                const int n = (int)(m / per_in);
+                const int rem = (int)(m - (int64_t)n * per_in);
+                const int t = rem / Wp, f = rem - t * Wp;
+                if (t >= a.T_out) continue;
+                if (a.out_f32) {
+                    if (f != 0) continue;
+                    float* o = a.out_f32 + ((int64_t)n * a.rows_out + t) * 96;
+#pragma unroll
+                    for (int j = 0; j < NP / 8; ++j) {
+                        const int c = j * 8 + 2 * q;
+                        if (c >= 96) continue;
+                        float2 r;
+                        r.x = fmaf(acc[4 * j + 2 * i], s_sb[c], s_sb[NP + c]);
+                        r.y = fmaf(acc[4 * j + 2 * i + 1], s_sb[c + 1], s_sb[NP + c + 1]);
+                        *reinterpret_cast<float2*>(o + c) = r;
+                    }
+                    continue;
                 }
-                continue;
-            }
-            const int64_t po = a.out_T ? (int64_t)n * a.out_T * Wp + (int64_t)(t + a.out_toff) * Wp + f
-                                       : (int64_t)n * per_out + (int64_t)t * Wp + f;
-            uint4* o = reinterpret_cast<uint4*>(a.out) + kGuard + po;
-            const bool pad = f == a.W;
+                const int64_t po = a.out_T ? (int64_t)n * a.out_T * Wp + (int64_t)(t + a.out_toff) * Wp + f
+                                           : (int64_t)n * per_out + (int64_t)t * Wp + f;
+                uint4* o = reinterpret_cast<uint4*>(a.out) + kGuard + po;
+                const bool pad = f == a.W;
 #pragma unroll
-            for (int k = 0; k < PH; ++k) {
-                const int g = pl0 + k;
-                __half2 h[4], l[4];
-#pragma unroll
-                for (int u = 0; u < 4; ++u) {
-                    const int c = g * 8 + u * 2;
-                    float y0 = fmaf(__uint_as_float(v[k * 8 + u * 2]), s_sb[c], s_sb[NP + c]);
-                    float y1 = fmaf(__uint_as_float(v[k * 8 + u * 2 + 1]), s_sb[c + 1], s_sb[NP + c + 1]);
+                for (int j = 0; j < NP / 8; ++j) {
+                    const int g = j;                                       // channel-group plane; this thread holds channels 2q, 2q+1
+                    if (g >= a.cg_out) continue;
+                    const int c = g * 8 + 2 * q;
+                    float y0 = fmaf(acc[4 * j + 2 * i], s_sb[c], s_sb[NP + c]);
+                    float y1 = fmaf(acc[4 * j + 2 * i + 1], s_sb[c + 1], s_sb[NP + c + 1]);
                     if (a.apply_act) { y0 = act(y0); y1 = act(y1); }
                     if (pad) { y0 = 0.f; y1 = 0.f; }
                     const __half h0 = __float2half_rn(y0), h1 = __float2half_rn(y1);
-                    h[u] = __halves2half2(h0, h1);
-                    l[u] = __floats2half2_rn(y0 - __half2float(h0), y1 - __half2float(h1));
-                }
-                if (g < a.cg_out) {
-                    o[(int64_t)g * a.out_plane] = *reinterpret_cast<uint4*>(h);
-                    if (po == 0) o[(int64_t)g * a.out_plane - 1] = make_uint4(0, 0, 0, 0);   // front guard (position -1)
+                    const __half2 h = __halves2half2(h0, h1);
+                    const __half2 l = __floats2half2_rn(y0 - __half2float(h0), y1 - __half2float(h1));
+                    const uint32_t hw = *reinterpret_cast<const uint32_t*>(&h), lw = *reinterpret_cast<const uint32_t*>(&l);
+                    reinterpret_cast<uint32_t*>(o + (int64_t)g * a.out_plane)[q] = hw;
+                    if (po == 0) reinterpret_cast<uint32_t*>(o + (int64_t)g * a.out_plane - 1)[q] = 0u;   // front guard (position -1)
                     if (a.out_split) {
-                        o[(int64_t)(a.cg_out + g) * a.out_plane] = *reinterpret_cast<uint4*>(l);
-                        if (po == 0) o[(int64_t)(a.cg_out + g) * a.out_plane - 1] = make_uint4(0, 0, 0, 0);
+                        reinterpret_cast<uint32_t*>(o + (int64_t)(a.cg_out + g) * a.out_plane)[q] = lw;
+                        if (po == 0) reinterpret_cast<uint32_t*>(o + (int64_t)(a.cg_out + g) * a.out_plane - 1)[q] = 0u;
                     }
 #pragma unroll
                     for (int kk = 0; kk < 2; ++kk)
                         if (a.out_b[kk]) {
                             uint4* ob = reinterpret_cast<uint4*>(a.out_b[kk]) + kGuard + (int64_t)n * a.out_T * Wp +
                                         (int64_t)(t + a.out_b_toff[kk]) * Wp + f;
-                            ob[(int64_t)g * a.out_plane] = *reinterpret_cast<uint4*>(h);
-                            if (a.out_split) ob[(int64_t)(a.cg_out + g) * a.out_plane] = *reinterpret_cast<uint4*>(l);
+                            reinterpret_cast<uint32_t*>(ob + (int64_t)g * a.out_plane)[q] = hw;
+                            if (a.out_split) reinterpret_cast<uint32_t*>(ob + (int64_t)(a.cg_out + g) * a.out_plane)[q] = lw;
                         }
                 }
             }
         }
-    }
-    tc_fence_before();
-    __syncthreads();
-    if (warp == 1) {
-        tc_fence_after();
-        asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "r"(256));
     }
 }
 
@@ -397,22 +354,18 @@ __global__ void __launch_bounds__(kTcThreads, 1) tc_conv_blk_kernel(TcBlkArgs a)
     const int half_bytes = CGP * units * 16;
     uint8_t* a_smem = smem + W_BYTES;                                      // slot 0: hi half, slot 1: lo half
     uint64_t* bars = reinterpret_cast<uint64_t*>(a_smem + 2 * half_bytes);
-    // bars: full[2], empty[2], tmem_full[A], tmem_empty[A], w_full
-    uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(bars + 4 + 2 * kAccStages + 1);
-    float* s_sb = reinterpret_cast<float*>(tmem_slot + 4);
+    // bars: full[2], empty[2], w_full
+    float* s_sb = reinterpret_cast<float*>(bars + 6);
     for (int i = threadIdx.x; i < NP; i += kTcThreads) { s_sb[i] = a.scale[i]; s_sb[NP + i] = a.bias[i]; }
 
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
     const uint32_t bar0 = smem_u32(bars);
     auto full_bar = [&](int h) { return bar0 + 8u * h; };
     auto empty_bar = [&](int h) { return bar0 + 8u * (2 + h); };
-    auto tfull_bar = [&](int s) { return bar0 + 8u * (4 + s); };
-    auto tempty_bar = [&](int s) { return bar0 + 8u * (4 + kAccStages + s); };
-    const uint32_t wfull_bar = bar0 + 8u * (4 + 2 * kAccStages);
+    const uint32_t wfull_bar = bar0 + 8u * 4;
 
     if (threadIdx.x == 0) {
-        for (int h = 0; h < 2; ++h) { mbar_init(full_bar(h), 1); mbar_init(empty_bar(h), 1); }
-        for (int s = 0; s < kAccStages; ++s) { mbar_init(tfull_bar(s), 1); mbar_init(tempty_bar(s), 8); }
+        for (int h = 0; h < 2; ++h) { mbar_init(full_bar(h), 1); mbar_init(empty_bar(h), 8); }       // one arrival per MMA warp
         mbar_init(wfull_bar, 1);
         asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
     }
@@ -423,17 +376,10 @@ __global__ void __launch_bounds__(kTcThreads, 1) tc_conv_blk_kernel(TcBlkArgs a)
             for (int i = threadIdx.x; i < (CGP - a.cg_in) * units; i += kTcThreads) pz[i] = make_uint4(0, 0, 0, 0);
         }
     asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
-    if (warp == 1) {
-        asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(tmem_slot)), "r"(256));
-        asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;");
-    }
-    tc_fence_before();
     __syncthreads();
-    tc_fence_after();
-    const uint32_t tmem_base = *tmem_slot;
     // Chain of dependent launches: the successor may be scheduled from now on (it waits for this grid's completion itself
-    // before it touches a tensor); this CTA's prologue - barriers, TMEM, the weight copy below - ran beside the
-    // predecessor's tail, and only now do we wait for the predecessor's outputs.
+    // before it touches a tensor); this CTA's prologue - barriers, the weight copy below - ran beside the predecessor's
+    // tail, and only now do we wait for the predecessor's outputs.
     pdl_trigger();
 
     if (warp == 0) {
@@ -454,141 +400,111 @@ __global__ void __launch_bounds__(kTcThreads, 1) tc_conv_blk_kernel(TcBlkArgs a)
                 phase ^= 1;
             }
         }
-    } else if (warp == 1) {
-        // ===================== MMA issuer (one elected lane; the warp stays converged) =====================
-        {
-            const uint32_t idesc = (1u << 4) | ((uint32_t)(NP >> 3) << 17) | ((uint32_t)(128 >> 4) << 24);
-            tc_warp_wait(wfull_bar, 0, lane);
-            uint32_t phase = 0; int acc = 0; uint32_t acc_phase = 0;
-            const uint32_t w_addr = smem_u32(w_smem), a_addr = smem_u32(a_smem);
-            const uint32_t lbo_a = (uint32_t)units * 16u;
-            const uint32_t tap16 = (uint32_t)a.tap * 16u;
-            for (int tile = blockIdx.x; tile < a.n_tiles; tile += gridDim.x) {
-                tc_warp_wait(tempty_bar(acc), acc_phase ^ 1, lane);
-                const uint32_t d_tmem = tmem_base + (uint32_t)acc * 128u;
+    } else if (warp >= 4) {
+        // ===================== MMA + epilogue: warpgroup wg owns accumulator rows [64 wg, 64 wg + 64) =====================
+        const int wg = (warp >> 2) - 1, wq = warp & 3, q = lane & 3;
+        const uint32_t row_off = (uint32_t)wg * 64u * 16u;
+        const uint32_t w_addr = smem_u32(w_smem), a_addr = smem_u32(a_smem) + row_off;
+        const uint32_t lbo_a = (uint32_t)units * 16u;
+        const uint32_t tap16 = (uint32_t)a.tap * 16u;
+        // accumulator rows of this thread -> (stream of the block, output row, column)
+        int tr[2], slr[2], fr[2]; bool okr[2];
 #pragma unroll
-                for (int h = 0; h < 2; ++h) {
-                    tc_warp_wait(full_bar(h), phase, lane);
-                    tc_fence_after();
-                    if (tc_elect_one()) {
-#pragma unroll
-                        for (int j = 0; j < 3; ++j) {
-#pragma unroll
-                            for (int q = 0; q < CGP / 2; ++q) {
-#pragma unroll
-                                for (int wt = 0; wt < (h == 0 ? 2 : 1); ++wt) {      // hi half: (hi,hi), (hi,lo); lo half: (lo,hi)
-                                    const uint32_t w_t = w_addr + (wt == 1 ? (uint32_t)W_TERM : 0u);
-                                    const uint64_t ad = make_desc(a_addr + (uint32_t)h * (uint32_t)half_bytes + (uint32_t)(2 * q) * lbo_a + (uint32_t)j * tap16,
-                                                                  lbo_a, 128u);
-                                    const uint64_t bd = make_desc(w_t + (uint32_t)((j * CGP + 2 * q) * NP) * 16u, NP * 16u, 128u);
-                                    tc_mma_f16(d_tmem, ad, bd, idesc, (h | j | q | wt) != 0);
-                                }
-                            }
-                        }
-                        tc_commit(empty_bar(h));
-                        if (h == 1) tc_commit(tfull_bar(acc));
-                    }
-                    __syncwarp();
-                }
-                phase ^= 1;
-                if (++acc == kAccStages) { acc = 0; acc_phase ^= 1; }
-            }
+        for (int i = 0; i < 2; ++i) {
+            const int row = wg * 64 + wq * 16 + (lane >> 2) + 8 * i;
+            int t, sl, f;
+            if (a.lay.kh3) { const int SW = a.lay.S * a.W; t = row / SW; sl = (row - t * SW) / a.W; f = row - t * SW - sl * a.W; }
+            else { const int per = a.lay.T * a.lay.Wq; sl = row / per; t = (row - sl * per) / a.lay.Wq; f = row - sl * per - t * a.lay.Wq; }
+            tr[i] = t; slr[i] = sl; fr[i] = f;
+            okr[i] = row < a.m_valid && f < a.W;                       // (1,3): the pad column computes nothing that is kept
         }
-    } else {
-        // ===================== epilogue: 8 warps = 4 TMEM lane quarters x 2 halves of the channel-group planes ============
-        const int quarter = warp & 3, half = (warp - 2) >> 2;
-        constexpr int NP8 = NP / 8, PH = NP8 / 2;
-        const int pl0 = half * PH;
-        const int row = quarter * 32 + lane;
-        // accumulator row -> (stream of the block, output row, column)
-        int t, sl, f;
-        if (a.lay.kh3) { const int SW = a.lay.S * a.W; t = row / SW; sl = (row - t * SW) / a.W; f = row - t * SW - sl * a.W; }
-        else { const int per = a.lay.T * a.lay.Wq; sl = row / per; t = (row - sl * per) / a.lay.Wq; f = row - sl * per - t * a.lay.Wq; }
-        const bool row_ok = row < a.m_valid && f < a.W;                 // (1,3): the pad column computes nothing that is kept
+        tc_warp_wait(wfull_bar, 0, lane);
         pdl_wait();                                                     // the stores below must follow the predecessor grid
-        int acc = 0; uint32_t acc_phase = 0;
+        uint32_t phase = 0;
         for (int tile = blockIdx.x; tile < a.n_tiles; tile += gridDim.x) {
-            mbar_wait(tfull_bar(acc), acc_phase);
-            tc_fence_after();
-            uint32_t v[PH * 8];
-            const uint32_t taddr = tmem_base + ((uint32_t)(quarter * 32) << 16) + (uint32_t)acc * 128u + (uint32_t)pl0 * 8u;
+            float acc[NP / 2];
 #pragma unroll
-            for (int k = 0; k < PH; ++k) tc_tmem_ld8(taddr + k * 8, v + k * 8);
-            tmem_wait_ld();
-            tc_fence_before();
-            __syncwarp();
-            if (lane == 0) mbar_arrive(tempty_bar(acc));
-            if (++acc == kAccStages) { acc = 0; acc_phase ^= 1; }
-
-            const int n = tile * a.lay.S + sl;
-            const bool live = row_ok && n < a.n;
-            if (a.out_f32) {
-                if (!live || f != 0) continue;
-                float* o = a.out_f32 + ((int64_t)n * a.rows_new + t) * 96;
+            for (int h = 0; h < 2; ++h) {
+                tc_warp_wait(full_bar(h), phase, lane);
+                wg_fence();
 #pragma unroll
-                for (int k = 0; k < PH; ++k) {
-                    const int c = (pl0 + k) * 8;
-                    if (c >= 96) continue;
-                    float4 r0, r1;
-                    r0.x = fmaf(__uint_as_float(v[k * 8 + 0]), s_sb[c + 0], s_sb[NP + c + 0]);
-                    r0.y = fmaf(__uint_as_float(v[k * 8 + 1]), s_sb[c + 1], s_sb[NP + c + 1]);
-                    r0.z = fmaf(__uint_as_float(v[k * 8 + 2]), s_sb[c + 2], s_sb[NP + c + 2]);
-                    r0.w = fmaf(__uint_as_float(v[k * 8 + 3]), s_sb[c + 3], s_sb[NP + c + 3]);
-                    r1.x = fmaf(__uint_as_float(v[k * 8 + 4]), s_sb[c + 4], s_sb[NP + c + 4]);
-                    r1.y = fmaf(__uint_as_float(v[k * 8 + 5]), s_sb[c + 5], s_sb[NP + c + 5]);
-                    r1.z = fmaf(__uint_as_float(v[k * 8 + 6]), s_sb[c + 6], s_sb[NP + c + 6]);
-                    r1.w = fmaf(__uint_as_float(v[k * 8 + 7]), s_sb[c + 7], s_sb[NP + c + 7]);
-                    reinterpret_cast<float4*>(o + c)[0] = r0;
-                    reinterpret_cast<float4*>(o + c)[1] = r1;
-                }
-                continue;
-            }
-            // unit of this position in the destination(s), plane 0.  Fused (1,2) pool: columns f and f^1 are adjacent
-            // accumulator rows = adjacent lanes; the even lane writes the maximum to column f/2.  The maximum of the fp32
-            // values, split afterwards, is the element the lexicographic (hi, lo) maximum of the separate pool pass picks.
-            const bool pooled = a.pool_f == 2;
-            const bool writer = live && (!pooled || (f & 1) == 0);
-            const int fo = pooled ? f >> 1 : f;
-            int64_t dst[3];
+                for (int j = 0; j < 3; ++j) {
 #pragma unroll
-            for (int kk = 0; kk < 3; ++kk)
-                dst[kk] = a.out_lay.S ? late_unit(a.out_lay, 0, live ? n : 0, t + a.out_toff[kk], fo)
-                                      : kGuard + ((int64_t)(live ? n : 0) * a.rows_new + t) * (a.W + 1) + f;
-            const int64_t pstride = a.out_lay.S ? (int64_t)a.out_lay.units : a.out_plane;
+                    for (int qq = 0; qq < CGP / 2; ++qq) {
 #pragma unroll
-            for (int k = 0; k < PH; ++k) {
-                const int g = pl0 + k;
-                __half2 h[4], l[4];
-#pragma unroll
-                for (int u = 0; u < 4; ++u) {
-                    const int c = g * 8 + u * 2;
-                    float y0 = fmaf(__uint_as_float(v[k * 8 + u * 2]), s_sb[c], s_sb[NP + c]);
-                    float y1 = fmaf(__uint_as_float(v[k * 8 + u * 2 + 1]), s_sb[c + 1], s_sb[NP + c + 1]);
-                    if (a.apply_act) { y0 = act(y0); y1 = act(y1); }
-                    if (pooled) {
-                        y0 = fmaxf(y0, __shfl_xor_sync(0xffffffffu, y0, 1));
-                        y1 = fmaxf(y1, __shfl_xor_sync(0xffffffffu, y1, 1));
+                        for (int wt = 0; wt < (h == 0 ? 2 : 1); ++wt) {      // hi half: (hi,hi), (hi,lo); lo half: (lo,hi)
+                            const uint32_t w_t = w_addr + (wt == 1 ? (uint32_t)W_TERM : 0u);
+                            const uint64_t ad = make_desc(a_addr + (uint32_t)h * (uint32_t)half_bytes + (uint32_t)(2 * qq) * lbo_a + (uint32_t)j * tap16,
+                                                          lbo_a, 128u);
+                            const uint64_t bd = make_desc(w_t + (uint32_t)((j * CGP + 2 * qq) * NP) * 16u, NP * 16u, 128u);
+                            wg_mma<NP>(acc, ad, bd, (h | j | qq | wt) != 0);
+                        }
                     }
-                    const __half h0 = __float2half_rn(y0), h1 = __float2half_rn(y1);
-                    h[u] = __halves2half2(h0, h1);
-                    l[u] = __floats2half2_rn(y0 - __half2float(h0), y1 - __half2float(h1));
                 }
-                if (g >= a.cg_out || !writer) continue;
+                wg_commit();
+                wg_wait_all();
+                __syncwarp();
+                if (lane == 0) mbar_arrive(empty_bar(h));
+            }
+            phase ^= 1;
+
+#pragma unroll
+            for (int i = 0; i < 2; ++i) {
+                const int t = tr[i], sl = slr[i], f = fr[i];
+                const int n = tile * a.lay.S + sl;
+                const bool live = okr[i] && n < a.n;
+                if (a.out_f32) {
+                    if (!live || f != 0) continue;
+                    float* o = a.out_f32 + ((int64_t)n * a.rows_new + t) * 96;
+#pragma unroll
+                    for (int j = 0; j < NP / 8; ++j) {
+                        const int c = j * 8 + 2 * q;
+                        if (c >= 96) continue;
+                        float2 r;
+                        r.x = fmaf(acc[4 * j + 2 * i], s_sb[c], s_sb[NP + c]);
+                        r.y = fmaf(acc[4 * j + 2 * i + 1], s_sb[c + 1], s_sb[NP + c + 1]);
+                        *reinterpret_cast<float2*>(o + c) = r;
+                    }
+                    continue;
+                }
+                // unit of this position in the destination(s), plane 0.  Fused (1,2) pool: columns f and f^1 are adjacent
+                // accumulator rows, i.e. lanes 4 apart in the fragment; the even one writes the maximum to column f/2.  The
+                // maximum of the fp32 values, split afterwards, is the element the lexicographic (hi, lo) maximum of the
+                // separate pool pass picks.
+                const bool pooled = a.pool_f == 2;
+                const bool writer = live && (!pooled || (f & 1) == 0);
+                const int fo = pooled ? f >> 1 : f;
+                int64_t dst[3];
 #pragma unroll
                 for (int kk = 0; kk < 3; ++kk)
-                    if (a.out[kk]) {
-                        uint4* o = reinterpret_cast<uint4*>(a.out[kk]) + dst[kk];
-                        o[(int64_t)g * pstride] = *reinterpret_cast<uint4*>(h);
-                        o[(int64_t)(a.cg_out + g) * pstride] = *reinterpret_cast<uint4*>(l);
+                    dst[kk] = a.out_lay.S ? late_unit(a.out_lay, 0, live ? n : 0, t + a.out_toff[kk], fo)
+                                          : kGuard + ((int64_t)(live ? n : 0) * a.rows_new + t) * (a.W + 1) + f;
+                const int64_t pstride = a.out_lay.S ? (int64_t)a.out_lay.units : a.out_plane;
+#pragma unroll
+                for (int j = 0; j < NP / 8; ++j) {
+                    const int g = j, c = g * 8 + 2 * q;
+                    float y0 = fmaf(acc[4 * j + 2 * i], s_sb[c], s_sb[NP + c]);
+                    float y1 = fmaf(acc[4 * j + 2 * i + 1], s_sb[c + 1], s_sb[NP + c + 1]);
+                    if (a.apply_act) { y0 = act(y0); y1 = act(y1); }
+                    if (pooled) {
+                        y0 = fmaxf(y0, __shfl_xor_sync(0xffffffffu, y0, 4));
+                        y1 = fmaxf(y1, __shfl_xor_sync(0xffffffffu, y1, 4));
                     }
+                    if (g >= a.cg_out || !writer) continue;
+                    const __half h0 = __float2half_rn(y0), h1 = __float2half_rn(y1);
+                    const __half2 hh = __halves2half2(h0, h1);
+                    const __half2 ll = __floats2half2_rn(y0 - __half2float(h0), y1 - __half2float(h1));
+                    const uint32_t hw = *reinterpret_cast<const uint32_t*>(&hh), lw = *reinterpret_cast<const uint32_t*>(&ll);
+#pragma unroll
+                    for (int kk = 0; kk < 3; ++kk)
+                        if (a.out[kk]) {
+                            uint4* o = reinterpret_cast<uint4*>(a.out[kk]) + dst[kk];
+                            reinterpret_cast<uint32_t*>(o + (int64_t)g * pstride)[q] = hw;
+                            reinterpret_cast<uint32_t*>(o + (int64_t)(a.cg_out + g) * pstride)[q] = lw;
+                        }
+                }
             }
         }
-    }
-    tc_fence_before();
-    __syncthreads();
-    if (warp == 1) {
-        tc_fence_after();
-        asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "r"(256));
     }
 }
 
@@ -684,8 +600,8 @@ template <int CGP, int NP, int TERMS>
 int launch_tc(oww_ctx* ctx, const TcConvArgs& a, cudaStream_t s) {
     constexpr int split = TERMS == 3 ? 2 : 1, stages = TERMS == 3 ? 2 : 4;
     const size_t smem = (size_t)split * 3 * CGP * NP * 16 + (size_t)stages * split * CGP * a.rows * 16 +
-                        8 * (2 * stages + 2 * kAccStages + 1) + 16 + 2 * NP * sizeof(float);
-    if (smem > 227 * 1024) return oww_fail(ctx, OWW_EUNSUPPORTED, "tcgen05 conv tile does not fit shared memory (%zu bytes)", smem);
+                        8 * (2 * stages + 2) + 2 * NP * sizeof(float);
+    if (smem > 227 * 1024) return oww_fail(ctx, OWW_EUNSUPPORTED, "tensor-core conv tile does not fit shared memory (%zu bytes)", smem);
     // the attribute is per (function, device): tracked per handle (one bit per kernel instance), not per process
     const uint32_t bit = 1u << (((CGP / 2 + NP / 16) + (TERMS == 3 ? 16 : 0)) & 31);     // distinct for the instances in use
     if (!(ctx->tc_attr_mask & bit)) {
@@ -700,7 +616,7 @@ int launch_tc(oww_ctx* ctx, const TcConvArgs& a, cudaStream_t s) {
 
 template <int CGP, int NP>
 int launch_tc_blk(oww_ctx* ctx, const TcBlkArgs& a, cudaStream_t s) {
-    const size_t smem = (size_t)2 * 3 * CGP * NP * 16 + (size_t)2 * CGP * a.lay.units * 16 + 8 * (4 + 2 * kAccStages + 1) + 16 + 2 * NP * sizeof(float);
+    const size_t smem = (size_t)2 * 3 * CGP * NP * 16 + (size_t)2 * CGP * a.lay.units * 16 + 8 * 6 + 2 * NP * sizeof(float);
     if (smem > 227 * 1024) return oww_fail(ctx, OWW_EUNSUPPORTED, "blocked late conv tile does not fit shared memory (%zu bytes)", smem);
     const uint32_t bit = 1u << (CGP / 2);
     if (!(ctx->tc_blk_attr_mask & bit)) {
@@ -840,7 +756,7 @@ static int dispatch_tc(oww_ctx* ctx, int cgp, int np, const TcConvArgs& a, cudaS
     if (cgp == 10 && np == 80) return launch_tc<10, 80, TERMS>(ctx, a, s);
     if (cgp == 10 && np == 96) return launch_tc<10, 96, TERMS>(ctx, a, s);
     if (cgp == 12 && np == 96) return launch_tc<12, 96, TERMS>(ctx, a, s);
-    return oww_fail(ctx, OWW_EUNSUPPORTED, "no tcgen05 conv instance for cgp=%d np=%d", cgp, np);
+    return oww_fail(ctx, OWW_EUNSUPPORTED, "no tensor-core conv instance for cgp=%d np=%d", cgp, np);
 }
 
 int oww_cnn_tc_pyramid_impl(oww_ctx* ctx, const WindowSrc& src, int n, int T0, int split_from, float* d_emb, int stop_layer,
@@ -929,7 +845,7 @@ int oww_cnn_tc_pyramid_impl(oww_ctx* ctx, const WindowSrc& src, int n, int T0, i
 // The fused step kernel (cnn_tc_inc.cu) runs the frontend and conv layers 0 .. L0-1 of the 8 new mel rows in shared
 // memory and leaves the pooled output of layer L0-1 (2 new rows per stream at L0 = 11) in HBM as fp16 hi/lo planes.
 // Layers L0 .. 19 - 1.3 of the 5.6 MMAC per frame, but the ones whose fp16 rounding dominates the embedding error -
-// then run here as the SAME tcgen05 conv / pool kernels as the window mode, with split (hi/lo) operands, on "windows"
+// then run here as the SAME tensor-core conv / pool kernels as the window mode, with split (hi/lo) operands, on "windows"
 // that are the incremental rows of every stream: a (3,1) layer's input holds [2 tail rows | new rows] per stream, and
 // every layer mirrors its new rows into the buffer(s) where they are tails of the following step(s) (two buffers for
 // tensors that gain two rows per step, three for the one that gains a single row), so no copy or shift pass exists.

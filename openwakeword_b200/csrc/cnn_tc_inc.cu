@@ -1,7 +1,7 @@
 // K2 (incremental tensor-core path): ONE persistent kernel runs all 20 layers of the speech-embedding
-// CNN for the 8 new mel rows of every stream, with every activation in shared memory / TMEM.
+// CNN for the 8 new mel rows of every stream, with every activation in shared memory.
 //
-// Why this is exact.  The CNN (reference embedding_model.onnx, /root/reference/openwakeword/utils.py:90-93,
+// Why this is exact.  The CNN (reference embedding_model.onnx, openwakeword/utils.py:90-93 of the original project,
 // spec notebooks/converting_google_speech_embedding_model.ipynb:871-951) is fully convolutional along
 // time with total stride 8, and the reference evaluates it on a 76-row window that slides by exactly
 // 8 rows per 80 ms chunk (utils.py:437-443; SURVEY.md F10).  So the newest window's activations are
@@ -13,39 +13,28 @@
 //
 // Mapping.  A CTA owns a group of G streams.  Positions are ordered (t, stream, f) with one zero pad
 // column, stored as fp16 channel-group planes (16-byte units) in two smem buffers X/Y, exactly the
-// no-swizzle K-major UMMA core-matrix order.  For layer l the A operand is read IN PLACE from the
+// no-swizzle K-major core-matrix order of a wgmma operand.  For layer l the A operand is read IN PLACE from the
 // previous layer's output planes: a conv tap is a shift of the descriptor start address
 // ((1,3): -1/0/+1 units; (3,1): 0/GWp/2GWp units), so there is no im2col and no copy.  Weights
 // (+ folded BN scale/bias) of layer l+1 stream into a double buffer by cp.async.bulk while layer l
-// computes.  D lives in TMEM (4 x 128 columns); 8 epilogue warps (2 per lane quarter) apply
-// BN + leaky + clamp, write the next layer's planes to smem, and spill the new tails to HBM.
-// Max-pools are an smem->smem pass of the same warps.  Warp 8 = weight producer, warp 9 = MMA issuer.
+// computes.  The 16 compute warps form 4 warpgroups; each takes 64-position tiles of the layer in turn, accumulates
+// them with wgmma in registers, applies BN + leaky + clamp, writes the next layer's planes to smem and spills the new
+// tails to HBM.  Max-pools are an smem->smem pass of the same warps.  Warp 16 = weight producer.
 #include "oww_internal.h"
 #include "tc_common.cuh"
 #include "mel_device.cuh"
 #include <cstring>
+#include <type_traits>
 
 namespace {
 
-constexpr int kIncEpiWarps = 16;                         // four per TMEM lane quarter, each a quarter of the columns
-constexpr int kIncThreads = (kIncEpiWarps + 2) * 32;      // 576
-constexpr int kIncAcc = 4;                                // TMEM accumulator stages (4 x 128 columns)
+constexpr int kIncEpiWarps = 16;                         // compute warps: four MMA warpgroups
+constexpr int kIncThreads = (kIncEpiWarps + 1) * 32;      // 544: + the weight producer
 constexpr int kIncMaxG = 7;
 constexpr int kMelNF = 2;                                  // frames a warp of the fused frontend processes at once
 
 __device__ __forceinline__ __half2 u32_as_half2(uint32_t v) {
     return __halves2half2(__ushort_as_half((unsigned short)(v & 0xFFFFu)), __ushort_as_half((unsigned short)(v >> 16)));
-}
-__device__ __forceinline__ bool elect_one() {
-    uint32_t pred;
-    asm volatile("{\n\t.reg .pred p;\n\telect.sync _|p, 0xffffffff;\n\tselp.u32 %0, 1, 0, p;\n\t}" : "=r"(pred));
-    return pred != 0;
-}
-__device__ __forceinline__ void named_bar_sync(int id, int n) { asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(n) : "memory"); }
-__device__ __forceinline__ void tmem_ld8(uint32_t taddr, uint32_t* v) {
-    asm volatile("tcgen05.ld.sync.aligned.32x32b.x8.b32 {%0,%1,%2,%3,%4,%5,%6,%7}, [%8];"
-                 : "=r"(v[0]), "=r"(v[1]), "=r"(v[2]), "=r"(v[3]), "=r"(v[4]), "=r"(v[5]), "=r"(v[6]), "=r"(v[7])
-                 : "r"(taddr));
 }
 
 struct IncArgs {
@@ -80,7 +69,6 @@ __device__ __forceinline__ int head_rows(int slot_bytes, int K, int D) {
     return r < K ? r : K;
 }
 
-// 96 registers is the ceiling for 18 warps: registers are allocated for warps in fours (20 x 32 x 96 = 61 440 of 65 536)
 // kNL: number of conv layers the kernel runs, fixed at compile time (20 = whole CNN, 11 / 15 = cuts before the
 // split-operand layers) or 0 = read from the plan (any other cut).  With the count known the full-depth instance
 // carries none of the cut layer's code.
@@ -90,10 +78,9 @@ __global__ void __launch_bounds__(kIncThreads, 1) tc_inc_kernel(const __grid_con
     const IncPlan& P = a.plan;
     const int NL = kNL ? kNL : P.n_layers;
     const int G = P.G;
-    // [0, 2048): barriers, TMEM slot, layer-0 weights.  Activations grow from 2048 up; the per-layer weight
+    // [0, 2048): barriers, per-group stream state, layer-0 weights.  Activations grow from 2048 up; the per-layer weight
     // slots sit at the top of the arena (offsets in the plan, checked against the activation extents).
     uint64_t* bars = reinterpret_cast<uint64_t*>(smem);
-    uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(bars + 14 + 2 * kIncAcc);      // 22 barriers: [0, 176)
     float* s_l0 = reinterpret_cast<float*>(smem + 704);              // 9*24 + 24 + 24 floats: [704, 1760)
     uint4* act0 = reinterpret_cast<uint4*>(smem + 2048);            // activation arena; tensors at plan offsets
 
@@ -102,16 +89,13 @@ __global__ void __launch_bounds__(kIncThreads, 1) tc_inc_kernel(const __grid_con
     const uint32_t bar0 = smem_u32(bars);
     auto wfull = [&](int i) { return bar0 + 8u * i; };
     auto wempty = [&](int i) { return bar0 + 8u * (2 + i); };
-    auto tfull = [&](int s) { return bar0 + 8u * (4 + s); };
-    auto tempty = [&](int s) { return bar0 + 8u * (4 + kIncAcc + s); };
-    const uint32_t tails_bar = bar0 + 8u * (4 + 2 * kIncAcc);
-    const uint32_t hstart_bar = bar0 + 8u * (5 + 2 * kIncAcc);
-    auto hfull = [&](int i) { return bar0 + 8u * (6 + 2 * kIncAcc + i); };
-    auto hempty = [&](int i) { return bar0 + 8u * (10 + 2 * kIncAcc + i); };
+    const uint32_t tails_bar = bar0 + 8u * 4;                         // 14 barriers: [0, 112)
+    const uint32_t hstart_bar = bar0 + 8u * 5;
+    auto hfull = [&](int i) { return bar0 + 8u * (6 + i); };
+    auto hempty = [&](int i) { return bar0 + 8u * (10 + i); };
 
     if (threadIdx.x == 0) {
         for (int i = 0; i < 2; ++i) { mbar_init(wfull(i), 1); mbar_init(wempty(i), 1); }
-        for (int s = 0; s < kIncAcc; ++s) { mbar_init(tfull(s), 1); mbar_init(tempty(s), kIncEpiWarps); }   // one arrival per epilogue warp
         mbar_init(tails_bar, 1);
         mbar_init(hstart_bar, 1);
         for (int i = 0; i < 4; ++i) { mbar_init(hfull(i), 1); mbar_init(hempty(i), kIncEpiWarps); }
@@ -120,14 +104,7 @@ __global__ void __launch_bounds__(kIncThreads, 1) tc_inc_kernel(const __grid_con
     for (int i = threadIdx.x; i < 9 * 24; i += kIncThreads) s_l0[i] = a.w0[i];
     if (threadIdx.x < 24) { s_l0[216 + threadIdx.x] = a.s0[threadIdx.x]; s_l0[240 + threadIdx.x] = a.b0[threadIdx.x]; }
     asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
-    if (warp == kIncEpiWarps + 1) {
-        asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(tmem_slot)), "r"(512));
-        asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;");
-    }
-    tc_fence_before();
     __syncthreads();
-    tc_fence_after();
-    const uint32_t tmem_base = __shfl_sync(0xffffffffu, *tmem_slot, 0);
 
     if (warp == kIncEpiWarps) {
         // ===================== weight producer =====================
@@ -176,118 +153,11 @@ __global__ void __launch_bounds__(kIncThreads, 1) tc_inc_kernel(const __grid_con
                 }
             }
         }
-    } else if (warp == kIncEpiWarps + 1) {
-        // ===================== MMA issuer =====================
-        uint32_t wpar[2] = {0, 0};
-        int acc = 0; uint32_t acc_par = 0;
-        bool have_prev = false; int prev_i = 0;
-        uint32_t tails_par = 0;
-        for (int grp = blockIdx.x; grp < P.n_groups; grp += gridDim.x) {
-            for (int l = 1; l < NL; ++l) {
-                const IncLayer& L = P.L[l];
-                named_bar_sync(1, (kIncEpiWarps + 1) * 32);       // layer l-1 output complete and fenced
-                tc_fence_after();
-                // layer l-1's epilogue (which reads scale/bias from its weight slot) is done: free that slot
-                if (lane == 0 && have_prev) mbar_arrive(wempty(prev_i));
-                if (L.kh3) { mbar_wait(tails_bar, tails_par); tails_par ^= 1; }   // rows 0..1 of the input have landed
-                const int i = l & 1;
-                const bool dbg = a.dbg_clock && blockIdx.x == 0 && grp == 0 && lane == 0;
-                long long c0 = 0;
-                if (dbg) c0 = clock64();
-                mbar_wait(wfull(i), wpar[i]);
-                wpar[i] ^= 1;
-                if (dbg) { const long long c1 = clock64(); a.dbg_clock[21 + l] = c1 - c0; c0 = c1; }
-                const uint32_t w_addr = smem_u32(smem + L.w_smem);
-                const uint32_t a_base = smem_u32(act0 + L.in_base);
-                const uint32_t idesc = (1u << 4) | ((uint32_t)(L.np >> 3) << 17) | ((uint32_t)(128 >> 4) << 24);
-                const int n_tiles = (L.M + 127) / 128;
-                // K = 16 = two channel-group planes per MMA; an odd plane count pairs the last plane with itself
-                // (LBO 0) against zero weights, so no pad plane has to exist in smem.  Only the 14-bit start
-                // address field changes between MMAs.  The issue block sits under elect.sync so that every
-                // operand is warp-uniform for the compiler (UTCHMMA straight from uniform registers - an
-                // `if (lane == 0)` region costs ~160 cycles per MMA in R2UR/waterfall code, see scripts/mma_probe.cu).
-                const int nq = L.cgp / 2;
-                const uint32_t a_hi_pair = (uint32_t)make_desc(0, (uint32_t)L.in_pitch * 16u, 128u);   // low word: LBO field
-                const uint32_t a_hi_self = (uint32_t)make_desc(0, 0u, 128u);
-                const uint32_t desc_hi = (uint32_t)(make_desc(0, 0u, 128u) >> 32);                    // SBO + version
-                const uint32_t b_lo0 = (uint32_t)make_desc(0, (uint32_t)L.np * 16u, 128u);
-                const uint32_t a_unit0 = (a_base >> 4) + 1u;
-                const uint32_t b_unit0 = w_addr >> 4;
-                // per-layer geometry in registers: inside the tile loop every L.field would be an indexed constant load
-                // again (P.L[l] with a run-time l, and the barrier asm statements are memory clobbers) - five dependent
-                // LDCUs per tile ahead of the first MMA
-                const uint32_t tap0 = (uint32_t)L.tap[0], tap1 = (uint32_t)L.tap[1], tap2 = (uint32_t)L.tap[2];
-                const uint32_t pitch2 = 2u * (uint32_t)L.in_pitch, np2 = 2u * (uint32_t)L.np, tap_w = (uint32_t)(L.cgp * L.np);
-                const int n_pair = L.cg_in / 2;                   // K steps whose second plane exists
-                // Odd plane count (24 or 72 channels): instead of padding every tap to an even number of planes (one
-                // half-empty MMA per tap), the K octets of the three taps are chained - the last plane of tap 0 shares an
-                // MMA with the first plane of tap 1 (the LBO field is just the distance of the two octets, whatever tap they
-                // belong to): (3 cg + 1) / 2 MMAs per tile instead of 3 (cg + 1) / 2 (5 instead of 6 at 24 channels).  The
-                // weights of such a layer are packed in the same octet order (oww_inc_setup).
-                const bool chained = (L.cg_in & 1) != 0;
-                const uint32_t a_cross = (uint32_t)make_desc(0, ((uint32_t)(L.cg_in - 1) * (uint32_t)L.in_pitch + tap0 - tap1) * 16u, 128u);
-                const uint32_t last_plane = (uint32_t)(L.cg_in - 1) * (uint32_t)L.in_pitch;
-                for (int tile = 0; tile < n_tiles; ++tile) {
-                    mbar_wait(tempty(acc), acc_par ^ 1);
-                    tc_fence_after();
-                    const uint32_t d_tmem = tmem_base + (uint32_t)acc * 128u;
-                    // one elect.sync per tile: the elected lane issues the tile's MMAs and the commit back to back
-                    if (elect_one()) {
-                        const uint32_t a_t0 = a_unit0 + (uint32_t)(tile * 128);
-                        const uint64_t dhi = (uint64_t)desc_hi << 32;
-                        if (chained) {
-                            uint32_t b = b_unit0;
-                            uint32_t accumulate = 0;
-                            for (int k = 0; k < n_pair; ++k) {            // tap 0: planes (0,1) (2,3) ...
-                                tc_mma_f16(d_tmem, dhi | a_hi_pair | ((a_t0 + tap0 + (uint32_t)k * pitch2) & 0x3FFFu), dhi | b_lo0 | (b & 0x3FFFu), idesc, accumulate);
-                                accumulate = 1; b += np2;
-                            }
-                            // (tap 1, plane 0) + (tap 0, last plane): the lower address first
-                            tc_mma_f16(d_tmem, dhi | a_cross | ((a_t0 + tap1) & 0x3FFFu), dhi | b_lo0 | (b & 0x3FFFu), idesc, accumulate);
-                            b += np2;
-                            for (int k = 0; k < n_pair; ++k) {            // tap 1: planes (1,2) (3,4) ...
-                                tc_mma_f16(d_tmem, dhi | a_hi_pair | ((a_t0 + tap1 + (uint32_t)L.in_pitch + (uint32_t)k * pitch2) & 0x3FFFu),
-                                           dhi | b_lo0 | (b & 0x3FFFu), idesc, 1u);
-                                b += np2;
-                            }
-                            for (int k = 0; k < n_pair; ++k) {            // tap 2: planes (0,1) (2,3) ...
-                                tc_mma_f16(d_tmem, dhi | a_hi_pair | ((a_t0 + tap2 + (uint32_t)k * pitch2) & 0x3FFFu), dhi | b_lo0 | (b & 0x3FFFu), idesc, 1u);
-                                b += np2;
-                            }
-                            // tap 2, last plane, paired with itself against a zero weight octet
-                            tc_mma_f16(d_tmem, dhi | a_hi_self | ((a_t0 + tap2 + last_plane) & 0x3FFFu), dhi | b_lo0 | (b & 0x3FFFu), idesc, 1u);
-                        } else {
-                        uint32_t accumulate = 0;
-#pragma unroll
-                        for (int j = 0; j < 3; ++j) {
-                            const uint32_t a_tap = a_t0 + (j == 0 ? tap0 : j == 1 ? tap1 : tap2);
-                            const uint32_t b_tap = b_unit0 + (uint32_t)j * tap_w;
-                            for (int q = 0; q < nq; ++q) {
-                                const uint32_t alo = (q < n_pair ? a_hi_pair : a_hi_self) | ((a_tap + (uint32_t)q * pitch2) & 0x3FFFu);
-                                const uint32_t blo = b_lo0 | ((b_tap + (uint32_t)q * np2) & 0x3FFFu);
-                                tc_mma_f16(d_tmem, dhi | alo, dhi | blo, idesc, accumulate);
-                                accumulate = 1;
-                            }
-                        }
-                        }
-                        tc_commit(tfull(acc));
-                    }
-                    __syncwarp();
-                    if (++acc == kIncAcc) { acc = 0; acc_par ^= 1; }
-                }
-                if (dbg) a.dbg_clock[41 + l] = clock64() - c0;      // MMA issue time of the layer
-                have_prev = true; prev_i = i;
-                __syncwarp();
-            }
-        }
     } else {
-        // ===================== epilogue / CUDA-core warps (256 threads) =====================
-        const int et = threadIdx.x;                               // 0..255
-        const int quarter = warp & 3, part = warp >> 2;
-        const int row = quarter * 32 + lane;
-        int acc = 0; uint32_t acc_par = 0;
+        // ===================== compute warps (512 threads): frontend, MMAs, epilogues, pools, heads =====================
+        const int et = threadIdx.x;                               // 0..511
         uint32_t epar[2] = {0, 0};
-        uint32_t epi_tails_par = 0;
+        uint32_t epi_tails_par = 0, mma_tails_par = 0;
         uint32_t hf_par = 0; int hchunk_e = 0;
         for (int grp = blockIdx.x; grp < P.n_groups; grp += gridDim.x) {
             const uint4* tin = a.tails_in + (int64_t)grp * P.tail_units;
@@ -417,6 +287,8 @@ __global__ void __launch_bounds__(kIncThreads, 1) tc_inc_kernel(const __grid_con
                     }
                     if (!L.final && et < L.cg_out) nx[et * L.nx_pitch] = make_uint4(0, 0, 0, 0);
                 };
+                // rows 0..1 of a (3,1) layer's input (the tails copy issued in the previous phase) must have landed
+                if (l > 0 && L.kh3) { mbar_wait(tails_bar, mma_tails_par); mma_tails_par ^= 1; }
                 if (!L.pool_t) fill_tails_and_guards();
                 else if (et < L.cg_out) (act0 + L.tmp_base)[et * L.tmp_pitch] = make_uint4(0, 0, 0, 0);
 
@@ -479,111 +351,158 @@ __global__ void __launch_bounds__(kIncThreads, 1) tc_inc_kernel(const __grid_con
                         }
                     }
                 } else {
-                    // ---- tcgen05 layer: drain TMEM tiles ----
+                    // ---- tensor-core layer: 64-position tiles, warpgroup w takes tiles w, w + 4, ... ----
                     mbar_wait(wfull(l & 1), epar[l & 1]);             // weights (and scale/bias) of layer l have landed
                     epar[l & 1] ^= 1;
                     const float* sb = reinterpret_cast<const float*>(smem + L.w_smem + 3 * L.cgp * L.np * 16);
-                    const int np8 = L.np / 8;
-                    // Work split of the 16 warps (4 lane quarters x 4 "parts").  A part owns up to 3 channel-group planes of a
-                    // tile; layers with few planes therefore need only PT = 1 or 2 parts per tile, and the other parts take
-                    // the NEXT tiles: 4/PT tiles are drained concurrently (one TMEM stage each), so the per-tile latency
-                    // chain (wait -> tcgen05.ld -> math -> store) of one part overlaps the others'.
-                    const int PT = L.final ? 4 : (L.cg_out <= 3 ? 1 : (L.cg_out <= 6 ? 2 : 4));
-                    const int sets = 4 / PT, my_set = part / PT, my_sub = part % PT;
-                    const int ph = PT == 4 ? (np8 + 3) / 4 : 3;
-                    const int pl0 = min(np8, my_sub * ph), pl1 = min(np8, pl0 + ph);
                     uint4* dst = L.pool_t ? (act0 + L.tmp_base) : nx;
                     const int dpitch = L.pool_t ? L.tmp_pitch : L.nx_pitch;
                     const int t_off_units = L.pool_t ? 0 : L.nx_t_off * G * L.Wp;
-                    const int n_tiles = (L.M + 127) / 128;
+                    const int n_t64 = (L.M + 63) / 64;
                     const int tail_start = (L.T_out - 2) * G * L.Wp;
                     const uint32_t wp_magic = 0xFFFFFFFFu / (uint32_t)L.Wp + 1u, g_magic = G > 1 ? 0xFFFFFFFFu / (uint32_t)G + 1u : 0u;
                     const bool edbg = a.dbg_clock && blockIdx.x == 0 && grp == 0 && et == 0;
                     long long e0 = 0;
                     if (edbg) e0 = clock64();
-                    const int acc0 = acc; const uint32_t par0 = acc_par;
-                    for (int tile = my_set; tile < n_tiles; tile += sets) {
-                        const int stage = (acc0 + tile) & (kIncAcc - 1);
-                        const uint32_t spar = par0 ^ (uint32_t)(((acc0 + tile) >> 2) & 1);
-                        mbar_wait(tfull(stage), spar);
-                        if (edbg && tile == 0) a.dbg_clock[61 + l] = clock64() - e0;     // phase start -> first accumulator ready
-                        tc_fence_after();
-                        uint32_t v[3][8];
-                        const uint32_t taddr = tmem_base + ((uint32_t)(quarter * 32) << 16) + (uint32_t)stage * 128u;
+                    const int wg = warp >> 2, wq = warp & 3, q = lane & 3;
+                    const uint32_t w_addr = smem_u32(smem + L.w_smem);
+                    const uint32_t a_base = smem_u32(act0 + L.in_base);
+                    // K = 16 = two channel-group planes per MMA; an odd plane count pairs the last plane with itself
+                    // (LBO 0) against zero weights, so no pad plane has to exist in smem.  Only the 14-bit start
+                    // address field changes between MMAs.
+                    const int nq = L.cgp / 2;
+                    const uint32_t a_hi_pair = (uint32_t)make_desc(0, (uint32_t)L.in_pitch * 16u, 128u);   // low word: LBO field
+                    const uint32_t a_hi_self = (uint32_t)make_desc(0, 0u, 128u);
+                    const uint64_t dhi = make_desc(0, 0u, 128u) & 0xFFFFFFFF00000000ull;                  // high word: SBO field
+                    const uint32_t b_lo0 = (uint32_t)make_desc(0, (uint32_t)L.np * 16u, 128u);
+                    const uint32_t a_unit0 = (a_base >> 4) + 1u;
+                    const uint32_t b_unit0 = w_addr >> 4;
+                    const uint32_t tap0 = (uint32_t)L.tap[0], tap1 = (uint32_t)L.tap[1], tap2 = (uint32_t)L.tap[2];
+                    const uint32_t pitch2 = 2u * (uint32_t)L.in_pitch, np2 = 2u * (uint32_t)L.np, tap_w = (uint32_t)(L.cgp * L.np);
+                    const int n_pair = L.cg_in / 2;                   // K steps whose second plane exists
+                    // Odd plane count (24 or 72 channels): instead of padding every tap to an even number of planes (one
+                    // half-empty MMA per tap), the K octets of the three taps are chained - the last plane of tap 0 shares an
+                    // MMA with the first plane of tap 1 (the LBO field is just the distance of the two octets, whatever tap they
+                    // belong to): (3 cg + 1) / 2 MMAs per tile instead of 3 (cg + 1) / 2 (5 instead of 6 at 24 channels).  The
+                    // weights of such a layer are packed in the same octet order (oww_inc_setup).
+                    const bool chained = (L.cg_in & 1) != 0;
+                    const int n_steps = chained ? 3 * n_pair + 2 : 3 * nq;
+                    const uint32_t a_cross = (uint32_t)make_desc(0, ((uint32_t)(L.cg_in - 1) * (uint32_t)L.in_pitch + tap0 - tap1) * 16u, 128u);
+                    const uint32_t last_plane = (uint32_t)(L.cg_in - 1) * (uint32_t)L.in_pitch;
+                    // Work items: (64-position tile, chunk of N: 32 columns, or 16 where N is 48 / 80); warpgroup w takes items
+                    // w, w + 4, ... two at a time (both MMA chains in flight, then both epilogues).  The chunks keep the
+                    // accumulators at 2 x 16 registers per thread next to the rest of the kernel's state.
+                    const int nc = (L.np & 31) ? 16 : 32;
+                    const int n_chunks = L.np / nc;
+                    const int n_items = n_t64 * n_chunks;
+                    // per-layer geometry in registers: inside the item loop every L.field would be an indexed parameter load
+                    const int lM = L.M, lWp = L.Wp, lW = L.W, lnp = L.np, lcg_out = L.cg_out, ltail = L.nx_tail_off;
+                    const bool lfinal = L.final != 0, lpool = L.pool_t != 0;
+                    const uint32_t lin_pitch = (uint32_t)L.in_pitch;
+                    const int tail_pitch = 2 * G * lWp;
+                    auto mma_item = [&](auto nc_const, auto ns_const, float* acc, int it) {
+                        constexpr int NP = decltype(nc_const)::value;          // columns of this chunk
+                        constexpr int NS = decltype(ns_const)::value;          // K steps (compile time: unrolled chain)
+                        constexpr bool kChained = NS % 3 == 2;
+                        constexpr int kPair = kChained ? (NS - 2) / 3 : NS / 3, kNq = NS / 3;
+                        const int t64 = it / n_chunks, c0 = (it - t64 * n_chunks) * NP;
+                        const uint32_t a_t0 = a_unit0 + (uint32_t)(t64 * 64);
+                        const uint32_t b_unit = b_unit0 + (uint32_t)c0;        // weight row n of an octet block: unit n
 #pragma unroll
-                        for (int k = 0; k < 3; ++k)
-                            if (pl0 + k < pl1) tmem_ld8(taddr + (pl0 + k) * 8, v[k]);
-                        tmem_wait_ld();
-                        tc_fence_before();
-                        __syncwarp();
-                        if (lane == 0) mbar_arrive_cnt(tempty(stage), (uint32_t)sets);   // 4*PT warps drain a tile: sets arrivals each = 16
-                        const int m = tile * 128 + row;
-                        if (m >= L.M) continue;
-                        // m = (t*G + g)*Wp + f; exact division by multiply-high (m < 2^16, divisors < 2^6)
-                        const int tg = (int)__umulhi((uint32_t)m, wp_magic);
-                        const int f = m - tg * L.Wp;
-                        const int g = G > 1 ? tg - (int)__umulhi((uint32_t)tg, g_magic) * G : 0;
-                        const bool live = s_live[g] != 0;
-                        if (L.final) {
-                            if (f != 0 || !live) continue;
-                            float* o = a.fused ? a.feat_ring + (int64_t)(grp * G + g) * a.feat_stride + (int64_t)(s_cnt[8 + g] & a.feat_mask) * 96
-                                               : a.emb + (int64_t)(grp * G + g) * 96;
-#pragma unroll
-                            for (int k = 0; k < 3; ++k) {
-                                if (pl0 + k >= pl1) continue;
-                                const int c = (pl0 + k) * 8;
-                                float4 r0, r1;
-                                r0.x = fmaf(__uint_as_float(v[k][0]), sb[c + 0], sb[L.np + c + 0]);
-                                r0.y = fmaf(__uint_as_float(v[k][1]), sb[c + 1], sb[L.np + c + 1]);
-                                r0.z = fmaf(__uint_as_float(v[k][2]), sb[c + 2], sb[L.np + c + 2]);
-                                r0.w = fmaf(__uint_as_float(v[k][3]), sb[c + 3], sb[L.np + c + 3]);
-                                r1.x = fmaf(__uint_as_float(v[k][4]), sb[c + 4], sb[L.np + c + 4]);
-                                r1.y = fmaf(__uint_as_float(v[k][5]), sb[c + 5], sb[L.np + c + 5]);
-                                r1.z = fmaf(__uint_as_float(v[k][6]), sb[c + 6], sb[L.np + c + 6]);
-                                r1.w = fmaf(__uint_as_float(v[k][7]), sb[c + 7], sb[L.np + c + 7]);
-                                reinterpret_cast<float4*>(o + c)[0] = r0;
-                                reinterpret_cast<float4*>(o + c)[1] = r1;
+                        for (int s = 0; s < NS; ++s) {
+                            uint32_t a_off, a_f, b_off;
+                            if (kChained) {
+                                const int k1 = s - kPair - 1, k2 = s - 2 * kPair - 1;
+                                a_off = s < kPair ? tap0 + (uint32_t)s * pitch2                         // tap 0: planes (0,1) (2,3) ...
+                                      : s == kPair ? tap1                                                // (tap 1, plane 0) + (tap 0, last plane)
+                                      : k1 < kPair ? tap1 + lin_pitch + (uint32_t)k1 * pitch2            // tap 1: planes (1,2) (3,4) ...
+                                      : k2 < kPair ? tap2 + (uint32_t)k2 * pitch2                        // tap 2: planes (0,1) (2,3) ...
+                                      : tap2 + last_plane;                                               // tap 2, last plane, with itself
+                                a_f = s == kPair ? a_cross : (k2 >= kPair ? a_hi_self : a_hi_pair);
+                                b_off = (uint32_t)s * np2;
+                            } else {
+                                const int j = s / kNq, qq = s - j * kNq;
+                                a_off = (j == 0 ? tap0 : j == 1 ? tap1 : tap2) + (uint32_t)qq * pitch2;
+                                a_f = a_hi_pair;                                                         // even plane count
+                                b_off = (uint32_t)j * tap_w + (uint32_t)qq * np2;
                             }
-                            continue;
+                            wg_mma<NP>(acc, dhi | a_f | ((a_t0 + a_off) & 0x3FFFu), dhi | b_lo0 | ((b_unit + b_off) & 0x3FFFu), s > 0);
                         }
-                        const bool pad = f == L.W;
-                        uint4* d0 = dst + (1 + t_off_units + m);
-                        const bool keep_tail = !L.pool_t && L.nx_tail_off >= 0 && m >= tail_start && live;
-                        uint4* t0 = tout + (L.nx_tail_off + (m - tail_start));
-                        const int n_pl = min(pl1, L.cg_out) - pl0;
+                    };
+                    auto epi_item = [&](auto nc_const, const float* acc, int it) {
+                        constexpr int NP = decltype(nc_const)::value;
+                        const int t64 = it / n_chunks, c0 = (it - t64 * n_chunks) * NP;
 #pragma unroll
-                        for (int k = 0; k < 3; ++k) {
-                            if (k >= n_pl) break;
-                            const int pl = pl0 + k;
-                            const float4* sc4 = reinterpret_cast<const float4*>(sb + pl * 8);
-                            const float4* bi4 = reinterpret_cast<const float4*>(sb + L.np + pl * 8);
-                            const float4 s0 = sc4[0], s1 = sc4[1], b0 = bi4[0], b1 = bi4[1];
-                            __half2 h[4];
-                            h[0] = __floats2half2_rn(act(fmaf(__uint_as_float(v[k][0]), s0.x, b0.x)), act(fmaf(__uint_as_float(v[k][1]), s0.y, b0.y)));
-                            h[1] = __floats2half2_rn(act(fmaf(__uint_as_float(v[k][2]), s0.z, b0.z)), act(fmaf(__uint_as_float(v[k][3]), s0.w, b0.w)));
-                            h[2] = __floats2half2_rn(act(fmaf(__uint_as_float(v[k][4]), s1.x, b1.x)), act(fmaf(__uint_as_float(v[k][5]), s1.y, b1.y)));
-                            h[3] = __floats2half2_rn(act(fmaf(__uint_as_float(v[k][6]), s1.z, b1.z)), act(fmaf(__uint_as_float(v[k][7]), s1.w, b1.w)));
-                            const uint4 pk = pad ? make_uint4(0, 0, 0, 0) : *reinterpret_cast<uint4*>(h);
-                            d0[pl * dpitch] = pk;
-                            if (keep_tail) t0[pl * (2 * G * L.Wp)] = pk;
-                            if (to_global) {
-                                // cut layer only (warp-uniform, one layer per step): the unpooled temp also keeps the lo parts
-                                // (y = hi + lo).  The values are recomputed here so the common path above carries no extra registers.
-                                const float sv[8] = {s0.x, s0.y, s0.z, s0.w, s1.x, s1.y, s1.z, s1.w};
-                                const float bv[8] = {b0.x, b0.y, b0.z, b0.w, b1.x, b1.y, b1.z, b1.w};
-                                __half2 lo[4];
+                        for (int i = 0; i < 2; ++i) {
+                            const int m = t64 * 64 + wq * 16 + (lane >> 2) + 8 * i;
+                            if (m >= lM) continue;
+                            // m = (t*G + g)*Wp + f; exact division by multiply-high (m < 2^16, divisors < 2^6)
+                            const int tg = (int)__umulhi((uint32_t)m, wp_magic);
+                            const int f = m - tg * lWp;
+                            const int g = G > 1 ? tg - (int)__umulhi((uint32_t)tg, g_magic) * G : 0;
+                            const bool live = s_live[g] != 0;
+                            if (lfinal) {
+                                if (f != 0 || !live) continue;
+                                float* o = a.fused ? a.feat_ring + (int64_t)(grp * G + g) * a.feat_stride + (int64_t)(s_cnt[8 + g] & a.feat_mask) * 96
+                                                   : a.emb + (int64_t)(grp * G + g) * 96;
 #pragma unroll
-                                for (int u = 0; u < 4; ++u) {
-                                    const float y0 = act(fmaf(__uint_as_float(v[k][2 * u]), sv[2 * u], bv[2 * u]));
-                                    const float y1 = act(fmaf(__uint_as_float(v[k][2 * u + 1]), sv[2 * u + 1], bv[2 * u + 1]));
-                                    lo[u] = __floats2half2_rn(y0 - __low2float(h[u]), y1 - __high2float(h[u]));
+                                for (int j = 0; j < NP / 8; ++j) {
+                                    const int c = c0 + j * 8 + 2 * q;
+                                    float2 r;
+                                    r.x = fmaf(acc[4 * j + 2 * i], sb[c], sb[lnp + c]);
+                                    r.y = fmaf(acc[4 * j + 2 * i + 1], sb[c + 1], sb[lnp + c + 1]);
+                                    *reinterpret_cast<float2*>(o + c) = r;
                                 }
-                                d0[(L.cg_out + pl) * dpitch] = pad ? make_uint4(0, 0, 0, 0) : *reinterpret_cast<uint4*>(lo);
+                                continue;
+                            }
+                            const bool pad = f == lW;
+                            uint4* d0 = dst + (1 + t_off_units + m);
+                            const bool keep_tail = !lpool && ltail >= 0 && m >= tail_start && live;
+                            uint4* t0 = tout + (ltail + (m - tail_start));
+                            // this thread holds channels 2q, 2q+1 of every plane: one 32-bit word of each 16-byte unit
+#pragma unroll
+                            for (int j = 0; j < NP / 8; ++j) {
+                                const int pl = c0 / 8 + j;
+                                if (pl >= lcg_out) break;
+                                const int c = pl * 8 + 2 * q;
+                                const float y0 = act(fmaf(acc[4 * j + 2 * i], sb[c], sb[lnp + c]));
+                                const float y1 = act(fmaf(acc[4 * j + 2 * i + 1], sb[c + 1], sb[lnp + c + 1]));
+                                const __half2 h = __floats2half2_rn(y0, y1);
+                                const uint32_t hw = pad ? 0u : *reinterpret_cast<const uint32_t*>(&h);
+                                reinterpret_cast<uint32_t*>(d0 + pl * dpitch)[q] = hw;
+                                if (keep_tail) reinterpret_cast<uint32_t*>(t0 + pl * tail_pitch)[q] = hw;
+                                if (to_global) {
+                                    // cut layer only (warp-uniform, one layer per step): the unpooled temp also keeps the
+                                    // lo parts (y = hi + lo)
+                                    const __half2 lo = __floats2half2_rn(y0 - __low2float(h), y1 - __high2float(h));
+                                    reinterpret_cast<uint32_t*>(d0 + (lcg_out + pl) * dpitch)[q] = pad ? 0u : *reinterpret_cast<const uint32_t*>(&lo);
+                                }
                             }
                         }
+                    };
+                    auto run_items = [&](auto nc_const, auto ns_const) {
+                        constexpr int NP = decltype(nc_const)::value;
+                        for (int it = wg; it < n_items; it += 4) {
+                            float acc0[NP / 2];
+                            wg_fence();
+                            mma_item(nc_const, ns_const, acc0, it);
+                            wg_commit();
+                            wg_wait_all();
+                            if (edbg && it == 0) a.dbg_clock[61 + l] = clock64() - e0;     // phase start -> first accumulator ready
+                            epi_item(nc_const, acc0, it);
+                        }
+                    };
+                    auto run_steps = [&](auto ns_const) {
+                        if (nc == 32) run_items(std::integral_constant<int, 32>{}, ns_const);
+                        else run_items(std::integral_constant<int, 16>{}, ns_const);
+                    };
+                    switch (n_steps) {
+                        case 5: run_steps(std::integral_constant<int, 5>{}); break;
+                        case 9: run_steps(std::integral_constant<int, 9>{}); break;
+                        case 14: run_steps(std::integral_constant<int, 14>{}); break;
+                        case 18: run_steps(std::integral_constant<int, 18>{}); break;
+                        default: __trap();                                // the plan only holds 24 / 48 / 72 / 96-channel inputs
                     }
-                    acc_par = par0 ^ (uint32_t)(((acc0 + n_tiles) >> 2) & 1);
-                    acc = (acc0 + n_tiles) & (kIncAcc - 1);
                     if (edbg) a.dbg_clock[81 + l] = clock64() - e0;                       // phase start -> last tile stored
                     if (L.pool_t) {
                         // ---- max-pool: tmp (unpooled conv output) -> nx ----
@@ -672,12 +591,11 @@ __global__ void __launch_bounds__(kIncThreads, 1) tc_inc_kernel(const __grid_con
                     }
                 }
                 if (L.nx_tail_off >= 0) epi_tails_par ^= 1;
-                // ---- phase done: make generic-proxy smem writes visible to the tensor core ----
+                // ---- phase done: make generic-proxy smem writes visible to the tensor core; once every warp is past
+                //      this barrier, layer l's weight slot (MMA operand, scale / bias) is free for the producer ----
                 asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
-                if (l < NL - 1) {
-                    tc_fence_before();
-                    named_bar_sync(1, (kIncEpiWarps + 1) * 32);
-                }
+                named_bar_sync(1, kIncEpiWarps * 32);
+                if (l > 0 && et == 0) mbar_arrive(wempty(l & 1));
             }
             if (a.dbg_clock && blockIdx.x == 0 && grp == 0 && et == 0) a.dbg_clock[OWW_N_CONV] = clock64();
             if (a.fused && NL == OWW_N_CONV) {
@@ -868,12 +786,6 @@ __global__ void __launch_bounds__(kIncThreads, 1) tc_inc_kernel(const __grid_con
             }
         }
     }
-    tc_fence_before();
-    __syncthreads();
-    if (warp == kIncEpiWarps + 1) {
-        tc_fence_after();
-        asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "r"(512));
-    }
 }
 
 // ---- capture of tails from the full-window planes (stream-major positions) ----------------------
@@ -902,7 +814,7 @@ int oww_inc_build_plan(oww_ctx* ctx, int G, int n_streams, int n_layers, IncPlan
     const int NL = n_layers;            // conv layers inside the kernel: 20, or a cut after a pooled layer (cut plan)
     if (NL < 3 || NL > OWW_N_CONV || (NL < OWW_N_CONV && !ctx->conv[NL - 1].pool_t))
         return oww_fail(ctx, OWW_EINVAL, "fused-CNN plan: cannot cut after layer %d", NL - 1);
-    constexpr int kTop = 227 * 1024;     // usable dynamic shared memory per CTA on sm_100
+    constexpr int kTop = 227 * 1024;     // usable dynamic shared memory per CTA on sm_90
     constexpr int kActBase = 2048;
     IncPlan P;
     std::memset(&P, 0, sizeof(P));
@@ -1071,8 +983,8 @@ int oww_inc_n_layers(const oww_ctx* ctx) {
 }
 
 int oww_inc_alloc_streams(oww_ctx* ctx) {
-    // Group size: a group's latency is mostly per-layer fixed cost (about 50 us + 6.5 us per stream on B200), so take
-    // the feasible G that minimises rounds(G) * T(G) for this stream count.
+    // Group size: a group's latency is mostly per-layer fixed cost plus a small share per stream (modelled as
+    // 50 + 6.5 G), so take the feasible G that minimises rounds(G) * T(G) for this stream count.
     int best_g = 0; double best_cost = 0;
     for (int g = 1; g <= kIncMaxG; ++g) {
         IncPlan P;
@@ -1247,7 +1159,7 @@ __global__ void fill_ones_kernel(float* p, int n) {
 }  // namespace
 
 // Tails of the all-ones window in the compact single-stream (G = 1) layout + the table reset_kernel scatters them with.
-// Runs the full-window tcgen05 pyramid (cnn_tc.cu) once on ones(76,32) with the tail capture pointed at a G = 1 plan;
+// Runs the full-window tensor-core pyramid (cnn_tc.cu) once on ones(76,32) with the tail capture pointed at a G = 1 plan;
 // the incremental kernel is bit-identical to that pyramid, so a stream seeded with these tails continues exactly as if
 // its (constant) history had been streamed through it.  Synchronous; called lazily by the first reset after a weight load.
 int oww_inc_build_template(oww_ctx* ctx) {

@@ -1,8 +1,8 @@
 // K3: wake-word classifier heads, one CTA per (tile of 32 streams, head).
 //
 // Replaces the per-head onnxruntime sessions of the reference
-// (/root/reference/openwakeword/model.py:137-138,153-159,287-302) for the DNN family of
-// /root/reference/openwakeword/train.py:56-83,144-165: Flatten([n_in,96]) -> Linear -> [LayerNorm]
+// (openwakeword/model.py:137-138,153-159,287-302) for the DNN family of
+// openwakeword/train.py:56-83,144-165: Flatten([n_in,96]) -> Linear -> [LayerNorm]
 // -> ReLU -> n x (Linear -> [LayerNorm] -> ReLU) -> Linear -> Sigmoid | (ReLU+)Softmax.
 // The input window is gathered straight from the per-stream feature ring (AudioFeatures.get_features,
 // utils.py:454-460), so predict() needs no host copy of the embeddings.  All loaded heads run in the

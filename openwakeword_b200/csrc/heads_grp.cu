@@ -1,76 +1,40 @@
-// K3 (grouped tensor-core path, streaming): every head that reads the same feature window, in ONE CTA per 128 streams.
+// K3 (tensor-core path, streaming and bulk clips): the heads on the fp16 mirror of the feature rings.
 //
-// Same graphs as heads.cu / heads_tc.cu (reference: <head>.onnx sessions, /root/reference/openwakeword/model.py:137-138,
-// 153-159,287-302; family /root/reference/openwakeword/train.py:56-83,144-165).  heads_tc.cu gives each (128 streams,
-// head) pair its own CTA: with 7 head networks every CTA converts the same fp32 feature window to fp16 hi/lo again and
-// pulls a whole first-layer matrix through shared memory for 128 streams - 653 MB of L2 -> SM traffic per step at 8192
-// streams, 0.32 ms.  Here
-//   * the feature rings have an fp16 hi/lo MIRROR in HBM, already in the no-swizzle K-major UMMA core-matrix order and
+// Same graphs as heads.cu / heads_tc.cu (reference: <head>.onnx sessions, openwakeword/model.py:137-138,153-159,287-302
+// of the original project; family openwakeword/train.py:56-83,144-165).  heads_tc.cu converts the fp32 feature window to
+// fp16 hi/lo again in every CTA.  Here
+//   * the feature rings have an fp16 hi/lo MIRROR in HBM, already in the no-swizzle K-major core-matrix order and
 //     addressed by a slot counter shared by all streams ([slot][tile of 128 streams][K chunk of 32][hi|lo][4 octets]
 //     [128 rows][8 halves]): the A operand of (tile, feature row, chunk) is one contiguous 16 KB block that arrives by
-//     ONE cp.async.bulk - no converter warps.  feat16_sync_kernel appends the rows each step added (and rewrites the
-//     window of a stream that was reset) from the fp32 ring, which stays the state the API reads;
-//   * heads with the same n_in form a group whose first-layer matrices are packed side by side along N
-//     ([feature row][chunk][hi|lo][4 octets][N_tot][8 halves], each head pre-scaled by its own 2^s): one A block feeds
-//     every head of the group with N <= 256 per MMA, the accumulators of all heads sit side by side in TMEM
-//     (N_tot <= 512 columns);
-//   * the later layers run as small GEMMs per head, in place on that head's TMEM columns: 16 epilogue warps in up to
-//     four teams (one TMEM lane quarter per warp) read the accumulator rows three times from TMEM (sum, centred
-//     squares, normalise: same fp32 arithmetic order as heads.cu), split to fp16 hi/lo and hand the A tile of the next
-//     GEMM to the MMA warp; each team owns one activation buffer and one weight slot and walks its heads in turn.
+//     ONE cp.async.bulk - no converter warps.  feat16_sync_kernel appends the rows each step added (and rewrites the window of a
+//     stream that was reset) from the fp32 ring, which stays the state the API reads;
+//   * a CTA owns a tile of 128 streams and one head: two warpgroups (64 streams each) accumulate the first layer in
+//     registers (N = the head's widest layer, <= 128) while the producer warp streams A chunks and first-layer weight
+//     blocks through a ring; the later layers and the store are heads_mma.cuh.
 // Three MMA terms per K step (hi*hi + lo*hi + hi*lo, fp32 accumulate), as in heads_tc.cu.
 #include "oww_internal.h"
-#include "tc_common.cuh"
+#include "heads_mma.cuh"
 #include <algorithm>
 #include <cmath>
 #include <cstring>
 
 namespace {
 
-constexpr int kHgEpiWarps = 16;
-constexpr int kHgThreads = (kHgEpiWarps + 2) * 32;   // 576: 16 epilogue warps, producer, MMA issuer
-constexpr int kHgTile = 128;
+constexpr int kHgThreads = 9 * 32;                    // two MMA warpgroups + producer warp
+constexpr int kHgTile = 128;                          // streams per mirror tile
 constexpr int kHgMaxStages = 6;
 constexpr int kHgChunkK = 32;                         // K per pipeline stage (4 octets)
-constexpr int kHgAPlane = 4 * kHgTile * 16;           // one hi or lo plane of an A chunk: 8 KB
+constexpr int kHgAPlane = 4 * kHgTile * 16;           // one hi or lo plane of a mirror A chunk: 8 KB
 constexpr int kHgABytes = 2 * kHgAPlane;              // hi + lo: 16 KB
 constexpr int kHgTileBytes = 3 * kHgABytes;           // one feature row of one tile: 48 KB
 constexpr int kHgSmem = 227 * 1024;
-constexpr int kHgMaxTeams = 4;
-constexpr int kHgRing0 = 1024 + kHgMaxTeams * 2 * 384 * 4;   // ring offset in shared memory: barriers, then the teams' parameter buffers
+constexpr int kHgRing0 = 1024;                        // ring offset in shared memory (barriers below)
 
-__device__ __forceinline__ bool hg_elect_one() {
-    uint32_t pred;
-    asm volatile("{\n\t.reg .pred p;\n\telect.sync _|p, 0xffffffff;\n\tselp.u32 %0, 1, 0, p;\n\t}" : "=r"(pred));
-    return pred != 0;
-}
 __device__ __forceinline__ void hg_warp_wait(uint32_t bar, uint32_t parity, int lane) {
     if (lane == 0) mbar_wait(bar, parity);
     __syncwarp();
 }
-// long waits (the epilogue teams during the first-layer mainloop): poll every ~0.25 us instead of spinning - sixteen
-// spinning lanes keep the barrier unit busy and slow the producer's and the MMA warp's own barrier traffic down
-__device__ __forceinline__ void hg_warp_wait_idle(uint32_t bar, uint32_t parity, int lane) {
-    if (lane == 0) {
-        uint32_t spins = 0;
-        while (!mbar_try_wait(bar, parity)) {
-            __nanosleep(256);
-            if (++spins > (1u << 22)) __trap();
-        }
-    }
-    __syncwarp();
-}
-__device__ __forceinline__ void hg_split8(const float* x, uint4& hi, uint4& lo) {
-    __half2 h[4], l[4];
-#pragma unroll
-    for (int e = 0; e < 4; ++e) {
-        const __half h0 = __float2half_rn(x[2 * e]), h1 = __float2half_rn(x[2 * e + 1]);
-        h[e] = __halves2half2(h0, h1);
-        l[e] = __floats2half2_rn(x[2 * e] - __half2float(h0), x[2 * e + 1] - __half2float(h1));
-    }
-    hi = *reinterpret_cast<uint4*>(h);
-    lo = *reinterpret_cast<uint4*>(l);
-}
+__device__ __forceinline__ void hg_split8(const float* x, uint4& hi, uint4& lo) { hm_split8(x, hi, lo); }
 
 // ---------------------------------------------------------------- fp16 mirror of the feature rings
 // Rows count[b]-1-k (k = 0..depth-1) of stream b's fp32 ring -> slots (pos - k) mod NS of the mirror (zeros where the
@@ -128,22 +92,18 @@ __global__ void __launch_bounds__(256) feat16_linear_kernel(const float* __restr
 }
 
 // ---------------------------------------------------------------- kernel arguments
-struct HgLayer { int K, D, Kp, NP; uint32_t w_off, w_bytes; float unscale; };
+using HgLayer = HmLayer;
 struct HgHead {
     HeadDev dev;                    // fp32 blob: biases, LayerNorm parameters
     const uint8_t* w;               // per-head packed fp16 hi/lo weights (layers >= 1 are read from here)
     HgLayer L[OWW_MAX_HEAD_LAYERS];
-    int col;                        // first TMEM column of this head's accumulators
 };
-struct HgGroup {
-    int n_heads, n_in, n_tot, tmem_cols;
-    int head[8];                    // indices into HeadsGrpArgs::head
+struct HgGroup {                    // one head on the mirror
+    int head, n_in, n_tot;          // index into HeadsGrpArgs::head; window rows; first-layer N (the head's widest layer)
     const uint8_t* w0;              // [n_in][3][hi|lo][4][n_tot][8] halves
     uint32_t w0_bytes;              // one (feature row, chunk) block, hi + lo
     int stages; uint32_t stage_bytes;
     int cpr;                        // K chunks of 32 per pipeline stage: 3 (a whole feature row) when two such stages fit, else 1
-    int teams; uint32_t a_bytes, wn_bytes;   // later layers: per-team activation tile (hi + lo) and weight slot
-    int max_units;                  // most later-layer GEMMs any team issues
 };
 struct HeadsGrpArgs {
     HgHead head[16];
@@ -151,19 +111,8 @@ struct HeadsGrpArgs {
     const uint8_t* f16; int n_tiles, NS, slot_end;     // slot_end: mirror slot of the newest row of the window
     int steps;                      // > 0: bulk clips, blockIdx.z = step: window ends at slot_end + z, output row = clip * steps + z
     int n; float* out; int out_stride, combine_max, n_terms;
-    long long* dbg;                 // [8 per group] clock64 stamps of tile 0's CTA (oww_debug_heads_clocks)
+    long long* dbg;                 // [8 per group] clock64 stamps of CTA 0 (oww_debug_heads_clocks)
 };
-
-// unit r of team t: which head (index within the group) and which layer (1..nl-1)?
-__device__ __forceinline__ bool hg_unit(const HeadsGrpArgs& a, const HgGroup& G, int t, int r, int& hi, int& l) {
-    int u = 0;
-    for (hi = t; hi < G.n_heads; hi += G.teams) {
-        const int nu = a.head[G.head[hi]].dev.n_layers - 1;
-        if (r < u + nu) { l = 1 + r - u; return true; }
-        u += nu;
-    }
-    return false;
-}
 
 __global__ void __launch_bounds__(kHgThreads, 1) heads_grp_kernel(const __grid_constant__ HeadsGrpArgs a) {
     extern __shared__ __align__(128) uint8_t smem[];
@@ -171,54 +120,38 @@ __global__ void __launch_bounds__(kHgThreads, 1) heads_grp_kernel(const __grid_c
     const int tile = blockIdx.x, s0 = tile * kHgTile;
     const int S = G.stages;
     uint64_t* bars = reinterpret_cast<uint64_t*>(smem);
-    uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(smem + 512);
     uint8_t* ring = smem + kHgRing0;
     const int warp = __shfl_sync(0xffffffffu, (int)(threadIdx.x >> 5), 0);
     const int lane = threadIdx.x & 31;
     const uint32_t bar0 = smem_u32(bars);
     auto full = [&](int s) { return bar0 + 8u * s; };
     auto empty = [&](int s) { return bar0 + 8u * (kHgMaxStages + s); };
-    const uint32_t acc0_full = bar0 + 8u * (2 * kHgMaxStages);
-    auto an_full = [&](int t) { return bar0 + 8u * (2 * kHgMaxStages + 1 + t); };
-    auto wn_full = [&](int t) { return bar0 + 8u * (2 * kHgMaxStages + 1 + kHgMaxTeams + t); };
-    auto acc_done = [&](int t) { return bar0 + 8u * (2 * kHgMaxStages + 1 + 2 * kHgMaxTeams + t); };
-    // after the first-layer mainloop the ring is dead: team t's activation tile (a_bytes) and weight slot (wn_bytes) live
-    // in it at t * (a_bytes + wn_bytes)
-
+    const uint32_t acc_done = bar0 + 8u * (2 * kHgMaxStages);          // a GEMM's operands have been read (one arrival per MMA warp)
+    const uint32_t wn_full = acc_done + 8u;
     if (threadIdx.x == 0) {
-        for (int s = 0; s < kHgMaxStages; ++s) { mbar_init(full(s), 1); mbar_init(empty(s), 1); }
-        mbar_init(acc0_full, 1);
-        for (int t = 0; t < kHgMaxTeams; ++t) { mbar_init(an_full(t), 4); mbar_init(wn_full(t), 1); mbar_init(acc_done(t), 1); }
+        for (int s = 0; s < kHgMaxStages; ++s) { mbar_init(full(s), 1); mbar_init(empty(s), 8); }
+        mbar_init(acc_done, 8);
+        mbar_init(wn_full, 1);
         asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
     }
-    if (warp == kHgEpiWarps + 1) {
-        asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(tmem_slot)), "r"(G.tmem_cols));
-        asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;");
-    }
-    tc_fence_before();
     __syncthreads();
-    tc_fence_after();
-    const uint32_t tmem_base = __shfl_sync(0xffffffffu, *tmem_slot, 0);
-    const uint32_t desc_hi = (uint32_t)(make_desc(0, 0u, 128u) >> 32);                 // SBO + version
     const bool split = a.n_terms >= 3;
     const int cpr = G.cpr;
-    const int n_it = G.n_in * 3 / cpr;
+    const int n_in = G.n_in, n_tot = G.n_tot, n_terms = a.n_terms;
+    const int n_it = n_in * 3 / cpr;
+    const HgHead& HH = a.head[G.head];
+    const uint32_t stage_bytes = G.stage_bytes, w0_bytes = G.w0_bytes;
+    const uint32_t ring_u = smem_u32(ring);
+    // after the first-layer mainloop the ring is dead: per warpgroup hidden rows | next A tile, then the later-layer weight slot
+    const uint32_t w_next = ring_u + 2 * kHmBufBytes;
     long long* dbg = (a.dbg && blockIdx.x == 0) ? a.dbg + 8 * blockIdx.y : nullptr;
     if (dbg && threadIdx.x == 0) dbg[0] = clock64();
-    pdl_trigger();              // dependent launch chain of a step (tc_common.cuh): barriers and TMEM are set up, now the
+    pdl_trigger();              // dependent launch chain of a step (tc_common.cuh): barriers are set up, now the
     pdl_wait();                 // predecessor's feature rows are needed
 
-    // Everything the loops below need is copied into registers first: `a` lives in constant memory and is addressed with
-    // a run-time index (blockIdx.y), and the asm statements around the barriers are memory clobbers, so a G.field inside
-    // a loop is a fresh indexed constant load (~100 cycles on the uniform path) every time it is touched.
-    const int n_tot = G.n_tot, n_in = G.n_in, teams = G.teams, max_units = G.max_units, n_terms = a.n_terms;
-    const uint32_t stage_bytes = G.stage_bytes, w0_bytes = G.w0_bytes, ga_bytes = G.a_bytes, gw_bytes = G.wn_bytes;
-    const uint32_t ring_u = smem_u32(ring);
-
-    if (warp == kHgEpiWarps) {
+    if (warp == 8) {
         // ===================== producer =====================
         if (lane == 0) {
-            const uint32_t a_bytes = split ? kHgABytes : kHgAPlane, w_bytes = split ? w0_bytes : w0_bytes / 2;
             const int NS = a.NS, n_tiles = a.n_tiles;
             int slot = (a.slot_end + (a.steps > 0 ? (int)blockIdx.z : 0) - n_in + 1) % NS;
             if (slot < 0) slot += NS;
@@ -227,20 +160,15 @@ __global__ void __launch_bounds__(kHgThreads, 1) heads_grp_kernel(const __grid_c
             const int64_t slot_pitch = (int64_t)n_tiles * kHgTileBytes;
             uint32_t stage = 0, par = 1, st = ring_u;
             const uint32_t a_off = (uint32_t)cpr * kHgABytes;            // stage: cpr A chunks (hi|lo each), then cpr W blocks
+            const uint32_t a_bytes = split ? kHgABytes : kHgAPlane, w_bytes = split ? w0_bytes : w0_bytes / 2;
             for (int c = 0; c < n_in; ++c) {
                 const uint8_t* arow = f16 + (int64_t)slot * slot_pitch;
                 for (int q = 0; q < 3; q += cpr) {
                     mbar_wait(empty(stage), par);
-                    if (split) {
-                        mbar_expect_tx(full(stage), (uint32_t)cpr * (kHgABytes + w0_bytes));
-                        bulk_g2s(st, arow + q * kHgABytes, (uint32_t)cpr * kHgABytes, full(stage));
-                        bulk_g2s(st + a_off, w0, (uint32_t)cpr * w0_bytes, full(stage));
-                    } else {                                                 // plain fp16 operands: the hi planes only
-                        mbar_expect_tx(full(stage), (uint32_t)cpr * (a_bytes + w_bytes));
-                        for (int k = 0; k < cpr; ++k) {
-                            bulk_g2s(st + k * kHgABytes, arow + (q + k) * kHgABytes, a_bytes, full(stage));
-                            bulk_g2s(st + a_off + k * w0_bytes, w0 + (size_t)k * w0_bytes, w_bytes, full(stage));
-                        }
+                    mbar_expect_tx(full(stage), (uint32_t)cpr * (a_bytes + w_bytes));
+                    for (int k = 0; k < cpr; ++k) {                      // plain fp16 operands: the hi planes only
+                        bulk_g2s(st + k * kHgABytes, arow + (q + k) * kHgABytes, a_bytes, full(stage));
+                        bulk_g2s(st + a_off + k * w0_bytes, w0 + (size_t)k * w0_bytes, w_bytes, full(stage));
                     }
                     w0 += (size_t)cpr * w0_bytes;
                     st += stage_bytes;
@@ -249,245 +177,59 @@ __global__ void __launch_bounds__(kHgThreads, 1) heads_grp_kernel(const __grid_c
                 if (++slot == NS) slot = 0;
             }
             if (dbg) dbg[1] = clock64();
-            for (int r = 0; r < max_units; ++r)
-                for (int t = 0; t < teams; ++t) {
-                    int hi, l;
-                    if (!hg_unit(a, G, t, r, hi, l)) continue;
-                    // the slot is free once the ring is dead (first unit) / the team's previous GEMM has completed
-                    if (r == 0) mbar_wait(acc0_full, 0); else mbar_wait(acc_done(t), (uint32_t)((r - 1) & 1));
-                    const HgHead& HH = a.head[G.head[hi]];
-                    const uint32_t lw = HH.L[l].w_bytes;
-                    const uint32_t wb = split ? lw : lw / 2;
-                    mbar_expect_tx(wn_full(t), wb);
-                    bulk_g2s(ring_u + (uint32_t)t * (ga_bytes + gw_bytes) + ga_bytes, HH.w + HH.L[l].w_off, wb, wn_full(t));
-                }
+            for (int l = 1; l < HH.dev.n_layers; ++l) {                  // later layers: the whole matrix, once the slot is free
+                mbar_wait(acc_done, (uint32_t)((l - 1) & 1));
+                const uint32_t wb = split ? HH.L[l].w_bytes : HH.L[l].w_bytes / 2;
+                mbar_expect_tx(wn_full, wb);
+                bulk_g2s(w_next, HH.w + HH.L[l].w_off, wb, wn_full);
+            }
         }
-    } else if (warp == kHgEpiWarps + 1) {
-        // ===================== MMA issuer =====================
-        {   // ---- first layer of every head of the group: A chunk x [W_0 | W_1 | ...] ----
-            const uint32_t a_lo_fields = (uint32_t)make_desc(0, (uint32_t)(kHgTile * 16), 128u);
-            const uint32_t b_lo_fields = (uint32_t)make_desc(0, (uint32_t)n_tot * 16u, 128u);
-            const uint32_t w_plane = (uint32_t)n_tot * 64u;                         // 4 octets x n_tot rows x 16 B
-            // N in at most two pieces of <= 256 columns
-            const int np0 = n_tot < 256 ? n_tot : 256, np1 = n_tot - np0;
-            const uint32_t idesc0 = (1u << 4) | ((uint32_t)(np0 >> 3) << 17) | ((uint32_t)(128 >> 4) << 24);
-            const uint32_t idesc1 = (1u << 4) | ((uint32_t)(np1 >> 3) << 17) | ((uint32_t)(128 >> 4) << 24);
-            const uint64_t dhi = (uint64_t)desc_hi << 32;
+    } else {
+        // ===================== MMA warpgroups (streams 64 wg ..): first layer over the ring, later layers, store =====================
+        const int wg = warp >> 2;
+        float acc[64];
+        const uint32_t w_plane = (uint32_t)n_tot * 64u;                  // 4 octets x n_tot rows x 16 B
+        // N, the chunks per stage and the term count as compile-time constants: one unrolled chain of MMAs per stage
+        wg_dispatch_n(n_tot, [&](auto nc) { dispatch_int<3, 1>(cpr, [&](auto cc) { dispatch_int<3, 1>(n_terms, [&](auto tc) {
+            constexpr int NN = decltype(nc)::value, CPR = decltype(cc)::value, PER_CHUNK = 2 * decltype(tc)::value;
+            float d[NN / 2];                                             // this chain's own registers (no aliasing with other N)
             uint32_t stage = 0, par = 0, st = ring_u;
             for (int it = 0; it < n_it; ++it) {
                 hg_warp_wait(full(stage), par, lane);
-                tc_fence_after();
-                if (hg_elect_one()) {
-                    for (int k = 0; k < cpr; ++k) {
-                        const uint32_t ab = st + (uint32_t)k * kHgABytes, wb = st + (uint32_t)cpr * kHgABytes + (uint32_t)k * w0_bytes;
+                wg_fence();
 #pragma unroll
-                        for (int t = 0; t < 3; ++t) {
-                            if (t >= n_terms) break;
-                            const uint32_t au = (ab + (t == 1 ? kHgAPlane : 0)) >> 4;             // term 1 = x_lo * w_hi
-                            const uint32_t wu = (wb + (t == 2 ? w_plane : 0u)) >> 4;              // term 2 = x_hi * w_lo
-#pragma unroll
-                            for (int ks = 0; ks < 2; ++ks) {
-                                const uint64_t ad = dhi | a_lo_fields | ((au + (uint32_t)(2 * ks) * (kHgTile * 16 >> 4)) & 0x3FFFu);
-                                const uint32_t wk = wu + (uint32_t)(2 * ks) * (uint32_t)n_tot;
-                                const uint32_t accumulate = (it | k | t | ks) != 0;      // the very first K step overwrites
-                                tc_mma_f16(tmem_base, ad, dhi | b_lo_fields | (wk & 0x3FFFu), idesc0, accumulate);
-                                if (np1) tc_mma_f16(tmem_base + 256u, ad, dhi | b_lo_fields | ((wk + 256u) & 0x3FFFu), idesc1, accumulate);
-                            }
-                        }
-                    }
-                    tc_commit(empty(stage));
-                    if (it == n_it - 1) tc_commit(acc0_full);
+                for (int s = 0; s < CPR * PER_CHUNK; ++s) {
+                    const int k = s / PER_CHUNK, r = s - k * PER_CHUNK, t = r >> 1, ks = r & 1;
+                    const uint32_t ab = st + (uint32_t)k * kHgABytes + (uint32_t)wg * kHmAPlane, wb = st + (uint32_t)cpr * kHgABytes + (uint32_t)k * w0_bytes;
+                    const uint32_t au = ab + (t == 1 ? (uint32_t)kHgAPlane : 0u);         // term 1 = x_lo * w_hi
+                    const uint32_t wu = wb + (t == 2 ? w_plane : 0u);                     // term 2 = x_hi * w_lo
+                    const uint64_t ad = make_desc(au + (uint32_t)(2 * ks) * (kHgTile * 16), kHgTile * 16, 128u);
+                    const uint64_t bd = make_desc(wu + (uint32_t)(2 * ks) * (uint32_t)NN * 16u, (uint32_t)NN * 16u, 128u);
+                    wg_mma<NN>(d, ad, bd, (it | s) != 0);                               // the very first K step overwrites
                 }
+                wg_commit();
+                wg_wait_all();
                 __syncwarp();
+                if (lane == 0) mbar_arrive(empty(stage));
                 st += stage_bytes;
                 if (++stage == (uint32_t)S) { stage = 0; par ^= 1u; st = ring_u; }
             }
-            if (dbg && lane == 0) dbg[2] = clock64();
+#pragma unroll
+            for (int k = 0; k < NN / 2; ++k) acc[k] = d[k];
+        }); }); });
+        __syncwarp();
+        if (lane == 0) mbar_arrive(acc_done);
+        if (dbg && threadIdx.x == 0) dbg[2] = clock64();
+        const int r = threadIdx.x & 127, sr = s0 + wg * kHmRows + r;
+        float* o = nullptr;
+        if (r < kHmRows && sr < a.n) {
+            const int64_t orow = a.steps > 0 ? (int64_t)sr * a.steps + blockIdx.z : (int64_t)sr;
+            o = a.out + orow * a.out_stride + HH.dev.col0;
         }
-        // ---- later layers: one small GEMM per (head, layer), in place on the head's TMEM columns ----
-        for (int r = 0; r < max_units; ++r)
-            for (int t = 0; t < teams; ++t) {
-                int hi, l;
-                if (!hg_unit(a, G, t, r, hi, l)) continue;
-                const HgHead& HH = a.head[G.head[hi]];
-                const int NP = HH.L[l].NP, Kp = HH.L[l].Kp;
-                const uint32_t lw = HH.L[l].w_bytes;
-                const uint32_t d_tmem = tmem_base + (uint32_t)HH.col;
-                hg_warp_wait(an_full(t), (uint32_t)(r & 1), lane);
-                hg_warp_wait(wn_full(t), (uint32_t)(r & 1), lane);
-                tc_fence_after();
-                if (dbg && blockIdx.y == 0 && t == 0 && lane == 0 && r < 6) dbg[16 + 8 * r + 2] = clock64();
-                const uint32_t idesc = (1u << 4) | ((uint32_t)(NP >> 3) << 17) | ((uint32_t)(128 >> 4) << 24);
-                const uint32_t a_lo_fields = (uint32_t)make_desc(0, (uint32_t)(kHgTile * 16), 128u);
-                const uint32_t b_lo_fields = (uint32_t)make_desc(0, (uint32_t)NP * 16u, 128u);
-                const uint32_t an = ring_u + (uint32_t)t * (ga_bytes + gw_bytes), wn = an + ga_bytes;
-                const uint32_t a_unit[2] = {an >> 4, (an + ga_bytes / 2) >> 4};
-                const uint32_t w_unit[2] = {wn >> 4, (wn + lw / 2) >> 4};
-                const uint64_t dhi = (uint64_t)desc_hi << 32;
-                if (hg_elect_one()) {
-                    uint32_t accumulate = 0;
-                    for (int tm = 0; tm < n_terms; ++tm) {
-                        const uint32_t au = a_unit[tm == 1 ? 1 : 0], wu = w_unit[tm == 2 ? 1 : 0];
-                        for (int q = 0; q < Kp / 16; ++q) {
-                            const uint32_t alo = a_lo_fields | ((au + (uint32_t)(2 * q) * (kHgTile * 16 >> 4)) & 0x3FFFu);
-                            const uint32_t blo = b_lo_fields | ((wu + (uint32_t)(2 * q * NP)) & 0x3FFFu);
-                            tc_mma_f16(d_tmem, dhi | alo, dhi | blo, idesc, accumulate);
-                            accumulate = 1;
-                        }
-                    }
-                    tc_commit(acc_done(t));
-                    if (dbg && blockIdx.y == 0 && t == 0 && r < 6) dbg[16 + 8 * r + 3] = clock64();
-                }
-                __syncwarp();
-            }
-    } else if ((warp >> 2) < teams) {
-        // ===================== epilogue teams: warp = 4 * team + TMEM lane quarter =====================
-        const int team = warp >> 2, quarter = warp & 3;
-        const int r = quarter * 32 + lane;                                   // row of the tile = TMEM lane
-        const uint32_t trow = tmem_base + ((uint32_t)(quarter * 32) << 16);
-        uint8_t* const A = ring + (size_t)team * (ga_bytes + gw_bytes);      // this team's activation tile
-        const int n_heads = G.n_heads;
-        float* const prm = reinterpret_cast<float*>(smem + 1024) + team * 768; // bias | gamma | beta of the layer in hand, x 2 buffers
-        int unit = 0, n_staged = 0;                                          // GEMMs requested / parameter sets staged so far
-        for (int hi = team; hi < n_heads; hi += teams) {
-            const HgHead& HH = a.head[G.head[hi]];
-            const int nl = HH.dev.n_layers, layernorm = HH.dev.layernorm, final_act = HH.dev.final_act;
-            const float* blob = HH.dev.blob;
-            const uint32_t tcol = trow + (uint32_t)HH.col;
-            for (int l = 0; l < nl; ++l) {
-                const int D = HH.L[l].D, NP = HH.L[l].NP;
-                const float us = HH.L[l].unscale;
-                const bool last = l == nl - 1;
-                // bias [gamma, beta] of this layer -> the team's parameter buffer, zero beyond D (two buffers: a warp that
-                // runs ahead fills the other one while its team mates still read).  Done before the wait: it overlaps the GEMM.
-                float* P = prm + (n_staged & 1) * 384;
-                {
-                    const float* bias = blob + HH.dev.b_off[l];
-                    P[r] = r < D ? __ldg(bias + r) : 0.f;
-                    if (!last && layernorm) {
-                        P[128 + r] = r < D ? __ldg(blob + HH.dev.g_off[l] + r) : 0.f;
-                        P[256 + r] = r < D ? __ldg(blob + HH.dev.h_off[l] + r) : 0.f;
-                    }
-                    asm volatile("bar.sync %0, 128;" ::"r"(1 + team) : "memory");
-                    ++n_staged;
-                }
-                // accumulators of layer l: the first-layer mainloop (l == 0) or this team's latest GEMM
-                if (l == 0) hg_warp_wait_idle(acc0_full, 0, lane); else hg_warp_wait(acc_done(team), (uint32_t)((unit - 1) & 1), lane);
-                tc_fence_after();
-                if (dbg && warp == 0 && lane == 0 && hi == 0 && l == 0) dbg[3] = clock64();
-                if (dbg && blockIdx.y == 0 && warp == 0 && lane == 0 && unit < 6) dbg[16 + 8 * unit] = clock64();
-                // x[0..15] = accumulator columns c0.. of this thread's row * 2^-s + bias
-                auto chunk = [&](int c0, float* x) {
-                    uint32_t v[16];
-                    tmem_ld16(tcol + c0, v);
-                    const float4 b0 = *reinterpret_cast<const float4*>(P + c0), b1 = *reinterpret_cast<const float4*>(P + c0 + 4),
-                                 b2 = *reinterpret_cast<const float4*>(P + c0 + 8), b3 = *reinterpret_cast<const float4*>(P + c0 + 12);
-                    const float b[16] = {b0.x, b0.y, b0.z, b0.w, b1.x, b1.y, b1.z, b1.w, b2.x, b2.y, b2.z, b2.w, b3.x, b3.y, b3.z, b3.w};
-                    tmem_wait_ld();
-#pragma unroll
-                    for (int e = 0; e < 16; ++e) x[e] = fmaf(__uint_as_float(v[e]), us, b[e]);
-                };
-                if (last) {
-                    // ---- last layer: final activation + store ----
-                    const int n_out = D;
-                    const bool live = s0 + r < a.n;
-                    const int64_t orow = a.steps > 0 ? (int64_t)(s0 + r) * a.steps + blockIdx.z : (int64_t)(s0 + r);
-                    float* o = a.out + orow * a.out_stride + HH.dev.col0;
-                    const int combine_max = a.combine_max;
-                    float m = -INFINITY, sum = 0.f;
-                    const bool soft = final_act == 2 || final_act == 3;
-                    const bool relu = final_act == 3 || final_act == 4;
-                    for (int pass = soft ? 0 : 2; pass < 3; ++pass) {
-                        for (int c0 = 0; c0 < NP; c0 += 16) {
-                            float x[16];
-                            chunk(c0, x);
-#pragma unroll
-                            for (int e = 0; e < 16; ++e) {
-                                const bool in = c0 + e < n_out;
-                                float y = relu ? fmaxf(x[e], 0.f) : x[e];
-                                if (pass == 0) { if (in) m = fmaxf(m, y); }
-                                else if (pass == 1) { if (in) sum += expf(y - m); }
-                                else {
-                                    if (soft) y = expf(y - m) / sum;
-                                    else if (final_act == 1) y = 1.0f / (1.0f + expf(-y));
-                                    if (in && live) o[c0 + e] = combine_max ? fmaxf(o[c0 + e], y) : y;
-                                }
-                            }
-                        }
-                    }
-                    tc_fence_before();
-                    break;
-                }
-                // ---- hidden layer: [LayerNorm] + ReLU in fp32 (heads.cu's arithmetic), then fp16 hi/lo A tile of layer l+1 ----
-                float mu = 0.f, rstd = 1.f;
-                if (layernorm) {
-                    float sum = 0.f;
-                    for (int c0 = 0; c0 < NP; c0 += 16) {
-                        float x[16];
-                        chunk(c0, x);
-                        if (c0 + 16 <= D) {
-#pragma unroll
-                            for (int e = 0; e < 16; ++e) sum += x[e];
-                        } else {
-#pragma unroll
-                            for (int e = 0; e < 16; ++e) if (c0 + e < D) sum += x[e];
-                        }
-                    }
-                    mu = sum / (float)D;
-                    float sq = 0.f;
-                    for (int c0 = 0; c0 < NP; c0 += 16) {
-                        float x[16];
-                        chunk(c0, x);
-                        if (c0 + 16 <= D) {
-#pragma unroll
-                            for (int e = 0; e < 16; ++e) { const float c = x[e] - mu; sq = fmaf(c, c, sq); }
-                        } else {
-#pragma unroll
-                            for (int e = 0; e < 16; ++e) if (c0 + e < D) { const float c = x[e] - mu; sq = fmaf(c, c, sq); }
-                        }
-                    }
-                    rstd = 1.0f / sqrtf(sq / (float)D + 1e-5f);
-                }
-                const int Kp = HH.L[l + 1].Kp;                 // = NP: both are D rounded up to 16
-                for (int c0 = 0; c0 < Kp; c0 += 16) {
-                    float x[16];
-                    chunk(c0, x);                              // columns >= D: accumulator 0 (zero weight columns) + bias 0
-                    if (layernorm) {
-                        const float4* g4 = reinterpret_cast<const float4*>(P + 128 + c0);
-                        const float4* h4 = reinterpret_cast<const float4*>(P + 256 + c0);
-                        const float4 ga = g4[0], gb = g4[1], gc = g4[2], gd = g4[3], ha = h4[0], hb4 = h4[1], hc = h4[2], hd = h4[3];
-                        const float g[16] = {ga.x, ga.y, ga.z, ga.w, gb.x, gb.y, gb.z, gb.w, gc.x, gc.y, gc.z, gc.w, gd.x, gd.y, gd.z, gd.w};
-                        const float h[16] = {ha.x, ha.y, ha.z, ha.w, hb4.x, hb4.y, hb4.z, hb4.w, hc.x, hc.y, hc.z, hc.w, hd.x, hd.y, hd.z, hd.w};
-#pragma unroll
-                        for (int e = 0; e < 16; ++e) x[e] = (x[e] - mu) * rstd * g[e] + h[e];    // zero gamma / beta beyond D
-                    }
-#pragma unroll
-                    for (int e = 0; e < 16; ++e) x[e] = fmaxf(x[e], 0.f);
-#pragma unroll
-                    for (int half = 0; half < 2; ++half) {
-                        uint4 hi4, lo4;
-                        hg_split8(x + 8 * half, hi4, lo4);
-                        const int off = ((c0 >> 3) + half) * (kHgTile * 16) + r * 16;
-                        *reinterpret_cast<uint4*>(A + off) = hi4;
-                        if (split) *reinterpret_cast<uint4*>(A + ga_bytes / 2 + off) = lo4;
-                    }
-                }
-                asm volatile("fence.proxy.async.shared::cta;" ::: "memory");       // generic-proxy stores -> visible to the tensor core
-                tc_fence_before();                                                 // the TMEM reads precede the in-place GEMM
-                __syncwarp();
-                if (lane == 0) mbar_arrive(an_full(team));
-                if (dbg && blockIdx.y == 0 && warp == 0 && lane == 0 && unit < 6) dbg[16 + 8 * unit + 1] = clock64();
-                ++unit;
-            }
-        }
-        if (dbg && warp == 0 && lane == 0) dbg[4] = clock64();
-    }
-    tc_fence_before();
-    __syncthreads();
-    if (dbg && threadIdx.x == 0) dbg[5] = clock64();
-    if (warp == kHgEpiWarps + 1) {
-        tc_fence_after();
-        asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "r"(G.tmem_cols));
+        named_bar_sync(3, 256);                                          // both warpgroups are done with the ring
+        hm_layers(acc, n_tot, HH.dev, HH.L, n_terms, ring + wg * kHmBufBytes, w_next, wn_full, acc_done, 1 + wg, o,
+                  a.combine_max);
+        if (dbg && threadIdx.x == 0) dbg[4] = clock64();
     }
 }
 
@@ -548,93 +290,64 @@ static int hg_build(oww_ctx* ctx) {
         const int cx = colw(x), cy = colw(y);
         return cx != cy ? cx > cy : x < y;
     });
-    std::vector<std::vector<int>> groups;
+    // one head per group: its first-layer accumulators fill the registers of the CTA's two MMA warpgroups (2 x 64 x <= 128)
     for (int i : cand) {
-        bool placed = false;
-        for (auto& G : groups) {
-            int tot = 0;
-            for (int j : G) tot += colw(j);
-            if (ctx->heads[G[0]].desc.n_in == ctx->heads[i].desc.n_in && tot + colw(i) <= 384 && G.size() < 8) { G.push_back(i); placed = true; break; }
-        }
-        if (!placed && groups.size() < 8) { groups.push_back({i}); placed = true; }
-    }
-    for (const auto& Gv : groups) {
+        if (g->n_groups >= 8) break;
         HgGroup& G = a.grp[g->n_groups];
         std::memset(&G, 0, sizeof(G));
-        G.n_heads = (int)Gv.size();
-        G.n_in = ctx->heads[Gv[0]].desc.n_in;
-        int col = 0, kp_max = 16, units_total = 0; uint32_t wn_max = 0;
-        for (int k = 0; k < G.n_heads; ++k) {
-            const int i = Gv[k];
-            const Head& h = ctx->heads[i];
-            HgHead& HH = a.head[i];
-            HeadDev& d = HH.dev;
-            d.blob = h.d_blob;
-            d.n_in = h.desc.n_in; d.n_layers = h.desc.n_layers; d.layernorm = h.desc.layernorm; d.final_act = h.desc.final_act;
-            for (int l = 0; l <= h.desc.n_layers; ++l) d.dims[l] = h.desc.dims[l];
-            for (int l = 0; l < h.desc.n_layers; ++l) {
-                d.w_off[l] = (int)h.w_off[l]; d.b_off[l] = (int)h.b_off[l];
-                d.g_off[l] = (int)h.g_off[l]; d.h_off[l] = (int)h.h_off[l];
-                const Head::TcLayer& T = h.tc_layers[l];
-                HH.L[l] = HgLayer{T.K, T.D, T.Kp, T.NP, T.w_off, T.w_bytes, T.unscale};
-                if (l >= 1) { kp_max = std::max(kp_max, T.Kp); wn_max = std::max(wn_max, T.w_bytes); }
-            }
-            d.col0 = h.col0;
-            HH.w = reinterpret_cast<const uint8_t*>(h.d_w1_tc);
-            HH.col = col;
-            G.head[k] = i;
-            col += colw(i);
-            units_total += h.desc.n_layers - 1;
+        const Head& h = ctx->heads[i];
+        G.head = i;
+        G.n_in = h.desc.n_in;
+        HgHead& HH = a.head[i];
+        HeadDev& d = HH.dev;
+        d.blob = h.d_blob;
+        d.n_in = h.desc.n_in; d.n_layers = h.desc.n_layers; d.layernorm = h.desc.layernorm; d.final_act = h.desc.final_act;
+        uint32_t wn_max = 0;
+        for (int l = 0; l <= h.desc.n_layers; ++l) d.dims[l] = h.desc.dims[l];
+        for (int l = 0; l < h.desc.n_layers; ++l) {
+            d.w_off[l] = (int)h.w_off[l]; d.b_off[l] = (int)h.b_off[l];
+            d.g_off[l] = (int)h.g_off[l]; d.h_off[l] = (int)h.h_off[l];
+            const Head::TcLayer& T = h.tc_layers[l];
+            HH.L[l] = HgLayer{T.K, T.D, T.Kp, T.NP, T.w_off, T.w_bytes, T.unscale};
+            if (l >= 1) wn_max = std::max(wn_max, T.w_bytes);
         }
-        G.n_tot = col;
-        G.tmem_cols = 32;
-        while (G.tmem_cols < G.n_tot) G.tmem_cols *= 2;
+        d.col0 = h.col0;
+        HH.w = reinterpret_cast<const uint8_t*>(h.d_w1_tc);
+        G.n_tot = colw(i);
         G.w0_bytes = (uint32_t)(2 * 4 * G.n_tot * 16);
-        // a stage carries a whole feature row (3 chunks: 18 MMAs per N piece between two barrier round trips) when two
-        // such stages fit, else one chunk
+        // a stage carries a whole feature row (3 chunks: 18 MMAs between two barrier round trips) when two such stages
+        // fit, else one chunk
         G.cpr = 2 * 3 * (kHgABytes + (int)G.w0_bytes) <= kHgSmem - kHgRing0 ? 3 : 1;
         G.stage_bytes = (uint32_t)(G.cpr * (kHgABytes + (int)G.w0_bytes));
         G.stages = std::min(kHgMaxStages, (kHgSmem - kHgRing0) / (int)G.stage_bytes);
-        G.a_bytes = (uint32_t)(2 * (kp_max / 8) * kHgTile * 16);
-        G.wn_bytes = (wn_max + 127u) & ~127u;
-        G.teams = std::min(kHgMaxTeams, G.n_heads);
-        while (G.teams > 1 && (size_t)G.teams * (G.a_bytes + G.wn_bytes) > (size_t)G.stages * G.stage_bytes) --G.teams;
-        const bool fits = G.stages >= 2 && (size_t)G.teams * (G.a_bytes + G.wn_bytes) <= (size_t)G.stages * G.stage_bytes;
-        if (!fits) continue;                                         // these heads stay with heads_tc.cu
-        for (int t = 0; t < G.teams; ++t) {
-            int u = 0;
-            for (int k = t; k < G.n_heads; k += G.teams) u += ctx->heads[Gv[k]].desc.n_layers - 1;
-            G.max_units = std::max(G.max_units, u);
-        }
-        // first-layer matrices side by side: [feature row][chunk][hi|lo][4 octets][n_tot][8]
+        const bool fits = G.stages >= 2 && 2 * (size_t)kHmBufBytes + ((wn_max + 127u) & ~127u) <= (size_t)(kHgSmem - kHgRing0);
+        if (!fits) continue;                                         // this head stays with heads_tc.cu
+        // first-layer matrix: [feature row][chunk][hi|lo][4 octets][n_tot][8]
         const size_t blk = (size_t)G.w0_bytes / 2;                   // halves per (row, chunk) block
         std::vector<__half> packed((size_t)G.n_in * 3 * blk, __float2half(0.f));
-        for (int k = 0; k < G.n_heads; ++k) {
-            const Head& h = ctx->heads[Gv[k]];
-            const int D = h.desc.dims[1], col0 = a.head[Gv[k]].col;
-            const float sc = 1.0f / h.tc_layers[0].unscale;
-            const float* w = h.tc_w0_host.data();
-            for (int c = 0; c < G.n_in; ++c)
-                for (int q = 0; q < 3; ++q) {
-                    __half* dst = packed.data() + ((size_t)c * 3 + q) * blk;
-                    for (int o = 0; o < 4; ++o)
-                        for (int n = 0; n < D; ++n)
-                            for (int e = 0; e < 8; ++e) {
-                                const int kk = c * 96 + q * kHgChunkK + o * 8 + e;
-                                const float v = w[(size_t)kk * D + n] * sc;
-                                const __half hi = __float2half_rn(v);
-                                const size_t at = ((size_t)o * G.n_tot + col0 + n) * 8 + e;
-                                dst[at] = hi;
-                                dst[at + blk / 2] = __float2half_rn(v - __half2float(hi));
-                            }
-                }
-        }
-        void* d = nullptr;
-        OWW_CUDA(ctx, cudaMalloc(&d, packed.size() * sizeof(__half)));
-        g->d_w0.push_back(d);
-        OWW_CUDA(ctx, cudaMemcpy(d, packed.data(), packed.size() * sizeof(__half), cudaMemcpyHostToDevice));
-        G.w0 = reinterpret_cast<const uint8_t*>(d);
-        for (int i : Gv) g->covered |= 1u << i;
+        const int D = h.desc.dims[1];
+        const float sc = 1.0f / h.tc_layers[0].unscale;
+        const float* w = h.tc_w0_host.data();
+        for (int c = 0; c < G.n_in; ++c)
+            for (int q = 0; q < 3; ++q) {
+                __half* dst = packed.data() + ((size_t)c * 3 + q) * blk;
+                for (int o = 0; o < 4; ++o)
+                    for (int n = 0; n < D; ++n)
+                        for (int e = 0; e < 8; ++e) {
+                            const int kk = c * 96 + q * kHgChunkK + o * 8 + e;
+                            const float v = w[(size_t)kk * D + n] * sc;
+                            const __half hi = __float2half_rn(v);
+                            const size_t at = ((size_t)o * G.n_tot + n) * 8 + e;
+                            dst[at] = hi;
+                            dst[at + blk / 2] = __float2half_rn(v - __half2float(hi));
+                        }
+            }
+        void* dw = nullptr;
+        OWW_CUDA(ctx, cudaMalloc(&dw, packed.size() * sizeof(__half)));
+        g->d_w0.push_back(dw);
+        OWW_CUDA(ctx, cudaMemcpy(dw, packed.data(), packed.size() * sizeof(__half), cudaMemcpyHostToDevice));
+        G.w0 = reinterpret_cast<const uint8_t*>(dw);
+        g->covered |= 1u << i;
         g->depth = std::max(g->depth, G.n_in);
         ++g->n_groups;
     }
@@ -655,7 +368,7 @@ static int hg_sync(oww_ctx* ctx, const int* d_ids, int n, int depth, cudaStream_
     oww_heads_grp* g = ctx->heads_grp;
     const int64_t total = (int64_t)n * 12 * depth;
     if (total <= 0) return OWW_OK;
-    const unsigned grid = (unsigned)std::min<int64_t>((total + 255) / 256, 148 * 16);
+    const unsigned grid = (unsigned)std::min<int64_t>((total + 255) / 256, (int64_t)ctx->sm_count * 16);
     OWW_CUDA(ctx, oww_launch_pdl(ctx->late_pdl, feat16_sync_kernel, dim3(grid), dim3(256), 0, s, (const float*)ctx->d_feat_ring,
                                  (int64_t)ctx->feat_rows * 96, ctx->feat_rows - 1, (const int*)ctx->d_feat_count, d_ids, n, depth,
                                  (int)(g->pos % g->NS), g->NS, g->n_tiles, g->d_f16));
@@ -742,7 +455,7 @@ uint32_t oww_heads_grp_bulk(oww_ctx* ctx, const FeatSrc& src, int n, float* d_ou
     if ((e = cudaMemsetAsync(g->d_f16_bulk, 0, bytes, s)) != cudaSuccess) return fail(e);
     {
         const int64_t total = (int64_t)m * 12 * n_rows;
-        const unsigned grid = (unsigned)std::min<int64_t>((total + 255) / 256, 148 * 32);
+        const unsigned grid = (unsigned)std::min<int64_t>((total + 255) / 256, (int64_t)ctx->sm_count * 32);
         feat16_linear_kernel<<<grid, 256, 0, s>>>(src.base, src.stride, m, n_rows, pad, n_tiles, g->d_f16_bulk);
         ctx->launches++;
     }
@@ -760,8 +473,8 @@ uint32_t oww_heads_grp_bulk(oww_ctx* ctx, const FeatSrc& src, int n, float* d_ou
     return g->covered;
 }
 
-// debug: clock64 stamps of the last grouped launch (tile 0 of each group): start, producer done, last first-layer MMA
-// issued, first-layer accumulators complete, team 0 done, CTA end.  First call arms the stamps.
+// debug: clock64 stamps of the last mirror-path launch (CTA 0 of each head): [0] start, [1] producer done, [2] first-layer
+// accumulators complete, [4] scores stored.  First call arms the stamps.
 extern "C" int oww_debug_heads_clocks(oww_ctx* ctx, int64_t* h_out64) {
     oww_heads_grp* g = ctx ? ctx->heads_grp : nullptr;
     if (!g) return OWW_EINVAL;

@@ -1,53 +1,46 @@
-// K3 (tensor-core path, per head): the wake-word heads as a chain of tcgen05 GEMMs, one CTA per (128 samples, head).
-// Streaming steps and bulk clips run heads_grp.cu (all heads of a window in one CTA, A operand from the fp16 mirror); this
-// kernel serves stateless calls on caller-supplied features and the heads no group covers.
+// K3 (tensor-core path, per head): the wake-word heads as a chain of wgmma GEMMs, one CTA per (64 samples, head).
+// Streaming steps and bulk clips run heads_grp.cu (A operand from the fp16 mirror of the feature rings); this kernel
+// serves stateless calls on caller-supplied features and the heads the mirror path does not cover.
 //
-// Same graphs as heads.cu (reference: <head>.onnx sessions, /root/reference/openwakeword/model.py:137-138,153-159,287-302;
-// family /root/reference/openwakeword/train.py:56-83,144-165).  heads.cu tiles 8 or 32 streams per CTA and streams the
-// first-layer matrix W1 (n_in*96 x D1, 0.4-1.7 MB) through shared memory once per tile: at 8192 streams x 6 heads that is
-// 0.78 ms per step, 7 % of its HBM roofline.  Here a CTA owns 128 streams of one head and every Linear layer is an MMA:
-//   layer 0:  D[128 x D1] (fp32, TMEM) = sum over the n_in feature rows c of  X_c[128 x 96] * W1_c[96 x D1]
-//             X_c is gathered from the per-stream feature rings (fp32) by 16 converter warps, split into fp16 hi + lo
-//             (x = hi + lo, |lo| <= ulp(hi)/2) and written to shared memory in the no-swizzle K-major UMMA core-matrix
-//             order ([k-octet][128 rows][16 B]; LBO = 2048 B, SBO = 128 B); W1_c is pre-packed on the host as fp16
+// Same graphs as heads.cu (reference: <head>.onnx sessions, openwakeword/model.py:137-138,153-159,287-302 of the
+// original project; family openwakeword/train.py:56-83,144-165).  heads.cu tiles 8 or 32 streams per CTA and runs every
+// layer on CUDA cores.  Here a CTA owns 64 streams of one head and every Linear layer is an MMA:
+//   layer 0:  D[64 x D1] (fp32, registers of one warpgroup) = sum over the n_in feature rows c of X_c[64 x 96] * W1_c[96 x D1]
+//             X_c is gathered from the per-stream feature rings (fp32) by 8 converter warps, split into fp16 hi + lo
+//             (x = hi + lo, |lo| <= ulp(hi)/2) and written to shared memory in the no-swizzle K-major core-matrix
+//             order ([k-octet][64 rows][16 B]; LBO = 1024 B, SBO = 128 B); W1_c is pre-packed on the host as fp16
 //             hi + lo of W * 2^s in the same order and arrives by one cp.async.bulk per feature row (3-stage ring).
-//   layer l:  the 128 accumulator rows come back with tcgen05.ld (one row per thread), get the exact 2^-s, the bias,
-//             [LayerNorm] and ReLU in fp32, are split into hi + lo again and become the A tile of the next GEMM
-//             (W_l pre-packed the same way, one bulk copy per layer, the two TMEM accumulators alternate).
+//   layer l:  heads_mma.cuh: the accumulators get the exact 2^-s, the bias, [LayerNorm] and ReLU in fp32, are split into
+//             hi + lo again and become the A tile of the next GEMM (W_l pre-packed the same way, one bulk copy per layer).
 // Three MMA terms per K step (hi*hi + lo*hi + hi*lo, fp32 accumulate) reproduce the fp32 product to ~2^-21 relative, so
 // the scores stay within a few 1e-5 of heads.cu / the oracle; n_terms = 1 is plain fp16 operands.  Sigmoid / softmax /
 // relu of the last layer and the store (with the max over chunk windows of a multi-chunk call) finish the CTA.
-// Warp roles: 0-15 converters (0-3 also epilogue: one TMEM lane quarter each), 16 = weight producer, 17 = TMEM owner +
-// MMA issuer.  Heads are launched heaviest first (blockIdx.y) so the long CTAs do not form the tail.
+// Warp roles: 0-3 MMA warpgroup + epilogue, 4 = weight producer, 5-12 converters.  Heads are launched heaviest first
+// (blockIdx.y) so the long CTAs do not form the tail.
 #include "oww_internal.h"
-#include "tc_common.cuh"
+#include "heads_mma.cuh"
 #include <algorithm>
 #include <cmath>
 #include <cstring>
 
 namespace {
 
-constexpr int kHtWorkers = 16;                       // converter warps
-constexpr int kHtThreads = (kHtWorkers + 2) * 32;    // 576
-constexpr int kHtTile = 128;                         // streams per CTA = MMA M
+constexpr int kHtWorkers = 8;                        // converter warps
+constexpr int kHtProducer = 4;                       // warp index of the weight producer
+constexpr int kHtThreads = (kHtProducer + 1 + kHtWorkers) * 32;   // 416
+constexpr int kHtTile = kHmRows;                     // streams per CTA = MMA M
 constexpr int kHtMaxStages = 3;
-constexpr int kHtAPlane = kHtTile * 16;              // bytes per k-octet plane of an A tile (LBO)
-constexpr int kHtABytes = 12 * kHtAPlane;            // one 128 x 96 fp16 tile: 24 KB
-constexpr int kHtHPitch = 129;                       // fp32 row pitch of the hidden-activation buffer (layers <= 128 wide)
+constexpr int kHtAPlane = kHmAPlane;                 // bytes per k-octet plane of an A tile (LBO)
+constexpr int kHtABytes = 12 * kHtAPlane;            // one 64 x 96 fp16 tile: 12 KB
 constexpr int kHtSmem = 227 * 1024;
 
-__device__ __forceinline__ bool ht_elect_one() {
-    uint32_t pred;
-    asm volatile("{\n\t.reg .pred p;\n\telect.sync _|p, 0xffffffff;\n\tselp.u32 %0, 1, 0, p;\n\t}" : "=r"(pred));
-    return pred != 0;
-}
-// one lane polls, the warp follows (512 polling threads would eat the issue slots the converters need)
+// one lane polls, the warp follows
 __device__ __forceinline__ void ht_warp_wait(uint32_t bar, uint32_t parity, int lane) {
     if (lane == 0) mbar_wait(bar, parity);
     __syncwarp();
 }
 
-struct HtLayer { int K, D, Kp, NP; uint32_t w_off, w_bytes; float unscale; };     // packed weights of one Linear layer
+using HtLayer = HmLayer;
 struct HtHead {
     HeadDev dev;                    // fp32 blob: biases, LayerNorm parameters
     const uint8_t* w;               // packed fp16 hi/lo weights of every layer
@@ -80,19 +73,6 @@ __device__ __forceinline__ HtRows ht_rows(const FeatSrc& src, int n_in, int s, i
     return w;
 }
 
-// eight fp32 values -> one 16-byte unit of fp16 hi parts and one of lo parts
-__device__ __forceinline__ void ht_split8(const float* x, uint4& hi, uint4& lo) {
-    __half2 h[4], l[4];
-#pragma unroll
-    for (int e = 0; e < 4; ++e) {
-        const __half h0 = __float2half_rn(x[2 * e]), h1 = __float2half_rn(x[2 * e + 1]);
-        h[e] = __halves2half2(h0, h1);
-        l[e] = __floats2half2_rn(x[2 * e] - __half2float(h0), x[2 * e + 1] - __half2float(h1));
-    }
-    hi = *reinterpret_cast<uint4*>(h);
-    lo = *reinterpret_cast<uint4*>(l);
-}
-
 __global__ void __launch_bounds__(kHtThreads, 1) heads_tc_kernel(const __grid_constant__ HeadsTcArgs a) {
     extern __shared__ __align__(128) uint8_t smem[];
     const HtHead& HH = a.head[blockIdx.y];
@@ -102,41 +82,28 @@ __global__ void __launch_bounds__(kHtThreads, 1) heads_tc_kernel(const __grid_co
     const int s0 = blockIdx.x * kHtTile;
     const int S = a.stages;
     uint64_t* bars = reinterpret_cast<uint64_t*>(smem);
-    uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(smem + 256);
     uint8_t* stage0 = smem + 1024;
     // after the mainloop the stage ring is dead and is reused as: hidden activations fp32 | next A tile (hi, lo) | W slot
-    float* hbuf = reinterpret_cast<float*>(stage0);                                     // [128][129] fp32, 66 048 B
-    uint8_t* a_next = stage0 + ((kHtTile * kHtHPitch * 4 + 127) & ~127);              // [hi | lo] x [Kp/8][128][16 B], <= 64 KB
-    uint8_t* w_next = a_next + 2 * 16 * kHtAPlane;                                     // [hi | lo] x [Kp/8][NP][16 B], <= 64 KB
+    uint8_t* w_next = stage0 + kHmBufBytes;                                  // [hi | lo] x [Kp/8][NP][16 B], <= 64 KB
     const int warp = __shfl_sync(0xffffffffu, (int)(threadIdx.x >> 5), 0);
     const int lane = threadIdx.x & 31;
     const uint32_t bar0 = smem_u32(bars);
     auto a_full = [&](int s) { return bar0 + 8u * s; };
     auto w_full = [&](int s) { return bar0 + 8u * (kHtMaxStages + s); };
     auto empty = [&](int s) { return bar0 + 8u * (2 * kHtMaxStages + s); };
-    const uint32_t acc_full = bar0 + 8u * (3 * kHtMaxStages);          // layer l's accumulators complete (phase = l & 1)
-    const uint32_t an_full = acc_full + 8u;                            // next A tile written by the 4 epilogue warps
-    const uint32_t wn_full = acc_full + 16u;                           // next layer's weights landed
+    const uint32_t acc_done = bar0 + 8u * (3 * kHtMaxStages);          // a GEMM's operands have been read (one arrival per MMA warp)
+    const uint32_t wn_full = acc_done + 8u;                            // next layer's weights landed
 
     if (threadIdx.x == 0) {
-        for (int s = 0; s < kHtMaxStages; ++s) { mbar_init(a_full(s), kHtWorkers); mbar_init(w_full(s), 1); mbar_init(empty(s), 1); }
-        mbar_init(acc_full, 1);
-        mbar_init(an_full, 4);
+        for (int s = 0; s < kHtMaxStages; ++s) { mbar_init(a_full(s), kHtWorkers); mbar_init(w_full(s), 1); mbar_init(empty(s), 4); }
+        mbar_init(acc_done, 4);
         mbar_init(wn_full, 1);
         asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
     }
-    if (warp == kHtWorkers + 1) {
-        asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(tmem_slot)), "r"(256));
-        asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;");
-    }
-    tc_fence_before();
     __syncthreads();
-    tc_fence_after();
-    const uint32_t tmem_base = __shfl_sync(0xffffffffu, *tmem_slot, 0);
     const uint32_t w_term_bytes = 12u * (uint32_t)NP * 16u;
-    const uint32_t desc_hi = (uint32_t)(make_desc(0, 0u, 128u) >> 32);                 // SBO + version
 
-    if (warp == kHtWorkers) {
+    if (warp == kHtProducer) {
         // ===================== weight producer =====================
         if (lane == 0) {
             const uint32_t bytes = w_term_bytes * (a.n_terms >= 3 ? 2u : 1u);
@@ -147,210 +114,100 @@ __global__ void __launch_bounds__(kHtThreads, 1) heads_tc_kernel(const __grid_co
                 bulk_g2s(smem_u32(stage0 + s * a.stage_bytes + 2 * kHtABytes), HH.w + (size_t)c * 2u * w_term_bytes, bytes, w_full(s));
             }
             for (int l = 1; l < n_layers; ++l) {                     // later layers: the whole matrix, once the slot is free
-                mbar_wait(acc_full, (uint32_t)((l - 1) & 1));        // layer l-1's MMAs are done: ring / previous W dead
+                mbar_wait(acc_done, (uint32_t)((l - 1) & 1));        // layer l-1's MMAs are done: ring / previous W dead
                 const uint32_t wb = a.n_terms >= 3 ? HH.L[l].w_bytes : HH.L[l].w_bytes / 2;
                 mbar_expect_tx(wn_full, wb);
                 bulk_g2s(smem_u32(w_next), HH.w + HH.L[l].w_off, wb, wn_full);
             }
         }
-    } else if (warp == kHtWorkers + 1) {
-        // ===================== MMA issuer =====================
-        {   // ---- layer 0 mainloop ----
-            const uint32_t idesc = (1u << 4) | ((uint32_t)(NP >> 3) << 17) | ((uint32_t)(128 >> 4) << 24);
-            const uint32_t a_lo_fields = (uint32_t)make_desc(0, (uint32_t)kHtAPlane, 128u);    // LBO in the low word
-            const uint32_t b_lo_fields = (uint32_t)make_desc(0, (uint32_t)NP * 16u, 128u);
-            uint32_t accumulate = 0;
+    } else if (warp < 4) {
+        // ===================== MMA warpgroup: layer 0 mainloop, then the later layers and the store =====================
+        float acc[64];
+        // N and the term count as compile-time constants: one unrolled chain of MMAs per feature row
+        wg_dispatch_n(NP, [&](auto nc) { dispatch_int<3, 1>(a.n_terms, [&](auto tc) {
+            constexpr int NN = decltype(nc)::value, NT = decltype(tc)::value;
+            float d[NN / 2];                                             // this chain's own registers (no aliasing with other N)
             for (int c = 0; c < n_in; ++c) {
                 const int s = c % S;
                 const uint32_t par = ((uint32_t)(c / S)) & 1u;
                 ht_warp_wait(a_full(s), par, lane);
                 ht_warp_wait(w_full(s), par, lane);
-                tc_fence_after();
                 const uint32_t st_addr = smem_u32(stage0 + s * a.stage_bytes);
-                const uint32_t a_unit[2] = {st_addr >> 4, (st_addr + kHtABytes) >> 4};
-                const uint32_t w_unit[2] = {(st_addr + 2 * kHtABytes) >> 4, (st_addr + 2 * kHtABytes + w_term_bytes) >> 4};
-                if (ht_elect_one()) {
-                    for (int t = 0; t < a.n_terms; ++t) {
-                        const uint32_t au = a_unit[t == 1 ? 1 : 0];       // term 1 = x_lo * w_hi
-                        const uint32_t wu = w_unit[t == 2 ? 1 : 0];       // term 2 = x_hi * w_lo
+                wg_fence();
 #pragma unroll
-                        for (int q = 0; q < 6; ++q) {
-                            const uint32_t alo = a_lo_fields | ((au + (uint32_t)(2 * q) * (kHtAPlane >> 4)) & 0x3FFFu);
-                            const uint32_t blo = b_lo_fields | ((wu + (uint32_t)(2 * q * NP)) & 0x3FFFu);
-                            tc_mma_f16(tmem_base, ((uint64_t)desc_hi << 32) | alo, ((uint64_t)desc_hi << 32) | blo, idesc, accumulate);
-                            accumulate = 1;
-                        }
-                    }
-                    tc_commit(empty(s));                                  // stage free once these MMAs have read it
-                    if (c == n_in - 1) tc_commit(acc_full);
+                for (int k = 0; k < NT * 6; ++k) {
+                    const int t = k / 6, q = k - t * 6;
+                    const uint32_t au = st_addr + (t == 1 ? (uint32_t)kHtABytes : 0u);                       // term 1 = x_lo * w_hi
+                    const uint32_t wu = st_addr + 2 * kHtABytes + (t == 2 ? w_term_bytes : 0u);             // term 2 = x_hi * w_lo
+                    const uint64_t ad = make_desc(au + (uint32_t)(2 * q) * kHtAPlane, kHtAPlane, 128u);
+                    const uint64_t bd = make_desc(wu + (uint32_t)(2 * q * NN) * 16u, (uint32_t)NN * 16u, 128u);
+                    wg_mma<NN>(d, ad, bd, (c | k) != 0);
                 }
+                wg_commit();
+                wg_wait_all();
                 __syncwarp();
+                if (lane == 0) mbar_arrive(empty(s));                     // stage free once these MMAs have read it
             }
-        }
-        // ---- later layers: one GEMM each, A = previous activations (hi/lo) written by the epilogue warps ----
-        for (int l = 1; l < n_layers; ++l) {
-            const HtLayer& L = HH.L[l];
-            ht_warp_wait(an_full, (uint32_t)((l - 1) & 1), lane);
-            ht_warp_wait(wn_full, (uint32_t)((l - 1) & 1), lane);
-            tc_fence_after();
-            const uint32_t idesc = (1u << 4) | ((uint32_t)(L.NP >> 3) << 17) | ((uint32_t)(128 >> 4) << 24);
-            const uint32_t a_lo_fields = (uint32_t)make_desc(0, (uint32_t)kHtAPlane, 128u);
-            const uint32_t b_lo_fields = (uint32_t)make_desc(0, (uint32_t)L.NP * 16u, 128u);
-            const uint32_t a_unit[2] = {smem_u32(a_next) >> 4, (smem_u32(a_next) + 16 * kHtAPlane) >> 4};
-            const uint32_t w_unit[2] = {smem_u32(w_next) >> 4, (smem_u32(w_next) + L.w_bytes / 2) >> 4};
-            const uint32_t d_tmem = tmem_base + (uint32_t)(l & 1) * 128u;
-            if (ht_elect_one()) {
-                uint32_t accumulate = 0;
-                for (int t = 0; t < a.n_terms; ++t) {
-                    const uint32_t au = a_unit[t == 1 ? 1 : 0], wu = w_unit[t == 2 ? 1 : 0];
-                    for (int q = 0; q < L.Kp / 16; ++q) {
-                        const uint32_t alo = a_lo_fields | ((au + (uint32_t)(2 * q) * (kHtAPlane >> 4)) & 0x3FFFu);
-                        const uint32_t blo = b_lo_fields | ((wu + (uint32_t)(2 * q * L.NP)) & 0x3FFFu);
-                        tc_mma_f16(d_tmem, ((uint64_t)desc_hi << 32) | alo, ((uint64_t)desc_hi << 32) | blo, idesc, accumulate);
-                        accumulate = 1;
-                    }
-                }
-                tc_commit(acc_full);
-            }
-            __syncwarp();
-        }
+#pragma unroll
+            for (int k = 0; k < NN / 2; ++k) acc[k] = d[k];
+        }); });
+        __syncwarp();
+        if (lane == 0) mbar_arrive(acc_done);
+        const int r = threadIdx.x;
+        float* o = (r < kHtTile && s0 + r < a.n) ? a.out + (int64_t)(s0 + r) * a.out_stride + H.col0 : nullptr;
+        // the ring is dead once every stage has been consumed by the MMAs above (all of this warpgroup's)
+        named_bar_sync(1, 128);
+        hm_layers(acc, NP, H, HH.L, a.n_terms, stage0, smem_u32(w_next), wn_full, acc_done, 1, o, a.combine_max);
     } else {
         // ===================== converters: fp32 ring rows -> fp16 hi/lo A tiles =====================
-        // thread = (row 8*warp + lane%8, octet quad lane/8): three octets (32 B of fp32 each) per feature row
-        const int row = 8 * warp + (lane & 7), jq = lane >> 3;
-        {
-            const int s = s0 + row;
-            float4 buf[2][6];
-            const HtRows rows_of = ht_rows(a.src, n_in, s, a.n);
-            auto load = [&](int c, float4* v) {
-                const float* p = nullptr;
-                if (c < n_in && rows_of.base) {
-                    const int r = rows_of.r0 + c;
-                    if (r >= 0) p = rows_of.base + (int64_t)(rows_of.mask >= 0 ? (r & rows_of.mask) : r) * 96;
-                }
+        // thread = (row 8*w + lane%8, octet quad lane/8): three octets (32 B of fp32 each) per feature row
+        const int row = 8 * (warp - kHtProducer - 1) + (lane & 7), jq = lane >> 3;
+        const int s = s0 + row;
+        float4 buf[2][6];
+        const HtRows rows_of = ht_rows(a.src, n_in, s, a.n);
+        auto load = [&](int c, float4* v) {
+            const float* p = nullptr;
+            if (c < n_in && rows_of.base) {
+                const int r = rows_of.r0 + c;
+                if (r >= 0) p = rows_of.base + (int64_t)(rows_of.mask >= 0 ? (r & rows_of.mask) : r) * 96;
+            }
 #pragma unroll
-                for (int i = 0; i < 3; ++i) {
-                    if (p) {
-                        const float4* q = reinterpret_cast<const float4*>(p + (4 * i + jq) * 8);
-                        v[2 * i] = __ldcg(q); v[2 * i + 1] = __ldcg(q + 1);
-                    } else {
-                        v[2 * i] = make_float4(0.f, 0.f, 0.f, 0.f); v[2 * i + 1] = v[2 * i];
-                    }
+            for (int i = 0; i < 3; ++i) {
+                if (p) {
+                    const float4* q = reinterpret_cast<const float4*>(p + (4 * i + jq) * 8);
+                    v[2 * i] = __ldcg(q); v[2 * i + 1] = __ldcg(q + 1);
+                } else {
+                    v[2 * i] = make_float4(0.f, 0.f, 0.f, 0.f); v[2 * i + 1] = v[2 * i];
                 }
-            };
-            auto convert_store = [&](int c, const float4* v) {
-                const int st = c % S;
-                ht_warp_wait(empty(st), (((uint32_t)(c / S)) & 1u) ^ 1u, lane);
-                uint8_t* A = stage0 + st * a.stage_bytes;
+            }
+        };
+        auto convert_store = [&](int c, const float4* v) {
+            const int st = c % S;
+            ht_warp_wait(empty(st), (((uint32_t)(c / S)) & 1u) ^ 1u, lane);
+            uint8_t* A = stage0 + st * a.stage_bytes;
 #pragma unroll
-                for (int i = 0; i < 3; ++i) {
-                    const float x[8] = {v[2 * i].x, v[2 * i].y, v[2 * i].z, v[2 * i].w, v[2 * i + 1].x, v[2 * i + 1].y, v[2 * i + 1].z, v[2 * i + 1].w};
-                    uint4 hi, lo;
-                    ht_split8(x, hi, lo);
-                    const int off = (4 * i + jq) * kHtAPlane + row * 16;
-                    *reinterpret_cast<uint4*>(A + off) = hi;
-                    if (a.n_terms >= 2) *reinterpret_cast<uint4*>(A + kHtABytes + off) = lo;
-                }
-                asm volatile("fence.proxy.async.shared::cta;" ::: "memory");       // generic-proxy stores -> visible to the tensor core
-                __syncwarp();
-                if (lane == 0) mbar_arrive(a_full(st));
-            };
-            load(0, buf[0]);
-            load(1, buf[1]);
-            for (int c = 0; c < n_in; c += 2) {
-                convert_store(c, buf[0]);
-                load(c + 2, buf[0]);
-                if (c + 1 < n_in) {
-                    convert_store(c + 1, buf[1]);
-                    load(c + 3, buf[1]);
-                }
+            for (int i = 0; i < 3; ++i) {
+                const float x[8] = {v[2 * i].x, v[2 * i].y, v[2 * i].z, v[2 * i].w, v[2 * i + 1].x, v[2 * i + 1].y, v[2 * i + 1].z, v[2 * i + 1].w};
+                uint4 hi, lo;
+                hm_split8(x, hi, lo);
+                const int off = (4 * i + jq) * kHtAPlane + row * 16;
+                *reinterpret_cast<uint4*>(A + off) = hi;
+                if (a.n_terms >= 2) *reinterpret_cast<uint4*>(A + kHtABytes + off) = lo;
+            }
+            asm volatile("fence.proxy.async.shared::cta;" ::: "memory");       // generic-proxy stores -> visible to the tensor core
+            __syncwarp();
+            if (lane == 0) mbar_arrive(a_full(st));
+        };
+        load(0, buf[0]);
+        load(1, buf[1]);
+        for (int c = 0; c < n_in; c += 2) {
+            convert_store(c, buf[0]);
+            load(c + 2, buf[0]);
+            if (c + 1 < n_in) {
+                convert_store(c + 1, buf[1]);
+                load(c + 3, buf[1]);
             }
         }
-        // ===================== epilogue (warps 0-3: one accumulator row per thread) =====================
-        if (warp < 4) {
-            const int r = warp * 32 + lane;                                  // row of the tile = TMEM lane
-            float* hrow = hbuf + r * kHtHPitch;
-            for (int l = 0; l < n_layers; ++l) {
-                const HtLayer& L = HH.L[l];
-                const int D = L.D;
-                ht_warp_wait(acc_full, (uint32_t)(l & 1), lane);
-                tc_fence_after();
-                // accumulators -> fp32 row in shared memory: exact 2^-s, bias
-                const float us = L.unscale;
-                const float* bias = H.blob + H.b_off[l];
-                const uint32_t taddr = tmem_base + ((uint32_t)(warp * 32) << 16) + (uint32_t)(l & 1) * 128u;
-                for (int c0 = 0; c0 < L.NP; c0 += 16) {
-                    uint32_t v[16];
-                    tmem_ld16(taddr + c0, v);
-                    tmem_wait_ld();
-#pragma unroll
-                    for (int e = 0; e < 16; ++e)
-                        if (c0 + e < D) hrow[c0 + e] = fmaf(__uint_as_float(v[e]), us, __ldg(bias + c0 + e));
-                }
-                tc_fence_before();
-                if (l == n_layers - 1) break;
-                // [LayerNorm] + ReLU in fp32 (same arithmetic as heads.cu), then the next GEMM's A tile as fp16 hi/lo
-                float mu = 0.f, rstd = 1.f;
-                if (H.layernorm) {
-                    float sum = 0.f;
-                    for (int d = 0; d < D; ++d) sum += hrow[d];
-                    mu = sum / (float)D;
-                    float sq = 0.f;
-                    for (int d = 0; d < D; ++d) { const float c = hrow[d] - mu; sq = fmaf(c, c, sq); }
-                    rstd = 1.0f / sqrtf(sq / (float)D + 1e-5f);
-                }
-                const float* g = H.blob + H.g_off[l];
-                const float* hb = H.blob + H.h_off[l];
-                const int Kp = HH.L[l + 1].Kp;
-                for (int j = 0; j < Kp / 8; ++j) {
-                    float x[8];
-#pragma unroll
-                    for (int e = 0; e < 8; ++e) {
-                        const int d = j * 8 + e;
-                        float v = 0.f;
-                        if (d < D) {
-                            v = hrow[d];
-                            if (H.layernorm) v = (v - mu) * rstd * __ldg(g + d) + __ldg(hb + d);
-                            v = fmaxf(v, 0.f);
-                        }
-                        x[e] = v;
-                    }
-                    uint4 hi, lo;
-                    ht_split8(x, hi, lo);
-                    *reinterpret_cast<uint4*>(a_next + j * kHtAPlane + r * 16) = hi;
-                    if (a.n_terms >= 2) *reinterpret_cast<uint4*>(a_next + 16 * kHtAPlane + j * kHtAPlane + r * 16) = lo;
-                }
-                asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
-                __syncwarp();
-                if (lane == 0) mbar_arrive(an_full);
-            }
-            // final activation + store
-            const int n_out = H.dims[n_layers];
-            if (s0 + r < a.n) {
-                if (H.final_act == 4) {
-                    for (int d = 0; d < n_out; ++d) hrow[d] = fmaxf(hrow[d], 0.f);
-                } else if (H.final_act == 1) {
-                    for (int d = 0; d < n_out; ++d) hrow[d] = 1.0f / (1.0f + expf(-hrow[d]));
-                } else if (H.final_act == 2 || H.final_act == 3) {
-                    float m = -INFINITY;
-                    for (int d = 0; d < n_out; ++d) {
-                        if (H.final_act == 3) hrow[d] = fmaxf(hrow[d], 0.f);
-                        m = fmaxf(m, hrow[d]);
-                    }
-                    float sum = 0.f;
-                    for (int d = 0; d < n_out; ++d) { hrow[d] = expf(hrow[d] - m); sum += hrow[d]; }
-                    for (int d = 0; d < n_out; ++d) hrow[d] = hrow[d] / sum;
-                }
-                float* o = a.out + (int64_t)(s0 + r) * a.out_stride + H.col0;
-                for (int d = 0; d < n_out; ++d) o[d] = a.combine_max ? fmaxf(o[d], hrow[d]) : hrow[d];
-            }
-        }
-    }
-    tc_fence_before();
-    __syncthreads();
-    if (warp == kHtWorkers + 1) {
-        tc_fence_after();
-        asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "r"(256));
     }
 }
 
@@ -364,7 +221,7 @@ int scale_exponent(const float* w, size_t n) {
     return std::min(24, std::max(-8, 14 - e));
 }
 
-// fp16 hi/lo of rows [k0, k0 + Kp) of w[K][D] * 2^s in UMMA K-major core-matrix order: [term][octet Kp/8][NP][8]
+// fp16 hi/lo of rows [k0, k0 + Kp) of w[K][D] * 2^s in K-major core-matrix order: [term][octet Kp/8][NP][8]
 void pack_block(const float* w, int K, int D, int k0, int Kp, int NP, float sc, __half* out) {
     const size_t term = (size_t)(Kp / 8) * NP * 8;
     for (int j = 0; j < Kp / 8; ++j)
@@ -385,7 +242,7 @@ void pack_block(const float* w, int K, int D, int k0, int Kp, int NP, float sc, 
 int oww_heads_tc_pack(oww_ctx* ctx, Head& h, const float* blob /* staging in device layout: tensors at h.w_off[] */) {
     const int n_in = h.desc.n_in, nl = h.desc.n_layers;
     h.tc_ok = false;
-    for (int l = 1; l <= nl; ++l) if (h.desc.dims[l] > 128) return OWW_OK;     // hidden buffers / TMEM accumulators are 128 wide
+    for (int l = 1; l <= nl; ++l) if (h.desc.dims[l] > 128) return OWW_OK;     // hidden buffers / register accumulators are 128 wide
     std::vector<__half> packed;
     h.tc_layers.assign(nl, Head::TcLayer{});
     for (int l = 0; l < nl; ++l) {

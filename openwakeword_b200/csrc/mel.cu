@@ -1,7 +1,7 @@
 // K1: int16 PCM -> log-mel rows, one CTA per (stream, call).
 //
 // Replaces the melspectrogram.onnx session of the reference
-// (/root/reference/openwakeword/utils.py:84-87,180-208; graph spec
+// (openwakeword/utils.py:84-87,180-208; graph spec
 // notebooks/converting_google_speech_embedding_model.ipynb:426-477): frames of 512 samples every
 // 160, periodic Hann(400) zero-padded to 512, |rFFT|^2, 32 Slaney mel filters (60-3800 Hz),
 // 10*log10(max(.,1e-10)), clamp at (max over the call) - 80 dB, then x/10+2.

@@ -1,7 +1,7 @@
 // Score metrics on the device (SURVEY.md section 8 f4): false positives per threshold with the reference's grouping rule
 // and the ROC counts, over [n_series][n_frames] score tensors that are already in HBM (bulk predict_clips leaves them there).
 //
-// Replaces /root/reference/openwakeword/metrics.py:24-45 (get_false_positives; the sequential grouping rule is restated
+// Replaces openwakeword/metrics.py:24-45 (get_false_positives; the sequential grouping rule is restated
 // in oracle/metrics.py and pinned against the reference's own function by tests/golden/metrics.npz), :48-78
 // (generate_roc_curve_fprs: the same count at 25 thresholds) and :81-100 (generate_roc_curve_tprs: count of scores >= t).
 // The reference walks one Python list per threshold; here one thread owns one (series, threshold) pair and the 32 lanes

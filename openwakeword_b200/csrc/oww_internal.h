@@ -30,7 +30,7 @@ struct Head {
     int col0;            // first score column
     float* d_blob;       // packed weights (layout of pack_head_blob)
     std::vector<size_t> w_off, b_off, g_off, h_off;   // float offsets per layer
-    // tensor-core path (heads_tc.cu): every Linear layer as fp16 hi/lo of W * 2^s in UMMA order, or tc_ok == false
+    // tensor-core path (heads_tc.cu): every Linear layer as fp16 hi/lo of W * 2^s in core-matrix order, or tc_ok == false
     struct TcLayer { int K, D, Kp, NP; uint32_t w_off, w_bytes; float unscale; };
     bool tc_ok = false;
     void* d_w1_tc = nullptr;         // packed weights of all layers
@@ -112,7 +112,7 @@ struct IncPlan {
 struct oww_ctx {
     oww_config cfg;
     int device = 0;
-    int sm_count = 148;
+    int sm_count = 132;
     std::string err;
     uint64_t launches = 0;
 
@@ -305,7 +305,7 @@ struct WindowSrc {
 int oww_cnn_clip_fp32(oww_ctx* ctx, const float* d_mel, int n, int T, float* d_emb, cudaStream_t s);
 // appends n_chunks embedding rows per stream; ids != nullptr: only the n_ids streams listed (d_emb rows are compact)
 int oww_feat_append(oww_ctx* ctx, const float* d_emb, int n_chunks, cudaStream_t s, const int* d_ids = nullptr, int n_ids = 0);
-// mode dispatch (fp32 window / tcgen05 window) with sub-batching over ctx->window_batch
+// mode dispatch (fp32 window / tensor-core window) with sub-batching over ctx->window_batch
 int oww_cnn_window(oww_ctx* ctx, const WindowSrc& src, int n_windows, float* d_emb, cudaStream_t s, bool capture_tails = false);
 
 // ---- cnn_tc.cu ----
@@ -355,12 +355,12 @@ struct FeatSrc {
 int oww_heads_launch(oww_ctx* ctx, int head_id, const FeatSrc& src, int n, float* d_out, int out_stride,
                      int out_col0, int combine_max, cudaStream_t s, uint32_t head_mask = 0xFFFFFFFFu);
 
-// ---- heads_tc.cu: first layer on tcgen05 (fp16 hi/lo split operands, fp32 accumulate) ----
+// ---- heads_tc.cu: every Linear layer on the tensor cores (wgmma, fp16 hi/lo split operands, fp32 accumulate) ----
 int oww_heads_tc_pack(oww_ctx* ctx, Head& h, const float* w1);
 bool oww_heads_tc_supported(const oww_ctx* ctx, int head_id);
 int oww_heads_tc_launch(oww_ctx* ctx, int head_id, const FeatSrc& src, int n, float* d_out, int out_stride,
                         int out_col0, int combine_max, cudaStream_t s, uint32_t head_mask = 0xFFFFFFFFu);
-// ---- heads_grp.cu: streaming heads grouped by window, A operand from the fp16 mirror of the feature rings ----
+// ---- heads_grp.cu: streaming / bulk heads, A operand from the fp16 mirror of the feature rings ----
 void oww_heads_grp_free(oww_ctx* ctx);
 void oww_heads_grp_drop_mirror(oww_ctx* ctx);
 void oww_feat16_invalidate(oww_ctx* ctx);        // rows were appended without oww_feat16_advance: rebuild at the next advance

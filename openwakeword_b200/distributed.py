@@ -167,7 +167,7 @@ class ShardedStreams:
     ``"nccl-overlap"`` - the all-gather of step k runs on a side stream while the compute stream already works on
     step k+1 (two score buffers; ``step`` returns a ``GatheredScores`` whose ``wait()`` yields the tensor);
     ``"peer"`` - every rank copies its score block into rank 0's buffer over NVLink, counters follow; no collective
-    (tests/test_gpu_multi.py, 2 x B200)."""
+    (tests/test_gpu_multi.py, two GPUs)."""
 
     def __init__(self, n_total, engine_factory, rank=None, world=None, gather="nccl"):
         r, w, _ = env_rank_world()

@@ -1,4 +1,4 @@
-"""B200 mirror of ``openwakeword.metrics`` (/root/reference/openwakeword/metrics.py:24-100): false positives per hour
+"""CUDA mirror of ``openwakeword.metrics`` (openwakeword/metrics.py:24-100): false positives per hour
 and ROC points from score sequences - evaluated on the device, so the ``[clips, steps]`` score tensors that
 ``Model.predict_clips_array`` / bulk prediction leave in HBM never have to come back as Python lists.
 

@@ -1,4 +1,4 @@
-"""B200 mirror of ``openwakeword.Model`` (/root/reference/openwakeword/model.py:32-504).
+"""CUDA mirror of ``openwakeword.Model`` (openwakeword/model.py:32-504).
 
 Same constructor keywords, ``predict`` / ``predict_clip`` / ``reset`` semantics, attribute names
 (``models``, ``model_inputs``, ``model_outputs``, ``class_mapping``, ``prediction_buffer``,

@@ -3,7 +3,7 @@ without the ``onnx`` package (absent in this image; field numbers from onnx.prot
 
 Readers:
   * ``head_from_onnx``      - wake-word heads of the DNN family the reference trains/exports
-                               (/root/reference/openwakeword/train.py:56-83,144-165, torch.onnx.export opset 13):
+                               (openwakeword/train.py:56-83,144-165, torch.onnx.export opset 13):
                                Flatten -> Gemm|MatMul+Add -> [LayerNorm] -> Relu -> ... -> Gemm -> Sigmoid | (Relu ->) Softmax.
                                LayerNorm may be the fused ``LayerNormalization`` op (opset >= 17) or the decomposed
                                ReduceMean/Sub/Pow/ReduceMean/Add/Sqrt/Div/Mul/Add chain (opset 13).

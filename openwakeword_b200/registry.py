@@ -1,4 +1,4 @@
-"""Model registry mirroring /root/reference/openwakeword/__init__.py:8-69 (names, file names, timer
+"""Model registry mirroring openwakeword/__init__.py:8-69 (names, file names, timer
 class mapping).  Paths point at ``resources/models/<name>_v0.1.npz`` - the b200 container written by
 ``weights.save_head`` (the reference's .tflite/.onnx assets are download-only and absent here)."""
 import os

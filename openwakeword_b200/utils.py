@@ -1,7 +1,7 @@
-"""B200 mirror of the reference's ``openwakeword.utils`` surface for the inference hot path.
+"""CUDA mirror of the reference's ``openwakeword.utils`` surface for the inference hot path.
 
 ``AudioFeatures`` keeps the reference's constructor / call / attribute surface
-(/root/reference/openwakeword/utils.py:33-463) but owns a libowwb200 ``Context``: the PCM tail,
+(openwakeword/utils.py:33-463) but owns a libowwb200 ``Context``: the PCM tail,
 mel ring and embedding ring live in HBM and one ``__call__`` is one C-ABI step for every stream.
 ``bulk_predict`` keeps the reference signature (utils.py:467-539) and runs clips through
 ``oww_predict_clips`` with fresh state per clip.  Host code here only moves arguments, shapes and
@@ -62,7 +62,7 @@ def load_embedding_weights(path):
 
 
 class AudioFeatures:
-    """PCM -> log-mel -> speech-embedding features, streaming and batch, on one B200.
+    """PCM -> log-mel -> speech-embedding features, streaming and batch, on one GPU.
 
     Extra keywords over the reference: ``n_streams`` (independent audio streams packed on the batch
     axis; 1 behaves exactly like the reference object), ``feature_init`` ([rows,96] initial content
@@ -309,7 +309,7 @@ def compute_features_from_generator(generator, n_total, clip_duration, output_fi
     ``[n, (T-76)//8+1, 96]`` to the ``.npy`` file ``output_file`` through a memmap, so the result may exceed host
     memory.  ``n_total`` may over-estimate the number of clips: the file is cut to the rows actually written (the
     reference trims trailing all-zero rows with ``data.trim_mmap`` - same result unless a clip embeds to exactly
-    zero).  ``device``/``ncpu`` are accepted for signature compatibility; the work runs on the B200.
+    zero).  ``device``/``ncpu`` are accepted for signature compatibility; the work runs on the GPU.
     ``audio_features`` lets a caller reuse an existing ``AudioFeatures`` (weights already on the device)."""
     from numpy.lib.format import open_memmap
     F = audio_features if audio_features is not None else AudioFeatures(device=device)

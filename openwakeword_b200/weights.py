@@ -1,8 +1,8 @@
-"""Weight containers for the B200 backend.
+"""Weight containers for the CUDA backend.
 
 The released model files of the reference (``melspectrogram.onnx``,
 ``embedding_model.onnx``, ``<head>_v0.1.onnx``; registry at
-/root/reference/openwakeword/__init__.py:8-51) are download-only and absent from
+openwakeword/__init__.py:8-51) are download-only and absent from
 this image, so every test and benchmark runs on *synthetic, seeded weights of
 the exact reference architecture* (SURVEY.md F3).  This module builds those,
 packs weights into the flat float32 blobs the C ABI takes

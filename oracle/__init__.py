@@ -9,7 +9,7 @@ of ``openwakeword/model.py`` and ``openwakeword/utils.py``.
 
 PARITY STATUS
   * state machine  : PINNED - driven against the reference's own plumbing
-    (``/root/reference/openwakeword`` imported with a stub ``onnxruntime`` whose
+    (``openwakeword`` (the original project) imported with a stub ``onnxruntime`` whose
     sessions call this oracle's graph functions; ``tests/golden/make_golden.py``)
     and frozen in ``tests/golden/*.npz``.
   * graph arithmetic: PARITY UNPINNED at the onnxruntime boundary - neither

@@ -1,6 +1,6 @@
 """Speech-embedding CNN restatement (the graph inside ``embedding_model.onnx``).
 
-Follows /root/reference/notebooks/converting_google_speech_embedding_model.ipynb
+Follows notebooks/converting_google_speech_embedding_model.ipynb
 lines 871-951 (layer code) and 521-859 (shapes): 20 bias-free dense convs
 (3x3 then alternating (1,3) 'same' / (3,1) 'valid'), each but the last followed
 by BatchNorm(eps=1e-3) -> max(0.2x, x) -> max(x, -0.4); the first conv also has

@@ -1,6 +1,6 @@
 """Wake-word classifier head restatement (the graphs inside ``<head>.onnx``).
 
-Family from /root/reference/openwakeword/train.py:56-83 (``Net``/``FCNBlock``:
+Family from openwakeword/train.py:56-83 (``Net``/``FCNBlock``:
 Flatten -> Linear -> LayerNorm -> ReLU -> n x [Linear -> LayerNorm -> ReLU] ->
 Linear -> Sigmoid | ReLU(+softmax at export, train.py:144-165)) and the model
 cards docs/models/alexa.md:11-36 (1536-64-64-1, LayerNorm) and

@@ -1,9 +1,9 @@
 """Log-mel frontend restatement (the graph inside ``melspectrogram.onnx``).
 
-Follows /root/reference/notebooks/converting_google_speech_embedding_model.ipynb
+Follows notebooks/converting_google_speech_embedding_model.ipynb
 lines 426-477 (torchlibrosa ``Spectrogram(center=False, n_fft=512, hop=160,
 win=400)`` -> ``LogmelFilterBank(sr=16000, n_mels=32, fmin=60, fmax=3800)`` with
-the patched ``power_to_db``) and /root/reference/openwakeword/utils.py:180-208
+the patched ``power_to_db``) and openwakeword/utils.py:180-208
 (int16 -> float32 *unscaled* in, ``x/10 + 2`` out).  torchlibrosa evaluates the
 STFT as a conv1d with windowed DFT filters in float32; ``dtype`` selects that
 (float32, faithful) or float64 (round-off yardstick).

@@ -1,7 +1,7 @@
 """A stand-in ``onnxruntime`` whose sessions evaluate this oracle's graphs.
 
 Used ONLY in the build container by tests/golden/make_golden.py: it lets the
-*unmodified reference plumbing* (/root/reference/openwakeword/model.py,
+*unmodified reference plumbing* (openwakeword/model.py,
 utils.py) run end to end although neither onnxruntime nor the released .onnx
 files exist here (SURVEY.md F2-F4).  The ORT surface emulated is exactly what
 the reference touches (utils.py:79-93; model.py:149-157): SessionOptions,

@@ -1,8 +1,8 @@
 """Streaming state machine restatement (single stream, NumPy).
 
-Restates /root/reference/openwakeword/utils.py:163-178,387-463 (AudioFeatures
+Restates openwakeword/utils.py:163-178,387-463 (AudioFeatures
 buffers, chunk accumulation, per-chunk mel + embedding) and
-/root/reference/openwakeword/model.py:232-426 (predict / predict_clip score
+openwakeword/model.py:232-426 (predict / predict_clip score
 assembly and post-processing); SURVEY.md Appendix D.  Written from that
 description, array-based (no deques), so it is an independent check of the
 reference plumbing: tests/golden/make_golden.py drives the reference's own

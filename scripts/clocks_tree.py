@@ -19,7 +19,7 @@ for rep in range(2):
     c = eng.ctx.debug_inc_clocks_read()
     st = list(c[:NL]) + [c[20]]
     print(f"{os.path.basename(tree)} B={B} split={split}: phase cyc:", np.diff(st).tolist(), " layers total", int(c[20] - c[0]), "cyc")
-    print("  mma issue    :", c[41:41 + NL].tolist())
+    print("  first accumulator:", c[61:61 + NL].tolist())
     print("  to last store:", c[81:81 + NL].tolist())
     print("  frontend:", int(c[0] - c[101]), " heads:", int(c[102] - c[20]) if c[102] else None)
     if c[92]:

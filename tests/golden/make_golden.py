@@ -1,8 +1,8 @@
 """Generate tests/golden/*.npz by running the UNMODIFIED reference plumbing.
 
-Run in the build container only (needs /root/reference):
-    python tests/golden/make_golden.py
-/root/reference/openwakeword is imported with ``oracle.ref_stub_ort`` standing in
+Needs a checkout of the original openWakeWord project (OWW_REFERENCE = its root directory):
+    OWW_REFERENCE=/path/to/openWakeWord python tests/golden/make_golden.py
+Its ``openwakeword`` package is imported with ``oracle.ref_stub_ort`` standing in
 for onnxruntime (absent here, SURVEY.md F2), so buffers, windowing, chunk
 accumulation and score post-processing are the reference's own code while the
 three graphs are evaluated by oracle/{mel,embedding,heads}.py on synthetic seeded
@@ -48,7 +48,8 @@ def main():
     heads.update({k: W.synthetic_gated_head(**v) for k, v in GATED_SPECS.items()})
     only_new = "--only-new" in sys.argv           # keep the committed round-1 fixtures byte-identical
     ref_stub_ort.install(emb, heads)
-    sys.path.insert(0, "/root/reference")
+    ref_root = os.environ["OWW_REFERENCE"]
+    sys.path.insert(0, ref_root)
     from openwakeword.model import Model            # the reference, unmodified
 
     tmp = tempfile.mkdtemp()
@@ -68,7 +69,7 @@ def main():
             m.class_mapping["timer_v0.1"] = dict(TIMER_MAP)
         return m, m.preprocessor.feature_buffer.astype(np.float32).copy()
 
-    wavs = {n: read_wav(f"/root/reference/tests/data/{n}.wav")
+    wavs = {n: read_wav(os.path.join(ref_root, "tests", "data", f"{n}.wav"))
             for n in ("alexa_test", "hey_mycroft_test", "hey_jane")}
     cases = {}
 

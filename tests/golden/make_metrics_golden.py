@@ -1,6 +1,6 @@
 """Generate tests/golden/metrics.npz from the UNMODIFIED reference functions
-(/root/reference/openwakeword/metrics.py).  Run in the build container only:
-    python tests/golden/make_metrics_golden.py
+(openwakeword/metrics.py of the original openWakeWord project, OWW_REFERENCE = its root directory):
+    OWW_REFERENCE=/path/to/openWakeWord python tests/golden/make_metrics_golden.py
 Series are built so that the reference does not raise (its grouping loop indexes one past a transition's 1, so a
 series whose final element is a fresh 0->1 rise makes it throw IndexError)."""
 import importlib.util
@@ -9,7 +9,7 @@ import sys
 
 import numpy as np
 
-spec = importlib.util.spec_from_file_location("ref_metrics", "/root/reference/openwakeword/metrics.py")
+spec = importlib.util.spec_from_file_location("ref_metrics", os.path.join(os.environ["OWW_REFERENCE"], "openwakeword", "metrics.py"))
 ref = importlib.util.module_from_spec(spec)
 spec.loader.exec_module(ref)
 

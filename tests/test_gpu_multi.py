@@ -1,6 +1,6 @@
 """gpu, needs two devices (skipped on a one-GPU box): the peer-memory score gather (distributed.PeerGather: every rank
 copies its score block into rank 0's buffer over NVLink, counters follow) against every rank's own local scores.
-Run with `gpurun --gpus 2 -- 'python -m pytest tests/test_gpu_multi.py -m gpu'` (passed on 2 x B200 in round 2); the
+Run on a machine with two GPUs: `python -m pytest tests/test_gpu_multi.py -m gpu`; the
 protocol is also covered on host memory by tests/test_distributed_cpu.py::test_peer_gather_protocol_threads."""
 import os
 import socket

@@ -20,7 +20,7 @@ def torch_cuda():
     return torch
 
 
-MODES = [0, 3]        # fp32 CUDA-core window path (bit-faithful check) and the default tcgen05 fused incremental path
+MODES = [0, 3]        # fp32 CUDA-core window path (bit-faithful check) and the default tensor-core fused incremental path
 
 
 @pytest.fixture(scope="module")
@@ -32,7 +32,7 @@ def af(torch_cuda, built_library):
 
 @pytest.fixture(scope="module")
 def af_default(torch_cuda, built_library):
-    """what a user gets: cnn_mode 3 (tcgen05, fp16 operands / fp32 accumulate)."""
+    """what a user gets: cnn_mode 3 (tensor cores, fp16 operands / fp32 accumulate)."""
     from openwakeword_b200 import AudioFeatures
     return AudioFeatures(embedding_model_path=emb_weights(), feature_init=np.zeros((41, 96), np.float32))
 
@@ -91,7 +91,7 @@ def test_embedding_windows_vs_oracle(af):
 
 
 def test_default_mode_is_tc_and_embedding_windows_within_fp16_budget(af_default):
-    """The default handle runs the tcgen05 kernels; stateless window embeddings stay within the fp16-operand budget
+    """The default handle runs the tensor-core kernels; stateless window embeddings stay within the fp16-operand budget
     (measured 3.4e-3 on |x| <= 5; gate 8e-3 = ~2x)."""
     from oracle import embedding
     from openwakeword_b200 import _native
@@ -157,7 +157,7 @@ def test_heads_vs_oracle(torch_cuda, built_library):
             got = m.model_prediction_function[name](f)[0]
             ref = heads.forward(head(name), f)
             assert got.shape == ref.shape == (n, m.model_outputs[name])
-            # default handle: first layer on tcgen05 with the fp16 hi/lo split (fp32-grade, measured 1.2e-5)
+            # default handle: first layer on the tensor cores with the fp16 hi/lo split (fp32-grade, measured 1.2e-5)
             assert np.abs(got - ref).max() < 2e-5, (name, np.abs(got - ref).max())
 
 
@@ -363,7 +363,7 @@ def test_bulk_predict_file_paths_on_reference_wavs(torch_cuda, built_library, tm
     """utils.bulk_predict(file_paths=...) end to end (reference signature, utils.py:467-539) on WAV files holding the
     audio of the reference's three test clips (tests/data/{alexa_test,hey_mycroft_test,hey_jane}.wav; their samples
     travel inside the golden fixtures) plus two synthetic clips of a shared length (one batched group): threaded RIFF
-    ingest -> pinned staging -> the bulk device path (one mel launch per slab, fully convolutional tcgen05 CNN, heads
+    ingest -> pinned staging -> the bulk device path (one mel launch per slab, fully convolutional tensor-core CNN, heads
     over all sliding windows).  Every clip's result must equal the golden scores the UNMODIFIED reference plumbing
     produced for predict_clip on a fresh model (1e-3), and the bulk path must be bit-identical to streaming the clip."""
     import openwakeword_b200 as owb
@@ -393,8 +393,8 @@ def test_bulk_predict_file_paths_on_reference_wavs(torch_cuda, built_library, tm
     print("bulk_predict(hey_jane.wav) vs reference-plumbing golden: max |delta| =", d)
     assert d < SCORE_TOL
     # every file: bulk == streaming predict_clip on a fresh model.  Mel, CNN and ring contents are bit-identical; the
-    # heads accumulate their first layer in a different order in the two paths (streaming: all heads of a window in one
-    # CTA, K chunks of 32; bulk: one CTA per head, K chunks of 96), so the scores agree to fp32 rounding
+    # heads may accumulate their first layer in a different order in the two paths (heads_grp.cu on the fp16 mirror,
+    # K chunks of 32, or heads_tc.cu, K chunks of 96), so the scores agree to fp32 rounding
     m = owb.Model(wakeword_models=specs, embedding_model_path=emb_weights(), feature_init=fi)
     for p in paths:
         m.reset()
@@ -413,7 +413,7 @@ def test_embed_clips_and_feature_generator_on_gpu(torch_cuda, built_library, tmp
     af = AudioFeatures(embedding_model_path=emb_weights())
     got = af.embed_clips(c["pcm"])
     d = np.abs(got - c["embeddings"]).max()
-    print("embed_clips (tcgen05 clip pass) vs golden: max |delta| =", d)
+    print("embed_clips (tensor-core clip pass) vs golden: max |delta| =", d)
     assert got.shape == (3, 16, 96) and d < 2e-3
     rng = np.random.default_rng(5)
     clips = np.clip(rng.normal(0, 4000, (10, 32000)), -32768, 32767).astype(np.int16)

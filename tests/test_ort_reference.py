@@ -2,7 +2,7 @@
 
 When ``onnxruntime`` is importable AND the released model files (melspectrogram.onnx, embedding_model.onnx, <head>.onnx)
 are found (oracle/probe.py), this test drives the unmodified ``openwakeword.Model(inference_framework="onnx")``
-(/root/reference/openwakeword/model.py:149-159, utils.py:79-93) and this repository's CUDA path on the same int16 frames
+(openwakeword/model.py:149-159, utils.py:79-93) and this repository's CUDA path on the same int16 frames
 with the same injected ``feature_buffer`` (SURVEY.md F6) and holds every per-frame, per-label score to the 1e-3 gate of
 BASELINE.json.  Neither exists in this image or on the GPU box (SURVEY.md F2/F3), so today the test SKIPS - it is the
 hook that turns "parity vs the NumPy restatement on synthetic weights" into "parity vs ONNX" the moment the assets appear.
@@ -22,9 +22,9 @@ pytestmark = [pytest.mark.gpu, pytest.mark.skipif(not _OK, reason=f"genuine refe
 
 
 def _import_reference():
-    """the unmodified reference package: installed, or from baseline/_ref, or from /root/reference"""
+    """the unmodified reference package: installed, or from baseline/_ref"""
     root = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-    for extra in (None, os.path.join(root, "baseline", "_ref"), "/root/reference"):
+    for extra in (None, os.path.join(root, "baseline", "_ref")):
         if extra and os.path.isdir(extra) and extra not in sys.path:
             sys.path.insert(0, extra)
         try:
