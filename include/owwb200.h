@@ -78,7 +78,10 @@ typedef struct oww_config {
                               instead of the block-major layout of tc_conv_blk_kernel;
                               bit 5: 1 = no programmatic dependent launches inside the late chain.
                               reserved[1]: first conv layer that takes fp16 hi/lo split operands in the
-                              tensor-core modes, 2..20 (0 = default 11; 20 = plain fp16 everywhere)           */
+                              tensor-core modes (0 = default 11; 20 = plain fp16 everywhere): 2..20 in
+                              OWW_CNN_TC_WINDOW; OWW_CNN_TC_INCREMENTAL accepts only 3, 7, 11, 15 and 20 (the
+                              split must start at a (1,3) layer behind a pool); with any other value
+                              oww_set_streams fails with OWW_EUNSUPPORTED                                       */
 } oww_config;
 
 typedef struct oww_head_desc {
@@ -189,8 +192,12 @@ int oww_debug_layer(oww_ctx* ctx, const float* d_windows, int n, int layer, floa
 
 /* Geometry plan of the fused incremental CNN kernel for groups of `group` streams, as raw int32
  * (struct IncPlan of csrc/oww_internal.h); returns the number of ints written (> 0) or an error.
+ * oww_debug_inc_plan: the full 20-layer plan.  oww_debug_inc_cut_plan: n_layers conv layers inside
+ * the kernel - 0 or 20 for the full plan, split_from for the cut plan of cnn_mode 3 (the fused kernel
+ * stops after the pooled layer split_from - 1).
  * Pure host computation (usable without a GPU): tests/test_inc_plan.py replays it in NumPy.          */
 int oww_debug_inc_plan(oww_ctx* ctx, int group, int n_streams, int32_t* out, int max_ints);
+int oww_debug_inc_cut_plan(oww_ctx* ctx, int group, int n_streams, int n_layers, int32_t* out, int max_ints);
 
 /* cnn_mode 3 only, instrumentation: oww_debug_inc_clocks arms a clock buffer; the next step then records clock64()
  * stamps taken by CTA 0 on its first group; oww_debug_inc_clocks_read synchronises and returns 104 values:

@@ -60,6 +60,7 @@ _SIGNATURES = {
     "oww_predict_clips": (C.c_int, [_P, _P, C.c_int, C.c_int, C.c_int, _P, C.c_int, _P, _P]),
     "oww_debug_layer": (C.c_int, [_P, _P, C.c_int, C.c_int, _P, _P]),
     "oww_debug_inc_plan": (C.c_int, [_P, C.c_int, C.c_int, _P, C.c_int]),
+    "oww_debug_inc_cut_plan": (C.c_int, [_P, C.c_int, C.c_int, C.c_int, _P, C.c_int]),
     "oww_debug_inc_clocks": (C.c_int, [_P, _P]),
     "oww_debug_inc_clocks_read": (C.c_int, [_P, _P]),
     "oww_debug_heads_clocks": (C.c_int, [_P, _P]),

@@ -837,11 +837,15 @@ int oww_debug_layer(oww_ctx* ctx, const float* d_windows, int n, int layer, floa
 }
 
 int oww_debug_inc_plan(oww_ctx* ctx, int group, int n_streams, int32_t* out, int max_ints) {
+    return oww_debug_inc_cut_plan(ctx, group, n_streams, 0, out, max_ints);
+}
+
+int oww_debug_inc_cut_plan(oww_ctx* ctx, int group, int n_streams, int n_layers, int32_t* out, int max_ints) {
     if (!out) return oww_fail(ctx, OWW_EINVAL, "null argument");
     oww_ctx local;                       // ctx may be NULL: the plan depends only on the fixed layer table
     if (!ctx) { fill_layer_table(&local); ctx = &local; }
     IncPlan P;
-    int rc = oww_inc_build_plan(ctx, group, n_streams, OWW_N_CONV, &P);
+    int rc = oww_inc_build_plan(ctx, group, n_streams, n_layers ? n_layers : OWW_N_CONV, &P);
     if (rc) return rc;
     const int n = (int)(sizeof(IncPlan) / sizeof(int32_t));
     if (max_ints < n) return oww_fail(ctx, OWW_EINVAL, "need room for %d ints", n);

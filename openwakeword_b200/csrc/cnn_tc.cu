@@ -302,9 +302,11 @@ __global__ void __launch_bounds__(kTcThreads, 1) tc_conv_kernel(TcConvArgs a) {
                         reinterpret_cast<uint32_t*>(o + (int64_t)(a.cg_out + g) * a.out_plane)[q] = lw;
                         if (po == 0) reinterpret_cast<uint32_t*>(o + (int64_t)(a.cg_out + g) * a.out_plane - 1)[q] = 0u;
                     }
+                    // a mirror takes only the rows that become tails there: with 4 new rows per step (split_from 3 / 7)
+                    // rows 0, 1 map before the stream's slot - for stream 0 before the start of the allocation
 #pragma unroll
                     for (int kk = 0; kk < 2; ++kk)
-                        if (a.out_b[kk]) {
+                        if (a.out_b[kk] && t + a.out_b_toff[kk] >= 0) {
                             uint4* ob = reinterpret_cast<uint4*>(a.out_b[kk]) + kGuard + (int64_t)n * a.out_T * Wp +
                                         (int64_t)(t + a.out_b_toff[kk]) * Wp + f;
                             reinterpret_cast<uint32_t*>(ob + (int64_t)g * a.out_plane)[q] = hw;
@@ -474,11 +476,15 @@ __global__ void __launch_bounds__(kTcThreads, 1) tc_conv_blk_kernel(TcBlkArgs a)
                 const bool pooled = a.pool_f == 2;
                 const bool writer = live && (!pooled || (f & 1) == 0);
                 const int fo = pooled ? f >> 1 : f;
-                int64_t dst[3];
+                // a mirror takes only the rows that become tails there (t + toff >= 0); no destination: nullptr
+                uint4* dst[3];
 #pragma unroll
                 for (int kk = 0; kk < 3; ++kk)
-                    dst[kk] = a.out_lay.S ? late_unit(a.out_lay, 0, live ? n : 0, t + a.out_toff[kk], fo)
-                                          : kGuard + ((int64_t)(live ? n : 0) * a.rows_new + t) * (a.W + 1) + f;
+                    dst[kk] = a.out[kk] && t + a.out_toff[kk] >= 0
+                                  ? reinterpret_cast<uint4*>(a.out[kk]) +
+                                        (a.out_lay.S ? late_unit(a.out_lay, 0, live ? n : 0, t + a.out_toff[kk], fo)
+                                                     : kGuard + ((int64_t)(live ? n : 0) * a.rows_new + t) * (a.W + 1) + f)
+                                  : nullptr;
                 const int64_t pstride = a.out_lay.S ? (int64_t)a.out_lay.units : a.out_plane;
 #pragma unroll
                 for (int j = 0; j < NP / 8; ++j) {
@@ -497,10 +503,9 @@ __global__ void __launch_bounds__(kTcThreads, 1) tc_conv_blk_kernel(TcBlkArgs a)
                     const uint32_t hw = *reinterpret_cast<const uint32_t*>(&hh), lw = *reinterpret_cast<const uint32_t*>(&ll);
 #pragma unroll
                     for (int kk = 0; kk < 3; ++kk)
-                        if (a.out[kk]) {
-                            uint4* o = reinterpret_cast<uint4*>(a.out[kk]) + dst[kk];
-                            reinterpret_cast<uint32_t*>(o + (int64_t)g * pstride)[q] = hw;
-                            reinterpret_cast<uint32_t*>(o + (int64_t)(a.cg_out + g) * pstride)[q] = lw;
+                        if (dst[kk]) {
+                            reinterpret_cast<uint32_t*>(dst[kk] + (int64_t)g * pstride)[q] = hw;
+                            reinterpret_cast<uint32_t*>(dst[kk] + (int64_t)(a.cg_out + g) * pstride)[q] = lw;
                         }
                 }
             }
@@ -560,7 +565,7 @@ __global__ void __launch_bounds__(256) tc_pool_kernel(const __half* in, int64_t 
         } else {
 #pragma unroll
             for (int k = 0; k < 3; ++k)
-                if (po.p[k]) {
+                if (po.p[k] && t + po.toff[k] >= 0) {                  // mirrors: only the rows that become tails
                     if (po.lay.S) {                                     // block-major: pad column untouched (zero since allocation)
                         if (f >= w_out) continue;
                         reinterpret_cast<uint4*>(po.p[k])[late_unit(po.lay, g, (int)s, t + po.toff[k], f)] = res;
@@ -946,7 +951,9 @@ int oww_late_chain(oww_ctx* ctx, float* d_emb, cudaStream_t s) {
             const int r = Y.rows_new;                       // 2 -> two buffers, 1 -> three
             for (int m = 0; m < Y.n_buf; ++m) {
                 p[m] = reinterpret_cast<__half*>(Y.buf[(k + m) % Y.n_buf]);
-                toff[m] = 2 - m * r;                        // this step: behind the two tails; later steps: as their tails
+                // this step: behind the two tails; later steps: as their tails.  With r = 4 (split_from 3 / 7) the mirror
+                // offset is -2: the kernels store only rows t with t + toff >= 0
+                toff[m] = 2 - m * r;
             }
             n_out = Y.n_buf;
         };

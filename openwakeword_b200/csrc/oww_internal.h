@@ -63,7 +63,8 @@ struct ResetLate {           // one tails-bearing tensor of the incremental late
     int64_t plane; int T_buf, Wp, n_planes;
     LateLay lay;             // lay.S > 0: block-major destination
 };
-struct ResetTails { uint4* tails; const uint4* tmpl; int G, tail_units, n_tab; int4 tab[OWW_N_CONV]; int n_late; ResetLate late[6]; };
+// late[]: one entry per tails-bearing late tensor X_l, l >= split_from (5 at the default split, 9 at split_from 3)
+struct ResetTails { uint4* tails; const uint4* tmpl; int G, tail_units, n_tab; int4 tab[OWW_N_CONV]; int n_late; ResetLate late[OWW_N_CONV]; };
 
 // conditional verifier pair (hey_jarvis, docs/models/hey_jarvis.md:38): score column `main_col` is replaced by column
 // `ver_col` wherever it exceeds `thr`

@@ -18,9 +18,9 @@ def torch_cuda():
     return torch
 
 
-def _ctx(mode, window_batch=0):
+def _ctx(mode, window_batch=0, split_from=None):
     from openwakeword_b200 import _native, weights as W
-    ctx = _native.Context(cnn_mode=mode, window_batch=window_batch)
+    ctx = _native.Context(cnn_mode=mode, window_batch=window_batch, split_from=split_from)
     ctx.load_mel()
     ctx.load_embedding(W.pack_embedding_blob(emb_weights()))
     return ctx
@@ -36,16 +36,65 @@ def _windows(rng, n):
     return np.stack(out).astype(np.float32)
 
 
-@pytest.mark.parametrize("n", [3, 130])
-def test_tc_layers_vs_oracle(torch_cuda, built_library, n):
-    torch = torch_cuda
+_LAYER_REF = {}
+
+
+def _layer_ref(n):
     from oracle import embedding
-    rng = np.random.default_rng(5)
-    wins = _windows(rng, n)
-    _, ref_layers = embedding.forward(emb_weights(), wins, return_all=True)
-    ctx = _ctx(TC)
+    if n not in _LAYER_REF:
+        wins = _windows(np.random.default_rng(5), n)
+        _LAYER_REF[n] = (wins, embedding.forward(emb_weights(), wins, return_all=True)[1],
+                         embedding.embed_windows(emb_weights(), wins))
+    return _LAYER_REF[n]
+
+
+def _layers_fp16_below(wins, split_from):
+    """The oracle's layer outputs (float64) with the quantisation points of the tensor-core path at this split point:
+    conv layers 1 .. split_from-1 take fp16-rounded activations and weights, a tensor feeding such a layer is stored
+    as fp16, and layers from split_from on compute exactly (their hi/lo split operands are fp32-grade)."""
+    from oracle import embedding as E
+    w = emb_weights()
+    x, out = wins[..., None].astype(np.float64), []
+    for li, (kh, kw, cin, cout, pool) in enumerate(E.LAYERS[:19]):
+        wt = w["conv"][li].astype(np.float64)
+        a = x
+        if 0 < li < split_from:
+            a, wt = a.astype(np.float16).astype(np.float64), wt.astype(np.float16).astype(np.float64)
+        x = E._conv(a, wt, np.float64)
+        if li == 0:
+            x = np.maximum(x, 0)
+        s, b = E.fold_bn(*[np.asarray(p, np.float64) for p in w["bn"][li]])
+        x = np.maximum(np.maximum(float(E.LEAK) * (x * s + b), x * s + b), float(E.FLOOR))
+        if pool is not None:
+            x = E._pool(x, *pool)
+        out.append(x.astype(np.float16).astype(np.float64) if li + 1 < split_from else x)
+    return out
+
+
+# per split point: (reference of the layers, max err / max(scale, 1), mean err, embedding max err vs the oracle).
+# 11 (default) and 20 (plain fp16): against the exact oracle with the fp16-operand budget, ~2x the worst layer of this
+# path (1.7e-3 x scale, mean 4.3e-4).  2: every layer from 2 on takes hi/lo split operands and layer 1 stays plain fp16
+# (the only run of the 24-channel split conv tc_conv_kernel<4,32,3>).  The error layer 1 leaves behind (6.9e-4 x scale)
+# carries into the next layers whatever their precision, so the layers are compared with the oracle run at the same
+# quantisation points (fp32-grade from layer 2 on); the embedding against the exact oracle (the CPU study: 1.3e-4).
+# Measured at 2 (130 windows): layers 1..18 within 3.4e-4 x scale, mean 4e-6; embedding 1.5e-4.
+LAYER_BUDGET = {11: ("exact", 4e-3, 9e-4, 7e-3), 20: ("exact", 4e-3, 9e-4, 7e-3), 2: ("fp16 below", 5e-4, 1e-4, 5e-4)}
+
+
+@pytest.mark.parametrize("n,split_from", [pytest.param(3, 11, id="3"), pytest.param(130, 11, id="130"),
+                                          pytest.param(3, 2, id="3-split2"), pytest.param(130, 2, id="130-split2"),
+                                          pytest.param(3, 20, id="3-split20"), pytest.param(130, 20, id="130-split20")])
+def test_tc_layers_vs_oracle(torch_cuda, built_library, n, split_from):
+    """cnn_mode 2 (full window) layer by layer against the oracle at the default split point, with split operands from
+    layer 2 on, and with plain fp16 everywhere."""
+    torch = torch_cuda
+    wins, ref_layers, ref_emb = _layer_ref(n)
+    kind, max_budget, mean_budget, emb_budget = LAYER_BUDGET[split_from]
+    if kind == "fp16 below":
+        ref_layers = _layers_fp16_below(wins, split_from)
+    ctx = _ctx(TC, split_from=split_from)
     d = torch.from_numpy(wins).cuda()
-    worst_rel = 0.0
+    stats = []                                      # (layer, finite, max err / max(scale, 1), mean err): every layer printed first
     for li in range(19):
         ref = ref_layers[li]
         out = torch.empty(ref.shape, dtype=torch.float32, device="cuda")
@@ -54,18 +103,22 @@ def test_tc_layers_vs_oracle(torch_cuda, built_library, n):
         got = out.cpu().numpy()
         err = np.abs(got - ref)
         scale = np.abs(ref).max()
-        print(f"layer {li:2d} shape {ref.shape} max|ref| {scale:7.3f} max err {err.max():.4e} mean err {err.mean():.3e}")
-        assert np.isfinite(got).all(), f"layer {li} has non-finite values"
-        # fp16-operand budget: gates at ~2x the worst max err (1.7e-3 x scale) and mean err (4.3e-4) of this path
-        assert err.max() < 4e-3 * max(scale, 1.0), f"layer {li}: max err {err.max()}"
-        assert err.mean() < 9e-4, f"layer {li}: mean err {err.mean()}"
-        worst_rel = max(worst_rel, err.max() / max(scale, 1.0))
+        print(f"split_from={split_from} layer {li:2d} shape {ref.shape} max|ref| {scale:7.3f} max err {err.max():.4e} "
+              f"mean err {err.mean():.3e} (vs {kind} oracle)")
+        stats.append((li, bool(np.isfinite(got).all()), float(err.max() / max(scale, 1.0)), float(err.mean())))
     emb = torch.empty((n, 96), dtype=torch.float32, device="cuda")
     ctx.embed_windows(d, n, emb)
     torch.cuda.synchronize()
-    e = np.abs(emb.cpu().numpy() - embedding.embed_windows(emb_weights(), wins))
-    print("embedding max err", e.max(), "worst relative layer err", worst_rel)
-    assert e.max() < 7e-3                       # measured 3.4e-3
+    e = np.abs(emb.cpu().numpy() - ref_emb)
+    print(f"split_from={split_from}: embedding max err", e.max(), "worst relative layer err", max(s[2] for s in stats))
+    for li, finite, rel, mean in stats:
+        # a tensor stored as fp16 for a plain layer (fp16-below reference) may round the other way than the oracle's
+        # float64 value where the two sit on either side of a rounding boundary: one fp16 ulp, <= 2^-10 x max(scale, 1)
+        budget = max(max_budget, 1.5 * 2.0 ** -10) if kind == "fp16 below" and li + 1 < split_from else max_budget
+        assert finite, f"layer {li} has non-finite values"
+        assert rel < budget, f"layer {li}: max err {rel} x max(scale, 1)"
+        assert mean < mean_budget, f"layer {li}: mean err {mean}"
+    assert e.max() < emb_budget
 
 
 def test_tc_scores_vs_fp32_and_oracle(torch_cuda, built_library):
@@ -474,30 +527,83 @@ def test_grouped_heads_match_per_head_kernels(torch_cuda, built_library):
     assert e_grp_tc < 5e-5 and e_grp_cc < 2e-4
 
 
-@pytest.mark.gpu
-@pytest.mark.parametrize("split_from,tol", [(15, 1e-3), (20, 1e-3)])
-def test_split_from_variants_vs_oracle(torch_cuda, built_library, split_from, tol):
-    """The other points of the precision / speed curve bench.py reports as `variants`: conv layers >= 15 on split operands
-    (tc_inc_kernel<15> + a 5-layer late chain) and plain fp16 everywhere (one launch per step), against the oracle."""
-    from openwakeword_b200.engine import StreamEngine
+_SPLIT_CASE = {}
+
+
+def _split_case():
+    """Input, call plan and oracle results of test_split_from_variants_vs_oracle (the same for every split point, so
+    the oracle runs once).  B = 151 is prime: the last group of the fused kernel is ragged for every group size 2..7,
+    and so is the last block of the block-major late tensors.  The plan has a 3-chunk call (the 2- and 3-buffer
+    rotations of the late tensors fall out of step with the call count), then a partial reset of the first stream, a
+    stream of the last group and one other, and a 2-chunk call."""
+    if _SPLIT_CASE:
+        return _SPLIT_CASE
     from oracle import streaming, heads as oheads
     rng = np.random.default_rng(41)
-    B, steps = 300, 12
+    B = 151
     hs = [head("alexa_v0.1"), head("timer_v0.1")]
     fi = rng.normal(0, 1, (41, 96)).astype(np.float32)
-    pcm = _mixes(rng, B, steps * 1280)
-    eng = StreamEngine(hs, B, embedding=emb_weights(), feature_init=fi, cnn_mode=3, split_from=split_from)
-    got = np.stack([eng.step_host(np.ascontiguousarray(pcm[:, k * 1280:(k + 1) * 1280]), 1).copy() for k in range(steps)])
-    eng.ctx.close()
-    worst = 0.0
-    for b in list(range(0, B, 23)) + [B - 1]:
-        o = streaming.OracleAudioFeatures(emb_weights(), feature_init=fi)
-        for k in range(steps):
-            o(pcm[b, k * 1280:(k + 1) * 1280])
-            col = 0
+    plan = [1, 1, 1, 3, 1, 1, 2, 1, 1, 1, 1]
+    reset_at, reset_ids = 4, [0, 77, B - 1]
+    base = _mixes(rng, 30, sum(plan) * 1280)
+    pcm = base[rng.integers(0, 30, B)]
+    fixed = sorted(set(list(range(8)) + list(range(B - 8, B)) + reset_ids))     # first groups, the ragged last ones
+    sample = sorted(fixed + [int(x) for x in rng.permutation(B) if x not in fixed][:56 - len(fixed)])
+    assert len(sample) >= 48
+    orc = {b: streaming.OracleAudioFeatures(emb_weights(), feature_init=fi) for b in sample}
+    ref, pos = [], 0
+    for si, nch in enumerate(plan):
+        if si == reset_at:
+            for b in reset_ids:
+                orc[b].reset(feature_init=fi)
+        rows = []
+        for b in sample:
+            assert orc[b](pcm[b, pos:pos + nch * 1280]) == nch * 1280
+            r = []
             for h in hs:
-                ref = oheads.forward(h, o.get_features(h["n_in"]))[0]
-                worst = max(worst, float(np.abs(ref - got[k, b, col:col + ref.size]).max()))
-                col += ref.size
-    print(f"split_from={split_from}: max |score - oracle| = {worst:.3e}")
-    assert worst < tol
+                g = [oheads.forward(h, orc[b].get_features(h["n_in"], -h["n_in"] - i))[0] for i in range(nch - 1, -1, -1)]
+                r.append(np.max(np.stack(g), axis=0))
+            rows.append(np.concatenate(r))
+        ref.append(np.stack(rows))
+        pos += nch * 1280
+    _SPLIT_CASE.update(B=B, hs=hs, fi=fi, plan=plan, reset_at=reset_at, reset_ids=reset_ids, pcm=pcm, sample=sample,
+                       ref=ref, mel={b: orc[b].melspectrogram_buffer[-76:].copy() for b in sample},
+                       feat={b: orc[b].feature_buffer[-40:].copy() for b in sample})
+    return _SPLIT_CASE
+
+
+# feature ring (last 40 rows) against the oracle: fp32-grade from layer 3 / 7 on; at 11 / 15 / 20 the budget of the
+# default-split tests (the CPU study predicts embedding errors of 1.9e-4 / 4.2e-4 / 5.4e-4 / 1.7e-3 / 3.3e-3 on 48 windows
+# for split 3 / 7 / 11 / 15 / 20)
+SPLIT_FEAT_TOL = {3: 2e-3, 7: 2e-3, 11: 8e-3, 15: 8e-3, 20: 8e-3}
+
+
+@pytest.mark.gpu
+@pytest.mark.parametrize("split_from,tol", [(3, 1e-3), (7, 1e-3), (11, 1e-3), (15, 1e-3), (20, 1e-3)])
+def test_split_from_variants_vs_oracle(torch_cuda, built_library, split_from, tol):
+    """Every split point cnn_mode 3 accepts, against the oracle: conv layers >= split_from on split operands (the fused
+    kernel runs layers 0 .. split_from-1: tc_inc_kernel<0> at 3 / 7 - whose late chain keeps the plane-major window
+    layout and runs the split convs <4,48>, <6,48>, <6,80>, <10,80> - and <11> / <15>), and plain fp16 everywhere
+    (20: one launch per step).  151 streams, 1-, 2- and 3-chunk calls and a partial reset (see _split_case)."""
+    from openwakeword_b200.engine import StreamEngine
+    c = _split_case()
+    B, pcm, sample = c["B"], c["pcm"], c["sample"]
+    eng = StreamEngine(c["hs"], B, embedding=emb_weights(), feature_init=c["fi"], cnn_mode=3, split_from=split_from,
+                       max_chunks=3)
+    worst, pos = 0.0, 0
+    for si, nch in enumerate(c["plan"]):
+        if si == c["reset_at"]:
+            eng.reset(c["fi"], stream_ids=c["reset_ids"])
+        got = eng.step_host(np.ascontiguousarray(pcm[:, pos:pos + nch * 1280]), nch)
+        pos += nch * 1280
+        d = np.abs(got[sample] - c["ref"][si])
+        assert np.isfinite(got).all()
+        assert d.max() < tol, (si, sample[int(np.argmax(d.max(1)))], float(d.max()))
+        worst = max(worst, float(d.max()))
+    mel_err = max(float(np.abs(eng.ctx.get_mel(b, 76) - c["mel"][b]).max()) for b in sample)
+    feat_err = max(float(np.abs(eng.ctx.get_features(b, 40) - c["feat"][b]).max()) for b in sample)
+    eng.ctx.close()
+    print(f"split_from={split_from}: max |score - oracle| = {worst:.3e}, mel ring {mel_err:.3e}, "
+          f"feature ring {feat_err:.3e} ({len(sample)} streams of {B})")
+    assert mel_err < 5e-3
+    assert feat_err < SPLIT_FEAT_TOL[split_from]

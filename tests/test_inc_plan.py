@@ -1,7 +1,7 @@
 """not-gpu: replay the fused incremental-CNN kernel's geometry plan (csrc/cnn_tc_inc.cu) in NumPy.
 
 The plan (buffer pitches, tap offsets, tail regions, pool geometry, smem offsets) is computed on
-the host by the library and exported through ``oww_debug_inc_plan``; this test executes the same
+the host by the library and exported through ``oww_debug_inc_plan`` (cut plans: ``oww_debug_inc_cut_plan``); this test executes the same
 data movement the kernel does - position order (t, stream, f), taps as unit shifts, tails loaded
 into rows 0..1, new tails written back - with exact float64 arithmetic, and checks that a stream
 of incremental steps reproduces the oracle's full 76-row-window embeddings (SURVEY.md F10).
@@ -20,15 +20,89 @@ NAMES = ("kh3 final W Wp rows_in T_out M cg_in cgp np cg_out in_buf out_buf in_b
 LEAK, FLOOR = float(embedding.LEAK), float(embedding.FLOOR)
 
 
-def get_plan(G, n_streams, built_library):
+OWW_EUNSUPPORTED = -4
+
+
+def get_plan(G, n_streams, built_library, n_layers=0):
+    """n_layers 0 = the full 20-layer plan; otherwise the cut plan of split_from = n_layers. None if the builder
+    rejects the plan as not fitting (OWW_EUNSUPPORTED)."""
     buf = (C.c_int32 * 4096)()
-    n = built_library.oww_debug_inc_plan(None, G, n_streams, buf, 4096)
+    if n_layers:
+        n = built_library.oww_debug_inc_cut_plan(None, G, n_streams, n_layers, buf, 4096)
+    else:
+        n = built_library.oww_debug_inc_plan(None, G, n_streams, buf, 4096)
+    if n == OWW_EUNSUPPORTED:
+        return None
     assert n > 0
     a = np.array(buf[:n])
     hdr = dict(zip("G n_groups tail_units x_units y_units w_total_bytes smem_bytes pad".split(), a[:8]))
     layers = [dict(zip(NAMES, map(int, row))) for row in a[8:8 + 20 * len(NAMES)].reshape(20, len(NAMES))]
-    assert int(a[8 + 20 * len(NAMES)]) == 20                      # n_layers: the exported plan is the full 20-layer one
+    assert int(a[8 + 20 * len(NAMES)]) == (n_layers or 20)       # n_layers: the conv layers inside the kernel
     return hdr, layers
+
+
+def check_plan_structure(hdr, layers, NL):
+    """Structural invariants of a plan with NL layers inside the kernel (the last one pooled and, for NL < 20, cut:
+    its unpooled hi/lo output stays in the temp and leaves the kernel).  Offsets are 16-byte units above the 2048-byte
+    arena base; weight slots are byte offsets."""
+    top = 227 * 1024
+    assert hdr["smem_bytes"] <= top
+    assert all(L["w_smem"] == 0 for L in layers[NL:])            # no weight slot for a layer outside the kernel
+    wsz = [((L["w_bytes"] + 127) & ~127) if 1 <= l < NL else 0 for l, L in enumerate(layers)]
+    act_end = [0] * NL
+    for l in range(NL):
+        L = layers[l]
+        cut = l == NL - 1 and NL < 20
+        if cut:
+            assert L["pool_t"], "a cut plan ends behind a pooled layer"
+        # tensors alive while the phase's MMAs run: its input, and its output (the unpooled temp of a pooled layer)
+        spans = []
+        if l > 0:
+            spans.append((L["in_base"], L["in_base"] + layers[l - 1]["nx_pitch"] * layers[l - 1]["cg_out"]))
+        if L["pool_t"]:
+            spans.append((L["tmp_base"], L["tmp_base"] + L["tmp_pitch"] * L["cg_out"] * (2 if cut else 1)))
+        if not L["final"] and not L["pool_t"] and not cut:
+            spans.append((L["nx_base"], L["nx_base"] + L["nx_pitch"] * L["cg_out"]))
+        spans.sort()
+        for (a0, a1), (b0, b1) in zip(spans, spans[1:]):
+            assert a1 <= b0, (NL, l, spans)
+        if L["pool_t"] and not cut:
+            # the pool pass reads the temp while it writes the pooled tensor (over the dead input)
+            t0, t1 = L["tmp_base"], L["tmp_base"] + L["tmp_pitch"] * L["cg_out"]
+            n0, n1 = L["nx_base"], L["nx_base"] + L["nx_pitch"] * L["cg_out"]
+            assert t1 <= n0 or n1 <= t0, (NL, l, (t0, t1), (n0, n1))
+            spans.append((n0, n1))
+        act_end[l] = 2048 + 16 * max((e for _, e in spans), default=0)
+        if l >= 1:
+            # weight slot of this layer and the prefetch of the next one: inside the arena, apart, above the activations
+            assert 0 < L["w_smem"] and L["w_smem"] + wsz[l] <= top, (NL, l)
+            if l + 1 < NL:
+                nxt = layers[l + 1]
+                assert nxt["w_smem"] + wsz[l + 1] <= L["w_smem"] or L["w_smem"] + wsz[l] <= nxt["w_smem"], (NL, l)
+            wl = min(L["w_smem"], layers[l + 1]["w_smem"] if l + 1 < NL else 1 << 30)
+            assert act_end[l] <= wl, (NL, l, spans, wl)
+            assert act_end[l - 1] <= L["w_smem"], (NL, l)        # slot l is filled during phase l - 1
+    return act_end
+
+
+@pytest.mark.parametrize("n_layers", [3, 7, 11, 15, 20])
+@pytest.mark.parametrize("G", list(range(1, 8)))
+def test_cut_plans_fit_shared_memory(built_library, n_layers, G):
+    """Every cut point mode 3 accepts (split_from 3 / 7 / 11 / 15, and 20 = no cut) and every group size 1..7: the
+    plan the library would build keeps its live tensors apart and clear of the weight slots.  Plans the builder
+    rejects as not fitting are the ones oww_inc_alloc_streams skips."""
+    got = get_plan(G, 151, built_library, n_layers)
+    if got is None:
+        pytest.skip(f"the builder rejects G={G} at n_layers={n_layers}")
+    hdr, layers = got
+    assert hdr["G"] == G and hdr["n_groups"] == (151 + G - 1) // G
+    check_plan_structure(hdr, layers, n_layers)
+
+
+def test_cut_plan_has_a_group_size(built_library):
+    """Each cut point has at least one feasible group size (else set_streams fails in mode 3)."""
+    for n_layers in (3, 7, 11, 15, 20):
+        assert any(get_plan(G, 151, built_library, n_layers) is not None for G in range(1, 8)), n_layers
 
 
 def act(x):
@@ -156,23 +230,8 @@ class Emu:
 @pytest.mark.parametrize("G", [7, 4, 1])
 def test_fused_plan_reproduces_full_window_embeddings(built_library, G):
     hdr, layers = get_plan(G, G, built_library)
-    assert hdr["smem_bytes"] <= 227 * 1024
-    # live tensors of a phase never overlap each other or the weight slots in use (weights start at w_smem - 2048 bytes)
-    for l, L in enumerate(layers):
-        spans = []
-        if l > 0:
-            spans.append((L["in_base"], L["in_base"] + layers[l - 1]["nx_pitch"] * layers[l - 1]["cg_out"]))
-        if L["pool_t"]:
-            spans.append((L["tmp_base"], L["tmp_base"] + L["tmp_pitch"] * L["cg_out"]))
-        if not L["final"] and not L["pool_t"]:
-            spans.append((L["nx_base"], L["nx_base"] + L["nx_pitch"] * L["cg_out"]))
-        spans.sort()
-        for (a0, a1), (b0, b1) in zip(spans, spans[1:]):
-            assert a1 <= b0, (l, spans)
-        if l >= 1:
-            wl = min(L["w_smem"], layers[l + 1]["w_smem"] if l + 1 < 20 else 1 << 30)
-            assert 2048 + 16 * max(e for _, e in spans) <= wl, (l, spans, wl)
-    # weight slots never overlap the activations alive in the same or the previous phase (checked by the builder)
+    # live tensors of a phase never overlap each other or the weight slots in use
+    check_plan_structure(hdr, layers, 20)
     w = emb_weights()
     rng = np.random.default_rng(3)
     n_steps = 3
