@@ -73,10 +73,8 @@ typedef struct oww_config {
                               bit 3: 1 = one tensor-core heads CTA per (128 streams, head) reading the fp32 rings
                               (heads_tc.cu) instead of one CTA per 128 streams for all heads that share a window,
                               fed from the fp16 mirror of the rings (heads_grp.cu);
-                              bit 4: 1 = the incremental late (3,1) layers keep the window-mode tensor layout
-                              (per-stream [tails | new rows] x (W+1): most accumulator rows of a tile are not outputs)
-                              instead of the block-major layout of tc_conv_blk_kernel;
-                              bit 5: 1 = no programmatic dependent launches inside the late chain.
+                              bit 5: 1 = no programmatic dependent launches inside the late chain;
+                              bit 4 and bits 6 and up are ignored.
                               reserved[1]: first conv layer that takes fp16 hi/lo split operands in the
                               tensor-core modes (0 = default 11; 20 = plain fp16 everywhere): 2..20 in
                               OWW_CNN_TC_WINDOW; OWW_CNN_TC_INCREMENTAL accepts only 3, 7, 11, 15 and 20 (the

@@ -121,14 +121,14 @@ class Context:
     """One handle = one GPU's weights + stream state (include/owwb200.h conventions)."""
 
     def __init__(self, device=0, max_chunks=4, cnn_mode=CNN_TC_INCREMENTAL, window_batch=0, fuse_step=True,
-                 tc_heads=True, tc_heads_terms=3, split_from=None, group_heads=True, late_blocked=True):
+                 tc_heads=True, tc_heads_terms=3, split_from=None, group_heads=True):
         """split_from: first conv layer that takes fp16 hi/lo split operands in the tensor-core modes (fp32-grade products;
         11 = default: scores within ~2e-4 of the fp32 graph; 20 = plain fp16 everywhere: the whole step as ONE fused
         launch, ~9e-4)."""
         self.lib = load_library()
         cfg = Config(device=device, max_chunks=max_chunks, cnn_mode=cnn_mode, window_batch=window_batch)
         cfg.reserved[0] = ((0 if fuse_step else 1) | (0 if tc_heads else 2) | (4 if tc_heads_terms == 1 else 0)
-                           | (0 if group_heads else 8) | (0 if late_blocked else 16)
+                           | (0 if group_heads else 8)
                            | int(os.environ.get("OWW_FLAGS", "0"), 0))      # extra reserved[0] bits for A/B runs (include/owwb200.h)
         if split_from is None:                      # library default (0), or OWW_SPLIT_FROM for experiments
             split_from = int(os.environ.get("OWW_SPLIT_FROM", "0"))

@@ -68,15 +68,10 @@ __global__ void reset_kernel(const int* ids, int n_ids, int n_streams, int16_t* 
             const ResetLate& T = rt.late[k];
             for (int i = threadIdx.x; i < T.n_planes * 2 * T.Wp; i += blockDim.x) {
                 const int pl = i / (2 * T.Wp), u = i - pl * 2 * T.Wp, r = u / T.Wp, f = u - r * T.Wp;
+                if (f >= T.lay.Wq) continue;                // block-major layout (cnn_tc.cu, tc_conv_blk_kernel): no pad column
                 const uint4 v = T.tmpl[i];
-                if (T.lay.S) {                              // block-major layout (cnn_tc.cu, tc_conv_blk_kernel): no pad column
-                    if (f >= T.lay.Wq) continue;
-                    T.now[late_unit(T.lay, pl, b, r, f)] = v;
-                    if (T.next && r == 1) T.next[late_unit(T.lay, pl, b, 0, f)] = v;
-                    continue;
-                }
-                T.now[(int64_t)pl * T.plane + 8 + ((int64_t)b * T.T_buf + r) * T.Wp + f] = v;
-                if (T.next && r == 1) T.next[(int64_t)pl * T.plane + 8 + ((int64_t)b * T.T_buf + 0) * T.Wp + f] = v;
+                T.now[late_unit(T.lay, pl, b, r, f)] = v;
+                if (T.next && r == 1) T.next[late_unit(T.lay, pl, b, 0, f)] = v;
             }
         }
     }
@@ -117,7 +112,7 @@ void free_streams(oww_ctx* c) {
     cudaFree(c->d_scores_tmp);
     oww_heads_grp_drop_mirror(c);
     for (auto& X : c->late_x) for (auto& b : X.buf) { cudaFree(b); b = nullptr; }
-    cudaFree(c->d_late_tmp[0]); c->d_late_tmp[0] = nullptr;
+    cudaFree(c->d_late_tmp); c->d_late_tmp = nullptr;
     cudaFree(c->d_late_template); c->d_late_template = nullptr;
     c->late_active = false;
     c->d_tail = nullptr; c->d_seen = c->d_mel_count = c->d_feat_count = nullptr;
@@ -283,8 +278,7 @@ int reset_enqueue(oww_ctx* ctx, const int32_t* h_stream_ids, int n, const float*
                 T.now = reinterpret_cast<uint4*>(X.buf[k % X.n_buf]);
                 T.next = X.n_buf == 3 ? reinterpret_cast<uint4*>(X.buf[(k + 1) % 3]) : nullptr;
                 T.tmpl = reinterpret_cast<const uint4*>(ctx->d_late_template) + X.tmpl_off;
-                T.plane = X.plane; T.T_buf = X.T_buf; T.Wp = X.W + 1; T.n_planes = 2 * X.cg;
-                T.lay = X.lay;
+                T.Wp = X.W + 1; T.n_planes = 2 * X.cg; T.lay = X.lay;
             }
         }
     }
@@ -335,7 +329,6 @@ int oww_create(const oww_config* cfg, oww_ctx** out) {
     ctx->split_from = (cfg->reserved[1] >= 2 && cfg->reserved[1] <= OWW_N_CONV) ? cfg->reserved[1] : 11;
     ctx->tc_heads_terms = (cfg->reserved[0] & 4) ? 1 : 3;
     ctx->grp_heads = (cfg->reserved[0] & 8) == 0;
-    ctx->late_blocked_ok = (cfg->reserved[0] & 16) == 0;
     ctx->late_pdl = (cfg->reserved[0] & 32) == 0;
     cudaStreamCreateWithFlags(&ctx->own_stream, cudaStreamNonBlocking);
     cudaStreamCreateWithFlags(&ctx->copy_stream, cudaStreamNonBlocking);

@@ -116,12 +116,6 @@ struct TcConvArgs {
     int n_tiles;
     int out_split;                          // 1: write fp16 hi planes [0, cg_out) and lo planes [cg_out, 2 cg_out) (y = hi + lo)
     int64_t rows_out;                       // final layer: embedding rows per window (T_out valid rows; fully convolutional clips)
-    // incremental late layers on plane-major tensors (the reserved[0] bit-4 fallback; the default chain runs
-    // tc_conv_blk_kernel below): the output rows land at row offset out_toff inside buffers that hold
-    // out_T rows per stream (tails in front), and are mirrored into up to two further buffers where they will serve as
-    // tails of later steps.  out_T == 0: plain layout (out_T = T_out, no offset, no mirrors).
-    int out_T, out_toff;
-    __half* out_b[2]; int out_b_toff[2];    // mirrors (nullptr = unused); same plane pitch as `out`
 };
 
 // TERMS = 1: fp16 operands.  TERMS = 3: split operands - the input holds hi planes [0, cg_in) and lo planes
@@ -279,8 +273,7 @@ __global__ void __launch_bounds__(kTcThreads, 1) tc_conv_kernel(TcConvArgs a) {
                     }
                     continue;
                 }
-                const int64_t po = a.out_T ? (int64_t)n * a.out_T * Wp + (int64_t)(t + a.out_toff) * Wp + f
-                                           : (int64_t)n * per_out + (int64_t)t * Wp + f;
+                const int64_t po = (int64_t)n * per_out + (int64_t)t * Wp + f;
                 uint4* o = reinterpret_cast<uint4*>(a.out) + kGuard + po;
                 const bool pad = f == a.W;
 #pragma unroll
@@ -302,16 +295,6 @@ __global__ void __launch_bounds__(kTcThreads, 1) tc_conv_kernel(TcConvArgs a) {
                         reinterpret_cast<uint32_t*>(o + (int64_t)(a.cg_out + g) * a.out_plane)[q] = lw;
                         if (po == 0) reinterpret_cast<uint32_t*>(o + (int64_t)(a.cg_out + g) * a.out_plane - 1)[q] = 0u;
                     }
-                    // a mirror takes only the rows that become tails there: with 4 new rows per step (split_from 3 / 7)
-                    // rows 0, 1 map before the stream's slot - for stream 0 before the start of the allocation
-#pragma unroll
-                    for (int kk = 0; kk < 2; ++kk)
-                        if (a.out_b[kk] && t + a.out_b_toff[kk] >= 0) {
-                            uint4* ob = reinterpret_cast<uint4*>(a.out_b[kk]) + kGuard + (int64_t)n * a.out_T * Wp +
-                                        (int64_t)(t + a.out_b_toff[kk]) * Wp + f;
-                            reinterpret_cast<uint32_t*>(ob + (int64_t)g * a.out_plane)[q] = hw;
-                            if (a.out_split) reinterpret_cast<uint32_t*>(ob + (int64_t)(a.cg_out + g) * a.out_plane)[q] = lw;
-                        }
                 }
             }
         }
@@ -319,11 +302,11 @@ __global__ void __launch_bounds__(kTcThreads, 1) tc_conv_kernel(TcConvArgs a) {
 }
 
 // ---------------------------------------------------------------- incremental late layers: block-major tensors
-// The window-mode kernel above can run a layer of the incremental chain on per-stream "windows" [2 tails | new rows] x
-// (W + 1) in plane-major HBM tensors.  Two things make that slow there: of the 128 accumulator rows of a (3,1) tile only
-// rows_new / T carry outputs and one column in W + 1 is padding (layer 16: 4 of 12 positions, layer 19: 1 of 6) while an
-// MMA costs the same; and a tile's channel-group planes are far apart in HBM, i.e. 24 bulk copies of 2-4 KB per tile.
-// Here a late tensor is stored in blocks of S streams, a block being [2*cg planes][units] CONTIGUOUS in HBM (LateLay):
+// The layers of the incremental chain see per-stream "windows" [2 tails | new rows].  In the plane-major layout of the
+// window-mode kernel above, only rows_new / T of a (3,1) tile's 128 accumulator rows would carry outputs and one column
+// in W + 1 would be padding (layer 16: 4 of 12 positions, layer 19: 1 of 6) while an MMA costs the same, and a tile's
+// channel-group planes would lie far apart in HBM (24 bulk copies of 2-4 KB per tile).
+// So a late tensor is stored in blocks of S streams, a block being [2*cg planes][units] CONTIGUOUS in HBM (LateLay):
 //   input of a (3,1) layer: time-major inside the block, no pad column: unit (row*S + s)*W + f.  Tap k of the conv reads
 //     rows k .. k + rows_new - 1 = one contiguous run of rows_new*S*W = 128 units at offset k*S*W: every accumulator row
 //     is an output;
@@ -516,7 +499,7 @@ __global__ void __launch_bounds__(kTcThreads, 1) tc_conv_blk_kernel(TcBlkArgs a)
 // ---------------------------------------------------------------- max-pool on fp16 planes
 // split != 0: planes [0, cg) hold hi parts and [cg, 2cg) lo parts of the same values; the pooled element is the one
 // with the largest hi + lo, i.e. the lexicographic maximum of (hi, lo) since |lo| <= ulp(hi)/2.
-struct PoolOut { __half* p[3]; int toff[3]; int out_T; LateLay lay = {0, 0, 0, 0, 0, 0}; };   // out_T == 0: plain [n][t_out][wp_out] into p[0]; lay.S > 0: block-major destination
+struct PoolOut { __half* p[3]; int toff[3]; LateLay lay = {0, 0, 0, 0, 0, 0}; };   // lay.S == 0: plain [n][t_out][wp_out] into p[0]; lay.S > 0: block-major destination(s)
 __global__ void __launch_bounds__(256) tc_pool_kernel(const __half* in, int64_t in_plane, PoolOut po, int64_t out_plane,
                                                       int n, int t_in, int w_in, int cg, int pt, int pf, int split) {
     __half* const out = po.p[0];
@@ -555,26 +538,19 @@ __global__ void __launch_bounds__(256) tc_pool_kernel(const __half* in, int64_t 
             res = *reinterpret_cast<uint4*>(mh);
             res_lo = *reinterpret_cast<uint4*>(ml);
         }
-        if (po.out_T == 0) {
+        if (po.lay.S == 0) {
             reinterpret_cast<uint4*>(out)[(int64_t)g * out_plane + kGuard + p] = res;
             if (p == 0) reinterpret_cast<uint4*>(out)[(int64_t)g * out_plane + kGuard - 1] = make_uint4(0, 0, 0, 0);
             if (split) {
                 reinterpret_cast<uint4*>(out)[(int64_t)(cg + g) * out_plane + kGuard + p] = res_lo;
                 if (p == 0) reinterpret_cast<uint4*>(out)[(int64_t)(cg + g) * out_plane + kGuard - 1] = make_uint4(0, 0, 0, 0);
             }
-        } else {
+        } else if (f < w_out) {                                         // block-major: pad column untouched (zero since allocation)
 #pragma unroll
             for (int k = 0; k < 3; ++k)
                 if (po.p[k] && t + po.toff[k] >= 0) {                  // mirrors: only the rows that become tails
-                    if (po.lay.S) {                                     // block-major: pad column untouched (zero since allocation)
-                        if (f >= w_out) continue;
-                        reinterpret_cast<uint4*>(po.p[k])[late_unit(po.lay, g, (int)s, t + po.toff[k], f)] = res;
-                        if (split) reinterpret_cast<uint4*>(po.p[k])[late_unit(po.lay, cg + g, (int)s, t + po.toff[k], f)] = res_lo;
-                        continue;
-                    }
-                    const int64_t q = kGuard + (s * po.out_T + t + po.toff[k]) * wp_out + f;
-                    reinterpret_cast<uint4*>(po.p[k])[(int64_t)g * out_plane + q] = res;
-                    if (split) reinterpret_cast<uint4*>(po.p[k])[(int64_t)(cg + g) * out_plane + q] = res_lo;
+                    reinterpret_cast<uint4*>(po.p[k])[late_unit(po.lay, g, (int)s, t + po.toff[k], f)] = res;
+                    if (split) reinterpret_cast<uint4*>(po.p[k])[late_unit(po.lay, cg + g, (int)s, t + po.toff[k], f)] = res_lo;
                 }
         }
     }
@@ -596,8 +572,6 @@ __global__ void tc_unpack_kernel(const __half* in, int64_t plane, float* out, in
         out[i] = v;
     }
 }
-
-struct TcLayerGeom { int T, W, cg, cgp, np, T_out, rows, lo, tap_off[3]; };
 
 inline int round8(int v) { return (v + 7) & ~7; }
 
@@ -623,20 +597,13 @@ template <int CGP, int NP>
 int launch_tc_blk(oww_ctx* ctx, const TcBlkArgs& a, cudaStream_t s) {
     const size_t smem = (size_t)2 * 3 * CGP * NP * 16 + (size_t)2 * CGP * a.lay.units * 16 + 8 * 6 + 2 * NP * sizeof(float);
     if (smem > 227 * 1024) return oww_fail(ctx, OWW_EUNSUPPORTED, "blocked late conv tile does not fit shared memory (%zu bytes)", smem);
-    const uint32_t bit = 1u << (CGP / 2);
+    const uint32_t bit = 1u << (CGP / 2 + NP / 16);                    // distinct for the instances in use
     if (!(ctx->tc_blk_attr_mask & bit)) {
         OWW_CUDA(ctx, cudaFuncSetAttribute(tc_conv_blk_kernel<CGP, NP>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
         ctx->tc_blk_attr_mask |= bit;
     }
     const int grid = ctx->sm_count < a.n_tiles ? ctx->sm_count : a.n_tiles;
-    cudaLaunchConfig_t cfg;
-    std::memset(&cfg, 0, sizeof(cfg));
-    cfg.gridDim = dim3(grid); cfg.blockDim = dim3(kTcThreads); cfg.dynamicSmemBytes = smem; cfg.stream = s;
-    cudaLaunchAttribute at[1];
-    at[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-    at[0].val.programmaticStreamSerializationAllowed = ctx->late_pdl ? 1 : 0;
-    cfg.attrs = at; cfg.numAttrs = 1;
-    OWW_CUDA(ctx, cudaLaunchKernelEx(&cfg, tc_conv_blk_kernel<CGP, NP>, a));
+    OWW_CUDA(ctx, oww_launch_pdl(ctx->late_pdl, tc_conv_blk_kernel<CGP, NP>, dim3(grid), dim3(kTcThreads), smem, s, a));
     OWW_LAUNCH_CHECK(ctx);
     return OWW_OK;
 }
@@ -848,12 +815,13 @@ int oww_cnn_tc_pyramid_impl(oww_ctx* ctx, const WindowSrc& src, int n, int T0, i
 // Incremental late layers (cnn_mode 3 with split_from < 20).
 //
 // The fused step kernel (cnn_tc_inc.cu) runs the frontend and conv layers 0 .. L0-1 of the 8 new mel rows in shared
-// memory and leaves the pooled output of layer L0-1 (2 new rows per stream at L0 = 11) in HBM as fp16 hi/lo planes.
-// Layers L0 .. 19 - 1.3 of the 5.6 MMAC per frame, but the ones whose fp16 rounding dominates the embedding error -
-// then run here as the SAME tensor-core conv / pool kernels as the window mode, with split (hi/lo) operands, on "windows"
-// that are the incremental rows of every stream: a (3,1) layer's input holds [2 tail rows | new rows] per stream, and
-// every layer mirrors its new rows into the buffer(s) where they are tails of the following step(s) (two buffers for
-// tensors that gain two rows per step, three for the one that gains a single row), so no copy or shift pass exists.
+// memory and leaves the pooled output of layer L0-1 (2 new rows per stream at L0 = 11) in HBM as fp16 hi/lo planes in
+// the block-major layout.  Layers L0 .. 19 - 1.3 of the 5.6 MMAC per frame at L0 = 11, but the ones whose fp16 rounding
+// dominates the embedding error - then run here as tc_conv_blk_kernel (the MMA terms of the window-mode conv, in the same
+// order; (1,2) pools fused into its epilogue) and tc_pool_kernel for the (2,2) pools, on the incremental rows of every
+// stream: a (3,1) layer's input holds [2 tail rows | new rows] per stream, and every layer mirrors its new rows into
+// the buffer(s) where they are tails of the following step(s) (two buffers for tensors that gain two or four rows per
+// step, three for the one that gains a single row), so no copy or shift pass exists.
 // A reset writes the tails of the all-ones window (template) into the slots the stream's next step reads.
 // ================================================================================================
 namespace {
@@ -872,7 +840,7 @@ __global__ void late_capture_kernel(const uint4* planes, int64_t plane_pitch, in
 int oww_late_alloc(oww_ctx* ctx) {
     // geometry of the incremental tensors X_l (input of conv layer l), l = L0 .. 19
     for (auto& X : ctx->late_x) for (auto& b : X.buf) { cudaFree(b); b = nullptr; }
-    for (auto& b : ctx->d_late_tmp) { cudaFree(b); b = nullptr; }
+    cudaFree(ctx->d_late_tmp); ctx->d_late_tmp = nullptr;
     cudaFree(ctx->d_late_template); ctx->d_late_template = nullptr;
     ctx->late_active = false;
     const int L0 = ctx->split_from;
@@ -883,34 +851,22 @@ int oww_late_alloc(oww_ctx* ctx) {
     int rows = 8, W = 32;
     for (int l = 0; l < L0; ++l) if (ctx->conv[l].pool_t) { rows /= ctx->conv[l].pool_t; W /= ctx->conv[l].pool_f; }
     size_t tmpl_units = 0, tmp_units = 0;
-    // the block-major kernel is instantiated for 72 / 96 -> 96 channels (every layer from 11 on)
-    bool blocked = ctx->late_blocked_ok;
-    for (int l = L0; l < OWW_N_CONV; ++l) if ((ctx->conv[l].cin != 96 && ctx->conv[l].cin != 72) || ctx->conv[l].cout != 96) blocked = false;
     for (int l = L0; l < OWW_N_CONV; ++l) {
         const ConvLayer& C = ctx->conv[l];
         oww_ctx::LateTensor& X = ctx->late_x[l];
         const bool kh3 = C.kh == 3;
         X.rows_new = rows; X.W = W; X.cg = C.cin / 8;
-        X.T_buf = rows + (kh3 ? 2 : 0);
         X.n_buf = kh3 ? (rows == 1 ? 3 : 2) : 1;
         // block-major layout (tc_conv_blk_kernel): S streams per block so that the block's positions fill the 128
         // accumulator rows ((3,1): rows*S*W outputs, and the whole [T][S][W] block <= 256 units per plane)
-        X.lay = LateLay{0, 0, 0, 0, 0, 0};
-        size_t buf_units;
-        if (blocked) {
-            LateLay& Y = X.lay;
-            Y.kh3 = kh3 ? 1 : 0; Y.T = X.T_buf; Y.Wq = kh3 ? W : W + 1;
-            Y.S = std::max(1, 128 / (rows * Y.Wq));
-            if (kh3) while (Y.S > 1 && X.T_buf * Y.S * W > 256) Y.S /= 2;
-            const int tap = kh3 ? Y.S * W : 1;
-            Y.units = round8(std::max((kh3 ? 0 : 1) + Y.T * Y.S * Y.Wq, 2 * tap + 128));
-            Y.blk_stride = (int64_t)2 * X.cg * Y.units;
-            buf_units = (size_t)((n + Y.S - 1) / Y.S) * Y.blk_stride;
-            X.plane = 0;
-        } else {
-            X.plane = (int64_t)((kGuard + (int64_t)n * X.T_buf * (W + 1) + kGuardBack + 7) & ~7LL);
-            buf_units = (size_t)2 * X.cg * X.plane;
-        }
+        LateLay& Y = X.lay;
+        Y.kh3 = kh3 ? 1 : 0; Y.T = rows + (kh3 ? 2 : 0); Y.Wq = kh3 ? W : W + 1;
+        Y.S = std::max(1, 128 / (rows * Y.Wq));
+        if (kh3) while (Y.S > 1 && Y.T * Y.S * W > 256) Y.S /= 2;
+        const int tap = kh3 ? Y.S * W : 1;
+        Y.units = round8(std::max((kh3 ? 0 : 1) + Y.T * Y.S * Y.Wq, 2 * tap + 128));
+        Y.blk_stride = (int64_t)2 * X.cg * Y.units;
+        const size_t buf_units = (size_t)((n + Y.S - 1) / Y.S) * Y.blk_stride;
         X.tmpl_off = kh3 ? (int)tmpl_units : -1;
         if (kh3) tmpl_units += (size_t)2 * X.cg * 2 * (W + 1);
         for (int k = 0; k < X.n_buf; ++k) {
@@ -924,8 +880,8 @@ int oww_late_alloc(oww_ctx* ctx) {
         }
     }
     if (tmp_units) {
-        OWW_CUDA(ctx, cudaMalloc(&ctx->d_late_tmp[0], tmp_units * 16));
-        OWW_CUDA(ctx, cudaMemset(ctx->d_late_tmp[0], 0, tmp_units * 16));
+        OWW_CUDA(ctx, cudaMalloc(&ctx->d_late_tmp, tmp_units * 16));
+        OWW_CUDA(ctx, cudaMemset(ctx->d_late_tmp, 0, tmp_units * 16));
     }
     OWW_CUDA(ctx, cudaMalloc(&ctx->d_late_template, std::max<size_t>(tmpl_units, 1) * 16));
     OWW_CUDA(ctx, cudaMemset(ctx->d_late_template, 0, std::max<size_t>(tmpl_units, 1) * 16));
@@ -943,110 +899,63 @@ int oww_late_chain(oww_ctx* ctx, float* d_emb, cudaStream_t s) {
         const oww_ctx::LateTensor& X = ctx->late_x[l];
         const bool last = l == OWW_N_CONV - 1;
         const int cg = C.cin / 8, cgp = (cg + 1) & ~1, np = (C.cout + 15) & ~15;
-        const int W = X.W, Wp = W + 1, T = X.T_buf, T_out = X.rows_new;
-        // where the output rows go: the next layer's input buffers (or the unpooled temp)
-        auto route = [&](const oww_ctx::LateTensor& Y, __half** p, int* toff, int& n_out) {
-            n_out = 0;
-            if (Y.n_buf == 1) { p[0] = reinterpret_cast<__half*>(Y.buf[0]); toff[0] = 0; n_out = 1; return; }
-            const int r = Y.rows_new;                       // 2 -> two buffers, 1 -> three
+        const int W = X.W, T_out = X.rows_new;
+        // where the output rows go: the next layer's input buffers
+        auto route = [&](const oww_ctx::LateTensor& Y, __half** p, int* toff) {
+            if (Y.n_buf == 1) { p[0] = reinterpret_cast<__half*>(Y.buf[0]); toff[0] = 0; return; }
             for (int m = 0; m < Y.n_buf; ++m) {
                 p[m] = reinterpret_cast<__half*>(Y.buf[(k + m) % Y.n_buf]);
-                // this step: behind the two tails; later steps: as their tails.  With r = 4 (split_from 3 / 7) the mirror
-                // offset is -2: the kernels store only rows t with t + toff >= 0
-                toff[m] = 2 - m * r;
+                // this step: behind the two tails; later steps: as their tails.  With 4 new rows (split_from 3 / 7) the
+                // mirror offset is -2: the kernels store only rows t with t + toff >= 0
+                toff[m] = 2 - m * Y.rows_new;
             }
-            n_out = Y.n_buf;
         };
-        const int64_t tmp_plane = (int64_t)((kGuard + (int64_t)n * T_out * Wp + kGuardBack + 7) & ~7LL);
-        int rc;
-        bool pool_fused = false;
-        if (X.lay.S) {
-            // block-major input: one tile per block of S streams
-            TcBlkArgs b;
-            std::memset(&b, 0, sizeof(b));
-            b.in = reinterpret_cast<const __half*>(X.buf[X.n_buf == 1 ? 0 : (int)(k % X.n_buf)]);
-            b.lay = X.lay;
-            b.w = reinterpret_cast<const __half*>(ctx->d_tc_w3) + 2 * ctx->tc_w_off[l];
-            b.scale = ctx->d_tc_sb3 + ctx->tc_sb_off[l]; b.bias = b.scale + np;
-            b.n = n; b.W = W; b.rows_new = T_out;
-            b.m_valid = T_out * X.lay.S * X.lay.Wq;
-            b.tap = C.kh == 3 ? X.lay.S * W : 1;
-            b.cg_in = cg; b.cg_out = C.cout / 8; b.apply_act = last ? 0 : 1;
-            b.n_tiles = (n + X.lay.S - 1) / X.lay.S;
-            const bool fuse_pool = !last && C.pool_t == 1 && C.pool_f == 2 && X.lay.kh3 && (W & 1) == 0 && ctx->late_x[l + 1].lay.S > 0;
-            if (last) {
-                b.out_f32 = d_emb;
-            } else if (fuse_pool) {
-                // (1,2) max-pool in the epilogue: straight into the next layer's tensor, no temp, no pool launch
-                const oww_ctx::LateTensor& Y = ctx->late_x[l + 1];
-                int n_out = 0;
-                route(Y, b.out, b.out_toff, n_out);
-                b.out_lay = Y.lay;
-                b.pool_f = 2;
-                pool_fused = true;
-            } else if (C.pool_t) {
-                b.out[0] = reinterpret_cast<__half*>(ctx->d_late_tmp[0]);
-                b.out_plane = tmp_plane;
-            } else {
-                const oww_ctx::LateTensor& Y = ctx->late_x[l + 1];
-                int n_out = 0;
-                route(Y, b.out, b.out_toff, n_out);
-                b.out_lay = Y.lay;
-            }
-            if (cgp == 12 && np == 96) rc = launch_tc_blk<12, 96>(ctx, b, s);
-            else if (cgp == 10 && np == 96) rc = launch_tc_blk<10, 96>(ctx, b, s);
-            else rc = oww_fail(ctx, OWW_EUNSUPPORTED, "no block-major late conv instance for cgp=%d np=%d", cgp, np);
-            if (rc) return rc;
-        } else {
-        TcConvArgs a;
-        std::memset(&a, 0, sizeof(a));
-        a.in = reinterpret_cast<const __half*>(X.buf[X.n_buf == 1 ? 0 : (int)(k % X.n_buf)]);
-        a.in_plane = X.plane;
-        a.w = reinterpret_cast<const __half*>(ctx->d_tc_w3) + 2 * ctx->tc_w_off[l];
-        a.scale = ctx->d_tc_sb3 + ctx->tc_sb_off[l]; a.bias = a.scale + np;
-        a.n = n; a.T = T; a.W = W; a.T_out = T_out;
-        if (C.kw == 3) { a.lo = 1; a.tap_off[0] = 0; a.tap_off[1] = 1; a.tap_off[2] = 2; a.rows = round8(128 + 2); }
-        else { a.lo = 0; a.tap_off[0] = 0; a.tap_off[1] = Wp; a.tap_off[2] = 2 * Wp; a.rows = round8(128 + 2 * Wp); }
-        a.cg_in = cg; a.cg_out = C.cout / 8; a.apply_act = last ? 0 : 1;
-        a.p_in = (int64_t)n * T * Wp;
-        a.n_tiles = (int)((a.p_in + 127) / 128);
-        a.rows_out = T_out;
+        const int64_t tmp_plane = (int64_t)((kGuard + (int64_t)n * T_out * (W + 1) + kGuardBack + 7) & ~7LL);
+        // one tile per block of S streams
+        TcBlkArgs b;
+        std::memset(&b, 0, sizeof(b));
+        b.in = reinterpret_cast<const __half*>(X.buf[X.n_buf == 1 ? 0 : (int)(k % X.n_buf)]);
+        b.lay = X.lay;
+        b.w = reinterpret_cast<const __half*>(ctx->d_tc_w3) + 2 * ctx->tc_w_off[l];
+        b.scale = ctx->d_tc_sb3 + ctx->tc_sb_off[l]; b.bias = b.scale + np;
+        b.n = n; b.W = W; b.rows_new = T_out;
+        b.m_valid = T_out * X.lay.S * X.lay.Wq;
+        b.tap = C.kh == 3 ? X.lay.S * W : 1;
+        b.cg_in = cg; b.cg_out = C.cout / 8; b.apply_act = last ? 0 : 1;
+        b.n_tiles = (n + X.lay.S - 1) / X.lay.S;
+        // (1,2) max-pool in the epilogue: straight into the next layer's tensor, no temp, no pool launch
+        const bool fuse_pool = !last && C.pool_t == 1 && C.pool_f == 2 && X.lay.kh3 && (W & 1) == 0;
         if (last) {
-            a.out_f32 = d_emb;
-        } else if (C.pool_t) {
-            a.out = reinterpret_cast<__half*>(ctx->d_late_tmp[0]);
-            a.out_plane = tmp_plane;
-            a.out_split = 1;
+            b.out_f32 = d_emb;
+        } else if (C.pool_t && !fuse_pool) {
+            b.out[0] = reinterpret_cast<__half*>(ctx->d_late_tmp);
+            b.out_plane = tmp_plane;
         } else {
             const oww_ctx::LateTensor& Y = ctx->late_x[l + 1];
-            __half* p[3] = {nullptr, nullptr, nullptr}; int toff[3] = {0, 0, 0}; int n_out = 0;
-            route(Y, p, toff, n_out);
-            a.out = p[0]; a.out_plane = Y.plane; a.out_split = 1;
-            a.out_T = Y.T_buf; a.out_toff = toff[0];
-            for (int m = 1; m < n_out; ++m) { a.out_b[m - 1] = p[m]; a.out_b_toff[m - 1] = toff[m]; }
+            route(Y, b.out, b.out_toff);
+            b.out_lay = Y.lay;
+            b.pool_f = fuse_pool ? 2 : 0;
         }
-        rc = dispatch_tc<3>(ctx, cgp, np, a, s);
+        int rc;
+        if (cgp == 4 && np == 48) rc = launch_tc_blk<4, 48>(ctx, b, s);
+        else if (cgp == 6 && np == 48) rc = launch_tc_blk<6, 48>(ctx, b, s);
+        else if (cgp == 6 && np == 80) rc = launch_tc_blk<6, 80>(ctx, b, s);
+        else if (cgp == 10 && np == 80) rc = launch_tc_blk<10, 80>(ctx, b, s);
+        else if (cgp == 10 && np == 96) rc = launch_tc_blk<10, 96>(ctx, b, s);
+        else if (cgp == 12 && np == 96) rc = launch_tc_blk<12, 96>(ctx, b, s);
+        else rc = oww_fail(ctx, OWW_EUNSUPPORTED, "no block-major late conv instance for cgp=%d np=%d", cgp, np);
         if (rc) return rc;
-        }
-        if (C.pool_t && !last && !pool_fused) {
+        if (C.pool_t && !last && !fuse_pool) {
             const oww_ctx::LateTensor& Y = ctx->late_x[l + 1];
-            PoolOut po{{nullptr, nullptr, nullptr}, {0, 0, 0}, Y.T_buf};
-            po.lay = Y.lay;
-            int n_out = 0;
-            route(Y, po.p, po.toff, n_out);
+            PoolOut po{{nullptr, nullptr, nullptr}, {0, 0, 0}, Y.lay};
+            route(Y, po.p, po.toff);
             const int cgo = C.cout / 8;
             const int64_t total = (int64_t)n * Y.rows_new * (Y.W + 1) * cgo;
             unsigned grid = (unsigned)((total + 255) / 256);
             if (grid > (unsigned)ctx->sm_count * 16) grid = ctx->sm_count * 16;
-            cudaLaunchConfig_t cfg;
-            std::memset(&cfg, 0, sizeof(cfg));
-            cfg.gridDim = dim3(grid); cfg.blockDim = dim3(256); cfg.stream = s;
-            cudaLaunchAttribute at[1];
-            at[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-            at[0].val.programmaticStreamSerializationAllowed = ctx->late_pdl ? 1 : 0;
-            cfg.attrs = at; cfg.numAttrs = 1;
-            OWW_CUDA(ctx, cudaLaunchKernelEx(&cfg, tc_pool_kernel, reinterpret_cast<const __half*>(ctx->d_late_tmp[0]), tmp_plane, po,
-                                             Y.plane, n, T_out, W, cgo, C.pool_t, C.pool_f, 1));
+            OWW_CUDA(ctx, oww_launch_pdl(ctx->late_pdl, tc_pool_kernel, dim3(grid), dim3(256), 0, s,
+                                         reinterpret_cast<const __half*>(ctx->d_late_tmp), tmp_plane, po, (int64_t)0, n, T_out, W,
+                                         cgo, C.pool_t, C.pool_f, 1));
             OWW_LAUNCH_CHECK(ctx);
         }
     }

@@ -58,9 +58,8 @@ struct IncArgs {
     int hring_off, hslot_bytes, hns;                          // smem ring the producer streams the heads' first-layer weights through
     const Gate* gates; int n_gates;                           // conditional verifier pairs, applied after the heads phase
     // cut plan (plan.n_layers < 20): the pooled output of the last fused layer leaves the kernel as fp16 hi/lo planes in
-    // the block-major layout of the first incremental late layer's input (gx_lay, cnn_tc.cu), or - fallback - the
-    // plane-major window layout [plane][stream][row][f + pad]
-    uint4* gx; int64_t gx_plane; LateLay gx_lay;     // gx_lay.S > 0: block-major destination (cnn_tc.cu)
+    // the block-major layout of the first incremental late layer's input (gx_lay, cnn_tc.cu)
+    uint4* gx; LateLay gx_lay;
 };
 
 // Rows of a later head layer (K x D floats) per ring chunk: a multiple of 4 rows (16-byte chunk starts) that fits a slot.
@@ -556,14 +555,9 @@ __global__ void __launch_bounds__(kIncThreads, 1) tc_inc_kernel(const __grid_con
                                     res_lo = make_uint4(bl[0], bl[1], bl[2], bl[3]);
                                 }
                                 if (s_live[g]) {
-                                    const int64_t q = kGuard + ((int64_t)(grp * G + g) * T2 + t) * L.nx_Wp + f;
-                                    if (a.gx_lay.S) {
-                                        a.gx[late_unit(a.gx_lay, pl, grp * G + g, t, f)] = res;
-                                        a.gx[late_unit(a.gx_lay, L.cg_out + pl, grp * G + g, t, f)] = res_lo;
-                                    } else {
-                                        a.gx[(int64_t)pl * a.gx_plane + q] = res;
-                                        a.gx[(int64_t)(L.cg_out + pl) * a.gx_plane + q] = res_lo;
-                                    }
+                                    const int64_t u = late_unit(a.gx_lay, pl, grp * G + g, t, f);
+                                    a.gx[u] = res;
+                                    a.gx[u + (int64_t)L.cg_out * a.gx_lay.units] = res_lo;
                                 }
                                 continue;
                             }
@@ -1081,7 +1075,6 @@ static void fill_inc_args(oww_ctx* ctx, IncArgs& a) {
     a.dbg_clock = reinterpret_cast<long long*>(ctx->d_inc_dbg);
     if (ctx->late_active) {
         a.gx = reinterpret_cast<uint4*>(ctx->late_x[ctx->split_from].buf[0]);
-        a.gx_plane = ctx->late_x[ctx->split_from].plane;
         a.gx_lay = ctx->late_x[ctx->split_from].lay;
     }
 }

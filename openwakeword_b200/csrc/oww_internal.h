@@ -60,8 +60,8 @@ struct ResetLate {           // one tails-bearing tensor of the incremental late
     uint4* now;              // buffer the stream's next step reads: rows 0, 1 <- template rows 0, 1
     uint4* next;             // tensors that gain ONE row per step: the buffer of the step after, row 0 <- template row 1
     const uint4* tmpl;       // [planes][2][Wp]
-    int64_t plane; int T_buf, Wp, n_planes;
-    LateLay lay;             // lay.S > 0: block-major destination
+    int Wp, n_planes;
+    LateLay lay;             // block-major layout of now / next
 };
 // late[]: one entry per tails-bearing late tensor X_l, l >= split_from (5 at the default split, 9 at split_from 3)
 struct ResetTails { uint4* tails; const uint4* tmpl; int G, tail_units, n_tab; int4 tab[OWW_N_CONV]; int n_late; ResetLate late[OWW_N_CONV]; };
@@ -175,15 +175,14 @@ struct oww_ctx {
     void* d_inc_tails[2] = {nullptr, nullptr};   // [n_groups][tail_units] 16-byte units, double-buffered per step
     int inc_cur = 0;                 // tails buffer the next step reads
     // Incremental late layers (cnn_tc.cu, bottom): tensors X_l = input of conv layer l >= split_from, per stream
-    // [tails | new rows], fp16 hi/lo: block-major (LateLay, the default) or plane-major in the window-mode layout
-    struct LateTensor { void* buf[3] = {nullptr, nullptr, nullptr}; int n_buf = 0, T_buf = 0, rows_new = 0, W = 0, cg = 0, tmpl_off = -1; int64_t plane = 0;
-                        LateLay lay = {0, 0, 0, 0, 0, 0}; };   // lay.S > 0: block-major (tc_conv_blk_kernel); else plane-major [n][T_buf][W + 1]
+    // [tails | new rows], fp16 hi/lo, in the block-major layout of tc_conv_blk_kernel (LateLay)
+    struct LateTensor { void* buf[3] = {nullptr, nullptr, nullptr}; int n_buf = 0, rows_new = 0, W = 0, cg = 0, tmpl_off = -1;
+                        LateLay lay = {0, 0, 0, 0, 0, 0}; };
     LateTensor late_x[OWW_N_CONV];
-    void* d_late_tmp[1] = {nullptr};             // unpooled output of a late layer that is followed by a pool
+    void* d_late_tmp = nullptr;                  // unpooled output of a late layer that is followed by a separate pool
     void* d_late_template = nullptr;             // tails of the all-ones window per tails-bearing late tensor: [plane][2][Wp]
     bool late_active = false;
     bool late_pdl = true;                        // programmatic dependent launches inside the late chain (reserved[0] bit 5 disables)
-    bool late_blocked_ok = true;                 // reserved[0] bit 4 keeps the plane-major window layout for every late tensor (A/B)
     long late_step = 0;                          // chunks processed since the buffers were allocated (buffer rotation)
 
     // Priming.  A reset stream's mel history is ones(76,32) (utils.py:165) and its first chunk yields 5 rows (F8).  A

@@ -15,11 +15,11 @@ from .utils import load_embedding_weights, _torch
 class StreamEngine:
     def __init__(self, heads, n_streams, embedding="synthetic:0", feature_init=None, device_index=0,
                  max_chunks=1, cnn_mode=_native.CNN_TC_INCREMENTAL, window_batch=0, fuse_step=True,
-                 tc_heads=True, tc_heads_terms=3, split_from=None, group_heads=True, late_blocked=True):
+                 tc_heads=True, tc_heads_terms=3, split_from=None, group_heads=True):
         """heads: list of head dicts (weights.synthetic_head / load_head; gated pairs allowed)."""
         self.ctx = _native.Context(device=device_index, max_chunks=max_chunks, cnn_mode=cnn_mode,
                                    window_batch=window_batch, fuse_step=fuse_step, tc_heads=tc_heads,
-                                   tc_heads_terms=tc_heads_terms, split_from=split_from, group_heads=group_heads, late_blocked=late_blocked)
+                                   tc_heads_terms=tc_heads_terms, split_from=split_from, group_heads=group_heads)
         self.ctx.load_mel()
         self.ctx.load_embedding(_weights.pack_embedding_blob(load_embedding_weights(embedding)))
         self.columns = []                       # per entry of `heads`: (first score column, n_out); a gated pair's

@@ -3,8 +3,7 @@ whose arithmetic they share by construction (and against the oracle where the ar
 
 * the bulk clip path (oww_predict_clips, one fully convolutional pass per layer) against streaming the same clips, at
   every split point cnn_mode 3 accepts;
-* the incremental late chain in its block-major and plane-major tensor layouts, and with and without programmatic
-  dependent launches;
+* the incremental late chain with and without programmatic dependent launches, at every split point that has one;
 * the sub-batching of the window modes over window_batch;
 * oww_predict_clips on its private stream set (heads that are not on the tensor cores, or cnn_mode 0)."""
 import numpy as np
@@ -92,7 +91,8 @@ def test_bulk_clips_equal_streaming_at_every_split(torch_cuda, built_library, sp
     split_from on, heads over every window) against the same padded clips streamed one chunk per call through a fresh
     engine at the same split.  Mel, CNN and feature rows are the same arithmetic; the heads may sum their first layer in
     another order (2e-6, as the bulk_predict test).  At 20 the streaming step runs the heads inside the fused kernel
-    (fp32 FMA chain): 2e-5.  At 3 / 7 the clip pass runs the 48- and 72-channel split convs too."""
+    (fp32 FMA chain): 2e-5.  At 3 / 7 the clip pass runs the 48- and 72-channel split convs too, in the window layout
+    (tc_conv_kernel<.,.,3>), against the block-major late chain of the streaming step."""
     from openwakeword_b200.engine import StreamEngine
     torch = torch_cuda
     c = _clip_case()
@@ -130,7 +130,7 @@ def test_predict_clips_private_stream_set(torch_cuda, built_library, kw):
 
 
 # ---------------------------------------------------------------------------------------------------- late chain
-def _late_run(torch, monkeypatch, B, split_from, late_blocked=True, pdl=True):
+def _late_run(torch, monkeypatch, B, split_from, pdl=True):
     """10 device-resident calls of B streams (a 2-chunk call, a stream-ordered reset of three streams) -> all scores
     of every call and the feature rings (last 40 rows) of 64 sampled streams."""
     from openwakeword_b200.engine import StreamEngine
@@ -145,8 +145,7 @@ def _late_run(torch, monkeypatch, B, split_from, late_blocked=True, pdl=True):
     sample = sorted(fixed + [int(x) for x in rng.permutation(B) if x not in fixed][:64 - len(fixed)])
     # reserved[0] bit 5 (no dependent launches) is read when the handle is created
     monkeypatch.setenv("OWW_FLAGS", "0" if pdl else "32")
-    eng = StreamEngine(hs, B, embedding=emb_weights(), feature_init=fi, cnn_mode=3, split_from=split_from, max_chunks=2,
-                       late_blocked=late_blocked)
+    eng = StreamEngine(hs, B, embedding=emb_weights(), feature_init=fi, cnn_mode=3, split_from=split_from, max_chunks=2)
     monkeypatch.delenv("OWW_FLAGS")
     scores, pos = [], 0
     for si, nch in enumerate(plan):
@@ -160,22 +159,18 @@ def _late_run(torch, monkeypatch, B, split_from, late_blocked=True, pdl=True):
     return np.stack(scores), feats
 
 
-@pytest.mark.parametrize("split_from", [11, 15])
-def test_late_chain_layouts_and_pdl_are_bit_identical(torch_cuda, built_library, monkeypatch, split_from):
-    """The incremental late layers three ways on 2048 streams: block-major tensors with dependent launches (default),
-    the plane-major window layout (late_blocked=False: tc_conv_kernel<.,.,3> and a separate (1,2) pool instead of the
-    fused one), and plain launches (OWW_FLAGS=32).  The conv terms are issued in the same order in both kernels and a
-    split after a max equals the lexicographic max of (hi, lo) pairs, so scores and rings must match bit for bit; the
-    comparison with plain launches is the race check of the griddepcontrol chain."""
+@pytest.mark.parametrize("split_from", [3, 7, 11, 15])
+def test_late_chain_pdl_is_bit_identical_at_every_split(torch_cuda, built_library, monkeypatch, split_from):
+    """The incremental late layers on 2048 streams with dependent launches (default) against plain launches
+    (OWW_FLAGS=32), at every split point that has a late chain (every tc_conv_blk_kernel instance, the fused (1,2) pool
+    of layers 6 and 14, the separate (2,2) pools of layers 10 and 18).  Scores and rings must match bit for bit: this is
+    the race check of the griddepcontrol chain."""
     torch = torch_cuda
     ref_s, ref_f = _late_run(torch, monkeypatch, 2048, split_from)
-    plane_s, plane_f = _late_run(torch, monkeypatch, 2048, split_from, late_blocked=False)
     nopdl_s, nopdl_f = _late_run(torch, monkeypatch, 2048, split_from, pdl=False)
-    print(f"split_from={split_from}: max |blocked - plane-major| = {np.abs(ref_s - plane_s).max():.3e} "
-          f"(features {np.abs(ref_f - plane_f).max():.3e}); max |PDL - plain| = {np.abs(ref_s - nopdl_s).max():.3e} "
+    print(f"split_from={split_from}: max |PDL - plain| = {np.abs(ref_s - nopdl_s).max():.3e} "
           f"(features {np.abs(ref_f - nopdl_f).max():.3e})")
     assert np.isfinite(ref_s).all() and np.isfinite(ref_f).all()
-    assert np.array_equal(ref_s, plane_s) and np.array_equal(ref_f, plane_f)
     assert np.array_equal(ref_s, nopdl_s) and np.array_equal(ref_f, nopdl_f)
 
 

@@ -582,8 +582,8 @@ SPLIT_FEAT_TOL = {3: 2e-3, 7: 2e-3, 11: 8e-3, 15: 8e-3, 20: 8e-3}
 @pytest.mark.parametrize("split_from,tol", [(3, 1e-3), (7, 1e-3), (11, 1e-3), (15, 1e-3), (20, 1e-3)])
 def test_split_from_variants_vs_oracle(torch_cuda, built_library, split_from, tol):
     """Every split point cnn_mode 3 accepts, against the oracle: conv layers >= split_from on split operands (the fused
-    kernel runs layers 0 .. split_from-1: tc_inc_kernel<0> at 3 / 7 - whose late chain keeps the plane-major window
-    layout and runs the split convs <4,48>, <6,48>, <6,80>, <10,80> - and <11> / <15>), and plain fp16 everywhere
+    kernel runs layers 0 .. split_from-1: tc_inc_kernel<0> at 3 / 7 - whose late chain runs the block-major split
+    convs <4,48>, <6,48>, <6,80>, <10,80> - and <11> / <15>), and plain fp16 everywhere
     (20: one launch per step).  151 streams, 1-, 2- and 3-chunk calls and a partial reset (see _split_case)."""
     from openwakeword_b200.engine import StreamEngine
     c = _split_case()
