@@ -111,6 +111,38 @@ int oww_add_head(oww_ctx* ctx, const oww_head_desc* desc, const float* h_blob, s
  * `main_head` exceeds `threshold` it is replaced by the score of single-output head `verifier_head`, per chunk, before
  * the max over a multi-chunk call.  Both columns stay in d_scores (the verifier's holds its raw score).          */
 int oww_add_gate(oww_ctx* ctx, int main_head, int verifier_head, float threshold);
+
+/* ---- custom verifier models (openwakeword/model.py:175-195,319-328; custom_verifier_model.py:91-113;
+ *      docs/custom_verifier_models.md) ------------------------------------------------------------------------------
+ * A verifier is the speaker-specific pipeline train_verifier_model pickles, FunctionTransformer(flatten_features) ->
+ * StandardScaler -> binary LogisticRegression, restated on the D = n_in*96 newest feature rows x of its parent head:
+ *     p = 1 / (1 + exp(-(bias + sum_j (x_j - mean_j) * weight_j)))   mean = scaler.mean_, weight = coef_ / scaler.scale_
+ * (host-computed in float64, stored as fp32; fp32 accumulation in a fixed order).  After the heads, the verifier gates
+ * and the max over the chunk windows of a step, every score column of the parent that is >= threshold (compared in
+ * fp32) is replaced by p of the stream's verifier on the newest window; columns below it keep their value.
+ *   oww_add_verifier_bank      - slots for up to `capacity` verifiers of head `head_id` (of a gated pair: the main head);
+ *                                every stream starts without a verifier (slot -1).  8*D bytes per slot.
+ *   oww_load_verifier          - copy one verifier into a slot; h_mean and h_weight hold D floats each.  Synchronises
+ *                                the device first, so steps already in flight use the old contents.
+ *   oww_assign_verifier        - stream-ordered, allocation-free: stream h_stream_ids[i] (NULL = all streams, then n is
+ *                                the stream count) uses slot h_slots[i] (-1 = none) from the next step enqueued on `stream`
+ *                                or submitted with oww_step_host / oww_step_host_submit
+ *   oww_set_verifier_clip_slot - the slot oww_predict_clips applies to every clip (-1 = none, the default)
+ *   oww_set_verifier_threshold - new threshold for the steps and clip calls enqueued from now on
+ *   oww_enable_verifiers       - 0: steps and clip calls enqueued from now on skip every bank (their scores are the
+ *                                heads' max over the chunk windows), 1 (default): they apply them.  For a caller that
+ *                                splits one long call into several steps and verifies the max itself.
+ *   oww_verifier_predict       - stateless and ungated: d_feats [n][n_in][96] -> d_out[n] = predict_proba(...)[:, -1]
+ * At most one bank per head.  oww_set_streams resets every assignment to -1; oww_reset / oww_reset_async leave them as
+ * they are (which user owns a stream is the caller's business).  A handle without banks launches nothing for verifiers. */
+int oww_add_verifier_bank(oww_ctx* ctx, int head_id, int capacity, float threshold, int* bank_id);
+int oww_load_verifier(oww_ctx* ctx, int bank, int slot, const float* h_mean, const float* h_weight, float bias);
+int oww_assign_verifier(oww_ctx* ctx, int bank, const int32_t* h_stream_ids, int n, const int32_t* h_slots, void* stream);
+int oww_set_verifier_clip_slot(oww_ctx* ctx, int bank, int slot);
+int oww_set_verifier_threshold(oww_ctx* ctx, int bank, float threshold);
+int oww_enable_verifiers(oww_ctx* ctx, int enabled);
+int oww_verifier_predict(oww_ctx* ctx, int bank, int slot, const float* d_feats, int n, float* d_out, void* stream);
+
 int oww_n_heads(const oww_ctx* ctx);
 int oww_n_outputs(const oww_ctx* ctx);          /* total score columns over all heads           */
 

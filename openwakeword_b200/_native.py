@@ -40,6 +40,13 @@ _SIGNATURES = {
     "oww_load_embedding": (C.c_int, [_P, _P, C.c_size_t]),
     "oww_add_head": (C.c_int, [_P, C.POINTER(HeadDesc), _P, C.c_size_t, C.POINTER(C.c_int)]),
     "oww_add_gate": (C.c_int, [_P, C.c_int, C.c_int, C.c_float]),
+    "oww_add_verifier_bank": (C.c_int, [_P, C.c_int, C.c_int, C.c_float, C.POINTER(C.c_int)]),
+    "oww_load_verifier": (C.c_int, [_P, C.c_int, C.c_int, _P, _P, C.c_float]),
+    "oww_assign_verifier": (C.c_int, [_P, C.c_int, _P, C.c_int, _P, _P]),
+    "oww_set_verifier_clip_slot": (C.c_int, [_P, C.c_int, C.c_int]),
+    "oww_set_verifier_threshold": (C.c_int, [_P, C.c_int, C.c_float]),
+    "oww_enable_verifiers": (C.c_int, [_P, C.c_int]),
+    "oww_verifier_predict": (C.c_int, [_P, C.c_int, C.c_int, _P, C.c_int, _P, _P]),
     "oww_n_heads": (C.c_int, [_P]),
     "oww_n_outputs": (C.c_int, [_P]),
     "oww_melspectrogram": (C.c_int, [_P, _P, C.c_int, C.c_int, _P, C.c_int, _P]),
@@ -140,6 +147,8 @@ class Context:
         self.h = h
         self.device = device
         self.max_chunks = max_chunks
+        self._head_n_in = []                # per head id: n_in (verifier banks take n_in*96 floats per slot)
+        self._bank_d = []                   # per verifier bank: D
 
     def close(self):
         if getattr(self, "h", None):
@@ -175,10 +184,59 @@ class Context:
         blob = np.ascontiguousarray(blob, np.float32)
         hid = C.c_int(-1)
         self._check(self.lib.oww_add_head(self.h, C.byref(d), _ptr(blob), blob.size, C.byref(hid)))
+        self._head_n_in.append(int(n_in))
         return hid.value
 
     def add_gate(self, main_head, verifier_head, threshold=0.5):
         self._check(self.lib.oww_add_gate(self.h, int(main_head), int(verifier_head), float(threshold)))
+
+    # ---- custom verifier banks (include/owwb200.h) ----
+    def add_verifier_bank(self, head_id, capacity, threshold):
+        bid = C.c_int(-1)
+        self._check(self.lib.oww_add_verifier_bank(self.h, int(head_id), int(capacity), float(threshold), C.byref(bid)))
+        self._bank_d.append(self._head_n_in[int(head_id)] * 96)
+        return bid.value
+
+    def load_verifier(self, bank, slot, mean, weight, bias):
+        """mean, weight: the bank's D = n_in*96 floats each (synchronises the device)."""
+        mean = np.ascontiguousarray(mean, np.float32).ravel()
+        weight = np.ascontiguousarray(weight, np.float32).ravel()
+        if not 0 <= int(bank) < len(self._bank_d):
+            raise NativeError(f"bad verifier bank {bank}")
+        D = self._bank_d[int(bank)]
+        if mean.size != D or weight.size != D:
+            raise ValueError(f"verifier bank {bank} takes {D} means and weights, got {mean.size} and {weight.size}")
+        self._check(self.lib.oww_load_verifier(self.h, int(bank), int(slot), _ptr(mean), _ptr(weight), float(bias)))
+
+    def assign_verifier(self, bank, stream_ids, slots, stream=None):
+        """Stream-ordered on `stream` and on the handle's own stream of step_host / submit: stream_ids None = all streams
+        (slots then has one entry per stream); slot -1 = none."""
+        ids = None if stream_ids is None else np.ascontiguousarray(stream_ids, np.int32)
+        sl = np.ascontiguousarray(slots, np.int32)
+        n = sl.size if ids is None else ids.size
+        if sl.size != n:
+            raise ValueError(f"{sl.size} slots for {n} streams")
+        self._check(self.lib.oww_assign_verifier(self.h, int(bank), _ptr(ids), n, _ptr(sl), stream))
+
+    def set_verifier_clip_slot(self, bank, slot):
+        self._check(self.lib.oww_set_verifier_clip_slot(self.h, int(bank), int(slot)))
+
+    def set_verifier_threshold(self, bank, threshold):
+        self._check(self.lib.oww_set_verifier_threshold(self.h, int(bank), float(threshold)))
+
+    def enable_verifiers(self, enabled):
+        self._check(self.lib.oww_enable_verifiers(self.h, int(bool(enabled))))
+
+    def verifier_predict(self, bank, slot, d_feats, n, d_out, stream=None):
+        self._check(self.lib.oww_verifier_predict(self.h, int(bank), int(slot), _ptr(d_feats), int(n), _ptr(d_out), stream))
+
+    def verifier_predict_host(self, bank, slot, feats):
+        """float32 [n, n_in, 96] host windows -> float32 [n] (synchronises)."""
+        import torch
+        x = torch.from_numpy(np.ascontiguousarray(feats, np.float32)).to(f"cuda:{self.device}")
+        out = torch.empty(x.shape[0], dtype=torch.float32, device=x.device)
+        self.verifier_predict(bank, slot, x, x.shape[0], out, torch.cuda.current_stream(x.device).cuda_stream)
+        return out.cpu().numpy()
 
     @property
     def n_outputs(self):

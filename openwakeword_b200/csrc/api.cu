@@ -110,6 +110,7 @@ void free_streams(oww_ctx* c) {
     cudaFree(c->d_emb_tmp); cudaFree(c->d_inc_tails[0]); cudaFree(c->d_inc_tails[1]);
     cudaFree(c->d_reset_ids); cudaFree(c->d_reset_init);
     cudaFree(c->d_scores_tmp);
+    oww_verifiers_free_streams(c);
     oww_heads_grp_drop_mirror(c);
     for (auto& X : c->late_x) for (auto& b : X.buf) { cudaFree(b); b = nullptr; }
     cudaFree(c->d_late_tmp); c->d_late_tmp = nullptr;
@@ -210,6 +211,7 @@ int step_core(oww_ctx* ctx, const int16_t* d_pcm, int64_t pcm_stride, int n_chun
         if (heads_inside) oww_feat16_invalidate(ctx);
         else if ((rc = oww_feat16_advance(ctx, 1, s))) return rc;
         if (!heads_inside && (rc = oww_heads_all(ctx, fs0, B, d_scores, out_stride, 0, s))) return rc;
+        if ((rc = oww_verifiers_apply(ctx, fs0, B, d_scores, out_stride, false, s))) return rc;
         if (ev) {
             if (heads_inside) ctx->ev_fused[slot] = 1;
             else { OWW_CUDA(ctx, cudaEventRecord(ev[3], s)); ctx->ev_fused[slot] = 2; }
@@ -240,6 +242,8 @@ int step_core(oww_ctx* ctx, const int16_t* d_pcm, int64_t pcm_stride, int n_chun
         FeatSrc fs = fs0; fs.back = i;
         if ((rc = oww_heads_all(ctx, fs, B, d_scores, out_stride, i != n_chunks - 1, s))) return rc;
     }
+    // custom verifiers: after the max over the chunk windows, on the newest window (model.py:319-328)
+    if ((rc = oww_verifiers_apply(ctx, fs0, B, d_scores, out_stride, false, s))) return rc;
     if (ev) { OWW_CUDA(ctx, cudaEventRecord(ev[3], s)); ctx->ev_steps++; }
     return OWW_OK;
 }
@@ -353,6 +357,8 @@ void oww_destroy(oww_ctx* ctx) {
     cudaFree(ctx->d_tc_act[0]); cudaFree(ctx->d_tc_act[1]); cudaFree(ctx->d_inc_w); cudaFree(ctx->d_head_devs);
     for (auto& h : ctx->heads) { cudaFree(h.d_blob); cudaFree(h.d_w1_tc); }
     cudaFree(ctx->d_gates); cudaFree(ctx->d_tails_template); cudaFree(ctx->d_peer_err);
+    for (auto& b : ctx->banks) { cudaFree(b.d_mean); cudaFree(b.d_weight); cudaFree(b.d_bias); }
+    for (auto e : ctx->ver_ev) if (e) cudaEventDestroy(e);
     for (auto& S : ctx->slot) {
         cudaFreeHost(S.h_pcm); cudaFreeHost(S.h_scores); cudaFree(S.d_pcm); cudaFree(S.d_scores);
         if (S.done) cudaEventDestroy(S.done);
@@ -514,6 +520,7 @@ int oww_set_streams(oww_ctx* ctx, int n_streams) {
     if ((rc = ensure_emb_tmp(ctx, (size_t)B * mc * 96))) return rc;
     if (ctx->cfg.cnn_mode == OWW_CNN_TC_INCREMENTAL && (rc = oww_late_alloc(ctx))) return rc;
     if (ctx->cfg.cnn_mode == OWW_CNN_TC_INCREMENTAL && (rc = oww_inc_alloc_streams(ctx))) return rc;
+    if ((rc = oww_verifiers_alloc_streams(ctx))) return rc;         // every stream starts without a verifier
     return oww_reset(ctx, nullptr, B, nullptr, OWW_INIT_FEATURE_ROWS);
 }
 
@@ -761,7 +768,9 @@ int oww_predict_clips(oww_ctx* ctx, const int16_t* d_pcm, int n_clips, int n_sam
                 if ((rc = oww_cnn_tc_clip_rows(ctx, src, m, T_v, d_f + (int64_t)init_rows * 96, init_rows + steps, s))) break;
                 FeatSrc fs{d_f, f_stride, nullptr, -1, 0};
                 fs.steps = steps; fs.row0 = init_rows;
-                rc = oww_heads_all(ctx, fs, m * steps, d_scores + (size_t)c0 * steps * ctx->n_out_total, ctx->n_out_total, 0, s);
+                float* out = d_scores + (size_t)c0 * steps * ctx->n_out_total;
+                if ((rc = oww_heads_all(ctx, fs, m * steps, out, ctx->n_out_total, 0, s))) break;
+                rc = oww_verifiers_apply(ctx, fs, m * steps, out, ctx->n_out_total, true, s);       // clip slot, every step
             }
             cudaFreeAsync(d_v, s); cudaFreeAsync(d_f, s);
             if (d_init) cudaFreeAsync(d_init, s);
@@ -790,11 +799,17 @@ int oww_predict_clips(oww_ctx* ctx, const int16_t* d_pcm, int n_clips, int n_sam
 
     c->heads = ctx->heads; c->n_out_total = ctx->n_out_total; c->max_n_in = ctx->max_n_in; c->d_head_devs = ctx->d_head_devs;
     c->gates = ctx->gates; c->d_gates = ctx->d_gates;
+    // verifier banks: the weights are shared, and every clip (stream of the private set) uses the bank's clip slot
+    std::vector<VerifierBank> clip_banks;
+    if (ctx->verifiers_on) clip_banks = ctx->banks;
+    for (auto& b : clip_banks) b.d_assign = nullptr;
     int rc = OWW_OK;
     for (int c0 = 0; c0 < n_clips && rc == OWW_OK; c0 += slab_max) {
         const int m = std::min(slab_max, n_clips - c0);
+        c->banks.clear();              // the private set allocates no assignment of its own
         if (c->n_streams != m) { if ((rc = oww_set_streams(c, m))) { ctx->err = c->err; break; } }
         if ((rc = oww_reset(c, nullptr, m, h_feature_init, h_feature_init ? n_rows : OWW_INIT_FEATURE_ROWS))) { ctx->err = c->err; break; }
+        c->banks = clip_banks;
         const size_t stage_bytes = (size_t)m * OWW_SAMPLES_PER_CHUNK * sizeof(int16_t);
         if (c->slot[0].pcm_bytes < stage_bytes) {
             cudaFree(c->slot[0].d_pcm); c->slot[0].d_pcm = nullptr;
@@ -814,6 +829,7 @@ int oww_predict_clips(oww_ctx* ctx, const int16_t* d_pcm, int n_clips, int n_sam
     c->heads.clear();   // do not let the child free shared blobs
     c->d_head_devs = nullptr;
     c->gates.clear(); c->d_gates = nullptr;
+    c->banks.clear();
     return rc;
 }
 

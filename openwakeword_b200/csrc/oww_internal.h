@@ -70,6 +70,19 @@ struct ResetTails { uint4* tails; const uint4* tmpl; int G, tail_units, n_tab; i
 // `ver_col` wherever it exceeds `thr`
 struct Gate { int main_col, ver_col; float thr; };
 
+// custom verifier bank (verifier.cu): up to `capacity` speaker verifiers of one head, each the linear form of the
+// reference's FunctionTransformer(flatten) -> StandardScaler -> LogisticRegression pipeline over the head's newest n_in
+// feature rows (D = n_in*96):  p = 1 / (1 + exp(-(bias + sum_j (x_j - mean_j) * weight_j)))
+struct VerifierBank {
+    int head_id, col0, n_cols, n_in, capacity;
+    float thr;                       // columns >= thr (fp32) are replaced by p
+    float* d_mean = nullptr;         // [capacity][D]
+    float* d_weight = nullptr;       // [capacity][D]
+    float* d_bias = nullptr;         // [capacity]
+    int* d_assign = nullptr;         // [n_streams] slot per stream, -1 = none (nullptr: every row uses clip_slot)
+    int clip_slot = -1;              // slot oww_predict_clips applies to every clip
+};
+
 // Ring row counters (rows ever written; ring slot = count & (rows-1)) would overflow int32 after ~248 days of
 // continuous streaming at 100 mel rows/s.  Past 2^30 they are rebased by a multiple of every ring size (rings are
 // powers of two <= 2^20 rows), which keeps the slot and leaves the count >= the ring size, so "row not yet written"
@@ -138,6 +151,10 @@ struct oww_ctx {
     Gate* d_gates = nullptr;
     float* d_scores_tmp = nullptr;   // [n_streams][n_out_total]: one chunk's raw scores when gates meet a multi-chunk call
     size_t scores_tmp_floats = 0;
+    std::vector<VerifierBank> banks; // custom verifiers, applied after the heads (and gates, and the max over chunks)
+    int* d_assign_stage = nullptr;   // [2][n_streams] staging of oww_assign_verifier (ids | slots)
+    bool verifiers_on = true;        // oww_enable_verifiers: steps and clip calls enqueued while false skip the banks
+    cudaEvent_t ver_ev[2] = {nullptr, nullptr};   // orders oww_assign_verifier with own_stream
 
     // streaming state
     int n_streams = 0;
@@ -371,3 +388,14 @@ uint32_t oww_heads_grp_bulk(oww_ctx* ctx, const FeatSrc& src, int n, float* d_ou
 int oww_heads_grp_launch(oww_ctx* ctx, int back, int n, float* d_out, int out_stride, int combine_max, cudaStream_t s);
 // every head (tensor-core kernel where a head allows it, heads.cu otherwise) + the verifier gates
 int oww_heads_all(oww_ctx* ctx, const FeatSrc& src, int n, float* d_out, int out_stride, int combine_max, cudaStream_t s);
+
+// ---- verifier.cu: custom verifier banks ----
+// every bank of the handle on n rows of final scores (one launch; nothing when the handle has no bank).  The window of
+// row r is the newest n_in rows of `src` (FeatSrc sample r).  Its slot is bank.d_assign[r] for streams (rows = streams
+// of the handle), or bank.clip_slot for clips (rows = (clip, step) of the bulk path) and when d_assign is nullptr (the
+// private stream set of oww_predict_clips).
+int oww_verifiers_apply(oww_ctx* ctx, const FeatSrc& src, int n, float* d_scores, int out_stride, bool clips,
+                        cudaStream_t s);
+// (re)allocate every bank's per-stream assignment for ctx->n_streams streams, all -1
+int oww_verifiers_alloc_streams(oww_ctx* ctx);
+void oww_verifiers_free_streams(oww_ctx* ctx);

@@ -10,6 +10,7 @@ import numpy as np
 from . import _native
 from . import weights as _weights
 from .utils import load_embedding_weights, _torch
+from .custom_verifier_model import load_verifier, linear_verifier_params
 
 
 class StreamEngine:
@@ -24,6 +25,7 @@ class StreamEngine:
         self.ctx.load_embedding(_weights.pack_embedding_blob(load_embedding_weights(embedding)))
         self.columns = []                       # per entry of `heads`: (first score column, n_out); a gated pair's
         col = 0                                 # verifier network occupies one further (raw) column
+        self.head_ids = []                      # per entry of `heads`: its (main) head id on the handle
         for h in heads:
             parts = [h["main"], h["verifier"]] if _weights.is_gated(h) else [h]
             ids = []
@@ -32,6 +34,7 @@ class StreamEngine:
                 ids.append(self.ctx.add_head(n_in, dims, ln, fin, _weights.pack_head_blob(q)))
             if len(ids) == 2:
                 self.ctx.add_gate(ids[0], ids[1], h["threshold"])
+            self.head_ids.append(ids[0])
             n_out = parts[0]["layers"][-1]["W"].shape[1]
             self.columns.append((col, n_out))
             col += n_out if len(ids) == 1 else 2
@@ -76,3 +79,27 @@ class StreamEngine:
             out = np.empty((self.n_streams, self.n_cols), np.float32)
         self.ctx.step_host_collect(ticket, out)
         return out
+
+    # ---- custom verifier models (include/owwb200.h, oww_add_verifier_bank) ----
+    def add_verifier_bank(self, head_index, capacity, threshold=0.1):
+        """Slots for `capacity` verifiers of entry `head_index` of `heads`; every stream starts without one."""
+        return self.ctx.add_verifier_bank(self.head_ids[head_index], capacity, threshold)
+
+    def load_verifier(self, bank, slot, verifier):
+        """verifier: a pickle path or pipeline of train_verifier_model's form, or (mean, weight, bias) arrays, on the head's
+        n_in*96 features.  Synchronises the device: steps already enqueued use the slot's old contents."""
+        if isinstance(verifier, tuple):
+            params = verifier
+        else:
+            params = linear_verifier_params(load_verifier(verifier) if isinstance(verifier, str) else verifier)
+            if params is None:
+                raise ValueError("not a linear verifier pipeline (FunctionTransformer -> StandardScaler -> LogisticRegression)")
+        self.ctx.load_verifier(bank, slot, *params)
+
+    def assign_verifier(self, bank, slots, stream_ids=None, stream=None):
+        """Stream stream_ids[i] (None = all) uses slot slots[i] (-1 = none) from the next ``step`` enqueued on the current
+        CUDA stream (or `stream`) and the next ``step_host`` / ``submit``."""
+        torch = _torch()
+        if stream is None:
+            stream = torch.cuda.current_stream(torch.device("cuda", self.device_index)).cuda_stream
+        self.ctx.assign_verifier(bank, stream_ids, slots, stream)

@@ -8,8 +8,8 @@ the batch axis (``predict`` then takes ``[n_streams, samples]`` and returns arra
 ``predict_clips`` (array-input bulk path) and ``feature_init``.
 """
 import os
-import pickle
 import time
+import warnings
 from collections import defaultdict, deque
 from functools import partial
 
@@ -19,6 +19,7 @@ from . import _native
 from . import weights as _weights
 from .utils import AudioFeatures, re_arg, _read_wav, CHUNK, _torch
 from . import registry as _registry
+from .custom_verifier_model import load_verifier, linear_verifier_params
 
 
 def _load_head_file(path):
@@ -64,7 +65,11 @@ class Model:
         self.model_prediction_function = {}
         self.class_mapping = {}
         self.custom_verifier_models = {}
+        self._host_verifiers = {}      # parent -> verifier run per stream on the host (not device-runnable)
+        self._vbanks = {}              # parent -> {"bank", "slots" int32[B], "objs"}: verifiers on the device (verifier.cu)
         self.custom_verifier_threshold = custom_verifier_threshold
+        self._head_ids = {}            # parent -> head id a verifier bank attaches to (a gated pair: its main head)
+        device_verifiers = {}          # parent -> {stream id or None (all): verifier}
 
         if enable_speex_noise_suppression:
             from speexdsp_ns import NoiseSuppression     # same optional dependency as the reference (model.py:200-205)
@@ -102,11 +107,13 @@ class Model:
                     raise ValueError(f"model '{name}': a verifier pair needs two single-output networks on the same input")
                 vid = ctx.add_head(v_in, v_dims, v_ln, v_fin, _weights.pack_head_blob(head["verifier"]))
                 ctx.add_gate(hid, vid, head["threshold"])
+                self._head_ids[name] = hid
                 self.model_prediction_function[name] = partial(self._gated_predict, hid, vid, n_in, head["threshold"])
                 width = 2
             else:
                 n_in, dims, ln, fin = _weights.head_desc(head)
                 hid = ctx.add_head(n_in, dims, ln, fin, _weights.pack_head_blob(head))
+                self._head_ids[name] = hid
                 self.model_prediction_function[name] = partial(self._head_predict, hid, n_in, dims[-1])
                 width = dims[-1]
             self.models[name] = hid
@@ -123,8 +130,17 @@ class Model:
             else:
                 self.class_mapping[name] = {str(i): str(i) for i in range(0, dims[-1])}
             if isinstance(custom_verifier_models, dict) and custom_verifier_models.get(name, False):
-                with open(custom_verifier_models[name], "rb") as fh:
-                    self.custom_verifier_models[name] = pickle.load(fh)
+                spec = custom_verifier_models[name]
+                if isinstance(spec, dict):              # {stream id: path or pipeline}: device-runnable only
+                    device_verifiers[name] = dict(spec)
+                    self.custom_verifier_models[name] = spec
+                else:                                   # the reference form: one verifier for every stream
+                    v = load_verifier(spec)
+                    self.custom_verifier_models[name] = v
+                    if self._device_params(name, v) is not None:
+                        device_verifiers[name] = {None: v}
+                    else:
+                        self._host_verifiers[name] = v
         if len(self.custom_verifier_models.keys()) < len(custom_verifier_models.keys()):
             raise ValueError("Custom verifier models were provided, but some were not matched with a base model!"
                              " Make sure that the keys provided in the `custom_verifier_models` dictionary argument"
@@ -132,6 +148,103 @@ class Model:
         self._n_cols = col
         self._scores = np.zeros((self.n_streams, max(col, 1)), np.float32)
         self._reset_history()
+        for name, per_stream in device_verifiers.items():
+            for b, v in per_stream.items():
+                self.set_custom_verifier(name, v, None if b is None else [b])
+
+    # ---- custom verifier models on the device (include/owwb200.h, oww_add_verifier_bank) ----
+    @property
+    def custom_verifier_threshold(self):
+        return self._verifier_threshold
+
+    @custom_verifier_threshold.setter
+    def custom_verifier_threshold(self, value):
+        """applies to the device banks from the next call on, as to the host loop"""
+        self._verifier_threshold = value
+        for st in self._vbanks.values():
+            self.preprocessor.ctx.set_verifier_threshold(st["bank"], value)
+
+    def _device_params(self, name, verifier):
+        """(mean, weight, bias) when `verifier` is the reference's linear pipeline on `name`'s input window, else None."""
+        params = linear_verifier_params(verifier)
+        if params is None or params[0].size != self.model_inputs[name] * 96:
+            return None
+        return params
+
+    def set_custom_verifier(self, name, verifier, streams=None):
+        """Attach, replace or remove (``verifier=None``) the custom verifier of model `name` on `streams` (stream ids;
+        None = every stream) from the next call on.  `verifier`: a pickle path or a loaded pipeline of the form
+        ``custom_verifier_model.train_verifier_model`` produces (FunctionTransformer(flatten_features) ->
+        StandardScaler -> binary LogisticRegression); anything else raises ValueError.  It runs on the device for those
+        streams and replaces any host-side verifier of `name`; ``verifier=None`` on every stream also removes a host-side
+        one.  ``predict_clips`` applies stream 0's verifier.  ``custom_verifier_models[name]`` follows: the verifier when
+        every stream has the same one, {stream id: verifier} otherwise, absent when no stream has one."""
+        if name not in self.models:
+            raise ValueError(f"no model named '{name}'")
+        B = self.n_streams
+        ids = np.arange(B) if streams is None else np.unique(np.asarray(streams, np.int64).ravel())
+        if ids.size == 0:
+            return
+        if ids.min() < 0 or ids.max() >= B:
+            raise ValueError(f"stream ids must lie in [0, {B})")
+        ctx = self.preprocessor.ctx
+        st = self._vbanks.get(name)
+        params = None
+        if verifier is not None:
+            v = load_verifier(verifier) if isinstance(verifier, (str, os.PathLike)) else verifier
+            params = self._device_params(name, v)
+            if params is None:
+                raise ValueError(f"model '{name}': only the linear verifier pipeline of train_verifier_model, on the "
+                                 f"model's {self.model_inputs[name]}-row input window, runs on the device")
+        if st is None:
+            if params is None:
+                if ids.size == B and self._host_verifiers.pop(name, None) is not None:
+                    self.custom_verifier_models.pop(name, None)
+                return
+            self.preprocessor._ensure_streams()
+            self.preprocessor._verifier_banks = True
+            st = {"bank": ctx.add_verifier_bank(self._head_ids[name], B, self.custom_verifier_threshold),
+                  "slots": np.full(B, -1, np.int32), "objs": [None] * B}
+            self._vbanks[name] = st
+        slot = -1
+        if params is not None:           # a slot no other stream uses (one always exists: capacity = n_streams)
+            others = np.ones(B, bool)
+            others[ids] = False
+            used = set(st["slots"][others].tolist())
+            slot = next(k for k in range(B) if k not in used)
+            ctx.load_verifier(st["bank"], slot, *params)
+        ctx.assign_verifier(st["bank"], None if ids.size == B else ids, np.full(ids.size, slot, np.int32))
+        st["slots"][ids] = slot
+        for b in ids:
+            st["objs"][b] = v if params is not None else None
+        ctx.set_verifier_clip_slot(st["bank"], int(st["slots"][0]))
+        self._host_verifiers.pop(name, None)
+        objs = st["objs"]
+        if all(o is None for o in objs):
+            self.custom_verifier_models.pop(name, None)
+        elif all(o is objs[0] for o in objs):
+            self.custom_verifier_models[name] = objs[0]
+        else:
+            self.custom_verifier_models[name] = {b: o for b, o in enumerate(objs) if o is not None}
+
+    def _reverify(self, mdl, predictions, labels):
+        """Verification on the host side of the stateless entry, on each stream's newest window (model.py:319-328): for
+        calls that run no step (< 1280 samples: the previous prediction is re-verified, as the reference does) and for
+        calls split into several device steps (> max_chunks chunks: those run without the banks, and the max over all
+        their chunk windows is verified here, once).  Streams with a device verifier and a label >= the threshold."""
+        st = self._vbanks[mdl]
+        thr = np.float32(self.custom_verifier_threshold)
+        hit = np.zeros(self.n_streams, bool)
+        for lab in labels:
+            hit |= predictions[lab] >= thr
+        hit &= st["slots"] >= 0
+        for slot in np.unique(st["slots"][hit]):
+            bs = np.nonzero(hit & (st["slots"] == slot))[0]
+            feats = np.concatenate([self.preprocessor.get_features(self.model_inputs[mdl], stream=int(b)) for b in bs])
+            p = self.preprocessor.ctx.verifier_predict_host(st["bank"], int(slot), feats)
+            for lab in labels:
+                sel = predictions[lab][bs] >= thr
+                predictions[lab][bs[sel]] = p[sel]
 
     # ---- per-label history (model.py:198; vectorised over streams) ----
     def _reset_history(self):
@@ -227,17 +340,21 @@ class Model:
                 pred = np.zeros((B, n_classes + 1), np.float32)
             if n_out == 1:
                 predictions[mdl] = pred[:, 0].copy()
+                labels = [mdl]
             else:
+                labels = list(self.class_mapping[mdl].values())
                 for int_label, cls in self.class_mapping[mdl].items():
                     predictions[cls] = pred[:, int(int_label)].copy()
+            if mdl in self._vbanks and (n_prepared < CHUNK or n_chunks > self.preprocessor.max_chunks):
+                self._reverify(mdl, predictions, labels)         # otherwise the device verified the step it ran
 
-            if self.custom_verifier_models != {}:
+            if self._host_verifiers != {}:
                 for cls in list(predictions.keys()):
                     parent = self.get_parent_model_from_label(cls)
-                    if self.custom_verifier_models.get(parent, False):
+                    if self._host_verifiers.get(parent, False):
                         for b in np.nonzero(predictions[cls] >= self.custom_verifier_threshold)[0]:
                             feats = self.preprocessor.get_features(self.model_inputs[mdl], stream=int(b))
-                            predictions[cls][b] = self.custom_verifier_models[parent].predict_proba(feats)[0][-1]
+                            predictions[cls][b] = self._host_verifiers[parent].predict_proba(feats)[0][-1]
 
             for cls in predictions.keys():                            # model.py:330-333
                 _, cnt = self._h(cls)
@@ -333,7 +450,12 @@ class Model:
         return labs
 
     def predict_clips_array(self, clips, padding=1, feature_init=None):
-        """-> (float32 [N, steps, n_labels], labels) with the first-5-steps zeroing of model.py:330-333 applied."""
+        """-> (float32 [N, steps, n_labels], labels) with the first-5-steps zeroing of model.py:330-333 applied.
+        Device verifiers apply (stream 0's); host-only verifiers do not, and a warning says so."""
+        if self._host_verifiers:
+            warnings.warn(f"custom verifiers of {sorted(self._host_verifiers)} are not device-runnable (only the linear "
+                          "pipeline of train_verifier_model is): predict_clips returns their models' unverified scores",
+                          stacklevel=2)
         torch = _torch()
         if isinstance(clips, torch.Tensor):            # CPU (ideally pinned) or CUDA int16 tensor: no host copy
             if clips.dtype != torch.int16:

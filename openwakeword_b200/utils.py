@@ -98,6 +98,7 @@ class AudioFeatures:
         self.feature_buffer_max_len = 120
         self._feature_init = None if feature_init is None else np.asarray(feature_init, np.float32)
         self._streams_ready = False
+        self._verifier_banks = False    # set by Model once the handle has a verifier bank (split calls skip the banks)
         # the three session callables of the reference (utils.py:87,93), numpy in / numpy out
         self.melspec_model_predict = self._melspec_model_predict
         self.embedding_model_predict = self._embedding_model_predict
@@ -244,12 +245,20 @@ class AudioFeatures:
             # a call longer than max_chunks*1280 samples (the reference accepts up to its 10 s raw buffer) runs as
             # several device calls of <= max_chunks chunks; per head the result is the max over all chunk windows, as in
             # model.py:287-298.  Only the scope of the mel graph's -80 dB clamp differs (per device call, not per host call).
+            # Custom verifiers run after that max, on the newest window (model.py:319-328): the parts run without the
+            # verifier banks and Model.predict verifies the max.
             part = np.empty_like(scores_out)
-            for k, c0 in enumerate(range(0, n_chunks, self.max_chunks)):
-                c1 = min(c0 + self.max_chunks, n_chunks)
-                self.ctx.step_host(np.ascontiguousarray(ready[:, c0 * CHUNK:c1 * CHUNK]), c1 - c0, scores_out if k == 0 else part)
-                if k:
-                    np.maximum(scores_out, part, out=scores_out)
+            if self._verifier_banks:
+                self.ctx.enable_verifiers(False)
+            try:
+                for k, c0 in enumerate(range(0, n_chunks, self.max_chunks)):
+                    c1 = min(c0 + self.max_chunks, n_chunks)
+                    self.ctx.step_host(np.ascontiguousarray(ready[:, c0 * CHUNK:c1 * CHUNK]), c1 - c0, scores_out if k == 0 else part)
+                    if k:
+                        np.maximum(scores_out, part, out=scores_out)
+            finally:
+                if self._verifier_banks:
+                    self.ctx.enable_verifiers(True)
         self.accumulated_samples = 0
         self._last_scores = scores_out
         return ready.shape[1], n_chunks
