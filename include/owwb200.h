@@ -198,7 +198,8 @@ int oww_embed_clips(oww_ctx* ctx, const int16_t* d_pcm, int n_clips, int n_sampl
 /* predict_clip for n_clips equal-length clips, each from a FRESH state seeded with h_feature_init
  * (SURVEY.md F9): pad_samples zeros each side, 1280-sample steps, steps = len(range(0, L-1280, 1280)).
  * d_scores [n_clips][steps][oww_n_outputs].  Raw head outputs (the first-5-zeroing of
- * model.py:330-333 is label bookkeeping done by the host wrapper).  Uses a private stream set.  */
+ * model.py:330-333 is label bookkeeping done by the host wrapper).  Equals streaming the padded clips through
+ * fresh streams of this handle's configuration; uses none of the handle's streams.  No heads: returns at once. */
 int oww_predict_clips(oww_ctx* ctx, const int16_t* d_pcm, int n_clips, int n_samples, int pad_samples,
                       const float* h_feature_init, int n_rows, float* d_scores, void* stream);
 

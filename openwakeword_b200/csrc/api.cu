@@ -88,15 +88,6 @@ __global__ void reset_kernel(const int* ids, int n_ids, int n_streams, int16_t* 
     }
 }
 
-__global__ void gather_chunk_kernel(const int16_t* pcm, int n_clips, int n_samples, int pad, int step, int16_t* out) {
-    const int64_t total = (int64_t)n_clips * OWW_SAMPLES_PER_CHUNK;
-    for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (int64_t)gridDim.x * blockDim.x) {
-        const int c = (int)(i / OWW_SAMPLES_PER_CHUNK), k = (int)(i % OWW_SAMPLES_PER_CHUNK);
-        const int64_t p = (int64_t)step * OWW_SAMPLES_PER_CHUNK + k - pad;
-        out[i] = (p >= 0 && p < n_samples) ? pcm[(int64_t)c * n_samples + p] : (int16_t)0;
-    }
-}
-
 }  // namespace
 // Tails of the all-ones window per tails-bearing tensor, in the compact G = 1 layout, computed once per weight set by
 // the full-window tensor-core kernels (cnn_tc.cu) - the state every freshly reset stream starts from (its mel history IS
@@ -125,32 +116,6 @@ void free_streams(oww_ctx* c) {
     c->n_streams = 0;
 }
 
-int ensure_act(oww_ctx* ctx, size_t floats) {
-    if (ctx->cfg.cnn_mode == OWW_CNN_TC_WINDOW || ctx->cfg.cnn_mode == OWW_CNN_TC_INCREMENTAL) {
-        // `floats` is n_windows * 74*32*24 (layer-1 output of the fp32 path): size the fp16 planes for the same windows
-        int n_win = (int)(floats / ((size_t)74 * 32 * 24));
-        if (n_win < 1) n_win = 1;
-        if (n_win > ctx->window_batch) n_win = ctx->window_batch;
-        const size_t units = oww_tc_act_units(ctx, n_win);
-        if (ctx->tc_act_units < units) {
-            cudaFree(ctx->d_tc_act[0]); cudaFree(ctx->d_tc_act[1]);
-            ctx->d_tc_act[0] = ctx->d_tc_act[1] = nullptr; ctx->tc_act_units = 0;
-            for (int i = 0; i < 2; ++i) {
-                OWW_CUDA(ctx, cudaMalloc(&ctx->d_tc_act[i], units * 16));
-                OWW_CUDA(ctx, cudaMemset(ctx->d_tc_act[i], 0, units * 16));
-            }
-            ctx->tc_act_units = units;
-        }
-    }
-    if (ctx->act_floats >= floats) return OWW_OK;
-    cudaFree(ctx->d_act[0]); cudaFree(ctx->d_act[1]);
-    ctx->d_act[0] = ctx->d_act[1] = nullptr; ctx->act_floats = 0;
-    OWW_CUDA(ctx, cudaMalloc(&ctx->d_act[0], floats * sizeof(float)));
-    OWW_CUDA(ctx, cudaMalloc(&ctx->d_act[1], floats * sizeof(float)));
-    ctx->act_floats = floats;
-    return OWW_OK;
-}
-
 // grow the fp16 plane scratch of the tensor-core window / clip passes to `units` 16-byte units per buffer
 int ensure_tc_units(oww_ctx* ctx, size_t units) {
     if (ctx->tc_act_units >= units) return OWW_OK;
@@ -161,6 +126,57 @@ int ensure_tc_units(oww_ctx* ctx, size_t units) {
         OWW_CUDA(ctx, cudaMemset(ctx->d_tc_act[i], 0, units * 16));
     }
     ctx->tc_act_units = units;
+    return OWW_OK;
+}
+
+int ensure_act(oww_ctx* ctx, size_t floats) {
+    if (ctx->cfg.cnn_mode == OWW_CNN_TC_WINDOW || ctx->cfg.cnn_mode == OWW_CNN_TC_INCREMENTAL) {
+        // `floats` is n_windows * 74*32*24 (layer-1 output of the fp32 path): size the fp16 planes for the same windows
+        int n_win = (int)(floats / ((size_t)74 * 32 * 24));
+        if (n_win < 1) n_win = 1;
+        if (n_win > ctx->window_batch) n_win = ctx->window_batch;
+        const int rc = ensure_tc_units(ctx, oww_tc_act_units(ctx, n_win));
+        if (rc) return rc;
+    }
+    if (ctx->act_floats >= floats) return OWW_OK;
+    cudaFree(ctx->d_act[0]); cudaFree(ctx->d_act[1]);
+    ctx->d_act[0] = ctx->d_act[1] = nullptr; ctx->act_floats = 0;
+    OWW_CUDA(ctx, cudaMalloc(&ctx->d_act[0], floats * sizeof(float)));
+    OWW_CUDA(ctx, cudaMalloc(&ctx->d_act[1], floats * sizeof(float)));
+    ctx->act_floats = floats;
+    return OWW_OK;
+}
+
+// clips per slab of a clip pass over T mel rows: 1 GiB of fp16 planes per buffer of the tensor-core CNN
+int clip_slab(const oww_ctx* ctx, int n, int T) {
+    return (int)std::min<size_t>(n, std::max<size_t>(1, ((size_t)1 << 26) / oww_tc_act_units_T(ctx, 1, T)));
+}
+
+// Fully convolutional CNN pass over linear mel [n][T][32] (T >= 76, SURVEY.md F10): the (T - 76) / 8 + 1 embedding rows
+// of input i land at d_emb + i * out_rows * 96.  Slabs of inputs bounded by the mode's activation scratch.
+int oww_cnn_clip(oww_ctx* ctx, const float* d_mel, int n, int T, float* d_emb, int out_rows, cudaStream_t s) {
+    if (!ctx->emb_loaded) return oww_fail(ctx, OWW_EINVAL, "embedding weights not loaded");
+    if (T < OWW_WINDOW_ROWS) return oww_fail(ctx, OWW_EINVAL, "need at least 76 mel rows");
+    const int t_use = OWW_WINDOW_ROWS + 8 * ((T - OWW_WINDOW_ROWS) / 8);
+    const bool tc = ctx->cfg.cnn_mode != OWW_CNN_FP32_WINDOW;
+    int slab, rc;
+    if (tc) {
+        slab = clip_slab(ctx, n, t_use);
+        rc = ensure_tc_units(ctx, oww_tc_act_units_T(ctx, slab, t_use));
+    } else {
+        const size_t per = (size_t)(t_use - 2) * 32 * 24;          // layer-1 output of one input, the largest tensor
+        rc = ensure_act(ctx, std::max(per, (size_t)ctx->window_batch * 74 * 32 * 24));
+        slab = (int)(ctx->act_floats / per);
+    }
+    if (rc) return rc;
+    for (int c0 = 0; c0 < n; c0 += slab) {
+        const int m = std::min(slab, n - c0);
+        const WindowSrc src{d_mel + (int64_t)c0 * T * 32, (int64_t)T * 32, nullptr, -1, 0, 0};
+        float* out = d_emb + (int64_t)c0 * out_rows * 96;
+        rc = tc ? oww_cnn_tc_pyramid(ctx, src, m, t_use, out, out_rows, -1, nullptr, s)
+                : oww_cnn_fp32_pyramid(ctx, src, m, t_use, out, out_rows, -1, nullptr, s);
+        if (rc) return rc;
+    }
     return OWW_OK;
 }
 
@@ -344,11 +360,6 @@ int oww_create(const oww_config* cfg, oww_ctx** out) {
 void oww_destroy(oww_ctx* ctx) {
     if (!ctx) return;
     cudaSetDevice(ctx->device);
-    if (ctx->clip_ctx) { oww_ctx* c = ctx->clip_ctx; ctx->clip_ctx = nullptr; free_streams(c);
-        cudaStreamDestroy(c->own_stream);
-        cudaFree(c->d_tails_template);
-        cudaFree(c->d_tc_act[0]); cudaFree(c->d_tc_act[1]);
-        cudaFree(c->slot[0].d_pcm); oww_heads_grp_free(c); delete c; }
     free_streams(ctx);
     oww_heads_grp_free(ctx);
     cudaFree(ctx->d_window); cudaFree(ctx->d_twiddle); cudaFree(ctx->d_mel_start); cudaFree(ctx->d_mel_len);
@@ -684,40 +695,18 @@ int oww_embed_clips(oww_ctx* ctx, const int16_t* d_pcm, int n_clips, int n_sampl
         return oww_fail(ctx, OWW_EINVAL, "Embedding model requires the input melspectrograms to have at least 76 frames");
     const int W = (T - OWW_WINDOW_ROWS) / 8 + 1;
     cudaStream_t s = (cudaStream_t)stream;
-    if (ctx->cfg.cnn_mode != OWW_CNN_FP32_WINDOW) {
-        // tensor-core modes: per-clip mel (one call per clip, as the reference's CPU path runs the graph), then ONE fully
-        // convolutional tensor-core pass over the clip's [T x 32] mel (SURVEY.md F10) - slabs bounded by a ~1 GB plane scratch
-        const int t_use = OWW_WINDOW_ROWS + 8 * (W - 1);
-        const size_t per1 = oww_tc_act_units_T(ctx, 1, t_use);
-        int slab = (int)std::max<size_t>(1, ((size_t)1 << 26) / per1);          // 2^26 units = 1 GiB per buffer
-        slab = std::min(slab, n_clips);
-        int rc = ensure_tc_units(ctx, oww_tc_act_units_T(ctx, slab, t_use));
-        if (rc) return rc;
-        float* d_mel = nullptr;
-        OWW_CUDA(ctx, cudaMallocAsync(&d_mel, (size_t)slab * T * 32 * sizeof(float), s));
-        for (int c0 = 0; c0 < n_clips; c0 += slab) {
-            const int m = std::min(slab, n_clips - c0);
-            MelLaunch ml{d_pcm + (size_t)c0 * n_samples, (int64_t)n_samples, n_samples, nullptr, nullptr, d_mel, (int64_t)T * 32,
-                         -1, nullptr, m, 1, 0};
-            if ((rc = oww_mel_launch(ctx, ml, s))) break;
-            if ((rc = oww_cnn_tc_clip(ctx, d_mel, m, T, d_emb + (size_t)c0 * W * 96, s))) break;
-        }
-        cudaFreeAsync(d_mel, s);
-        return rc;
-    }
-    // slabs bounded by the activation scratch (~512 windows' worth of layer-1 output)
-    const size_t per_clip = (size_t)(T - 2) * 32 * 24;
-    int rc = ensure_act(ctx, std::max(ctx->act_floats, std::max(per_clip, (size_t)ctx->window_batch * 74 * 32 * 24)));
-    if (rc) return rc;
-    const int slab = (int)std::max<size_t>(1, ctx->act_floats / per_clip);
+    // per slab of clips: the mel of each clip (one call per clip, as the reference's CPU path runs the graph), then ONE
+    // fully convolutional CNN pass over the clips' [T x 32] mel (SURVEY.md F10)
+    const int slab = clip_slab(ctx, n_clips, OWW_WINDOW_ROWS + 8 * (W - 1));
     float* d_mel = nullptr;
-    OWW_CUDA(ctx, cudaMallocAsync(&d_mel, (size_t)std::min(slab, n_clips) * T * 32 * sizeof(float), s));
+    OWW_CUDA(ctx, cudaMallocAsync(&d_mel, (size_t)slab * T * 32 * sizeof(float), s));
+    int rc = OWW_OK;
     for (int c0 = 0; c0 < n_clips; c0 += slab) {
         const int m = std::min(slab, n_clips - c0);
         MelLaunch ml{d_pcm + (size_t)c0 * n_samples, (int64_t)n_samples, n_samples, nullptr, nullptr, d_mel, (int64_t)T * 32,
                      -1, nullptr, m, 1, 0};
         if ((rc = oww_mel_launch(ctx, ml, s))) break;
-        if ((rc = oww_cnn_clip_fp32(ctx, d_mel, m, T, d_emb + (size_t)c0 * W * 96, s))) break;
+        if ((rc = oww_cnn_clip(ctx, d_mel, m, T, d_emb + (size_t)c0 * W * 96, W, s))) break;
     }
     cudaFreeAsync(d_mel, s);
     return rc;
@@ -727,109 +716,51 @@ int oww_predict_clips(oww_ctx* ctx, const int16_t* d_pcm, int n_clips, int n_sam
                       const float* h_feature_init, int n_rows, float* d_scores, void* stream) {
     if (!ctx || !d_pcm || !d_scores) return oww_fail(ctx, OWW_EINVAL, "null argument");
     if (n_clips < 1 || n_samples < 1 || pad_samples < 0) return oww_fail(ctx, OWW_EINVAL, "bad clip geometry");
+    if (h_feature_init && n_rows < 0) return oww_fail(ctx, OWW_EINVAL, "n_rows=%d", n_rows);
     OWW_CUDA(ctx, cudaSetDevice(ctx->device));
     const int64_t L = (int64_t)n_samples + 2 * (int64_t)pad_samples;
     const int steps = L > OWW_SAMPLES_PER_CHUNK ? (int)((L - OWW_SAMPLES_PER_CHUNK + OWW_SAMPLES_PER_CHUNK - 1) / OWW_SAMPLES_PER_CHUNK) : 0;
-    if (steps == 0) return OWW_OK;
+    if (steps == 0 || ctx->heads.empty()) return OWW_OK;
     cudaStream_t s = (cudaStream_t)stream;
-    {
-        // ---- bulk path (SURVEY.md F10): per slab of clips ONE mel launch over the padded clips (frames grouped and
-        //      clamped per streaming call, behind the 71 rows of ones a fresh stream's window starts with), ONE fully
-        //      convolutional tensor-core pass per conv layer over [76 + 8 (steps-1)] x 32, then the heads over all sliding
-        //      windows of [feature_init rows | embeddings] in one launch.  Bit-identical to streaming the clips.
-        bool tc_all = ctx->cfg.cnn_mode != OWW_CNN_FP32_WINDOW && steps <= 8192 && !ctx->heads.empty();
-        for (size_t i = 0; i < ctx->heads.size(); ++i) tc_all = tc_all && oww_heads_tc_supported(ctx, (int)i);
-        if (tc_all) {
-            const int T_v = OWW_WINDOW_ROWS + 8 * (steps - 1);
-            const int init_rows = h_feature_init ? n_rows : OWW_INIT_FEATURE_ROWS;
-            const int64_t f_stride = (int64_t)(init_rows + steps) * 96;
-            const size_t per1 = oww_tc_act_units_T(ctx, 1, T_v);
-            int slab = (int)std::max<size_t>(1, ((size_t)1 << 26) / per1);      // 1 GiB of fp16 planes per buffer
-            slab = std::min(slab, n_clips);
-            int rc = ensure_tc_units(ctx, oww_tc_act_units_T(ctx, slab, T_v));
-            if (rc) return rc;
-            float *d_v = nullptr, *d_f = nullptr, *d_init = nullptr;
-            OWW_CUDA(ctx, cudaMallocAsync(&d_v, (size_t)slab * T_v * 32 * sizeof(float), s));
-            OWW_CUDA(ctx, cudaMallocAsync(&d_f, (size_t)slab * f_stride * sizeof(float), s));
-            if (h_feature_init && init_rows > 0) {
-                OWW_CUDA(ctx, cudaMallocAsync(&d_init, (size_t)init_rows * 96 * sizeof(float), s));
-                OWW_CUDA(ctx, cudaMemcpyAsync(d_init, h_feature_init, (size_t)init_rows * 96 * sizeof(float), cudaMemcpyHostToDevice, s));
-            }
-            for (int c0 = 0; c0 < n_clips && rc == OWW_OK; c0 += slab) {
-                const int m = std::min(slab, n_clips - c0);
-                if ((rc = oww_mel_clips_launch(ctx, d_pcm + (size_t)c0 * n_samples, n_samples, m, n_samples, pad_samples, steps, d_v,
-                                               (int64_t)T_v * 32, s))) break;
-                if (init_rows > 0) {
-                    fill_init_rows_kernel<<<std::min(1024, (m * init_rows * 24 + 255) / 256), 256, 0, s>>>(d_f, f_stride, m, d_init, init_rows);
-                    ctx->launches++;
-                }
-                // embeddings of step st land at row init_rows + st of the clip's feature array
-                WindowSrc src{d_v, (int64_t)T_v * 32, nullptr, -1, 0, 0};
-                if ((rc = oww_cnn_tc_clip_rows(ctx, src, m, T_v, d_f + (int64_t)init_rows * 96, init_rows + steps, s))) break;
-                FeatSrc fs{d_f, f_stride, nullptr, -1, 0};
-                fs.steps = steps; fs.row0 = init_rows;
-                float* out = d_scores + (size_t)c0 * steps * ctx->n_out_total;
-                if ((rc = oww_heads_all(ctx, fs, m * steps, out, ctx->n_out_total, 0, s))) break;
-                rc = oww_verifiers_apply(ctx, fs, m * steps, out, ctx->n_out_total, true, s);       // clip slot, every step
-            }
-            cudaFreeAsync(d_v, s); cudaFreeAsync(d_f, s);
-            if (d_init) cudaFreeAsync(d_init, s);
-            return rc;
-        }
+    // Bulk path (SURVEY.md F10), per slab of clips: for each segment of at most 8192 steps ONE mel launch over the padded
+    // clips (frames grouped and clamped per streaming call, behind the 71 rows of ones a fresh stream's window starts
+    // with) and ONE fully convolutional CNN pass over its rows; then the heads and the verifiers over all sliding windows
+    // of [feature_init rows | embeddings].  The same arithmetic as streaming the clips through fresh streams.
+    const int seg_steps = std::min(steps, 8192);
+    const int T_seg = OWW_WINDOW_ROWS + 8 * (seg_steps - 1);
+    const int init_rows = h_feature_init ? n_rows : OWW_INIT_FEATURE_ROWS;
+    const int64_t f_stride = (int64_t)(init_rows + steps) * 96;
+    const int slab = clip_slab(ctx, n_clips, T_seg);
+    float *d_v = nullptr, *d_f = nullptr, *d_init = nullptr;
+    OWW_CUDA(ctx, cudaMallocAsync(&d_v, (size_t)slab * T_seg * 32 * sizeof(float), s));
+    OWW_CUDA(ctx, cudaMallocAsync(&d_f, (size_t)slab * f_stride * sizeof(float), s));
+    if (h_feature_init && init_rows > 0) {
+        OWW_CUDA(ctx, cudaMallocAsync(&d_init, (size_t)init_rows * 96 * sizeof(float), s));
+        OWW_CUDA(ctx, cudaMemcpyAsync(d_init, h_feature_init, (size_t)init_rows * 96 * sizeof(float), cudaMemcpyHostToDevice, s));
     }
-    const int slab_max = 16384;
-    // the private stream set shares this handle's weights (shallow copy, non-owning)
-    if (!ctx->clip_ctx) {
-        oww_ctx* c = new (std::nothrow) oww_ctx();
-        if (!c) return oww_fail(ctx, OWW_ENOMEM, "out of host memory");
-        c->cfg = ctx->cfg; c->cfg.max_chunks = 1; c->device = ctx->device; c->sm_count = ctx->sm_count;
-        c->window_batch = ctx->window_batch;
-        c->fuse_step = ctx->fuse_step; c->tc_heads = ctx->tc_heads; c->tc_heads_terms = ctx->tc_heads_terms;
-        cudaStreamCreateWithFlags(&c->own_stream, cudaStreamNonBlocking);
-        ctx->clip_ctx = c;
-    }
-    oww_ctx* c = ctx->clip_ctx;
-    c->mel_loaded = ctx->mel_loaded; c->d_window = ctx->d_window; c->d_twiddle = ctx->d_twiddle;
-    c->d_mel_start = ctx->d_mel_start; c->d_mel_len = ctx->d_mel_len; c->d_mel_w = ctx->d_mel_w; c->mel_kmax = ctx->mel_kmax;
-    if (c->emb_loaded != ctx->emb_loaded || c->d_inc_w != ctx->d_inc_w) c->tails_template_valid = false;
-    c->emb_loaded = ctx->emb_loaded;
-    for (int li = 0; li < OWW_N_CONV; ++li) { c->conv[li] = ctx->conv[li]; c->tc_w_off[li] = ctx->tc_w_off[li]; c->tc_sb_off[li] = ctx->tc_sb_off[li]; }
-    c->d_tc_w = ctx->d_tc_w; c->d_tc_sb = ctx->d_tc_sb; c->d_inc_w = ctx->d_inc_w;
-    c->d_tc_w3 = ctx->d_tc_w3; c->d_tc_sb3 = ctx->d_tc_sb3; c->split_from = ctx->split_from;
-
-    c->heads = ctx->heads; c->n_out_total = ctx->n_out_total; c->max_n_in = ctx->max_n_in; c->d_head_devs = ctx->d_head_devs;
-    c->gates = ctx->gates; c->d_gates = ctx->d_gates;
-    // verifier banks: the weights are shared, and every clip (stream of the private set) uses the bank's clip slot
-    std::vector<VerifierBank> clip_banks;
-    if (ctx->verifiers_on) clip_banks = ctx->banks;
-    for (auto& b : clip_banks) b.d_assign = nullptr;
     int rc = OWW_OK;
-    for (int c0 = 0; c0 < n_clips && rc == OWW_OK; c0 += slab_max) {
-        const int m = std::min(slab_max, n_clips - c0);
-        c->banks.clear();              // the private set allocates no assignment of its own
-        if (c->n_streams != m) { if ((rc = oww_set_streams(c, m))) { ctx->err = c->err; break; } }
-        if ((rc = oww_reset(c, nullptr, m, h_feature_init, h_feature_init ? n_rows : OWW_INIT_FEATURE_ROWS))) { ctx->err = c->err; break; }
-        c->banks = clip_banks;
-        const size_t stage_bytes = (size_t)m * OWW_SAMPLES_PER_CHUNK * sizeof(int16_t);
-        if (c->slot[0].pcm_bytes < stage_bytes) {
-            cudaFree(c->slot[0].d_pcm); c->slot[0].d_pcm = nullptr;
-            OWW_CUDA(ctx, cudaMalloc(&c->slot[0].d_pcm, stage_bytes));
-            c->slot[0].pcm_bytes = stage_bytes;
+    for (int c0 = 0; c0 < n_clips && rc == OWW_OK; c0 += slab) {
+        const int m = std::min(slab, n_clips - c0);
+        for (int k0 = 0; k0 < steps && rc == OWW_OK; k0 += seg_steps) {
+            const int k1 = std::min(steps, k0 + seg_steps), T = OWW_WINDOW_ROWS + 8 * (k1 - k0 - 1);
+            if ((rc = oww_mel_clips_launch(ctx, d_pcm + (size_t)c0 * n_samples, n_samples, m, n_samples, pad_samples, k0, k1, d_v,
+                                           (int64_t)T * 32, s))) break;
+            if (k0 == 0 && init_rows > 0) {
+                fill_init_rows_kernel<<<std::min(1024, (m * init_rows * 24 + 255) / 256), 256, 0, s>>>(d_f, f_stride, m, d_init, init_rows);
+                ctx->launches++;
+            }
+            // embeddings of step st land at row init_rows + st of the clip's feature array
+            rc = oww_cnn_clip(ctx, d_v, m, T, d_f + (int64_t)(init_rows + k0) * 96, init_rows + steps, s);
         }
-        for (int st = 0; st < steps; ++st) {
-            unsigned grid = (unsigned)std::min<int64_t>(((int64_t)m * OWW_SAMPLES_PER_CHUNK + 255) / 256, (int64_t)ctx->sm_count * 32);
-            gather_chunk_kernel<<<grid, 256, 0, s>>>(d_pcm + (size_t)c0 * n_samples, m, n_samples, pad_samples, st, c->slot[0].d_pcm);
-            c->launches++;
-            rc = step_core(c, c->slot[0].d_pcm, OWW_SAMPLES_PER_CHUNK, 1,
-                           d_scores + ((size_t)c0 * steps + st) * ctx->n_out_total, steps * ctx->n_out_total, s);
-            if (rc) { ctx->err = c->err; break; }
-        }
+        if (rc) break;
+        FeatSrc fs{d_f, f_stride, nullptr, -1, 0};
+        fs.steps = steps; fs.row0 = init_rows;
+        float* out = d_scores + (size_t)c0 * steps * ctx->n_out_total;
+        if ((rc = oww_heads_all(ctx, fs, m * steps, out, ctx->n_out_total, 0, s))) break;
+        rc = oww_verifiers_apply(ctx, fs, m * steps, out, ctx->n_out_total, true, s);       // clip slot, every step
     }
-    ctx->launches += c->launches; c->launches = 0;
-    c->heads.clear();   // do not let the child free shared blobs
-    c->d_head_devs = nullptr;
-    c->gates.clear(); c->d_gates = nullptr;
-    c->banks.clear();
+    cudaFreeAsync(d_v, s); cudaFreeAsync(d_f, s);
+    if (d_init) cudaFreeAsync(d_init, s);
     return rc;
 }
 
@@ -841,8 +772,9 @@ int oww_debug_layer(oww_ctx* ctx, const float* d_windows, int n, int layer, floa
     int rc = ensure_act(ctx, (size_t)std::min(n, ctx->window_batch) * 74 * 32 * 24);
     if (rc) return rc;
     WindowSrc src{d_windows, (int64_t)OWW_WINDOW_ROWS * 32, nullptr, -1, 0, 0};
-    if (ctx->cfg.cnn_mode == OWW_CNN_TC_WINDOW) return oww_cnn_tc_pyramid(ctx, src, n, nullptr, layer, d_out, (cudaStream_t)stream);
-    return oww_cnn_fp32_pyramid(ctx, src, n, nullptr, layer, d_out, (cudaStream_t)stream);
+    if (ctx->cfg.cnn_mode == OWW_CNN_TC_WINDOW)
+        return oww_cnn_tc_pyramid(ctx, src, n, OWW_WINDOW_ROWS, nullptr, 1, layer, d_out, (cudaStream_t)stream);
+    return oww_cnn_fp32_pyramid(ctx, src, n, OWW_WINDOW_ROWS, nullptr, 1, layer, d_out, (cudaStream_t)stream);
 }
 
 int oww_debug_inc_plan(oww_ctx* ctx, int group, int n_streams, int32_t* out, int max_ints) {

@@ -284,9 +284,10 @@ int dispatch_conv(oww_ctx* ctx, const ConvLayer& L, const ConvArgs& a, cudaStrea
     return oww_fail(ctx, OWW_EUNSUPPORTED, "no conv kernel for %dx%d %d->%d", L.kh, L.kw, L.cin, L.cout);
 }
 
-// Runs layers 0..19 on n samples whose mel source has t_mel rows; result [n][W][96] in d_out.
-int run_pyramid(oww_ctx* ctx, const WindowSrc& src, int n, int t_mel, float* d_out, cudaStream_t s, int stop_layer = -1,
-                float* d_dbg = nullptr) {
+// Runs layers 0..19 on n samples whose mel source has t_mel rows; the W embedding rows of sample i land at
+// d_out + i * out_stride.
+int run_pyramid(oww_ctx* ctx, const WindowSrc& src, int n, int t_mel, float* d_out, int64_t out_stride, cudaStream_t s,
+                int stop_layer = -1, float* d_dbg = nullptr) {
     float* bufs[2] = {ctx->d_act[0], ctx->d_act[1]};
     int cur = 0;
     int t = t_mel, f = 32;
@@ -296,7 +297,7 @@ int run_pyramid(oww_ctx* ctx, const WindowSrc& src, int n, int t_mel, float* d_o
         const int t_out = t - (L.kh - 1);
         const bool last = li == OWW_N_CONV - 1;
         float* out = last ? d_out : bufs[cur];
-        const int64_t stride_out = (int64_t)t_out * f * L.cout;
+        const int64_t stride_out = last ? out_stride : (int64_t)t_out * f * L.cout;
         if (!last && (size_t)stride_out * n > ctx->act_floats)
             return oww_fail(ctx, OWW_ENOMEM, "activation scratch too small");
         if (li == 0) {
@@ -334,8 +335,9 @@ int run_pyramid(oww_ctx* ctx, const WindowSrc& src, int n, int t_mel, float* d_o
 
 }  // namespace
 
-int oww_cnn_fp32_pyramid(oww_ctx* ctx, const WindowSrc& src, int n, float* d_emb, int stop_layer, float* d_dbg, cudaStream_t s) {
-    return run_pyramid(ctx, src, n, OWW_WINDOW_ROWS, d_emb, s, stop_layer, d_dbg);
+int oww_cnn_fp32_pyramid(oww_ctx* ctx, const WindowSrc& src, int n, int T0, float* d_emb, int out_rows, int stop_layer,
+                         float* d_dbg, cudaStream_t s) {
+    return run_pyramid(ctx, src, n, T0, d_emb, (int64_t)out_rows * OWW_EMBEDDING_DIM, s, stop_layer, d_dbg);
 }
 
 int oww_cnn_window(oww_ctx* ctx, const WindowSrc& src, int n_windows, float* d_emb, cudaStream_t s, bool capture_tails) {
@@ -377,27 +379,10 @@ int oww_cnn_window(oww_ctx* ctx, const WindowSrc& src, int n_windows, float* d_e
             }
             rc = oww_cnn_tc_pyramid_cap(ctx, sub, n, o, cap.n_win ? &cap : nullptr, s);
         } else {
-            rc = run_pyramid(ctx, sub, n, OWW_WINDOW_ROWS, o, s);
+            rc = run_pyramid(ctx, sub, n, OWW_WINDOW_ROWS, o, OWW_EMBEDDING_DIM, s);
         }
         if (rc) return rc;
         w0 += n;
-    }
-    return OWW_OK;
-}
-
-int oww_cnn_clip_fp32(oww_ctx* ctx, const float* d_mel, int n, int T, float* d_emb, cudaStream_t s) {
-    if (!ctx->emb_loaded) return oww_fail(ctx, OWW_EINVAL, "embedding weights not loaded");
-    if (T < OWW_WINDOW_ROWS) return oww_fail(ctx, OWW_EINVAL, "need at least 76 mel rows");
-    const int W = (T - OWW_WINDOW_ROWS) / 8 + 1;
-    const int t_use = OWW_WINDOW_ROWS + 8 * (W - 1);
-    const int64_t per = (int64_t)(t_use - 2) * 32 * 24;
-    int nb = (int)(ctx->act_floats / per);
-    if (nb < 1) return oww_fail(ctx, OWW_ENOMEM, "clip too long for the activation scratch");
-    for (int c0 = 0; c0 < n; c0 += nb) {
-        const int m = (n - c0 < nb) ? n - c0 : nb;
-        WindowSrc src{d_mel + (int64_t)c0 * T * 32, (int64_t)T * 32, nullptr, -1, 0, 0};
-        int rc = run_pyramid(ctx, src, m, t_use, d_emb + (int64_t)c0 * W * OWW_EMBEDDING_DIM, s);
-        if (rc) return rc;
     }
     return OWW_OK;
 }

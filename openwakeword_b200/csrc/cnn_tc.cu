@@ -693,30 +693,18 @@ size_t oww_tc_act_units_T(const oww_ctx* ctx, int n, int T0) {
 }
 size_t oww_tc_act_units(const oww_ctx* ctx, int n_windows) { return oww_tc_act_units_T(ctx, n_windows, OWW_WINDOW_ROWS); }
 
-// Runs the pyramid in tensor-core mode on n inputs of T0 mel rows each (n windows of 76 rows, or n clips: the CNN is
-// fully convolutional in time, SURVEY.md F10) -> d_emb [n][(T0 - 76) / 8 + 1][96] fp32.  Layers >= split_from take split
-// (hi/lo) operands.  stop_layer >= 0: stop after that layer (and its pool) and unpack it to NHWC fp32 in d_dbg.
-int oww_cnn_tc_pyramid_impl(oww_ctx* ctx, const WindowSrc& src, int n, int T0, int split_from, float* d_emb, int stop_layer,
-                            float* d_dbg, const TailCapture* cap, cudaStream_t s);
-int oww_cnn_tc_pyramid(oww_ctx* ctx, const WindowSrc& src, int n, float* d_emb, int stop_layer, float* d_dbg, cudaStream_t s) {
-    return oww_cnn_tc_pyramid_impl(ctx, src, n, OWW_WINDOW_ROWS, ctx->split_from, d_emb, stop_layer, d_dbg, nullptr, s);
+// Runs the pyramid in tensor-core mode (contract of oww_cnn_tc_pyramid, oww_internal.h).  Layers >= split_from take split
+// (hi/lo) operands.
+int oww_cnn_tc_pyramid_impl(oww_ctx* ctx, const WindowSrc& src, int n, int T0, int split_from, float* d_emb, int out_rows,
+                            int stop_layer, float* d_dbg, const TailCapture* cap, cudaStream_t s);
+int oww_cnn_tc_pyramid(oww_ctx* ctx, const WindowSrc& src, int n, int T0, float* d_emb, int out_rows, int stop_layer,
+                       float* d_dbg, cudaStream_t s) {
+    return oww_cnn_tc_pyramid_impl(ctx, src, n, T0, ctx->split_from, d_emb, out_rows, stop_layer, d_dbg, nullptr, s);
 }
 int oww_cnn_tc_pyramid_cap(oww_ctx* ctx, const WindowSrc& src, int n, float* d_emb, const TailCapture* cap, cudaStream_t s) {
     // tails of the layers inside the fused kernel (all below split_from: plain fp16 there as here) go to the group
     // layout through oww_inc_capture; tails of the incremental late layers (hi/lo) to the late template
-    return oww_cnn_tc_pyramid_impl(ctx, src, n, OWW_WINDOW_ROWS, ctx->split_from, d_emb, -1, nullptr, cap, s);
-}
-int oww_cnn_tc_clip(oww_ctx* ctx, const float* d_mel, int n, int T, float* d_emb, cudaStream_t s) {
-    WindowSrc src{d_mel, (int64_t)T * 32, nullptr, -1, 0, 0};
-    const int W = (T - OWW_WINDOW_ROWS) / 8 + 1;
-    return oww_cnn_tc_pyramid_impl(ctx, src, n, OWW_WINDOW_ROWS + 8 * (W - 1), ctx->split_from, d_emb, -1, nullptr, nullptr, s);
-}
-// same, the embeddings of input i landing at d_emb + i * out_rows * 96 (rows of a larger per-input array)
-int oww_cnn_tc_clip_rows(oww_ctx* ctx, const WindowSrc& src, int n, int T, float* d_emb, int out_rows, cudaStream_t s) {
-    ctx->tc_rows_out_override = out_rows;
-    int rc = oww_cnn_tc_pyramid_impl(ctx, src, n, T, ctx->split_from, d_emb, -1, nullptr, nullptr, s);
-    ctx->tc_rows_out_override = 0;
-    return rc;
+    return oww_cnn_tc_pyramid_impl(ctx, src, n, OWW_WINDOW_ROWS, ctx->split_from, d_emb, 1, -1, nullptr, cap, s);
 }
 
 template <int TERMS>
@@ -731,8 +719,8 @@ static int dispatch_tc(oww_ctx* ctx, int cgp, int np, const TcConvArgs& a, cudaS
     return oww_fail(ctx, OWW_EUNSUPPORTED, "no tensor-core conv instance for cgp=%d np=%d", cgp, np);
 }
 
-int oww_cnn_tc_pyramid_impl(oww_ctx* ctx, const WindowSrc& src, int n, int T0, int split_from, float* d_emb, int stop_layer,
-                            float* d_dbg, const TailCapture* cap, cudaStream_t s) {
+int oww_cnn_tc_pyramid_impl(oww_ctx* ctx, const WindowSrc& src, int n, int T0, int split_from, float* d_emb, int out_rows,
+                            int stop_layer, float* d_dbg, const TailCapture* cap, cudaStream_t s) {
     if (oww_tc_act_units_T(ctx, n, T0) > ctx->tc_act_units)
         return oww_fail(ctx, OWW_ENOMEM, "tensor-core activation scratch too small for %d x %d rows", n, T0);
     __half* bufs[2] = {reinterpret_cast<__half*>(ctx->d_tc_act[0]), reinterpret_cast<__half*>(ctx->d_tc_act[1])};
@@ -778,7 +766,7 @@ int oww_cnn_tc_pyramid_impl(oww_ctx* ctx, const WindowSrc& src, int n, int T0, i
             a.p_in = (int64_t)n * T * Wp;
             a.n_tiles = (int)((a.p_in + 127) / 128);
             a.out_split = out_split ? 1 : 0;
-            a.rows_out = (last && ctx->tc_rows_out_override) ? ctx->tc_rows_out_override : T_out;
+            a.rows_out = last ? out_rows : T_out;
             int rc = in_split ? dispatch_tc<3>(ctx, cgp, np, a, s) : dispatch_tc<1>(ctx, cgp, np, a, s);
             if (rc) return rc;
         }

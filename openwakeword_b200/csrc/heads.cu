@@ -69,18 +69,8 @@ __device__ __forceinline__ void dense_gather(const HeadDev& H, const FeatSrc& sr
             for (int q = tid; q < TB * (KC / 4); q += NTHREADS) {
                 const int tb = q / (KC / 4), k4 = (q % (KC / 4)) * 4;
                 const int s = s0 + tb;
-                const float* g = src.base;
-                bool ok = s < n;
-                if (ok) {
-                    if (src.count) {
-                        const int r = src.count[s] - src.back - H.n_in + frow;
-                        ok = r >= 0;
-                        g = src.base + (int64_t)s * src.stride + (int64_t)(r & src.rows_mask) * 96 + fcol + k4;
-                    } else {
-                        g = src.base + (int64_t)s * src.stride + (int64_t)frow * 96 + fcol + k4;
-                    }
-                }
-                cp_async16(xs + tb * XS_LD + k4, g, ok);
+                const float* row = s < n ? feat_row(feat_rows(src, H.n_in, s), frow) : nullptr;
+                cp_async16(xs + tb * XS_LD + k4, row ? row + fcol + k4 : src.base, row != nullptr);   // nullptr: zeros
             }
             // W tile: [KC][DP] in smem; DP is a power of two so the item -> (row, column) split is shifts; columns
             // beyond the real width D are zero-filled by cp.async (src-size 0)
@@ -275,7 +265,6 @@ int oww_heads_launch(oww_ctx* ctx, int head_id, const FeatSrc& src, int n, float
         for (int i = 0; i < (int)ctx->heads.size(); ++i) if (head_mask >> i & 1u) sel[nh++] = i;
     }
     if (nh == 0) return OWW_OK;
-    if (src.steps > 0) return oww_fail(ctx, OWW_EUNSUPPORTED, "sliding feature windows need the tensor-core heads kernel");
     HeadsArgs a;
     for (int i = 0; i < nh; ++i) {
         const Head& h = ctx->heads[sel[i]];

@@ -54,25 +54,6 @@ struct HeadsTcArgs {
     int stages, stage_bytes;
 };
 
-// Where sample s's window starts: row index r0 of feature row 0 (rows r0 + c, c = 0..n_in-1; negative = not available ->
-// zeros), the row mask (ring) or -1 (linear), and the sample's base pointer.
-struct HtRows { const float* base; int r0, mask; };
-__device__ __forceinline__ HtRows ht_rows(const FeatSrc& src, int n_in, int s, int n) {
-    HtRows w{nullptr, 0, -1};
-    if (s >= n) return w;
-    if (src.count) {                                       // per-stream ring
-        w.base = src.base + (int64_t)s * src.stride;
-        w.r0 = src.count[s] - src.back - n_in; w.mask = src.rows_mask;
-    } else if (src.steps > 0) {                            // sliding windows over per-clip linear feature rows (bulk path)
-        const int clip = s / src.steps, st = s - clip * src.steps;
-        w.base = src.base + (int64_t)clip * src.stride;
-        w.r0 = src.row0 + st + 1 - n_in;
-    } else {                                               // linear [n][n_in][96]
-        w.base = src.base + (int64_t)s * src.stride;
-    }
-    return w;
-}
-
 __global__ void __launch_bounds__(kHtThreads, 1) heads_tc_kernel(const __grid_constant__ HeadsTcArgs a) {
     extern __shared__ __align__(128) uint8_t smem[];
     const HtHead& HH = a.head[blockIdx.y];
@@ -164,13 +145,9 @@ __global__ void __launch_bounds__(kHtThreads, 1) heads_tc_kernel(const __grid_co
         const int row = 8 * (warp - kHtProducer - 1) + (lane & 7), jq = lane >> 3;
         const int s = s0 + row;
         float4 buf[2][6];
-        const HtRows rows_of = ht_rows(a.src, n_in, s, a.n);
+        const FeatRows rows_of = s < a.n ? feat_rows(a.src, n_in, s) : FeatRows{nullptr, 0, -1};
         auto load = [&](int c, float4* v) {
-            const float* p = nullptr;
-            if (c < n_in && rows_of.base) {
-                const int r = rows_of.r0 + c;
-                if (r >= 0) p = rows_of.base + (int64_t)(rows_of.mask >= 0 ? (r & rows_of.mask) : r) * 96;
-            }
+            const float* p = (c < n_in && rows_of.base) ? feat_row(rows_of, c) : nullptr;
 #pragma unroll
             for (int i = 0; i < 3; ++i) {
                 if (p) {

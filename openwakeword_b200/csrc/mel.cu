@@ -104,29 +104,38 @@ __global__ void __launch_bounds__(kThreads) mel_kernel(MelLaunch p, MelDev c) {
 // convolutional CNN pass needs:  out[clip] = [ones x 71 | frames 0..4 of call 0 | 8 frames of call 1 | ...],
 // 76 + 8 (steps - 1) rows.  The -80 dB clamp is per CALL (F7): frames are grouped [0,5), [5,13), [13,21), ... and each
 // group is clamped against its own maximum.  pad_samples zeros are virtual (nothing is copied).
-__global__ void __launch_bounds__(kThreads) mel_clip_kernel(const int16_t* pcm, int64_t clip_stride, int n_samples, int pad, int steps,
-                                                            float* out, int64_t out_stride, MelDev c) {
+// A launch covers the steps [k0, k1): virtual rows [8 k0, 76 + 8 (k1 - 1)), i.e. frames up to 8 k1 - 3 and, at k0 > 0,
+// from 8 k0 - 71 on.  From k0 = 9 on, that first frame lies 4 frames into its group: the kernel computes those 4 frames
+// for the group's maximum and does not write them.
+__host__ __device__ __forceinline__ int clip_group(int f) { return f < 5 ? 0 : (f - 5) / 8 + 1; }   // the call of frame f
+__host__ __device__ __forceinline__ int clip_first_group(int k0) { return clip_group(8 * k0 > 71 ? 8 * k0 - 71 : 0); }
+
+__global__ void __launch_bounds__(kThreads) mel_clip_kernel(const int16_t* pcm, int64_t clip_stride, int n_samples, int pad, int k0,
+                                                            int k1, float* out, int64_t out_stride, MelDev c) {
     extern __shared__ __align__(16) uint8_t dyn[];
     float2 (*s_buf)[2][256] = reinterpret_cast<float2 (*)[2][256]>(dyn);               // [kWarps][2][256]
     float2* s_tw = reinterpret_cast<float2*>(dyn + kWarps * 2 * 256 * sizeof(float2));
     float* s_win = reinterpret_cast<float*>(s_tw + 512);
     float (*s_pow)[264] = reinterpret_cast<float (*)[264]>(s_win + 512);
     int16_t (*s_frame)[512] = reinterpret_cast<int16_t (*)[512]>(s_pow + kWarps);       // [kWarps][512] padded-clip samples of a frame
-    int* s_gmax = reinterpret_cast<int*>(s_frame + kWarps);                              // [steps] per-call maxima (ordered-int encoding)
+    int* s_gmax = reinterpret_cast<int*>(s_frame + kWarps);                              // [k1 - g0] per-call maxima (ordered-int encoding)
     const int clip = blockIdx.x;
     const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+    const int v0 = 8 * k0;                                   // first virtual row written (output row 0)
+    const int g0 = clip_first_group(k0);
+    const int f0 = g0 == 0 ? 0 : 8 * g0 - 3;                 // first frame of group g0
+    const int n_frames = 8 * k1 - 3;
     for (int i = tid; i < 512; i += kThreads) { s_tw[i] = c.twiddle[i]; s_win[i] = c.window[i]; }
-    for (int i = tid; i < steps; i += kThreads) s_gmax[i] = INT_MIN;
+    for (int i = tid; i < k1 - g0; i += kThreads) s_gmax[i] = INT_MIN;
     const int16_t* body = pcm + (int64_t)clip * clip_stride;
     float* o = out + (int64_t)clip * out_stride;
-    const int n_frames = 8 * steps - 3;
-    for (int i = tid; i < 71 * 32; i += kThreads) o[i] = 1.0f;
+    for (int i = tid; i < (71 - v0) * 32; i += kThreads) o[i] = 1.0f;
     __syncthreads();
     const int my_start = c.mel_start[lane];
     const int my_len = c.mel_len[lane];
     const float* my_w = c.mel_w + lane * OWW_MEL_MAXSUPPORT;
     auto enc = [](float v) { int i = __float_as_int(v); return i >= 0 ? i : i ^ 0x7FFFFFFF; };   // order-preserving float -> int
-    for (int f = warp; f < n_frames; f += kWarps) {
+    for (int f = f0 + warp; f < n_frames; f += kWarps) {
         // stage the frame's 512 samples of the zero-padded clip, then run the ordinary frame routine on them
         for (int j = lane; j < 512; j += 32) {
             const int64_t p = (int64_t)f * OWW_HOP + j - pad;
@@ -135,19 +144,20 @@ __global__ void __launch_bounds__(kThreads) mel_clip_kernel(const int16_t* pcm, 
         __syncwarp();
         const float db = mel_frame_db<false>(nullptr, 0, s_frame[warp], 0, s_buf[warp][0], s_buf[warp][1], s_pow[warp], s_tw, s_win, c.kmax,
                                       my_start, my_len, my_w, lane);
-        o[(int64_t)(71 + f) * 32 + lane] = db;
+        if (71 + f >= v0) o[(int64_t)(71 + f - v0) * 32 + lane] = db;
         float m = db;
 #pragma unroll
         for (int k = 16; k > 0; k >>= 1) m = fmaxf(m, __shfl_xor_sync(0xffffffffu, m, k));
-        if (lane == 0) atomicMax(&s_gmax[f < 5 ? 0 : (f - 5) / 8 + 1], enc(m));
+        if (lane == 0) atomicMax(&s_gmax[clip_group(f) - g0], enc(m));
         __syncwarp();
     }
     __syncthreads();
-    for (int i = tid; i < n_frames * 32; i += kThreads) {
-        const int f = i >> 5;
-        const int e = s_gmax[f < 5 ? 0 : (f - 5) / 8 + 1];
+    const int fw = max(f0, v0 - 71);                         // first frame written
+    for (int i = tid; i < (n_frames - fw) * 32; i += kThreads) {
+        const int f = fw + (i >> 5);
+        const int e = s_gmax[clip_group(f) - g0];
         const float gmax = __int_as_float(e >= 0 ? e : e ^ 0x7FFFFFFF);
-        float* q = o + (int64_t)(71 + f) * 32 + (i & 31);
+        float* q = o + (int64_t)(71 + f - v0) * 32 + (i & 31);
         *q = fmaxf(*q, gmax - 80.0f) / 10.0f + 2.0f;
     }
 }
@@ -177,19 +187,20 @@ int oww_mel_launch(oww_ctx* ctx, const MelLaunch& p, cudaStream_t s) {
     return OWW_OK;
 }
 
-int oww_mel_clips_launch(oww_ctx* ctx, const int16_t* d_pcm, int64_t clip_stride, int n_clips, int n_samples, int pad, int steps,
-                         float* d_out, int64_t out_stride, cudaStream_t s) {
+int oww_mel_clips_launch(oww_ctx* ctx, const int16_t* d_pcm, int64_t clip_stride, int n_clips, int n_samples, int pad, int k0,
+                         int k1, float* d_out, int64_t out_stride, cudaStream_t s) {
     if (!ctx->mel_loaded) return oww_fail(ctx, OWW_EINVAL, "mel constants not loaded");
-    if (n_clips <= 0 || steps <= 0) return OWW_OK;
-    if (steps > 8192) return oww_fail(ctx, OWW_EUNSUPPORTED, "clip of %d steps is too long for the one-pass bulk frontend", steps);
+    if (n_clips <= 0 || k1 <= k0) return OWW_OK;
+    if (k0 < 0 || k1 - k0 > 8192) return oww_fail(ctx, OWW_EINVAL, "step range [%d,%d) is not a bulk frontend segment", k0, k1);
     MelDev c{ctx->d_window, ctx->d_twiddle, ctx->d_mel_start, ctx->d_mel_len, ctx->d_mel_w, ctx->mel_kmax};
     const size_t smem = (size_t)kWarps * 2 * 256 * sizeof(float2) + 512 * sizeof(float2) + 512 * sizeof(float) +
-                        (size_t)kWarps * 264 * sizeof(float) + (size_t)kWarps * 512 * sizeof(int16_t) + (size_t)steps * sizeof(int);
+                        (size_t)kWarps * 264 * sizeof(float) + (size_t)kWarps * 512 * sizeof(int16_t) +
+                        (size_t)(k1 - clip_first_group(k0)) * sizeof(int);
     if (!ctx->mel_clip_attr_set) {
         OWW_CUDA(ctx, cudaFuncSetAttribute(mel_clip_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 100 * 1024));
         ctx->mel_clip_attr_set = true;
     }
-    mel_clip_kernel<<<n_clips, kThreads, smem, s>>>(d_pcm, clip_stride, n_samples, pad, steps, d_out, out_stride, c);
+    mel_clip_kernel<<<n_clips, kThreads, smem, s>>>(d_pcm, clip_stride, n_samples, pad, k0, k1, d_out, out_stride, c);
     OWW_LAUNCH_CHECK(ctx);
     return OWW_OK;
 }

@@ -79,7 +79,7 @@ struct VerifierBank {
     float* d_mean = nullptr;         // [capacity][D]
     float* d_weight = nullptr;       // [capacity][D]
     float* d_bias = nullptr;         // [capacity]
-    int* d_assign = nullptr;         // [n_streams] slot per stream, -1 = none (nullptr: every row uses clip_slot)
+    int* d_assign = nullptr;         // [n_streams] slot per stream, -1 = none
     int clip_slot = -1;              // slot oww_predict_clips applies to every clip
 };
 
@@ -179,7 +179,6 @@ struct oww_ctx {
     float* d_tc_sb = nullptr;        // padded scale/bias per layer
     void* d_tc_w3 = nullptr;         // split variant: per layer [hi block | lo block] of W * 2^s (offsets = 2 x tc_w_off)
     float* d_tc_sb3 = nullptr;       // scale * 2^-s | bias
-    int tc_rows_out_override = 0;    // clip pass: embedding rows per input in the caller's array (0 = tightly packed)
     int split_from = 11;             // window / clip passes: conv layers >= split_from take fp16 hi/lo split operands
                                      // (fp32-grade products); OWW_N_CONV = plain fp16 everywhere
     size_t tc_w_off[OWW_N_CONV] = {0};
@@ -247,9 +246,6 @@ struct oww_ctx {
     bool grp_heads = true;           // streaming: heads that share a window run in one CTA per 128 streams (heads_grp.cu; reserved[0] bit 3 disables)
     struct oww_heads_grp* heads_grp = nullptr;
     int tc_heads_terms = 3;          // 3 = hi*hi + lo*hi + hi*lo (fp32-grade), 1 = plain fp16 operands
-
-    // private stream set for oww_predict_clips
-    oww_ctx* clip_ctx = nullptr;
 };
 
 int oww_fail(oww_ctx* ctx, int code, const char* fmt, ...);
@@ -302,10 +298,11 @@ struct MelLaunch {
     const int* ids = nullptr;      // streaming only: clip j is stream ids[j] (body / tail / seen / ring rows of that stream)
 };
 int oww_mel_launch(oww_ctx* ctx, const MelLaunch& p, cudaStream_t s);
-// bulk path: mel rows of whole padded clips, grouped and clamped per streaming call, behind 71 rows of ones:
-// d_out [n_clips][76 + 8 (steps - 1)][32] (the virtual history a fully convolutional CNN pass reproduces predict_clip from)
-int oww_mel_clips_launch(oww_ctx* ctx, const int16_t* d_pcm, int64_t clip_stride, int n_clips, int n_samples, int pad, int steps,
-                         float* d_out, int64_t out_stride, cudaStream_t s);
+// bulk path: mel rows of whole padded clips, grouped and clamped per streaming call, behind 71 rows of ones - the
+// virtual history a fully convolutional CNN pass reproduces predict_clip from.  Steps [k0, k1) (at most 8192) write its
+// rows [8 k0, 76 + 8 (k1 - 1)) to d_out [n_clips][76 + 8 (k1 - k0 - 1)][32].
+int oww_mel_clips_launch(oww_ctx* ctx, const int16_t* d_pcm, int64_t clip_stride, int n_clips, int n_samples, int pad, int k0,
+                         int k1, float* d_out, int64_t out_stride, cudaStream_t s);
 
 // ---- cnn_fp32.cu ----
 // Window-mode embedding CNN on n windows.  Source of window j:
@@ -318,26 +315,27 @@ struct WindowSrc {
     int n_streams; int n_chunks;
     const int* ids = nullptr;           // ring addressing of a stream subset: local stream b is stream ids[b]
 };
-// Fully-convolutional pass over linear mel [n][T][32] -> [n][(T-76)/8+1][96] (SURVEY.md F10).
-int oww_cnn_clip_fp32(oww_ctx* ctx, const float* d_mel, int n, int T, float* d_emb, cudaStream_t s);
 // appends n_chunks embedding rows per stream; ids != nullptr: only the n_ids streams listed (d_emb rows are compact)
 int oww_feat_append(oww_ctx* ctx, const float* d_emb, int n_chunks, cudaStream_t s, const int* d_ids = nullptr, int n_ids = 0);
 // mode dispatch (fp32 window / tensor-core window) with sub-batching over ctx->window_batch
 int oww_cnn_window(oww_ctx* ctx, const WindowSrc& src, int n_windows, float* d_emb, cudaStream_t s, bool capture_tails = false);
+// fp32 pyramid, same contract as oww_cnn_tc_pyramid (cnn_tc.cu)
+int oww_cnn_fp32_pyramid(oww_ctx* ctx, const WindowSrc& src, int n, int T0, float* d_emb, int out_rows, int stop_layer,
+                         float* d_dbg, cudaStream_t s);
 
 // ---- cnn_tc.cu ----
 int oww_tc_pack_weights(oww_ctx* ctx, const float* h_blob);
 size_t oww_tc_act_units(const oww_ctx* ctx, int n_windows);
 size_t oww_tc_act_units_T(const oww_ctx* ctx, int n, int T0);
-// fully-convolutional pass over linear mel [n][T][32] -> [n][(T-76)/8+1][96] on the tensor cores
-int oww_cnn_tc_clip(oww_ctx* ctx, const float* d_mel, int n, int T, float* d_emb, cudaStream_t s);
-int oww_cnn_tc_clip_rows(oww_ctx* ctx, const WindowSrc& src, int n, int T, float* d_emb, int out_rows, cudaStream_t s);
 // incremental late layers of mode 3 (split operands)
 int oww_late_alloc(oww_ctx* ctx);
 int oww_late_chain(oww_ctx* ctx, float* d_emb, cudaStream_t s);
 int oww_late_capture(oww_ctx* ctx, int next_layer, const void* planes, int64_t plane_pitch, int T, int W, cudaStream_t s);
-int oww_cnn_tc_pyramid(oww_ctx* ctx, const WindowSrc& src, int n, float* d_emb, int stop_layer, float* d_dbg, cudaStream_t s);
-// fp32 pyramid with an optional early stop that leaves NHWC fp32 [n][T][W][C] of `stop_layer` in d_dbg
+// Pyramid over n inputs of T0 mel rows each (n windows of 76 rows, or clips: the CNN is fully convolutional in time,
+// SURVEY.md F10): the embeddings of input i land at d_emb + i * out_rows * 96, rows 0 .. (T0 - 76) / 8.  stop_layer >= 0:
+// stop after that layer (and its pool) and leave it as NHWC fp32 [n][T][W][C] in d_dbg.
+int oww_cnn_tc_pyramid(oww_ctx* ctx, const WindowSrc& src, int n, int T0, float* d_emb, int out_rows, int stop_layer,
+                       float* d_dbg, cudaStream_t s);
 // capture descriptor: which local windows of a full-window pass are the newest window of which streams
 struct TailCapture { int win0, n_win, stream0; const int* ids = nullptr; bool late = false; };   // ids: local stream -> stream id;
                                                                   // late: window 0 is the template window of the incremental late layers
@@ -357,7 +355,6 @@ int oww_fused_step(oww_ctx* ctx, const int16_t* d_pcm, int64_t pcm_stride, float
 int oww_heads_sync_devs(oww_ctx* ctx);
 int oww_inc_capture(oww_ctx* ctx, int layer, const void* planes, int64_t plane_pitch, int T, int W, int win0, int n_win,
                     int stream0, const int* d_ids, cudaStream_t s);
-int oww_cnn_fp32_pyramid(oww_ctx* ctx, const WindowSrc& src, int n, float* d_emb, int stop_layer, float* d_dbg, cudaStream_t s);
 
 // ---- heads.cu ----
 struct FeatSrc {
@@ -368,6 +365,24 @@ struct FeatSrc {
     // [row0 + st + 1 - n_in, row0 + st] of clip's linear rows at base + clip * stride (negative rows read as zeros)
     int steps = 0, row0 = 0;
 };
+#ifdef __CUDACC__
+// Where sample s's window of n_in rows starts: feature row c of the window is row r0 + c of `base` (ring: slot
+// (r0 + c) & mask; linear: mask = -1).  Rows below 0 were never written and read as zeros.
+struct FeatRows { const float* base; int r0, mask; };
+__device__ __forceinline__ FeatRows feat_rows(const FeatSrc& src, int n_in, int s) {
+    if (src.count) return FeatRows{src.base + (int64_t)s * src.stride, src.count[s] - src.back - n_in, src.rows_mask};
+    if (src.steps > 0) {
+        const int clip = s / src.steps, st = s - clip * src.steps;
+        return FeatRows{src.base + (int64_t)clip * src.stride, src.row0 + st + 1 - n_in, -1};
+    }
+    return FeatRows{src.base + (int64_t)s * src.stride, 0, -1};
+}
+// feature row c of the window, or nullptr where it reads as zeros
+__device__ __forceinline__ const float* feat_row(const FeatRows& w, int c) {
+    const int r = w.r0 + c;
+    return r < 0 ? nullptr : w.base + (int64_t)(w.mask >= 0 ? (r & w.mask) : r) * 96;
+}
+#endif
 // head_id < 0: every head whose bit is set in head_mask (blockIdx.y walks the selected heads)
 int oww_heads_launch(oww_ctx* ctx, int head_id, const FeatSrc& src, int n, float* d_out, int out_stride,
                      int out_col0, int combine_max, cudaStream_t s, uint32_t head_mask = 0xFFFFFFFFu);
@@ -392,8 +407,7 @@ int oww_heads_all(oww_ctx* ctx, const FeatSrc& src, int n, float* d_out, int out
 // ---- verifier.cu: custom verifier banks ----
 // every bank of the handle on n rows of final scores (one launch; nothing when the handle has no bank).  The window of
 // row r is the newest n_in rows of `src` (FeatSrc sample r).  Its slot is bank.d_assign[r] for streams (rows = streams
-// of the handle), or bank.clip_slot for clips (rows = (clip, step) of the bulk path) and when d_assign is nullptr (the
-// private stream set of oww_predict_clips).
+// of the handle), or bank.clip_slot for clips (rows = (clip, step) of the bulk path).
 int oww_verifiers_apply(oww_ctx* ctx, const FeatSrc& src, int n, float* d_scores, int out_stride, bool clips,
                         cudaStream_t s);
 // (re)allocate every bank's per-stream assignment for ctx->n_streams streams, all -1

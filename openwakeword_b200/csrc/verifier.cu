@@ -50,29 +50,17 @@ __global__ void __launch_bounds__(kVerWarps * 32) verifier_kernel(const __grid_c
     } else {
         mine = lane == 0 ? 1u : 0u;
     }
-    const FeatSrc& S = a.src;
     const int n_in = B.n_in;
-    const float* base;
-    int r0 = 0, mask = -1;
-    if (S.count) {                                          // per-stream ring: rows count-back-n_in .. count-back-1
-        base = S.base + (int64_t)r * S.stride;
-        r0 = S.count[r] - S.back - n_in; mask = S.rows_mask;
-    } else if (S.steps > 0) {                               // bulk clips: the window that ends at the step's row
-        const int clip = r / S.steps, st = r - clip * S.steps;
-        base = S.base + (int64_t)clip * S.stride;
-        r0 = S.row0 + st + 1 - n_in;
-    } else {                                                // linear [n][n_in][96]
-        base = S.base + (int64_t)r * S.stride;
-    }
+    const FeatRows win = feat_rows(a.src, n_in, r);
     const int64_t D = (int64_t)n_in * 96;
     const float4* mu = reinterpret_cast<const float4*>(B.mean + slot * D);
     const float4* w = reinterpret_cast<const float4*>(B.weight + slot * D);
     float acc = 0.f;
     for (int j = lane; j < n_in * 24; j += 32) {
         const int row = j / 24, c4 = j - row * 24;
-        const int rr = r0 + row;
+        const float* p = feat_row(win, row);
         float4 x = make_float4(0.f, 0.f, 0.f, 0.f);         // rows before the stream's first: zeros, as the heads read them
-        if (rr >= 0) x = reinterpret_cast<const float4*>(base + (int64_t)(mask >= 0 ? (rr & mask) : rr) * 96)[c4];
+        if (p) x = reinterpret_cast<const float4*>(p)[c4];
         const float4 m = __ldg(mu + j), v = __ldg(w + j);
         acc = fmaf(x.x - m.x, v.x, acc);
         acc = fmaf(x.y - m.y, v.y, acc);
@@ -111,9 +99,8 @@ int oww_verifiers_apply(oww_ctx* ctx, const FeatSrc& src, int n, float* d_scores
     VerArgs a;
     int nb = 0;
     for (const VerifierBank& b : ctx->banks) {
-        const int* assign = clips ? nullptr : b.d_assign;
-        if (!assign && b.clip_slot < 0) continue;            // clips, and no clip verifier for this head
-        a.bank[nb++] = bank_dev(b, b.clip_slot, assign);
+        if (clips && b.clip_slot < 0) continue;              // no clip verifier for this head
+        a.bank[nb++] = bank_dev(b, b.clip_slot, clips ? nullptr : b.d_assign);
     }
     a.src = src; a.n = n; a.out = d_scores; a.out_stride = out_stride; a.gated = 1;
     return launch(ctx, a, nb, s);

@@ -5,7 +5,8 @@ whose arithmetic they share by construction (and against the oracle where the ar
   every split point cnn_mode 3 accepts;
 * the incremental late chain with and without programmatic dependent launches, at every split point that has one;
 * the sub-batching of the window modes over window_batch;
-* oww_predict_clips on its private stream set (heads that are not on the tensor cores, or cnn_mode 0)."""
+* the bulk clip path with heads that are not on the tensor cores, or cnn_mode 0, and on clips longer than one
+  8192-step segment of its frontend."""
 import numpy as np
 import pytest
 
@@ -69,18 +70,29 @@ def _clip_case():
         for s in range(steps):
             o(padded[c, s * 1280:(s + 1) * 1280])
             ref[c, s] = np.concatenate([oheads.forward(h, o.get_features(h["n_in"]))[0] for h in hs])
-    _CLIPS.update(hs=hs, fi=fi, clips=clips, padded=padded, steps=steps, ref=ref)
+    _CLIPS.update(hs=hs, fi=fi, clips=clips, pad=PAD, padded=padded, steps=steps, ref=ref)
     return _CLIPS
 
 
 def _predict_clips(torch, c, **kw):
     from openwakeword_b200.engine import StreamEngine
     eng = StreamEngine(c["hs"], 1, embedding=emb_weights(), feature_init=c["fi"], **kw)
+    n, length = c["clips"].shape
     d = torch.from_numpy(c["clips"]).cuda()
-    out = torch.full((N_CLIPS, c["steps"], eng.n_cols), -7.0, dtype=torch.float32, device="cuda")
-    eng.ctx.predict_clips(d, N_CLIPS, CLIP_SAMPLES, PAD, c["fi"], out)
+    out = torch.full((n, c["steps"], eng.n_cols), -7.0, dtype=torch.float32, device="cuda")
+    eng.ctx.predict_clips(d, n, length, c["pad"], c["fi"], out)
     torch.cuda.synchronize()
     got = out.cpu().numpy()
+    eng.ctx.close()
+    return got
+
+
+def _stream_clips(c, **kw):
+    """The padded clips streamed one chunk per call through a fresh engine of one stream per clip."""
+    from openwakeword_b200.engine import StreamEngine
+    eng = StreamEngine(c["hs"], len(c["padded"]), embedding=emb_weights(), feature_init=c["fi"], **kw)
+    got = np.stack([eng.step_host(np.ascontiguousarray(c["padded"][:, s * 1280:(s + 1) * 1280]), 1).copy()
+                    for s in range(c["steps"])], 1)
     eng.ctx.close()
     return got
 
@@ -93,14 +105,10 @@ def test_bulk_clips_equal_streaming_at_every_split(torch_cuda, built_library, sp
     another order (2e-6, as the bulk_predict test).  At 20 the streaming step runs the heads inside the fused kernel
     (fp32 FMA chain): 2e-5.  At 3 / 7 the clip pass runs the 48- and 72-channel split convs too, in the window layout
     (tc_conv_kernel<.,.,3>), against the block-major late chain of the streaming step."""
-    from openwakeword_b200.engine import StreamEngine
     torch = torch_cuda
     c = _clip_case()
     bulk = _predict_clips(torch, c, cnn_mode=3, split_from=split_from)
-    eng = StreamEngine(c["hs"], N_CLIPS, embedding=emb_weights(), feature_init=c["fi"], cnn_mode=3, split_from=split_from)
-    stream = np.stack([eng.step_host(np.ascontiguousarray(c["padded"][:, s * 1280:(s + 1) * 1280]), 1).copy()
-                       for s in range(c["steps"])], 1)
-    eng.ctx.close()
+    stream = _stream_clips(c, cnn_mode=3, split_from=split_from)
     d = float(np.abs(bulk - stream).max())
     e_bulk, e_stream = float(np.abs(bulk - c["ref"]).max()), float(np.abs(stream - c["ref"]).max())
     print(f"split_from={split_from}: max |bulk - streaming| = {d:.3e}; max |score - oracle|: bulk {e_bulk:.3e}, "
@@ -113,20 +121,56 @@ def test_bulk_clips_equal_streaming_at_every_split(torch_cuda, built_library, sp
 @pytest.mark.parametrize("kw", [pytest.param(dict(cnn_mode=3, tc_heads=False), id="mode3-cuda-core-heads"),
                                 pytest.param(dict(cnn_mode=3, tc_heads=False, split_from=7), id="mode3-split7-cuda-core-heads"),
                                 pytest.param(dict(cnn_mode=0), id="mode0")])
-def test_predict_clips_private_stream_set(torch_cuda, built_library, kw):
-    """oww_predict_clips falls back to stepping the clips through a private stream set when a head is not on the tensor
-    cores (tc_heads=False) or the CNN runs in fp32 (mode 0).  Against the oracle (1e-3) and against the bulk path of a
-    default handle: CUDA-core vs tensor-core heads, 2e-4 relative (the bound of the grouped-heads test)."""
+def test_predict_clips_bulk_path_without_tensor_core_heads(torch_cuda, built_library, kw):
+    """oww_predict_clips with heads that are not on the tensor cores (tc_heads=False: heads.cu over the sliding windows)
+    or with the fp32 CNN (mode 0: fully convolutional fp32 pass, heads.cu).  Bit for bit against streaming the same padded
+    clips through a fresh engine of the same configuration (the same heads kernel on the same feature rows), against the
+    oracle (1e-3), and against the bulk path of a default handle: CUDA-core vs tensor-core heads, 2e-4 relative (the
+    bound of the grouped-heads test)."""
     torch = torch_cuda
     c = _clip_case()
     got = _predict_clips(torch, c, **kw)
+    stream = _stream_clips(c, **kw)
     bulk = _predict_clips(torch, c)
     e_ref = float(np.abs(got - c["ref"]).max())
     e_bulk = float((np.abs(got - bulk) / np.maximum(1.0, np.abs(bulk))).max())
-    print(f"{kw}: max |score - oracle| = {e_ref:.3e}; max relative |private - bulk| = {e_bulk:.3e}")
+    print(f"{kw}: max |score - oracle| = {e_ref:.3e}; max relative |got - default bulk| = {e_bulk:.3e}; "
+          f"max |got - streaming| = {np.abs(got - stream).max():.3e}")
     assert np.isfinite(got).all()
+    assert np.array_equal(got, stream)
     assert e_ref < 1e-3
     assert e_bulk < 2e-4
+
+
+@pytest.mark.parametrize("mode", [0, 3])
+def test_predict_clips_longer_than_one_frontend_segment(torch_cuda, built_library, mode):
+    """Two clips of 8230 steps (about 11 minutes): the bulk frontend runs them as two segments, [0, 8192) and
+    [8192, 8230).  The second segment's first mel row is frame 65465, 4 frames into the streaming call (clamp group) of
+    frames 65461..65468.  A loud burst covers only the first 4 of those frames and near-silence the rest, so the -80 dB
+    clamp of the written frames depends on frames the second segment computes but does not write.  Against the same
+    clips streamed through a 2-stream engine: bit for bit in mode 0 (heads.cu on both sides), 2e-6 in mode 3 (grouped
+    heads over the clips' feature rows against the fp16 mirror of the rings)."""
+    torch = torch_cuda
+    rng = np.random.default_rng(83)
+    steps = 8230
+    length = 1280 * (steps + 1)
+    burst = (160 * 65461, 160 * 65465)            # samples seen by frames 65461..65464 and none after them
+    quiet = (burst[1], 160 * 65477 + 512)         # the rest of the group and the one after it
+    clips = np.clip(rng.normal(0, 1000, (2, length)), -32768, 32767).astype(np.int16)
+    clips[:, quiet[0]:quiet[1]] = rng.integers(-2, 3, (2, quiet[1] - quiet[0]))
+    clips[:, burst[0]:burst[1]] = np.clip(rng.normal(0, 20000, (2, burst[1] - burst[0])), -32768, 32767)
+    clips[1, burst[0]:burst[1]] //= 4
+    c = dict(hs=[head("alexa_v0.1"), head("timer_v0.1")], fi=rng.normal(0, 1, (41, 96)).astype(np.float32),
+             clips=clips, pad=0, padded=clips, steps=steps)
+    got = _predict_clips(torch, c, cnn_mode=mode)
+    stream = _stream_clips(c, cnn_mode=mode)
+    d = float(np.abs(got - stream).max())
+    print(f"cnn_mode {mode}: {steps} steps, max |bulk - streaming| = {d:.3e}")
+    assert np.isfinite(got).all() and np.isfinite(stream).all()
+    if mode == 0:
+        assert np.array_equal(got, stream)
+    else:
+        assert d <= 2e-6
 
 
 # ---------------------------------------------------------------------------------------------------- late chain

@@ -211,8 +211,9 @@ def test_151_streams_vs_oracle_and_host_path(torch_cuda, built_library, mode, sp
 
 @pytest.mark.parametrize("mode", [0, 3])
 def test_predict_clips_equals_streaming_predict_clip(torch_cuda, built_library, mode):
-    """cnn_mode 3 takes the tensor-core bulk branch of oww_predict_clips, cnn_mode 0 the private-stream-set fallback;
-    both apply stream 0's verifier (the clip slot) and must equal predict_clip after a reset bit for bit."""
+    """The bulk path of oww_predict_clips with the tensor-core CNN and heads (cnn_mode 3) and with the fp32 CNN and
+    heads.cu (cnn_mode 0) applies stream 0's verifier (the clip slot) and must equal predict_clip after a reset bit for
+    bit."""
     c = load_case("verifier_alexa_c1280")
     parent, thr = str(c["parent"]), float(c["threshold"])
     m = _model(c, cnn_mode=mode, custom_verifier_models={parent: os.path.join(GOLDEN, str(c["verifier"]))},
