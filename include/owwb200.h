@@ -14,7 +14,8 @@
  *                        -> AudioFeatures buffers + _streaming_features + the per-head window reads of
  *                           Model.predict                         openwakeword/utils.py:163-178,387-460; model.py:282-302
  *   oww_embed_clips      -> AudioFeatures.embed_clips             openwakeword/utils.py:358-385
- *   oww_predict_clips    -> Model.predict_clip over many clips (bulk_predict's inner loop)
+ *   oww_predict_clips / oww_predict_clips_ragged
+ *                        -> Model.predict_clip over many clips (bulk_predict's inner loop)
  *                                                                 openwakeword/model.py:388-426; utils.py:467-539
  *   oww_get_features / oww_get_mel
  *                        -> AudioFeatures.get_features / .melspectrogram_buffer   openwakeword/utils.py:454-460,165
@@ -199,9 +200,34 @@ int oww_embed_clips(oww_ctx* ctx, const int16_t* d_pcm, int n_clips, int n_sampl
  * (SURVEY.md F9): pad_samples zeros each side, 1280-sample steps, steps = len(range(0, L-1280, 1280)).
  * d_scores [n_clips][steps][oww_n_outputs].  Raw head outputs (the first-5-zeroing of
  * model.py:330-333 is label bookkeeping done by the host wrapper).  Equals streaming the padded clips through
- * fresh streams of this handle's configuration; uses none of the handle's streams.  No heads: returns at once. */
+ * fresh streams of this handle's configuration; uses none of the handle's streams.  No heads: returns at once.
+ * The equal-length, chunk_size 1280 case of oww_predict_clips_ragged (every call steps one chunk).               */
 int oww_predict_clips(oww_ctx* ctx, const int16_t* d_pcm, int n_clips, int n_samples, int pad_samples,
                       const float* h_feature_init, int n_rows, float* d_scores, void* stream);
+/* Call schedule of predict_clip(clip, padding, chunk_size): on n_padded_samples = len + 2*pad samples it makes
+ * len(range(0, L - chunk_size, chunk_size)) predict calls; AudioFeatures._streaming_features steps whole 1280-sample
+ * chunks and keeps the remainder for the next call, so call j steps floor((j+1) c / 1280) - floor(j c / 1280) chunks
+ * (0: the call only accumulated samples).  Writes that count for the first min(calls, max) calls (h_chunks_per_call may
+ * be NULL) and returns the number of calls.  Pure host computation, usable without a GPU; the bulk path uses the same
+ * arithmetic (csrc/oww_internal.h).                                                                                 */
+int oww_clip_schedule(int chunk_size, int64_t n_padded_samples, int32_t* h_chunks_per_call, int max);
+/* predict_clip over clips of any lengths, in one call, each from a FRESH state (as oww_predict_clips).  Clip i is
+ * d_pcm[h_offsets[i] .. h_offsets[i+1]) (host int64 sample offsets, monotone; any lengths, 0 included); pad_samples
+ * zeros each side; chunk_size samples per predict call, 1 .. max_chunks*1280.  Score rows are the clips' calls in input
+ * order (clip i's rows start at the total call count of clips 0..i-1; oww_clip_schedule gives the counts):
+ *   d_scores [rows][oww_n_outputs]: for a call that steps, per head the max over its chunk windows (verifier gates per
+ *            chunk before the max, custom verifiers after it on the call's newest window: what oww_step returns for
+ *            the same call).  Rows of calls that step no chunk are not written.
+ *   d_stepped [rows] (may be NULL): set to 1 on the rows of calls that step; other bytes are not written.
+ *   d_emb (may be NULL) [sum of the clips' steps][96]: the embedding rows each clip's steps appended, clip by clip.
+ * Clips are sorted by length into slabs of neighbours; a shorter clip of a slab runs on over virtual zeros, which leaves
+ * its own calls' rows unchanged (oww_clip_slab_plan reports the steps this computes).  No heads: returns at once.   */
+int oww_predict_clips_ragged(oww_ctx* ctx, const int16_t* d_pcm, const int64_t* h_offsets, int n_clips, int pad_samples,
+                             int chunk_size, const float* h_feature_init, int n_rows, float* d_scores, uint8_t* d_stepped,
+                             float* d_emb, void* stream);
+/* The slabs oww_predict_clips_ragged would run for clips of h_steps[i] chunks each (ctx may be NULL: the default
+ * configuration): returns the slab count, and the steps the slabs compute and the steps the clips need.  Pure host. */
+int oww_clip_slab_plan(oww_ctx* ctx, const int32_t* h_steps, int n_clips, int64_t* h_steps_computed, int64_t* h_steps_needed);
 
 /* ---- score metrics on the device (openwakeword/metrics.py:24-100) --------------------------------
  * d_scores holds n_series score sequences of n_frames float32 each, series i at d_scores + i*series_stride.

@@ -65,6 +65,9 @@ _SIGNATURES = {
     "oww_get_counts": (C.c_int, [_P, C.c_int, C.POINTER(C.c_int), C.POINTER(C.c_int)]),
     "oww_embed_clips": (C.c_int, [_P, _P, C.c_int, C.c_int, _P, _P]),
     "oww_predict_clips": (C.c_int, [_P, _P, C.c_int, C.c_int, C.c_int, _P, C.c_int, _P, _P]),
+    "oww_clip_schedule": (C.c_int, [C.c_int, C.c_int64, _P, C.c_int]),
+    "oww_predict_clips_ragged": (C.c_int, [_P, _P, _P, C.c_int, C.c_int, C.c_int, _P, C.c_int, _P, _P, _P, _P]),
+    "oww_clip_slab_plan": (C.c_int, [_P, _P, C.c_int, C.POINTER(C.c_int64), C.POINTER(C.c_int64)]),
     "oww_debug_layer": (C.c_int, [_P, _P, C.c_int, C.c_int, _P, _P]),
     "oww_debug_inc_plan": (C.c_int, [_P, C.c_int, C.c_int, _P, C.c_int]),
     "oww_debug_inc_cut_plan": (C.c_int, [_P, C.c_int, C.c_int, C.c_int, _P, C.c_int]),
@@ -111,6 +114,30 @@ def load_library():
 
 class NativeError(RuntimeError):
     pass
+
+
+def clip_schedule(chunk_size, n_padded_samples):
+    """Chunks each predict call of predict_clip(chunk_size) steps on n_padded_samples samples -> int32 [calls]
+    (oww_clip_schedule: pure host code, no GPU needed)."""
+    lib = load_library()
+    n = lib.oww_clip_schedule(int(chunk_size), int(n_padded_samples), None, 0)
+    if n < 0:
+        raise NativeError(f"oww_clip_schedule failed ({n}): {lib.oww_last_error(None).decode()}")
+    out = np.zeros(n, np.int32)
+    if n:
+        lib.oww_clip_schedule(int(chunk_size), int(n_padded_samples), _ptr(out), n)
+    return out
+
+
+def clip_slab_plan(steps, ctx=None):
+    """Slabs the ragged bulk path runs for clips of `steps` chunks -> (slabs, steps computed, steps needed); pure host."""
+    lib = load_library()
+    st = np.ascontiguousarray(steps, np.int32)
+    done, need = C.c_int64(0), C.c_int64(0)
+    n = lib.oww_clip_slab_plan(ctx, _ptr(st), st.size, C.byref(done), C.byref(need))
+    if n < 0:
+        raise NativeError(f"oww_clip_slab_plan failed ({n})")
+    return n, done.value, need.value
 
 
 def _ptr(a):
@@ -320,6 +347,16 @@ class Context:
         fi = None if feature_init is None else np.ascontiguousarray(feature_init, np.float32)
         self._check(self.lib.oww_predict_clips(self.h, _ptr(d_pcm), n_clips, n_samples, pad_samples, _ptr(fi),
                                                41 if fi is None else fi.shape[0], _ptr(d_scores), stream))
+
+    def predict_clips_ragged(self, d_pcm, offsets, pad_samples, chunk_size, feature_init, d_scores, d_stepped, d_emb=None,
+                             stream=None):
+        """offsets: host int64 [n_clips + 1] sample offsets into d_pcm; d_scores [rows][n_outputs], d_stepped uint8 [rows],
+        d_emb [steps][96] or None (include/owwb200.h, oww_predict_clips_ragged)."""
+        off = np.ascontiguousarray(offsets, np.int64)
+        fi = None if feature_init is None else np.ascontiguousarray(feature_init, np.float32)
+        self._check(self.lib.oww_predict_clips_ragged(self.h, _ptr(d_pcm), _ptr(off), off.size - 1, int(pad_samples),
+                                                      int(chunk_size), _ptr(fi), 41 if fi is None else fi.shape[0],
+                                                      _ptr(d_scores), _ptr(d_stepped), _ptr(d_emb), stream))
 
     def debug_layer(self, d_windows, n, layer, d_out, stream=None):
         self._check(self.lib.oww_debug_layer(self.h, _ptr(d_windows), n, layer, _ptr(d_out), stream))

@@ -5,6 +5,8 @@
 #include <cstdlib>
 #include <cstring>
 #include <algorithm>
+#include <climits>
+#include <functional>
 
 static thread_local std::string g_create_error;
 
@@ -197,6 +199,66 @@ int ensure_emb_tmp(oww_ctx* ctx, size_t floats) {
     OWW_CUDA(ctx, cudaMalloc(&ctx->d_emb_tmp, floats * sizeof(float)));
     ctx->emb_tmp_floats = floats;
     return OWW_OK;
+}
+
+// Slabs of the bulk clip path over clips sorted by step count, longest first: neighbours in that order, at most the clips
+// whose planes fit the clip pass's scratch at the slab's longest clip (clip_slab), and none more than 1/20 of that
+// clip's steps shorter.  Every clip of a slab runs for the longest one's K steps, so the steps computed exceed the steps
+// needed by at most 5 %.  Clips of equal length at chunk_size 1280 form the slabs oww_predict_clips always had.
+struct ClipSlab { int b, e, K; };
+std::vector<ClipSlab> plan_slabs(const oww_ctx* ctx, const std::vector<int>& steps_desc) {
+    std::vector<ClipSlab> out;
+    const int n = (int)steps_desc.size();
+    for (int b = 0; b < n;) {
+        const int K = steps_desc[b], seg = std::min(K, 8192);
+        const int cap = clip_slab(ctx, n - b, OWW_WINDOW_ROWS + 8 * (seg - 1));
+        int e = b + 1;
+        while (e < n && e - b < cap && 20 * (int64_t)(K - steps_desc[e]) <= K) ++e;
+        out.push_back(ClipSlab{b, e, K});
+        b = e;
+    }
+    return out;
+}
+
+// Score row of a call = per column the max over its chunks' rows (verifier gates were applied per chunk by the heads):
+// dst[out_row[r]] = max(src[q_last[r] - k[r] + 1 .. q_last[r]]), stepped[out_row[r]] = 1.  q_last / k nullptr: one row, r;
+// out_row nullptr: row r (compact).
+__global__ void call_max_kernel(const float* src, int n_out, const int* q_last, const int* k, int n, float* dst,
+                                const int* out_row, uint8_t* stepped) {
+    const int64_t total = (int64_t)n * n_out;
+    for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (int64_t)gridDim.x * blockDim.x) {
+        const int r = (int)(i / n_out), col = (int)(i - (int64_t)r * n_out);
+        const int q = q_last ? q_last[r] : r, kr = k ? k[r] : 1;
+        float v = src[(int64_t)q * n_out + col];
+        for (int j = 1; j < kr; ++j) v = fmaxf(v, src[(int64_t)(q - j) * n_out + col]);
+        const int64_t o = out_row ? out_row[r] : r;
+        dst[o * n_out + col] = v;
+        if (stepped && col == 0) stepped[o] = 1;
+    }
+}
+
+int call_max_launch(oww_ctx* ctx, const float* src, int n_out, const int* q_last, const int* k, int n, float* dst,
+                    const int* out_row, uint8_t* stepped, cudaStream_t s) {
+    if (n <= 0 || n_out <= 0) return OWW_OK;
+    const int64_t total = (int64_t)n * n_out;
+    call_max_kernel<<<(int)std::min<int64_t>(4096, (total + 255) / 256), 256, 0, s>>>(src, n_out, q_last, k, n, dst, out_row, stepped);
+    OWW_LAUNCH_CHECK(ctx);
+    return OWW_OK;
+}
+
+// the embedding rows each clip's own steps appended: feature rows [init_rows, init_rows + steps[p]) of slab clip p ->
+// d_emb rows from emb0[p] on
+__global__ void emb_rows_kernel(const float* feats, int64_t clip_stride, int init_rows, int K, int m, const int* steps,
+                                const int64_t* emb0, float* d_emb) {
+    const int64_t total = (int64_t)m * K * 24;
+    for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (int64_t)gridDim.x * blockDim.x) {
+        const int c4 = (int)(i % 24);
+        const int r = (int)((i / 24) % K);
+        const int p = (int)(i / ((int64_t)24 * K));
+        if (r >= steps[p]) continue;
+        reinterpret_cast<float4*>(d_emb + (emb0[p] + r) * 96)[c4] =
+            reinterpret_cast<const float4*>(feats + p * clip_stride + (int64_t)(init_rows + r) * 96)[c4];
+    }
 }
 
 int step_core(oww_ctx* ctx, const int16_t* d_pcm, int64_t pcm_stride, int n_chunks, float* d_scores, int out_stride,
@@ -716,50 +778,217 @@ int oww_predict_clips(oww_ctx* ctx, const int16_t* d_pcm, int n_clips, int n_sam
                       const float* h_feature_init, int n_rows, float* d_scores, void* stream) {
     if (!ctx || !d_pcm || !d_scores) return oww_fail(ctx, OWW_EINVAL, "null argument");
     if (n_clips < 1 || n_samples < 1 || pad_samples < 0) return oww_fail(ctx, OWW_EINVAL, "bad clip geometry");
+    std::vector<int64_t> off((size_t)n_clips + 1);
+    for (int i = 0; i <= n_clips; ++i) off[i] = (int64_t)i * n_samples;
+    return oww_predict_clips_ragged(ctx, d_pcm, off.data(), n_clips, pad_samples, OWW_SAMPLES_PER_CHUNK, h_feature_init, n_rows,
+                                    d_scores, nullptr, nullptr, stream);
+}
+
+int oww_clip_schedule(int chunk_size, int64_t n_padded_samples, int32_t* h_chunks_per_call, int max) {
+    if (chunk_size < 1 || n_padded_samples < 0) return oww_fail(nullptr, OWW_EINVAL, "bad chunk_size / length");
+    const int64_t n = oww_clip_calls(n_padded_samples, chunk_size);
+    if (n > INT32_MAX) return oww_fail(nullptr, OWW_EINVAL, "too many calls");
+    for (int64_t j = 0; h_chunks_per_call && j < std::min<int64_t>(n, max); ++j)
+        h_chunks_per_call[j] = (int32_t)(oww_call_first_step(j + 1, chunk_size) - oww_call_first_step(j, chunk_size));
+    return (int)n;
+}
+
+int oww_clip_slab_plan(oww_ctx* ctx, const int32_t* h_steps, int n_clips, int64_t* h_steps_computed, int64_t* h_steps_needed) {
+    if (!h_steps || n_clips < 0) return oww_fail(ctx, OWW_EINVAL, "null argument");
+    oww_ctx local;                       // ctx may be NULL: the slab bound depends only on the layer table and split_from
+    if (!ctx) { fill_layer_table(&local); ctx = &local; }
+    std::vector<int> steps;
+    for (int i = 0; i < n_clips; ++i)
+        if (h_steps[i] > 0) steps.push_back(h_steps[i]);
+    std::stable_sort(steps.begin(), steps.end(), std::greater<int>());
+    const std::vector<ClipSlab> plan = plan_slabs(ctx, steps);
+    int64_t computed = 0, needed = 0;
+    for (const ClipSlab& sl : plan) computed += (int64_t)(sl.e - sl.b) * sl.K;
+    for (int k : steps) needed += k;
+    if (h_steps_computed) *h_steps_computed = computed;
+    if (h_steps_needed) *h_steps_needed = needed;
+    return (int)plan.size();
+}
+
+int oww_predict_clips_ragged(oww_ctx* ctx, const int16_t* d_pcm, const int64_t* h_offsets, int n_clips, int pad_samples,
+                             int chunk_size, const float* h_feature_init, int n_rows, float* d_scores, uint8_t* d_stepped,
+                             float* d_emb, void* stream) {
+    if (!ctx || !h_offsets) return oww_fail(ctx, OWW_EINVAL, "null argument");
+    if (n_clips < 0 || pad_samples < 0) return oww_fail(ctx, OWW_EINVAL, "bad clip geometry");
+    if (chunk_size < 1 || chunk_size > ctx->cfg.max_chunks * OWW_SAMPLES_PER_CHUNK)
+        return oww_fail(ctx, OWW_EINVAL, "chunk_size=%d outside [1, max_chunks*1280 = %d]", chunk_size,
+                        ctx->cfg.max_chunks * OWW_SAMPLES_PER_CHUNK);
     if (h_feature_init && n_rows < 0) return oww_fail(ctx, OWW_EINVAL, "n_rows=%d", n_rows);
+    if (h_offsets[0] < 0) return oww_fail(ctx, OWW_EINVAL, "offset 0 is negative");
+    for (int i = 0; i < n_clips; ++i)
+        if (h_offsets[i + 1] < h_offsets[i] || h_offsets[i + 1] - h_offsets[i] > INT32_MAX - 2 * (int64_t)pad_samples)
+            return oww_fail(ctx, OWW_EINVAL, "offsets[%d..%d] = %lld, %lld are not monotone (or the clip is too long)", i, i + 1,
+                            (long long)h_offsets[i], (long long)h_offsets[i + 1]);
+    if (ctx->heads.empty() || n_clips == 0) return OWW_OK;
     OWW_CUDA(ctx, cudaSetDevice(ctx->device));
-    const int64_t L = (int64_t)n_samples + 2 * (int64_t)pad_samples;
-    const int steps = L > OWW_SAMPLES_PER_CHUNK ? (int)((L - OWW_SAMPLES_PER_CHUNK + OWW_SAMPLES_PER_CHUNK - 1) / OWW_SAMPLES_PER_CHUNK) : 0;
-    if (steps == 0 || ctx->heads.empty()) return OWW_OK;
     cudaStream_t s = (cudaStream_t)stream;
-    // Bulk path (SURVEY.md F10), per slab of clips: for each segment of at most 8192 steps ONE mel launch over the padded
-    // clips (frames grouped and clamped per streaming call, behind the 71 rows of ones a fresh stream's window starts
-    // with) and ONE fully convolutional CNN pass over its rows; then the heads and the verifiers over all sliding windows
-    // of [feature_init rows | embeddings].  The same arithmetic as streaming the clips through fresh streams.
-    const int seg_steps = std::min(steps, 8192);
-    const int T_seg = OWW_WINDOW_ROWS + 8 * (seg_steps - 1);
+    const int c = chunk_size, n_out = ctx->n_out_total;
+    // per clip: its calls, the chunks they step, its first score row and first embedding row (input order)
+    std::vector<int> steps(n_clips);
+    std::vector<int64_t> row0(n_clips), emb0(n_clips);
+    int64_t rows = 0, emb_rows = 0;
+    for (int i = 0; i < n_clips; ++i) {
+        const int64_t calls = oww_clip_calls(h_offsets[i + 1] - h_offsets[i] + 2 * (int64_t)pad_samples, c);
+        steps[i] = (int)oww_call_first_step(calls, c);
+        row0[i] = rows; emb0[i] = emb_rows;
+        rows += calls; emb_rows += steps[i];
+    }
+    if (rows > INT32_MAX) return oww_fail(ctx, OWW_EINVAL, "%lld score rows in one call", (long long)rows);
+    // slabs: clips that step, longest first (ties in input order), neighbours in that order (plan_slabs)
+    std::vector<int> order;
+    for (int i = 0; i < n_clips; ++i)
+        if (steps[i] > 0) order.push_back(i);
+    std::stable_sort(order.begin(), order.end(), [&](int x, int y) { return steps[x] > steps[y]; });
+    const int n_act = (int)order.size();
+    if (n_act == 0) return OWW_OK;
+    if (!d_scores || (!d_pcm && h_offsets[n_clips] > h_offsets[0])) return oww_fail(ctx, OWW_EINVAL, "null argument");
+    std::vector<int> st_sorted(n_act);
+    for (int p = 0; p < n_act; ++p) st_sorted[p] = steps[order[p]];
+    const std::vector<ClipSlab> plan = plan_slabs(ctx, st_sorted);
+
+    // One host table, one upload: per sorted clip {sample offset, length, steps, first embedding row}, then per slab the
+    // rows of its stepping calls {last chunk row in the slab's step rows, chunks stepped, score row}.  Equal-step slabs of
+    // consecutive clips at chunk_size 1280 (every call one step) need no call table: the heads write d_scores directly.
+    const bool one_chunk_calls = c == OWW_SAMPLES_PER_CHUNK;
+    std::vector<uint8_t> direct(plan.size(), 0);
+    std::vector<int64_t> call0(plan.size() + 1, 0);
+    size_t max_v = 0, max_f = 0, max_tmp = 0;
+    int max_calls = 0;
     const int init_rows = h_feature_init ? n_rows : OWW_INIT_FEATURE_ROWS;
-    const int64_t f_stride = (int64_t)(init_rows + steps) * 96;
-    const int slab = clip_slab(ctx, n_clips, T_seg);
-    float *d_v = nullptr, *d_f = nullptr, *d_init = nullptr;
-    OWW_CUDA(ctx, cudaMallocAsync(&d_v, (size_t)slab * T_seg * 32 * sizeof(float), s));
-    OWW_CUDA(ctx, cudaMallocAsync(&d_f, (size_t)slab * f_stride * sizeof(float), s));
+    for (size_t k = 0; k < plan.size(); ++k) {
+        const ClipSlab& sl = plan[k];
+        const int m = sl.e - sl.b;
+        bool d = one_chunk_calls;
+        for (int p = sl.b; d && p < sl.e; ++p) d = steps[order[p]] == sl.K && order[p] == order[sl.b] + (p - sl.b);
+        direct[k] = d;
+        int n_calls = 0;
+        if (!d)
+            for (int p = sl.b; p < sl.e; ++p) {
+                const int64_t calls = oww_clip_calls(h_offsets[order[p] + 1] - h_offsets[order[p]] + 2 * (int64_t)pad_samples, c);
+                for (int64_t j = 0; j < calls; ++j) n_calls += oww_call_first_step(j + 1, c) > oww_call_first_step(j, c);
+            }
+        call0[k + 1] = call0[k] + n_calls;
+        max_calls = std::max(max_calls, n_calls);
+        const int seg = std::min(sl.K, 8192);
+        max_v = std::max(max_v, (size_t)m * (OWW_WINDOW_ROWS + 8 * (seg - 1)) * 32);
+        max_f = std::max(max_f, (size_t)m * (init_rows + sl.K) * 96);
+        if (!d) max_tmp = std::max(max_tmp, (size_t)m * sl.K * n_out);
+    }
+    const int64_t n_call_rows = call0.back();
+    const size_t sz_off = (size_t)n_act * 8, sz_emb0 = (size_t)n_act * 8, sz_len = (size_t)n_act * 4, sz_st = (size_t)n_act * 4;
+    const size_t sz_calls = (size_t)n_call_rows * 4;
+    std::vector<uint8_t> tab(sz_off + sz_emb0 + sz_len + sz_st + 3 * sz_calls);
+    int64_t* t_off = reinterpret_cast<int64_t*>(tab.data());
+    int64_t* t_emb0 = t_off + n_act;
+    int* t_len = reinterpret_cast<int*>(t_emb0 + n_act);
+    int* t_st = t_len + n_act;
+    int* t_qlast = t_st + n_act;
+    int* t_k = t_qlast + n_call_rows;
+    int* t_row = t_k + n_call_rows;
+    for (int p = 0; p < n_act; ++p) {
+        const int i = order[p];
+        t_off[p] = h_offsets[i]; t_len[p] = (int)(h_offsets[i + 1] - h_offsets[i]); t_st[p] = steps[i]; t_emb0[p] = emb0[i];
+    }
+    for (size_t k = 0; k < plan.size(); ++k) {
+        if (direct[k]) continue;
+        const ClipSlab& sl = plan[k];
+        int64_t r = call0[k];
+        for (int p = sl.b; p < sl.e; ++p) {
+            const int i = order[p];
+            const int64_t calls = oww_clip_calls(h_offsets[i + 1] - h_offsets[i] + 2 * (int64_t)pad_samples, c);
+            for (int64_t j = 0; j < calls; ++j) {
+                const int64_t f0 = oww_call_first_step(j, c), f1 = oww_call_first_step(j + 1, c);
+                if (f1 == f0) continue;                       // the call only accumulates samples: its row is the host's
+                t_qlast[r] = (p - sl.b) * sl.K + (int)f1 - 1; t_k[r] = (int)(f1 - f0); t_row[r] = (int)(row0[i] + j);
+                ++r;
+            }
+        }
+    }
+    const bool verify_calls = oww_verifiers_clip_active(ctx);
+    uint8_t* d_tab = nullptr;
+    float *d_v = nullptr, *d_f = nullptr, *d_init = nullptr, *d_tmp = nullptr, *d_call = nullptr;
+    OWW_CUDA(ctx, cudaMallocAsync(&d_tab, tab.size(), s));
+    OWW_CUDA(ctx, cudaMemcpyAsync(d_tab, tab.data(), tab.size(), cudaMemcpyHostToDevice, s));   // pageable: staged before return
+    const int64_t* d_off = reinterpret_cast<const int64_t*>(d_tab);
+    const int64_t* d_emb0 = d_off + n_act;
+    const int* d_len = reinterpret_cast<const int*>(d_emb0 + n_act);
+    const int* d_st = d_len + n_act;
+    const int* d_qlast = d_st + n_act;
+    const int* d_k = d_qlast + n_call_rows;
+    const int* d_row = d_k + n_call_rows;
+    OWW_CUDA(ctx, cudaMallocAsync(&d_v, max_v * sizeof(float), s));
+    OWW_CUDA(ctx, cudaMallocAsync(&d_f, max_f * sizeof(float), s));
+    if (max_tmp) OWW_CUDA(ctx, cudaMallocAsync(&d_tmp, max_tmp * sizeof(float), s));
+    if (max_tmp && verify_calls) OWW_CUDA(ctx, cudaMallocAsync(&d_call, (size_t)max_calls * n_out * sizeof(float), s));
     if (h_feature_init && init_rows > 0) {
         OWW_CUDA(ctx, cudaMallocAsync(&d_init, (size_t)init_rows * 96 * sizeof(float), s));
         OWW_CUDA(ctx, cudaMemcpyAsync(d_init, h_feature_init, (size_t)init_rows * 96 * sizeof(float), cudaMemcpyHostToDevice, s));
     }
+    // Bulk path (SURVEY.md F10), per slab of clips: for each segment of at most 8192 steps (ending on a call boundary) ONE
+    // mel launch over the padded clips (frames grouped and clamped per streaming call, behind the 71 rows of ones a fresh
+    // stream's window starts with) and ONE fully convolutional CNN pass over its rows; then the heads over all sliding
+    // windows of [feature_init rows | embeddings], the max over each call's chunk rows and the verifiers on each call's
+    // newest window.  The same arithmetic as streaming the clips through fresh streams.  A clip shorter than its slab's
+    // longest runs on over virtual zeros: a step's rows depend only on samples up to its call's end, so its own calls'
+    // rows do not change, and the rows past them are not read.
     int rc = OWW_OK;
-    for (int c0 = 0; c0 < n_clips && rc == OWW_OK; c0 += slab) {
-        const int m = std::min(slab, n_clips - c0);
-        for (int k0 = 0; k0 < steps && rc == OWW_OK; k0 += seg_steps) {
-            const int k1 = std::min(steps, k0 + seg_steps), T = OWW_WINDOW_ROWS + 8 * (k1 - k0 - 1);
-            if ((rc = oww_mel_clips_launch(ctx, d_pcm + (size_t)c0 * n_samples, n_samples, m, n_samples, pad_samples, k0, k1, d_v,
-                                           (int64_t)T * 32, s))) break;
+    for (size_t k = 0; k < plan.size() && rc == OWW_OK; ++k) {
+        const ClipSlab& sl = plan[k];
+        const int m = sl.e - sl.b, K = sl.K;
+        const int64_t f_stride = (int64_t)(init_rows + K) * 96;
+        for (int k0 = 0; k0 < K && rc == OWW_OK;) {
+            const int k1 = K - k0 <= 8192 ? K : (int)oww_call_first_step(oww_call_of_step(k0 + 8192, c), c);
+            const int T = OWW_WINDOW_ROWS + 8 * (k1 - k0 - 1);
+            if ((rc = oww_mel_clips_launch(ctx, d_pcm, d_off + sl.b, d_len + sl.b, m, pad_samples, c, k0, k1, d_v, (int64_t)T * 32, s)))
+                break;
             if (k0 == 0 && init_rows > 0) {
                 fill_init_rows_kernel<<<std::min(1024, (m * init_rows * 24 + 255) / 256), 256, 0, s>>>(d_f, f_stride, m, d_init, init_rows);
                 ctx->launches++;
             }
             // embeddings of step st land at row init_rows + st of the clip's feature array
-            rc = oww_cnn_clip(ctx, d_v, m, T, d_f + (int64_t)(init_rows + k0) * 96, init_rows + steps, s);
+            rc = oww_cnn_clip(ctx, d_v, m, T, d_f + (int64_t)(init_rows + k0) * 96, init_rows + K, s);
+            k0 = k1;
         }
         if (rc) break;
         FeatSrc fs{d_f, f_stride, nullptr, -1, 0};
-        fs.steps = steps; fs.row0 = init_rows;
-        float* out = d_scores + (size_t)c0 * steps * ctx->n_out_total;
-        if ((rc = oww_heads_all(ctx, fs, m * steps, out, ctx->n_out_total, 0, s))) break;
-        rc = oww_verifiers_apply(ctx, fs, m * steps, out, ctx->n_out_total, true, s);       // clip slot, every step
+        fs.steps = K; fs.row0 = init_rows;
+        if (direct[k]) {
+            const int64_t r0 = row0[order[sl.b]];
+            float* out = d_scores + r0 * n_out;
+            if ((rc = oww_heads_all(ctx, fs, m * K, out, n_out, 0, s))) break;
+            if ((rc = oww_verifiers_apply(ctx, fs, m * K, out, n_out, true, s))) break;       // clip slot, every step
+            if (d_stepped) OWW_CUDA(ctx, cudaMemsetAsync(d_stepped + r0, 1, (size_t)m * K, s));
+        } else {
+            const int nc = (int)(call0[k + 1] - call0[k]);
+            const int* qlast = d_qlast + call0[k];
+            const int* kk = d_k + call0[k];
+            const int* orow = d_row + call0[k];
+            if ((rc = oww_heads_all(ctx, fs, m * K, d_tmp, n_out, 0, s))) break;
+            if (!verify_calls) {
+                if ((rc = call_max_launch(ctx, d_tmp, n_out, qlast, kk, nc, d_scores, orow, d_stepped, s))) break;
+            } else {
+                // verifiers after the max, on the call's newest window: on compact call rows, then scattered to their place
+                if ((rc = call_max_launch(ctx, d_tmp, n_out, qlast, kk, nc, d_call, nullptr, nullptr, s))) break;
+                fs.idx = qlast;
+                if ((rc = oww_verifiers_apply(ctx, fs, nc, d_call, n_out, true, s))) break;
+                if ((rc = call_max_launch(ctx, d_call, n_out, nullptr, nullptr, nc, d_scores, orow, d_stepped, s))) break;
+            }
+        }
+        if (d_emb) {
+            const int total = m * K * 24;
+            emb_rows_kernel<<<std::min(4096, (total + 255) / 256), 256, 0, s>>>(d_f, f_stride, init_rows, K, m, d_st + sl.b, d_emb0 + sl.b,
+                                                                            d_emb);
+            OWW_LAUNCH_CHECK(ctx);
+        }
     }
-    cudaFreeAsync(d_v, s); cudaFreeAsync(d_f, s);
+    cudaFreeAsync(d_v, s); cudaFreeAsync(d_f, s); cudaFreeAsync(d_tab, s);
+    if (d_tmp) cudaFreeAsync(d_tmp, s);
+    if (d_call) cudaFreeAsync(d_call, s);
     if (d_init) cudaFreeAsync(d_init, s);
     return rc;
 }

@@ -101,17 +101,22 @@ __global__ void __launch_bounds__(kThreads) mel_kernel(MelLaunch p, MelDev c) {
 
 // Bulk path (predict_clip over many clips, SURVEY.md F10): one CTA per clip computes the mel rows of the WHOLE padded clip
 // exactly as the streaming calls would have produced them and lays them out as the virtual history the fully
-// convolutional CNN pass needs:  out[clip] = [ones x 71 | frames 0..4 of call 0 | 8 frames of call 1 | ...],
-// 76 + 8 (steps - 1) rows.  The -80 dB clamp is per CALL (F7): frames are grouped [0,5), [5,13), [13,21), ... and each
-// group is clamped against its own maximum.  pad_samples zeros are virtual (nothing is copied).
-// A launch covers the steps [k0, k1): virtual rows [8 k0, 76 + 8 (k1 - 1)), i.e. frames up to 8 k1 - 3 and, at k0 > 0,
-// from 8 k0 - 71 on.  From k0 = 9 on, that first frame lies 4 frames into its group: the kernel computes those 4 frames
-// for the group's maximum and does not write them.
-__host__ __device__ __forceinline__ int clip_group(int f) { return f < 5 ? 0 : (f - 5) / 8 + 1; }   // the call of frame f
-__host__ __device__ __forceinline__ int clip_first_group(int k0) { return clip_group(8 * k0 > 71 ? 8 * k0 - 71 : 0); }
+// convolutional CNN pass needs:  out[clip] = [ones x 71 | frames 0..4 of step 0 | 8 frames of step 1 | ...],
+// 76 + 8 (steps - 1) rows.  The -80 dB clamp is per CALL (F7): a call that steps k chunks clamps its 8 k frames (5 + 8 (k - 1)
+// for the first call of the clip) against their own maximum; with 1280-sample calls the groups are [0,5), [5,13), ...
+// pad_samples zeros are virtual (nothing is copied), as is everything after the clip's own samples.
+// A launch covers the steps [k0, k1), k1 on a call boundary: virtual rows [8 k0, 76 + 8 (k1 - 1)), i.e. frames up to
+// 8 k1 - 3 and, at k0 > 0, from 8 k0 - 71 on.  When that first frame lies inside its call's group, the kernel computes the
+// group's earlier frames for its maximum and does not write them.
+__host__ __device__ __forceinline__ int clip_frame_step(int f) { return f < 5 ? 0 : (f - 5) / 8 + 1; }   // the step of frame f
+// the group of frame f: the first step of the call that steps it
+__host__ __device__ __forceinline__ int clip_group(int f, int chunk) {
+    return (int)oww_call_first_step(oww_call_of_step(clip_frame_step(f), chunk), chunk);
+}
+__host__ __device__ __forceinline__ int clip_first_group(int k0, int chunk) { return clip_group(8 * k0 > 71 ? 8 * k0 - 71 : 0, chunk); }
 
-__global__ void __launch_bounds__(kThreads) mel_clip_kernel(const int16_t* pcm, int64_t clip_stride, int n_samples, int pad, int k0,
-                                                            int k1, float* out, int64_t out_stride, MelDev c) {
+__global__ void __launch_bounds__(kThreads) mel_clip_kernel(const int16_t* pcm, const int64_t* clip_off, const int* clip_len, int pad,
+                                                            int chunk, int k0, int k1, float* out, int64_t out_stride, MelDev c) {
     extern __shared__ __align__(16) uint8_t dyn[];
     float2 (*s_buf)[2][256] = reinterpret_cast<float2 (*)[2][256]>(dyn);               // [kWarps][2][256]
     float2* s_tw = reinterpret_cast<float2*>(dyn + kWarps * 2 * 256 * sizeof(float2));
@@ -122,12 +127,13 @@ __global__ void __launch_bounds__(kThreads) mel_clip_kernel(const int16_t* pcm, 
     const int clip = blockIdx.x;
     const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
     const int v0 = 8 * k0;                                   // first virtual row written (output row 0)
-    const int g0 = clip_first_group(k0);
+    const int g0 = clip_first_group(k0, chunk);
     const int f0 = g0 == 0 ? 0 : 8 * g0 - 3;                 // first frame of group g0
     const int n_frames = 8 * k1 - 3;
     for (int i = tid; i < 512; i += kThreads) { s_tw[i] = c.twiddle[i]; s_win[i] = c.window[i]; }
     for (int i = tid; i < k1 - g0; i += kThreads) s_gmax[i] = INT_MIN;
-    const int16_t* body = pcm + (int64_t)clip * clip_stride;
+    const int16_t* body = pcm + clip_off[clip];
+    const int n_samples = clip_len[clip];
     float* o = out + (int64_t)clip * out_stride;
     for (int i = tid; i < (71 - v0) * 32; i += kThreads) o[i] = 1.0f;
     __syncthreads();
@@ -148,14 +154,14 @@ __global__ void __launch_bounds__(kThreads) mel_clip_kernel(const int16_t* pcm, 
         float m = db;
 #pragma unroll
         for (int k = 16; k > 0; k >>= 1) m = fmaxf(m, __shfl_xor_sync(0xffffffffu, m, k));
-        if (lane == 0) atomicMax(&s_gmax[clip_group(f) - g0], enc(m));
+        if (lane == 0) atomicMax(&s_gmax[clip_group(f, chunk) - g0], enc(m));
         __syncwarp();
     }
     __syncthreads();
     const int fw = max(f0, v0 - 71);                         // first frame written
     for (int i = tid; i < (n_frames - fw) * 32; i += kThreads) {
         const int f = fw + (i >> 5);
-        const int e = s_gmax[clip_group(f) - g0];
+        const int e = s_gmax[clip_group(f, chunk) - g0];
         const float gmax = __int_as_float(e >= 0 ? e : e ^ 0x7FFFFFFF);
         float* q = o + (int64_t)(71 + f - v0) * 32 + (i & 31);
         *q = fmaxf(*q, gmax - 80.0f) / 10.0f + 2.0f;
@@ -187,20 +193,21 @@ int oww_mel_launch(oww_ctx* ctx, const MelLaunch& p, cudaStream_t s) {
     return OWW_OK;
 }
 
-int oww_mel_clips_launch(oww_ctx* ctx, const int16_t* d_pcm, int64_t clip_stride, int n_clips, int n_samples, int pad, int k0,
-                         int k1, float* d_out, int64_t out_stride, cudaStream_t s) {
+int oww_mel_clips_launch(oww_ctx* ctx, const int16_t* d_pcm, const int64_t* d_off, const int* d_len, int n_clips, int pad,
+                         int chunk, int k0, int k1, float* d_out, int64_t out_stride, cudaStream_t s) {
     if (!ctx->mel_loaded) return oww_fail(ctx, OWW_EINVAL, "mel constants not loaded");
     if (n_clips <= 0 || k1 <= k0) return OWW_OK;
-    if (k0 < 0 || k1 - k0 > 8192) return oww_fail(ctx, OWW_EINVAL, "step range [%d,%d) is not a bulk frontend segment", k0, k1);
+    if (k0 < 0 || k1 - k0 > 8192 || chunk < 1 || oww_call_first_step(oww_call_of_step(k1, chunk), chunk) != k1)
+        return oww_fail(ctx, OWW_EINVAL, "step range [%d,%d) is not a bulk frontend segment", k0, k1);
     MelDev c{ctx->d_window, ctx->d_twiddle, ctx->d_mel_start, ctx->d_mel_len, ctx->d_mel_w, ctx->mel_kmax};
     const size_t smem = (size_t)kWarps * 2 * 256 * sizeof(float2) + 512 * sizeof(float2) + 512 * sizeof(float) +
                         (size_t)kWarps * 264 * sizeof(float) + (size_t)kWarps * 512 * sizeof(int16_t) +
-                        (size_t)(k1 - clip_first_group(k0)) * sizeof(int);
+                        (size_t)(k1 - clip_first_group(k0, chunk)) * sizeof(int);
     if (!ctx->mel_clip_attr_set) {
         OWW_CUDA(ctx, cudaFuncSetAttribute(mel_clip_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 100 * 1024));
         ctx->mel_clip_attr_set = true;
     }
-    mel_clip_kernel<<<n_clips, kThreads, smem, s>>>(d_pcm, clip_stride, n_samples, pad, k0, k1, d_out, out_stride, c);
+    mel_clip_kernel<<<n_clips, kThreads, smem, s>>>(d_pcm, d_off, d_len, pad, chunk, k0, k1, d_out, out_stride, c);
     OWW_LAUNCH_CHECK(ctx);
     return OWW_OK;
 }

@@ -284,6 +284,20 @@ __device__ __forceinline__ void oww_pdl_sync() {        // trigger the successor
                             cudaGetErrorString(e__), __FILE__, __LINE__);                      \
     } while (0)
 
+// ---- call schedule of the bulk clip path ----
+// predict_clip(clip, chunk_size = c) makes len(range(0, L - c, c)) calls of c samples on the L padded samples, and
+// AudioFeatures._streaming_features steps whole 1280-sample chunks only, keeping the remainder for the next call: after
+// calls 0 .. j - 1, floor(j c / 1280) chunks have been stepped.  oww_clip_schedule (api.cu) exports these for the host.
+#ifdef __CUDACC__
+#define OWW_HD __host__ __device__ __forceinline__
+#else
+#define OWW_HD inline
+#endif
+OWW_HD int64_t oww_clip_calls(int64_t L, int c) { return L > c ? (L - 1) / c : 0; }
+OWW_HD int64_t oww_call_first_step(int64_t j, int c) { return j * c / OWW_SAMPLES_PER_CHUNK; }
+// the call that steps chunk s: the first j with (j + 1) c >= 1280 (s + 1)
+OWW_HD int64_t oww_call_of_step(int64_t s, int c) { return ((int64_t)OWW_SAMPLES_PER_CHUNK * (s + 1) + c - 1) / c - 1; }
+
 // ---- mel.cu ----
 // Log-mel of n_clips virtual clips.  Clip c = [prefix (prefix_len samples, may be 0) | body (n_body samples)].
 // Streaming: prefix = d_tail row, out rows go to the mel ring at the stream's count; fresh streams
@@ -298,11 +312,12 @@ struct MelLaunch {
     const int* ids = nullptr;      // streaming only: clip j is stream ids[j] (body / tail / seen / ring rows of that stream)
 };
 int oww_mel_launch(oww_ctx* ctx, const MelLaunch& p, cudaStream_t s);
-// bulk path: mel rows of whole padded clips, grouped and clamped per streaming call, behind 71 rows of ones - the
-// virtual history a fully convolutional CNN pass reproduces predict_clip from.  Steps [k0, k1) (at most 8192) write its
-// rows [8 k0, 76 + 8 (k1 - 1)) to d_out [n_clips][76 + 8 (k1 - k0 - 1)][32].
-int oww_mel_clips_launch(oww_ctx* ctx, const int16_t* d_pcm, int64_t clip_stride, int n_clips, int n_samples, int pad, int k0,
-                         int k1, float* d_out, int64_t out_stride, cudaStream_t s);
+// bulk path: mel rows of whole padded clips, grouped and clamped per streaming call of `chunk` samples, behind 71 rows of
+// ones - the virtual history a fully convolutional CNN pass reproduces predict_clip from.  Clip i is the d_len[i] samples
+// at d_pcm + d_off[i], with `pad` virtual zeros on each side and virtual zeros after that.  Steps [k0, k1) (at most 8192;
+// k1 on a call boundary) write its rows [8 k0, 76 + 8 (k1 - 1)) to d_out [n_clips][76 + 8 (k1 - k0 - 1)][32].
+int oww_mel_clips_launch(oww_ctx* ctx, const int16_t* d_pcm, const int64_t* d_off, const int* d_len, int n_clips, int pad,
+                         int chunk, int k0, int k1, float* d_out, int64_t out_stride, cudaStream_t s);
 
 // ---- cnn_fp32.cu ----
 // Window-mode embedding CNN on n windows.  Source of window j:
@@ -364,6 +379,7 @@ struct FeatSrc {
     // sliding mode (count == nullptr, steps > 0; bulk clips): sample s = clip * steps + st reads rows
     // [row0 + st + 1 - n_in, row0 + st] of clip's linear rows at base + clip * stride (negative rows read as zeros)
     int steps = 0, row0 = 0;
+    const int* idx = nullptr;            // sliding mode: sample s reads the window of sliding sample idx[s] (call rows)
 };
 #ifdef __CUDACC__
 // Where sample s's window of n_in rows starts: feature row c of the window is row r0 + c of `base` (ring: slot
@@ -372,7 +388,8 @@ struct FeatRows { const float* base; int r0, mask; };
 __device__ __forceinline__ FeatRows feat_rows(const FeatSrc& src, int n_in, int s) {
     if (src.count) return FeatRows{src.base + (int64_t)s * src.stride, src.count[s] - src.back - n_in, src.rows_mask};
     if (src.steps > 0) {
-        const int clip = s / src.steps, st = s - clip * src.steps;
+        const int q = src.idx ? src.idx[s] : s;
+        const int clip = q / src.steps, st = q - clip * src.steps;
         return FeatRows{src.base + (int64_t)clip * src.stride, src.row0 + st + 1 - n_in, -1};
     }
     return FeatRows{src.base + (int64_t)s * src.stride, 0, -1};
@@ -412,4 +429,6 @@ int oww_verifiers_apply(oww_ctx* ctx, const FeatSrc& src, int n, float* d_scores
                         cudaStream_t s);
 // (re)allocate every bank's per-stream assignment for ctx->n_streams streams, all -1
 int oww_verifiers_alloc_streams(oww_ctx* ctx);
+// true when oww_verifiers_apply(..., clips = true) would launch (a bank with a clip slot, verifiers enabled)
+bool oww_verifiers_clip_active(const oww_ctx* ctx);
 void oww_verifiers_free_streams(oww_ctx* ctx);

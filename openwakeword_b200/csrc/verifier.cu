@@ -106,6 +106,13 @@ int oww_verifiers_apply(oww_ctx* ctx, const FeatSrc& src, int n, float* d_scores
     return launch(ctx, a, nb, s);
 }
 
+bool oww_verifiers_clip_active(const oww_ctx* ctx) {
+    if (!ctx->verifiers_on) return false;
+    for (const VerifierBank& b : ctx->banks)
+        if (b.clip_slot >= 0) return true;
+    return false;
+}
+
 int oww_verifiers_alloc_streams(oww_ctx* ctx) {
     oww_verifiers_free_streams(ctx);
     if (ctx->banks.empty() || ctx->n_streams <= 0) return OWW_OK;

@@ -5,7 +5,7 @@ Same constructor keywords, ``predict`` / ``predict_clip`` / ``reset`` semantics,
 ``preprocessor``) and ``ValueError`` behaviour; the three inference sessions and the buffers between
 them are replaced by one libowwb200 step per call.  Additions: ``n_streams`` independent streams on
 the batch axis (``predict`` then takes ``[n_streams, samples]`` and returns arrays per label),
-``predict_clips`` (array-input bulk path) and ``feature_init``.
+``predict_clips`` / ``predict_clips_ragged`` (bulk path over clips of any lengths) and ``feature_init``.
 """
 import os
 import time
@@ -431,13 +431,138 @@ class Model:
                         hits[lbl].append(context)
         return {lbl: np.vstack(v) for lbl, v in hits.items() if v}
 
-    def predict_clips(self, clips, padding=1, feature_init=None):
-        """Array-input bulk path (extension; SURVEY.md F9): int16 [N,S] equal-length clips, each from a
-        fresh state, 1280-sample steps.  Returns a list (per clip) of lists (per step) of {label: float},
-        i.e. what predict_clip would return for each clip after reset(feature_init)."""
-        scores, labels = self.predict_clips_array(clips, padding, feature_init)
-        return [[{lab: float(scores[c, s, j]) for j, lab in enumerate(labels)} for s in range(scores.shape[1])]
-                for c in range(scores.shape[0])]
+    def predict_clips(self, clips, padding=1, feature_init=None, chunk_size=1280):
+        """Bulk path (extension; SURVEY.md F9): each clip from a fresh state, in one device call.  ``clips``: an int16
+        [N,S] array or tensor, or a sequence of 1-D int16 arrays of any lengths.  Returns a list (per clip) of lists (per
+        call) of {label: float}, i.e. what predict_clip(clip, padding, chunk_size) would return for each clip after
+        reset(feature_init)."""
+        torch = _torch()
+        if chunk_size == CHUNK and (isinstance(clips, torch.Tensor) or (isinstance(clips, np.ndarray) and clips.ndim == 2)):
+            scores, labels = self.predict_clips_array(clips, padding, feature_init)
+            return [[{lab: float(scores[c, s, j]) for j, lab in enumerate(labels)} for s in range(scores.shape[1])]
+                    for c in range(scores.shape[0])]
+        pcm, offsets = _concat_clips(clips)
+        scores, row_off, labels = self.predict_clips_ragged(pcm, offsets, padding, chunk_size, feature_init)
+        return _rows_to_dicts(scores, row_off, labels)
+
+    def predict_clips_ragged(self, pcm, offsets, padding=1, chunk_size=1280, feature_init=None):
+        """Array form of the bulk path over clips of any lengths: clip i is ``pcm[offsets[i]:offsets[i+1]]`` (int16 1-D
+        array or tensor, int64 offsets).  Returns (float32 [rows, n_labels], int64 row_offsets [N+1], labels): clip i's
+        rows ``row_offsets[i]:row_offsets[i+1]`` are the predictions predict_clip(clip, padding, chunk_size) returns after
+        reset(feature_init), one per call."""
+        return self._predict_ragged(pcm, offsets, padding, chunk_size, feature_init)[:3]
+
+    def _predict_ragged(self, pcm, offsets, padding, chunk_size, feature_init, want_features=False):
+        """-> (scores, row_offsets, labels, embeddings [steps, 96] or None, step_offsets [N+1], feature_init rows).
+        One oww_predict_clips_ragged call; the host fills the rows of calls that stepped no chunk as Model.predict does
+        (the previous prediction of single-output heads, zeros for multi-class heads, re-verified), then zeroes each
+        clip's first 5 calls (model.py:330-333).  Vectorised over rows."""
+        if self._host_verifiers:
+            warnings.warn(f"custom verifiers of {sorted(self._host_verifiers)} are not device-runnable (only the linear "
+                          "pipeline of train_verifier_model is): predict_clips returns their models' unverified scores",
+                          stacklevel=3)
+        torch = _torch()
+        chunk_size = int(chunk_size)
+        limit = self.preprocessor.max_chunks * CHUNK
+        if not 1 <= chunk_size <= limit:
+            raise ValueError(f"chunk_size={chunk_size}: the bulk path takes 1 .. max_chunks*1280 = {limit} samples per call "
+                             f"(max_chunks={self.preprocessor.max_chunks}); construct the Model with a larger max_chunks")
+        offsets = np.ascontiguousarray(offsets, np.int64)
+        n = offsets.size - 1
+        pad = 16000 * int(padding)
+        lengths = np.diff(offsets)
+        calls = np.array([_native.clip_schedule(chunk_size, int(x) + 2 * pad).size for x in lengths], np.int64)
+        row_off = np.concatenate([[0], np.cumsum(calls)]).astype(np.int64)
+        steps = calls * chunk_size // CHUNK                          # chunks stepped by a clip's calls (oww_clip_schedule)
+        step_off = np.concatenate([[0], np.cumsum(steps)]).astype(np.int64)
+        rows = int(row_off[-1])
+        fi = feature_init if feature_init is not None else self.preprocessor._feature_init
+        if fi is None:
+            fi = self.preprocessor._get_embeddings(np.random.randint(-1000, 1000, 16000 * 4).astype(np.int16))
+        fi = np.ascontiguousarray(fi, np.float32)
+        cols, labels, single = [], [], []
+        for mdl in self.models:
+            col0, n_out = self._columns[mdl]
+            if n_out == 1:
+                cols.append(col0); labels.append(mdl); single.append(True)
+            else:
+                for k, lab in self.class_mapping[mdl].items():
+                    cols.append(col0 + int(k)); labels.append(lab); single.append(False)
+        dev = f"cuda:{self.preprocessor.device_index}"
+        if isinstance(pcm, torch.Tensor):
+            d = pcm.to(device=dev, dtype=torch.int16, non_blocking=True).contiguous()
+        else:
+            d = torch.from_numpy(np.ascontiguousarray(pcm, np.int16)).to(dev)
+        raw = torch.zeros((rows, max(self._n_cols, 1)), dtype=torch.float32, device=dev)
+        stepped = torch.zeros(rows, dtype=torch.uint8, device=dev)
+        need_emb = want_features or (chunk_size < CHUNK and bool(self._vbanks))
+        emb = torch.zeros((int(step_off[-1]), 96), dtype=torch.float32, device=dev) if need_emb else None
+        self.preprocessor.ctx.predict_clips_ragged(d, offsets, pad, chunk_size, fi, raw, stepped, emb,
+                                                   torch.cuda.current_stream(d.device).cuda_stream)
+        out = raw.cpu().numpy()[:, cols]
+        stepped = stepped.cpu().numpy().astype(bool)
+        emb = emb.cpu().numpy() if emb is not None else None
+        if rows:
+            clip = np.repeat(np.arange(n), calls)
+            idx = np.arange(rows)
+            local = idx - row_off[clip]
+            first5 = local < 5
+            out[first5] = 0.0
+            # a row is its own source when it stepped or is zeroed; other rows repeat the final value of the source row
+            # before them (re-verification on an unchanged window is idempotent, so repeating a repeat is the same)
+            src = np.maximum.accumulate(np.where(stepped | first5, idx, -1))
+            rep = ~(stepped | first5)
+            single = np.asarray(single)
+            out[rep] = np.where(single[None, :], out[src[rep]], np.float32(0.0))
+            if rep.any():
+                self._reverify_rows(out, rep, local, clip, step_off, chunk_size, emb, fi, labels)
+        return out, row_off, labels, emb, step_off, fi
+
+    def _reverify_rows(self, out, rep, local, clip, step_off, chunk_size, emb, fi, labels):
+        """_reverify on the rows of calls that stepped no chunk: labels of a device-verified model >= the threshold take
+        the verifier's p on the clip's newest window ([feature_init rows | the clip's embeddings] up to the last step)."""
+        thr = np.float32(self.custom_verifier_threshold)
+        for mdl, st in self._vbanks.items():
+            slot = int(st["slots"][0])
+            if slot < 0:
+                continue
+            js = [j for j, lab in enumerate(labels) if self.get_parent_model_from_label(lab) == mdl]
+            hit_rows = np.nonzero(rep & (out[:, js] >= thr).any(axis=1))[0]
+            if hit_rows.size == 0:
+                continue
+            n_in = self.model_inputs[mdl]
+            done = (local[hit_rows] + 1) * chunk_size // CHUNK       # chunks stepped up to and including the call
+            feats = np.stack([_window(fi, emb, step_off[clip[r]], int(k), n_in) for r, k in zip(hit_rows, done)])
+            p = self.preprocessor.ctx.verifier_predict_host(st["bank"], slot, feats)
+            for j in js:
+                sel = out[hit_rows, j] >= thr
+                out[hit_rows[sel], j] = p[sel]
+
+    def _positive_frames_bulk(self, pcms, threshold=0.5, return_type="features"):
+        """_get_positive_prediction_frames over many clips in one device call (padding 0, 1280-sample calls): per clip
+        {label: stacked array} of what produced a score >= threshold."""
+        if return_type not in ("features", "audio"):
+            raise ValueError("return_type must be 'features' or 'audio'")
+        pcm, offsets = _concat_clips(pcms)
+        scores, row_off, labels, emb, step_off, fi = self._predict_ragged(pcm, offsets, 0, CHUNK, None,
+                                                                          want_features=return_type == "features")
+        n_in = {lab: self.model_inputs[self.get_parent_model_from_label(lab)] for lab in labels}
+        res = []
+        for c, data in enumerate(pcms):
+            hits = {}
+            for s in range(int(row_off[c + 1] - row_off[c])):
+                for j, lab in enumerate(labels):
+                    if scores[row_off[c] + s, j] < threshold:
+                        continue
+                    if return_type == "features":
+                        hits.setdefault(lab, []).append(_window(fi, emb, step_off[c], s + 1, n_in[lab])[None])
+                    else:
+                        i = s * CHUNK
+                        context = data[max(0, i - 16000 * 3):i + 16000]
+                        if len(context) == 16000 * 4:
+                            hits.setdefault(lab, []).append(context)
+            res.append({lab: np.vstack(v) for lab, v in hits.items() if v})
+        return res
 
     def labels(self):
         """Output labels in score-column order (binary heads: model name; multi-class: mapped labels)."""
@@ -487,3 +612,34 @@ class Model:
         out = raw[:, :, cols]
         out[:, :5, :] = 0.0
         return out, labels
+
+
+def _concat_clips(clips):
+    """[N,S] array / tensor or a sequence of 1-D int16 arrays -> (one int16 array or tensor, int64 offsets [N+1])"""
+    torch = _torch()
+    if isinstance(clips, torch.Tensor) and clips.dim() == 2:
+        n, s = clips.shape
+        return clips.reshape(-1), np.arange(n + 1, dtype=np.int64) * s
+    if isinstance(clips, np.ndarray) and clips.ndim == 2:
+        n, s = clips.shape
+        return np.ascontiguousarray(clips, np.int16).reshape(-1), np.arange(n + 1, dtype=np.int64) * s
+    parts = [np.asarray(c).astype(np.int16, copy=False).ravel() for c in clips]
+    offsets = np.concatenate([[0], np.cumsum([p.size for p in parts])]).astype(np.int64)
+    pcm = np.concatenate(parts) if parts else np.zeros(0, np.int16)
+    return pcm, offsets
+
+
+def _rows_to_dicts(scores, row_off, labels):
+    return [[{lab: float(v) for lab, v in zip(labels, row)} for row in scores[row_off[c]:row_off[c + 1]]]
+            for c in range(row_off.size - 1)]
+
+
+def _window(fi, emb, step0, done, n_in):
+    """the newest n_in feature rows of a clip after `done` of its steps: rows of [feature_init | its embeddings] ending
+    at row len(fi) + done, rows before the first read as zeros (AudioFeatures.get_features) -> [n_in, 96]"""
+    rows = np.concatenate([fi, emb[step0:step0 + done]]) if done else fi
+    w = np.zeros((n_in, 96), np.float32)
+    k = min(n_in, rows.shape[0])
+    if k:
+        w[n_in - k:] = rows[rows.shape[0] - k:]
+    return w

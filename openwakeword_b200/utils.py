@@ -3,8 +3,8 @@
 ``AudioFeatures`` keeps the reference's constructor / call / attribute surface
 (openwakeword/utils.py:33-463) but owns a libowwb200 ``Context``: the PCM tail,
 mel ring and embedding ring live in HBM and one ``__call__`` is one C-ABI step for every stream.
-``bulk_predict`` keeps the reference signature (utils.py:467-539) and runs clips through
-``oww_predict_clips`` with fresh state per clip.  Host code here only moves arguments, shapes and
+``bulk_predict`` keeps the reference signature (utils.py:467-539) and runs clips of any lengths through
+``oww_predict_clips_ragged`` with fresh state per clip.  Host code here only moves arguments, shapes and
 errors; all arithmetic is in the CUDA library.
 """
 import functools
@@ -353,34 +353,61 @@ def compute_features_from_generator(generator, n_total, clip_duration, output_fi
         os.replace(tmp, output_file)
 
 
+# pinned host staging per device call of bulk_predict: the files of one batch, int16 (a corpus larger than host memory
+# streams through in batches of about this size)
+BULK_STAGING_BYTES = 256 << 20
+
+
+def _wav_batches(paths, budget):
+    """consecutive groups of paths whose files total at most `budget` bytes (a larger file forms a group of its own)"""
+    batch, size = [], 0
+    for p in paths:
+        b = os.path.getsize(p)
+        if batch and size + b > budget:
+            yield batch
+            batch, size = [], 0
+        batch.append(p)
+        size += b
+    if batch:
+        yield batch
+
+
 def bulk_predict(file_paths, wakeword_models, prediction_function="predict_clip", ncpu=1,
                  inference_framework="b200", **kwargs):
     """Reference signature (utils.py:467-539).  Clips are batched on the GPU instead of forked across ``ncpu``
     processes; ``ncpu`` is the number of host threads that read the WAV files.  Each clip starts from a fresh state (the
-    reference bleeds state across the clips of one worker, SURVEY.md F9).  Returns {path: list of dicts}."""
-    from .model import Model
-    if prediction_function != "predict_clip":
-        raise ValueError("the b200 bulk path implements prediction_function='predict_clip'")
+    reference bleeds state across the clips of one worker, SURVEY.md F9).  Files of any lengths go through one device call
+    per batch of about BULK_STAGING_BYTES of audio (Model.predict_clips_ragged).  As in the reference, keyword arguments
+    go to the Model constructor and to the prediction function where they name one of its parameters, and are dropped
+    otherwise.  ``prediction_function``: "predict_clip" (``padding``, ``chunk_size``) or
+    "_get_positive_prediction_frames" (``threshold``, ``return_type``).  Returns {path: result of the function}."""
+    from .model import Model, _rows_to_dicts
+    if prediction_function not in ("predict_clip", "_get_positive_prediction_frames"):
+        raise ValueError("the b200 bulk path implements prediction_function='predict_clip' and "
+                         "'_get_positive_prediction_frames'")
     import inspect
     init_names = set(inspect.signature(Model.__init__).parameters) | set(inspect.signature(AudioFeatures.__init__).parameters)
     init_kw = {k: v for k, v in kwargs.items() if k in init_names}
-    clip_kw = {k: v for k, v in kwargs.items() if k not in init_names}
+    fn_names = set(inspect.signature(getattr(Model, prediction_function)).parameters) - {"self", "kwargs"}
+    fn_kw = {k: v for k, v in kwargs.items() if k in fn_names}
     mdl = Model(wakeword_models=wakeword_models, inference_framework=inference_framework, **init_kw)
-    clips = _read_wavs(file_paths, ncpu)                       # RIFF parsing on ncpu host threads, order kept
-    out = {}
-    by_len = {}
-    for p, c in zip(file_paths, clips):
-        by_len.setdefault(c.shape[0], []).append(p)
-    lookup = dict(zip(file_paths, clips))
     torch = _torch()
-    for length, paths in by_len.items():
-        # equal-length clips form one device batch; they are gathered in page-locked memory so the H2D copy is a single
-        # asynchronous DMA (the reference forks one process per ncpu instead, utils.py:505-536)
-        stage = torch.empty((len(paths), length), dtype=torch.int16, pin_memory=True)
+    out = {}
+    for paths in _wav_batches(list(file_paths), BULK_STAGING_BYTES):
+        clips = _read_wavs(paths, ncpu)                        # RIFF parsing on ncpu host threads, order kept
+        if prediction_function == "_get_positive_prediction_frames":
+            res = mdl._positive_frames_bulk(clips, threshold=fn_kw.get("threshold", 0.5),
+                                            return_type=fn_kw.get("return_type", "features"))
+            out.update(zip(paths, res))
+            continue
+        # the batch is gathered in page-locked memory so the H2D copy is a single asynchronous DMA (the reference forks
+        # one process per ncpu instead, utils.py:505-536)
+        offsets = np.concatenate([[0], np.cumsum([c.shape[0] for c in clips])]).astype(np.int64)
+        stage = torch.empty(int(offsets[-1]), dtype=torch.int16, pin_memory=True)
         view = stage.numpy()
-        for i, p in enumerate(paths):
-            view[i] = lookup[p]
-        res = mdl.predict_clips(stage, **clip_kw)
-        for p, r in zip(paths, res):
-            out[p] = r
+        for c, o in zip(clips, offsets):
+            view[o:o + c.shape[0]] = c
+        scores, row_off, labels = mdl.predict_clips_ragged(stage, offsets, padding=fn_kw.get("padding", 1),
+                                                           chunk_size=fn_kw.get("chunk_size", CHUNK))
+        out.update(zip(paths, _rows_to_dicts(scores, row_off, labels)))
     return out
