@@ -184,6 +184,24 @@ int oww_step_host(oww_ctx* ctx, const int16_t* h_pcm, int64_t pcm_stride, int n_
  * of step k.  collect blocks until that step's scores are in h_scores.                          */
 int oww_step_host_submit(oww_ctx* ctx, const int16_t* h_pcm, int64_t pcm_stride, int n_chunks, int* ticket);
 int oww_step_host_collect(oww_ctx* ctx, int ticket, float* h_scores);
+/* Ragged step: streams advance at their own pace.  Stream b steps h_chunks[b] chunks (host memory, 0..max_chunks),
+ * the first h_chunks[b]*1280 samples of row b; pcm_stride >= max(h_chunks)*1280.  Afterwards stream b is exactly a
+ * stream that was given those samples by oww_step(h_chunks[b]): its row of d_scores is what that call returns for it
+ * (per head the max over its own chunk windows, gates per chunk, custom verifiers after the max) and its -80 dB clamp
+ * spans its own chunks.  A stream with h_chunks[b] == 0 is held: its state (PCM tail, mel and feature rings, conv
+ * tails) does not change, bit for bit, a fresh stream stays fresh, and its row of d_scores is not written.
+ * All counts equal to n >= 1: the call is oww_step(n).  All 0: nothing is enqueued.  A count outside 0..max_chunks
+ * or a short stride fails with OWW_EINVAL before anything is enqueued.  Stream-ordered; no device allocation after
+ * the first call.  The counts are staged through a ring of four pinned buffers of the handle: a call waits (host
+ * side) for the count copy of the call four staging uses back - backpressure once the host runs that far ahead of
+ * the device (a multi-chunk call whose one-chunk streams take the fused launch on their own uses two).  The host
+ * side sorts the counts in small heap buffers.                                                                     */
+int oww_step_ragged(oww_ctx* ctx, const int16_t* d_pcm, int64_t pcm_stride, const int32_t* h_chunks, float* d_scores,
+                    void* stream);
+/* Same, host buffers (submit + collect, or the pipelined submit completed by oww_step_host_collect).  The collect
+ * leaves the rows of held streams in h_scores as the caller had them.                                               */
+int oww_step_host_ragged(oww_ctx* ctx, const int16_t* h_pcm, int64_t pcm_stride, const int32_t* h_chunks, float* h_scores);
+int oww_step_host_ragged_submit(oww_ctx* ctx, const int16_t* h_pcm, int64_t pcm_stride, const int32_t* h_chunks, int* ticket);
 /* last n rows of one stream's feature ring, ending `back` rows before the newest -> h_out[n][96];
  * rows older than the ring holds come back as zeros.  Synchronises.                             */
 int oww_get_features(oww_ctx* ctx, int stream_id, int n, int back, float* h_out);

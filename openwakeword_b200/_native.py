@@ -60,6 +60,9 @@ _SIGNATURES = {
     "oww_step_host": (C.c_int, [_P, _P, C.c_int64, C.c_int, _P]),
     "oww_step_host_submit": (C.c_int, [_P, _P, C.c_int64, C.c_int, C.POINTER(C.c_int)]),
     "oww_step_host_collect": (C.c_int, [_P, C.c_int, _P]),
+    "oww_step_ragged": (C.c_int, [_P, _P, C.c_int64, _P, _P, _P]),
+    "oww_step_host_ragged": (C.c_int, [_P, _P, C.c_int64, _P, _P]),
+    "oww_step_host_ragged_submit": (C.c_int, [_P, _P, C.c_int64, _P, C.POINTER(C.c_int)]),
     "oww_get_features": (C.c_int, [_P, C.c_int, C.c_int, C.c_int, _P]),
     "oww_get_mel": (C.c_int, [_P, C.c_int, C.c_int, _P]),
     "oww_get_counts": (C.c_int, [_P, C.c_int, C.POINTER(C.c_int), C.POINTER(C.c_int)]),
@@ -322,6 +325,32 @@ class Context:
     def step_host_collect(self, ticket, scores_out):
         assert scores_out.dtype == np.float32 and scores_out.flags.c_contiguous
         self._check(self.lib.oww_step_host_collect(self.h, ticket, _ptr(scores_out)))
+
+    def _chunks(self, chunks):
+        c = np.ascontiguousarray(chunks, np.int32)
+        if c.shape != (self.n_streams,):
+            raise ValueError(f"chunks has shape {c.shape}, the handle has {self.n_streams} streams")
+        return c
+
+    def step_ragged(self, d_pcm, pcm_stride, chunks, d_scores, stream=None):
+        """Stream b steps chunks[b] (host int32 [B], 0..max_chunks) chunks: the first chunks[b]*1280 samples of row b.
+        Rows of d_scores of streams with 0 chunks are not written (include/owwb200.h, oww_step_ragged)."""
+        c = self._chunks(chunks)
+        self._check(self.lib.oww_step_ragged(self.h, _ptr(d_pcm), int(pcm_stride), _ptr(c), _ptr(d_scores), stream))
+
+    def step_host_ragged(self, pcm, chunks, scores_out):
+        """pcm: C-contiguous int16 [B, >= max(chunks)*1280]; rows of scores_out of held streams are left as they were."""
+        assert pcm.dtype == np.int16 and pcm.flags.c_contiguous
+        assert scores_out.dtype == np.float32 and scores_out.flags.c_contiguous
+        c = self._chunks(chunks)
+        self._check(self.lib.oww_step_host_ragged(self.h, _ptr(pcm), pcm.shape[1], _ptr(c), _ptr(scores_out)))
+
+    def step_host_ragged_submit(self, pcm, chunks):
+        assert pcm.dtype == np.int16 and pcm.flags.c_contiguous
+        c = self._chunks(chunks)
+        t = C.c_int(-1)
+        self._check(self.lib.oww_step_host_ragged_submit(self.h, _ptr(pcm), pcm.shape[1], _ptr(c), C.byref(t)))
+        return t.value
 
     def get_features(self, stream_id, n, back=0):
         out = np.empty((n, 96), np.float32)

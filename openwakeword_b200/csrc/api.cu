@@ -90,6 +90,70 @@ __global__ void reset_kernel(const int* ids, int n_ids, int n_streams, int16_t* 
     }
 }
 
+// Ragged step, mode 3: the streams ids[0..n_ids) did not step in the CNN launch that just ran (dead slots: it wrote no
+// tails for them).  Their tails state moves unchanged to the buffers the next launch reads - reset_kernel's scatter with
+// the stream's own pre-launch rows as the source (ResetTails: tmpl = the G-group tails buffer the launch read, late[].tmpl
+// = the late buffer it read; the late chain left rows 0..1 of those untouched).
+__global__ void carry_kernel(const int* ids, int n_ids, ResetTails rt) {
+    oww_pdl_sync();
+    const int b = ids[blockIdx.x];
+    const int grp = b / rt.G, g = b - grp * rt.G;
+    const uint4* src = rt.tmpl + (int64_t)grp * rt.tail_units;
+    uint4* dst = rt.tails + (int64_t)grp * rt.tail_units;
+    for (int k = 0; k < rt.n_tab; ++k) {
+        const int offG = rt.tab[k].y, cg = rt.tab[k].z, Wp = rt.tab[k].w;
+        for (int i = threadIdx.x; i < cg * 2 * Wp; i += blockDim.x) {
+            const int pl = i / (2 * Wp), u = i - pl * 2 * Wp, r = u / Wp, f = u - r * Wp;
+            const int64_t at = offG + pl * (2 * rt.G * Wp) + (r * rt.G + g) * Wp + f;
+            dst[at] = src[at];
+        }
+    }
+    for (int k = 0; k < rt.n_late; ++k) {
+        const ResetLate& T = rt.late[k];
+        for (int i = threadIdx.x; i < T.n_planes * 2 * T.Wp; i += blockDim.x) {
+            const int pl = i / (2 * T.Wp), u = i - pl * 2 * T.Wp, r = u / T.Wp, f = u - r * T.Wp;
+            if (f >= T.lay.Wq) continue;
+            const uint4 v = T.tmpl[late_unit(T.lay, pl, b, r, f)];
+            T.now[late_unit(T.lay, pl, b, r, f)] = v;
+            if (T.next && r == 1) T.next[late_unit(T.lay, pl, b, 0, f)] = v;
+        }
+    }
+}
+
+// Ragged step: stream b appends embedding rows n - cnt[b] .. n - 1 of emb [n][B][96] (its own chunks, oldest first) to
+// its feature ring and advances its count by cnt[b].  One warp per stream.
+__global__ void __launch_bounds__(256) feat_append_ragged_kernel(const float* emb, float* ring, int* count, int B, int n,
+                                                                 const int* cnt, int rows_mask, int64_t ring_stride) {
+    oww_pdl_sync();
+    const int b = blockIdx.x * 8 + (threadIdx.x >> 5), lane = threadIdx.x & 31;
+    if (b >= B) return;
+    const int c = cnt[b];
+    if (c == 0) return;
+    const int c0 = count[b];
+    for (int i = lane; i < c * 24; i += 32) {
+        const int j = i / 24, c4 = i - j * 24;           // j-th of the stream's chunks = launch n - c + j
+        reinterpret_cast<float4*>(ring + (int64_t)b * ring_stride + (int64_t)((c0 + j) & rows_mask) * 96)[c4] =
+            __ldg(reinterpret_cast<const float4*>(emb + ((int64_t)(n - c + j) * B + b) * 96) + c4);
+    }
+    __syncwarp();
+    if (lane == 0) count[b] = oww_wrap_count(c0 + c);
+}
+
+// Ragged step: score row of stream b = per column the max over its own cnt[b] chunk windows (src [back][B][n_out], back 0
+// = newest; verifier gates were applied per window by the heads).  Rows of held streams (cnt 0) are not written.
+__global__ void ragged_max_kernel(const float* src, int B, int n_out, const int* cnt, float* dst, int out_stride) {
+    oww_pdl_sync();
+    const int64_t total = (int64_t)B * n_out;
+    for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (int64_t)gridDim.x * blockDim.x) {
+        const int b = (int)(i / n_out), col = (int)(i - (int64_t)b * n_out);
+        const int k = cnt[b];
+        if (k == 0) continue;
+        float v = src[i];
+        for (int j = 1; j < k; ++j) v = fmaxf(v, src[(int64_t)j * total + i]);
+        dst[(int64_t)b * out_stride + col] = v;
+    }
+}
+
 }  // namespace
 // Tails of the all-ones window per tails-bearing tensor, in the compact G = 1 layout, computed once per weight set by
 // the full-window tensor-core kernels (cnn_tc.cu) - the state every freshly reset stream starts from (its mel history IS
@@ -103,6 +167,11 @@ void free_streams(oww_ctx* c) {
     cudaFree(c->d_emb_tmp); cudaFree(c->d_inc_tails[0]); cudaFree(c->d_inc_tails[1]);
     cudaFree(c->d_reset_ids); cudaFree(c->d_reset_init);
     cudaFree(c->d_scores_tmp);
+    cudaFree(c->d_rag_scores); c->d_rag_scores = nullptr; c->rag_scores_floats = 0;
+    for (int j = 0; j < oww_ctx::kRagSlots; ++j) {       // set_streams / destroy synchronise the device first
+        cudaFreeHost(c->h_rag[j]); cudaFree(c->d_rag[j]); c->h_rag[j] = nullptr; c->d_rag[j] = nullptr;
+    }
+    c->rag_streams = 0;
     oww_verifiers_free_streams(c);
     oww_heads_grp_drop_mirror(c);
     for (auto& X : c->late_x) for (auto& b : X.buf) { cudaFree(b); b = nullptr; }
@@ -326,6 +395,195 @@ int step_core(oww_ctx* ctx, const int16_t* d_pcm, int64_t pcm_stride, int n_chun
     return OWW_OK;
 }
 
+// Mode 3: where the tails state the next CNN launch reads lives - the G-group tails buffer d_inc_tails[inc_cur] and, per
+// tails-bearing late tensor, rows 0..1 of buf[k % n_buf] (+ row 0 of buf[(k + 1) % 3] for tensors that gain one row per
+// step) at k = late_step.  The sources (tmpl) are the caller's: reset_kernel's template or carry_kernel's own state.
+int next_step_tables(oww_ctx* ctx, ResetTails& rt) {
+    std::memset(&rt, 0, sizeof(rt));
+    if (!ctx->tails_template_valid) { int rc = oww_inc_build_template(ctx); if (rc) return rc; }   // fills tail_tab
+    rt.tails = reinterpret_cast<uint4*>(ctx->d_inc_tails[ctx->inc_cur]);
+    rt.G = ctx->inc_plan.G; rt.tail_units = ctx->inc_plan.tail_units; rt.n_tab = ctx->n_tail_tab;
+    for (int k = 0; k < ctx->n_tail_tab; ++k) rt.tab[k] = ctx->tail_tab[k];
+    if (ctx->late_active) {
+        const long k = ctx->late_step;                      // index of the next chunk any stream processes
+        for (int l = ctx->split_from; l < OWW_N_CONV; ++l) {
+            const oww_ctx::LateTensor& X = ctx->late_x[l];
+            if (X.tmpl_off < 0) continue;
+            ResetLate& T = rt.late[rt.n_late++];
+            T.now = reinterpret_cast<uint4*>(X.buf[k % X.n_buf]);
+            T.next = X.n_buf == 3 ? reinterpret_cast<uint4*>(X.buf[(k + 1) % 3]) : nullptr;
+            T.Wp = X.W + 1; T.n_planes = 2 * X.cg; T.lay = X.lay;
+        }
+    }
+    return OWW_OK;
+}
+
+// After a CNN launch (and its late chain) of a ragged step: carry the tails state of the n held streams listed at d_ids.
+int carry_launch(oww_ctx* ctx, const int* d_ids, int n, cudaStream_t s) {
+    if (n <= 0) return OWW_OK;
+    ResetTails rt;
+    int rc = next_step_tables(ctx, rt);
+    if (rc) return rc;
+    rt.tmpl = reinterpret_cast<const uint4*>(ctx->d_inc_tails[ctx->inc_cur ^ 1]);   // the buffer the launch read
+    for (int i = 0, l = ctx->split_from; i < rt.n_late; ++l) {
+        const oww_ctx::LateTensor& X = ctx->late_x[l];
+        if (X.tmpl_off >= 0) rt.late[i++].tmpl = reinterpret_cast<const uint4*>(X.buf[(ctx->late_step - 1) % X.n_buf]);
+    }
+    OWW_CUDA(ctx, oww_launch_pdl(ctx->late_pdl, carry_kernel, dim3(n), dim3(256), 0, s, d_ids, n, rt));
+    OWW_LAUNCH_CHECK(ctx);
+    return OWW_OK;
+}
+
+// Ragged step (oww_step_ragged): stream b steps cnt[b] = h_chunks[b] chunks, the first cnt[b]*1280 samples of its row;
+// n = max cnt >= 1 and the counts are not all equal (the caller runs those as oww_step).  Streams that do not step in a
+// launch are dead slots there: no state, ring or score write; carry_kernel moves their rotating tails.  Multi-chunk
+// calls run right-aligned: CNN launch i steps the streams with cnt >= n - i, so its window offset 8*(n-1-i) is right
+// relative to each stream's own mel count.
+int step_ragged_core(oww_ctx* ctx, const int16_t* d_pcm, int64_t pcm_stride, const int32_t* h_chunks, int n, float* d_scores,
+                     int out_stride, cudaStream_t s) {
+    const int B = ctx->n_streams, n_out = ctx->n_out_total, mc = ctx->cfg.max_chunks;
+    int rc;
+    const bool inc = ctx->cfg.cnn_mode == OWW_CNN_TC_INCREMENTAL;
+    if (inc && n > 1 && oww_fused_heads_supported(ctx)) {
+        // oww_step(1) runs the heads inside the fused kernel (its own summation order): streams with one chunk take
+        // that launch as a ragged step of their own, the others the general path
+        std::vector<int32_t> one(B), more(B);
+        bool any_one = false;
+        for (int b = 0; b < B; ++b) {
+            one[b] = h_chunks[b] == 1;
+            more[b] = h_chunks[b] >= 2 ? h_chunks[b] : 0;
+            any_one = any_one || h_chunks[b] == 1;
+        }
+        if (any_one) {
+            if ((rc = step_ragged_core(ctx, d_pcm, pcm_stride, one.data(), 1, d_scores, out_stride, s))) return rc;
+            return step_ragged_core(ctx, d_pcm, pcm_stride, more.data(), n, d_scores, out_stride, s);
+        }
+    }
+    // staging: [B counts | B stream ids by ascending count]; below[c] = number of streams with fewer than c chunks
+    if (ctx->rag_streams != B) {
+        for (int j = 0; j < oww_ctx::kRagSlots; ++j) {
+            if (ctx->rag_ev[j]) OWW_CUDA(ctx, cudaEventSynchronize(ctx->rag_ev[j]));
+            cudaFreeHost(ctx->h_rag[j]); cudaFree(ctx->d_rag[j]); ctx->h_rag[j] = nullptr; ctx->d_rag[j] = nullptr;
+        }
+        ctx->rag_streams = 0;
+        for (int j = 0; j < oww_ctx::kRagSlots; ++j) {
+            OWW_CUDA(ctx, cudaMallocHost(&ctx->h_rag[j], (size_t)2 * B * sizeof(int32_t)));
+            OWW_CUDA(ctx, cudaMalloc(&ctx->d_rag[j], (size_t)2 * B * sizeof(int32_t)));
+            if (!ctx->rag_ev[j]) OWW_CUDA(ctx, cudaEventCreateWithFlags(&ctx->rag_ev[j], cudaEventDisableTiming));
+        }
+        ctx->rag_streams = B;
+    }
+    const size_t need = (size_t)mc * B * n_out;
+    if (ctx->rag_scores_floats < need) {
+        cudaFree(ctx->d_rag_scores); ctx->d_rag_scores = nullptr; ctx->rag_scores_floats = 0;
+        OWW_CUDA(ctx, cudaMalloc(&ctx->d_rag_scores, need * sizeof(float)));
+        ctx->rag_scores_floats = need;
+    }
+    const int j = ctx->rag_next;
+    ctx->rag_next = (j + 1) % oww_ctx::kRagSlots;
+    OWW_CUDA(ctx, cudaEventSynchronize(ctx->rag_ev[j]));          // the copy of the call kRagSlots back has run
+    int32_t* h = ctx->h_rag[j];
+    std::vector<int> below(mc + 2, 0);
+    for (int b = 0; b < B; ++b) below[h_chunks[b] + 1]++;
+    for (int c = 1; c <= mc + 1; ++c) below[c] += below[c - 1];
+    {
+        std::vector<int> at(below.begin(), below.end() - 1);
+        for (int b = 0; b < B; ++b) { h[b] = h_chunks[b]; h[B + at[h_chunks[b]]++] = b; }
+    }
+    OWW_CUDA(ctx, cudaMemcpyAsync(ctx->d_rag[j], h, (size_t)2 * B * sizeof(int32_t), cudaMemcpyHostToDevice, s));
+    OWW_CUDA(ctx, cudaEventRecord(ctx->rag_ev[j], s));
+    const int* d_cnt = ctx->d_rag[j];
+    const int* d_ord = d_cnt + B;
+    const FeatSrc fs0{ctx->d_feat_ring, (int64_t)ctx->feat_rows * 96, ctx->d_feat_count, ctx->feat_rows - 1, 0};
+    auto append = [&](int n_launch) {
+        OWW_CUDA(ctx, oww_launch_pdl(ctx->late_pdl, feat_append_ragged_kernel, dim3((B + 7) / 8), dim3(256), 0, s,
+                                     (const float*)ctx->d_emb_tmp, ctx->d_feat_ring, ctx->d_feat_count, B, n_launch, d_cnt,
+                                     ctx->feat_rows - 1, (int64_t)ctx->feat_rows * 96));
+        OWW_LAUNCH_CHECK(ctx);
+        return OWW_OK;
+    };
+    // heads of every stream on its windows back = 0 .. n-1, then the max over each stream's own cnt windows
+    auto heads = [&](int n_launch) {
+        if (n_out == 0) return OWW_OK;
+        for (int i = 0; i < n_launch; ++i) {
+            FeatSrc fs = fs0; fs.back = i;
+            int r = oww_heads_all(ctx, fs, B, ctx->d_rag_scores + (size_t)i * B * n_out, n_out, 0, s);
+            if (r) return r;
+        }
+        const int64_t total = (int64_t)B * n_out;
+        OWW_CUDA(ctx, oww_launch_pdl(ctx->late_pdl, ragged_max_kernel, dim3((unsigned)std::min<int64_t>(4096, (total + 255) / 256)),
+                                     dim3(256), 0, s, (const float*)ctx->d_rag_scores, B, n_out, d_cnt, d_scores, out_stride));
+        OWW_LAUNCH_CHECK(ctx);
+        return OWW_OK;
+    };
+
+    if (inc && n == 1 && oww_fused_frontend_supported(ctx)) {
+        // one chunk: the fused launch with the held streams (cnt 0 = ord[0 .. below[1])) as dead slots
+        const bool heads_inside = oww_fused_heads_supported(ctx);
+        if ((rc = oww_fused_step(ctx, d_pcm, pcm_stride, d_scores, out_stride, heads_inside, s, d_cnt, 1))) return rc;
+        if (ctx->late_active) {
+            if ((rc = oww_late_chain(ctx, ctx->d_emb_tmp, s))) return rc;
+            if ((rc = append(1))) return rc;
+        }
+        if ((rc = carry_launch(ctx, d_ord, below[1], s))) return rc;
+        if (heads_inside) {
+            oww_feat16_invalidate(ctx);
+        } else {
+            if ((rc = oww_feat16_advance(ctx, 1, s))) return rc;
+            if ((rc = oww_feat16_resync(ctx, d_ord, below[1], s))) return rc;     // held: their window did not move
+            if ((rc = heads(1))) return rc;
+        }
+        return oww_verifiers_apply(ctx, fs0, B, d_scores, out_stride, false, s, d_cnt);
+    }
+
+    // ---- general path: one mel launch per distinct count on its streams, the CNN launch by launch, masked append ----
+    for (int c = 1; c <= n; ++c) {
+        const int m = below[c + 1] - below[c];
+        if (m == 0) continue;
+        MelLaunch ml{d_pcm, pcm_stride, c * OWW_SAMPLES_PER_CHUNK, ctx->d_tail, ctx->d_seen, ctx->d_mel_ring,
+                     (int64_t)ctx->mel_rows * 32, ctx->mel_rows - 1, ctx->d_mel_count, m, 1, c};
+        ml.ids = d_ord + below[c];
+        if ((rc = oww_mel_launch(ctx, ml, s))) return rc;
+    }
+    if (inc) {
+        for (int i = 0; i < n; ++i) {
+            if ((rc = oww_cnn_inc_step(ctx, 8 * (n - 1 - i), ctx->d_emb_tmp + (size_t)i * B * 96, s, d_cnt, n - i))) return rc;
+            if ((rc = carry_launch(ctx, d_ord, below[n - i], s))) return rc;
+        }
+    } else {
+        // every stream's n newest window positions; those before a stream's own chunks are computed and not appended
+        WindowSrc ws{ctx->d_mel_ring, (int64_t)ctx->mel_rows * 32, ctx->d_mel_count, ctx->mel_rows - 1, B, n};
+        if ((rc = oww_cnn_window(ctx, ws, B * n, ctx->d_emb_tmp, s, false))) return rc;
+    }
+    if ((rc = append(n))) return rc;
+    if ((rc = oww_feat16_advance(ctx, n, s))) return rc;
+    if ((rc = oww_feat16_resync(ctx, d_ord, below[n], s))) return rc;       // streams that appended fewer than n rows
+    if ((rc = heads(n))) return rc;
+    return oww_verifiers_apply(ctx, fs0, B, d_scores, out_stride, false, s, d_cnt);
+}
+
+// validation shared by the ragged entry points: counts in [0, max_chunks], stride for the largest; -> n = max count
+int ragged_check(oww_ctx* ctx, const int32_t* h_chunks, int64_t pcm_stride, int* n_max, bool* all_equal) {
+    const int B = ctx->n_streams;
+    if (B <= 0) return oww_fail(ctx, OWW_EINVAL, "oww_set_streams has not been called");
+    if (!ctx->mel_loaded || !ctx->emb_loaded) return oww_fail(ctx, OWW_EINVAL, "weights not loaded");
+    int n = 0;
+    bool eq = true;
+    for (int b = 0; b < B; ++b) {
+        if (h_chunks[b] < 0 || h_chunks[b] > ctx->cfg.max_chunks)
+            return oww_fail(ctx, OWW_EINVAL, "chunks[%d]=%d outside [0,%d]", b, h_chunks[b], ctx->cfg.max_chunks);
+        n = std::max(n, (int)h_chunks[b]);
+        eq = eq && h_chunks[b] == h_chunks[0];
+    }
+    if (n > 0 && pcm_stride < (int64_t)n * OWW_SAMPLES_PER_CHUNK)
+        return oww_fail(ctx, OWW_EINVAL, "pcm_stride=%lld < %d samples (max chunks %d)", (long long)pcm_stride,
+                        n * OWW_SAMPLES_PER_CHUNK, n);
+    *n_max = n; *all_equal = eq;
+    return OWW_OK;
+}
+
+int host_submit(oww_ctx* ctx, const int16_t* h_pcm, int64_t pcm_stride, int n_chunks, const int32_t* h_chunks, int* ticket);
+
 // shared by oww_reset (synchronous) and oww_reset_async: enqueue the state reset of the listed streams on `s`
 int reset_enqueue(oww_ctx* ctx, const int32_t* h_stream_ids, int n, const float* h_feature_init, int n_rows, cudaStream_t s) {
     if (ctx->n_streams <= 0) return oww_fail(ctx, OWW_EINVAL, "oww_set_streams has not been called");
@@ -346,23 +604,12 @@ int reset_enqueue(oww_ctx* ctx, const int32_t* h_stream_ids, int n, const float*
     ResetTails rt;
     std::memset(&rt, 0, sizeof(rt));
     if (ctx->cfg.cnn_mode == OWW_CNN_TC_INCREMENTAL) {
-        if (!ctx->tails_template_valid) { int rc = oww_inc_build_template(ctx); if (rc) return rc; }
-        rt.tails = reinterpret_cast<uint4*>(ctx->d_inc_tails[ctx->inc_cur]);      // the buffer the next step reads
+        int rc = next_step_tables(ctx, rt);
+        if (rc) return rc;
         rt.tmpl = reinterpret_cast<const uint4*>(ctx->d_tails_template);
-        rt.G = ctx->inc_plan.G; rt.tail_units = ctx->inc_plan.tail_units; rt.n_tab = ctx->n_tail_tab;
-        for (int k = 0; k < ctx->n_tail_tab; ++k) rt.tab[k] = ctx->tail_tab[k];
-        if (ctx->late_active) {
-            const long k = ctx->late_step;                      // index of the next chunk any stream processes
-            for (int l = ctx->split_from; l < OWW_N_CONV; ++l) {
-                const oww_ctx::LateTensor& X = ctx->late_x[l];
-                if (X.tmpl_off < 0) continue;
-                ResetLate& T = rt.late[rt.n_late++];
-                T.now = reinterpret_cast<uint4*>(X.buf[k % X.n_buf]);
-                T.next = X.n_buf == 3 ? reinterpret_cast<uint4*>(X.buf[(k + 1) % 3]) : nullptr;
-                T.tmpl = reinterpret_cast<const uint4*>(ctx->d_late_template) + X.tmpl_off;
-                T.Wp = X.W + 1; T.n_planes = 2 * X.cg; T.lay = X.lay;
-            }
-        }
+        for (int i = 0, l = ctx->split_from; i < rt.n_late; ++l)
+            if (ctx->late_x[l].tmpl_off >= 0)
+                rt.late[i++].tmpl = reinterpret_cast<const uint4*>(ctx->d_late_template) + ctx->late_x[l].tmpl_off;
     }
     reset_kernel<<<n, 256, 0, s>>>(h_stream_ids ? ctx->d_reset_ids : nullptr, n, ctx->n_streams, ctx->d_tail, ctx->d_seen,
                                    ctx->d_mel_count, ctx->d_feat_count, ctx->d_mel_ring, ctx->mel_rows, ctx->d_feat_ring,
@@ -432,6 +679,7 @@ void oww_destroy(oww_ctx* ctx) {
     cudaFree(ctx->d_gates); cudaFree(ctx->d_tails_template); cudaFree(ctx->d_peer_err);
     for (auto& b : ctx->banks) { cudaFree(b.d_mean); cudaFree(b.d_weight); cudaFree(b.d_bias); }
     for (auto e : ctx->ver_ev) if (e) cudaEventDestroy(e);
+    for (auto e : ctx->rag_ev) if (e) cudaEventDestroy(e);
     for (auto& S : ctx->slot) {
         cudaFreeHost(S.h_pcm); cudaFreeHost(S.h_scores); cudaFree(S.d_pcm); cudaFree(S.d_scores);
         if (S.done) cudaEventDestroy(S.done);
@@ -627,6 +875,50 @@ int oww_step_host_submit(oww_ctx* ctx, const int16_t* h_pcm, int64_t pcm_stride,
     if (B <= 0) return oww_fail(ctx, OWW_EINVAL, "oww_set_streams has not been called");
     if (n_chunks < 1 || n_chunks > ctx->cfg.max_chunks)
         return oww_fail(ctx, OWW_EINVAL, "n_chunks=%d outside [1,%d]", n_chunks, ctx->cfg.max_chunks);
+    return host_submit(ctx, h_pcm, pcm_stride, n_chunks, nullptr, ticket);
+}
+
+int oww_step_ragged(oww_ctx* ctx, const int16_t* d_pcm, int64_t pcm_stride, const int32_t* h_chunks, float* d_scores,
+                    void* stream) {
+    if (!ctx || !h_chunks || !d_scores) return oww_fail(ctx, OWW_EINVAL, "null argument");
+    OWW_CUDA(ctx, cudaSetDevice(ctx->device));
+    int n = 0; bool eq = false;
+    int rc = ragged_check(ctx, h_chunks, pcm_stride, &n, &eq);
+    if (rc) return rc;
+    if (n == 0) return OWW_OK;
+    if (!d_pcm) return oww_fail(ctx, OWW_EINVAL, "null argument");
+    if (eq) return step_core(ctx, d_pcm, pcm_stride, n, d_scores, ctx->n_out_total, (cudaStream_t)stream);
+    return step_ragged_core(ctx, d_pcm, pcm_stride, h_chunks, n, d_scores, ctx->n_out_total, (cudaStream_t)stream);
+}
+
+int oww_step_host_ragged_submit(oww_ctx* ctx, const int16_t* h_pcm, int64_t pcm_stride, const int32_t* h_chunks, int* ticket) {
+    if (!ctx || !h_chunks || !ticket) return oww_fail(ctx, OWW_EINVAL, "null argument");
+    OWW_CUDA(ctx, cudaSetDevice(ctx->device));
+    int n = 0; bool eq = false;
+    int rc = ragged_check(ctx, h_chunks, pcm_stride, &n, &eq);
+    if (rc) return rc;
+    if (n > 0 && !h_pcm) return oww_fail(ctx, OWW_EINVAL, "null argument");
+    return host_submit(ctx, h_pcm, pcm_stride, n, h_chunks, ticket);
+}
+
+int oww_step_host_ragged(oww_ctx* ctx, const int16_t* h_pcm, int64_t pcm_stride, const int32_t* h_chunks, float* h_scores) {
+    if (!ctx || !h_scores) return oww_fail(ctx, OWW_EINVAL, "null argument");
+    for (int i = 0; i < 2; ++i)
+        if (ctx->slot[i].busy) return oww_fail(ctx, OWW_EINVAL, "a submitted step is still in flight: collect it first");
+    int ticket = -1;
+    int rc = oww_step_host_ragged_submit(ctx, h_pcm, pcm_stride, h_chunks, &ticket);
+    if (rc) return rc;
+    return oww_step_host_collect(ctx, ticket, h_scores);
+}
+
+}  // extern "C"
+
+namespace {
+
+// Host-buffer step on the handle's own stream.  h_chunks == nullptr: every stream steps n_chunks; else the ragged counts
+// (validated, n_chunks = their max, which may be 0: nothing is launched and the ticket completes at once).
+int host_submit(oww_ctx* ctx, const int16_t* h_pcm, int64_t pcm_stride, int n_chunks, const int32_t* h_chunks, int* ticket) {
+    const int B = ctx->n_streams;
     const int si = ctx->next_slot;
     oww_ctx::HostSlot& S = ctx->slot[si];
     if (S.busy) return oww_fail(ctx, OWW_EINVAL, "both host slots are in flight: collect a ticket first");
@@ -653,23 +945,34 @@ int oww_step_host_submit(oww_ctx* ctx, const int16_t* h_pcm, int64_t pcm_stride,
     const bool pinned = pcm_stride == (int64_t)row && cudaPointerGetAttributes(&attr, h_pcm) == cudaSuccess &&
                         attr.type == cudaMemoryTypeHost;
     cudaGetLastError();                                     // unregistered host memory reports an error on older drivers
-    if (pinned) {
-        src = h_pcm;
-    } else if (pcm_stride == (int64_t)row) {
-        std::memcpy(S.h_pcm, h_pcm, pcm_bytes);
-    } else {
-        for (int b = 0; b < B; ++b)
-            std::memcpy(S.h_pcm + (size_t)b * row, h_pcm + (size_t)b * pcm_stride, row * sizeof(int16_t));
-    }
-    OWW_CUDA(ctx, cudaMemcpyAsync(S.d_pcm, src, pcm_bytes, cudaMemcpyHostToDevice, ctx->copy_stream));
-    OWW_CUDA(ctx, cudaEventRecord(S.h2d_done, ctx->copy_stream));
     cudaStream_t s = ctx->own_stream;
-    OWW_CUDA(ctx, cudaStreamWaitEvent(s, S.h2d_done, 0));
-    int rc = step_core(ctx, S.d_pcm, (int64_t)row, n_chunks, S.d_scores, ctx->n_out_total, s);
-    if (rc) return rc;
-    if (ctx->n_out_total > 0)
-        OWW_CUDA(ctx, cudaMemcpyAsync(S.h_scores, S.d_scores, (size_t)B * ctx->n_out_total * sizeof(float),
-                                      cudaMemcpyDeviceToHost, s));
+    // every row written by the step: a lockstep call, or ragged counts all equal to n_chunks >= 1 (all 0: no row)
+    bool all_step = h_chunks == nullptr;
+    if (h_chunks && n_chunks > 0) {
+        all_step = true;
+        for (int b = 0; b < B && all_step; ++b) all_step = h_chunks[b] == n_chunks;
+    }
+    if (all_step) ctx->slot_chunks[si].clear();
+    else ctx->slot_chunks[si].assign(h_chunks, h_chunks + B);
+    if (n_chunks > 0) {
+        if (pinned) {
+            src = h_pcm;
+        } else if (pcm_stride == (int64_t)row) {
+            std::memcpy(S.h_pcm, h_pcm, pcm_bytes);
+        } else {
+            for (int b = 0; b < B; ++b)
+                std::memcpy(S.h_pcm + (size_t)b * row, h_pcm + (size_t)b * pcm_stride, row * sizeof(int16_t));
+        }
+        OWW_CUDA(ctx, cudaMemcpyAsync(S.d_pcm, src, pcm_bytes, cudaMemcpyHostToDevice, ctx->copy_stream));
+        OWW_CUDA(ctx, cudaEventRecord(S.h2d_done, ctx->copy_stream));
+        OWW_CUDA(ctx, cudaStreamWaitEvent(s, S.h2d_done, 0));
+        int rc = all_step ? step_core(ctx, S.d_pcm, (int64_t)row, n_chunks, S.d_scores, ctx->n_out_total, s)
+                          : step_ragged_core(ctx, S.d_pcm, (int64_t)row, h_chunks, n_chunks, S.d_scores, ctx->n_out_total, s);
+        if (rc) return rc;
+        if (ctx->n_out_total > 0)
+            OWW_CUDA(ctx, cudaMemcpyAsync(S.h_scores, S.d_scores, (size_t)B * ctx->n_out_total * sizeof(float),
+                                          cudaMemcpyDeviceToHost, s));
+    }
     OWW_CUDA(ctx, cudaEventRecord(S.done, s));
     S.busy = true;
     ctx->next_slot = si ^ 1;
@@ -677,13 +980,25 @@ int oww_step_host_submit(oww_ctx* ctx, const int16_t* h_pcm, int64_t pcm_stride,
     return OWW_OK;
 }
 
+}  // namespace
+
+extern "C" {
+
 int oww_step_host_collect(oww_ctx* ctx, int ticket, float* h_scores) {
     if (!ctx || !h_scores) return oww_fail(ctx, OWW_EINVAL, "null argument");
     if (ticket < 0 || ticket > 1 || !ctx->slot[ticket].busy) return oww_fail(ctx, OWW_EINVAL, "ticket %d is not in flight", ticket);
     OWW_CUDA(ctx, cudaSetDevice(ctx->device));
     oww_ctx::HostSlot& S = ctx->slot[ticket];
     OWW_CUDA(ctx, cudaEventSynchronize(S.done));
-    if (ctx->n_out_total > 0) std::memcpy(h_scores, S.h_scores, (size_t)ctx->n_streams * ctx->n_out_total * sizeof(float));
+    const int n_out = ctx->n_out_total;
+    const std::vector<int32_t>& cnt = ctx->slot_chunks[ticket];
+    if (n_out > 0 && cnt.empty()) {
+        std::memcpy(h_scores, S.h_scores, (size_t)ctx->n_streams * n_out * sizeof(float));
+    } else if (n_out > 0) {
+        // ragged step: the rows of held streams stay as the caller had them (all held: none is copied)
+        for (int b = 0; b < ctx->n_streams; ++b)
+            if (cnt[b] > 0) std::memcpy(h_scores + (size_t)b * n_out, S.h_scores + (size_t)b * n_out, n_out * sizeof(float));
+    }
     S.busy = false;
     return OWW_OK;
 }

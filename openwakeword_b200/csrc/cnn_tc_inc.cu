@@ -45,6 +45,9 @@ struct IncArgs {
     const uint4* tails_in; uint4* tails_out;                  // [n_groups][tail_units]
     float* emb;                                               // [B][96]
     int B;
+    // ragged step (oww_step_ragged): stream b takes part in this launch iff live_chunks[b] >= live_min; a stream that
+    // does not is a dead slot (no state, ring or score write) and its tails are carried by the caller
+    const int* live_chunks; int live_min;
     long long* dbg_clock;                                     // optional: 21 clock64 stamps of CTA 0's first group
     // ---- fused step (fused != 0): the same launch also runs the log-mel frontend before layer 0, appends the embedding
     //      to the feature ring and evaluates every head, i.e. PCM in -> scores out ----
@@ -168,7 +171,7 @@ __global__ void __launch_bounds__(kIncThreads, 1) tc_inc_kernel(const __grid_con
             named_bar_sync(2, kIncEpiWarps * 32);                  // every warp is done with the previous group's s_live / s_cnt
             if (et < G) {
                 const int b = grp * G + et;
-                s_live[et] = b < a.B;
+                s_live[et] = b < a.B && (!a.live_chunks || a.live_chunks[b] >= a.live_min);
             }
             named_bar_sync(2, kIncEpiWarps * 32);
             if (a.fused) {
@@ -1082,9 +1085,10 @@ static void fill_inc_args(oww_ctx* ctx, IncArgs& a) {
 // One launch per step: frontend, 20-layer CNN and ring append for every stream, plus - with_heads - every head and
 // the verifier gates, i.e. PCM in -> scores out.
 int oww_fused_step(oww_ctx* ctx, const int16_t* d_pcm, int64_t pcm_stride, float* d_scores, int out_stride, bool with_heads,
-                   cudaStream_t s) {
+                   cudaStream_t s, const int* d_chunks, int min_chunks) {
     IncArgs a;
     fill_inc_args(ctx, a);
+    a.live_chunks = d_chunks; a.live_min = min_chunks;
     a.fused = 1;
     a.pcm = d_pcm; a.pcm_stride = pcm_stride;
     a.tail = ctx->d_tail; a.seen = ctx->d_seen; a.mel_rw = ctx->d_mel_ring; a.mel_count_rw = ctx->d_mel_count;
@@ -1115,9 +1119,10 @@ int oww_fused_step(oww_ctx* ctx, const int16_t* d_pcm, int64_t pcm_stride, float
 }
 
 // One incremental CNN pass for every stream: mel rows ending `back` rows before the newest.
-int oww_cnn_inc_step(oww_ctx* ctx, int back, float* d_emb, cudaStream_t s) {
+int oww_cnn_inc_step(oww_ctx* ctx, int back, float* d_emb, cudaStream_t s, const int* d_chunks, int min_chunks) {
     IncArgs a;
     fill_inc_args(ctx, a);
+    a.live_chunks = d_chunks; a.live_min = min_chunks;
     a.back = back;
     a.emb = d_emb;
     const int grid = a.plan.n_groups < ctx->sm_count ? a.plan.n_groups : ctx->sm_count;

@@ -64,6 +64,9 @@ struct ResetLate {           // one tails-bearing tensor of the incremental late
     LateLay lay;             // block-major layout of now / next
 };
 // late[]: one entry per tails-bearing late tensor X_l, l >= split_from (5 at the default split, 9 at split_from 3)
+// The carry of a held stream in a ragged step (api.cu, carry_kernel) fills the same tables with the stream's own state
+// as the source: tmpl = the G-group tails buffer the launch read, ResetLate::tmpl = the late buffer it read (same
+// layouts as tails / now).
 struct ResetTails { uint4* tails; const uint4* tmpl; int G, tail_units, n_tab; int4 tab[OWW_N_CONV]; int n_late; ResetLate late[OWW_N_CONV]; };
 
 // conditional verifier pair (hey_jarvis, docs/models/hey_jarvis.md:38): score column `main_col` is replaced by column
@@ -227,6 +230,17 @@ struct oww_ctx {
         bool busy = false;
     } slot[2];
     int next_slot = 0;
+    std::vector<int32_t> slot_chunks[2];   // per host slot: the ragged counts of its step (empty: every row stepped)
+
+    // ragged steps (oww_step_ragged): per call [B counts | B stream ids ordered by count], staged through a ring of
+    // pinned buffers (a slot is reused once the copy of the call kRagSlots calls back has run)
+    static constexpr int kRagSlots = 4;
+    int32_t* h_rag[kRagSlots] = {nullptr, nullptr, nullptr, nullptr};
+    int32_t* d_rag[kRagSlots] = {nullptr, nullptr, nullptr, nullptr};
+    cudaEvent_t rag_ev[kRagSlots] = {nullptr, nullptr, nullptr, nullptr};
+    int rag_next = 0, rag_streams = 0;
+    float* d_rag_scores = nullptr;   // [max_chunks][n_streams][n_out_total]: per chunk window, before the masked max
+    size_t rag_scores_floats = 0;
 
     // stage timing
     bool timing = false;
@@ -361,12 +375,14 @@ int oww_inc_build_plan(oww_ctx* ctx, int G, int n_streams, int n_layers, IncPlan
 int oww_inc_n_layers(const oww_ctx* ctx);
 int oww_inc_setup(oww_ctx* ctx, const float* h_blob);
 int oww_inc_alloc_streams(oww_ctx* ctx);
-int oww_cnn_inc_step(oww_ctx* ctx, int back, float* d_emb, cudaStream_t s);
+// d_chunks != nullptr (ragged step): only the streams with d_chunks[b] >= min_chunks step in this launch; the others are
+// dead slots whose tails state the caller carries (api.cu, carry_kernel)
+int oww_cnn_inc_step(oww_ctx* ctx, int back, float* d_emb, cudaStream_t s, const int* d_chunks = nullptr, int min_chunks = 0);
 // whole step in one launch (n_chunks == 1, primed): PCM -> mel -> CNN -> ring append -> heads -> scores
 bool oww_fused_frontend_supported(const oww_ctx* ctx);
 bool oww_fused_heads_supported(const oww_ctx* ctx);
 int oww_fused_step(oww_ctx* ctx, const int16_t* d_pcm, int64_t pcm_stride, float* d_scores, int out_stride, bool with_heads,
-                   cudaStream_t s);
+                   cudaStream_t s, const int* d_chunks = nullptr, int min_chunks = 0);
 int oww_heads_sync_devs(oww_ctx* ctx);
 int oww_inc_capture(oww_ctx* ctx, int layer, const void* planes, int64_t plane_pitch, int T, int W, int win0, int n_win,
                     int stream0, const int* d_ids, cudaStream_t s);
@@ -425,8 +441,9 @@ int oww_heads_all(oww_ctx* ctx, const FeatSrc& src, int n, float* d_out, int out
 // every bank of the handle on n rows of final scores (one launch; nothing when the handle has no bank).  The window of
 // row r is the newest n_in rows of `src` (FeatSrc sample r).  Its slot is bank.d_assign[r] for streams (rows = streams
 // of the handle), or bank.clip_slot for clips (rows = (clip, step) of the bulk path).
+// d_chunks != nullptr (ragged step): rows with d_chunks[r] == 0 did not step and are skipped.
 int oww_verifiers_apply(oww_ctx* ctx, const FeatSrc& src, int n, float* d_scores, int out_stride, bool clips,
-                        cudaStream_t s);
+                        cudaStream_t s, const int* d_chunks = nullptr);
 // (re)allocate every bank's per-stream assignment for ctx->n_streams streams, all -1
 int oww_verifiers_alloc_streams(oww_ctx* ctx);
 // true when oww_verifiers_apply(..., clips = true) would launch (a bank with a clip slot, verifiers enabled)

@@ -29,13 +29,14 @@ struct VerArgs {
     FeatSrc src;
     int n; float* out; int out_stride;
     int gated;                          // 0: stateless call, write p to column col0 of every row unconditionally
+    const int* step;                    // ragged step: rows with step[r] == 0 were held (their score row is not written)
 };
 
 __global__ void __launch_bounds__(kVerWarps * 32) verifier_kernel(const __grid_constant__ VerArgs a) {
     oww_pdl_sync();
     const int lane = threadIdx.x & 31;
     const int r = blockIdx.x * kVerWarps + (threadIdx.x >> 5);
-    if (r >= a.n) return;
+    if (r >= a.n || (a.step && a.step[r] == 0)) return;
     const VerBankDev& B = a.bank[blockIdx.y];
     const int slot = B.assign ? B.assign[r] : B.slot_all;
     if (slot < 0) return;
@@ -94,9 +95,10 @@ VerBankDev bank_dev(const VerifierBank& b, int slot_all, const int* assign) {
 }  // namespace
 
 int oww_verifiers_apply(oww_ctx* ctx, const FeatSrc& src, int n, float* d_scores, int out_stride, bool clips,
-                        cudaStream_t s) {
+                        cudaStream_t s, const int* d_chunks) {
     if (ctx->banks.empty() || !ctx->verifiers_on) return OWW_OK;
     VerArgs a;
+    a.step = d_chunks;
     int nb = 0;
     for (const VerifierBank& b : ctx->banks) {
         if (clips && b.clip_slot < 0) continue;              // no clip verifier for this head
@@ -249,7 +251,7 @@ int oww_verifier_predict(oww_ctx* ctx, int bank, int slot, const float* d_feats,
     a.bank[0] = bank_dev(b, slot, nullptr);
     a.bank[0].col0 = 0; a.bank[0].n_cols = 1;
     a.src = FeatSrc{d_feats, (int64_t)b.n_in * 96, nullptr, -1, 0};
-    a.n = n; a.out = d_out; a.out_stride = 1; a.gated = 0;
+    a.n = n; a.out = d_out; a.out_stride = 1; a.gated = 0; a.step = nullptr;
     return launch(ctx, a, 1, (cudaStream_t)stream);
 }
 

@@ -75,10 +75,33 @@ class StreamEngine:
         return self.ctx.step_host_submit(pcm, n_chunks)
 
     def collect(self, ticket, out=None):
+        """Scores of a submitted step; with out None the rows a ragged ticket held come back as NaN."""
         if out is None:
-            out = np.empty((self.n_streams, self.n_cols), np.float32)
+            out = np.full((self.n_streams, self.n_cols), np.nan, np.float32)
         self.ctx.step_host_collect(ticket, out)
         return out
+
+    # ---- ragged steps: every stream at its own pace (include/owwb200.h, oww_step_ragged) ----
+    def step_ragged(self, d_pcm, chunks, out=None):
+        """Stream b consumes chunks[b] (host ints, 0..max_chunks) chunks, the first chunks[b]*1280 samples of row b of
+        d_pcm.  A stream with 0 chunks is held: its state does not change and its row of `out` is not written."""
+        torch = _torch()
+        if out is None:
+            out = torch.full((self.n_streams, self.n_cols), float("nan"), dtype=torch.float32, device=d_pcm.device)
+        self.ctx.step_ragged(d_pcm, d_pcm.stride(0), chunks, out, torch.cuda.current_stream(d_pcm.device).cuda_stream)
+        return out
+
+    def step_host_ragged(self, pcm, chunks, out=None):
+        """Host form of ``step_ragged``; held rows of `out` keep their values (NaN when `out` is None)."""
+        if out is None:
+            out = np.full((self.n_streams, self.n_cols), np.nan, np.float32)
+        self.ctx.step_host_ragged(pcm, chunks, out)
+        return out
+
+    def submit_ragged(self, pcm, chunks):
+        """Pipelined ragged host step; complete it with ``collect`` (held rows of its `out` are left as they were, NaN
+        when `out` is None)."""
+        return self.ctx.step_host_ragged_submit(pcm, chunks)
 
     # ---- custom verifier models (include/owwb200.h, oww_add_verifier_bank) ----
     def add_verifier_bank(self, head_index, capacity, threshold=0.1):

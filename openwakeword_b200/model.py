@@ -227,17 +227,18 @@ class Model:
         else:
             self.custom_verifier_models[name] = {b: o for b, o in enumerate(objs) if o is not None}
 
-    def _reverify(self, mdl, predictions, labels):
+    def _reverify(self, mdl, predictions, labels, streams):
         """Verification on the host side of the stateless entry, on each stream's newest window (model.py:319-328): for
         calls that run no step (< 1280 samples: the previous prediction is re-verified, as the reference does) and for
         calls split into several device steps (> max_chunks chunks: those run without the banks, and the max over all
-        their chunk windows is verified here, once).  Streams with a device verifier and a label >= the threshold."""
+        their chunk windows is verified here, once).  Of `streams` (bool [B]): those with a device verifier and a label >=
+        the threshold."""
         st = self._vbanks[mdl]
         thr = np.float32(self.custom_verifier_threshold)
         hit = np.zeros(self.n_streams, bool)
         for lab in labels:
             hit |= predictions[lab] >= thr
-        hit &= st["slots"] >= 0
+        hit &= (st["slots"] >= 0) & streams
         for slot in np.unique(st["slots"][hit]):
             bs = np.nonzero(hit & (st["slots"] == slot))[0]
             feats = np.concatenate([self.preprocessor.get_features(self.model_inputs[mdl], stream=int(b)) for b in bs])
@@ -258,21 +259,34 @@ class Model:
         return self._hist[label], self._count[label]
 
     def _recent(self, label, n):
-        """last n appended predictions per stream -> [<=n, B] oldest first (deque(maxlen=30) view)."""
+        """Per stream its own last min(n_b, count_b, 30) appended predictions (deque(maxlen=30) view): -> (float32
+        [30, B] each stream's history oldest first, bool [30, B] which entries are among those).  n: int or int [B]."""
         hist, cnt = self._h(label)
-        c = int(cnt[0])                      # streams advance in lockstep
-        k = min(n, c, 30)
-        idx = [(c - k + i) % 30 for i in range(k)]
-        return hist[idx]
+        i = np.arange(30)[:, None]
+        ordered = hist[(cnt[None, :] - 30 + i) % 30, np.arange(self.n_streams)[None, :]]
+        k = np.minimum(np.minimum(np.asarray(n, np.int64), cnt), 30)
+        return ordered, i >= 30 - k[None, :]
 
     @property
     def prediction_buffer(self):
         """defaultdict(deque(maxlen=30)) of stream 0's history, like the reference attribute."""
         buf = defaultdict(partial(deque, maxlen=30))
         for label in self._hist:
-            for v in self._recent(label, 30)[:, 0]:
+            ordered, valid = self._recent(label, 30)
+            for v in ordered[valid[:, 0], 0]:
                 buf[label].append(float(v))
         return buf
+
+    def reset_streams(self, stream_ids, feature_init=None):
+        """Reset the listed streams only: device state, samples not yet stepped and prediction history (a new client on
+        a stream gets the first-5 zeroing of model.py:330-333 again).  The other streams are untouched."""
+        ids = np.asarray(stream_ids, np.int64).ravel()
+        if ids.size and (ids.min() < 0 or ids.max() >= self.n_streams):
+            raise ValueError(f"stream ids must be in [0, {self.n_streams})")
+        self.preprocessor.reset(feature_init, stream_ids=ids.astype(np.int32))
+        for label in self._hist:
+            self._hist[label][:, ids] = 0.0
+            self._count[label][ids] = 0
 
     def get_parent_model_from_label(self, label):
         parent = ""
@@ -313,31 +327,74 @@ class Model:
         if not isinstance(x, np.ndarray):
             raise ValueError(f"The input audio data (x) must by a Numpy array, instead received an object of type {type(x)}.")
         single = self.n_streams == 1
-        if timing:
-            timing_dict = {"models": {}}
-            t0 = time.time()
+        t0 = time.time()
         if self.speex_ns:
             if not single:
                 raise ValueError("Speex noise suppression is single-stream")
             x = self._suppress_noise_with_speex(x)
-        n_prepared, n_chunks = self.preprocessor._streaming_features(x, self._scores)
-        if timing:
-            timing_dict["models"]["preprocessor"] = time.time() - t0
+        if self.preprocessor.pending_ragged:
+            # the streams hold different remainders (after predict_ragged / reset_streams): per-stream accumulation
+            n_prepared, n_chunks, split = self.preprocessor._streaming_features_ragged(list(self.preprocessor._coerce(x)),
+                                                                                       self._scores)
+        else:
+            n_prepared, n_chunks = self.preprocessor._streaming_features(x, self._scores)
+            split = n_chunks > self.preprocessor.max_chunks
+            n_prepared = np.full(self.n_streams, n_prepared, np.int64)
+        return self._finish(n_prepared, split, patience, threshold, debounce_time, timing, t0, single)
 
+    def predict_ragged(self, x, patience={}, threshold={}, debounce_time=0.0, timing=False):
+        """One streaming step in which every stream gets its own samples: x is a sequence of n_streams 1-D NumPy arrays of
+        any lengths (0 included).  Stream b's result, state and history are those of an independent reference
+        ``Model`` that was given the same arrays: it steps the whole chunks of its own remainder + x[b] and keeps the
+        rest; with fewer than 1280 samples prepared it returns its previous prediction (one-output heads) or zeros, and
+        first-5 zeroing, patience and debounce use its own history and sample count.  A stream with no samples prepared
+        at all (n_prepared == 0) has a debounce window of its whole 30-entry history, the limit of the reference's
+        formula (which divides by zero there).  Returns {label: float32[B]} (a float per label for one stream)."""
         B = self.n_streams
+        try:
+            n = len(x)
+        except TypeError:
+            raise ValueError(f"predict_ragged takes a sequence of {B} 1-D NumPy arrays, got {type(x)}") from None
+        if n != B:
+            raise ValueError(f"predict_ragged takes one array per stream ({B}), got {n}")
+        xs = []
+        for b, a in enumerate(x):
+            if not isinstance(a, np.ndarray):
+                raise ValueError(f"The input audio data (x[{b}]) must by a Numpy array, instead received an object of "
+                                 f"type {type(a)}.")
+            if a.ndim != 1:
+                raise ValueError(f"x[{b}] must be 1-D, got shape {a.shape}")
+            xs.append(a if a.dtype == np.int16 else a.astype(np.int16))
+        t0 = time.time()
+        if self.speex_ns:
+            if B != 1:
+                raise ValueError("Speex noise suppression is single-stream")
+            xs = [self._suppress_noise_with_speex(xs[0])]
+        n_prepared, _, split = self.preprocessor._streaming_features_ragged(xs, self._scores)
+        return self._finish(n_prepared, split, patience, threshold, debounce_time, timing, t0, B == 1)
+
+    def _finish(self, n_prepared, split, patience, threshold, debounce_time, timing, t0, single):
+        """model.py:285-386 per stream after the device step(s): stream b prepared n_prepared[b] samples (its row of
+        self._scores holds the step's scores when >= 1280); split: the steps ran without the verifier banks."""
+        if timing:
+            timing_dict = {"models": {"preprocessor": time.time() - t0}}
+        B = self.n_streams
+        ar = np.arange(B)
+        stepped = n_prepared >= CHUNK
+        reverify = ~stepped | split
         predictions = {}
         for mdl in self.models.keys():
             if timing:
                 t1 = time.time()
             col0, n_out = self._columns[mdl]
-            if n_prepared >= CHUNK:
-                pred = self._scores[:, col0:col0 + n_out]            # max over chunk windows done on device
-            elif n_out == 1:
+            if n_out == 1:
                 hist, cnt = self._h(mdl)
-                pred = (hist[(int(cnt[0]) - 1) % 30] if cnt[0] > 0 else np.zeros(B, np.float32))[:, None]
+                prev = np.where(cnt > 0, hist[(cnt - 1) % 30, ar], np.float32(0.0))
+                pred = np.where(stepped, self._scores[:, col0], prev).astype(np.float32)[:, None]
             else:
                 n_classes = max(int(i) for i in self.class_mapping[mdl].keys())
-                pred = np.zeros((B, n_classes + 1), np.float32)
+                pred = np.zeros((B, max(n_classes + 1, n_out)), np.float32)
+                pred[stepped, :n_out] = self._scores[stepped, col0:col0 + n_out]   # max over chunk windows done on device
             if n_out == 1:
                 predictions[mdl] = pred[:, 0].copy()
                 labels = [mdl]
@@ -345,8 +402,8 @@ class Model:
                 labels = list(self.class_mapping[mdl].values())
                 for int_label, cls in self.class_mapping[mdl].items():
                     predictions[cls] = pred[:, int(int_label)].copy()
-            if mdl in self._vbanks and (n_prepared < CHUNK or n_chunks > self.preprocessor.max_chunks):
-                self._reverify(mdl, predictions, labels)         # otherwise the device verified the step it ran
+            if mdl in self._vbanks and reverify.any():
+                self._reverify(mdl, predictions, labels, reverify)   # otherwise the device verified the step it ran
 
             if self._host_verifiers != {}:
                 for cls in list(predictions.keys()):
@@ -372,19 +429,20 @@ class Model:
                 parent = self.get_parent_model_from_label(lab)
                 nz = predictions[lab] != 0.0
                 if parent in patience.keys():
-                    sc = self._recent(lab, patience[parent])
-                    fail = (sc >= threshold[parent]).sum(axis=0) < patience[parent]
+                    sc, valid = self._recent(lab, patience[parent])
+                    fail = ((sc >= threshold[parent]) & valid).sum(axis=0) < patience[parent]
                     predictions[lab] = np.where(nz & fail, np.float32(0.0), predictions[lab])
                 elif debounce_time > 0 and parent in threshold.keys():
-                    n_frames = int(np.ceil(debounce_time / (n_prepared / 16000)))
-                    rec = self._recent(lab, n_frames)
-                    hit = (rec >= threshold[parent]).sum(axis=0) > 0
+                    with np.errstate(divide="ignore"):
+                        n_frames = np.where(n_prepared > 0, np.ceil(debounce_time / (n_prepared / 16000)), 30)
+                    rec, valid = self._recent(lab, n_frames.astype(np.int64))
+                    hit = ((rec >= threshold[parent]) & valid).sum(axis=0) > 0
                     predictions[lab] = np.where(nz & (predictions[lab] >= threshold[parent]) & hit,
                                                 np.float32(0.0), predictions[lab])
 
         for lab in predictions.keys():
             hist, cnt = self._h(lab)
-            hist[int(cnt[0]) % 30] = predictions[lab]
+            hist[cnt % 30, ar] = predictions[lab]
             cnt += 1
 
         out = {k: (float(v[0]) if single else v) for k, v in predictions.items()}

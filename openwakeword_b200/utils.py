@@ -98,6 +98,8 @@ class AudioFeatures:
         self.feature_buffer_max_len = 120
         self._feature_init = None if feature_init is None else np.asarray(feature_init, np.float32)
         self._streams_ready = False
+        self._pending = np.zeros((self.n_streams, 0), np.int16)
+        self._rpend = None
         self._verifier_banks = False    # set by Model once the handle has a verifier bank (split calls skip the banks)
         # the three session callables of the reference (utils.py:87,93), numpy in / numpy out
         self.melspec_model_predict = self._melspec_model_predict
@@ -122,7 +124,35 @@ class AudioFeatures:
         self.ctx.reset(stream_ids, np.asarray(fi, np.float32))
         if stream_ids is None:
             self._pending = np.zeros((self.n_streams, 0), np.int16)
+            self._rpend = None
             self.accumulated_samples = 0
+        else:
+            buf, lens = self._ragged_pending()
+            lens[np.asarray(stream_ids, np.int64)] = 0
+            self._set_ragged_pending(buf, lens)
+
+    # ---- per-stream remainders: `_pending` [B, L] while every stream holds the same number of samples, else
+    #      `_rpend` = (int16 [B, 1279], lengths [B]) ----
+    def _ragged_pending(self):
+        if self._rpend is not None:
+            return self._rpend[0].copy(), self._rpend[1].copy()
+        buf = np.zeros((self.n_streams, CHUNK - 1), np.int16)
+        L = self._pending.shape[1]
+        buf[:, :L] = self._pending
+        return buf, np.full(self.n_streams, L, np.int64)
+
+    def _set_ragged_pending(self, buf, lens):
+        if (lens == lens[0]).all():
+            self._pending = buf[:, :int(lens[0])].copy()
+            self._rpend = None
+        else:
+            self._rpend = (buf, lens)
+
+    @property
+    def pending_ragged(self):
+        """True while the streams hold different numbers of not yet stepped samples (lockstep input then runs through
+        the ragged path)."""
+        return self._rpend is not None
 
     # ---- session-shaped calls ----
     def _melspec_model_predict(self, x):
@@ -226,6 +256,12 @@ class AudioFeatures:
         Returns (n_prepared_samples, n_chunks_run).  Scores land in scores_out when a step ran."""
         self._ensure_streams()
         x = self._coerce(x)
+        if scores_out is None:
+            scores_out = np.empty((self.n_streams, max(self.ctx.n_outputs, 1)), np.float32)
+        if self._rpend is not None:         # the streams hold different remainders: per-stream accumulation
+            n_prepared, n_chunks, _ = self._streaming_features_ragged(list(x), scores_out)
+            self._last_scores = scores_out
+            return n_prepared, n_chunks
         buf = np.concatenate((self._pending, x), axis=1) if self._pending.shape[1] else x
         total = buf.shape[1]
         if total >= CHUNK:
@@ -262,6 +298,49 @@ class AudioFeatures:
         self.accumulated_samples = 0
         self._last_scores = scores_out
         return ready.shape[1], n_chunks
+
+    def _streaming_features_ragged(self, xs, scores_out):
+        """Chunk accumulation of utils.py:409-452 per stream: stream b gets xs[b] (1-D int16, any length), steps the
+        whole chunks of its remainder + xs[b] and keeps the rest.  One oww_step_host_ragged call per max_chunks chunks.
+        Returns (n_prepared [B], n_chunks [B], split): n_prepared as the reference's AudioFeatures.__call__ returns it
+        (the samples stepped, or the samples accumulated when no chunk was stepped); rows of scores_out of streams that
+        stepped nothing are not written.  split: a stream stepped more than max_chunks chunks, so the calls ran without
+        the verifier banks (the caller verifies the max over all chunk windows)."""
+        self._ensure_streams()
+        B = self.n_streams
+        buf, lens = self._ragged_pending()
+        tot = lens + np.array([x.shape[0] for x in xs], np.int64)
+        n_chunks = tot // CHUNK
+        ready = [np.concatenate((buf[b, :lens[b]], xs[b])) if lens[b] else xs[b] for b in range(B)]
+        new_buf = np.zeros_like(buf)
+        new_lens = tot - n_chunks * CHUNK
+        for b in range(B):
+            if new_lens[b]:
+                new_buf[b, :new_lens[b]] = ready[b][n_chunks[b] * CHUNK:]
+        split = bool((n_chunks > self.max_chunks).any())
+        part = np.empty_like(scores_out) if split else scores_out
+        if split and self._verifier_banks:
+            self.ctx.enable_verifiers(False)
+        try:
+            done = np.zeros(B, np.int64)
+            while (done < n_chunks).any():
+                c = np.minimum(n_chunks - done, self.max_chunks).astype(np.int32)
+                pcm = np.zeros((B, int(c.max()) * CHUNK), np.int16)
+                for b in np.nonzero(c)[0]:
+                    pcm[b, :c[b] * CHUNK] = ready[b][done[b] * CHUNK:(done[b] + c[b]) * CHUNK]
+                first = (done == 0) & (c > 0)
+                self.ctx.step_host_ragged(pcm, c, part)
+                if split:               # per stream the max over all its parts
+                    scores_out[first] = part[first]
+                    later = (done > 0) & (c > 0)
+                    scores_out[later] = np.maximum(scores_out[later], part[later])
+                done += c
+        finally:
+            if split and self._verifier_banks:
+                self.ctx.enable_verifiers(True)
+        self._set_ragged_pending(new_buf, new_lens)
+        n_prepared = np.where(n_chunks > 0, n_chunks * CHUNK, tot)
+        return n_prepared, n_chunks, split
 
     def __call__(self, x):
         return self._streaming_features(x)[0]
