@@ -269,7 +269,8 @@ int oww_debug_layer(oww_ctx* ctx, const float* d_windows, int n, int layer, floa
  * (struct IncPlan of csrc/oww_internal.h); returns the number of ints written (> 0) or an error.
  * oww_debug_inc_plan: the full 20-layer plan.  oww_debug_inc_cut_plan: n_layers conv layers inside
  * the kernel - 0 or 20 for the full plan, split_from for the cut plan of cnn_mode 3 (the fused kernel
- * stops after the pooled layer split_from - 1).
+ * stops after the pooled layer split_from - 1).  group 0 with a handle: the plan that handle's fused kernel runs,
+ * whose first int is the group size the library chose for its stream count (n_streams, n_layers ignored).
  * Pure host computation (usable without a GPU): tests/test_inc_plan.py replays it in NumPy.          */
 int oww_debug_inc_plan(oww_ctx* ctx, int group, int n_streams, int32_t* out, int max_ints);
 int oww_debug_inc_cut_plan(oww_ctx* ctx, int group, int n_streams, int n_layers, int32_t* out, int max_ints);

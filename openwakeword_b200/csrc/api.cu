@@ -1330,8 +1330,14 @@ int oww_debug_inc_cut_plan(oww_ctx* ctx, int group, int n_streams, int n_layers,
     oww_ctx local;                       // ctx may be NULL: the plan depends only on the fixed layer table
     if (!ctx) { fill_layer_table(&local); ctx = &local; }
     IncPlan P;
-    int rc = oww_inc_build_plan(ctx, group, n_streams, n_layers ? n_layers : OWW_N_CONV, &P);
-    if (rc) return rc;
+    if (group == 0 && ctx != &local) {
+        // the plan the handle's fused kernel runs (its group size as oww_inc_alloc_streams chose it)
+        if (ctx->inc_plan.G == 0) return oww_fail(ctx, OWW_EINVAL, "the handle has no fused-CNN plan (cnn_mode 3 streams)");
+        P = ctx->inc_plan;
+    } else {
+        int rc = oww_inc_build_plan(ctx, group, n_streams, n_layers ? n_layers : OWW_N_CONV, &P);
+        if (rc) return rc;
+    }
     const int n = (int)(sizeof(IncPlan) / sizeof(int32_t));
     if (max_ints < n) return oww_fail(ctx, OWW_EINVAL, "need room for %d ints", n);
     std::memcpy(out, &P, sizeof(IncPlan));
