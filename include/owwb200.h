@@ -144,8 +144,40 @@ int oww_set_verifier_threshold(oww_ctx* ctx, int bank, float threshold);
 int oww_enable_verifiers(oww_ctx* ctx, int enabled);
 int oww_verifier_predict(oww_ctx* ctx, int bank, int slot, const float* d_feats, int n, float* d_out, void* stream);
 
+/* ---- per-stream head banks (a different wake-word model on every stream; each slot replaces one <head>.onnx session
+ *      of Model.model_prediction_function, openwakeword/model.py:137-138,158-159, for the streams assigned to it) -------
+ * A bank holds `capacity` slots, each a head of the one graph shape `desc` (the train.py family, openwakeword/train.py:
+ * 56-83).  Its n_out = desc->dims[n_layers] score columns are appended when the bank is added, in call order with
+ * oww_add_head (oww_n_outputs counts them; banks do not count against the 16 heads of a handle).  In every step, a stream
+ * assigned slot k gets in those columns what head k would give as an ordinary head on that stream (per chunk window,
+ * the max over the windows of a multi-chunk call; held streams of a ragged step are not written); a stream on slot -1
+ * gets 0.0.  A slot runs the tensor-core heads kernel with the operand split, term count and accumulation order of
+ * oww_head_predict, so it equals an ordinary head of the same weights bit for bit where that head runs that kernel
+ * (oww_head_predict in cnn_modes 2/3, and streaming with reserved[0] bit 3).  Gates and custom verifiers apply to
+ * ordinary heads only.  reserved[0] bit 2 (plain fp16 operands) applies to banks; bits 1 and 3 do not.
+ *   oww_add_head_bank        - capacity slots of shape desc, allocated here: per slot the fp16 hi/lo packing of every
+ *                              layer plus the fp32 biases and LayerNorm parameters (415 672 B at 16x96 -> 64 -> 64
+ *                              -> 1, 863 672 B at 16x96 -> 128 -> 128 -> 1, descriptor included).  Every stream starts on slot -1.
+ *                              OWW_EUNSUPPORTED in cnn_mode 0 and for any layer wider than 128.
+ *   oww_load_bank_head       - copy a head (pack_head_blob layout of the bank's shape) into a slot.  Synchronises the
+ *                              device first, so steps already in flight keep the old weights.
+ *   oww_assign_bank_head     - stream-ordered, allocation-free: stream h_stream_ids[i] (NULL = all streams, then n is the
+ *                              stream count) uses slot h_slots[i] (-1 = none; a slot must hold a head) from the next step
+ *                              enqueued on `stream` or submitted with oww_step_host*.  The host sorts the streams by slot
+ *                              and stages the work table through pinned memory (it waits for the copy of the previous
+ *                              assignment of the bank).
+ *   oww_set_head_bank_clip_slot - the slot oww_predict_clips / _ragged apply to every clip (-1, the default: zeros)
+ *   oww_bank_head_predict    - stateless: d_feats [n][n_in][96] -> d_out [n][n_out] with the head of `slot`
+ * oww_set_streams resets every assignment to -1; oww_reset / oww_reset_async leave them as they are.  A bad bank,
+ * slot or stream id fails with OWW_EINVAL.  A handle without banks launches nothing for them.                        */
+int oww_add_head_bank(oww_ctx* ctx, const oww_head_desc* desc, int capacity, int* bank_id);
+int oww_load_bank_head(oww_ctx* ctx, int bank, int slot, const float* h_blob, size_t n_floats);
+int oww_assign_bank_head(oww_ctx* ctx, int bank, const int32_t* h_stream_ids, int n, const int32_t* h_slots, void* stream);
+int oww_set_head_bank_clip_slot(oww_ctx* ctx, int bank, int slot);
+int oww_bank_head_predict(oww_ctx* ctx, int bank, int slot, const float* d_feats, int n, float* d_out, void* stream);
+
 int oww_n_heads(const oww_ctx* ctx);
-int oww_n_outputs(const oww_ctx* ctx);          /* total score columns over all heads           */
+int oww_n_outputs(const oww_ctx* ctx);          /* total score columns over all heads and head banks */
 
 /* ---- stateless graph calls (drop-in for the three ORT sessions) --------------------------- */
 /* d_pcm [n_clips][n_samples] int16 -> d_mel [n_clips][T][32], T = (n_samples-512)/160+1.

@@ -47,6 +47,11 @@ _SIGNATURES = {
     "oww_set_verifier_threshold": (C.c_int, [_P, C.c_int, C.c_float]),
     "oww_enable_verifiers": (C.c_int, [_P, C.c_int]),
     "oww_verifier_predict": (C.c_int, [_P, C.c_int, C.c_int, _P, C.c_int, _P, _P]),
+    "oww_add_head_bank": (C.c_int, [_P, C.POINTER(HeadDesc), C.c_int, C.POINTER(C.c_int)]),
+    "oww_load_bank_head": (C.c_int, [_P, C.c_int, C.c_int, _P, C.c_size_t]),
+    "oww_assign_bank_head": (C.c_int, [_P, C.c_int, _P, C.c_int, _P, _P]),
+    "oww_set_head_bank_clip_slot": (C.c_int, [_P, C.c_int, C.c_int]),
+    "oww_bank_head_predict": (C.c_int, [_P, C.c_int, C.c_int, _P, C.c_int, _P, _P]),
     "oww_n_heads": (C.c_int, [_P]),
     "oww_n_outputs": (C.c_int, [_P]),
     "oww_melspectrogram": (C.c_int, [_P, _P, C.c_int, C.c_int, _P, C.c_int, _P]),
@@ -205,17 +210,50 @@ class Context:
         blob = np.ascontiguousarray(blob, np.float32)
         self._check(self.lib.oww_load_embedding(self.h, _ptr(blob), blob.size))
 
-    def add_head(self, n_in, dims, layernorm, final_act, blob):
+    @staticmethod
+    def _desc(n_in, dims, layernorm, final_act):
         d = HeadDesc(n_in=n_in, n_layers=len(dims) - 1, layernorm=int(layernorm), final_act=int(final_act))
         if len(dims) - 1 > MAX_HEAD_LAYERS:
             raise NativeError("too many head layers")
         for i, v in enumerate(dims):
             d.dims[i] = int(v)
+        return d
+
+    def add_head(self, n_in, dims, layernorm, final_act, blob):
+        d = self._desc(n_in, dims, layernorm, final_act)
         blob = np.ascontiguousarray(blob, np.float32)
         hid = C.c_int(-1)
         self._check(self.lib.oww_add_head(self.h, C.byref(d), _ptr(blob), blob.size, C.byref(hid)))
         self._head_n_in.append(int(n_in))
         return hid.value
+
+    # ---- per-stream head banks (include/owwb200.h, oww_add_head_bank) ----
+    def add_head_bank(self, n_in, dims, layernorm, final_act, capacity):
+        """`capacity` slots of one head shape; its n_out columns are appended to the score row."""
+        d = self._desc(n_in, dims, layernorm, final_act)
+        bid = C.c_int(-1)
+        self._check(self.lib.oww_add_head_bank(self.h, C.byref(d), int(capacity), C.byref(bid)))
+        return bid.value
+
+    def load_bank_head(self, bank, slot, blob):
+        """blob: weights.pack_head_blob of a head of the bank's shape (synchronises the device)."""
+        blob = np.ascontiguousarray(blob, np.float32)
+        self._check(self.lib.oww_load_bank_head(self.h, int(bank), int(slot), _ptr(blob), blob.size))
+
+    def assign_bank_head(self, bank, stream_ids, slots, stream=None):
+        """Stream-ordered like assign_verifier: stream_ids None = all streams; slot -1 = none (zeros)."""
+        ids = None if stream_ids is None else np.ascontiguousarray(stream_ids, np.int32)
+        sl = np.ascontiguousarray(slots, np.int32)
+        n = sl.size if ids is None else ids.size
+        if sl.size != n:
+            raise ValueError(f"{sl.size} slots for {n} streams")
+        self._check(self.lib.oww_assign_bank_head(self.h, int(bank), _ptr(ids), n, _ptr(sl), stream))
+
+    def set_head_bank_clip_slot(self, bank, slot):
+        self._check(self.lib.oww_set_head_bank_clip_slot(self.h, int(bank), int(slot)))
+
+    def bank_head_predict(self, bank, slot, d_feats, n, d_out, stream=None):
+        self._check(self.lib.oww_bank_head_predict(self.h, int(bank), int(slot), _ptr(d_feats), int(n), _ptr(d_out), stream))
 
     def add_gate(self, main_head, verifier_head, threshold=0.5):
         self._check(self.lib.oww_add_gate(self.h, int(main_head), int(verifier_head), float(threshold)))

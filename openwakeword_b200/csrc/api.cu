@@ -358,6 +358,7 @@ int step_core(oww_ctx* ctx, const int16_t* d_pcm, int64_t pcm_stride, int n_chun
         if (heads_inside) oww_feat16_invalidate(ctx);
         else if ((rc = oww_feat16_advance(ctx, 1, s))) return rc;
         if (!heads_inside && (rc = oww_heads_all(ctx, fs0, B, d_scores, out_stride, 0, s))) return rc;
+        if (heads_inside && (rc = oww_head_banks_launch(ctx, fs0, B, d_scores, out_stride, 0, s))) return rc;
         if ((rc = oww_verifiers_apply(ctx, fs0, B, d_scores, out_stride, false, s))) return rc;
         if (ev) {
             if (heads_inside) ctx->ev_fused[slot] = 1;
@@ -528,6 +529,7 @@ int step_ragged_core(oww_ctx* ctx, const int16_t* d_pcm, int64_t pcm_stride, con
         if ((rc = carry_launch(ctx, d_ord, below[1], s))) return rc;
         if (heads_inside) {
             oww_feat16_invalidate(ctx);
+            if ((rc = oww_head_banks_launch(ctx, fs0, B, d_scores, out_stride, 0, s, d_cnt))) return rc;
         } else {
             if ((rc = oww_feat16_advance(ctx, 1, s))) return rc;
             if ((rc = oww_feat16_resync(ctx, d_ord, below[1], s))) return rc;     // held: their window did not move
@@ -671,6 +673,7 @@ void oww_destroy(oww_ctx* ctx) {
     cudaSetDevice(ctx->device);
     free_streams(ctx);
     oww_heads_grp_free(ctx);
+    oww_head_banks_free(ctx);
     cudaFree(ctx->d_window); cudaFree(ctx->d_twiddle); cudaFree(ctx->d_mel_start); cudaFree(ctx->d_mel_len);
     cudaFree(ctx->d_mel_w); cudaFree(ctx->d_emb_blob); cudaFree(ctx->d_tc_w); cudaFree(ctx->d_tc_sb);
     cudaFree(ctx->d_tc_w3); cudaFree(ctx->d_tc_sb3);
@@ -717,20 +720,23 @@ int oww_load_embedding(oww_ctx* ctx, const float* h_blob, size_t n_floats) {
     return oww_inc_setup(ctx, h_blob);
 }
 
-int oww_add_head(oww_ctx* ctx, const oww_head_desc* desc, const float* h_blob, size_t n_floats, int* head_id) {
-    if (!ctx || !desc || !h_blob) return oww_fail(ctx, OWW_EINVAL, "null argument");
+}  // extern "C"
+
+int oww_check_head_desc(oww_ctx* ctx, const oww_head_desc* desc) {
     if (desc->n_layers < 1 || desc->n_layers > OWW_MAX_HEAD_LAYERS)
         return oww_fail(ctx, OWW_EUNSUPPORTED, "head has %d Linear layers (1..%d supported)", desc->n_layers, OWW_MAX_HEAD_LAYERS);
     if (desc->n_in < 1 || desc->dims[0] != desc->n_in * OWW_EMBEDDING_DIM)
         return oww_fail(ctx, OWW_EINVAL, "dims[0]=%d must equal n_in*96=%d", desc->dims[0], desc->n_in * OWW_EMBEDDING_DIM);
     if (desc->final_act < 0 || desc->final_act > 4) return oww_fail(ctx, OWW_EINVAL, "bad final_act");
-    if (ctx->heads.size() >= 16) return oww_fail(ctx, OWW_EUNSUPPORTED, "at most 16 heads per handle");
-    Head h;
+    return OWW_OK;
+}
+
+int oww_stage_head(oww_ctx* ctx, const oww_head_desc* desc, const float* h_blob, size_t n_floats, Head& h,
+                   std::vector<float>& staged) {
     h.desc = *desc;
     // Device layout: the caller's tensors in order, each starting on a 16-byte boundary (the fused step kernel streams
     // weight rows with bulk copies, which need 16-byte aligned sources).  `src` walks the packed host blob.
     size_t off = 0, src = 0;
-    std::vector<float> staged;
     auto place = [&](size_t n) {
         off = (off + 3) & ~(size_t)3;
         const size_t at = off;
@@ -752,13 +758,24 @@ int oww_add_head(oww_ctx* ctx, const oww_head_desc* desc, const float* h_blob, s
         } else { h.g_off.push_back(0); h.h_off.push_back(0); }
     }
     if (src != n_floats) return oww_fail(ctx, OWW_EINVAL, "head blob has %zu floats, descriptor needs %zu", n_floats, src);
+    return OWW_OK;
+}
+
+extern "C" {
+
+int oww_add_head(oww_ctx* ctx, const oww_head_desc* desc, const float* h_blob, size_t n_floats, int* head_id) {
+    if (!ctx || !desc || !h_blob) return oww_fail(ctx, OWW_EINVAL, "null argument");
+    int rc = oww_check_head_desc(ctx, desc);
+    if (rc) return rc;
+    if (ctx->heads.size() >= 16) return oww_fail(ctx, OWW_EUNSUPPORTED, "at most 16 heads per handle");
+    Head h;
+    std::vector<float> staged;
+    if ((rc = oww_stage_head(ctx, desc, h_blob, n_floats, h, staged))) return rc;
     OWW_CUDA(ctx, cudaSetDevice(ctx->device));
     OWW_CUDA(ctx, cudaMalloc(&h.d_blob, staged.size() * sizeof(float)));
     OWW_CUDA(ctx, cudaMemcpy(h.d_blob, staged.data(), staged.size() * sizeof(float), cudaMemcpyHostToDevice));
-    {   // tensor-core packing of the first layer (heads_tc.cu); heads it does not cover keep tc_ok == false
-        int rc = oww_heads_tc_pack(ctx, h, staged.data());
-        if (rc) { cudaFree(h.d_blob); return rc; }
-    }
+    // tensor-core packing of the first layer (heads_tc.cu); heads it does not cover keep tc_ok == false
+    if ((rc = oww_heads_tc_pack(ctx, h, staged.data()))) { cudaFree(h.d_blob); return rc; }
     h.n_out = desc->dims[desc->n_layers];
     h.col0 = ctx->n_out_total;
     ctx->n_out_total += h.n_out;
@@ -842,6 +859,7 @@ int oww_set_streams(oww_ctx* ctx, int n_streams) {
     if (ctx->cfg.cnn_mode == OWW_CNN_TC_INCREMENTAL && (rc = oww_late_alloc(ctx))) return rc;
     if (ctx->cfg.cnn_mode == OWW_CNN_TC_INCREMENTAL && (rc = oww_inc_alloc_streams(ctx))) return rc;
     if ((rc = oww_verifiers_alloc_streams(ctx))) return rc;         // every stream starts without a verifier
+    if ((rc = oww_head_banks_alloc_streams(ctx))) return rc;        // ... and without a bank head
     return oww_reset(ctx, nullptr, B, nullptr, OWW_INIT_FEATURE_ROWS);
 }
 
@@ -1139,7 +1157,7 @@ int oww_predict_clips_ragged(oww_ctx* ctx, const int16_t* d_pcm, const int64_t* 
         if (h_offsets[i + 1] < h_offsets[i] || h_offsets[i + 1] - h_offsets[i] > INT32_MAX - 2 * (int64_t)pad_samples)
             return oww_fail(ctx, OWW_EINVAL, "offsets[%d..%d] = %lld, %lld are not monotone (or the clip is too long)", i, i + 1,
                             (long long)h_offsets[i], (long long)h_offsets[i + 1]);
-    if (ctx->heads.empty() || n_clips == 0) return OWW_OK;
+    if (ctx->n_out_total == 0 || n_clips == 0) return OWW_OK;
     OWW_CUDA(ctx, cudaSetDevice(ctx->device));
     cudaStream_t s = (cudaStream_t)stream;
     const int c = chunk_size, n_out = ctx->n_out_total;

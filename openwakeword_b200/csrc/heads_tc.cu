@@ -1,6 +1,7 @@
 // K3 (tensor-core path, per head): the wake-word heads as a chain of wgmma GEMMs, one CTA per (64 samples, head).
 // Streaming steps and bulk clips run heads_grp.cu (A operand from the fp16 mirror of the feature rings); this kernel
-// serves stateless calls on caller-supplied features and the heads the mirror path does not cover.
+// serves stateless calls on caller-supplied features, the heads the mirror path does not cover and the per-stream head
+// banks (heads_tc_kernel<true>: one CTA per work item of up to 64 streams that share a slot; bottom of this file).
 //
 // Same graphs as heads.cu (reference: <head>.onnx sessions, openwakeword/model.py:137-138,153-159,287-302 of the
 // original project; family openwakeword/train.py:56-83,144-165).  heads.cu tiles 8 or 32 streams per CTA and runs every
@@ -52,15 +53,35 @@ struct HeadsTcArgs {
     int n; float* out; int out_stride; int combine_max;
     int n_terms;                  // 1: hi*hi   3: + lo*hi + hi*lo (default)
     int stages, stage_bytes;
+    // head bank (heads_tc_kernel<true>): CTA i runs item items[i] = {slot, first, rows}, the streams perm[first ..
+    // first + rows) with the head slots[slot]; slot -1 only stores zeros in the columns of head[0] (the bank's shape).
+    // step != nullptr: streams with step[b] == 0 are not written.
+    const int4* items; const int* perm; const HtHead* slots; const int* step;
 };
 
+template <bool kBank>
 __global__ void __launch_bounds__(kHtThreads, 1) heads_tc_kernel(const __grid_constant__ HeadsTcArgs a) {
     extern __shared__ __align__(128) uint8_t smem[];
-    const HtHead& HH = a.head[blockIdx.y];
+    const HtHead* hp = &a.head[blockIdx.y];
+    int s0 = blockIdx.x * kHtTile, n_rows = 0;
+    if constexpr (kBank) {
+        const int4 it = a.items[blockIdx.x];
+        s0 = it.y; n_rows = it.z;
+        if (it.x < 0) {
+            const HeadDev& D0 = a.head[0].dev;
+            const int n_out = D0.dims[D0.n_layers];
+            for (int i = threadIdx.x; i < n_rows * n_out; i += blockDim.x) {
+                const int r = i / n_out, b = a.perm[s0 + r];
+                if (!a.step || a.step[b] != 0) a.out[(int64_t)b * a.out_stride + D0.col0 + (i - r * n_out)] = 0.f;
+            }
+            return;
+        }
+        hp = a.slots + it.x;
+    }
+    const HtHead& HH = *hp;
     const HeadDev& H = HH.dev;
     const int NP = HH.L[0].NP;
     const int n_in = H.n_in, n_layers = H.n_layers;
-    const int s0 = blockIdx.x * kHtTile;
     const int S = a.stages;
     uint64_t* bars = reinterpret_cast<uint64_t*>(smem);
     uint8_t* stage0 = smem + 1024;
@@ -135,7 +156,13 @@ __global__ void __launch_bounds__(kHtThreads, 1) heads_tc_kernel(const __grid_co
         __syncwarp();
         if (lane == 0) mbar_arrive(acc_done);
         const int r = threadIdx.x;
-        float* o = (r < kHtTile && s0 + r < a.n) ? a.out + (int64_t)(s0 + r) * a.out_stride + H.col0 : nullptr;
+        float* o = nullptr;
+        if constexpr (kBank) {
+            const int b = r < n_rows ? a.perm[s0 + r] : -1;
+            if (b >= 0 && (!a.step || a.step[b] != 0)) o = a.out + (int64_t)b * a.out_stride + H.col0;
+        } else {
+            o = (r < kHtTile && s0 + r < a.n) ? a.out + (int64_t)(s0 + r) * a.out_stride + H.col0 : nullptr;
+        }
         // the ring is dead once every stage has been consumed by the MMAs above (all of this warpgroup's)
         named_bar_sync(1, 128);
         hm_layers(acc, NP, H, HH.L, a.n_terms, stage0, smem_u32(w_next), wn_full, acc_done, 1, o, a.combine_max);
@@ -143,9 +170,14 @@ __global__ void __launch_bounds__(kHtThreads, 1) heads_tc_kernel(const __grid_co
         // ===================== converters: fp32 ring rows -> fp16 hi/lo A tiles =====================
         // thread = (row 8*w + lane%8, octet quad lane/8): three octets (32 B of fp32 each) per feature row
         const int row = 8 * (warp - kHtProducer - 1) + (lane & 7), jq = lane >> 3;
-        const int s = s0 + row;
         float4 buf[2][6];
-        const FeatRows rows_of = s < a.n ? feat_rows(a.src, n_in, s) : FeatRows{nullptr, 0, -1};
+        FeatRows rows_of{nullptr, 0, -1};
+        if constexpr (kBank) {
+            if (row < n_rows) rows_of = feat_rows(a.src, n_in, a.perm[s0 + row]);
+        } else {
+            const int s = s0 + row;
+            if (s < a.n) rows_of = feat_rows(a.src, n_in, s);
+        }
         auto load = [&](int c, float4* v) {
             const float* p = (c < n_in && rows_of.base) ? feat_row(rows_of, c) : nullptr;
 #pragma unroll
@@ -213,14 +245,15 @@ void pack_block(const float* w, int K, int D, int k0, int Kp, int NP, float sc, 
             }
 }
 
-}  // namespace
+// a head the tensor-core kernel covers: every Linear layer at most 128 wide (hidden buffers / register accumulators)
+bool tc_covers(const oww_head_desc& d) {
+    for (int l = 1; l <= d.n_layers; ++l) if (d.dims[l] > 128) return false;
+    return true;
+}
 
-// Host side: pack every Linear layer of a head for the tensor-core kernel (layer 0 in blocks of one feature row).
-int oww_heads_tc_pack(oww_ctx* ctx, Head& h, const float* blob /* staging in device layout: tensors at h.w_off[] */) {
+// pack every Linear layer of a head the kernel covers (layer 0 in blocks of one feature row) -> packed, h.tc_layers
+void pack_layers(Head& h, const float* blob, std::vector<__half>& packed) {
     const int n_in = h.desc.n_in, nl = h.desc.n_layers;
-    h.tc_ok = false;
-    for (int l = 1; l <= nl; ++l) if (h.desc.dims[l] > 128) return OWW_OK;     // hidden buffers / register accumulators are 128 wide
-    std::vector<__half> packed;
     h.tc_layers.assign(nl, Head::TcLayer{});
     for (int l = 0; l < nl; ++l) {
         const int K = h.desc.dims[l], D = h.desc.dims[l + 1];
@@ -240,6 +273,16 @@ int oww_heads_tc_pack(oww_ctx* ctx, Head& h, const float* blob /* staging in dev
         T.w_bytes = (uint32_t)(n_blocks * per * sizeof(__half));
         while (packed.size() % 64) packed.push_back(__float2half(0.f));    // 128-byte aligned blocks for the bulk copies
     }
+}
+
+}  // namespace
+
+// Host side: pack every Linear layer of a head for the tensor-core kernel.
+int oww_heads_tc_pack(oww_ctx* ctx, Head& h, const float* blob /* staging in device layout: tensors at h.w_off[] */) {
+    h.tc_ok = false;
+    if (!tc_covers(h.desc)) return OWW_OK;
+    std::vector<__half> packed;
+    pack_layers(h, blob, packed);
     cudaFree(h.d_w1_tc); h.d_w1_tc = nullptr;
     OWW_CUDA(ctx, cudaMalloc(&h.d_w1_tc, packed.size() * sizeof(__half)));
     OWW_CUDA(ctx, cudaMemcpy(h.d_w1_tc, packed.data(), packed.size() * sizeof(__half), cudaMemcpyHostToDevice));
@@ -276,7 +319,9 @@ __global__ void max_combine_kernel(float* dst, const float* src, int n, int cols
 }  // namespace
 
 int oww_heads_all(oww_ctx* ctx, const FeatSrc& src, int n, float* d_out, int out_stride, int combine_max, cudaStream_t s) {
-    if (ctx->heads.empty() || n <= 0) return OWW_OK;
+    if (ctx->heads.empty() || n <= 0) {
+        return n > 0 ? oww_head_banks_launch(ctx, src, n, d_out, out_stride, combine_max, s) : OWW_OK;
+    }
     uint32_t tc_mask = 0, cc_mask = 0;
     for (int i = 0; i < (int)ctx->heads.size(); ++i) {
         if (oww_heads_tc_supported(ctx, i)) tc_mask |= 1u << i; else cc_mask |= 1u << i;
@@ -308,6 +353,7 @@ int oww_heads_all(oww_ctx* ctx, const FeatSrc& src, int n, float* d_out, int out
     }
     if (tc_mask && (rc = oww_heads_tc_launch(ctx, -1, src, n, out, stride, 0, comb, s, tc_mask))) return rc;
     if (cc_mask && (rc = oww_heads_launch(ctx, -1, src, n, out, stride, 0, comb, s, cc_mask))) return rc;
+    if ((rc = oww_head_banks_launch(ctx, src, n, out, stride, comb, s))) return rc;
     if (!ctx->gates.empty()) {
         const int total = n * (int)ctx->gates.size();
         OWW_CUDA(ctx, oww_launch_pdl(ctx->late_pdl, gate_kernel, dim3((total + 255) / 256), dim3(256), 0, s, out, n, stride,
@@ -319,6 +365,24 @@ int oww_heads_all(oww_ctx* ctx, const FeatSrc& src, int n, float* d_out, int out
         max_combine_kernel<<<(total + 255) / 256, 256, 0, s>>>(d_out, ctx->d_scores_tmp, n, ctx->n_out_total, out_stride);
         OWW_LAUNCH_CHECK(ctx);
     }
+    return OWW_OK;
+}
+
+// stage ring for first-layer tiles of up to np_max columns, then the launch
+template <bool kBank>
+static int ht_run(oww_ctx* ctx, HeadsTcArgs& a, int np_max, dim3 grid, cudaStream_t s) {
+    a.n_terms = ctx->tc_heads_terms;
+    a.stage_bytes = 2 * kHtABytes + 2 * 12 * np_max * 16;
+    a.stages = (kHtSmem - 1024) / a.stage_bytes;
+    if (a.stages > kHtMaxStages) a.stages = kHtMaxStages;
+    if (a.stages < 2) return oww_fail(ctx, OWW_EUNSUPPORTED, "tensor-core heads: stage of %d bytes does not fit twice", a.stage_bytes);
+    if (!ctx->heads_tc_attr_set) {
+        OWW_CUDA(ctx, cudaFuncSetAttribute(heads_tc_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, kHtSmem));
+        OWW_CUDA(ctx, cudaFuncSetAttribute(heads_tc_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, kHtSmem));
+        ctx->heads_tc_attr_set = true;
+    }
+    heads_tc_kernel<kBank><<<grid, kHtThreads, kHtSmem, s>>>(a);
+    OWW_LAUNCH_CHECK(ctx);
     return OWW_OK;
 }
 
@@ -360,17 +424,285 @@ int oww_heads_tc_launch(oww_ctx* ctx, int head_id, const FeatSrc& src, int n, fl
         if (h.tc_layers[0].NP > np_max) np_max = h.tc_layers[0].NP;
     }
     a.src = src; a.n = n; a.out = d_out; a.out_stride = out_stride; a.combine_max = combine_max;
-    a.n_terms = ctx->tc_heads_terms;
-    a.stage_bytes = 2 * kHtABytes + 2 * 12 * np_max * 16;
-    a.stages = (kHtSmem - 1024) / a.stage_bytes;
-    if (a.stages > kHtMaxStages) a.stages = kHtMaxStages;
-    if (a.stages < 2) return oww_fail(ctx, OWW_EUNSUPPORTED, "tensor-core heads: stage of %d bytes does not fit twice", a.stage_bytes);
-    if (!ctx->heads_tc_attr_set) {
-        OWW_CUDA(ctx, cudaFuncSetAttribute(heads_tc_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, kHtSmem));
-        ctx->heads_tc_attr_set = true;
+    return ht_run<false>(ctx, a, np_max, dim3((n + kHtTile - 1) / kHtTile, nh), s);
+}
+
+// ================================ head banks ================================
+namespace {
+
+// the kernel descriptor of slot k (its unscale factors: per layer, from that slot's weights)
+HtHead bank_slot_head(const HeadBank& b, int k, const float* unscale) {
+    HtHead t;
+    std::memset(&t, 0, sizeof(t));
+    const oww_head_desc& d = b.shape.desc;
+    HeadDev& H = t.dev;
+    H.blob = b.d_p + (size_t)k * b.p_floats;
+    H.n_in = d.n_in; H.n_layers = d.n_layers; H.layernorm = d.layernorm; H.final_act = d.final_act;
+    for (int l = 0; l <= d.n_layers; ++l) H.dims[l] = d.dims[l];
+    for (int l = 0; l < d.n_layers; ++l) {
+        H.b_off[l] = b.p_off[3 * l]; H.g_off[l] = b.p_off[3 * l + 1]; H.h_off[l] = b.p_off[3 * l + 2];
+        const Head::TcLayer& T = b.shape.tc_layers[l];
+        t.L[l] = HtLayer{T.K, T.D, T.Kp, T.NP, T.w_off, T.w_bytes, unscale ? unscale[l] : 1.f};
     }
-    dim3 grid((n + kHtTile - 1) / kHtTile, nh);
-    heads_tc_kernel<<<grid, kHtThreads, kHtSmem, s>>>(a);
-    OWW_LAUNCH_CHECK(ctx);
+    H.col0 = b.shape.col0;
+    t.w = b.d_w + (size_t)k * b.w_bytes;
+    return t;
+}
+
+const HtHead& host_slot(const HeadBank& b, int k) { return reinterpret_cast<const HtHead*>(b.h_slots.data())[k]; }
+
+// items of at most kHtTile streams per slot, streams ordered by slot (-1 first) -> h[0 .. 4B) items, h[4B .. 5B) ids
+int build_items(const std::vector<int>& assign, int* h) {
+    const int B = (int)assign.size();
+    int* perm = h + 4 * B;
+    for (int b = 0; b < B; ++b) perm[b] = b;
+    std::stable_sort(perm, perm + B, [&](int x, int y) { return assign[x] < assign[y]; });
+    int n = 0;
+    for (int i = 0; i < B;) {
+        int j = i;
+        while (j < B && assign[perm[j]] == assign[perm[i]] && j - i < kHtTile) ++j;
+        h[4 * n] = assign[perm[i]]; h[4 * n + 1] = i; h[4 * n + 2] = j - i; h[4 * n + 3] = 0;
+        ++n; i = j;
+    }
+    return n;
+}
+
+// upload the item table of b.assign on s through the pinned staging (the copy of the previous upload has run)
+int upload_items(oww_ctx* ctx, HeadBank& b, cudaStream_t s) {
+    const int B = (int)b.assign.size();
+    OWW_CUDA(ctx, cudaEventSynchronize(b.stage_ev));
+    b.n_items = build_items(b.assign, b.h_stage);
+    OWW_CUDA(ctx, cudaMemcpyAsync(b.d_table, b.h_stage, (size_t)5 * B * sizeof(int), cudaMemcpyHostToDevice, s));
+    OWW_CUDA(ctx, cudaEventRecord(b.stage_ev, s));
     return OWW_OK;
 }
+
+void bank_free_streams(HeadBank& b) {
+    if (b.stage_ev) cudaEventSynchronize(b.stage_ev);
+    cudaFree(b.d_table); cudaFreeHost(b.h_stage);
+    b.d_table = nullptr; b.h_stage = nullptr; b.assign.clear(); b.n_items = 0;
+}
+
+int bank_alloc_streams(oww_ctx* ctx, HeadBank& b) {
+    bank_free_streams(b);
+    const int B = ctx->n_streams;
+    if (B <= 0) return OWW_OK;
+    if (!b.stage_ev) OWW_CUDA(ctx, cudaEventCreateWithFlags(&b.stage_ev, cudaEventDisableTiming));
+    OWW_CUDA(ctx, cudaMalloc(&b.d_table, (size_t)5 * B * sizeof(int)));
+    OWW_CUDA(ctx, cudaMallocHost(&b.h_stage, (size_t)5 * B * sizeof(int)));
+    b.assign.assign(B, -1);
+    int rc = upload_items(ctx, b, nullptr);
+    if (rc) return rc;
+    OWW_CUDA(ctx, cudaEventSynchronize(b.stage_ev));
+    return OWW_OK;
+}
+
+int check_bank(oww_ctx* ctx, int bank) {
+    if (!ctx) return OWW_EINVAL;
+    if (bank < 0 || bank >= (int)ctx->head_banks.size()) return oww_fail(ctx, OWW_EINVAL, "bad head bank %d", bank);
+    return OWW_OK;
+}
+
+int check_slot(oww_ctx* ctx, const HeadBank& b, int slot, bool none_ok) {
+    if (none_ok && slot == -1) return OWW_OK;
+    if (slot < 0 || slot >= b.capacity)
+        return oww_fail(ctx, OWW_EINVAL, "slot %d outside [%d,%d)", slot, none_ok ? -1 : 0, b.capacity);
+    if (!b.loaded[slot]) return oww_fail(ctx, OWW_EINVAL, "slot %d holds no head (oww_load_bank_head)", slot);
+    return OWW_OK;
+}
+
+}  // namespace
+
+int oww_head_banks_launch(oww_ctx* ctx, const FeatSrc& src, int n, float* d_out, int out_stride, int combine_max,
+                          cudaStream_t s, const int* d_step) {
+    if (n <= 0) return OWW_OK;
+    const bool streams = src.count && src.base == ctx->d_feat_ring && n == ctx->n_streams;
+    for (const HeadBank& b : ctx->head_banks) {
+        const int np = std::max(16, b.shape.tc_layers[0].NP);
+        HeadsTcArgs a;
+        std::memset(&a, 0, sizeof(a));
+        a.src = src; a.n = n; a.out = d_out; a.out_stride = out_stride; a.combine_max = combine_max;
+        int rc;
+        if (streams) {
+            // one CTA per item; head[0] carries the bank's columns for the items of unassigned streams
+            a.head[0] = bank_slot_head(b, 0, nullptr);
+            a.items = reinterpret_cast<const int4*>(b.d_table);
+            a.perm = b.d_table + 4 * ctx->n_streams;
+            a.slots = reinterpret_cast<const HtHead*>(b.d_slots);
+            a.step = d_step;
+            rc = ht_run<true>(ctx, a, np, dim3(b.n_items), s);
+        } else if (b.clip_slot >= 0) {       // rows of the bulk path: every row on the clip slot
+            a.head[0] = host_slot(b, b.clip_slot);
+            rc = ht_run<false>(ctx, a, np, dim3((n + kHtTile - 1) / kHtTile), s);
+        } else {
+            OWW_CUDA(ctx, cudaMemset2DAsync(d_out + b.shape.col0, (size_t)out_stride * sizeof(float), 0,
+                                            (size_t)b.shape.n_out * sizeof(float), n, s));
+            rc = OWW_OK;
+        }
+        if (rc) return rc;
+    }
+    return OWW_OK;
+}
+
+int oww_head_banks_alloc_streams(oww_ctx* ctx) {
+    for (HeadBank& b : ctx->head_banks) {
+        int rc = bank_alloc_streams(ctx, b);
+        if (rc) return rc;
+    }
+    return OWW_OK;
+}
+
+void oww_head_banks_free(oww_ctx* ctx) {
+    for (HeadBank& b : ctx->head_banks) {
+        bank_free_streams(b);
+        if (b.stage_ev) cudaEventDestroy(b.stage_ev);
+        cudaFree(b.d_w); cudaFree(b.d_p); cudaFree(b.d_slots);
+    }
+    ctx->head_banks.clear();
+}
+
+extern "C" {
+
+int oww_add_head_bank(oww_ctx* ctx, const oww_head_desc* desc, int capacity, int* bank_id) {
+    if (!ctx || !desc) return oww_fail(ctx, OWW_EINVAL, "null argument");
+    int rc = oww_check_head_desc(ctx, desc);
+    if (rc) return rc;
+    if (ctx->cfg.cnn_mode == OWW_CNN_FP32_WINDOW)
+        return oww_fail(ctx, OWW_EUNSUPPORTED, "head banks run on the tensor cores: not in cnn_mode 0");
+    if (!tc_covers(*desc)) return oww_fail(ctx, OWW_EUNSUPPORTED, "head banks cover layers up to 128 wide");
+    if (capacity < 1 || capacity > (1 << 20)) return oww_fail(ctx, OWW_EINVAL, "capacity %d outside [1, 2^20]", capacity);
+    HeadBank b;
+    b.capacity = capacity;
+    // the packing layout from a zero blob of the shape (every slot's packing has the same layout)
+    size_t n_floats = 0;
+    for (int l = 0; l < desc->n_layers; ++l) {
+        const size_t dout = (size_t)desc->dims[l + 1];
+        n_floats += (size_t)desc->dims[l] * dout + dout + (desc->layernorm && l < desc->n_layers - 1 ? 2 * dout : 0);
+    }
+    {
+        std::vector<float> zeros(n_floats, 0.f), staged;
+        if ((rc = oww_stage_head(ctx, desc, zeros.data(), n_floats, b.shape, staged))) return rc;
+        std::vector<__half> packed;
+        pack_layers(b.shape, staged.data(), packed);
+        b.w_bytes = packed.size() * sizeof(__half);
+    }
+    for (int l = 0; l < desc->n_layers; ++l) {     // bias | gamma | beta per layer, each on a 16-byte boundary
+        const int D = desc->dims[l + 1], Dp = (D + 3) & ~3;
+        const bool ln = desc->layernorm && l < desc->n_layers - 1;
+        b.p_off.push_back((int)b.p_floats); b.p_floats += Dp;
+        b.p_off.push_back(ln ? (int)b.p_floats : 0); b.p_floats += ln ? Dp : 0;
+        b.p_off.push_back(ln ? (int)b.p_floats : 0); b.p_floats += ln ? Dp : 0;
+    }
+    b.shape.n_out = desc->dims[desc->n_layers];
+    b.shape.col0 = ctx->n_out_total;
+    OWW_CUDA(ctx, cudaSetDevice(ctx->device));
+    auto fail = [&](cudaError_t e) {
+        cudaFree(b.d_w); cudaFree(b.d_p); cudaFree(b.d_slots);
+        return oww_fail(ctx, OWW_ENOMEM, "head bank of %d slots: %s", capacity, cudaGetErrorString(e));
+    };
+    cudaError_t e;
+    if ((e = cudaMalloc(&b.d_w, (size_t)capacity * b.w_bytes)) != cudaSuccess) return fail(e);
+    if ((e = cudaMalloc(&b.d_p, (size_t)capacity * b.p_floats * sizeof(float))) != cudaSuccess) return fail(e);
+    if ((e = cudaMalloc(&b.d_slots, (size_t)capacity * sizeof(HtHead))) != cudaSuccess) return fail(e);
+    for (auto& ev : ctx->ver_ev)     // orders oww_assign_bank_head with own_stream, as for the verifier banks
+        if (!ev && (e = cudaEventCreateWithFlags(&ev, cudaEventDisableTiming)) != cudaSuccess) return fail(e);
+    b.h_slots.assign((size_t)capacity * sizeof(HtHead), 0);
+    b.loaded.assign(capacity, 0);
+    ctx->head_banks.push_back(b);
+    ctx->n_out_total += b.shape.n_out;
+    if ((rc = bank_alloc_streams(ctx, ctx->head_banks.back()))) return rc;
+    if (bank_id) *bank_id = (int)ctx->head_banks.size() - 1;
+    return OWW_OK;
+}
+
+int oww_load_bank_head(oww_ctx* ctx, int bank, int slot, const float* h_blob, size_t n_floats) {
+    int rc = check_bank(ctx, bank);
+    if (rc) return rc;
+    if (!h_blob) return oww_fail(ctx, OWW_EINVAL, "null argument");
+    HeadBank& b = ctx->head_banks[bank];
+    if (slot < 0 || slot >= b.capacity) return oww_fail(ctx, OWW_EINVAL, "slot %d outside [0,%d)", slot, b.capacity);
+    Head h;
+    std::vector<float> staged;
+    if ((rc = oww_stage_head(ctx, &b.shape.desc, h_blob, n_floats, h, staged))) return rc;
+    std::vector<__half> packed;
+    pack_layers(h, staged.data(), packed);
+    std::vector<float> prm(b.p_floats, 0.f), unscale(h.desc.n_layers);
+    for (int l = 0; l < h.desc.n_layers; ++l) {
+        const int D = h.desc.dims[l + 1];
+        std::memcpy(prm.data() + b.p_off[3 * l], staged.data() + h.b_off[l], D * sizeof(float));
+        if (h.desc.layernorm && l < h.desc.n_layers - 1) {
+            std::memcpy(prm.data() + b.p_off[3 * l + 1], staged.data() + h.g_off[l], D * sizeof(float));
+            std::memcpy(prm.data() + b.p_off[3 * l + 2], staged.data() + h.h_off[l], D * sizeof(float));
+        }
+        unscale[l] = h.tc_layers[l].unscale;
+    }
+    const HtHead t = bank_slot_head(b, slot, unscale.data());
+    OWW_CUDA(ctx, cudaSetDevice(ctx->device));
+    OWW_CUDA(ctx, cudaDeviceSynchronize());           // steps in flight on any stream finish with the old contents
+    OWW_CUDA(ctx, cudaMemcpy(b.d_w + (size_t)slot * b.w_bytes, packed.data(), b.w_bytes, cudaMemcpyHostToDevice));
+    OWW_CUDA(ctx, cudaMemcpy(b.d_p + (size_t)slot * b.p_floats, prm.data(), b.p_floats * sizeof(float), cudaMemcpyHostToDevice));
+    OWW_CUDA(ctx, cudaMemcpy(reinterpret_cast<HtHead*>(b.d_slots) + slot, &t, sizeof(t), cudaMemcpyHostToDevice));
+    std::memcpy(b.h_slots.data() + (size_t)slot * sizeof(HtHead), &t, sizeof(t));
+    b.loaded[slot] = 1;
+    return OWW_OK;
+}
+
+int oww_assign_bank_head(oww_ctx* ctx, int bank, const int32_t* h_stream_ids, int n, const int32_t* h_slots, void* stream) {
+    int rc = check_bank(ctx, bank);
+    if (rc) return rc;
+    if (!h_slots) return oww_fail(ctx, OWW_EINVAL, "null argument");
+    if (ctx->n_streams <= 0) return oww_fail(ctx, OWW_EINVAL, "oww_set_streams has not been called");
+    HeadBank& b = ctx->head_banks[bank];
+    if (!h_stream_ids) n = ctx->n_streams;
+    if (n <= 0) return OWW_OK;
+    if (n > ctx->n_streams) return oww_fail(ctx, OWW_EINVAL, "more stream ids (%d) than streams (%d)", n, ctx->n_streams);
+    for (int i = 0; i < n; ++i) {
+        if (h_stream_ids && (h_stream_ids[i] < 0 || h_stream_ids[i] >= ctx->n_streams))
+            return oww_fail(ctx, OWW_EINVAL, "stream id %d out of range", h_stream_ids[i]);
+        if ((rc = check_slot(ctx, b, h_slots[i], true))) return rc;
+    }
+    OWW_CUDA(ctx, cudaSetDevice(ctx->device));
+    cudaStream_t s = (cudaStream_t)stream;
+    // the host-buffer steps run on the handle's own stream: order the new table after the steps already submitted there
+    // and before the ones submitted later, as on `stream` itself
+    const bool other = s != ctx->own_stream;
+    if (other) {
+        OWW_CUDA(ctx, cudaEventRecord(ctx->ver_ev[0], ctx->own_stream));
+        OWW_CUDA(ctx, cudaStreamWaitEvent(s, ctx->ver_ev[0], 0));
+    }
+    for (int i = 0; i < n; ++i) b.assign[h_stream_ids ? h_stream_ids[i] : i] = h_slots[i];
+    if ((rc = upload_items(ctx, b, s))) return rc;
+    if (other) {
+        OWW_CUDA(ctx, cudaEventRecord(ctx->ver_ev[1], s));
+        OWW_CUDA(ctx, cudaStreamWaitEvent(ctx->own_stream, ctx->ver_ev[1], 0));
+    }
+    return OWW_OK;
+}
+
+int oww_set_head_bank_clip_slot(oww_ctx* ctx, int bank, int slot) {
+    int rc = check_bank(ctx, bank);
+    if (rc) return rc;
+    if ((rc = check_slot(ctx, ctx->head_banks[bank], slot, true))) return rc;
+    ctx->head_banks[bank].clip_slot = slot;
+    return OWW_OK;
+}
+
+int oww_bank_head_predict(oww_ctx* ctx, int bank, int slot, const float* d_feats, int n, float* d_out, void* stream) {
+    int rc = check_bank(ctx, bank);
+    if (rc) return rc;
+    if (!d_feats || !d_out) return oww_fail(ctx, OWW_EINVAL, "null argument");
+    const HeadBank& b = ctx->head_banks[bank];
+    if ((rc = check_slot(ctx, b, slot, false))) return rc;
+    if (n < 0) return oww_fail(ctx, OWW_EINVAL, "n=%d", n);
+    if (n == 0) return OWW_OK;
+    OWW_CUDA(ctx, cudaSetDevice(ctx->device));
+    HeadsTcArgs a;
+    std::memset(&a, 0, sizeof(a));
+    a.head[0] = host_slot(b, slot);
+    a.head[0].dev.col0 = 0;
+    a.src = FeatSrc{d_feats, (int64_t)b.shape.desc.n_in * 96, nullptr, -1, 0};
+    a.n = n; a.out = d_out; a.out_stride = b.shape.n_out; a.combine_max = 0;
+    return ht_run<false>(ctx, a, std::max(16, b.shape.tc_layers[0].NP), dim3((n + kHtTile - 1) / kHtTile), (cudaStream_t)stream);
+}
+
+}  // extern "C"

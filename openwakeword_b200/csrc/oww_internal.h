@@ -86,6 +86,30 @@ struct VerifierBank {
     int clip_slot = -1;              // slot oww_predict_clips applies to every clip
 };
 
+// wake-word head bank (heads_tc.cu): `capacity` slots that each hold a head of one shape, run by the tensor-core heads
+// kernel.  Every stream picks a slot (-1: zeros in the bank's columns).  At assignment time the host sorts the streams by
+// slot and cuts each slot's streams into work items of at most 64 (one CTA each).
+struct HeadBank {
+    Head shape;                      // desc, n_out, col0, the staging offsets of a pack_head_blob blob, tc_layers
+    int capacity = 0;
+    size_t w_bytes = 0;              // packed fp16 hi/lo weights of one slot (oww_heads_tc_pack's layout)
+    size_t p_floats = 0;             // biases | LayerNorm parameters of one slot
+    std::vector<int> p_off;          // per layer: offsets of bias, gamma, beta in a slot's parameters (3 per layer)
+    uint8_t* d_w = nullptr;          // [capacity][w_bytes]
+    float* d_p = nullptr;            // [capacity][p_floats]
+    void* d_slots = nullptr;         // [capacity] kernel descriptors of the slots (heads_tc.cu)
+    std::vector<uint8_t> h_slots;    // host copy of d_slots
+    std::vector<uint8_t> loaded;     // per slot: a head has been loaded
+    int clip_slot = -1;              // slot the bulk clip path applies to every clip
+    // streams: host mirror of the assignment, and the item table the steps read ([B] int4 {slot, first, rows, 0} |
+    // [B] stream ids ordered by slot), staged through pinned memory
+    std::vector<int> assign;
+    int n_items = 0;
+    int* d_table = nullptr;
+    int* h_stage = nullptr;
+    cudaEvent_t stage_ev = nullptr;
+};
+
 // Ring row counters (rows ever written; ring slot = count & (rows-1)) would overflow int32 after ~248 days of
 // continuous streaming at 100 mel rows/s.  Past 2^30 they are rebased by a multiple of every ring size (rings are
 // powers of two <= 2^20 rows), which keeps the slot and leaves the count >= the ring size, so "row not yet written"
@@ -148,6 +172,7 @@ struct oww_ctx {
     float* d_emb_blob = nullptr;
 
     std::vector<Head> heads;
+    std::vector<HeadBank> head_banks;  // per-stream head banks: their columns are counted in n_out_total
     int n_out_total = 0;
     int max_n_in = 0;
     std::vector<Gate> gates;         // applied to every chunk's scores before the max over chunks
@@ -420,8 +445,21 @@ __device__ __forceinline__ const float* feat_row(const FeatRows& w, int c) {
 int oww_heads_launch(oww_ctx* ctx, int head_id, const FeatSrc& src, int n, float* d_out, int out_stride,
                      int out_col0, int combine_max, cudaStream_t s, uint32_t head_mask = 0xFFFFFFFFu);
 
+// ---- api.cu: a head blob (weights.py:pack_head_blob) in the device layout: tensors on 16-byte boundaries ----
+int oww_check_head_desc(oww_ctx* ctx, const oww_head_desc* desc);
+// fills h.desc and h.w_off / b_off / g_off / h_off; staged = the blob at those offsets
+int oww_stage_head(oww_ctx* ctx, const oww_head_desc* desc, const float* h_blob, size_t n_floats, Head& h,
+                   std::vector<float>& staged);
+
 // ---- heads_tc.cu: every Linear layer on the tensor cores (wgmma, fp16 hi/lo split operands, fp32 accumulate) ----
 int oww_heads_tc_pack(oww_ctx* ctx, Head& h, const float* w1);
+// every head bank on n rows: streams of the handle (src = the feature ring, n = n_streams: each stream's slot) or rows
+// of the bulk path (the clip slot).  d_step != nullptr (ragged step): streams with d_step[b] == 0 are not written.
+int oww_head_banks_launch(oww_ctx* ctx, const FeatSrc& src, int n, float* d_out, int out_stride, int combine_max,
+                          cudaStream_t s, const int* d_step = nullptr);
+// (re)allocate every bank's per-stream table for ctx->n_streams streams, every stream on slot -1 (synchronous)
+int oww_head_banks_alloc_streams(oww_ctx* ctx);
+void oww_head_banks_free(oww_ctx* ctx);
 bool oww_heads_tc_supported(const oww_ctx* ctx, int head_id);
 int oww_heads_tc_launch(oww_ctx* ctx, int head_id, const FeatSrc& src, int n, float* d_out, int out_stride,
                         int out_col0, int combine_max, cudaStream_t s, uint32_t head_mask = 0xFFFFFFFFu);

@@ -122,7 +122,37 @@ class StreamEngine:
     def assign_verifier(self, bank, slots, stream_ids=None, stream=None):
         """Stream stream_ids[i] (None = all) uses slot slots[i] (-1 = none) from the next ``step`` enqueued on the current
         CUDA stream (or `stream`) and the next ``step_host`` / ``submit``."""
-        torch = _torch()
+        self.ctx.assign_verifier(bank, stream_ids, slots, self._stream(stream))
+
+    def _stream(self, stream):
         if stream is None:
+            torch = _torch()
             stream = torch.cuda.current_stream(torch.device("cuda", self.device_index)).cuda_stream
-        self.ctx.assign_verifier(bank, stream_ids, slots, stream)
+        return stream
+
+    # ---- per-stream head banks (include/owwb200.h, oww_add_head_bank) ----
+    def add_head_bank(self, shape, capacity):
+        """Slots for `capacity` heads of the shape of head dict `shape` (one network, not a gated pair); every stream
+        starts on slot -1 (zeros).  Its columns follow the current ones: returns (bank id, first column, n_out)."""
+        n_in, dims, ln, fin = _weights.head_desc(shape)
+        col0 = self.ctx.n_outputs
+        bank = self.ctx.add_head_bank(n_in, dims, ln, fin, capacity)
+        self.n_cols = self.ctx.n_outputs
+        return bank, col0, dims[-1]
+
+    def load_bank_head(self, bank, slot, head):
+        """head: a head dict of the bank's shape.  Synchronises the device: steps already enqueued keep the old one."""
+        self.ctx.load_bank_head(bank, slot, _weights.pack_head_blob(head))
+
+    def assign_bank_head(self, bank, slots, stream_ids=None, stream=None):
+        """Stream stream_ids[i] (None = all) runs the head of slot slots[i] (-1 = none) from the next ``step`` enqueued on
+        the current CUDA stream (or `stream`) and the next ``step_host`` / ``submit``."""
+        self.ctx.assign_bank_head(bank, stream_ids, slots, self._stream(stream))
+
+    def set_head_bank_clip_slot(self, bank, slot):
+        self.ctx.set_head_bank_clip_slot(bank, slot)
+
+    def bank_head_predict(self, bank, slot, d_feats, out):
+        """d_feats: CUDA float32 [n, n_in, 96] -> out [n, n_out] with the head of `slot` (stateless)."""
+        self.ctx.bank_head_predict(bank, slot, d_feats, d_feats.shape[0], out, self._stream(None))
+        return out

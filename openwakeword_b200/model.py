@@ -37,7 +37,9 @@ class Model:
     @re_arg({"wakeword_model_paths": "wakeword_models"})
     def __init__(self, wakeword_models=[], class_mapping_dicts=[], enable_speex_noise_suppression=False,
                  vad_threshold=0, custom_verifier_models={}, custom_verifier_threshold=0.1,
-                 inference_framework="b200", **kwargs):
+                 inference_framework="b200", stream_models={}, stream_model_capacity=256, **kwargs):
+        """stream_models: {name: {stream id or None (every stream): model}} - a model per stream under one label
+        (``set_stream_model``); stream_model_capacity: distinct models each such name can hold at once."""
         if inference_framework != "b200":
             raise ValueError(f"openwakeword_b200.Model only provides inference_framework='b200' (got '{inference_framework}')")
         pretrained_paths = _registry.get_pretrained_model_paths(inference_framework)
@@ -141,6 +143,31 @@ class Model:
                         device_verifiers[name] = {None: v}
                     else:
                         self._host_verifiers[name] = v
+        self._sbanks = {}              # name -> per-stream head bank state (set_stream_model)
+        for name, per_stream in stream_models.items():
+            if name in self.models:
+                raise ValueError(f"stream model name '{name}' is also a wakeword_models name")
+            if name in custom_verifier_models:
+                raise ValueError(f"custom verifier models apply to wakeword_models, not to the stream models '{name}'")
+            models = [m for m in per_stream.values() if m is not None]
+            if not models:
+                raise ValueError(f"stream models '{name}': no model given, so the shape is unknown")
+            first = per_stream[None] if per_stream.get(None) is not None else models[0]
+            head, file_map = self._read_stream_model(first)
+            n_in, dims, ln, fin = _weights.head_desc(head)
+            bank = ctx.add_head_bank(n_in, dims, ln, fin, stream_model_capacity)
+            self._sbanks[name] = {"bank": bank, "shape": (n_in, list(dims), ln, fin), "capacity": stream_model_capacity,
+                                  "slots": None, "keys": None}
+            self.models[name] = bank
+            self.model_inputs[name] = n_in
+            self.model_outputs[name] = dims[-1]
+            self.model_prediction_function[name] = partial(self._bank_predict, name, n_in, dims[-1])
+            self._columns[name] = (col, dims[-1])
+            col += dims[-1]
+            if dims[-1] == 1:
+                self.class_mapping[name] = {"0": name}
+            else:
+                self.class_mapping[name] = file_map or {str(i): str(i) for i in range(0, dims[-1])}
         if len(self.custom_verifier_models.keys()) < len(custom_verifier_models.keys()):
             raise ValueError("Custom verifier models were provided, but some were not matched with a base model!"
                              " Make sure that the keys provided in the `custom_verifier_models` dictionary argument"
@@ -151,6 +178,85 @@ class Model:
         for name, per_stream in device_verifiers.items():
             for b, v in per_stream.items():
                 self.set_custom_verifier(name, v, None if b is None else [b])
+        for name, per_stream in stream_models.items():
+            if None in per_stream:
+                self.set_stream_model(name, per_stream[None])
+            for b, m in per_stream.items():
+                if b is not None:
+                    self.set_stream_model(name, m, [b])
+
+    # ---- a model per stream (include/owwb200.h, oww_add_head_bank) ----
+    @staticmethod
+    def _read_stream_model(model):
+        """(head dict, class mapping or None) of an .onnx / .npz path or an in-memory head dict."""
+        if isinstance(model, dict):
+            return model, None
+        if isinstance(model, (str, os.PathLike)):
+            path = os.fspath(model)
+            if not os.path.exists(path):
+                raise ValueError(f"Model file '{path}' not found")
+            return _load_head_file(path)
+        raise ValueError(f"a stream model is an .onnx / .npz path or a head dict, got {type(model)}")
+
+    def set_stream_model(self, name, model, streams=None):
+        """Run `model` (an .onnx / .npz path or a head dict of the shape of `name`'s first model; None removes it) on
+        `streams` (stream ids; None = every stream) under label `name` from the next call on.  The same path or object
+        on many streams shares one slot of the bank; a slot no stream uses is free again.  A stream without a model
+        reads 0.0.  The streams keep their label history (``reset_streams`` starts a new client afresh)."""
+        st = self._sbanks.get(name)
+        if st is None:
+            raise ValueError(f"no stream models named '{name}'")
+        B = self.n_streams
+        ids = np.arange(B) if streams is None else np.unique(np.asarray(streams, np.int64).ravel())
+        if ids.size == 0:
+            return
+        if ids.min() < 0 or ids.max() >= B:
+            raise ValueError(f"stream ids must lie in [0, {B})")
+        ctx = self.preprocessor.ctx
+        if st["slots"] is None:
+            self.preprocessor._ensure_streams()
+            st["slots"], st["keys"] = np.full(B, -1, np.int32), [None] * B
+        slots, keys = st["slots"], st["keys"]
+        slot = -1
+        key = None
+        if model is not None:
+            key = os.fspath(model) if isinstance(model, (str, os.PathLike)) else model
+            others = np.ones(B, bool)
+            others[ids] = False
+            live = {int(slots[b]): keys[b] for b in np.nonzero(others & (slots >= 0))[0]}
+            same = [k for k, v in live.items() if v is key or (isinstance(key, str) and v == key)]
+            if same:
+                slot = same[0]
+            else:
+                head, _ = self._read_stream_model(model)
+                n_in, dims, ln, fin = _weights.head_desc(head)
+                if (n_in, list(dims), ln, fin) != st["shape"]:
+                    raise ValueError(f"stream models '{name}' have the shape {st['shape']}, got {(n_in, list(dims), ln, fin)}")
+                free = [k for k in range(st["capacity"]) if k not in live]
+                if not free:
+                    raise ValueError(f"stream models '{name}': more than {st['capacity']} distinct models in use "
+                                     "(stream_model_capacity)")
+                slot = free[0]
+                ctx.load_bank_head(st["bank"], slot, _weights.pack_head_blob(head))
+        ctx.assign_bank_head(st["bank"], None if ids.size == B else ids, np.full(ids.size, slot, np.int32))
+        slots[ids] = slot
+        for b in ids:
+            keys[b] = key
+        ctx.set_head_bank_clip_slot(st["bank"], int(slots[0]))
+
+    def _bank_predict(self, name, n_in, n_out, x):
+        """model_prediction_function of stream models: stream 0's model (zeros without one)."""
+        torch = _torch()
+        st = self._sbanks[name]
+        x = np.ascontiguousarray(np.asarray(x, np.float32).reshape(-1, n_in, 96))
+        slot = -1 if st["slots"] is None else int(st["slots"][0])
+        if slot < 0:
+            return [np.zeros((x.shape[0], n_out), np.float32)]
+        dev = f"cuda:{self.preprocessor.device_index}"
+        d = torch.from_numpy(x).to(dev)
+        out = torch.empty((x.shape[0], n_out), dtype=torch.float32, device=dev)
+        self.preprocessor.ctx.bank_head_predict(st["bank"], slot, d, x.shape[0], out, torch.cuda.current_stream(d.device).cuda_stream)
+        return [out.cpu().numpy()]
 
     # ---- custom verifier models on the device (include/owwb200.h, oww_add_verifier_bank) ----
     @property
@@ -181,6 +287,8 @@ class Model:
         every stream has the same one, {stream id: verifier} otherwise, absent when no stream has one."""
         if name not in self.models:
             raise ValueError(f"no model named '{name}'")
+        if name in self._sbanks:
+            raise ValueError(f"custom verifier models apply to wakeword_models, not to the stream models '{name}'")
         B = self.n_streams
         ids = np.arange(B) if streams is None else np.unique(np.asarray(streams, np.int64).ravel())
         if ids.size == 0:
