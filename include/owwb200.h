@@ -243,6 +243,33 @@ int oww_get_mel(oww_ctx* ctx, int stream_id, int n_rows, float* h_out);   /* las
  * (utils.py:400-401,449-450).  Either pointer may be NULL.  Synchronises.                                     */
 int oww_get_counts(oww_ctx* ctx, int stream_id, int* mel_rows, int* feature_rows);
 
+/* ---- moving live streams: stream records ----------------------------------------------------------------------------
+ * A stream record is one stream's complete state - PCM tail, counters, the newest 76 mel rows and 120 feature rows, and
+ * in cnn_mode 3 the conv tails of the fused kernel and the late layers as stored - in a layout that depends only on the
+ * cnn_mode, split_from and the loaded weights, not on the stream count, max_chunks, the heads or the other reserved
+ * flags.  It starts with a header (format version, record size, configuration key); the size is a multiple of 16 bytes.
+ *   oww_stream_state_info   - the record size of this handle and its configuration key (a hash of the format version,
+ *                             cnn_mode, split_from in mode 3, the mel constants and the embedding blob).  Needs
+ *                             oww_set_streams first.
+ *   oww_export_streams      - stream h_stream_ids[i] -> record i of d_records [n][record_bytes] (device memory of the
+ *                             handle's device).  Duplicate ids are allowed.
+ *   oww_import_streams      - record i -> stream h_stream_ids[i] (no duplicates).  Afterwards that stream is exactly the
+ *                             stream the record was taken from: its next steps of any kind give the same scores and leave
+ *                             the same rings and counts, bit for bit wherever both handles run the same arithmetic.  The
+ *                             fp16 feature mirror of the targets is resynced as after a reset.  No other stream changes,
+ *                             and no stream's verifier or head-bank assignment changes (targets included).
+ *   oww_stream_state_status - records the imports since the last call skipped (*n_rejected); synchronises; clears.
+ * Export and import are stream-ordered and allocation-free after the first call, like oww_reset_async, and ordered
+ * against oww_step_host / oww_step_host_submit on the handle's own stream: an export enqueued between two steps
+ * captures exactly the state between them.  No oww_set_streams yet, an id out of range, n greater than the stream
+ * count or a duplicate id in an import fails with OWW_EINVAL before anything is enqueued.  A record whose header does
+ * not match this handle's size and key is skipped on the device: its stream is left unchanged and the rejection is
+ * counted for oww_stream_state_status.                                                                                 */
+int oww_stream_state_info(const oww_ctx* ctx, size_t* record_bytes, uint64_t* config_key);
+int oww_export_streams(oww_ctx* ctx, const int32_t* h_stream_ids, int n, void* d_records, void* stream);
+int oww_import_streams(oww_ctx* ctx, const int32_t* h_stream_ids, int n, const void* d_records, void* stream);
+int oww_stream_state_status(oww_ctx* ctx, int* n_rejected);
+
 /* ---- batch paths --------------------------------------------------------------------------- */
 /* d_pcm [n_clips][n_samples] -> d_emb [n_clips][W][96], W = (T-76)/8+1 (utils.py:322).           */
 int oww_embed_clips(oww_ctx* ctx, const int16_t* d_pcm, int n_clips, int n_samples, float* d_emb, void* stream);

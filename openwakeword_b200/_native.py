@@ -71,6 +71,10 @@ _SIGNATURES = {
     "oww_get_features": (C.c_int, [_P, C.c_int, C.c_int, C.c_int, _P]),
     "oww_get_mel": (C.c_int, [_P, C.c_int, C.c_int, _P]),
     "oww_get_counts": (C.c_int, [_P, C.c_int, C.POINTER(C.c_int), C.POINTER(C.c_int)]),
+    "oww_stream_state_info": (C.c_int, [_P, C.POINTER(C.c_size_t), C.POINTER(C.c_uint64)]),
+    "oww_export_streams": (C.c_int, [_P, _P, C.c_int, _P, _P]),
+    "oww_import_streams": (C.c_int, [_P, _P, C.c_int, _P, _P]),
+    "oww_stream_state_status": (C.c_int, [_P, C.POINTER(C.c_int)]),
     "oww_embed_clips": (C.c_int, [_P, _P, C.c_int, C.c_int, _P, _P]),
     "oww_predict_clips": (C.c_int, [_P, _P, C.c_int, C.c_int, C.c_int, _P, C.c_int, _P, _P]),
     "oww_clip_schedule": (C.c_int, [C.c_int, C.c_int64, _P, C.c_int]),
@@ -405,6 +409,65 @@ class Context:
         out = np.empty((n_rows, 32), np.float32)
         self._check(self.lib.oww_get_mel(self.h, stream_id, n_rows, _ptr(out)))
         return out
+
+    # ---- stream records: moving live streams (include/owwb200.h, oww_export_streams) ----
+    def stream_state_info(self):
+        """-> (record bytes, configuration key) of this handle's stream records."""
+        n, key = C.c_size_t(0), C.c_uint64(0)
+        self._check(self.lib.oww_stream_state_info(self.h, C.byref(n), C.byref(key)))
+        return n.value, key.value
+
+    def export_streams(self, stream_ids, d_records, stream=None):
+        """Stream stream_ids[i] -> record i of d_records (device, [n][record bytes]); stream-ordered."""
+        ids = np.ascontiguousarray(stream_ids, np.int32).ravel()
+        self._check(self.lib.oww_export_streams(self.h, _ptr(ids), ids.size, _ptr(d_records), stream))
+
+    def import_streams(self, stream_ids, d_records, stream=None):
+        """Record i of d_records -> stream stream_ids[i] (distinct ids); stream-ordered.  Records of another
+        configuration are skipped on the device and counted (stream_state_rejected)."""
+        ids = np.ascontiguousarray(stream_ids, np.int32).ravel()
+        self._check(self.lib.oww_import_streams(self.h, _ptr(ids), ids.size, _ptr(d_records), stream))
+
+    def stream_state_rejected(self):
+        """Records the imports since the last call skipped (synchronises the device; clears the count)."""
+        v = C.c_int(0)
+        self._check(self.lib.oww_stream_state_status(self.h, C.byref(v)))
+        return v.value
+
+    def export_records(self, stream_ids, stream=None):
+        """export_streams into a new torch.uint8 [n, record bytes] on the handle's device; stream None: the current CUDA
+        stream of that device."""
+        import torch
+        ids = np.ascontiguousarray(stream_ids, np.int32).ravel()
+        n_bytes, _ = self.stream_state_info()
+        dev = torch.device("cuda", self.device)
+        out = torch.empty((ids.size, n_bytes), dtype=torch.uint8, device=dev)
+        self.export_streams(ids, out, torch.cuda.current_stream(dev).cuda_stream if stream is None else stream)
+        return out
+
+    def import_records(self, stream_ids, records, stream=None):
+        """import_streams from a torch.uint8 [n, record bytes] on any device or the CPU (moved with .to()).  Records of
+        another configuration raise ValueError before anything is enqueued."""
+        import torch
+        ids = np.ascontiguousarray(stream_ids, np.int32).ravel()
+        n_bytes, key = self.stream_state_info()
+        if records.dtype != torch.uint8 or records.dim() != 2 or records.shape[0] != ids.size:
+            raise ValueError(f"records must be uint8 [{ids.size}, {n_bytes}], got {records.dtype} {tuple(records.shape)}")
+        if records.shape[1] != n_bytes:
+            raise ValueError(f"records of {records.shape[1]} bytes; this configuration's have {n_bytes}")
+        if ids.size:
+            keys = np.ascontiguousarray(records[:, 8:16].cpu().numpy()).view(np.uint64).ravel()
+            if (keys != np.uint64(key)).any():
+                raise ValueError("records of another configuration (cnn_mode, split_from or weights)")
+        dev = torch.device("cuda", self.device)
+        d = records.to(dev).contiguous()                   # on the current CUDA stream of the device
+        if stream is None:
+            self.import_streams(ids, d, torch.cuda.current_stream(dev).cuda_stream)
+        else:                                              # after that copy, whose memory must outlive the import
+            ext = torch.cuda.ExternalStream(stream, device=dev)
+            ext.wait_stream(torch.cuda.current_stream(dev))
+            self.import_streams(ids, d, stream)
+            d.record_stream(ext)
 
     # ---- batch ----
     def embed_clips(self, d_pcm, n_clips, n_samples, d_emb, stream=None):

@@ -47,36 +47,46 @@ void fill_layer_table(oww_ctx* ctx) {
 
 int next_pow2(int v) { int p = 1; while (p < v) p <<= 1; return p; }
 
+// Mode 3: every 16-byte unit of stream b's conv tails state, in the CTA's threads.  early(t, at): unit t of the compact
+// G = 1 layout (the template, a stream record) is unit `at` of the G-group tails buffers - layout [(r*G + g)*Wp + f] of
+// each tails-bearing tensor.  late(T, i, pl, r, f, at): unit i of late tensor T's [plane][2][Wp] rows is unit `at` of its
+// block-major layout (cnn_tc.cu, tc_conv_blk_kernel: no pad column, so cells f >= Wq are not visited).
+template <class Early, class Late>
+__device__ __forceinline__ void for_each_tail_unit(const ResetTails& rt, int b, Early early, Late late) {
+    const int grp = b / rt.G, g = b - grp * rt.G;
+    const int64_t base = (int64_t)grp * rt.tail_units;
+    for (int k = 0; k < rt.n_tab; ++k) {
+        const int off1 = rt.tab[k].x, offG = rt.tab[k].y, cg = rt.tab[k].z, Wp = rt.tab[k].w;
+        for (int i = threadIdx.x; i < cg * 2 * Wp; i += blockDim.x) {
+            const int pl = i / (2 * Wp), u = i - pl * 2 * Wp, r = u / Wp, f = u - r * Wp;
+            early(off1 + i, base + offG + pl * (2 * rt.G * Wp) + (r * rt.G + g) * Wp + f);
+        }
+    }
+    for (int k = 0; k < rt.n_late; ++k) {
+        const ResetLate& T = rt.late[k];
+        for (int i = threadIdx.x; i < T.n_planes * 2 * T.Wp; i += blockDim.x) {
+            const int pl = i / (2 * T.Wp), u = i - pl * 2 * T.Wp, r = u / T.Wp, f = u - r * T.Wp;
+            if (f < T.lay.Wq) late(T, i, pl, r, f, late_unit(T.lay, pl, b, r, f));
+        }
+    }
+}
+
+// a late tails row the next step reads: rows 0, 1 of `now`; tensors that gain one row per step also read row 1 as row 0
+// of the buffer of the step after
+__device__ __forceinline__ void put_late(const ResetLate& T, int b, int pl, int r, int f, int64_t at, uint4 v) {
+    T.now[at] = v;
+    if (T.next && r == 1) T.next[late_unit(T.lay, pl, b, 0, f)] = v;
+}
+
 __global__ void reset_kernel(const int* ids, int n_ids, int n_streams, int16_t* tail, int* seen, int* mel_count,
                              int* feat_count, float* mel_ring, int mel_rows, float* feat_ring, int feat_rows,
                              const float* feat_init, int n_rows, ResetTails rt) {
     const int j = blockIdx.x;
     const int b = ids ? ids[j] : j;
     if (b < 0 || b >= n_streams) return;
-    if (rt.tails) {
-        // mode 3: the stream's conv tails become those of the all-ones window (its history after a reset), scattered from
-        // the compact per-stream template into the group layout [(r*G + g)*Wp + f] of each tails-bearing tensor
-        const int grp = b / rt.G, g = b - grp * rt.G;
-        uint4* dst = rt.tails + (int64_t)grp * rt.tail_units;
-        for (int k = 0; k < rt.n_tab; ++k) {
-            const int off1 = rt.tab[k].x, offG = rt.tab[k].y, cg = rt.tab[k].z, Wp = rt.tab[k].w;
-            for (int i = threadIdx.x; i < cg * 2 * Wp; i += blockDim.x) {
-                const int pl = i / (2 * Wp), u = i - pl * 2 * Wp, r = u / Wp, f = u - r * Wp;
-                dst[offG + pl * (2 * rt.G * Wp) + (r * rt.G + g) * Wp + f] = rt.tmpl[off1 + i];
-            }
-        }
-        // incremental late layers: tails rows of the buffers the next step (and, for single-row tensors, the one after) reads
-        for (int k = 0; k < rt.n_late; ++k) {
-            const ResetLate& T = rt.late[k];
-            for (int i = threadIdx.x; i < T.n_planes * 2 * T.Wp; i += blockDim.x) {
-                const int pl = i / (2 * T.Wp), u = i - pl * 2 * T.Wp, r = u / T.Wp, f = u - r * T.Wp;
-                if (f >= T.lay.Wq) continue;                // block-major layout (cnn_tc.cu, tc_conv_blk_kernel): no pad column
-                const uint4 v = T.tmpl[i];
-                T.now[late_unit(T.lay, pl, b, r, f)] = v;
-                if (T.next && r == 1) T.next[late_unit(T.lay, pl, b, 0, f)] = v;
-            }
-        }
-    }
+    if (rt.tails)       // mode 3: the conv tails of the all-ones window (the stream's history after a reset)
+        for_each_tail_unit(rt, b, [&](int t, int64_t at) { rt.tails[at] = rt.tmpl[t]; },
+                           [&](const ResetLate& T, int i, int pl, int r, int f, int64_t at) { put_late(T, b, pl, r, f, at, T.tmpl[i]); });
     for (int i = threadIdx.x; i < OWW_TAIL; i += blockDim.x) tail[(int64_t)b * OWW_TAIL + i] = 0;
     float* mr = mel_ring + (int64_t)b * mel_rows * 32;
     for (int i = threadIdx.x; i < mel_rows * 32; i += blockDim.x) mr[i] = 1.0f;     // np.ones((76,32)), utils.py:165
@@ -97,27 +107,96 @@ __global__ void reset_kernel(const int* ids, int n_ids, int n_streams, int16_t* 
 __global__ void carry_kernel(const int* ids, int n_ids, ResetTails rt) {
     oww_pdl_sync();
     const int b = ids[blockIdx.x];
-    const int grp = b / rt.G, g = b - grp * rt.G;
-    const uint4* src = rt.tmpl + (int64_t)grp * rt.tail_units;
-    uint4* dst = rt.tails + (int64_t)grp * rt.tail_units;
-    for (int k = 0; k < rt.n_tab; ++k) {
-        const int offG = rt.tab[k].y, cg = rt.tab[k].z, Wp = rt.tab[k].w;
-        for (int i = threadIdx.x; i < cg * 2 * Wp; i += blockDim.x) {
-            const int pl = i / (2 * Wp), u = i - pl * 2 * Wp, r = u / Wp, f = u - r * Wp;
-            const int64_t at = offG + pl * (2 * rt.G * Wp) + (r * rt.G + g) * Wp + f;
-            dst[at] = src[at];
-        }
+    for_each_tail_unit(rt, b, [&](int, int64_t at) { rt.tails[at] = rt.tmpl[at]; },
+                       [&](const ResetLate& T, int, int pl, int r, int f, int64_t at) { put_late(T, b, pl, r, f, at, T.tmpl[at]); });
+}
+
+// ---- stream records (include/owwb200.h, oww_export_streams): one stream's state in a layout that depends only on the
+//      cnn_mode, split_from and the weights.  16-byte units:
+//        [0, 2)     header: version, record bytes, configuration key | seen, mel count, feature count, 0
+//        [2, 62)    the 480-sample PCM tail
+//        [62, 670)  the newest 76 mel rows, oldest first
+//        [670, 3550) the newest 120 feature rows, oldest first (rows before the stream's first read as zeros)
+//        [3550, +u_tails)   mode 3: the conv tails in the compact G = 1 layout of the template (tail_tab)
+//        [.., +u_late)      mode 3: rows 0..1 of each tails-bearing late tensor, [plane][2][Wp] at its template offset
+constexpr uint32_t kRecVersion = 1;
+constexpr int kRecPcm = 2, kRecMel = 62, kRecFeat = 670, kRecTails = 3550;
+constexpr int kRecMelRows = OWW_WINDOW_ROWS, kRecFeatRows = 120;      // 120: the reference's feature_buffer cap
+
+struct StreamState {
+    int16_t* tail; int* seen; int* mel_count; int* feat_count;
+    float* mel_ring; int mel_rows; float* feat_ring; int feat_rows;
+    int64_t rec_units;               // units per record
+    int u_tails;                     // units of the early conv tails section (the late section follows it)
+    uint32_t bytes; uint64_t key;
+    int* rejected;
+};
+
+// one CTA per record: stream ids[j]'s state -> record j
+__global__ void __launch_bounds__(256) stream_export_kernel(const int* ids, StreamState a, ResetTails rt, uint4* rec) {
+    const int b = ids[blockIdx.x];
+    uint4* r = rec + (int64_t)blockIdx.x * a.rec_units;
+    const int mc = a.mel_count[b], fc = a.feat_count[b];
+    if (threadIdx.x == 0) {
+        r[0] = make_uint4(kRecVersion, a.bytes, (uint32_t)a.key, (uint32_t)(a.key >> 32));
+        r[1] = make_uint4((uint32_t)a.seen[b], (uint32_t)mc, (uint32_t)fc, 0u);
     }
-    for (int k = 0; k < rt.n_late; ++k) {
-        const ResetLate& T = rt.late[k];
-        for (int i = threadIdx.x; i < T.n_planes * 2 * T.Wp; i += blockDim.x) {
-            const int pl = i / (2 * T.Wp), u = i - pl * 2 * T.Wp, r = u / T.Wp, f = u - r * T.Wp;
-            if (f >= T.lay.Wq) continue;
-            const uint4 v = T.tmpl[late_unit(T.lay, pl, b, r, f)];
-            T.now[late_unit(T.lay, pl, b, r, f)] = v;
-            if (T.next && r == 1) T.next[late_unit(T.lay, pl, b, 0, f)] = v;
-        }
+    const uint4* tail = reinterpret_cast<const uint4*>(a.tail + (int64_t)b * OWW_TAIL);
+    for (int i = threadIdx.x; i < OWW_TAIL / 8; i += blockDim.x) r[kRecPcm + i] = tail[i];
+    const uint4* mel = reinterpret_cast<const uint4*>(a.mel_ring + (int64_t)b * a.mel_rows * 32);
+    for (int i = threadIdx.x; i < kRecMelRows * 8; i += blockDim.x) {
+        const int k = i >> 3;
+        r[kRecMel + i] = mel[((mc - kRecMelRows + k) & (a.mel_rows - 1)) * 8 + (i & 7)];
     }
+    const uint4* feat = reinterpret_cast<const uint4*>(a.feat_ring + (int64_t)b * a.feat_rows * 96);
+    for (int i = threadIdx.x; i < kRecFeatRows * 24; i += blockDim.x) {
+        const int k = i / 24, row = fc - kRecFeatRows + k;
+        r[kRecFeat + i] = row < 0 ? make_uint4(0, 0, 0, 0) : feat[(row & (a.feat_rows - 1)) * 24 + (i - k * 24)];
+    }
+    if (!rt.tails) return;
+    uint4* tails = r + kRecTails;
+    uint4* late = tails + a.u_tails;
+    const int64_t n_tails = a.rec_units - kRecTails;                 // pad cells the gather does not visit stay zero
+    for (int64_t i = threadIdx.x; i < n_tails; i += blockDim.x) tails[i] = make_uint4(0, 0, 0, 0);
+    __syncthreads();
+    for_each_tail_unit(rt, b, [&](int t, int64_t at) { tails[t] = rt.tails[at]; },
+                       [&](const ResetLate& T, int i, int, int, int, int64_t at) { late[T.off + i] = T.now[at]; });
+}
+
+// one CTA per record: record j -> stream ids[j] (reset_kernel's scatter with the record as the source).  A record whose
+// header does not match the handle (or whose counts are impossible) is skipped and counted.
+__global__ void __launch_bounds__(256) stream_import_kernel(const int* ids, StreamState a, ResetTails rt, const uint4* rec) {
+    const int b = ids[blockIdx.x];
+    const uint4* r = rec + (int64_t)blockIdx.x * a.rec_units;
+    const uint4 h0 = r[0], h1 = r[1];
+    const int seen = (int)h1.x, mc = (int)h1.y, fc = (int)h1.z;
+    if (h0.x != kRecVersion || h0.y != a.bytes || h0.z != (uint32_t)a.key || h0.w != (uint32_t)(a.key >> 32) ||
+        seen < 0 || mc < kRecMelRows || fc < 0) {
+        if (threadIdx.x == 0) atomicAdd(a.rejected, 1);
+        return;
+    }
+    uint4* tail = reinterpret_cast<uint4*>(a.tail + (int64_t)b * OWW_TAIL);
+    for (int i = threadIdx.x; i < OWW_TAIL / 8; i += blockDim.x) tail[i] = r[kRecPcm + i];
+    // ring slot s holds row mc - rows + ((s - mc) & mask); the record's row k = that row - (mc - 76).  Older slots get
+    // what a reset leaves there (ones / zeros): no step and no read reaches them.
+    const float one = 1.0f;
+    const uint32_t ones = __float_as_uint(one);
+    uint4* mel = reinterpret_cast<uint4*>(a.mel_ring + (int64_t)b * a.mel_rows * 32);
+    for (int i = threadIdx.x; i < a.mel_rows * 8; i += blockDim.x) {
+        const int k = kRecMelRows - a.mel_rows + (((i >> 3) - mc) & (a.mel_rows - 1));
+        mel[i] = k < 0 ? make_uint4(ones, ones, ones, ones) : r[kRecMel + k * 8 + (i & 7)];
+    }
+    uint4* feat = reinterpret_cast<uint4*>(a.feat_ring + (int64_t)b * a.feat_rows * 96);
+    for (int i = threadIdx.x; i < a.feat_rows * 24; i += blockDim.x) {
+        const int s = i / 24, k = kRecFeatRows - a.feat_rows + ((s - fc) & (a.feat_rows - 1));
+        feat[i] = k < 0 ? make_uint4(0, 0, 0, 0) : r[kRecFeat + k * 24 + (i - s * 24)];
+    }
+    if (threadIdx.x == 0) { a.seen[b] = seen; a.mel_count[b] = mc; a.feat_count[b] = fc; }
+    if (!rt.tails) return;
+    const uint4* tails = r + kRecTails;
+    const uint4* late = tails + a.u_tails;
+    for_each_tail_unit(rt, b, [&](int t, int64_t at) { rt.tails[at] = tails[t]; },
+                       [&](const ResetLate& T, int i, int pl, int rr, int f, int64_t at) { put_late(T, b, pl, rr, f, at, late[T.off + i]); });
 }
 
 // Ragged step: stream b appends embedding rows n - cnt[b] .. n - 1 of emb [n][B][96] (its own chunks, oldest first) to
@@ -166,6 +245,7 @@ void free_streams(oww_ctx* c) {
     cudaFree(c->d_mel_ring); cudaFree(c->d_feat_ring); cudaFree(c->d_act[0]); cudaFree(c->d_act[1]);
     cudaFree(c->d_emb_tmp); cudaFree(c->d_inc_tails[0]); cudaFree(c->d_inc_tails[1]);
     cudaFree(c->d_reset_ids); cudaFree(c->d_reset_init);
+    cudaFree(c->d_state_ids); c->d_state_ids = nullptr;
     cudaFree(c->d_scores_tmp);
     cudaFree(c->d_rag_scores); c->d_rag_scores = nullptr; c->rag_scores_floats = 0;
     for (int j = 0; j < oww_ctx::kRagSlots; ++j) {       // set_streams / destroy synchronise the device first
@@ -413,7 +493,7 @@ int next_step_tables(oww_ctx* ctx, ResetTails& rt) {
             ResetLate& T = rt.late[rt.n_late++];
             T.now = reinterpret_cast<uint4*>(X.buf[k % X.n_buf]);
             T.next = X.n_buf == 3 ? reinterpret_cast<uint4*>(X.buf[(k + 1) % 3]) : nullptr;
-            T.Wp = X.W + 1; T.n_planes = 2 * X.cg; T.lay = X.lay;
+            T.Wp = X.W + 1; T.n_planes = 2 * X.cg; T.off = X.tmpl_off; T.lay = X.lay;
         }
     }
     return OWW_OK;
@@ -620,6 +700,90 @@ int reset_enqueue(oww_ctx* ctx, const int32_t* h_stream_ids, int n, const float*
     return oww_feat16_resync(ctx, h_stream_ids ? ctx->d_reset_ids : nullptr, n, s);     // fp16 mirror of the rings (heads_grp.cu)
 }
 
+// Units of a stream record's two conv tails sections (0 outside mode 3).  tail_tab is filled by the reset that
+// oww_set_streams ends with.
+void record_units(const oww_ctx* ctx, int* u_tails, int* u_late) {
+    *u_tails = *u_late = 0;
+    if (ctx->cfg.cnn_mode != OWW_CNN_TC_INCREMENTAL) return;
+    for (int k = 0; k < ctx->n_tail_tab; ++k)
+        *u_tails = std::max(*u_tails, ctx->tail_tab[k].x + ctx->tail_tab[k].z * 2 * ctx->tail_tab[k].w);
+    if (!ctx->late_active) return;
+    for (int l = ctx->split_from; l < OWW_N_CONV; ++l) {
+        const oww_ctx::LateTensor& X = ctx->late_x[l];
+        if (X.tmpl_off >= 0) *u_late = std::max(*u_late, X.tmpl_off + 2 * X.cg * 2 * (X.W + 1));
+    }
+}
+
+int64_t record_bytes(const oww_ctx* ctx) {
+    int u_tails, u_late;
+    record_units(ctx, &u_tails, &u_late);
+    return ((int64_t)kRecTails + u_tails + u_late) * 16;
+}
+
+// what a record's state is only valid under: its format, the CNN mode and split point, the mel constants and the
+// embedding weights (the conv tails and the rings are their products)
+uint64_t record_key(const oww_ctx* ctx) {
+    const int32_t cfg[3] = {(int32_t)kRecVersion, ctx->cfg.cnn_mode,
+                            ctx->cfg.cnn_mode == OWW_CNN_TC_INCREMENTAL ? ctx->split_from : 0};
+    uint64_t h = oww_fnv1a(cfg, sizeof(cfg));
+    h = oww_fnv1a(&ctx->mel_key, sizeof(uint64_t), h);
+    return oww_fnv1a(&ctx->emb_key, sizeof(uint64_t), h);
+}
+
+// shared by oww_export_streams / oww_import_streams: checks on the host, then one launch on `s`, ordered with own_stream
+int state_enqueue(oww_ctx* ctx, const int32_t* h_ids, int n, void* d_records, bool import, cudaStream_t s) {
+    const int B = ctx->n_streams;
+    if (B <= 0) return oww_fail(ctx, OWW_EINVAL, "oww_set_streams has not been called");
+    if (n < 0 || n > B) return oww_fail(ctx, OWW_EINVAL, "n=%d outside [0,%d]", n, B);
+    if (n == 0) return OWW_OK;
+    if (!h_ids || !d_records) return oww_fail(ctx, OWW_EINVAL, "null argument");
+    std::vector<uint8_t> hit(import ? B : 0, 0);
+    for (int i = 0; i < n; ++i) {
+        if (h_ids[i] < 0 || h_ids[i] >= B) return oww_fail(ctx, OWW_EINVAL, "stream id %d out of range", h_ids[i]);
+        if (import && hit[h_ids[i]]++) return oww_fail(ctx, OWW_EINVAL, "stream id %d imported twice", h_ids[i]);
+    }
+    if (!ctx->d_state_ids) OWW_CUDA(ctx, cudaMalloc(&ctx->d_state_ids, (size_t)B * sizeof(int)));
+    if (!ctx->d_state_rejected) {
+        OWW_CUDA(ctx, cudaMalloc(&ctx->d_state_rejected, sizeof(int)));
+        OWW_CUDA(ctx, cudaMemset(ctx->d_state_rejected, 0, sizeof(int)));
+    }
+    for (auto& e : ctx->state_ev)
+        if (!e) OWW_CUDA(ctx, cudaEventCreateWithFlags(&e, cudaEventDisableTiming));
+    StreamState a{ctx->d_tail, ctx->d_seen, ctx->d_mel_count, ctx->d_feat_count, ctx->d_mel_ring, ctx->mel_rows,
+                  ctx->d_feat_ring, ctx->feat_rows, record_bytes(ctx) / 16, 0, (uint32_t)record_bytes(ctx), record_key(ctx),
+                  ctx->d_state_rejected};
+    int u_late = 0;
+    record_units(ctx, &a.u_tails, &u_late);
+    ResetTails rt;
+    std::memset(&rt, 0, sizeof(rt));
+    if (ctx->cfg.cnn_mode == OWW_CNN_TC_INCREMENTAL) {
+        int rc = next_step_tables(ctx, rt);            // where the state between the last step and the next one lives
+        if (rc) return rc;
+    }
+    // the host-buffer steps run on the handle's own stream: after the steps submitted there so far, before later ones
+    const bool other = s != ctx->own_stream;
+    if (other) {
+        OWW_CUDA(ctx, cudaEventRecord(ctx->state_ev[0], ctx->own_stream));
+        OWW_CUDA(ctx, cudaStreamWaitEvent(s, ctx->state_ev[0], 0));
+    }
+    // pageable source: staged by the driver before the call returns; stream-ordered on the device
+    OWW_CUDA(ctx, cudaMemcpyAsync(ctx->d_state_ids, h_ids, (size_t)n * sizeof(int), cudaMemcpyHostToDevice, s));
+    if (import) {
+        stream_import_kernel<<<n, 256, 0, s>>>(ctx->d_state_ids, a, rt, static_cast<const uint4*>(d_records));
+        OWW_LAUNCH_CHECK(ctx);
+        int rc = oww_feat16_resync(ctx, ctx->d_state_ids, n, s);          // fp16 mirror of the rings, as after a reset
+        if (rc) return rc;
+    } else {
+        stream_export_kernel<<<n, 256, 0, s>>>(ctx->d_state_ids, a, rt, static_cast<uint4*>(d_records));
+        OWW_LAUNCH_CHECK(ctx);
+    }
+    if (other) {
+        OWW_CUDA(ctx, cudaEventRecord(ctx->state_ev[1], s));
+        OWW_CUDA(ctx, cudaStreamWaitEvent(ctx->own_stream, ctx->state_ev[1], 0));
+    }
+    return OWW_OK;
+}
+
 }  // namespace
 
 extern "C" {
@@ -679,7 +843,8 @@ void oww_destroy(oww_ctx* ctx) {
     cudaFree(ctx->d_tc_w3); cudaFree(ctx->d_tc_sb3);
     cudaFree(ctx->d_tc_act[0]); cudaFree(ctx->d_tc_act[1]); cudaFree(ctx->d_inc_w); cudaFree(ctx->d_head_devs);
     for (auto& h : ctx->heads) { cudaFree(h.d_blob); cudaFree(h.d_w1_tc); }
-    cudaFree(ctx->d_gates); cudaFree(ctx->d_tails_template); cudaFree(ctx->d_peer_err);
+    cudaFree(ctx->d_gates); cudaFree(ctx->d_tails_template); cudaFree(ctx->d_peer_err); cudaFree(ctx->d_state_rejected);
+    for (auto e : ctx->state_ev) if (e) cudaEventDestroy(e);
     for (auto& b : ctx->banks) { cudaFree(b.d_mean); cudaFree(b.d_weight); cudaFree(b.d_bias); }
     for (auto e : ctx->ver_ev) if (e) cudaEventDestroy(e);
     for (auto e : ctx->rag_ev) if (e) cudaEventDestroy(e);
@@ -714,6 +879,7 @@ int oww_load_embedding(oww_ctx* ctx, const float* h_blob, size_t n_floats) {
         L.d_bias = ctx->d_emb_blob + off; off += L.cout;
     }
     ctx->emb_loaded = true;
+    ctx->emb_key = oww_fnv1a(h_blob, need * sizeof(float));
     ctx->tails_template_valid = false;                 // depends on the weights: rebuilt at the next reset
     int rc = oww_tc_pack_weights(ctx, h_blob);
     if (rc) return rc;
@@ -878,6 +1044,37 @@ int oww_reset_async(oww_ctx* ctx, const int32_t* h_stream_ids, int n, const floa
     if (!ctx) return OWW_EINVAL;
     OWW_CUDA(ctx, cudaSetDevice(ctx->device));
     return reset_enqueue(ctx, h_stream_ids, n, h_feature_init, n_rows, (cudaStream_t)stream);
+}
+
+int oww_stream_state_info(const oww_ctx* ctx, size_t* record_bytes_out, uint64_t* config_key) {
+    if (!ctx) return OWW_EINVAL;
+    if (ctx->n_streams <= 0) return oww_fail(const_cast<oww_ctx*>(ctx), OWW_EINVAL, "oww_set_streams has not been called");
+    if (record_bytes_out) *record_bytes_out = (size_t)record_bytes(ctx);
+    if (config_key) *config_key = record_key(ctx);
+    return OWW_OK;
+}
+
+int oww_export_streams(oww_ctx* ctx, const int32_t* h_stream_ids, int n, void* d_records, void* stream) {
+    if (!ctx) return OWW_EINVAL;
+    OWW_CUDA(ctx, cudaSetDevice(ctx->device));
+    return state_enqueue(ctx, h_stream_ids, n, d_records, false, (cudaStream_t)stream);
+}
+
+int oww_import_streams(oww_ctx* ctx, const int32_t* h_stream_ids, int n, const void* d_records, void* stream) {
+    if (!ctx) return OWW_EINVAL;
+    OWW_CUDA(ctx, cudaSetDevice(ctx->device));
+    return state_enqueue(ctx, h_stream_ids, n, const_cast<void*>(d_records), true, (cudaStream_t)stream);
+}
+
+int oww_stream_state_status(oww_ctx* ctx, int* n_rejected) {
+    if (!ctx || !n_rejected) return oww_fail(ctx, OWW_EINVAL, "null argument");
+    *n_rejected = 0;
+    if (!ctx->d_state_rejected) return OWW_OK;
+    OWW_CUDA(ctx, cudaSetDevice(ctx->device));
+    OWW_CUDA(ctx, cudaDeviceSynchronize());              // imports may be in flight on any stream
+    OWW_CUDA(ctx, cudaMemcpy(n_rejected, ctx->d_state_rejected, sizeof(int), cudaMemcpyDeviceToHost));
+    if (*n_rejected) OWW_CUDA(ctx, cudaMemset(ctx->d_state_rejected, 0, sizeof(int)));
+    return OWW_OK;
 }
 
 int oww_step(oww_ctx* ctx, const int16_t* d_pcm, int64_t pcm_stride, int n_chunks, float* d_scores, void* stream) {

@@ -263,6 +263,7 @@ extern "C" int oww_load_mel(oww_ctx* ctx, const float* h_window512, const float*
         if (hi + 1 > kmax) kmax = hi + 1;
     }
     ctx->mel_kmax = kmax;
+    ctx->mel_key = oww_fnv1a(fb.data(), fb.size() * sizeof(float), oww_fnv1a(win.data(), win.size() * sizeof(float)));
     auto up = [&](void** d, const void* h, size_t bytes) -> cudaError_t {
         if (!*d) { cudaError_t e = cudaMalloc(d, bytes); if (e != cudaSuccess) return e; }
         return cudaMemcpy(*d, h, bytes, cudaMemcpyHostToDevice);

@@ -61,6 +61,7 @@ struct ResetLate {           // one tails-bearing tensor of the incremental late
     uint4* next;             // tensors that gain ONE row per step: the buffer of the step after, row 0 <- template row 1
     const uint4* tmpl;       // [planes][2][Wp]
     int Wp, n_planes;
+    int off;                 // unit offset of the tensor's [planes][2][Wp] rows in the late template (and a stream record)
     LateLay lay;             // block-major layout of now / next
 };
 // late[]: one entry per tails-bearing late tensor X_l, l >= split_from (5 at the default split, 9 at split_from 3)
@@ -239,6 +240,12 @@ struct oww_ctx {
     int n_tail_tab = 0;
     int* d_reset_ids = nullptr;      // [n_streams] staging for oww_reset / oww_reset_async
     float* d_reset_init = nullptr;   // [feat_rows][96]
+
+    // stream records (oww_export_streams / oww_import_streams): configuration key inputs, id staging, rejection count
+    uint64_t mel_key = 0, emb_key = 0;           // hashes of the mel constants / embedding blob last loaded
+    int* d_state_ids = nullptr;                  // [n_streams]
+    int* d_state_rejected = nullptr;             // records an import skipped since oww_stream_state_status last read it
+    cudaEvent_t state_ev[2] = {nullptr, nullptr};   // orders the calls with own_stream
     IncPlan inc_plan;
     void* d_inc_dbg = nullptr;
     HeadDev* d_head_devs = nullptr;  // device copy of the head descriptors (fused step kernel)
@@ -288,6 +295,12 @@ struct oww_ctx {
 };
 
 int oww_fail(oww_ctx* ctx, int code, const char* fmt, ...);
+// 64-bit FNV-1a of `bytes` bytes, continuing from h (the stream record's configuration key)
+inline uint64_t oww_fnv1a(const void* p, size_t bytes, uint64_t h = 14695981039346656037ull) {
+    const unsigned char* c = static_cast<const unsigned char*>(p);
+    for (size_t i = 0; i < bytes; ++i) h = (h ^ c[i]) * 1099511628211ull;
+    return h;
+}
 #define OWW_CUDA(ctx, call)                                                                    \
     do {                                                                                       \
         cudaError_t e__ = (call);                                                              \

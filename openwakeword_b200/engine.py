@@ -57,6 +57,25 @@ class StreamEngine:
             stream = torch.cuda.current_stream(torch.device("cuda", self.device_index)).cuda_stream
         self.ctx.reset_async(stream_ids, fi, stream)
 
+    def set_streams(self, n_streams, feature_init=None):
+        """Reallocate for n_streams streams: every stream starts afresh, without a verifier or bank head (export the
+        streams to keep first, then import them and reassign)."""
+        self.ctx.set_streams(n_streams)
+        self.n_streams = n_streams
+        self.reset(feature_init)
+
+    # ---- stream records: moving live streams (include/owwb200.h, oww_export_streams) ----
+    def export_streams(self, stream_ids, stream=None):
+        """The state of streams stream_ids -> torch.uint8 [n, record bytes] on the engine's device, enqueued on the current
+        CUDA stream (or `stream`) after the steps enqueued there and the submitted host steps."""
+        return self.ctx.export_records(stream_ids, stream)
+
+    def import_streams(self, stream_ids, records, stream=None):
+        """Stream stream_ids[i] (distinct) becomes the stream record i was exported from.  records: uint8 [n, record
+        bytes] on any device or the CPU.  Records of another configuration (cnn_mode, split_from, weights) raise
+        ValueError before anything is enqueued.  Verifier and head-bank assignments stay as they are."""
+        self.ctx.import_records(stream_ids, records, stream)
+
     def step(self, d_pcm, n_chunks=1, out=None):
         torch = _torch()
         if out is None:

@@ -396,6 +396,58 @@ class Model:
             self._hist[label][:, ids] = 0.0
             self._count[label][ids] = 0
 
+    # ---- moving live streams (include/owwb200.h, oww_export_streams) ----
+    def export_streams(self, stream_ids):
+        """-> StreamState of the listed streams: their device state, the samples they hold not yet stepped and their
+        prediction history.  ``import_streams`` on a Model of the same configuration continues them exactly."""
+        ids = self._ids(stream_ids)
+        pre = self.preprocessor
+        pre._ensure_streams()
+        _, key = pre.ctx.stream_state_info()
+        records = pre.ctx.export_records(ids)
+        buf, lens = pre._ragged_pending()
+        labels = self.labels()
+        return StreamState(records, key, labels, [buf[b, :lens[b]].copy() for b in ids],
+                           {lab: self._h(lab)[0][:, ids].copy() for lab in labels},
+                           {lab: self._h(lab)[1][ids].copy() for lab in labels})
+
+    def import_streams(self, stream_ids, state):
+        """Streams stream_ids (distinct) become the streams `state` was exported from: device state, samples not yet
+        stepped and prediction history (first-5 zeroing, patience, debounce).  Their stream models and verifiers stay as
+        they are here.  ValueError: another configuration (cnn_mode, split_from, weights), another label set, or Speex
+        noise suppression on (its state cannot be exported)."""
+        ids = self._ids(stream_ids)
+        if self.speex_ns:
+            raise ValueError("streams cannot be imported with Speex noise suppression on: its state is not exported")
+        if ids.size != len(state):
+            raise ValueError(f"{ids.size} stream ids for {len(state)} exported streams")
+        if len(set(ids.tolist())) != ids.size:
+            raise ValueError("stream ids must be distinct")
+        pre = self.preprocessor
+        pre._ensure_streams()
+        if state.key != pre.ctx.stream_state_info()[1]:
+            raise ValueError("the streams were exported under another configuration (cnn_mode, split_from or weights)")
+        if list(state.labels) != self.labels():
+            raise ValueError(f"the streams were exported with the labels {list(state.labels)}, this Model has {self.labels()}")
+        pre.ctx.import_records(ids, state.records)
+        buf, lens = pre._ragged_pending()
+        for i, b in enumerate(ids):
+            p = state.pending[i]
+            buf[b] = 0
+            buf[b, :p.size] = p
+            lens[b] = p.size
+        pre._set_ragged_pending(buf, lens)
+        for lab in state.labels:
+            hist, cnt = self._h(lab)
+            hist[:, ids] = state.history[lab]
+            cnt[ids] = state.counts[lab]
+
+    def _ids(self, stream_ids):
+        ids = np.asarray(stream_ids, np.int64).ravel()
+        if ids.size and (ids.min() < 0 or ids.max() >= self.n_streams):
+            raise ValueError(f"stream ids must be in [0, {self.n_streams})")
+        return ids.astype(np.int32)
+
     def get_parent_model_from_label(self, label):
         parent = ""
         for mdl in self.class_mapping.keys():
@@ -778,6 +830,24 @@ class Model:
         out = raw[:, :, cols]
         out[:, :5, :] = 0.0
         return out, labels
+
+
+class StreamState:
+    """Streams exported by ``Model.export_streams``, in export order: ``records`` (torch.uint8 [n, record bytes], the
+    device state of include/owwb200.h), ``key`` (the configuration the records are valid under), ``labels``, and per
+    stream what the host keeps: ``pending`` (int16 samples not yet stepped), ``history`` / ``counts`` ({label: float32
+    [30, n] prediction ring, int64 [n] predictions appended}).  ``to(device)`` moves the records; on the CPU it
+    pickles."""
+
+    def __init__(self, records, key, labels, pending, history, counts):
+        self.records, self.key, self.labels = records, int(key), list(labels)
+        self.pending, self.history, self.counts = pending, history, counts
+
+    def __len__(self):
+        return len(self.pending)
+
+    def to(self, device):
+        return StreamState(self.records.to(device), self.key, self.labels, self.pending, self.history, self.counts)
 
 
 def _concat_clips(clips):
