@@ -203,7 +203,9 @@ int oww_reset(oww_ctx* ctx, const int32_t* h_stream_ids, int n, const float* h_f
  * yields 5 mel rows, utils.py:393-398) on a side stream while every other stream keeps the incremental fused kernel. */
 int oww_reset_async(oww_ctx* ctx, const int32_t* h_stream_ids, int n, const float* h_feature_init, int n_rows, void* stream);
 /* One predict() worth of work for every stream: n_chunks*1280 new samples per stream.
- * d_pcm row b starts at d_pcm + b*pcm_stride (samples).  d_scores [n_streams][oww_n_outputs]:
+ * d_pcm row b starts at d_pcm + b*pcm_stride (samples); any stride >= n_chunks*1280 and any 2-byte aligned
+ * d_pcm are accepted, a shorter stride fails with OWW_EINVAL before anything is enqueued (so does it in
+ * oww_step_host and oww_step_host_submit).  d_scores [n_streams][oww_n_outputs]:
  * per head the element-wise max over the n_chunks window positions (model.py:287-298).          */
 int oww_step(oww_ctx* ctx, const int16_t* d_pcm, int64_t pcm_stride, int n_chunks,
              float* d_scores, void* stream);

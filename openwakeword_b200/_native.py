@@ -128,6 +128,11 @@ class NativeError(RuntimeError):
     pass
 
 
+class ArgumentError(NativeError, ValueError):
+    """A buffer the library would read or write out of bounds, refused in Python before the call.  A ValueError, and a
+    NativeError like the library's own refusal of a short stride, so callers that catch either keep working."""
+
+
 def clip_schedule(chunk_size, n_padded_samples):
     """Chunks each predict call of predict_clip(chunk_size) steps on n_padded_samples samples -> int32 [calls]
     (oww_clip_schedule: pure host code, no GPU needed)."""
@@ -353,20 +358,35 @@ class Context:
         self._check(self.lib.oww_step(self.h, _ptr(d_pcm), pcm_stride, n_chunks, _ptr(d_scores), stream))
 
     def step_host(self, pcm, n_chunks, scores_out):
-        """pcm: C-contiguous int16 [B, n_chunks*1280]; scores_out: float32 [B, n_outputs]."""
-        assert pcm.dtype == np.int16 and pcm.flags.c_contiguous
-        assert scores_out.dtype == np.float32 and scores_out.flags.c_contiguous
+        """pcm: C-contiguous int16 [B, >= n_chunks*1280]; scores_out: float32 [B, n_outputs]."""
+        self._host_pcm(pcm, n_chunks)
+        self._host_scores(scores_out)
         self._check(self.lib.oww_step_host(self.h, _ptr(pcm), pcm.shape[1], n_chunks, _ptr(scores_out)))
 
     def step_host_submit(self, pcm, n_chunks):
-        assert pcm.dtype == np.int16 and pcm.flags.c_contiguous
+        self._host_pcm(pcm, n_chunks)
         t = C.c_int(-1)
         self._check(self.lib.oww_step_host_submit(self.h, _ptr(pcm), pcm.shape[1], n_chunks, C.byref(t)))
         return t.value
 
     def step_host_collect(self, ticket, scores_out):
-        assert scores_out.dtype == np.float32 and scores_out.flags.c_contiguous
+        self._host_scores(scores_out)
         self._check(self.lib.oww_step_host_collect(self.h, ticket, _ptr(scores_out)))
+
+    def _host_pcm(self, pcm, n_chunks):
+        """The library reads n_chunks*1280 samples of each of the n_streams rows of a host buffer: refuse a shorter one."""
+        if not isinstance(pcm, np.ndarray) or pcm.dtype != np.int16 or pcm.ndim != 2 or not pcm.flags.c_contiguous:
+            raise ArgumentError("pcm must be a C-contiguous int16 numpy array [n_streams, samples]")
+        if pcm.shape[0] != self.n_streams or pcm.shape[1] < int(n_chunks) * 1280:
+            raise ArgumentError(f"pcm has shape {pcm.shape}; this call reads [{self.n_streams}, {int(n_chunks) * 1280}]")
+
+    def _host_scores(self, scores_out):
+        """The collect writes n_streams rows of n_outputs floats (nothing when there are no outputs)."""
+        if not isinstance(scores_out, np.ndarray) or scores_out.dtype != np.float32 or not scores_out.flags.c_contiguous:
+            raise ArgumentError("scores_out must be a C-contiguous float32 numpy array")
+        B, n_out = self.n_streams, self.n_outputs
+        if scores_out.ndim != 2 or scores_out.shape[0] != B or (n_out and scores_out.shape[1] != n_out):
+            raise ArgumentError(f"scores_out has shape {scores_out.shape}, the handle writes [{B}, {n_out}]")
 
     def _chunks(self, chunks):
         c = np.ascontiguousarray(chunks, np.int32)
@@ -382,14 +402,14 @@ class Context:
 
     def step_host_ragged(self, pcm, chunks, scores_out):
         """pcm: C-contiguous int16 [B, >= max(chunks)*1280]; rows of scores_out of held streams are left as they were."""
-        assert pcm.dtype == np.int16 and pcm.flags.c_contiguous
-        assert scores_out.dtype == np.float32 and scores_out.flags.c_contiguous
         c = self._chunks(chunks)
+        self._host_pcm(pcm, c.max(initial=0))
+        self._host_scores(scores_out)
         self._check(self.lib.oww_step_host_ragged(self.h, _ptr(pcm), pcm.shape[1], _ptr(c), _ptr(scores_out)))
 
     def step_host_ragged_submit(self, pcm, chunks):
-        assert pcm.dtype == np.int16 and pcm.flags.c_contiguous
         c = self._chunks(chunks)
+        self._host_pcm(pcm, c.max(initial=0))
         t = C.c_int(-1)
         self._check(self.lib.oww_step_host_ragged_submit(self.h, _ptr(pcm), pcm.shape[1], _ptr(c), C.byref(t)))
         return t.value

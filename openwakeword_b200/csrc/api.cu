@@ -410,14 +410,23 @@ __global__ void emb_rows_kernel(const float* feats, int64_t clip_stride, int ini
     }
 }
 
+// rows of n_chunks * 1280 samples must not overlap: a shorter stride would step one stream on its neighbour's samples
+int stride_check(oww_ctx* ctx, int64_t pcm_stride, int n_chunks) {
+    if (pcm_stride < (int64_t)n_chunks * OWW_SAMPLES_PER_CHUNK)
+        return oww_fail(ctx, OWW_EINVAL, "pcm_stride=%lld < %d samples (%d chunks)", (long long)pcm_stride,
+                        n_chunks * OWW_SAMPLES_PER_CHUNK, n_chunks);
+    return OWW_OK;
+}
+
 int step_core(oww_ctx* ctx, const int16_t* d_pcm, int64_t pcm_stride, int n_chunks, float* d_scores, int out_stride,
               cudaStream_t s) {
     const int B = ctx->n_streams;
+    int rc;
     if (B <= 0) return oww_fail(ctx, OWW_EINVAL, "oww_set_streams has not been called");
     if (n_chunks < 1 || n_chunks > ctx->cfg.max_chunks)
         return oww_fail(ctx, OWW_EINVAL, "n_chunks=%d outside [1,%d]", n_chunks, ctx->cfg.max_chunks);
+    if ((rc = stride_check(ctx, pcm_stride, n_chunks))) return rc;
     if (!ctx->mel_loaded || !ctx->emb_loaded) return oww_fail(ctx, OWW_EINVAL, "weights not loaded");
-    int rc;
     const long slot = ctx->timing ? ctx->ev_steps % ctx->ev_slots : 0;
     cudaEvent_t* ev = ctx->timing ? &ctx->ev[4 * slot] : nullptr;
     const bool inc = ctx->cfg.cnn_mode == OWW_CNN_TC_INCREMENTAL;
@@ -657,9 +666,10 @@ int ragged_check(oww_ctx* ctx, const int32_t* h_chunks, int64_t pcm_stride, int*
         n = std::max(n, (int)h_chunks[b]);
         eq = eq && h_chunks[b] == h_chunks[0];
     }
-    if (n > 0 && pcm_stride < (int64_t)n * OWW_SAMPLES_PER_CHUNK)
-        return oww_fail(ctx, OWW_EINVAL, "pcm_stride=%lld < %d samples (max chunks %d)", (long long)pcm_stride,
-                        n * OWW_SAMPLES_PER_CHUNK, n);
+    if (n > 0) {
+        const int rc = stride_check(ctx, pcm_stride, n);
+        if (rc) return rc;
+    }
     *n_max = n; *all_equal = eq;
     return OWW_OK;
 }
@@ -1090,6 +1100,8 @@ int oww_step_host_submit(oww_ctx* ctx, const int16_t* h_pcm, int64_t pcm_stride,
     if (B <= 0) return oww_fail(ctx, OWW_EINVAL, "oww_set_streams has not been called");
     if (n_chunks < 1 || n_chunks > ctx->cfg.max_chunks)
         return oww_fail(ctx, OWW_EINVAL, "n_chunks=%d outside [1,%d]", n_chunks, ctx->cfg.max_chunks);
+    const int rc = stride_check(ctx, pcm_stride, n_chunks);
+    if (rc) return rc;
     return host_submit(ctx, h_pcm, pcm_stride, n_chunks, nullptr, ticket);
 }
 

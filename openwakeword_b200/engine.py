@@ -76,11 +76,30 @@ class StreamEngine:
         ValueError before anything is enqueued.  Verifier and head-bank assignments stay as they are."""
         self.ctx.import_records(stream_ids, records, stream)
 
+    def _check_step(self, d_pcm, n_chunks, out):
+        """-> the row stride of d_pcm, after refusing what the library would read or write out of bounds: d_pcm must be
+        int16 [n_streams, >= n_chunks*1280] with unit inner stride (rows may be column slices of a wider buffer), out
+        float32 [n_streams, n_cols] contiguous, both on the engine's device."""
+        torch = _torch()
+        dev = torch.device("cuda", self.device_index)
+        if not isinstance(d_pcm, torch.Tensor) or d_pcm.dtype != torch.int16 or d_pcm.dim() != 2 or d_pcm.device != dev:
+            raise _native.ArgumentError(f"d_pcm must be an int16 [n_streams, samples] tensor on {dev}")
+        if d_pcm.shape[0] != self.n_streams or d_pcm.shape[1] < n_chunks * 1280 or d_pcm.stride(1) != 1:
+            raise _native.ArgumentError(f"d_pcm has shape {tuple(d_pcm.shape)} and strides {d_pcm.stride()}; this call "
+                                        f"reads [{self.n_streams}, {n_chunks * 1280}] with unit inner stride")
+        if out is not None and (not isinstance(out, torch.Tensor) or out.dtype != torch.float32 or out.device != dev
+                                or tuple(out.shape) != (self.n_streams, self.n_cols) or not out.is_contiguous()):
+            raise _native.ArgumentError(f"out must be a contiguous float32 [{self.n_streams}, {self.n_cols}] tensor "
+                                        f"on {dev}")
+        # a one-stream view may carry any stride for its single row
+        return d_pcm.stride(0) if self.n_streams > 1 else max(d_pcm.stride(0), d_pcm.shape[1])
+
     def step(self, d_pcm, n_chunks=1, out=None):
         torch = _torch()
+        stride = self._check_step(d_pcm, n_chunks, out)
         if out is None:
             out = torch.empty((self.n_streams, self.n_cols), dtype=torch.float32, device=d_pcm.device)
-        self.ctx.step(d_pcm, d_pcm.stride(0), n_chunks, out, torch.cuda.current_stream(d_pcm.device).cuda_stream)
+        self.ctx.step(d_pcm, stride, n_chunks, out, torch.cuda.current_stream(d_pcm.device).cuda_stream)
         return out
 
     def step_host(self, pcm, n_chunks=1, out=None):
@@ -105,9 +124,11 @@ class StreamEngine:
         """Stream b consumes chunks[b] (host ints, 0..max_chunks) chunks, the first chunks[b]*1280 samples of row b of
         d_pcm.  A stream with 0 chunks is held: its state does not change and its row of `out` is not written."""
         torch = _torch()
+        # counts above max_chunks are the library's to refuse; the rows must hold the largest count it accepts
+        stride = self._check_step(d_pcm, min(int(np.max(chunks, initial=0)), self.ctx.max_chunks), out)
         if out is None:
             out = torch.full((self.n_streams, self.n_cols), float("nan"), dtype=torch.float32, device=d_pcm.device)
-        self.ctx.step_ragged(d_pcm, d_pcm.stride(0), chunks, out, torch.cuda.current_stream(d_pcm.device).cuda_stream)
+        self.ctx.step_ragged(d_pcm, stride, chunks, out, torch.cuda.current_stream(d_pcm.device).cuda_stream)
         return out
 
     def step_host_ragged(self, pcm, chunks, out=None):

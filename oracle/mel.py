@@ -75,19 +75,37 @@ def mel_filterbank():
     return W.T.astype(np.float32)
 
 
-def dft_filters(dtype=np.float32):
-    """Windowed DFT filters as torchlibrosa builds them: real/imag [512, 257]."""
+def dft_filters(dtype=np.float32, window=None):
+    """Windowed DFT filters as torchlibrosa builds them: real/imag [512, 257].  window: 512 taps (None: the padded
+    Hann), taken as float32 values as oww_load_mel takes them."""
     n = np.arange(N_FFT, dtype=np.float64)[:, None]
     k = np.arange(N_BINS, dtype=np.float64)[None, :]
     ang = -2.0 * np.pi * n * k / N_FFT
-    w = hann_window_padded()[:, None]
-    return (np.cos(ang) * w).astype(dtype), (np.sin(ang) * w).astype(dtype)
+    w = hann_window_padded() if window is None else _window(window)
+    return (np.cos(ang) * w[:, None]).astype(dtype), (np.sin(ang) * w[:, None]).astype(dtype)
+
+
+def _window(window):
+    w = np.asarray(window, dtype=np.float32).astype(np.float64)
+    if w.shape != (N_FFT,):
+        raise ValueError(f"window must have {N_FFT} taps, got shape {w.shape}")
+    return w
+
+
+def _filterbank(mel_fb):
+    fb = np.asarray(mel_fb, dtype=np.float32)
+    if fb.shape != (N_BINS, N_MELS):
+        raise ValueError(f"mel_fb must be [{N_BINS}, {N_MELS}], got shape {fb.shape}")
+    return fb
 
 
 _CACHE = {}
 
 
-def _consts(dtype):
+def _consts(dtype, window=None, mel_fb=None):
+    if window is not None or mel_fb is not None:        # custom constants: not cached
+        cr, ci = dft_filters(dtype, window)
+        return cr, ci, (mel_filterbank() if mel_fb is None else _filterbank(mel_fb)).astype(dtype)
     key = np.dtype(dtype).name
     if key not in _CACHE:
         cr, ci = dft_filters(dtype)
@@ -99,17 +117,23 @@ def n_frames(n_samples):
     return (n_samples - N_FFT) // HOP + 1 if n_samples >= N_FFT else 0
 
 
-def melspectrogram_raw(x, dtype=np.float32):
-    """One ``melspec_model_predict`` call on ONE clip: x int16/float [n] ->
-    dB log-mel [T, 32] *before* the x/10+2 affine.  The ``top_db`` clamp uses the
-    max over the whole output of this call (nb/conv:449-452; SURVEY.md F7)."""
+def _frames(x):
     x = np.asarray(x)
     if x.ndim != 1:
-        raise ValueError("melspectrogram_raw takes one 1-D clip")
+        raise ValueError("the frontend takes one 1-D clip")
     T = n_frames(x.shape[0])
     if T <= 0:
         raise ValueError("need at least 512 samples")
-    cr, ci, melW = _consts(dtype)
+    return x, T
+
+
+def melspectrogram_raw(x, dtype=np.float32, window=None, mel_fb=None):
+    """One ``melspec_model_predict`` call on ONE clip: x int16/float [n] ->
+    dB log-mel [T, 32] *before* the x/10+2 affine.  The ``top_db`` clamp uses the
+    max over the whole output of this call (nb/conv:449-452; SURVEY.md F7).
+    window [512] / mel_fb [257, 32]: the constants oww_load_mel takes (None: the built-in ones)."""
+    x, T = _frames(x)
+    cr, ci, melW = _consts(dtype, window, mel_fb)
     xf = x.astype(np.float32).astype(dtype)           # utils.py:199 - no scaling
     idx = np.arange(T)[:, None] * HOP + np.arange(N_FFT)[None, :]
     frames = xf[idx]                                  # [T, 512]
@@ -122,6 +146,18 @@ def melspectrogram_raw(x, dtype=np.float32):
     log_spec = log_spec - ten * np.log(np.maximum(dtype(AMIN), dtype(1.0))) / np.log(ten)
     log_spec = np.maximum(log_spec, log_spec.max() - dtype(TOP_DB))
     return log_spec.astype(np.float32)
+
+
+def mel_power_f64(x, window=None, mel_fb=None):
+    """float64 yardstick of one clip's frontend before the log: (m [T, 32], E [T]) with m[t, j] = sum_k W[k, j] |X_k|^2
+    and E[t] = sum_k |X_k|^2 over all 257 bins, X = rfft of frame t (512 samples at hop 160) times the window."""
+    x, T = _frames(x)
+    w = hann_window_padded() if window is None else _window(window)
+    fb = (mel_filterbank() if mel_fb is None else _filterbank(mel_fb)).astype(np.float64)
+    idx = np.arange(T)[:, None] * HOP + np.arange(N_FFT)[None, :]
+    X = np.fft.rfft(x.astype(np.float64)[idx] * w[None, :], axis=1)
+    p = X.real * X.real + X.imag * X.imag
+    return p @ fb, p.sum(axis=1)
 
 
 def melspectrogram(x, dtype=np.float32):
