@@ -143,6 +143,34 @@ int oww_set_verifier_clip_slot(oww_ctx* ctx, int bank, int slot);
 int oww_set_verifier_threshold(oww_ctx* ctx, int bank, float threshold);
 int oww_enable_verifiers(oww_ctx* ctx, int enabled);
 int oww_verifier_predict(oww_ctx* ctx, int bank, int slot, const float* d_feats, int n, float* d_out, void* stream);
+/* Training verifiers (custom_verifier_model.py:95-113, train_verifier_model), many users in one launch.
+ *   oww_fit_verifiers  - user u's samples are i in [h_sample_offsets[u], h_sample_offsets[u+1]) (host int64, n_users+1
+ *                        entries, non-decreasing, first >= 0); sample i is the window of n_in consecutive rows of
+ *                        d_rows [n_rows][96] (fp32, 16-byte aligned) starting at row d_first_row[i] (device int64), with
+ *                        label d_labels[i] (device uint8; nonzero = positive).  Windows may overlap; a plain [N][n_in][96]
+ *                        array is the case first_row[i] = i*n_in.  Per user, in float64: StandardScaler's mean_ and
+ *                        var_ (ddof 0; scale_ = sqrt(var_), 1 for the features scikit-learn treats as constant) ->
+ *                        d_mean, d_var [n_users][D]; the unique minimiser of 1/2 |w|^2 + C sum_i log(1 + exp(-s_i (w.z_i
+ *                        + b))), z = (x - mean_)/scale_, s_i = +-1, intercept unpenalised -> d_coef [n_users][D] (coef_,
+ *                        standardized space), d_intercept [n_users]; Newton iterations -> d_iters; d_status:
+ *                          0 converged: max |gradient| <= tol * C * n_u (scikit-learn's scaling of its tol)
+ *                          1 max_iter Newton iterations reached, or no further descent: the outputs are the last iterate
+ *                          2 n_u = 0 or one class only      3 a non-finite value, or a window not inside [0, n_rows)
+ *                        (statuses 2 and 3 zero the user's outputs).  A user's outputs are the same bits whatever the
+ *                        other users of the call.  Stream-ordered; allocation-free after the first call at a given size
+ *                        (the scratch is the handle's: do not overlap two fits of one handle on different streams).
+ *                        OWW_EINVAL before anything is enqueued for C <= 0 or non-finite, n_in outside [1, 120], max_iter
+ *                        < 1, tol < 0 or non-finite, decreasing offsets, or a misaligned d_rows.
+ *   oww_load_verifiers - slot h_slots[i] (distinct, host) of bank `bank` <- d_mean[i], d_weight[i] (device, [n][D] fp32;
+ *                        weight = coef_ / scale_) and d_bias[i] (device fp32 [n]).  Stream-ordered on `stream` and ordered
+ *                        against the handle's own stream, like oww_assign_verifier; no synchronisation.  Load slots no
+ *                        stream is assigned to, then assign them: steps in flight never see a half-written slot.     */
+int oww_fit_verifiers(oww_ctx* ctx, const float* d_rows, int64_t n_rows, int n_in, const int64_t* d_first_row,
+                      const int64_t* h_sample_offsets, const uint8_t* d_labels, int n_users, double C, int max_iter,
+                      double tol, double* d_mean, double* d_var, double* d_coef, double* d_intercept, int32_t* d_iters,
+                      int32_t* d_status, void* stream);
+int oww_load_verifiers(oww_ctx* ctx, int bank, const int32_t* h_slots, int n, const float* d_mean,
+                       const float* d_weight, const float* d_bias, void* stream);
 
 /* ---- per-stream head banks (a different wake-word model on every stream; each slot replaces one <head>.onnx session
  *      of Model.model_prediction_function, openwakeword/model.py:137-138,158-159, for the streams assigned to it) -------

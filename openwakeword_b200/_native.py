@@ -47,6 +47,9 @@ _SIGNATURES = {
     "oww_set_verifier_threshold": (C.c_int, [_P, C.c_int, C.c_float]),
     "oww_enable_verifiers": (C.c_int, [_P, C.c_int]),
     "oww_verifier_predict": (C.c_int, [_P, C.c_int, C.c_int, _P, C.c_int, _P, _P]),
+    "oww_fit_verifiers": (C.c_int, [_P, _P, C.c_int64, C.c_int, _P, _P, _P, C.c_int, C.c_double, C.c_int, C.c_double,
+                                    _P, _P, _P, _P, _P, _P, _P]),
+    "oww_load_verifiers": (C.c_int, [_P, C.c_int, _P, C.c_int, _P, _P, _P, _P]),
     "oww_add_head_bank": (C.c_int, [_P, C.POINTER(HeadDesc), C.c_int, C.POINTER(C.c_int)]),
     "oww_load_bank_head": (C.c_int, [_P, C.c_int, C.c_int, _P, C.c_size_t]),
     "oww_assign_bank_head": (C.c_int, [_P, C.c_int, _P, C.c_int, _P, _P]),
@@ -314,6 +317,64 @@ class Context:
         out = torch.empty(x.shape[0], dtype=torch.float32, device=x.device)
         self.verifier_predict(bank, slot, x, x.shape[0], out, torch.cuda.current_stream(x.device).cuda_stream)
         return out.cpu().numpy()
+
+    def _cuda(self, name, t, dtype, shape=None):
+        """Refuse a tensor the library would misread: not a contiguous `dtype` tensor on this handle's device, or (with
+        `shape`, -1 = any extent) of another shape."""
+        import torch
+        if not isinstance(t, torch.Tensor) or t.dtype != dtype or t.device != torch.device("cuda", self.device):
+            raise ArgumentError(f"{name} must be a {dtype} tensor on cuda:{self.device}")
+        if not t.is_contiguous():
+            raise ArgumentError(f"{name} must be contiguous")
+        if shape is not None and (t.dim() != len(shape) or any(s >= 0 and s != e for s, e in zip(shape, t.shape))):
+            raise ArgumentError(f"{name} has shape {tuple(t.shape)}, expected {tuple(shape)} (-1: any)")
+        return t
+
+    def fit_verifiers(self, rows, n_in, first_row, sample_offsets, labels, C=0.001, max_iter=100, tol=1e-10, stream=None):
+        """Train one verifier per user on the device (include/owwb200.h, oww_fit_verifiers).  rows: float32 [R, 96];
+        first_row: int64 [N] (sample i = rows[first_row[i] : first_row[i] + n_in]); labels: uint8 [N]; sample_offsets:
+        host int64 [U + 1], user u owns samples offsets[u] .. offsets[u+1].  -> dict of new tensors mean, var, coef
+        (float64 [U, n_in*96]), intercept (float64 [U]), iters, status (int32 [U]); enqueued on `stream` (None: the
+        device's current stream)."""
+        import torch
+        self._cuda("rows", rows, torch.float32, (-1, 96))
+        if rows.data_ptr() % 16:
+            raise ArgumentError("rows must start on a 16-byte boundary")
+        off = np.ascontiguousarray(sample_offsets, np.int64).ravel()
+        if off.size < 1 or off[0] != 0 or (np.diff(off) < 0).any():
+            raise ArgumentError("sample_offsets must start at 0 and not decrease")
+        N, U = int(off[-1]), off.size - 1
+        self._cuda("first_row", first_row, torch.int64, (N,))
+        self._cuda("labels", labels, torch.uint8, (N,))
+        if not 1 <= int(n_in) <= 120:
+            raise ArgumentError(f"n_in={n_in} outside [1, 120]")
+        dev = torch.device("cuda", self.device)
+        D = int(n_in) * 96
+        f64 = dict(dtype=torch.float64, device=dev)
+        out = {"mean": torch.empty((U, D), **f64), "var": torch.empty((U, D), **f64), "coef": torch.empty((U, D), **f64),
+               "intercept": torch.empty(U, **f64), "iters": torch.empty(U, dtype=torch.int32, device=dev),
+               "status": torch.empty(U, dtype=torch.int32, device=dev)}
+        s = torch.cuda.current_stream(dev).cuda_stream if stream is None else stream
+        self._check(self.lib.oww_fit_verifiers(self.h, _ptr(rows), rows.shape[0], int(n_in), _ptr(first_row), _ptr(off),
+                                               _ptr(labels), U, float(C), int(max_iter), float(tol), _ptr(out["mean"]),
+                                               _ptr(out["var"]), _ptr(out["coef"]), _ptr(out["intercept"]),
+                                               _ptr(out["iters"]), _ptr(out["status"]), s))
+        return out
+
+    def load_verifiers(self, bank, slots, mean, weight, bias, stream=None):
+        """Slots `slots` (distinct) of verifier bank `bank` <- float32 device tensors mean, weight [n, D] and bias [n];
+        stream-ordered (include/owwb200.h, oww_load_verifiers; stream None: the device's current stream)."""
+        import torch
+        if not 0 <= int(bank) < len(self._bank_d):
+            raise ArgumentError(f"bad verifier bank {bank}")
+        sl = np.ascontiguousarray(slots, np.int32).ravel()
+        D = self._bank_d[int(bank)]
+        self._cuda("mean", mean, torch.float32, (sl.size, D))
+        self._cuda("weight", weight, torch.float32, (sl.size, D))
+        self._cuda("bias", bias, torch.float32, (sl.size,))
+        s = torch.cuda.current_stream(torch.device("cuda", self.device)).cuda_stream if stream is None else stream
+        self._check(self.lib.oww_load_verifiers(self.h, int(bank), _ptr(sl), sl.size, _ptr(mean), _ptr(weight),
+                                                _ptr(bias), s))
 
     @property
     def n_outputs(self):

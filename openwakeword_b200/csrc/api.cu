@@ -848,6 +848,7 @@ void oww_destroy(oww_ctx* ctx) {
     free_streams(ctx);
     oww_heads_grp_free(ctx);
     oww_head_banks_free(ctx);
+    oww_verifier_fit_free(ctx);
     cudaFree(ctx->d_window); cudaFree(ctx->d_twiddle); cudaFree(ctx->d_mel_start); cudaFree(ctx->d_mel_len);
     cudaFree(ctx->d_mel_w); cudaFree(ctx->d_emb_blob); cudaFree(ctx->d_tc_w); cudaFree(ctx->d_tc_sb);
     cudaFree(ctx->d_tc_w3); cudaFree(ctx->d_tc_sb3);

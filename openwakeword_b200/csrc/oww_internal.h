@@ -183,7 +183,16 @@ struct oww_ctx {
     std::vector<VerifierBank> banks; // custom verifiers, applied after the heads (and gates, and the max over chunks)
     int* d_assign_stage = nullptr;   // [2][n_streams] staging of oww_assign_verifier (ids | slots)
     bool verifiers_on = true;        // oww_enable_verifiers: steps and clip calls enqueued while false skip the banks
-    cudaEvent_t ver_ev[2] = {nullptr, nullptr};   // orders oww_assign_verifier with own_stream
+    cudaEvent_t ver_ev[2] = {nullptr, nullptr};   // orders oww_assign_verifier / oww_load_verifiers with own_stream
+    // verifier training (verifier_fit.cu): float64 scratch (per-CTA vectors | per-sample arrays), staged sample offsets,
+    // staged slots of oww_load_verifiers; grown on demand
+    double* d_fit_scratch = nullptr;
+    size_t fit_scratch_doubles = 0;
+    int64_t* d_fit_off = nullptr;
+    size_t fit_off_cap = 0;
+    int* d_load_slots = nullptr;
+    size_t load_slots_cap = 0;
+    bool fit_attr_set = false;
 
     // streaming state
     int n_streams = 0;
@@ -295,6 +304,7 @@ struct oww_ctx {
 };
 
 int oww_fail(oww_ctx* ctx, int code, const char* fmt, ...);
+void oww_verifier_fit_free(oww_ctx* ctx);          // verifier_fit.cu: the training scratch
 // 64-bit FNV-1a of `bytes` bytes, continuing from h (the stream record's configuration key)
 inline uint64_t oww_fnv1a(const void* p, size_t bytes, uint64_t h = 14695981039346656037ull) {
     const unsigned char* c = static_cast<const unsigned char*>(p);

@@ -325,7 +325,11 @@ class Model:
         st["slots"][ids] = slot
         for b in ids:
             st["objs"][b] = v if params is not None else None
-        ctx.set_verifier_clip_slot(st["bank"], int(st["slots"][0]))
+        self._verifier_bookkeeping(name)
+
+    def _verifier_bookkeeping(self, name):
+        st = self._vbanks[name]
+        self.preprocessor.ctx.set_verifier_clip_slot(st["bank"], int(st["slots"][0]))
         self._host_verifiers.pop(name, None)
         objs = st["objs"]
         if all(o is None for o in objs):
@@ -334,6 +338,73 @@ class Model:
             self.custom_verifier_models[name] = objs[0]
         else:
             self.custom_verifier_models[name] = {b: o for b, o in enumerate(objs) if o is not None}
+
+    def train_custom_verifiers(self, name, enrollments, N=5, threshold=0.5):
+        """Train and attach a speaker verifier of model `name` for many streams at once.  enrollments: {stream id:
+        (positive clips, negative clips)}, clips as WAV paths or int16 arrays.  Each user's verifier equals what
+        ``custom_verifier_model.train_custom_verifier`` trains for that user alone on a Model of this configuration and
+        feature_init, bit for bit, when the NumPy global RNG is in the same state before that user's offset draws
+        (users draw in the order of `enrollments`; a Model without feature_init first draws one, as a fresh reference
+        Model does).  The capture runs on the bulk path with the verifier banks off, so a Model that already verifies
+        `name` captures the unverified scores.  Fitted verifiers (status 0 or 1) are loaded into `name`'s bank with
+        oww_load_verifiers and assigned to their streams; other streams, and streams whose fit failed, keep what they
+        had.  Returns {stream id: (pipeline or None, status)} (statuses of include/owwb200.h, oww_fit_verifiers).  N and
+        threshold are the reference's positive-pass settings; only N=5 and threshold=0.5 are supported."""
+        from .custom_verifier_model import enroll
+        if name not in self.models:
+            raise ValueError(f"no model named '{name}'")
+        if name in self._sbanks:
+            raise ValueError(f"custom verifier models apply to wakeword_models, not to the stream models '{name}'")
+        if self.model_outputs[name] != 1:
+            raise ValueError(f"model '{name}' has {self.model_outputs[name]} outputs; verifiers are trained on binary models")
+        if self.speex_ns is not None:
+            raise ValueError("train_custom_verifiers does not run with Speex noise suppression")
+        if N != 5 or threshold != 0.5:
+            raise ValueError("train_custom_verifiers captures as train_custom_verifier does: N=5, threshold=0.5")
+        ids = np.array([int(b) for b in enrollments], np.int64)
+        if ids.size == 0:
+            return {}
+        if ids.min() < 0 or ids.max() >= self.n_streams:
+            raise ValueError(f"stream ids must lie in [0, {self.n_streams})")
+        read = lambda c: _read_wav(c) if isinstance(c, (str, os.PathLike)) else np.asarray(c, np.int16)   # noqa: E731
+        users = [([read(c) for c in pos], [read(c) for c in neg]) for pos, neg in enrollments.values()]
+        pre, ctx = self.preprocessor, self.preprocessor.ctx
+        fi = pre._feature_init
+        if fi is None:
+            fi = pre._get_embeddings(np.random.randint(-1000, 1000, 16000 * 4).astype(np.int16))
+        if self._vbanks:
+            ctx.enable_verifiers(False)
+        try:
+            res = enroll(self, name, users, feature_init=fi)
+        finally:
+            if self._vbanks:
+                ctx.enable_verifiers(True)
+        ok = [i for i, r in enumerate(res) if r["status"] in (0, 1)]
+        if ok:
+            torch = _torch()
+            B = self.n_streams
+            st = self._vbanks.get(name)
+            if st is None:
+                pre._ensure_streams()
+                pre._verifier_banks = True
+                st = {"bank": ctx.add_verifier_bank(self._head_ids[name], B, self.custom_verifier_threshold),
+                      "slots": np.full(B, -1, np.int32), "objs": [None] * B}
+                self._vbanks[name] = st
+            sid = ids[ok]
+            others = np.ones(B, bool)
+            others[sid] = False
+            used = set(st["slots"][others].tolist())
+            slots = np.array([k for k in range(B) if k not in used][:sid.size], np.int32)
+            dev = torch.device("cuda", pre.device_index)
+            t = lambda key: torch.from_numpy(np.stack([res[i][key] for i in ok])).to(dev)   # noqa: E731
+            ctx.load_verifiers(st["bank"], slots, t("mean"), t("weight"), t("bias"),
+                               torch.cuda.current_stream(dev).cuda_stream)
+            ctx.assign_verifier(st["bank"], sid, slots, torch.cuda.current_stream(dev).cuda_stream)
+            st["slots"][sid] = slots
+            for i, b in zip(ok, sid):
+                st["objs"][b] = res[i]["pipeline"]
+            self._verifier_bookkeeping(name)
+        return {int(b): (r["pipeline"], r["status"]) for b, r in zip(ids, res)}
 
     def _reverify(self, mdl, predictions, labels, streams):
         """Verification on the host side of the stateless entry, on each stream's newest window (model.py:319-328): for
