@@ -123,20 +123,27 @@ int oww_add_gate(oww_ctx* ctx, int main_head, int verifier_head, float threshold
  * fp32) is replaced by p of the stream's verifier on the newest window; columns below it keep their value.
  *   oww_add_verifier_bank      - slots for up to `capacity` verifiers of head `head_id` (of a gated pair: the main head);
  *                                every stream starts without a verifier (slot -1).  8*D bytes per slot.
+ *   oww_add_bank_verifier_bank - the same for the per-stream head bank `head_bank` (below): its score columns, its n_in.
+ *                                A stream (or bulk row) whose head-bank slot is -1 has no model and is never verified: its
+ *                                columns stay 0.0 whatever the threshold.  Every other call here takes either kind of bank.
  *   oww_load_verifier          - copy one verifier into a slot; h_mean and h_weight hold D floats each.  Synchronises
  *                                the device first, so steps already in flight use the old contents.
  *   oww_assign_verifier        - stream-ordered, allocation-free: stream h_stream_ids[i] (NULL = all streams, then n is
  *                                the stream count) uses slot h_slots[i] (-1 = none) from the next step enqueued on `stream`
  *                                or submitted with oww_step_host / oww_step_host_submit
- *   oww_set_verifier_clip_slot - the slot oww_predict_clips applies to every clip (-1 = none, the default)
+ *   oww_set_verifier_clip_slot - the slot oww_predict_clips applies to every clip (-1 = none, the default; a bank of a
+ *                                head bank verifies clips only while that bank's clip slot is not -1)
  *   oww_set_verifier_threshold - new threshold for the steps and clip calls enqueued from now on
  *   oww_enable_verifiers       - 0: steps and clip calls enqueued from now on skip every bank (their scores are the
  *                                heads' max over the chunk windows), 1 (default): they apply them.  For a caller that
  *                                splits one long call into several steps and verifies the max itself.
  *   oww_verifier_predict       - stateless and ungated: d_feats [n][n_in][96] -> d_out[n] = predict_proba(...)[:, -1]
- * At most one bank per head.  oww_set_streams resets every assignment to -1; oww_reset / oww_reset_async leave them as
- * they are (which user owns a stream is the caller's business).  A handle without banks launches nothing for verifiers. */
+ * At most one bank per head or head bank, 16 banks of heads and 16 of head banks per handle (OWW_EUNSUPPORTED past
+ * that).  Every bank of both kinds runs in one launch per step, after everything else.  oww_set_streams resets every
+ * assignment to -1; oww_reset / oww_reset_async leave them as they are (which user owns a stream is the caller's
+ * business).  A handle without banks launches nothing for verifiers.                                                  */
 int oww_add_verifier_bank(oww_ctx* ctx, int head_id, int capacity, float threshold, int* bank_id);
+int oww_add_bank_verifier_bank(oww_ctx* ctx, int head_bank, int capacity, float threshold, int* bank_id);
 int oww_load_verifier(oww_ctx* ctx, int bank, int slot, const float* h_mean, const float* h_weight, float bias);
 int oww_assign_verifier(oww_ctx* ctx, int bank, const int32_t* h_stream_ids, int n, const int32_t* h_slots, void* stream);
 int oww_set_verifier_clip_slot(oww_ctx* ctx, int bank, int slot);
@@ -181,8 +188,9 @@ int oww_load_verifiers(oww_ctx* ctx, int bank, const int32_t* h_slots, int n, co
  * the max over the windows of a multi-chunk call; held streams of a ragged step are not written); a stream on slot -1
  * gets 0.0.  A slot runs the tensor-core heads kernel with the operand split, term count and accumulation order of
  * oww_head_predict, so it equals an ordinary head of the same weights bit for bit where that head runs that kernel
- * (oww_head_predict in cnn_modes 2/3, and streaming with reserved[0] bit 3).  Gates and custom verifiers apply to
- * ordinary heads only.  reserved[0] bit 2 (plain fp16 operands) applies to banks; bits 1 and 3 do not.
+ * (oww_head_predict in cnn_modes 2/3, and streaming with reserved[0] bit 3).  Gates apply to ordinary heads only;
+ * custom verifiers attach to a bank with oww_add_bank_verifier_bank.  reserved[0] bit 2 (plain fp16 operands) applies
+ * to banks; bits 1 and 3 do not.
  *   oww_add_head_bank        - capacity slots of shape desc, allocated here: per slot the fp16 hi/lo packing of every
  *                              layer plus the fp32 biases and LayerNorm parameters (415 672 B at 16x96 -> 64 -> 64
  *                              -> 1, 863 672 B at 16x96 -> 128 -> 128 -> 1, descriptor included).  Every stream starts on slot -1.
@@ -194,7 +202,8 @@ int oww_load_verifiers(oww_ctx* ctx, int bank, const int32_t* h_slots, int n, co
  *                              enqueued on `stream` or submitted with oww_step_host*.  The host sorts the streams by slot
  *                              and stages the work table through pinned memory (it waits for the copy of the previous
  *                              assignment of the bank).
- *   oww_set_head_bank_clip_slot - the slot oww_predict_clips / _ragged apply to every clip (-1, the default: zeros)
+ *   oww_set_head_bank_clip_slot - the slot oww_predict_clips / _ragged apply to every clip (-1, the default: zeros;
+ *                              oww_predict_clips_streams uses each clip's stream instead)
  *   oww_bank_head_predict    - stateless: d_feats [n][n_in][96] -> d_out [n][n_out] with the head of `slot`
  * oww_set_streams resets every assignment to -1; oww_reset / oww_reset_async leave them as they are.  A bad bank,
  * slot or stream id fails with OWW_EINVAL.  A handle without banks launches nothing for them.                        */
@@ -332,6 +341,13 @@ int oww_clip_schedule(int chunk_size, int64_t n_padded_samples, int32_t* h_chunk
 int oww_predict_clips_ragged(oww_ctx* ctx, const int16_t* d_pcm, const int64_t* h_offsets, int n_clips, int pad_samples,
                              int chunk_size, const float* h_feature_init, int n_rows, float* d_scores, uint8_t* d_stepped,
                              float* d_emb, void* stream);
+/* Same, but clip i is scored as stream h_clip_streams[i] (host, in [0, n_streams); repeats allowed) would score it: the
+ * head-bank slots and verifier slots that stream is assigned when the call is enqueued, instead of the clip slots, for
+ * the banks of ordinary heads and of head banks alike.  Needs oww_set_streams; the handle's streams are not touched.
+ * An id out of range, or h_clip_streams NULL with n_clips > 0, fails with OWW_EINVAL before anything is enqueued.    */
+int oww_predict_clips_streams(oww_ctx* ctx, const int16_t* d_pcm, const int64_t* h_offsets, int n_clips, int pad_samples,
+                              int chunk_size, const float* h_feature_init, int n_rows, float* d_scores, uint8_t* d_stepped,
+                              float* d_emb, const int32_t* h_clip_streams, void* stream);
 /* The slabs oww_predict_clips_ragged would run for clips of h_steps[i] chunks each (ctx may be NULL: the default
  * configuration): returns the slab count, and the steps the slabs compute and the steps the clips need.  Pure host. */
 int oww_clip_slab_plan(oww_ctx* ctx, const int32_t* h_steps, int n_clips, int64_t* h_steps_computed, int64_t* h_steps_needed);

@@ -41,6 +41,7 @@ _SIGNATURES = {
     "oww_add_head": (C.c_int, [_P, C.POINTER(HeadDesc), _P, C.c_size_t, C.POINTER(C.c_int)]),
     "oww_add_gate": (C.c_int, [_P, C.c_int, C.c_int, C.c_float]),
     "oww_add_verifier_bank": (C.c_int, [_P, C.c_int, C.c_int, C.c_float, C.POINTER(C.c_int)]),
+    "oww_add_bank_verifier_bank": (C.c_int, [_P, C.c_int, C.c_int, C.c_float, C.POINTER(C.c_int)]),
     "oww_load_verifier": (C.c_int, [_P, C.c_int, C.c_int, _P, _P, C.c_float]),
     "oww_assign_verifier": (C.c_int, [_P, C.c_int, _P, C.c_int, _P, _P]),
     "oww_set_verifier_clip_slot": (C.c_int, [_P, C.c_int, C.c_int]),
@@ -82,6 +83,7 @@ _SIGNATURES = {
     "oww_predict_clips": (C.c_int, [_P, _P, C.c_int, C.c_int, C.c_int, _P, C.c_int, _P, _P]),
     "oww_clip_schedule": (C.c_int, [C.c_int, C.c_int64, _P, C.c_int]),
     "oww_predict_clips_ragged": (C.c_int, [_P, _P, _P, C.c_int, C.c_int, C.c_int, _P, C.c_int, _P, _P, _P, _P]),
+    "oww_predict_clips_streams": (C.c_int, [_P, _P, _P, C.c_int, C.c_int, C.c_int, _P, C.c_int, _P, _P, _P, _P, _P]),
     "oww_clip_slab_plan": (C.c_int, [_P, _P, C.c_int, C.POINTER(C.c_int64), C.POINTER(C.c_int64)]),
     "oww_debug_layer": (C.c_int, [_P, _P, C.c_int, C.c_int, _P, _P]),
     "oww_debug_inc_plan": (C.c_int, [_P, C.c_int, C.c_int, _P, C.c_int]),
@@ -196,6 +198,7 @@ class Context:
         self.max_chunks = max_chunks
         self._head_n_in = []                # per head id: n_in (verifier banks take n_in*96 floats per slot)
         self._bank_d = []                   # per verifier bank: D
+        self._head_bank_n_in = []           # per head bank: n_in
 
     def close(self):
         if getattr(self, "h", None):
@@ -245,6 +248,7 @@ class Context:
         d = self._desc(n_in, dims, layernorm, final_act)
         bid = C.c_int(-1)
         self._check(self.lib.oww_add_head_bank(self.h, C.byref(d), int(capacity), C.byref(bid)))
+        self._head_bank_n_in.append(int(n_in))
         return bid.value
 
     def load_bank_head(self, bank, slot, blob):
@@ -275,6 +279,14 @@ class Context:
         bid = C.c_int(-1)
         self._check(self.lib.oww_add_verifier_bank(self.h, int(head_id), int(capacity), float(threshold), C.byref(bid)))
         self._bank_d.append(self._head_n_in[int(head_id)] * 96)
+        return bid.value
+
+    def add_bank_verifier_bank(self, head_bank, capacity, threshold):
+        """A verifier bank whose parent is head bank `head_bank` (its other calls are those of add_verifier_bank's)."""
+        bid = C.c_int(-1)
+        self._check(self.lib.oww_add_bank_verifier_bank(self.h, int(head_bank), int(capacity), float(threshold),
+                                                        C.byref(bid)))
+        self._bank_d.append(self._head_bank_n_in[int(head_bank)] * 96)
         return bid.value
 
     def load_verifier(self, bank, slot, mean, weight, bias):
@@ -560,14 +572,21 @@ class Context:
                                                41 if fi is None else fi.shape[0], _ptr(d_scores), stream))
 
     def predict_clips_ragged(self, d_pcm, offsets, pad_samples, chunk_size, feature_init, d_scores, d_stepped, d_emb=None,
-                             stream=None):
+                             stream=None, clip_streams=None):
         """offsets: host int64 [n_clips + 1] sample offsets into d_pcm; d_scores [rows][n_outputs], d_stepped uint8 [rows],
-        d_emb [steps][96] or None (include/owwb200.h, oww_predict_clips_ragged)."""
+        d_emb [steps][96] or None (include/owwb200.h, oww_predict_clips_ragged).  clip_streams: host int32 [n_clips],
+        clip i scored with the models and verifiers of stream clip_streams[i] (oww_predict_clips_streams)."""
         off = np.ascontiguousarray(offsets, np.int64)
         fi = None if feature_init is None else np.ascontiguousarray(feature_init, np.float32)
-        self._check(self.lib.oww_predict_clips_ragged(self.h, _ptr(d_pcm), _ptr(off), off.size - 1, int(pad_samples),
-                                                      int(chunk_size), _ptr(fi), 41 if fi is None else fi.shape[0],
-                                                      _ptr(d_scores), _ptr(d_stepped), _ptr(d_emb), stream))
+        args = (self.h, _ptr(d_pcm), _ptr(off), off.size - 1, int(pad_samples), int(chunk_size), _ptr(fi),
+                41 if fi is None else fi.shape[0], _ptr(d_scores), _ptr(d_stepped), _ptr(d_emb))
+        if clip_streams is None:
+            self._check(self.lib.oww_predict_clips_ragged(*args, stream))
+            return
+        cs = np.ascontiguousarray(clip_streams, np.int32)
+        if cs.size != off.size - 1:
+            raise ValueError(f"{cs.size} clip streams for {off.size - 1} clips")
+        self._check(self.lib.oww_predict_clips_streams(*args, _ptr(cs), stream))
 
     def debug_layer(self, d_windows, n, layer, d_out, stream=None):
         self._check(self.lib.oww_debug_layer(self.h, _ptr(d_windows), n, layer, _ptr(d_out), stream))

@@ -7,6 +7,7 @@
 #include <algorithm>
 #include <climits>
 #include <functional>
+#include <numeric>
 
 static thread_local std::string g_create_error;
 
@@ -1353,9 +1354,12 @@ int oww_clip_slab_plan(oww_ctx* ctx, const int32_t* h_steps, int n_clips, int64_
     return (int)plan.size();
 }
 
-int oww_predict_clips_ragged(oww_ctx* ctx, const int16_t* d_pcm, const int64_t* h_offsets, int n_clips, int pad_samples,
-                             int chunk_size, const float* h_feature_init, int n_rows, float* d_scores, uint8_t* d_stepped,
-                             float* d_emb, void* stream) {
+}  // extern "C"
+
+// oww_predict_clips_ragged (h_clip_streams == nullptr: every clip on the clip slots) and oww_predict_clips_streams
+static int predict_clips(oww_ctx* ctx, const int16_t* d_pcm, const int64_t* h_offsets, int n_clips, int pad_samples,
+                         int chunk_size, const float* h_feature_init, int n_rows, float* d_scores, uint8_t* d_stepped,
+                         float* d_emb, const int32_t* h_clip_streams, void* stream) {
     if (!ctx || !h_offsets) return oww_fail(ctx, OWW_EINVAL, "null argument");
     if (n_clips < 0 || pad_samples < 0) return oww_fail(ctx, OWW_EINVAL, "bad clip geometry");
     if (chunk_size < 1 || chunk_size > ctx->cfg.max_chunks * OWW_SAMPLES_PER_CHUNK)
@@ -1367,6 +1371,9 @@ int oww_predict_clips_ragged(oww_ctx* ctx, const int16_t* d_pcm, const int64_t* 
         if (h_offsets[i + 1] < h_offsets[i] || h_offsets[i + 1] - h_offsets[i] > INT32_MAX - 2 * (int64_t)pad_samples)
             return oww_fail(ctx, OWW_EINVAL, "offsets[%d..%d] = %lld, %lld are not monotone (or the clip is too long)", i, i + 1,
                             (long long)h_offsets[i], (long long)h_offsets[i + 1]);
+    for (int i = 0; h_clip_streams && i < n_clips; ++i)
+        if (h_clip_streams[i] < 0 || h_clip_streams[i] >= ctx->n_streams)
+            return oww_fail(ctx, OWW_EINVAL, "clip %d: stream %d outside [0,%d)", i, h_clip_streams[i], ctx->n_streams);
     if (ctx->n_out_total == 0 || n_clips == 0) return OWW_OK;
     OWW_CUDA(ctx, cudaSetDevice(ctx->device));
     cudaStream_t s = (cudaStream_t)stream;
@@ -1452,7 +1459,51 @@ int oww_predict_clips_ragged(oww_ctx* ctx, const int16_t* d_pcm, const int64_t* 
             }
         }
     }
-    const bool verify_calls = oww_verifiers_clip_active(ctx);
+    // Per-clip streams: the stream of each sorted clip (the verifiers take its slots), and per slab and head bank an item
+    // table over the slab's rows (sample = slab-local clip * K + step): clips grouped by the slot of their stream (host
+    // mirror of the assignment), each clip's rows contiguous, items of at most 64 rows of one slot.  They go up with the
+    // call's one table upload below: pageable, so the driver stages them before cudaMemcpyAsync returns (a host-side copy
+    // of about 4 bytes per row and head bank), so `tab` may be freed when the call returns.
+    const int n_hb = h_clip_streams ? (int)ctx->head_banks.size() : 0;
+    std::vector<std::vector<int>> hb_items(plan.size() * n_hb), hb_perm(plan.size() * n_hb);
+    for (size_t k = 0; k < plan.size() && n_hb; ++k) {
+        const ClipSlab& sl = plan[k];
+        const int m = sl.e - sl.b, K = sl.K;
+        for (int h = 0; h < n_hb; ++h) {
+            const std::vector<int>& assign = ctx->head_banks[h].assign;
+            std::vector<int> slot(m), lc(m);
+            for (int p = 0; p < m; ++p) slot[p] = assign[h_clip_streams[order[sl.b + p]]];
+            std::iota(lc.begin(), lc.end(), 0);
+            std::stable_sort(lc.begin(), lc.end(), [&](int x, int y) { return slot[x] < slot[y]; });
+            std::vector<int>& items = hb_items[k * n_hb + h];
+            std::vector<int>& perm = hb_perm[k * n_hb + h];
+            for (int i = 0; i < m; ++i)
+                for (int st = 0; st < K; ++st) {
+                    const int first = (int)perm.size();
+                    if (items.empty() || items[items.size() - 4] != slot[lc[i]] || first - items[items.size() - 3] == 64)
+                        items.insert(items.end(), {slot[lc[i]], first, 0, 0});
+                    items[items.size() - 2]++;
+                    perm.push_back(lc[i] * K + st);
+                }
+            while (perm.size() % 4) perm.push_back(0);               // the next table's items stay 16-byte aligned
+        }
+    }
+    const size_t sz_cs = h_clip_streams ? (size_t)n_act * 4 : 0;
+    size_t sz_hb = 0;
+    for (size_t i = 0; i < hb_items.size(); ++i) sz_hb += (hb_items[i].size() + hb_perm[i].size()) * 4;
+    const size_t hb0 = (tab.size() + sz_cs + 15) & ~(size_t)15;
+    if (h_clip_streams) tab.resize(hb0 + sz_hb);
+    int* t_cs = reinterpret_cast<int*>(tab.data() + sz_off + sz_emb0 + sz_len + sz_st + 3 * sz_calls);
+    for (int p = 0; p < (int)sz_cs / 4; ++p) t_cs[p] = h_clip_streams[order[p]];
+    std::vector<size_t> hb_at(hb_items.size());
+    for (size_t i = 0, at = hb0; i < hb_items.size(); ++i) {
+        hb_at[i] = at;
+        std::memcpy(tab.data() + at, hb_items[i].data(), hb_items[i].size() * 4);
+        at += hb_items[i].size() * 4;
+        std::memcpy(tab.data() + at, hb_perm[i].data(), hb_perm[i].size() * 4);
+        at += hb_perm[i].size() * 4;
+    }
+    const bool verify_calls = oww_verifiers_clip_active(ctx, h_clip_streams != nullptr);
     uint8_t* d_tab = nullptr;
     float *d_v = nullptr, *d_f = nullptr, *d_init = nullptr, *d_tmp = nullptr, *d_call = nullptr;
     OWW_CUDA(ctx, cudaMallocAsync(&d_tab, tab.size(), s));
@@ -1464,6 +1515,12 @@ int oww_predict_clips_ragged(oww_ctx* ctx, const int16_t* d_pcm, const int64_t* 
     const int* d_qlast = d_st + n_act;
     const int* d_k = d_qlast + n_call_rows;
     const int* d_row = d_k + n_call_rows;
+    const int* d_cs = h_clip_streams ? d_row + n_call_rows : nullptr;
+    std::vector<BankRows> bank_rows(hb_items.size());
+    for (size_t i = 0; i < hb_items.size(); ++i) {
+        const int4* items = reinterpret_cast<const int4*>(d_tab + hb_at[i]);
+        bank_rows[i] = BankRows{items, reinterpret_cast<const int*>(items + hb_items[i].size() / 4), (int)hb_items[i].size() / 4};
+    }
     OWW_CUDA(ctx, cudaMallocAsync(&d_v, max_v * sizeof(float), s));
     OWW_CUDA(ctx, cudaMallocAsync(&d_f, max_f * sizeof(float), s));
     if (max_tmp) OWW_CUDA(ctx, cudaMallocAsync(&d_tmp, max_tmp * sizeof(float), s));
@@ -1500,25 +1557,27 @@ int oww_predict_clips_ragged(oww_ctx* ctx, const int16_t* d_pcm, const int64_t* 
         if (rc) break;
         FeatSrc fs{d_f, f_stride, nullptr, -1, 0};
         fs.steps = K; fs.row0 = init_rows;
+        const BankRows* brows = n_hb ? bank_rows.data() + k * n_hb : nullptr;
+        const int* cs = d_cs ? d_cs + sl.b : nullptr;
         if (direct[k]) {
             const int64_t r0 = row0[order[sl.b]];
             float* out = d_scores + r0 * n_out;
-            if ((rc = oww_heads_all(ctx, fs, m * K, out, n_out, 0, s))) break;
-            if ((rc = oww_verifiers_apply(ctx, fs, m * K, out, n_out, true, s))) break;       // clip slot, every step
+            if ((rc = oww_heads_all(ctx, fs, m * K, out, n_out, 0, s, brows))) break;
+            if ((rc = oww_verifiers_apply(ctx, fs, m * K, out, n_out, true, s, nullptr, cs))) break;   // every step
             if (d_stepped) OWW_CUDA(ctx, cudaMemsetAsync(d_stepped + r0, 1, (size_t)m * K, s));
         } else {
             const int nc = (int)(call0[k + 1] - call0[k]);
             const int* qlast = d_qlast + call0[k];
             const int* kk = d_k + call0[k];
             const int* orow = d_row + call0[k];
-            if ((rc = oww_heads_all(ctx, fs, m * K, d_tmp, n_out, 0, s))) break;
+            if ((rc = oww_heads_all(ctx, fs, m * K, d_tmp, n_out, 0, s, brows))) break;
             if (!verify_calls) {
                 if ((rc = call_max_launch(ctx, d_tmp, n_out, qlast, kk, nc, d_scores, orow, d_stepped, s))) break;
             } else {
                 // verifiers after the max, on the call's newest window: on compact call rows, then scattered to their place
                 if ((rc = call_max_launch(ctx, d_tmp, n_out, qlast, kk, nc, d_call, nullptr, nullptr, s))) break;
                 fs.idx = qlast;
-                if ((rc = oww_verifiers_apply(ctx, fs, nc, d_call, n_out, true, s))) break;
+                if ((rc = oww_verifiers_apply(ctx, fs, nc, d_call, n_out, true, s, nullptr, cs))) break;
                 if ((rc = call_max_launch(ctx, d_call, n_out, nullptr, nullptr, nc, d_scores, orow, d_stepped, s))) break;
             }
         }
@@ -1534,6 +1593,24 @@ int oww_predict_clips_ragged(oww_ctx* ctx, const int16_t* d_pcm, const int64_t* 
     if (d_call) cudaFreeAsync(d_call, s);
     if (d_init) cudaFreeAsync(d_init, s);
     return rc;
+}
+
+extern "C" {
+
+int oww_predict_clips_ragged(oww_ctx* ctx, const int16_t* d_pcm, const int64_t* h_offsets, int n_clips, int pad_samples,
+                             int chunk_size, const float* h_feature_init, int n_rows, float* d_scores, uint8_t* d_stepped,
+                             float* d_emb, void* stream) {
+    return predict_clips(ctx, d_pcm, h_offsets, n_clips, pad_samples, chunk_size, h_feature_init, n_rows, d_scores,
+                         d_stepped, d_emb, nullptr, stream);
+}
+
+int oww_predict_clips_streams(oww_ctx* ctx, const int16_t* d_pcm, const int64_t* h_offsets, int n_clips, int pad_samples,
+                              int chunk_size, const float* h_feature_init, int n_rows, float* d_scores, uint8_t* d_stepped,
+                              float* d_emb, const int32_t* h_clip_streams, void* stream) {
+    if (!ctx) return OWW_EINVAL;
+    if (!h_clip_streams && n_clips > 0) return oww_fail(ctx, OWW_EINVAL, "null argument (h_clip_streams)");
+    return predict_clips(ctx, d_pcm, h_offsets, n_clips, pad_samples, chunk_size, h_feature_init, n_rows, d_scores,
+                         d_stepped, d_emb, h_clip_streams, stream);
 }
 
 int oww_debug_layer(oww_ctx* ctx, const float* d_windows, int n, int layer, float* d_out, void* stream) {

@@ -318,9 +318,10 @@ __global__ void max_combine_kernel(float* dst, const float* src, int n, int cols
 }
 }  // namespace
 
-int oww_heads_all(oww_ctx* ctx, const FeatSrc& src, int n, float* d_out, int out_stride, int combine_max, cudaStream_t s) {
+int oww_heads_all(oww_ctx* ctx, const FeatSrc& src, int n, float* d_out, int out_stride, int combine_max, cudaStream_t s,
+                  const BankRows* bank_rows) {
     if (ctx->heads.empty() || n <= 0) {
-        return n > 0 ? oww_head_banks_launch(ctx, src, n, d_out, out_stride, combine_max, s) : OWW_OK;
+        return n > 0 ? oww_head_banks_launch(ctx, src, n, d_out, out_stride, combine_max, s, nullptr, bank_rows) : OWW_OK;
     }
     uint32_t tc_mask = 0, cc_mask = 0;
     for (int i = 0; i < (int)ctx->heads.size(); ++i) {
@@ -353,7 +354,7 @@ int oww_heads_all(oww_ctx* ctx, const FeatSrc& src, int n, float* d_out, int out
     }
     if (tc_mask && (rc = oww_heads_tc_launch(ctx, -1, src, n, out, stride, 0, comb, s, tc_mask))) return rc;
     if (cc_mask && (rc = oww_heads_launch(ctx, -1, src, n, out, stride, 0, comb, s, cc_mask))) return rc;
-    if ((rc = oww_head_banks_launch(ctx, src, n, out, stride, comb, s))) return rc;
+    if ((rc = oww_head_banks_launch(ctx, src, n, out, stride, comb, s, nullptr, bank_rows))) return rc;
     if (!ctx->gates.empty()) {
         const int total = n * (int)ctx->gates.size();
         OWW_CUDA(ctx, oww_launch_pdl(ctx->late_pdl, gate_kernel, dim3((total + 255) / 256), dim3(256), 0, s, out, n, stride,
@@ -451,11 +452,13 @@ HtHead bank_slot_head(const HeadBank& b, int k, const float* unscale) {
 
 const HtHead& host_slot(const HeadBank& b, int k) { return reinterpret_cast<const HtHead*>(b.h_slots.data())[k]; }
 
-// items of at most kHtTile streams per slot, streams ordered by slot (-1 first) -> h[0 .. 4B) items, h[4B .. 5B) ids
+// items of at most kHtTile streams per slot, streams ordered by slot (-1 first) -> h[0 .. 4B) items, h[4B .. 5B) ids,
+// h[5B .. 6B) the slot of each stream
 int build_items(const std::vector<int>& assign, int* h) {
     const int B = (int)assign.size();
     int* perm = h + 4 * B;
     for (int b = 0; b < B; ++b) perm[b] = b;
+    std::copy(assign.begin(), assign.end(), h + 5 * B);
     std::stable_sort(perm, perm + B, [&](int x, int y) { return assign[x] < assign[y]; });
     int n = 0;
     for (int i = 0; i < B;) {
@@ -472,7 +475,7 @@ int upload_items(oww_ctx* ctx, HeadBank& b, cudaStream_t s) {
     const int B = (int)b.assign.size();
     OWW_CUDA(ctx, cudaEventSynchronize(b.stage_ev));
     b.n_items = build_items(b.assign, b.h_stage);
-    OWW_CUDA(ctx, cudaMemcpyAsync(b.d_table, b.h_stage, (size_t)5 * B * sizeof(int), cudaMemcpyHostToDevice, s));
+    OWW_CUDA(ctx, cudaMemcpyAsync(b.d_table, b.h_stage, (size_t)6 * B * sizeof(int), cudaMemcpyHostToDevice, s));
     OWW_CUDA(ctx, cudaEventRecord(b.stage_ev, s));
     return OWW_OK;
 }
@@ -488,8 +491,8 @@ int bank_alloc_streams(oww_ctx* ctx, HeadBank& b) {
     const int B = ctx->n_streams;
     if (B <= 0) return OWW_OK;
     if (!b.stage_ev) OWW_CUDA(ctx, cudaEventCreateWithFlags(&b.stage_ev, cudaEventDisableTiming));
-    OWW_CUDA(ctx, cudaMalloc(&b.d_table, (size_t)5 * B * sizeof(int)));
-    OWW_CUDA(ctx, cudaMallocHost(&b.h_stage, (size_t)5 * B * sizeof(int)));
+    OWW_CUDA(ctx, cudaMalloc(&b.d_table, (size_t)6 * B * sizeof(int)));
+    OWW_CUDA(ctx, cudaMallocHost(&b.h_stage, (size_t)6 * B * sizeof(int)));
     b.assign.assign(B, -1);
     int rc = upload_items(ctx, b, nullptr);
     if (rc) return rc;
@@ -514,10 +517,11 @@ int check_slot(oww_ctx* ctx, const HeadBank& b, int slot, bool none_ok) {
 }  // namespace
 
 int oww_head_banks_launch(oww_ctx* ctx, const FeatSrc& src, int n, float* d_out, int out_stride, int combine_max,
-                          cudaStream_t s, const int* d_step) {
+                          cudaStream_t s, const int* d_step, const BankRows* rows) {
     if (n <= 0) return OWW_OK;
     const bool streams = src.count && src.base == ctx->d_feat_ring && n == ctx->n_streams;
-    for (const HeadBank& b : ctx->head_banks) {
+    for (size_t i = 0; i < ctx->head_banks.size(); ++i) {
+        const HeadBank& b = ctx->head_banks[i];
         const int np = std::max(16, b.shape.tc_layers[0].NP);
         HeadsTcArgs a;
         std::memset(&a, 0, sizeof(a));
@@ -531,6 +535,12 @@ int oww_head_banks_launch(oww_ctx* ctx, const FeatSrc& src, int n, float* d_out,
             a.slots = reinterpret_cast<const HtHead*>(b.d_slots);
             a.step = d_step;
             rc = ht_run<true>(ctx, a, np, dim3(b.n_items), s);
+        } else if (rows) {                   // rows of the bulk path, each on the slot of its clip's stream
+            a.head[0] = bank_slot_head(b, 0, nullptr);
+            a.items = rows[i].items;
+            a.perm = rows[i].perm;
+            a.slots = reinterpret_cast<const HtHead*>(b.d_slots);
+            rc = rows[i].n_items > 0 ? ht_run<true>(ctx, a, np, dim3(rows[i].n_items), s) : OWW_OK;
         } else if (b.clip_slot >= 0) {       // rows of the bulk path: every row on the clip slot
             a.head[0] = host_slot(b, b.clip_slot);
             rc = ht_run<false>(ctx, a, np, dim3((n + kHtTile - 1) / kHtTile), s);
@@ -542,6 +552,11 @@ int oww_head_banks_launch(oww_ctx* ctx, const FeatSrc& src, int n, float* d_out,
         if (rc) return rc;
     }
     return OWW_OK;
+}
+
+const int* oww_head_bank_stream_slots(const oww_ctx* ctx, int bank) {
+    const HeadBank& b = ctx->head_banks[bank];
+    return b.d_table ? b.d_table + 5 * ctx->n_streams : nullptr;
 }
 
 int oww_head_banks_alloc_streams(oww_ctx* ctx) {

@@ -79,6 +79,8 @@ struct Gate { int main_col, ver_col; float thr; };
 // feature rows (D = n_in*96):  p = 1 / (1 + exp(-(bias + sum_j (x_j - mean_j) * weight_j)))
 struct VerifierBank {
     int head_id, col0, n_cols, n_in, capacity;
+    int head_bank = -1;              // >= 0: the parent is this head bank (head_id = -1); a row whose bank slot is -1
+                                     // (no model) is never verified
     float thr;                       // columns >= thr (fp32) are replaced by p
     float* d_mean = nullptr;         // [capacity][D]
     float* d_weight = nullptr;       // [capacity][D]
@@ -103,7 +105,7 @@ struct HeadBank {
     std::vector<uint8_t> loaded;     // per slot: a head has been loaded
     int clip_slot = -1;              // slot the bulk clip path applies to every clip
     // streams: host mirror of the assignment, and the item table the steps read ([B] int4 {slot, first, rows, 0} |
-    // [B] stream ids ordered by slot), staged through pinned memory
+    // [B] stream ids ordered by slot | [B] slot per stream, read by the bank's verifiers), staged through pinned memory
     std::vector<int> assign;
     int n_items = 0;
     int* d_table = nullptr;
@@ -476,10 +478,16 @@ int oww_stage_head(oww_ctx* ctx, const oww_head_desc* desc, const float* h_blob,
 
 // ---- heads_tc.cu: every Linear layer on the tensor cores (wgmma, fp16 hi/lo split operands, fp32 accumulate) ----
 int oww_heads_tc_pack(oww_ctx* ctx, Head& h, const float* w1);
+// per head bank, an item table over rows of the bulk path: CTA i runs items[i] = {slot, first, rows, 0} on the rows
+// perm[first .. first + rows) (row = FeatSrc sample = output row)
+struct BankRows { const int4* items; const int* perm; int n_items; };
 // every head bank on n rows: streams of the handle (src = the feature ring, n = n_streams: each stream's slot) or rows
-// of the bulk path (the clip slot).  d_step != nullptr (ragged step): streams with d_step[b] == 0 are not written.
+// of the bulk path (rows[i] != nullptr: head bank i's item table; otherwise the clip slot).  d_step != nullptr (ragged
+// step): streams with d_step[b] == 0 are not written.
 int oww_head_banks_launch(oww_ctx* ctx, const FeatSrc& src, int n, float* d_out, int out_stride, int combine_max,
-                          cudaStream_t s, const int* d_step = nullptr);
+                          cudaStream_t s, const int* d_step = nullptr, const BankRows* rows = nullptr);
+// head bank `bank`'s slot of every stream on the device ([n_streams], -1 = none), uploaded with its item table
+const int* oww_head_bank_stream_slots(const oww_ctx* ctx, int bank);
 // (re)allocate every bank's per-stream table for ctx->n_streams streams, every stream on slot -1 (synchronous)
 int oww_head_banks_alloc_streams(oww_ctx* ctx);
 void oww_head_banks_free(oww_ctx* ctx);
@@ -495,18 +503,21 @@ int oww_feat16_resync(oww_ctx* ctx, const int* d_ids, int n, cudaStream_t s);
 uint32_t oww_heads_grp_covered(oww_ctx* ctx);
 uint32_t oww_heads_grp_bulk(oww_ctx* ctx, const FeatSrc& src, int n, float* d_out, int out_stride, cudaStream_t s, int* rc_out);
 int oww_heads_grp_launch(oww_ctx* ctx, int back, int n, float* d_out, int out_stride, int combine_max, cudaStream_t s);
-// every head (tensor-core kernel where a head allows it, heads.cu otherwise) + the verifier gates
-int oww_heads_all(oww_ctx* ctx, const FeatSrc& src, int n, float* d_out, int out_stride, int combine_max, cudaStream_t s);
+// every head (tensor-core kernel where a head allows it, heads.cu otherwise) + the verifier gates; bank_rows: as in
+// oww_head_banks_launch
+int oww_heads_all(oww_ctx* ctx, const FeatSrc& src, int n, float* d_out, int out_stride, int combine_max, cudaStream_t s,
+                  const BankRows* bank_rows = nullptr);
 
 // ---- verifier.cu: custom verifier banks ----
 // every bank of the handle on n rows of final scores (one launch; nothing when the handle has no bank).  The window of
 // row r is the newest n_in rows of `src` (FeatSrc sample r).  Its slot is bank.d_assign[r] for streams (rows = streams
-// of the handle), or bank.clip_slot for clips (rows = (clip, step) of the bulk path).
+// of the handle), or bank.clip_slot for clips (rows = (clip, step) of the bulk path).  d_clip_streams != nullptr
+// (clips): row r takes the slots of stream d_clip_streams[q / src.steps], q = its sliding sample (src.idx[r] or r).
 // d_chunks != nullptr (ragged step): rows with d_chunks[r] == 0 did not step and are skipped.
 int oww_verifiers_apply(oww_ctx* ctx, const FeatSrc& src, int n, float* d_scores, int out_stride, bool clips,
-                        cudaStream_t s, const int* d_chunks = nullptr);
+                        cudaStream_t s, const int* d_chunks = nullptr, const int* d_clip_streams = nullptr);
 // (re)allocate every bank's per-stream assignment for ctx->n_streams streams, all -1
 int oww_verifiers_alloc_streams(oww_ctx* ctx);
-// true when oww_verifiers_apply(..., clips = true) would launch (a bank with a clip slot, verifiers enabled)
-bool oww_verifiers_clip_active(const oww_ctx* ctx);
+// true when oww_verifiers_apply(..., clips = true, d_clip_streams given or not) would launch
+bool oww_verifiers_clip_active(const oww_ctx* ctx, bool clip_streams = false);
 void oww_verifiers_free_streams(oww_ctx* ctx);

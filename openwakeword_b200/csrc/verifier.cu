@@ -5,6 +5,9 @@
 //   p = 1 / (1 + exp(-(b + sum_j (x_j - mu_j) * w_j)))     mu = mean_, w = coef_ / scale_, b = intercept_
 // and keeps the centred form: with a small scale_ the folded bias b - sum mu_j w_j cancels catastrophically in fp32.
 //
+// The parent is an ordinary head (oww_add_verifier_bank) or a per-stream head bank (oww_add_bank_verifier_bank).  A row
+// whose head-bank slot is -1 has no model: its columns stay 0.0 and it is never verified, whatever the threshold.
+//
 // One warp per row (a stream, a (clip, step) of the bulk path, or a window of the stateless call) and bank.  The warp
 // reads the row's slot and the parent's score columns and leaves when no column reaches the threshold, so a step in
 // which nothing fires costs one slot and one score read per stream.  Otherwise it streams the D = n_in*96 features, mu
@@ -15,12 +18,15 @@
 
 namespace {
 
-constexpr int kVerMaxBanks = 16;        // one bank per parent head, at most 16 heads per handle
+constexpr int kVerMaxHeadBanks = 16;    // banks of ordinary heads: one per parent head, at most 16 heads per handle
+constexpr int kVerMaxBankBanks = 16;    // banks of head banks: one per head bank
+constexpr int kVerMaxBanks = kVerMaxHeadBanks + kVerMaxBankBanks;   // 32 x 64 B (VerBankDev) = 2 KB of kernel parameters
 constexpr int kVerWarps = 8;
 
 struct VerBankDev {
     const float* mean; const float* weight; const float* bias;
-    const int* assign;                  // per-row slot, or nullptr: every row uses slot_all
+    const int* assign;                  // per-stream slot, or nullptr: every row uses slot_all
+    const int* hslot;                   // parent head bank: its slot per stream (rows on -1 are not verified), or nullptr
     int slot_all, col0, n_cols, n_in;
     float thr;
 };
@@ -30,6 +36,7 @@ struct VerArgs {
     int n; float* out; int out_stride;
     int gated;                          // 0: stateless call, write p to column col0 of every row unconditionally
     const int* step;                    // ragged step: rows with step[r] == 0 were held (their score row is not written)
+    const int* clip_streams;            // bulk rows: stream of each slab-local clip (its slots apply), or nullptr
 };
 
 __global__ void __launch_bounds__(kVerWarps * 32) verifier_kernel(const __grid_constant__ VerArgs a) {
@@ -38,7 +45,10 @@ __global__ void __launch_bounds__(kVerWarps * 32) verifier_kernel(const __grid_c
     const int r = blockIdx.x * kVerWarps + (threadIdx.x >> 5);
     if (r >= a.n || (a.step && a.step[r] == 0)) return;
     const VerBankDev& B = a.bank[blockIdx.y];
-    const int slot = B.assign ? B.assign[r] : B.slot_all;
+    int b = r;                          // the stream whose slots row r takes
+    if (a.clip_streams) b = a.clip_streams[(a.src.idx ? a.src.idx[r] : r) / a.src.steps];
+    if (B.hslot && B.hslot[b] < 0) return;
+    const int slot = B.assign ? B.assign[b] : B.slot_all;
     if (slot < 0) return;
     float* o = a.out + (int64_t)r * a.out_stride + B.col0;
     uint32_t mine = 0;                  // bit k: column 32k + lane reaches the threshold
@@ -88,30 +98,38 @@ int launch(oww_ctx* ctx, const VerArgs& a, int n_banks, cudaStream_t s) {
     return OWW_OK;
 }
 
-VerBankDev bank_dev(const VerifierBank& b, int slot_all, const int* assign) {
-    return VerBankDev{b.d_mean, b.d_weight, b.d_bias, assign, slot_all, b.col0, b.n_cols, b.n_in, b.thr};
+VerBankDev bank_dev(const VerifierBank& b, int slot_all, const int* assign, const int* hslot) {
+    return VerBankDev{b.d_mean, b.d_weight, b.d_bias, assign, hslot, slot_all, b.col0, b.n_cols, b.n_in, b.thr};
+}
+
+// the one-clip-slot bulk path: the bank's clip slot verifies, under a model (a head bank's clip slot is not -1)
+bool clip_slot_on(const oww_ctx* ctx, const VerifierBank& b) {
+    return b.clip_slot >= 0 && (b.head_bank < 0 || ctx->head_banks[b.head_bank].clip_slot >= 0);
 }
 
 }  // namespace
 
 int oww_verifiers_apply(oww_ctx* ctx, const FeatSrc& src, int n, float* d_scores, int out_stride, bool clips,
-                        cudaStream_t s, const int* d_chunks) {
+                        cudaStream_t s, const int* d_chunks, const int* d_clip_streams) {
     if (ctx->banks.empty() || !ctx->verifiers_on) return OWW_OK;
     VerArgs a;
     a.step = d_chunks;
+    a.clip_streams = clips ? d_clip_streams : nullptr;
+    const bool per_stream = !clips || d_clip_streams;
     int nb = 0;
     for (const VerifierBank& b : ctx->banks) {
-        if (clips && b.clip_slot < 0) continue;              // no clip verifier for this head
-        a.bank[nb++] = bank_dev(b, b.clip_slot, clips ? nullptr : b.d_assign);
+        if (!per_stream && !clip_slot_on(ctx, b)) continue;   // no clip verifier for this head
+        const int* hslot = per_stream && b.head_bank >= 0 ? oww_head_bank_stream_slots(ctx, b.head_bank) : nullptr;
+        a.bank[nb++] = bank_dev(b, b.clip_slot, per_stream ? b.d_assign : nullptr, hslot);
     }
     a.src = src; a.n = n; a.out = d_scores; a.out_stride = out_stride; a.gated = 1;
     return launch(ctx, a, nb, s);
 }
 
-bool oww_verifiers_clip_active(const oww_ctx* ctx) {
+bool oww_verifiers_clip_active(const oww_ctx* ctx, bool clip_streams) {
     if (!ctx->verifiers_on) return false;
     for (const VerifierBank& b : ctx->banks)
-        if (b.clip_slot >= 0) return true;
+        if (clip_streams || clip_slot_on(ctx, b)) return true;
     return false;
 }
 
@@ -132,20 +150,13 @@ void oww_verifiers_free_streams(oww_ctx* ctx) {
     cudaFree(ctx->d_assign_stage); ctx->d_assign_stage = nullptr;
 }
 
-extern "C" {
+namespace {
 
-int oww_add_verifier_bank(oww_ctx* ctx, int head_id, int capacity, float threshold, int* bank_id) {
-    if (!ctx) return OWW_EINVAL;
-    if (head_id < 0 || head_id >= (int)ctx->heads.size()) return oww_fail(ctx, OWW_EINVAL, "bad head_id %d", head_id);
-    if (capacity < 1 || capacity > (1 << 20)) return oww_fail(ctx, OWW_EINVAL, "capacity %d outside [1, 2^20]", capacity);
-    if (ctx->banks.size() >= (size_t)kVerMaxBanks) return oww_fail(ctx, OWW_EUNSUPPORTED, "at most %d verifier banks per handle", kVerMaxBanks);
-    for (const VerifierBank& o : ctx->banks)     // two banks would write the same score columns in one launch
-        if (o.head_id == head_id) return oww_fail(ctx, OWW_EINVAL, "head %d already has a verifier bank", head_id);
+// allocate bank b (its parent, columns, n_in, capacity and threshold set) and append it
+int add_bank(oww_ctx* ctx, VerifierBank b, int* bank_id) {
+    const int capacity = b.capacity;
     OWW_CUDA(ctx, cudaSetDevice(ctx->device));
-    const Head& h = ctx->heads[head_id];
-    VerifierBank b;
-    b.head_id = head_id; b.col0 = h.col0; b.n_cols = h.n_out; b.n_in = h.desc.n_in; b.capacity = capacity; b.thr = threshold;
-    const size_t D = (size_t)h.desc.n_in * 96;
+    const size_t D = (size_t)b.n_in * 96;
     auto fail = [&](cudaError_t e) {
         cudaFree(b.d_mean); cudaFree(b.d_weight); cudaFree(b.d_bias); cudaFree(b.d_assign);
         return oww_fail(ctx, OWW_ENOMEM, "verifier bank of %d slots: %s", capacity, cudaGetErrorString(e));
@@ -165,6 +176,46 @@ int oww_add_verifier_bank(oww_ctx* ctx, int head_id, int capacity, float thresho
     ctx->banks.push_back(b);
     if (bank_id) *bank_id = (int)ctx->banks.size() - 1;
     return OWW_OK;
+}
+
+int count_banks(const oww_ctx* ctx, bool of_head_banks) {
+    int n = 0;
+    for (const VerifierBank& o : ctx->banks) n += (o.head_bank >= 0) == of_head_banks;
+    return n;
+}
+
+}  // namespace
+
+extern "C" {
+
+int oww_add_verifier_bank(oww_ctx* ctx, int head_id, int capacity, float threshold, int* bank_id) {
+    if (!ctx) return OWW_EINVAL;
+    if (head_id < 0 || head_id >= (int)ctx->heads.size()) return oww_fail(ctx, OWW_EINVAL, "bad head_id %d", head_id);
+    if (capacity < 1 || capacity > (1 << 20)) return oww_fail(ctx, OWW_EINVAL, "capacity %d outside [1, 2^20]", capacity);
+    if (count_banks(ctx, false) >= kVerMaxHeadBanks)
+        return oww_fail(ctx, OWW_EUNSUPPORTED, "at most %d verifier banks per handle", kVerMaxHeadBanks);
+    for (const VerifierBank& o : ctx->banks)     // two banks would write the same score columns in one launch
+        if (o.head_id == head_id) return oww_fail(ctx, OWW_EINVAL, "head %d already has a verifier bank", head_id);
+    const Head& h = ctx->heads[head_id];
+    VerifierBank b;
+    b.head_id = head_id; b.col0 = h.col0; b.n_cols = h.n_out; b.n_in = h.desc.n_in; b.capacity = capacity; b.thr = threshold;
+    return add_bank(ctx, b, bank_id);
+}
+
+int oww_add_bank_verifier_bank(oww_ctx* ctx, int head_bank, int capacity, float threshold, int* bank_id) {
+    if (!ctx) return OWW_EINVAL;
+    if (head_bank < 0 || head_bank >= (int)ctx->head_banks.size())
+        return oww_fail(ctx, OWW_EINVAL, "bad head bank %d", head_bank);
+    if (capacity < 1 || capacity > (1 << 20)) return oww_fail(ctx, OWW_EINVAL, "capacity %d outside [1, 2^20]", capacity);
+    if (count_banks(ctx, true) >= kVerMaxBankBanks)
+        return oww_fail(ctx, OWW_EUNSUPPORTED, "at most %d verifier banks of head banks per handle", kVerMaxBankBanks);
+    for (const VerifierBank& o : ctx->banks)
+        if (o.head_bank == head_bank) return oww_fail(ctx, OWW_EINVAL, "head bank %d already has a verifier bank", head_bank);
+    const HeadBank& h = ctx->head_banks[head_bank];
+    VerifierBank b;
+    b.head_id = -1; b.head_bank = head_bank;
+    b.col0 = h.shape.col0; b.n_cols = h.shape.n_out; b.n_in = h.shape.desc.n_in; b.capacity = capacity; b.thr = threshold;
+    return add_bank(ctx, b, bank_id);
 }
 
 int oww_load_verifier(oww_ctx* ctx, int bank, int slot, const float* h_mean, const float* h_weight, float bias) {
@@ -248,10 +299,10 @@ int oww_verifier_predict(oww_ctx* ctx, int bank, int slot, const float* d_feats,
     if (n < 0) return oww_fail(ctx, OWW_EINVAL, "n=%d", n);
     OWW_CUDA(ctx, cudaSetDevice(ctx->device));
     VerArgs a;
-    a.bank[0] = bank_dev(b, slot, nullptr);
+    a.bank[0] = bank_dev(b, slot, nullptr, nullptr);
     a.bank[0].col0 = 0; a.bank[0].n_cols = 1;
     a.src = FeatSrc{d_feats, (int64_t)b.n_in * 96, nullptr, -1, 0};
-    a.n = n; a.out = d_out; a.out_stride = 1; a.gated = 0; a.step = nullptr;
+    a.n = n; a.out = d_out; a.out_stride = 1; a.gated = 0; a.step = nullptr; a.clip_streams = nullptr;
     return launch(ctx, a, 1, (cudaStream_t)stream);
 }
 

@@ -243,14 +243,15 @@ def enrollment_clip(pos, neg, passes):
     return np.concatenate(parts), (np.concatenate(lab) if lab else np.zeros(0, np.int8))
 
 
-def enroll(oww, model_name, users, feature_init=None):
+def enroll(oww, model_name, users, feature_init=None, streams=None):
     """Capture and fit the verifiers of several users on one Model, without touching its streams or banks.
 
     users: list of (positive clips, negative clips), each clip an int16 array.  For every user in turn, the NumPy
     global RNG draws that user's pass offsets (``enrollment_passes``); the user's passes become one clip
     (``enrollment_clip``).  All users' clips then run in one bulk call (padding 0, 1280-sample calls) from the Model's
     fresh state, and every captured window becomes a first-row index into [feature_init | that user's embedding rows]
-    for one ``oww_fit_verifiers`` call.  Returns per user a dict: pipeline (None unless status 0 or 1), status, passes,
+    for one ``oww_fit_verifiers`` call.  streams (stream models): user u's clip is scored by stream streams[u]'s own
+    model (``Model.predict_clips(..., streams=)``).  Returns per user a dict: pipeline (None unless status 0 or 1), status, passes,
     counts (windows captured per pass), and the device parameters mean, weight (float32 [D]) and bias (float32)."""
     n_in = oww.model_inputs[model_name]
     passes = [enrollment_passes([len(c) for c in pos], [len(c) for c in neg]) for pos, neg in users]
@@ -258,7 +259,7 @@ def enroll(oww, model_name, users, feature_init=None):
     pcm = np.concatenate([c for c, _ in clips])
     offsets = np.concatenate([[0], np.cumsum([c.size for c, _ in clips])]).astype(np.int64)
     scores, row_off, labels, emb, step_off, fi = oww._predict_ragged(pcm, offsets, 0, 1280, feature_init,
-                                                                     want_features=True)
+                                                                     want_features=True, streams=streams)
     if model_name not in labels:          # a multi-output model has no label of its own name
         raise KeyError(model_name)
     if n_in > len(fi):

@@ -148,6 +148,11 @@ class StreamEngine:
         """Slots for `capacity` verifiers of entry `head_index` of `heads`; every stream starts without one."""
         return self.ctx.add_verifier_bank(self.head_ids[head_index], capacity, threshold)
 
+    def add_bank_verifier_bank(self, bank, capacity, threshold=0.1):
+        """Slots for `capacity` verifiers of head bank `bank` (add_head_bank); a stream verifies only while it has a
+        model in that bank."""
+        return self.ctx.add_bank_verifier_bank(bank, capacity, threshold)
+
     def load_verifier(self, bank, slot, verifier):
         """verifier: a pickle path or pipeline of train_verifier_model's form, or (mean, weight, bias) arrays, on the head's
         n_in*96 features.  Synchronises the device: steps already enqueued use the slot's old contents."""

@@ -37,9 +37,10 @@ class Model:
     @re_arg({"wakeword_model_paths": "wakeword_models"})
     def __init__(self, wakeword_models=[], class_mapping_dicts=[], enable_speex_noise_suppression=False,
                  vad_threshold=0, custom_verifier_models={}, custom_verifier_threshold=0.1,
-                 inference_framework="b200", stream_models={}, stream_model_capacity=256, **kwargs):
+                 inference_framework="b200", stream_models={}, stream_model_capacity=256, stream_verifiers={}, **kwargs):
         """stream_models: {name: {stream id or None (every stream): model}} - a model per stream under one label
-        (``set_stream_model``); stream_model_capacity: distinct models each such name can hold at once."""
+        (``set_stream_model``); stream_model_capacity: distinct models each such name can hold at once;
+        stream_verifiers: {name of stream_models: {stream id or None: verifier}} (``set_stream_verifier``)."""
         if inference_framework != "b200":
             raise ValueError(f"openwakeword_b200.Model only provides inference_framework='b200' (got '{inference_framework}')")
         pretrained_paths = _registry.get_pretrained_model_paths(inference_framework)
@@ -69,6 +70,8 @@ class Model:
         self.custom_verifier_models = {}
         self._host_verifiers = {}      # parent -> verifier run per stream on the host (not device-runnable)
         self._vbanks = {}              # parent -> {"bank", "slots" int32[B], "objs"}: verifiers on the device (verifier.cu)
+        self._svbanks = {}             # stream-model name -> the same, for a verifier bank of its head bank
+        self.stream_verifiers = {}     # stream-model name -> verifier, or {stream id: verifier} (set_stream_verifier)
         self.custom_verifier_threshold = custom_verifier_threshold
         self._head_ids = {}            # parent -> head id a verifier bank attaches to (a gated pair: its main head)
         device_verifiers = {}          # parent -> {stream id or None (all): verifier}
@@ -184,6 +187,14 @@ class Model:
             for b, m in per_stream.items():
                 if b is not None:
                     self.set_stream_model(name, m, [b])
+        for name, per_stream in stream_verifiers.items():
+            if name not in self._sbanks:
+                raise ValueError(f"stream verifiers apply to stream models; '{name}' is not one")
+            if None in per_stream:
+                self.set_stream_verifier(name, per_stream[None])
+            for b, v in per_stream.items():
+                if b is not None:
+                    self.set_stream_verifier(name, v, [b])
 
     # ---- a model per stream (include/owwb200.h, oww_add_head_bank) ----
     @staticmethod
@@ -267,7 +278,7 @@ class Model:
     def custom_verifier_threshold(self, value):
         """applies to the device banks from the next call on, as to the host loop"""
         self._verifier_threshold = value
-        for st in self._vbanks.values():
+        for st in list(self._vbanks.values()) + list(self._svbanks.values()):
             self.preprocessor.ctx.set_verifier_threshold(st["bank"], value)
 
     def _device_params(self, name, verifier):
@@ -289,6 +300,31 @@ class Model:
             raise ValueError(f"no model named '{name}'")
         if name in self._sbanks:
             raise ValueError(f"custom verifier models apply to wakeword_models, not to the stream models '{name}'")
+        self._set_device_verifier(name, verifier, streams, False)
+
+    def set_stream_verifier(self, name, verifier, streams=None):
+        """Attach, replace or remove (``verifier=None``) the verifier of stream models `name` on `streams` (stream ids;
+        None = every stream) from the next call on: where a stream's score is >= custom_verifier_threshold, p of its
+        verifier on the newest window replaces it.  A stream without a model (slot -1 of the bank) is never verified and
+        stays 0.0.  `verifier`: a pickle path or pipeline of train_verifier_model's form on the model's input window;
+        anything else raises ValueError.  Slots are shared and freed as in ``set_custom_verifier``, and
+        ``stream_verifiers[name]`` follows as ``custom_verifier_models[name]`` does there."""
+        if name not in self._sbanks:
+            raise ValueError(f"no stream models named '{name}'")
+        self._set_device_verifier(name, verifier, streams, True)
+
+    def _new_vbank(self, name, stream_model):
+        pre, B = self.preprocessor, self.n_streams
+        pre._ensure_streams()
+        pre._verifier_banks = True
+        thr = self.custom_verifier_threshold
+        bank = (pre.ctx.add_bank_verifier_bank(self._sbanks[name]["bank"], B, thr) if stream_model
+                else pre.ctx.add_verifier_bank(self._head_ids[name], B, thr))
+        st = {"bank": bank, "slots": np.full(B, -1, np.int32), "objs": [None] * B}
+        (self._svbanks if stream_model else self._vbanks)[name] = st
+        return st
+
+    def _set_device_verifier(self, name, verifier, streams, stream_model):
         B = self.n_streams
         ids = np.arange(B) if streams is None else np.unique(np.asarray(streams, np.int64).ravel())
         if ids.size == 0:
@@ -296,7 +332,7 @@ class Model:
         if ids.min() < 0 or ids.max() >= B:
             raise ValueError(f"stream ids must lie in [0, {B})")
         ctx = self.preprocessor.ctx
-        st = self._vbanks.get(name)
+        st = (self._svbanks if stream_model else self._vbanks).get(name)
         params = None
         if verifier is not None:
             v = load_verifier(verifier) if isinstance(verifier, (str, os.PathLike)) else verifier
@@ -306,14 +342,10 @@ class Model:
                                  f"model's {self.model_inputs[name]}-row input window, runs on the device")
         if st is None:
             if params is None:
-                if ids.size == B and self._host_verifiers.pop(name, None) is not None:
+                if not stream_model and ids.size == B and self._host_verifiers.pop(name, None) is not None:
                     self.custom_verifier_models.pop(name, None)
                 return
-            self.preprocessor._ensure_streams()
-            self.preprocessor._verifier_banks = True
-            st = {"bank": ctx.add_verifier_bank(self._head_ids[name], B, self.custom_verifier_threshold),
-                  "slots": np.full(B, -1, np.int32), "objs": [None] * B}
-            self._vbanks[name] = st
+            st = self._new_vbank(name, stream_model)
         slot = -1
         if params is not None:           # a slot no other stream uses (one always exists: capacity = n_streams)
             others = np.ones(B, bool)
@@ -325,19 +357,21 @@ class Model:
         st["slots"][ids] = slot
         for b in ids:
             st["objs"][b] = v if params is not None else None
-        self._verifier_bookkeeping(name)
+        self._verifier_bookkeeping(name, stream_model)
 
-    def _verifier_bookkeeping(self, name):
-        st = self._vbanks[name]
+    def _verifier_bookkeeping(self, name, stream_model=False):
+        st = (self._svbanks if stream_model else self._vbanks)[name]
+        attr = self.stream_verifiers if stream_model else self.custom_verifier_models
         self.preprocessor.ctx.set_verifier_clip_slot(st["bank"], int(st["slots"][0]))
-        self._host_verifiers.pop(name, None)
+        if not stream_model:
+            self._host_verifiers.pop(name, None)
         objs = st["objs"]
         if all(o is None for o in objs):
-            self.custom_verifier_models.pop(name, None)
+            attr.pop(name, None)
         elif all(o is objs[0] for o in objs):
-            self.custom_verifier_models[name] = objs[0]
+            attr[name] = objs[0]
         else:
-            self.custom_verifier_models[name] = {b: o for b, o in enumerate(objs) if o is not None}
+            attr[name] = {b: o for b, o in enumerate(objs) if o is not None}
 
     def train_custom_verifiers(self, name, enrollments, N=5, threshold=0.5):
         """Train and attach a speaker verifier of model `name` for many streams at once.  enrollments: {stream id:
@@ -350,11 +384,22 @@ class Model:
         oww_load_verifiers and assigned to their streams; other streams, and streams whose fit failed, keep what they
         had.  Returns {stream id: (pipeline or None, status)} (statuses of include/owwb200.h, oww_fit_verifiers).  N and
         threshold are the reference's positive-pass settings; only N=5 and threshold=0.5 are supported."""
-        from .custom_verifier_model import enroll
         if name not in self.models:
             raise ValueError(f"no model named '{name}'")
         if name in self._sbanks:
             raise ValueError(f"custom verifier models apply to wakeword_models, not to the stream models '{name}'")
+        return self._train_verifiers(name, enrollments, N, threshold, False)
+
+    def train_stream_verifiers(self, name, enrollments, N=5, threshold=0.5):
+        """``train_custom_verifiers`` for stream models `name`: each user's capture clip is scored by the model of that
+        user's stream, and the fitted verifiers go to `name`'s stream verifiers (``set_stream_verifier``).  A stream
+        without a model raises ValueError, as do multi-output models."""
+        if name not in self._sbanks:
+            raise ValueError(f"no stream models named '{name}'")
+        return self._train_verifiers(name, enrollments, N, threshold, True)
+
+    def _train_verifiers(self, name, enrollments, N, threshold, stream_model):
+        from .custom_verifier_model import enroll
         if self.model_outputs[name] != 1:
             raise ValueError(f"model '{name}' has {self.model_outputs[name]} outputs; verifiers are trained on binary models")
         if self.speex_ns is not None:
@@ -366,30 +411,32 @@ class Model:
             return {}
         if ids.min() < 0 or ids.max() >= self.n_streams:
             raise ValueError(f"stream ids must lie in [0, {self.n_streams})")
+        if stream_model:
+            slots = self._sbanks[name]["slots"]
+            bare = ids if slots is None else ids[slots[ids] < 0]
+            if bare.size:
+                raise ValueError(f"stream models '{name}': streams {bare.tolist()} have no model to enroll against")
         read = lambda c: _read_wav(c) if isinstance(c, (str, os.PathLike)) else np.asarray(c, np.int16)   # noqa: E731
         users = [([read(c) for c in pos], [read(c) for c in neg]) for pos, neg in enrollments.values()]
         pre, ctx = self.preprocessor, self.preprocessor.ctx
         fi = pre._feature_init
         if fi is None:
             fi = pre._get_embeddings(np.random.randint(-1000, 1000, 16000 * 4).astype(np.int16))
-        if self._vbanks:
+        banks = self._vbanks or self._svbanks
+        if banks:
             ctx.enable_verifiers(False)
         try:
-            res = enroll(self, name, users, feature_init=fi)
+            res = enroll(self, name, users, feature_init=fi, streams=ids if stream_model else None)
         finally:
-            if self._vbanks:
+            if banks:
                 ctx.enable_verifiers(True)
         ok = [i for i, r in enumerate(res) if r["status"] in (0, 1)]
         if ok:
             torch = _torch()
             B = self.n_streams
-            st = self._vbanks.get(name)
+            st = (self._svbanks if stream_model else self._vbanks).get(name)
             if st is None:
-                pre._ensure_streams()
-                pre._verifier_banks = True
-                st = {"bank": ctx.add_verifier_bank(self._head_ids[name], B, self.custom_verifier_threshold),
-                      "slots": np.full(B, -1, np.int32), "objs": [None] * B}
-                self._vbanks[name] = st
+                st = self._new_vbank(name, stream_model)
             sid = ids[ok]
             others = np.ones(B, bool)
             others[sid] = False
@@ -403,7 +450,7 @@ class Model:
             st["slots"][sid] = slots
             for i, b in zip(ok, sid):
                 st["objs"][b] = res[i]["pipeline"]
-            self._verifier_bookkeeping(name)
+            self._verifier_bookkeeping(name, stream_model)
         return {int(b): (r["pipeline"], r["status"]) for b, r in zip(ids, res)}
 
     def _reverify(self, mdl, predictions, labels, streams):
@@ -412,12 +459,12 @@ class Model:
         calls split into several device steps (> max_chunks chunks: those run without the banks, and the max over all
         their chunk windows is verified here, once).  Of `streams` (bool [B]): those with a device verifier and a label >=
         the threshold."""
-        st = self._vbanks[mdl]
+        st = self._vbanks.get(mdl) or self._svbanks[mdl]
         thr = np.float32(self.custom_verifier_threshold)
         hit = np.zeros(self.n_streams, bool)
         for lab in labels:
             hit |= predictions[lab] >= thr
-        hit &= (st["slots"] >= 0) & streams
+        hit &= (st["slots"] >= 0) & streams & self._has_model(mdl, np.arange(self.n_streams))
         for slot in np.unique(st["slots"][hit]):
             bs = np.nonzero(hit & (st["slots"] == slot))[0]
             feats = np.concatenate([self.preprocessor.get_features(self.model_inputs[mdl], stream=int(b)) for b in bs])
@@ -425,6 +472,13 @@ class Model:
             for lab in labels:
                 sel = predictions[lab][bs] >= thr
                 predictions[lab][bs[sel]] = p[sel]
+
+    def _has_model(self, mdl, streams):
+        """bool per stream id: `mdl` scores it (always, but for stream models on slot -1: never verified)"""
+        sb = self._sbanks.get(mdl)
+        if sb is None:
+            return np.ones(len(streams), bool)
+        return np.zeros(len(streams), bool) if sb["slots"] is None else sb["slots"][streams] >= 0
 
     # ---- per-label history (model.py:198; vectorised over streams) ----
     def _reset_history(self):
@@ -633,7 +687,7 @@ class Model:
                 labels = list(self.class_mapping[mdl].values())
                 for int_label, cls in self.class_mapping[mdl].items():
                     predictions[cls] = pred[:, int(int_label)].copy()
-            if mdl in self._vbanks and reverify.any():
+            if (mdl in self._vbanks or mdl in self._svbanks) and reverify.any():
                 self._reverify(mdl, predictions, labels, reverify)   # otherwise the device verified the step it ran
 
             if self._host_verifiers != {}:
@@ -720,28 +774,30 @@ class Model:
                         hits[lbl].append(context)
         return {lbl: np.vstack(v) for lbl, v in hits.items() if v}
 
-    def predict_clips(self, clips, padding=1, feature_init=None, chunk_size=1280):
+    def predict_clips(self, clips, padding=1, feature_init=None, chunk_size=1280, streams=None):
         """Bulk path (extension; SURVEY.md F9): each clip from a fresh state, in one device call.  ``clips``: an int16
         [N,S] array or tensor, or a sequence of 1-D int16 arrays of any lengths.  Returns a list (per clip) of lists (per
         call) of {label: float}, i.e. what predict_clip(clip, padding, chunk_size) would return for each clip after
-        reset(feature_init)."""
+        reset(feature_init).  streams (N stream ids, or None: stream 0's models and verifiers): clip i is predicted as
+        stream streams[i] would predict it, with its stream models and device verifiers."""
         torch = _torch()
-        if chunk_size == CHUNK and (isinstance(clips, torch.Tensor) or (isinstance(clips, np.ndarray) and clips.ndim == 2)):
+        if streams is None and chunk_size == CHUNK and (isinstance(clips, torch.Tensor)
+                                                        or (isinstance(clips, np.ndarray) and clips.ndim == 2)):
             scores, labels = self.predict_clips_array(clips, padding, feature_init)
             return [[{lab: float(scores[c, s, j]) for j, lab in enumerate(labels)} for s in range(scores.shape[1])]
                     for c in range(scores.shape[0])]
         pcm, offsets = _concat_clips(clips)
-        scores, row_off, labels = self.predict_clips_ragged(pcm, offsets, padding, chunk_size, feature_init)
+        scores, row_off, labels = self.predict_clips_ragged(pcm, offsets, padding, chunk_size, feature_init, streams)
         return _rows_to_dicts(scores, row_off, labels)
 
-    def predict_clips_ragged(self, pcm, offsets, padding=1, chunk_size=1280, feature_init=None):
+    def predict_clips_ragged(self, pcm, offsets, padding=1, chunk_size=1280, feature_init=None, streams=None):
         """Array form of the bulk path over clips of any lengths: clip i is ``pcm[offsets[i]:offsets[i+1]]`` (int16 1-D
         array or tensor, int64 offsets).  Returns (float32 [rows, n_labels], int64 row_offsets [N+1], labels): clip i's
         rows ``row_offsets[i]:row_offsets[i+1]`` are the predictions predict_clip(clip, padding, chunk_size) returns after
-        reset(feature_init), one per call."""
-        return self._predict_ragged(pcm, offsets, padding, chunk_size, feature_init)[:3]
+        reset(feature_init), one per call.  streams: as in predict_clips."""
+        return self._predict_ragged(pcm, offsets, padding, chunk_size, feature_init, streams=streams)[:3]
 
-    def _predict_ragged(self, pcm, offsets, padding, chunk_size, feature_init, want_features=False):
+    def _predict_ragged(self, pcm, offsets, padding, chunk_size, feature_init, want_features=False, streams=None):
         """-> (scores, row_offsets, labels, embeddings [steps, 96] or None, step_offsets [N+1], feature_init rows).
         One oww_predict_clips_ragged call; the host fills the rows of calls that stepped no chunk as Model.predict does
         (the previous prediction of single-output heads, zeros for multi-class heads, re-verified), then zeroes each
@@ -758,6 +814,13 @@ class Model:
                              f"(max_chunks={self.preprocessor.max_chunks}); construct the Model with a larger max_chunks")
         offsets = np.ascontiguousarray(offsets, np.int64)
         n = offsets.size - 1
+        if streams is not None:
+            streams = np.asarray(streams, np.int64).ravel()
+            if streams.size != n:
+                raise ValueError(f"{streams.size} stream ids for {n} clips")
+            if streams.size and (streams.min() < 0 or streams.max() >= self.n_streams):
+                raise ValueError(f"stream ids must lie in [0, {self.n_streams})")
+            self.preprocessor._ensure_streams()
         pad = 16000 * int(padding)
         lengths = np.diff(offsets)
         calls = np.array([_native.clip_schedule(chunk_size, int(x) + 2 * pad).size for x in lengths], np.int64)
@@ -784,10 +847,11 @@ class Model:
             d = torch.from_numpy(np.ascontiguousarray(pcm, np.int16)).to(dev)
         raw = torch.zeros((rows, max(self._n_cols, 1)), dtype=torch.float32, device=dev)
         stepped = torch.zeros(rows, dtype=torch.uint8, device=dev)
-        need_emb = want_features or (chunk_size < CHUNK and bool(self._vbanks))
+        need_emb = want_features or (chunk_size < CHUNK and bool(self._vbanks or self._svbanks))
         emb = torch.zeros((int(step_off[-1]), 96), dtype=torch.float32, device=dev) if need_emb else None
         self.preprocessor.ctx.predict_clips_ragged(d, offsets, pad, chunk_size, fi, raw, stepped, emb,
-                                                   torch.cuda.current_stream(d.device).cuda_stream)
+                                                   torch.cuda.current_stream(d.device).cuda_stream,
+                                                   clip_streams=streams)
         out = raw.cpu().numpy()[:, cols]
         stepped = stepped.cpu().numpy().astype(bool)
         emb = emb.cpu().numpy() if emb is not None else None
@@ -804,28 +868,28 @@ class Model:
             single = np.asarray(single)
             out[rep] = np.where(single[None, :], out[src[rep]], np.float32(0.0))
             if rep.any():
-                self._reverify_rows(out, rep, local, clip, step_off, chunk_size, emb, fi, labels)
+                self._reverify_rows(out, rep, local, clip, step_off, chunk_size, emb, fi, labels, streams)
         return out, row_off, labels, emb, step_off, fi
 
-    def _reverify_rows(self, out, rep, local, clip, step_off, chunk_size, emb, fi, labels):
+    def _reverify_rows(self, out, rep, local, clip, step_off, chunk_size, emb, fi, labels, streams=None):
         """_reverify on the rows of calls that stepped no chunk: labels of a device-verified model >= the threshold take
-        the verifier's p on the clip's newest window ([feature_init rows | the clip's embeddings] up to the last step)."""
+        the verifier's p on the clip's newest window ([feature_init rows | the clip's embeddings] up to the last step).
+        A row takes the slots of its clip's stream (streams[clip], or stream 0)."""
         thr = np.float32(self.custom_verifier_threshold)
-        for mdl, st in self._vbanks.items():
-            slot = int(st["slots"][0])
-            if slot < 0:
-                continue
+        row_stream = np.zeros(out.shape[0], np.int64) if streams is None else streams[clip]
+        for mdl, st in list(self._vbanks.items()) + list(self._svbanks.items()):
+            slots = np.where(self._has_model(mdl, row_stream), st["slots"][row_stream], -1)
             js = [j for j, lab in enumerate(labels) if self.get_parent_model_from_label(lab) == mdl]
-            hit_rows = np.nonzero(rep & (out[:, js] >= thr).any(axis=1))[0]
-            if hit_rows.size == 0:
-                continue
+            hit = rep & (slots >= 0) & (out[:, js] >= thr).any(axis=1)
             n_in = self.model_inputs[mdl]
-            done = (local[hit_rows] + 1) * chunk_size // CHUNK       # chunks stepped up to and including the call
-            feats = np.stack([_window(fi, emb, step_off[clip[r]], int(k), n_in) for r, k in zip(hit_rows, done)])
-            p = self.preprocessor.ctx.verifier_predict_host(st["bank"], slot, feats)
-            for j in js:
-                sel = out[hit_rows, j] >= thr
-                out[hit_rows[sel], j] = p[sel]
+            for slot in np.unique(slots[hit]):
+                hit_rows = np.nonzero(hit & (slots == slot))[0]
+                done = (local[hit_rows] + 1) * chunk_size // CHUNK       # chunks stepped up to and including the call
+                feats = np.stack([_window(fi, emb, step_off[clip[r]], int(k), n_in) for r, k in zip(hit_rows, done)])
+                p = self.preprocessor.ctx.verifier_predict_host(st["bank"], int(slot), feats)
+                for j in js:
+                    sel = out[hit_rows, j] >= thr
+                    out[hit_rows[sel], j] = p[sel]
 
     def _positive_frames_bulk(self, pcms, threshold=0.5, return_type="features"):
         """_get_positive_prediction_frames over many clips in one device call (padding 0, 1280-sample calls): per clip
