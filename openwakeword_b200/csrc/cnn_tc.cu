@@ -20,6 +20,7 @@
 // producer.  Persistent CTAs, grid = #SMs.
 #include "oww_internal.h"
 #include "tc_common.cuh"
+#include <algorithm>
 #include <cmath>
 #include <cstring>
 
@@ -610,9 +611,10 @@ int launch_tc_blk(oww_ctx* ctx, const TcBlkArgs& a, cudaStream_t s) {
 
 }  // namespace
 
-// Host-side packing per layer 1..19: fp16 weights [3][CGP][NP][8] + padded scale/bias (TERMS = 1), and for the split
-// variant the hi and lo blocks of W * 2^s (s per layer: max |W| * 2^s in [2^13, 2^14), so the lo parts are normal fp16
-// numbers) with 2^-s folded exactly into the scale.
+// Host-side packing per layer 1..19: fp16 weights [3][CGP][NP][8] of W * 2^s + padded scale/bias (TERMS = 1), and for
+// the split variant the hi and lo blocks of W * 2^s (the lo parts are normal fp16 numbers), both with 2^-s folded
+// exactly into the scale (s = oww_weight_scale_exponent).  A BN-folded layer is the same function for any scale of its
+// weights; packed this way its fp16 weights neither overflow nor fall into the subnormal range whatever that scale is.
 int oww_tc_pack_weights(oww_ctx* ctx, const float* h_blob) {
     size_t off = 0, total_h = 0, total_f = 0;
     for (int li = 1; li < OWW_N_CONV; ++li) {
@@ -632,10 +634,7 @@ int oww_tc_pack_weights(oww_ctx* ctx, const float* h_blob) {
         if (li == 0) continue;
         const int cg = L.cin / 8, cgp = (cg + 1) & ~1, np = (L.cout + 15) & ~15;
         ctx->tc_w_off[li] = oh; ctx->tc_sb_off[li] = of;
-        float amax = 0.f;
-        for (size_t i = 0; i < nw; ++i) amax = std::fmax(amax, std::fabs(w[i]));
-        int sexp = 0;
-        if (amax > 0.f && std::isfinite(amax)) { int e; std::frexp(amax, &e); sexp = 14 - e; if (sexp > 24) sexp = 24; if (sexp < -8) sexp = -8; }
+        const int sexp = oww_weight_scale_exponent(w, nw);
         const float up = std::ldexp(1.0f, sexp), down = std::ldexp(1.0f, -sexp);
         const size_t term = (size_t)3 * cgp * np * 8;
         std::fill(hw.begin() + oh, hw.begin() + oh + term, __float2half(0.f));     // pad octets of the chained order stay zero
@@ -649,15 +648,15 @@ int oww_tc_pack_weights(oww_ctx* ctx, const float* h_blob) {
                         // plain weights of a layer with an odd plane count: chained octet order (tc_conv_kernel, TERMS = 1)
                         int oc = j * cgp + g;
                         if ((cg & 1) && g < cg) oc = j == 0 ? (g < cg - 1 ? g : cg) : j == 1 ? (g == 0 ? cg - 1 : cg + g) : 2 * cg + g;
-                        if (!(cg & 1) || g < cg) hw[oh + ((size_t)oc * np + n) * 8 + e] = __float2half_rn(v);
                         const __half hi = __float2half_rn(v * up);
+                        if (!(cg & 1) || g < cg) hw[oh + ((size_t)oc * np + n) * 8 + e] = hi;
                         hw3[2 * oh + at] = hi;
                         hw3[2 * oh + term + at] = __float2half_rn(v * up - __half2float(hi));
                     }
         oh += term;
         for (int n = 0; n < np; ++n) {
-            hf[of + n] = n < L.cout ? sc[n] : 0.f; hf[of + np + n] = n < L.cout ? bi[n] : 0.f;
-            hf3[of + n] = hf[of + n] * down; hf3[of + np + n] = hf[of + np + n];
+            hf[of + n] = n < L.cout ? sc[n] * down : 0.f; hf[of + np + n] = n < L.cout ? bi[n] : 0.f;
+            hf3[of + n] = hf[of + n]; hf3[of + np + n] = hf[of + np + n];
         }
         of += 2 * (size_t)np;
     }

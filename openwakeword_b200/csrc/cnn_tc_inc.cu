@@ -23,6 +23,7 @@
 #include "oww_internal.h"
 #include "tc_common.cuh"
 #include "mel_device.cuh"
+#include <cmath>
 #include <cstring>
 #include <type_traits>
 
@@ -943,7 +944,8 @@ int oww_inc_build_plan(oww_ctx* ctx, int G, int n_streams, int n_layers, IncPlan
 }
 
 int oww_inc_setup(oww_ctx* ctx, const float* h_blob) {
-    // packed blob for the fused kernel: per layer fp16 [3][CGP][NP][8] | scale[NP] | bias[NP], 128-byte aligned
+    // packed blob for the fused kernel: per layer fp16 [3][CGP][NP][8] of W * 2^s | scale[NP] * 2^-s | bias[NP], 128-byte
+    // aligned; s as oww_tc_pack_weights packs it, so streaming stays bit-identical to the window and clip passes
     IncPlan P;
     int rc = oww_inc_build_plan(ctx, 1, 1, OWW_N_CONV, &P);
     if (rc) return rc;
@@ -956,6 +958,8 @@ int oww_inc_setup(oww_ctx* ctx, const float* h_blob) {
         off += nw + 2 * (size_t)C.cout;
         if (li == 0) continue;
         const IncLayer& L = P.L[li];
+        const int sexp = oww_weight_scale_exponent(w, nw);
+        const float up = std::ldexp(1.0f, sexp), down = std::ldexp(1.0f, -sexp);
         __half* hw = reinterpret_cast<__half*>(blob.data() + L.w_off);
         // octet (tap j, plane g) -> position in the packed block [octet][np][8].  Even plane count: tap-major with the
         // pad plane zero.  Odd plane count: the chained order of the MMA loop in tc_inc_kernel -
@@ -973,10 +977,10 @@ int oww_inc_setup(oww_ctx* ctx, const float* h_blob) {
                     for (int e = 0; e < 8; ++e) {
                         const int c = g * 8 + e;
                         const float v = (c < C.cin && n < C.cout) ? w[((size_t)j * C.cin + c) * C.cout + n] : 0.f;
-                        hw[(((size_t)octet_at(j, g)) * L.np + n) * 8 + e] = __float2half_rn(v);
+                        hw[(((size_t)octet_at(j, g)) * L.np + n) * 8 + e] = __float2half_rn(v * up);
                     }
         float* sb = reinterpret_cast<float*>(blob.data() + L.w_off + (size_t)3 * L.cgp * L.np * 16);
-        for (int n = 0; n < L.np; ++n) { sb[n] = n < C.cout ? sc[n] : 0.f; sb[L.np + n] = n < C.cout ? bi[n] : 0.f; }
+        for (int n = 0; n < L.np; ++n) { sb[n] = n < C.cout ? sc[n] * down : 0.f; sb[L.np + n] = n < C.cout ? bi[n] : 0.f; }
     }
     if (!ctx->d_inc_w) OWW_CUDA(ctx, cudaMalloc(&ctx->d_inc_w, blob.size()));
     OWW_CUDA(ctx, cudaMemcpy(ctx->d_inc_w, blob.data(), blob.size(), cudaMemcpyHostToDevice));

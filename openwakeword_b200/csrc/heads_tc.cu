@@ -220,16 +220,6 @@ __global__ void __launch_bounds__(kHtThreads, 1) heads_tc_kernel(const __grid_co
     }
 }
 
-// exponent s with amax * 2^s in [2^13, 2^14): the fp16 lo parts of W * 2^s stay in the normal range
-int scale_exponent(const float* w, size_t n) {
-    float amax = 0.f;
-    for (size_t i = 0; i < n; ++i) amax = std::fmax(amax, std::fabs(w[i]));
-    if (!(amax > 0.f) || !std::isfinite(amax)) return 0;
-    int e;
-    std::frexp(amax, &e);                                          // amax = m * 2^e, m in [0.5, 1)
-    return std::min(24, std::max(-8, 14 - e));
-}
-
 // fp16 hi/lo of rows [k0, k0 + Kp) of w[K][D] * 2^s in K-major core-matrix order: [term][octet Kp/8][NP][8]
 void pack_block(const float* w, int K, int D, int k0, int Kp, int NP, float sc, __half* out) {
     const size_t term = (size_t)(Kp / 8) * NP * 8;
@@ -261,7 +251,7 @@ void pack_layers(Head& h, const float* blob, std::vector<__half>& packed) {
         T.K = K; T.D = D; T.NP = (D + 15) & ~15;
         T.Kp = l == 0 ? 96 : (K + 15) & ~15;
         const float* w = blob + h.w_off[l];
-        const int s = scale_exponent(w, (size_t)K * D);
+        const int s = oww_weight_scale_exponent(w, (size_t)K * D);
         const float sc = std::ldexp(1.0f, s);
         T.unscale = std::ldexp(1.0f, -s);
         T.w_off = (uint32_t)(packed.size() * sizeof(__half));

@@ -1,12 +1,26 @@
 // Internal declarations shared by the .cu translation units of libowwb200.so.
 #pragma once
 #include <cuda_runtime.h>
+#include <algorithm>
+#include <cmath>
 #include <cstdint>
 #include <cstdio>
 #include <string>
 #include <utility>
 #include <vector>
 #include "owwb200.h"
+
+// Exponent s of the fp16 weight packings (conv layers, head Linear layers): max |w| * 2^s in [2^13, 2^14), clamped to
+// [-8, 24].  W * 2^s is packed and 2^-s folded exactly into the scale that follows, so the fp16 weights (and the lo
+// parts of hi/lo splits) stay in the normal range whatever the scale of the weights.
+inline int oww_weight_scale_exponent(const float* w, size_t n) {
+    float amax = 0.f;
+    for (size_t i = 0; i < n; ++i) amax = std::fmax(amax, std::fabs(w[i]));
+    if (!(amax > 0.f) || !std::isfinite(amax)) return 0;
+    int e;
+    std::frexp(amax, &e);                                          // amax = m * 2^e, m in [0.5, 1)
+    return std::min(24, std::max(-8, 14 - e));
+}
 
 #define OWW_N_CONV 20
 #define OWW_FFT_N 512
