@@ -309,6 +309,60 @@ int oww_export_streams(oww_ctx* ctx, const int32_t* h_stream_ids, int n, void* d
 int oww_import_streams(oww_ctx* ctx, const int32_t* h_stream_ids, int n, const void* d_records, void* stream);
 int oww_stream_state_status(oww_ctx* ctx, int* n_rejected);
 
+/* ---- detections on the device (openwakeword/model.py:303-363: the prediction history, the zeroing of the first five
+ *      predictions, patience, debounce_time, the repeat of the previous prediction below 1280 samples, the threshold) ---
+ * A detector turns the score matrix of a step into detections, per stream, with the history on the device.  It has
+ * n_labels labels (<= 256); label j reads score column `column` (-1: always 0.0, a class mapped past its head's outputs)
+ * and has `repeats` (1: a label of a single-output head, which repeats its previous prediction when fewer than 1280
+ * samples were prepared; 0: a class of a multi-output head, which reads 0.0 then), `threshold` (NaN = none) and `patience`
+ * (0 = none, else 1..30); debounce_time (seconds, 0 = off) is one per handle.  Per stream the handle keeps the last 30
+ * final predictions of every label and one count of predictions appended since the stream's reset (11 labels: 1324 B).
+ *   oww_set_detector  - configure, reconfigure or (n_labels 0) remove the detector.  Synchronises the device.  The same
+ *                       columns and repeats as before keep the histories (the reference takes thresholds, patience and
+ *                       debounce per predict call); another label set starts every stream with an empty history.  Before
+ *                       oww_set_streams the state is allocated by that call.  OWW_EINVAL: a column outside
+ *                       -1..oww_n_outputs-1, a patience outside 0..30, a patience without a threshold, a patience together
+ *                       with a debounce_time, n_labels > 256.
+ *   oww_detect        - one prediction for every stream from d_scores [n_streams][oww_n_outputs] (what oww_step* wrote).
+ *                       Stream b prepared p = h_prepared[b] samples in this call (host int32 [n_streams]; NULL: p =
+ *                       prepared_all for every stream) - what AudioFeatures.__call__ returns:
+ *                         p < 0:      the stream is skipped: nothing is read, appended or reported (a stream held with 0
+ *                                     chunks in oww_step_ragged), and its row of d_final is not written;
+ *                         p >= 1280:  prediction = d_scores[b][column] (0.0 for column -1);
+ *                         0 <= p < 1280: the newest history entry of a `repeats` label (0.0 when the history is empty),
+ *                                     0.0 for any other label; the row of d_scores is not read.
+ *                       Then, with count = predictions appended so far and the history = the last min(count, 30) of them:
+ *                       (1) count < 5 -> 0; (2) patience: the prediction is nonzero and fewer than `patience` of the last
+ *                       min(patience, count) entries are >= threshold -> 0; (3) else debounce: the label has a threshold,
+ *                       the prediction is nonzero and >= threshold, and one of the last n entries is >= threshold -> 0,
+ *                       n = ceil(debounce_time / (p / 16000)) in double (the whole history for p == 0), capped by the
+ *                       entries present; (4) the prediction is appended, count += 1.  Comparisons are in fp32.
+ *                       d_final [n_streams][n_labels] (may be NULL) receives the predictions.  d_n_events (may be NULL,
+ *                       then so is d_events) receives the number of (stream, label) pairs whose label has a threshold and
+ *                       whose prediction is >= it; d_events (may be NULL with max_events 0) receives the first
+ *                       min(that number, max_events) of them in ascending (stream, label) order - the order never
+ *                       depends on scheduling - with `index` = the stream's count before the append.  Memory past those
+ *                       is not written.  Stream-ordered, no allocation, no synchronisation: one launch, two with
+ *                       d_n_events.  h_prepared is staged through a ring of four pinned buffers: a call waits (host
+ *                       side) for the copy of the call four staging uses back.  OWW_EINVAL before anything is enqueued:
+ *                       no detector (or no streams), d_scores NULL, max_events < 0 or > 0 without d_events, d_events
+ *                       without d_n_events, d_final and d_n_events both NULL.
+ *   oww_detector_export / _import - the history of streams h_stream_ids[i] <-> d_hist [n][n_labels][30] (oldest first:
+ *                       entry k was appended 30 - k predictions ago; zeros where the stream has fewer) and d_counts [n];
+ *                       stream-ordered on `stream`.  Duplicate ids fail an import with OWW_EINVAL.  Stream records
+ *                       (oww_export_streams) do not carry this history: move it with these two calls.
+ * oww_reset / oww_reset_async clear the history of the streams they reset (one more launch), oww_set_streams that of
+ * all.  The count is rebased by a multiple of 30 past 2^30, like the ring counters.  A handle without a detector
+ * launches nothing for it.                                                                                             */
+typedef struct oww_detect_label { int32_t column; int32_t repeats; float threshold; int32_t patience; } oww_detect_label;
+typedef struct oww_event { int32_t stream; int32_t label; float score; int32_t index; } oww_event;
+int oww_set_detector(oww_ctx* ctx, const oww_detect_label* h_labels, int n_labels, double debounce_time);
+int oww_detect(oww_ctx* ctx, const float* d_scores, int prepared_all, const int32_t* h_prepared, float* d_final,
+               oww_event* d_events, int max_events, int32_t* d_n_events, void* stream);
+int oww_detector_export(oww_ctx* ctx, const int32_t* h_stream_ids, int n, float* d_hist, int32_t* d_counts, void* stream);
+int oww_detector_import(oww_ctx* ctx, const int32_t* h_stream_ids, int n, const float* d_hist, const int32_t* d_counts,
+                        void* stream);
+
 /* ---- batch paths --------------------------------------------------------------------------- */
 /* d_pcm [n_clips][n_samples] -> d_emb [n_clips][W][96], W = (T-76)/8+1 (utils.py:322).           */
 int oww_embed_clips(oww_ctx* ctx, const int16_t* d_pcm, int n_clips, int n_samples, float* d_emb, void* stream);

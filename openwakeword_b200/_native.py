@@ -29,6 +29,14 @@ class HeadDesc(C.Structure):
                 ("layernorm", C.c_int32), ("final_act", C.c_int32)]
 
 
+class DetectLabel(C.Structure):
+    _fields_ = [("column", C.c_int32), ("repeats", C.c_int32), ("threshold", C.c_float), ("patience", C.c_int32)]
+
+
+# one record of oww_detect's event list (oww_event): 16 bytes
+EVENT_DTYPE = np.dtype([("stream", "<i4"), ("label", "<i4"), ("score", "<f4"), ("index", "<i4")])
+
+
 # name -> (restype, argtypes): every symbol include/owwb200.h declares
 _P = C.c_void_p
 _SIGNATURES = {
@@ -79,6 +87,10 @@ _SIGNATURES = {
     "oww_export_streams": (C.c_int, [_P, _P, C.c_int, _P, _P]),
     "oww_import_streams": (C.c_int, [_P, _P, C.c_int, _P, _P]),
     "oww_stream_state_status": (C.c_int, [_P, C.POINTER(C.c_int)]),
+    "oww_set_detector": (C.c_int, [_P, C.POINTER(DetectLabel), C.c_int, C.c_double]),
+    "oww_detect": (C.c_int, [_P, _P, C.c_int, _P, _P, _P, C.c_int, _P, _P]),
+    "oww_detector_export": (C.c_int, [_P, _P, C.c_int, _P, _P, _P]),
+    "oww_detector_import": (C.c_int, [_P, _P, C.c_int, _P, _P, _P]),
     "oww_embed_clips": (C.c_int, [_P, _P, C.c_int, C.c_int, _P, _P]),
     "oww_predict_clips": (C.c_int, [_P, _P, C.c_int, C.c_int, C.c_int, _P, C.c_int, _P, _P]),
     "oww_clip_schedule": (C.c_int, [C.c_int, C.c_int64, _P, C.c_int]),
@@ -199,6 +211,8 @@ class Context:
         self._head_n_in = []                # per head id: n_in (verifier banks take n_in*96 floats per slot)
         self._bank_d = []                   # per verifier bank: D
         self._head_bank_n_in = []           # per head bank: n_in
+        self.n_detect_labels = 0            # labels of the detector (set_detector)
+        self._det_buf = None                # device event list and count of detect_events
 
     def close(self):
         if getattr(self, "h", None):
@@ -561,6 +575,96 @@ class Context:
             ext.wait_stream(torch.cuda.current_stream(dev))
             self.import_streams(ids, d, stream)
             d.record_stream(ext)
+
+    # ---- detections on the device (include/owwb200.h, oww_set_detector) ----
+    def set_detector(self, labels, debounce_time=0.0):
+        """labels: [(column, repeats, threshold or None / NaN, patience)], one per label; [] removes the detector.
+        Synchronises the device.  The same columns and repeats as before keep the histories."""
+        arr = (DetectLabel * max(len(labels), 1))()
+        for i, (col, rep, thr, pat) in enumerate(labels):
+            arr[i] = DetectLabel(int(col), int(bool(rep)), float("nan") if thr is None else float(thr), int(pat))
+        self._check(self.lib.oww_set_detector(self.h, arr, len(labels), float(debounce_time)))
+        self.n_detect_labels = len(labels)
+        self._det_buf = None
+
+    def detect(self, d_scores, prepared, d_final, d_events, max_events, d_n_events, stream=None):
+        """oww_detect: prepared is one int for every stream or host int32 [n_streams] (< 0: the stream is skipped)."""
+        if np.ndim(prepared) == 0:
+            all_, per = int(prepared), None
+        else:
+            all_, per = 0, np.ascontiguousarray(prepared, np.int32)
+            if per.shape != (self.n_streams,):
+                raise ValueError(f"prepared has shape {per.shape}, the handle has {self.n_streams} streams")
+        self._check(self.lib.oww_detect(self.h, _ptr(d_scores), all_, _ptr(per), _ptr(d_final), _ptr(d_events),
+                                        int(max_events), _ptr(d_n_events), stream))
+
+    def detector_export(self, stream_ids, d_hist, d_counts, stream=None):
+        ids = np.ascontiguousarray(stream_ids, np.int32).ravel()
+        self._check(self.lib.oww_detector_export(self.h, _ptr(ids), ids.size, _ptr(d_hist), _ptr(d_counts), stream))
+
+    def detector_import(self, stream_ids, d_hist, d_counts, stream=None):
+        ids = np.ascontiguousarray(stream_ids, np.int32).ravel()
+        self._check(self.lib.oww_detector_import(self.h, _ptr(ids), ids.size, _ptr(d_hist), _ptr(d_counts), stream))
+
+    def _current_stream(self):
+        import torch
+        return torch.cuda.current_stream(torch.device("cuda", self.device)).cuda_stream
+
+    def new_scores(self):
+        """a device score matrix [n_streams, n_outputs] for step_ragged_pcm / detect_events"""
+        import torch
+        return torch.zeros((self.n_streams, self.n_outputs), dtype=torch.float32, device=torch.device("cuda", self.device))
+
+    def step_pcm(self, pcm, n_chunks, d_scores):
+        """step on a host int16 [n_streams, >= n_chunks*1280] array, uploaded and stepped on the current CUDA stream; the
+        scores stay on the device."""
+        import torch
+        self._host_pcm(pcm, n_chunks)
+        d = torch.from_numpy(pcm).to(d_scores.device)
+        self.step(d, pcm.shape[1], int(n_chunks), d_scores, self._current_stream())
+
+    def step_ragged_pcm(self, pcm, chunks, d_scores):
+        """step_ragged on a host int16 [n_streams, >= max(chunks)*1280] array: uploaded and stepped on the current CUDA
+        stream; the scores stay on the device."""
+        import torch
+        c = self._chunks(chunks)
+        self._host_pcm(pcm, c.max(initial=0))
+        d = torch.from_numpy(pcm).to(d_scores.device)
+        self.step_ragged(d, pcm.shape[1], c, d_scores, self._current_stream())
+
+    def detect_events(self, d_scores, prepared, d_final=None, max_events=None):
+        """oww_detect on the current CUDA stream, then the event count and that many events to the host (synchronises):
+        -> (EVENT_DTYPE array of min(n, max_events) events in ascending (stream, label) order, n).  max_events None:
+        n_streams * n_labels, which never truncates."""
+        import torch
+        cap = self.n_streams * self.n_detect_labels if max_events is None else int(max_events)
+        if self._det_buf is None or self._det_buf[0].shape[0] < cap:
+            dev = torch.device("cuda", self.device)
+            self._det_buf = (torch.empty((cap, 4), dtype=torch.int32, device=dev),
+                             torch.zeros(1, dtype=torch.int32, device=dev))
+        ev, n_ev = self._det_buf
+        self.detect(d_scores, prepared, d_final, ev if cap else None, cap, n_ev, self._current_stream())
+        n = int(n_ev.item())
+        return ev[:min(n, cap)].cpu().numpy().view(EVENT_DTYPE).reshape(-1), n
+
+    def detector_history(self, stream_ids):
+        """-> (float32 [n, n_labels, 30] oldest first, int32 [n] counts) of the listed streams (synchronises)"""
+        import torch
+        ids = np.ascontiguousarray(stream_ids, np.int32).ravel()
+        dev = torch.device("cuda", self.device)
+        hist = torch.empty((ids.size, self.n_detect_labels, 30), dtype=torch.float32, device=dev)
+        cnt = torch.empty(ids.size, dtype=torch.int32, device=dev)
+        self.detector_export(ids, hist, cnt, self._current_stream())
+        return hist.cpu().numpy(), cnt.cpu().numpy()
+
+    def set_detector_history(self, stream_ids, hist, counts):
+        """the reverse of detector_history (distinct ids), on the current CUDA stream"""
+        import torch
+        ids = np.ascontiguousarray(stream_ids, np.int32).ravel()
+        dev = torch.device("cuda", self.device)
+        h = torch.from_numpy(np.ascontiguousarray(hist, np.float32).reshape(ids.size, self.n_detect_labels, 30)).to(dev)
+        c = torch.from_numpy(np.ascontiguousarray(counts, np.int32).reshape(ids.size)).to(dev)
+        self.detector_import(ids, h, c, self._current_stream())
 
     # ---- batch ----
     def embed_clips(self, d_pcm, n_clips, n_samples, d_emb, stream=None):

@@ -254,6 +254,7 @@ void free_streams(oww_ctx* c) {
     }
     c->rag_streams = 0;
     oww_verifiers_free_streams(c);
+    oww_detect_free_streams(c);
     oww_heads_grp_drop_mirror(c);
     for (auto& X : c->late_x) for (auto& b : X.buf) { cudaFree(b); b = nullptr; }
     cudaFree(c->d_late_tmp); c->d_late_tmp = nullptr;
@@ -708,6 +709,8 @@ int reset_enqueue(oww_ctx* ctx, const int32_t* h_stream_ids, int n, const float*
                                    ctx->d_mel_count, ctx->d_feat_count, ctx->d_mel_ring, ctx->mel_rows, ctx->d_feat_ring,
                                    ctx->feat_rows, have_init ? ctx->d_reset_init : nullptr, n_rows, rt);
     OWW_LAUNCH_CHECK(ctx);
+    int rc = oww_detect_reset(ctx, h_stream_ids ? ctx->d_reset_ids : nullptr, n, s);    // the detector's history of those streams
+    if (rc) return rc;
     return oww_feat16_resync(ctx, h_stream_ids ? ctx->d_reset_ids : nullptr, n, s);     // fp16 mirror of the rings (heads_grp.cu)
 }
 
@@ -850,6 +853,7 @@ void oww_destroy(oww_ctx* ctx) {
     oww_heads_grp_free(ctx);
     oww_head_banks_free(ctx);
     oww_verifier_fit_free(ctx);
+    oww_detect_free(ctx);
     cudaFree(ctx->d_window); cudaFree(ctx->d_twiddle); cudaFree(ctx->d_mel_start); cudaFree(ctx->d_mel_len);
     cudaFree(ctx->d_mel_w); cudaFree(ctx->d_emb_blob); cudaFree(ctx->d_tc_w); cudaFree(ctx->d_tc_sb);
     cudaFree(ctx->d_tc_w3); cudaFree(ctx->d_tc_sb3);
@@ -1038,6 +1042,7 @@ int oww_set_streams(oww_ctx* ctx, int n_streams) {
     if (ctx->cfg.cnn_mode == OWW_CNN_TC_INCREMENTAL && (rc = oww_inc_alloc_streams(ctx))) return rc;
     if ((rc = oww_verifiers_alloc_streams(ctx))) return rc;         // every stream starts without a verifier
     if ((rc = oww_head_banks_alloc_streams(ctx))) return rc;        // ... and without a bank head
+    if ((rc = oww_detect_alloc_streams(ctx))) return rc;            // ... and with an empty detector history
     return oww_reset(ctx, nullptr, B, nullptr, OWW_INIT_FEATURE_ROWS);
 }
 

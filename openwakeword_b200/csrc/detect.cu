@@ -1,0 +1,331 @@
+// Detections on the device: the half of Model.predict that turns a step's scores into detections (openwakeword/model.py:
+// 303-363) - per-stream prediction history, zeroing of the first five predictions, patience, debounce, the "repeat the
+// previous prediction below 1280 samples" rule and the threshold - for every (stream, label) in one kernel, and the
+// detections returned as a compact, ordered event list.  Semantics: include/owwb200.h (oww_set_detector, oww_detect);
+// restated per stream in oracle/detect.py.
+//
+// State: hist [30][B * n_labels] fp32 (ring slot s of pair p = stream * n_labels + label at hist[s * P + p]: the threads of
+// a warp read one slot of neighbouring pairs, so every history pass is coalesced) and count [B] int32 (predictions
+// appended since the stream's reset; ring slot = count % 30).
+//
+// Event compaction is two launches rather than one pass with decoupled look-back: detect_kernel leaves each CTA's event
+// count and each pair's fired score, detect_events_kernel sums the counts of the CTAs before it (a few hundred ints at
+// 8192 streams) and writes its events behind them.  No CTA ever waits for another, so nothing can spin on a device that
+// is shared, and the order - ascending (stream, label) - follows from the thread mapping alone.
+#include <cstring>
+#include "oww_internal.h"
+
+#define DET_HIST 30
+#define DET_THREADS 256
+#define DET_MAX_LABELS 256
+// count is rebased by a multiple of 30 past 2^30 (2.7 years at 12.5 predictions/s): the ring slot and min(count, 30) stay
+#define DET_COUNT_REBASE (35791392 * 30)
+
+struct oww_detector {
+    std::vector<oww_detect_label> labels;
+    double debounce = 0.0;
+    oww_detect_label* d_labels = nullptr;
+    int n_streams = 0;                 // streams the state below is allocated for
+    float* d_hist = nullptr;           // [30][B * L]
+    int* d_count = nullptr;            // [B]
+    float* d_fire = nullptr;           // [B * L] final score of the pairs that fired in the last call, NaN elsewhere
+    int* d_cta = nullptr;              // [CTAs] events per CTA of the last call
+    int* d_ids = nullptr;              // [B] staging of export / import ids
+    // per-stream `prepared` of a call, staged like the counts of oww_step_ragged
+    static constexpr int kSlots = 4;
+    int32_t* h_prep[kSlots] = {nullptr, nullptr, nullptr, nullptr};
+    int32_t* d_prep[kSlots] = {nullptr, nullptr, nullptr, nullptr};
+    cudaEvent_t ev[kSlots] = {nullptr, nullptr, nullptr, nullptr};
+    int next = 0;
+};
+
+static __device__ __forceinline__ int det_wrap(int c) { return c >= OWW_COUNT_WRAP ? c - DET_COUNT_REBASE : c; }
+
+// streams per CTA: whole streams only, so that the one count of a stream is read by all its threads before it is written
+static inline int det_streams_per_cta(int L) { return DET_THREADS / L; }
+
+// The kernels stay outside the anonymous namespace: their names in a profile do not depend on the build.
+// One thread per (stream, label); CTA `blockIdx.x` owns streams [blockIdx.x * S, +S).
+__global__ void __launch_bounds__(DET_THREADS) detect_kernel(const float* __restrict__ scores, int n_out, int B, int L, int S,
+                                                             const oww_detect_label* __restrict__ labels, double debounce,
+                                                             int prepared_all, const int* __restrict__ prepared,
+                                                             float* __restrict__ hist, int* __restrict__ count,
+                                                             float* __restrict__ d_final, float* __restrict__ fire,
+                                                             int* __restrict__ cta_events) {
+    const int sl = threadIdx.x / L, j = threadIdx.x - sl * L;
+    const int b = blockIdx.x * S + sl;
+    const bool live = sl < S && b < B;
+    const size_t P = (size_t)B * L, p = (size_t)b * L + j;
+    int prep = -1, c = 0;
+    if (live) {
+        prep = prepared ? prepared[b] : prepared_all;
+        c = count[b];
+    }
+    bool fired = false;
+    float pred = 0.f;
+    if (prep >= 0) {
+        const oww_detect_label lab = labels[j];
+        const int n = min(c, DET_HIST);
+        if (prep >= OWW_SAMPLES_PER_CHUNK) pred = lab.column >= 0 ? scores[(size_t)b * n_out + lab.column] : 0.f;
+        else if (lab.repeats && c > 0) pred = hist[(size_t)((c - 1) % DET_HIST) * P + p];
+        if (c < 5) pred = 0.f;
+        const bool has_thr = !isnan(lab.threshold);
+        if (lab.patience > 0) {
+            if (pred != 0.f) {
+                const int k = min(lab.patience, n);
+                int ge = 0;
+                for (int i = 0; i < k; ++i) ge += hist[(size_t)((c - 1 - i) % DET_HIST) * P + p] >= lab.threshold;
+                if (ge < lab.patience) pred = 0.f;
+            }
+        } else if (debounce > 0.0 && has_thr && pred != 0.f && pred >= lab.threshold) {
+            int k = n;
+            if (prep > 0) {
+                const double nf = ceil(debounce / ((double)prep / 16000.0));
+                if (nf < (double)k) k = (int)nf;
+            }
+            bool hit = false;
+            for (int i = 0; i < k; ++i) hit = hit || hist[(size_t)((c - 1 - i) % DET_HIST) * P + p] >= lab.threshold;
+            if (hit) pred = 0.f;
+        }
+        fired = has_thr && pred >= lab.threshold;
+        hist[(size_t)(c % DET_HIST) * P + p] = pred;
+        if (d_final) d_final[p] = pred;
+    }
+    if (live) fire[p] = fired ? pred : __int_as_float(0x7fc00000);
+    const int n_fired = __syncthreads_count(fired);          // also: every thread of a stream has read its count
+    if (prep >= 0 && j == 0) count[b] = det_wrap(c + 1);
+    if (threadIdx.x == 0) cta_events[blockIdx.x] = n_fired;
+}
+
+// Same grid and thread mapping.  Events of this CTA start behind those of the CTAs before it.
+__global__ void __launch_bounds__(DET_THREADS) detect_events_kernel(const float* __restrict__ fire, const int* __restrict__ count,
+                                                                    const int* __restrict__ cta_events, int B, int L, int S,
+                                                                    oww_event* __restrict__ events, int max_events,
+                                                                    int* __restrict__ n_events) {
+    __shared__ int s_sum[DET_THREADS / 32];
+    __shared__ int s_fired[DET_THREADS / 32];
+    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+    int part = 0;
+    for (int i = threadIdx.x; i < (int)blockIdx.x; i += DET_THREADS) part += cta_events[i];
+    for (int o = 16; o; o >>= 1) part += __shfl_xor_sync(0xffffffffu, part, o);
+    const int sl = threadIdx.x / L, j = threadIdx.x - sl * L;
+    const int b = blockIdx.x * S + sl;
+    const bool live = sl < S && b < B;
+    const float sc = live ? fire[(size_t)b * L + j] : __int_as_float(0x7fc00000);
+    const bool f = !isnan(sc);
+    const unsigned m = __ballot_sync(0xffffffffu, f);
+    if (lane == 0) { s_sum[warp] = part; s_fired[warp] = __popc(m); }
+    __syncthreads();
+    int base = 0, before = 0;
+    for (int w = 0; w < DET_THREADS / 32; ++w) {
+        base += s_sum[w];
+        if (w < warp) before += s_fired[w];
+    }
+    if (blockIdx.x == gridDim.x - 1 && threadIdx.x == 0 && n_events) *n_events = base + cta_events[blockIdx.x];
+    const int pos = base + before + __popc(m & ((1u << lane) - 1u));
+    if (f && events && pos < max_events) events[pos] = oww_event{b, j, sc, count[b] - 1};
+}
+
+// streams ids[0..n) (nullptr: stream blockIdx.x) start afresh: an empty history
+__global__ void detect_clear_kernel(const int* ids, int B, int L, float* hist, int* count) {
+    const int b = ids ? ids[blockIdx.x] : blockIdx.x;
+    const size_t P = (size_t)B * L;
+    for (int i = threadIdx.x; i < DET_HIST * L; i += blockDim.x) hist[(size_t)(i / L) * P + (size_t)b * L + i % L] = 0.f;
+    if (threadIdx.x == 0) count[b] = 0;
+}
+
+// record i <-> stream ids[i]: [L][30] oldest first (entry k = the prediction 30 - k appends ago; zeros before the first)
+__global__ void detect_export_kernel(const int* ids, int B, int L, const float* hist, const int* count, float* out, int* out_count) {
+    const int b = ids[blockIdx.x], c = count[b];
+    const size_t P = (size_t)B * L;
+    for (int i = threadIdx.x; i < DET_HIST * L; i += blockDim.x) {
+        const int j = i / DET_HIST, k = i - j * DET_HIST;
+        out[(size_t)blockIdx.x * L * DET_HIST + i] = hist[(size_t)((c % DET_HIST + k) % DET_HIST) * P + (size_t)b * L + j];
+    }
+    if (threadIdx.x == 0) out_count[blockIdx.x] = c;
+}
+
+__global__ void detect_import_kernel(const int* ids, int B, int L, float* hist, int* count, const float* in, const int* in_count) {
+    const int b = ids[blockIdx.x];
+    const int c = det_wrap(max(in_count[blockIdx.x], 0));
+    const size_t P = (size_t)B * L;
+    for (int i = threadIdx.x; i < DET_HIST * L; i += blockDim.x) {
+        const int j = i / DET_HIST, k = i - j * DET_HIST;
+        hist[(size_t)((c % DET_HIST + k) % DET_HIST) * P + (size_t)b * L + j] = in[(size_t)blockIdx.x * L * DET_HIST + i];
+    }
+    if (threadIdx.x == 0) count[b] = c;
+}
+
+namespace {
+
+void free_stream_state(oww_detector* d) {
+    cudaFree(d->d_hist); cudaFree(d->d_count); cudaFree(d->d_fire); cudaFree(d->d_cta); cudaFree(d->d_ids);
+    d->d_hist = d->d_fire = nullptr;
+    d->d_count = d->d_cta = d->d_ids = nullptr;
+    for (int j = 0; j < oww_detector::kSlots; ++j) {
+        cudaFreeHost(d->h_prep[j]); cudaFree(d->d_prep[j]);
+        d->h_prep[j] = d->d_prep[j] = nullptr;
+    }
+    d->n_streams = 0;
+}
+
+// the detector's per-stream state for ctx->n_streams streams, every history empty; the device is idle
+int alloc_stream_state(oww_ctx* ctx) {
+    oww_detector* d = ctx->det;
+    free_stream_state(d);
+    const int B = ctx->n_streams, L = (int)d->labels.size();
+    if (B <= 0) return OWW_OK;
+    const size_t P = (size_t)B * L;
+    const int ctas = (B + det_streams_per_cta(L) - 1) / det_streams_per_cta(L);
+    OWW_CUDA(ctx, cudaMalloc(&d->d_hist, DET_HIST * P * sizeof(float)));
+    OWW_CUDA(ctx, cudaMalloc(&d->d_count, (size_t)B * sizeof(int)));
+    OWW_CUDA(ctx, cudaMalloc(&d->d_fire, P * sizeof(float)));
+    OWW_CUDA(ctx, cudaMalloc(&d->d_cta, (size_t)ctas * sizeof(int)));
+    OWW_CUDA(ctx, cudaMalloc(&d->d_ids, (size_t)B * sizeof(int)));
+    OWW_CUDA(ctx, cudaMemset(d->d_hist, 0, DET_HIST * P * sizeof(float)));
+    OWW_CUDA(ctx, cudaMemset(d->d_count, 0, (size_t)B * sizeof(int)));
+    for (int j = 0; j < oww_detector::kSlots; ++j) {
+        OWW_CUDA(ctx, cudaMallocHost(&d->h_prep[j], (size_t)B * sizeof(int32_t)));
+        OWW_CUDA(ctx, cudaMalloc(&d->d_prep[j], (size_t)B * sizeof(int32_t)));
+        if (!d->ev[j]) OWW_CUDA(ctx, cudaEventCreateWithFlags(&d->ev[j], cudaEventDisableTiming));
+    }
+    d->n_streams = B;
+    return OWW_OK;
+}
+
+// checks shared by export and import; stages the ids on `s`
+int stage_ids(oww_ctx* ctx, const int32_t* h_ids, int n, bool distinct, cudaStream_t s) {
+    const oww_detector* d = ctx->det;
+    if (!d || !d->d_hist) return oww_fail(ctx, OWW_EINVAL, "no detector configured (oww_set_detector, oww_set_streams)");
+    const int B = ctx->n_streams;
+    if (n < 0 || n > B) return oww_fail(ctx, OWW_EINVAL, "n=%d outside [0,%d]", n, B);
+    if (n && !h_ids) return oww_fail(ctx, OWW_EINVAL, "null argument");
+    std::vector<uint8_t> hit(distinct ? B : 0, 0);
+    for (int i = 0; i < n; ++i) {
+        if (h_ids[i] < 0 || h_ids[i] >= B) return oww_fail(ctx, OWW_EINVAL, "stream id %d out of range", h_ids[i]);
+        if (distinct && hit[h_ids[i]]++) return oww_fail(ctx, OWW_EINVAL, "stream id %d imported twice", h_ids[i]);
+    }
+    // pageable source: staged by the driver before the call returns; stream-ordered on the device
+    if (n) OWW_CUDA(ctx, cudaMemcpyAsync(d->d_ids, h_ids, (size_t)n * sizeof(int), cudaMemcpyHostToDevice, s));
+    return OWW_OK;
+}
+
+}  // namespace
+
+void oww_detect_free(oww_ctx* ctx) {
+    oww_detector* d = ctx->det;
+    if (!d) return;
+    free_stream_state(d);
+    for (auto e : d->ev) if (e) cudaEventDestroy(e);
+    cudaFree(d->d_labels);
+    delete d;
+    ctx->det = nullptr;
+}
+
+void oww_detect_free_streams(oww_ctx* ctx) { if (ctx->det) free_stream_state(ctx->det); }
+
+int oww_detect_alloc_streams(oww_ctx* ctx) { return ctx->det ? alloc_stream_state(ctx) : OWW_OK; }
+
+int oww_detect_reset(oww_ctx* ctx, const int* d_ids, int n, cudaStream_t s) {
+    const oww_detector* d = ctx->det;
+    if (!d || !d->d_hist || n <= 0) return OWW_OK;
+    detect_clear_kernel<<<n, DET_THREADS, 0, s>>>(d_ids, ctx->n_streams, (int)d->labels.size(), d->d_hist, d->d_count);
+    OWW_LAUNCH_CHECK(ctx);
+    return OWW_OK;
+}
+
+extern "C" {
+
+int oww_set_detector(oww_ctx* ctx, const oww_detect_label* h_labels, int n_labels, double debounce_time) {
+    if (!ctx) return OWW_EINVAL;
+    if (n_labels < 0 || n_labels > DET_MAX_LABELS) return oww_fail(ctx, OWW_EINVAL, "n_labels=%d outside [0,%d]", n_labels, DET_MAX_LABELS);
+    if (n_labels && !h_labels) return oww_fail(ctx, OWW_EINVAL, "null argument");
+    if (!(debounce_time >= 0.0) || !std::isfinite(debounce_time)) return oww_fail(ctx, OWW_EINVAL, "debounce_time must be finite and >= 0");
+    for (int j = 0; j < n_labels; ++j) {
+        const oww_detect_label& l = h_labels[j];
+        if (l.column < -1 || l.column >= ctx->n_out_total)
+            return oww_fail(ctx, OWW_EINVAL, "label %d: column %d outside [-1,%d)", j, l.column, ctx->n_out_total);
+        if (l.patience < 0 || l.patience > DET_HIST) return oww_fail(ctx, OWW_EINVAL, "label %d: patience %d outside [0,%d]", j, l.patience, DET_HIST);
+        if (l.patience > 0 && std::isnan(l.threshold)) return oww_fail(ctx, OWW_EINVAL, "label %d: patience needs a threshold", j);
+        if (l.patience > 0 && debounce_time > 0.0) return oww_fail(ctx, OWW_EINVAL, "patience and debounce_time cannot be used together");
+    }
+    OWW_CUDA(ctx, cudaSetDevice(ctx->device));
+    OWW_CUDA(ctx, cudaDeviceSynchronize());              // detect calls may be in flight on any stream
+    if (n_labels == 0) { oww_detect_free(ctx); return OWW_OK; }
+    oww_detector* d = ctx->det;
+    bool same = d && (int)d->labels.size() == n_labels;
+    for (int j = 0; same && j < n_labels; ++j)
+        same = d->labels[j].column == h_labels[j].column && (d->labels[j].repeats != 0) == (h_labels[j].repeats != 0);
+    if (!same) {                                         // another label set: the histories mean nothing under it
+        oww_detect_free(ctx);
+        d = ctx->det = new (std::nothrow) oww_detector();
+        if (!d) return oww_fail(ctx, OWW_ENOMEM, "out of host memory");
+        OWW_CUDA(ctx, cudaMalloc(&d->d_labels, (size_t)n_labels * sizeof(oww_detect_label)));
+    }
+    d->labels.assign(h_labels, h_labels + n_labels);
+    d->debounce = debounce_time;
+    OWW_CUDA(ctx, cudaMemcpy(d->d_labels, h_labels, (size_t)n_labels * sizeof(oww_detect_label), cudaMemcpyHostToDevice));
+    return same ? OWW_OK : alloc_stream_state(ctx);
+}
+
+int oww_detect(oww_ctx* ctx, const float* d_scores, int prepared_all, const int32_t* h_prepared, float* d_final,
+               oww_event* d_events, int max_events, int32_t* d_n_events, void* stream) {
+    if (!ctx) return OWW_EINVAL;
+    oww_detector* d = ctx->det;
+    if (!d || !d->d_hist) return oww_fail(ctx, OWW_EINVAL, "no detector configured (oww_set_detector, oww_set_streams)");
+    if (!d_scores) return oww_fail(ctx, OWW_EINVAL, "null argument");
+    if (max_events < 0) return oww_fail(ctx, OWW_EINVAL, "max_events=%d is negative", max_events);
+    if (!d_final && !d_n_events && !d_events) return oww_fail(ctx, OWW_EINVAL, "no output: d_final and the event list are both NULL");
+    if (max_events > 0 && !d_events) return oww_fail(ctx, OWW_EINVAL, "max_events=%d without d_events", max_events);
+    if (d_events && !d_n_events) return oww_fail(ctx, OWW_EINVAL, "d_events without d_n_events");
+    OWW_CUDA(ctx, cudaSetDevice(ctx->device));
+    cudaStream_t s = (cudaStream_t)stream;
+    const int B = ctx->n_streams, L = (int)d->labels.size(), S = det_streams_per_cta(L);
+    const int ctas = (B + S - 1) / S;
+    const int* d_prep = nullptr;
+    if (h_prepared) {
+        const int j = d->next;
+        d->next = (j + 1) % oww_detector::kSlots;
+        OWW_CUDA(ctx, cudaEventSynchronize(d->ev[j]));   // the copy of the call kSlots calls back has run
+        std::memcpy(d->h_prep[j], h_prepared, (size_t)B * sizeof(int32_t));
+        OWW_CUDA(ctx, cudaMemcpyAsync(d->d_prep[j], d->h_prep[j], (size_t)B * sizeof(int32_t), cudaMemcpyHostToDevice, s));
+        OWW_CUDA(ctx, cudaEventRecord(d->ev[j], s));
+        d_prep = d->d_prep[j];
+    }
+    detect_kernel<<<ctas, DET_THREADS, 0, s>>>(d_scores, ctx->n_out_total, B, L, S, d->d_labels, d->debounce, prepared_all,
+                                               d_prep, d->d_hist, d->d_count, d_final, d->d_fire, d->d_cta);
+    OWW_LAUNCH_CHECK(ctx);
+    if (d_n_events) {
+        detect_events_kernel<<<ctas, DET_THREADS, 0, s>>>(d->d_fire, d->d_count, d->d_cta, B, L, S, d_events, max_events, d_n_events);
+        OWW_LAUNCH_CHECK(ctx);
+    }
+    return OWW_OK;
+}
+
+int oww_detector_export(oww_ctx* ctx, const int32_t* h_stream_ids, int n, float* d_hist, int32_t* d_counts, void* stream) {
+    if (!ctx) return OWW_EINVAL;
+    OWW_CUDA(ctx, cudaSetDevice(ctx->device));
+    if (n > 0 && (!d_hist || !d_counts)) return oww_fail(ctx, OWW_EINVAL, "null argument");
+    int rc = stage_ids(ctx, h_stream_ids, n, false, (cudaStream_t)stream);
+    if (rc || n == 0) return rc;
+    const oww_detector* d = ctx->det;
+    detect_export_kernel<<<n, DET_THREADS, 0, (cudaStream_t)stream>>>(d->d_ids, ctx->n_streams, (int)d->labels.size(), d->d_hist,
+                                                                      d->d_count, d_hist, d_counts);
+    OWW_LAUNCH_CHECK(ctx);
+    return OWW_OK;
+}
+
+int oww_detector_import(oww_ctx* ctx, const int32_t* h_stream_ids, int n, const float* d_hist, const int32_t* d_counts, void* stream) {
+    if (!ctx) return OWW_EINVAL;
+    OWW_CUDA(ctx, cudaSetDevice(ctx->device));
+    if (n > 0 && (!d_hist || !d_counts)) return oww_fail(ctx, OWW_EINVAL, "null argument");
+    int rc = stage_ids(ctx, h_stream_ids, n, true, (cudaStream_t)stream);
+    if (rc || n == 0) return rc;
+    const oww_detector* d = ctx->det;
+    detect_import_kernel<<<n, DET_THREADS, 0, (cudaStream_t)stream>>>(d->d_ids, ctx->n_streams, (int)d->labels.size(), d->d_hist,
+                                                                      d->d_count, d_hist, d_counts);
+    OWW_LAUNCH_CHECK(ctx);
+    return OWW_OK;
+}
+
+}  // extern "C"

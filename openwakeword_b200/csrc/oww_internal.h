@@ -317,6 +317,7 @@ struct oww_ctx {
     bool grp_heads = true;           // streaming: heads that share a window run in one CTA per 128 streams (heads_grp.cu; reserved[0] bit 3 disables)
     struct oww_heads_grp* heads_grp = nullptr;
     int tc_heads_terms = 3;          // 3 = hi*hi + lo*hi + hi*lo (fp32-grade), 1 = plain fp16 operands
+    struct oww_detector* det = nullptr;   // detections on the device (detect.cu); nullptr: no detector configured
 };
 
 int oww_fail(oww_ctx* ctx, int code, const char* fmt, ...);
@@ -521,6 +522,13 @@ int oww_heads_grp_launch(oww_ctx* ctx, int back, int n, float* d_out, int out_st
 // oww_head_banks_launch
 int oww_heads_all(oww_ctx* ctx, const FeatSrc& src, int n, float* d_out, int out_stride, int combine_max, cudaStream_t s,
                   const BankRows* bank_rows = nullptr);
+
+// ---- detect.cu: the detector's per-stream prediction history (nothing happens on a handle without a detector) ----
+void oww_detect_free(oww_ctx* ctx);
+void oww_detect_free_streams(oww_ctx* ctx);
+int oww_detect_alloc_streams(oww_ctx* ctx);      // for ctx->n_streams streams, every history empty; the device is idle
+// the listed streams (d_ids == nullptr: streams 0..n-1) start afresh: one launch on `s`
+int oww_detect_reset(oww_ctx* ctx, const int* d_ids, int n, cudaStream_t s);
 
 // ---- verifier.cu: custom verifier banks ----
 // every bank of the handle on n rows of final scores (one launch; nothing when the handle has no bank).  The window of

@@ -143,6 +143,47 @@ class StreamEngine:
         when `out` is None)."""
         return self.ctx.step_host_ragged_submit(pcm, chunks)
 
+    # ---- detections on the device (include/owwb200.h, oww_set_detector) ----
+    def set_detector(self, labels, threshold, patience={}, debounce_time=0.0):
+        """Configure the detector.  labels: one (column, repeats) per label - the score column it reads (-1: always 0.0)
+        and whether it repeats its previous prediction when fewer than 1280 samples were prepared (True for the label of a
+        single-output head, False for a class of a multi-output head).  threshold: one float for every label, or {label
+        index: float} (a label without one never fires); patience: {label index: 1..30}; debounce_time: seconds.
+        Patience needs a threshold and excludes a debounce_time (NativeError, as the reference's ValueErrors).  New
+        thresholds, patience or debounce_time under the same labels keep the streams' histories; other labels clear them.
+        Synchronises the device."""
+        table = []
+        for j, (col, rep) in enumerate(labels):
+            thr = threshold.get(j) if isinstance(threshold, dict) else threshold
+            table.append((col, rep, thr, patience.get(j, 0)))
+        self.ctx.set_detector(table, debounce_time)
+
+    def detect(self, scores, prepared=1280, final=None, max_events=None):
+        """The detections of the step that wrote `scores` (float32 [n_streams, n_cols] on the engine's device).
+        prepared: the samples every stream prepared in that step, or host ints [n_streams] (< 0: the stream is skipped,
+        as for one held in step_ragged; 0..1279: it repeats its previous prediction).  final: float32 [n_streams, n_labels]
+        on the device, receives every prediction after the first-5 zeroing, patience and debounce (optional).
+        -> (events, n): n = the (stream, label) pairs at or above their threshold; events = the first min(n, max_events)
+        of them, ascending by stream then label, as a host NumPy array of dtype _native.EVENT_DTYPE (fields stream, label,
+        score, index = which prediction of the stream since its reset).  max_events None: n_streams * n_labels.
+        Runs on the current CUDA stream and synchronises it to read the count; only the count and the events are copied.
+        Typical loop:  scores = eng.step_ragged(pcm, chunks);
+                       ev, n = eng.detect(scores, np.where(chunks > 0, chunks * 1280, -1))"""
+        torch = _torch()
+        self.ctx._cuda("scores", scores, torch.float32, (self.n_streams, self.n_cols))
+        if final is not None:
+            self.ctx._cuda("final", final, torch.float32, (self.n_streams, self.ctx.n_detect_labels))
+        return self.ctx.detect_events(scores, prepared, final, max_events)
+
+    def detector_history(self, stream_ids):
+        """-> (float32 [n, n_labels, 30] oldest first, int32 [n] predictions since the reset) of the listed streams"""
+        return self.ctx.detector_history(stream_ids)
+
+    def set_detector_history(self, stream_ids, hist, counts):
+        """Streams stream_ids (distinct) continue from the history `detector_history` returned for other streams, of this
+        engine or another with the same labels."""
+        self.ctx.set_detector_history(stream_ids, hist, counts)
+
     # ---- custom verifier models (include/owwb200.h, oww_add_verifier_bank) ----
     def add_verifier_bank(self, head_index, capacity, threshold=0.1):
         """Slots for `capacity` verifiers of entry `head_index` of `heads`; every stream starts without one."""

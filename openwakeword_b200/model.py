@@ -484,6 +484,31 @@ class Model:
     def _reset_history(self):
         self._hist = {}        # label -> float32 [30, B] ring of the last predictions
         self._count = {}       # label -> int64 [B] predictions appended so far
+        # True once detect* has run: the device detector then holds the history, and _hist / _count are refreshed from
+        # it where they are read (_pull_history); the next predict* takes it back
+        self._hist_on_device = False
+
+    def _pull_history(self):
+        """_hist / _count <- the device detector's history, while it is the one in use"""
+        if not self._hist_on_device:
+            return
+        hist, cnt = self.preprocessor.ctx.detector_history(np.arange(self.n_streams, dtype=np.int32))
+        cnt = cnt.astype(np.int64)
+        slot = (np.arange(30)[:, None] - cnt[None, :]) % 30       # ring slot s holds the entry (s - count) % 30 of oldest-first
+        for j, lab in enumerate(self.labels()):
+            h, c = self._h(lab)
+            h[:] = hist[:, j, :].T[slot, np.arange(self.n_streams)[None, :]]
+            c[:] = cnt
+
+    def _push_history(self, ids):
+        """the device detector's history of streams ids <- _hist / _count"""
+        ids = np.asarray(ids, np.int64)
+        labels = self.labels()
+        hist = np.zeros((ids.size, len(labels), 30), np.float32)
+        cnt = self._h(labels[0])[1][ids]
+        for j, lab in enumerate(labels):
+            hist[:, j, :] = self._recent(lab, 30)[0][:, ids].T
+        self.preprocessor.ctx.set_detector_history(ids.astype(np.int32), hist, np.minimum(cnt, 2 ** 30).astype(np.int32))
 
     def _h(self, label):
         if label not in self._hist:
@@ -503,6 +528,7 @@ class Model:
     @property
     def prediction_buffer(self):
         """defaultdict(deque(maxlen=30)) of stream 0's history, like the reference attribute."""
+        self._pull_history()
         buf = defaultdict(partial(deque, maxlen=30))
         for label in self._hist:
             ordered, valid = self._recent(label, 30)
@@ -532,6 +558,7 @@ class Model:
         records = pre.ctx.export_records(ids)
         buf, lens = pre._ragged_pending()
         labels = self.labels()
+        self._pull_history()
         return StreamState(records, key, labels, [buf[b, :lens[b]].copy() for b in ids],
                            {lab: self._h(lab)[0][:, ids].copy() for lab in labels},
                            {lab: self._h(lab)[1][ids].copy() for lab in labels})
@@ -566,6 +593,8 @@ class Model:
             hist, cnt = self._h(lab)
             hist[:, ids] = state.history[lab]
             cnt[ids] = state.counts[lab]
+        if self._hist_on_device and ids.size:
+            self._push_history(ids)
 
     def _ids(self, stream_ids):
         ids = np.asarray(stream_ids, np.int64).ravel()
@@ -658,9 +687,118 @@ class Model:
         n_prepared, _, split = self.preprocessor._streaming_features_ragged(xs, self._scores)
         return self._finish(n_prepared, split, patience, threshold, debounce_time, timing, t0, B == 1)
 
+    # ---- detections on the device (include/owwb200.h, oww_set_detector / oww_detect) ----
+    def detect(self, x, threshold, patience={}, debounce_time=0.0):
+        """``predict(x, patience, threshold, debounce_time)`` that returns only the detections of this call: a list of
+        (stream id, label, score) for every label whose prediction is >= the threshold of its model, ordered by stream,
+        then by label in ``labels()`` order.  threshold: {model name: float} as in the reference (a model without one
+        never fires), or one float for every model.  State and history advance exactly as in ``predict``; the history,
+        the first-5 zeroing, patience and debounce run on the device (csrc/detect.cu), the scores stay there, and only
+        the event count and the events are copied back.  ``predict*`` and ``detect*`` may be mixed freely: the history
+        moves between host and device at each switch (one copy of [n_streams, labels, 30] floats), and
+        ``prediction_buffer``, ``reset``, ``reset_streams``, ``export_streams`` and ``import_streams`` see it wherever it is.
+
+        ValueError, so that no call needs per-stream host work: a custom verifier that only runs on the host; Speex noise
+        suppression with more than one stream; a stream that prepares more than ``max_chunks`` chunks in one call while
+        device verifier banks are loaded (``predict`` re-verifies that case on the host).
+
+        One difference from ``predict``, only on models with device verifier banks: a stream that prepares fewer than
+        1280 samples repeats its previous prediction as stored; ``predict`` passes the repeated value through the
+        verifier once more."""
+        if not isinstance(x, np.ndarray):
+            raise ValueError(f"The input audio data (x) must by a Numpy array, instead received an object of type {type(x)}.")
+        self._detect_refusals()
+        if self.speex_ns:
+            x = self._suppress_noise_with_speex(x)
+        return self._detect(self.preprocessor._coerce(x), threshold, patience, debounce_time)
+
+    def detect_ragged(self, x, threshold, patience={}, debounce_time=0.0):
+        """``detect`` with the inputs of ``predict_ragged``: one 1-D array of any length per stream."""
+        B = self.n_streams
+        try:
+            n = len(x)
+        except TypeError:
+            raise ValueError(f"detect_ragged takes a sequence of {B} 1-D NumPy arrays, got {type(x)}") from None
+        if n != B:
+            raise ValueError(f"detect_ragged takes one array per stream ({B}), got {n}")
+        xs = []
+        for b, a in enumerate(x):
+            if not isinstance(a, np.ndarray) or a.ndim != 1:
+                raise ValueError(f"x[{b}] must be a 1-D NumPy array")
+            xs.append(a if a.dtype == np.int16 else a.astype(np.int16))
+        self._detect_refusals()
+        if self.speex_ns:
+            xs = [self._suppress_noise_with_speex(xs[0])]
+        return self._detect(xs, threshold, patience, debounce_time)
+
+    def _detect_refusals(self):
+        if self._host_verifiers:
+            raise ValueError(f"detect: the custom verifiers of {sorted(self._host_verifiers)} run on the host only (only "
+                             "the linear pipeline of train_verifier_model runs on the device); use predict")
+        if self.speex_ns and self.n_streams != 1:
+            raise ValueError("Speex noise suppression is single-stream")
+
+    def _detector_table(self, threshold, patience, debounce_time):
+        """-> [(column, repeats, threshold or None, patience)] per label of labels(), as predict applies its arguments"""
+        if patience != {} and debounce_time > 0:
+            raise ValueError("Error! The `patience` and `debounce_time` arguments cannot be used together!")
+        table = []
+        for mdl in self.models:
+            col0, n_out = self._columns[mdl]
+            if n_out == 1:
+                entries = [(mdl, col0, True)]
+            else:
+                entries = [(cls, col0 + int(k) if int(k) < n_out else -1, False) for k, cls in self.class_mapping[mdl].items()]
+            for lab, col, repeats in entries:
+                parent = self.get_parent_model_from_label(lab)
+                thr = threshold.get(parent) if isinstance(threshold, dict) else threshold
+                pat = int(patience.get(parent, 0))
+                if pat and thr is None:
+                    raise ValueError("Error! When using the `patience` argument, threshold "
+                                     "values must be provided via the `threshold` argument!")
+                if not 0 <= pat <= 30:
+                    raise ValueError(f"patience of '{parent}' must lie in 0..30 (the history holds 30 predictions)")
+                table.append((col, repeats, None if thr is None else float(thr), pat))
+        return table
+
+    def _detect(self, xs, threshold, patience, debounce_time):
+        pre = self.preprocessor
+        pre._ensure_streams()
+        ctx = pre.ctx
+        labels = self.labels()
+        if not labels:
+            raise ValueError("detect needs at least one model")
+        table = self._detector_table(threshold, patience, debounce_time)
+        lockstep = isinstance(xs, np.ndarray) and not pre.pending_ragged      # as predict: one length, one remainder
+        if not lockstep:
+            xs = list(xs)
+        held = pre._pending.shape[1] if not pre.pending_ragged else pre._ragged_pending()[1]
+        if (self._vbanks or self._svbanks) and \
+                ((held + np.array([a.shape[0] for a in xs], np.int64)) // CHUNK > pre.max_chunks).any():
+            raise ValueError(f"detect: a stream prepares more than max_chunks={pre.max_chunks} chunks in this call while "
+                             "custom verifiers are loaded; construct the Model with a larger max_chunks, or use predict")
+        config = (table, float(debounce_time))
+        if getattr(self, "_detector_config", None) != config:      # oww_set_detector synchronises: only on a change
+            ctx.set_detector(table, debounce_time)
+            self._detector_config = config
+        if not self._hist_on_device:
+            if self._hist:
+                self._push_history(np.arange(self.n_streams))
+            self._hist_on_device = True
+        if getattr(self, "_d_scores", None) is None:
+            self._d_scores = ctx.new_scores()
+        if lockstep:
+            n_prepared = pre._streaming_features(xs, self._d_scores, device=True)[0]
+        else:
+            n_prepared = pre._streaming_features_ragged(xs, self._d_scores, device=True)[0].astype(np.int32)
+        events, n = ctx.detect_events(self._d_scores, n_prepared)
+        return list(zip(events["stream"].tolist(), [labels[j] for j in events["label"].tolist()], events["score"].tolist()))
+
     def _finish(self, n_prepared, split, patience, threshold, debounce_time, timing, t0, single):
         """model.py:285-386 per stream after the device step(s): stream b prepared n_prepared[b] samples (its row of
         self._scores holds the step's scores when >= 1280); split: the steps ran without the verifier banks."""
+        self._pull_history()                     # after detect*: the history comes back to the host
+        self._hist_on_device = False
         if timing:
             timing_dict = {"models": {"preprocessor": time.time() - t0}}
         B = self.n_streams

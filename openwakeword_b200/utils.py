@@ -251,15 +251,17 @@ class AudioFeatures:
             raise ValueError(f"expected audio for {self.n_streams} stream(s), got {x.shape[0]}")
         return x
 
-    def _streaming_features(self, x, scores_out=None):
+    def _streaming_features(self, x, scores_out=None, device=False):
         """Chunk accumulation of utils.py:409-452, shared by all streams (same lengths).
-        Returns (n_prepared_samples, n_chunks_run).  Scores land in scores_out when a step ran."""
+        Returns (n_prepared_samples, n_chunks_run).  Scores land in scores_out when a step ran.  device: scores_out is a
+        device score matrix (Context.new_scores) and the steps run on the current CUDA stream without a copy back."""
         self._ensure_streams()
         x = self._coerce(x)
+        step = self.ctx.step_pcm if device else self.ctx.step_host
         if scores_out is None:
             scores_out = np.empty((self.n_streams, max(self.ctx.n_outputs, 1)), np.float32)
         if self._rpend is not None:         # the streams hold different remainders: per-stream accumulation
-            n_prepared, n_chunks, _ = self._streaming_features_ragged(list(x), scores_out)
+            n_prepared, n_chunks, _ = self._streaming_features_ragged(list(x), scores_out, device)
             self._last_scores = scores_out
             return n_prepared, n_chunks
         buf = np.concatenate((self._pending, x), axis=1) if self._pending.shape[1] else x
@@ -276,22 +278,23 @@ class AudioFeatures:
         if scores_out is None:
             scores_out = np.empty((self.n_streams, max(self.ctx.n_outputs, 1)), np.float32)
         if n_chunks <= self.max_chunks:
-            self.ctx.step_host(np.ascontiguousarray(ready), n_chunks, scores_out)
+            step(np.ascontiguousarray(ready), n_chunks, scores_out)
         else:
             # a call longer than max_chunks*1280 samples (the reference accepts up to its 10 s raw buffer) runs as
             # several device calls of <= max_chunks chunks; per head the result is the max over all chunk windows, as in
             # model.py:287-298.  Only the scope of the mel graph's -80 dB clamp differs (per device call, not per host call).
             # Custom verifiers run after that max, on the newest window (model.py:319-328): the parts run without the
             # verifier banks and Model.predict verifies the max.
-            part = np.empty_like(scores_out)
+            part = self.ctx.new_scores() if device else np.empty_like(scores_out)
+            every = np.ones(self.n_streams, bool)
             if self._verifier_banks:
                 self.ctx.enable_verifiers(False)
             try:
                 for k, c0 in enumerate(range(0, n_chunks, self.max_chunks)):
                     c1 = min(c0 + self.max_chunks, n_chunks)
-                    self.ctx.step_host(np.ascontiguousarray(ready[:, c0 * CHUNK:c1 * CHUNK]), c1 - c0, scores_out if k == 0 else part)
+                    step(np.ascontiguousarray(ready[:, c0 * CHUNK:c1 * CHUNK]), c1 - c0, scores_out if k == 0 else part)
                     if k:
-                        np.maximum(scores_out, part, out=scores_out)
+                        _take_rows(scores_out, part, every, True)
             finally:
                 if self._verifier_banks:
                     self.ctx.enable_verifiers(True)
@@ -299,15 +302,17 @@ class AudioFeatures:
         self._last_scores = scores_out
         return ready.shape[1], n_chunks
 
-    def _streaming_features_ragged(self, xs, scores_out):
+    def _streaming_features_ragged(self, xs, scores_out, device=False):
         """Chunk accumulation of utils.py:409-452 per stream: stream b gets xs[b] (1-D int16, any length), steps the
         whole chunks of its remainder + xs[b] and keeps the rest.  One oww_step_host_ragged call per max_chunks chunks.
         Returns (n_prepared [B], n_chunks [B], split): n_prepared as the reference's AudioFeatures.__call__ returns it
         (the samples stepped, or the samples accumulated when no chunk was stepped); rows of scores_out of streams that
         stepped nothing are not written.  split: a stream stepped more than max_chunks chunks, so the calls ran without
-        the verifier banks (the caller verifies the max over all chunk windows)."""
+        the verifier banks (the caller verifies the max over all chunk windows).  device: scores_out is a device score
+        matrix (Context.new_scores) and the steps run on the current CUDA stream without a copy back."""
         self._ensure_streams()
         B = self.n_streams
+        step = self.ctx.step_ragged_pcm if device else self.ctx.step_host_ragged
         buf, lens = self._ragged_pending()
         tot = lens + np.array([x.shape[0] for x in xs], np.int64)
         n_chunks = tot // CHUNK
@@ -318,7 +323,7 @@ class AudioFeatures:
             if new_lens[b]:
                 new_buf[b, :new_lens[b]] = ready[b][n_chunks[b] * CHUNK:]
         split = bool((n_chunks > self.max_chunks).any())
-        part = np.empty_like(scores_out) if split else scores_out
+        part = (self.ctx.new_scores() if device else np.empty_like(scores_out)) if split else scores_out
         if split and self._verifier_banks:
             self.ctx.enable_verifiers(False)
         try:
@@ -329,11 +334,10 @@ class AudioFeatures:
                 for b in np.nonzero(c)[0]:
                     pcm[b, :c[b] * CHUNK] = ready[b][done[b] * CHUNK:(done[b] + c[b]) * CHUNK]
                 first = (done == 0) & (c > 0)
-                self.ctx.step_host_ragged(pcm, c, part)
+                step(pcm, c, part)
                 if split:               # per stream the max over all its parts
-                    scores_out[first] = part[first]
-                    later = (done > 0) & (c > 0)
-                    scores_out[later] = np.maximum(scores_out[later], part[later])
+                    _take_rows(scores_out, part, first, False)
+                    _take_rows(scores_out, part, (done > 0) & (c > 0), True)
                 done += c
         finally:
             if split and self._verifier_banks:
@@ -372,6 +376,16 @@ class AudioFeatures:
     def melspectrogram_buffer(self):
         self._ensure_streams()
         return self.ctx.get_mel(0, 76)
+
+
+def _take_rows(dst, src, rows, maximum):
+    """dst[rows] = src[rows], or the element-wise max of the two; host arrays or device tensors, rows: bool [B]"""
+    if not isinstance(dst, np.ndarray):
+        torch = _torch()
+        rows = torch.from_numpy(rows).to(dst.device)
+        dst[rows] = torch.maximum(dst[rows], src[rows]) if maximum else src[rows]
+    else:
+        dst[rows] = np.maximum(dst[rows], src[rows]) if maximum else src[rows]
 
 
 def _read_wav(path):
