@@ -3,7 +3,8 @@
 // One warpgroup holds the accumulators of a Linear layer for 64 streams in registers (wgmma fragment, tc_common.cuh).
 // Per layer they are written to shared memory as fp32 rows (x 2^-s, + bias); thread r < 64 of the warpgroup
 // then runs the row-wise part in heads.cu's fp32 arithmetic order ([LayerNorm], ReLU or the final activation) and
-// writes the next GEMM's A tile as fp16 hi + lo in the no-swizzle K-major core-matrix order ([octet][64 rows][16 B]).
+// writes the next GEMM's A tile as fp16 hi + lo in the no-swizzle K-major core-matrix order ([octet][64 rows][16 B]),
+// each row times its own power of two 2^e (max in [2^13, 2^14), e in [-100, 100]), which the next epilogue undoes.
 // The next layer's weights (packed [hi | lo][Kp/8][NP][8] by oww_heads_tc_pack) arrive in `w_next` from the CTA's
 // producer warp; the three MMA terms per K step are hi*hi + lo*hi + hi*lo (n_terms = 1: hi*hi).
 #pragma once
@@ -14,6 +15,7 @@ namespace {
 constexpr int kHmRows = 64;                          // streams per tile = wgmma M
 constexpr int kHmAPlane = kHmRows * 16;              // bytes per k-octet plane of a 64-row A tile (LBO)
 constexpr int kHmPitch = 129;                        // fp32 row pitch of the hidden-activation buffer (layers <= 128 wide)
+constexpr int kHmRowScale = 128;                     // the row's spare column: 2^-e of the A tile it last wrote
 constexpr int kHmHBytes = (kHmRows * kHmPitch * 4 + 127) & ~127;
 constexpr int kHmABytes = 2 * 16 * kHmAPlane;        // next A tile: [hi | lo] x 16 octets (K <= 128)
 constexpr int kHmPBytes = 3 * 128 * 4;               // bias | gamma | beta of the layer in hand
@@ -59,12 +61,15 @@ __device__ __forceinline__ void hm_layers(float* acc, int n0, const HeadDev& H, 
             }
         }
         named_bar_sync(bar, 128);
-        // accumulators -> fp32 rows: exact 2^-s, bias
+        // accumulators -> fp32 rows: exact 2^-s (and 2^-e of the row's A tile for the later layers), bias
+        const int row0 = 16 * wq + (lane >> 2);
+        const float us0 = l ? us * hbuf[row0 * kHmPitch + kHmRowScale] : us;
+        const float us1 = l ? us * hbuf[(row0 + 8) * kHmPitch + kHmRowScale] : us;
 #pragma unroll
         for (int k = 0; k < 64; ++k) {
             const int j = k >> 2, i = (k >> 1) & 1, e = k & 1;
-            const int col = 8 * j + 2 * q + e, row = 16 * wq + (lane >> 2) + 8 * i;
-            if (8 * j < ncols && col < D) hbuf[row * kHmPitch + col] = fmaf(acc[k], us, prm[col]);
+            const int col = 8 * j + 2 * q + e, row = row0 + 8 * i;
+            if (8 * j < ncols && col < D) hbuf[row * kHmPitch + col] = fmaf(acc[k], i ? us1 : us0, prm[col]);
         }
         named_bar_sync(bar, 128);
         float* hrow = hbuf + tid * kHmPitch;
@@ -104,18 +109,25 @@ __device__ __forceinline__ void hm_layers(float* acc, int n0, const HeadDev& H, 
             }
             const float* g = prm + 128;
             const float* hb = prm + 256;
+            float vmax = 0.f;
+            for (int d = 0; d < D; ++d) {
+                float v = hrow[d];
+                if (H.layernorm) v = (v - mu) * rstd * g[d] + hb[d];
+                v = fmaxf(v, 0.f);
+                hrow[d] = v;
+                vmax = fmaxf(vmax, v);
+            }
+            // the row enters the A tile as v 2^e (max in [2^13, 2^14)): its hi parts cannot overflow and its lo parts
+            // stay normal whatever the scale of the layer; the next epilogue takes 2^-e back exactly
+            const int ex = oww_scale_exponent_of_max(vmax, -100, 100);
+            const float up = ldexpf(1.f, ex);
+            hrow[kHmRowScale] = ldexpf(1.f, -ex);
             for (int j = 0; j < N.Kp / 8; ++j) {
                 float x[8];
 #pragma unroll
                 for (int e = 0; e < 8; ++e) {
                     const int d = j * 8 + e;
-                    float v = 0.f;
-                    if (d < D) {
-                        v = hrow[d];
-                        if (H.layernorm) v = (v - mu) * rstd * g[d] + hb[d];
-                        v = fmaxf(v, 0.f);
-                    }
-                    x[e] = v;
+                    x[e] = d < D ? hrow[d] * up : 0.f;
                 }
                 uint4 hi, lo;
                 hm_split8(x, hi, lo);

@@ -13,13 +13,19 @@
 // Exponent s of the fp16 weight packings (conv layers, head Linear layers): max |w| * 2^s in [2^13, 2^14), clamped to
 // [-8, 24].  W * 2^s is packed and 2^-s folded exactly into the scale that follows, so the fp16 weights (and the lo
 // parts of hi/lo splits) stay in the normal range whatever the scale of the weights.
+// The rule on the largest magnitude alone, clamped to [lo, hi].  The tensor-core heads apply it per row to their hidden
+// activations with [-100, 100], which keeps 2^e and every 2^-(s + e) they fold back normal fp32 numbers.
+__host__ __device__ inline int oww_scale_exponent_of_max(float amax, int lo = -8, int hi = 24) {
+    if (!(amax > 0.f) || !(amax <= 3.402823466e38f)) return 0;     // zero, inf or NaN
+    int e;
+    frexpf(amax, &e);                                              // amax = m * 2^e, m in [0.5, 1)
+    e = 14 - e;
+    return e < lo ? lo : (e > hi ? hi : e);
+}
 inline int oww_weight_scale_exponent(const float* w, size_t n) {
     float amax = 0.f;
     for (size_t i = 0; i < n; ++i) amax = std::fmax(amax, std::fabs(w[i]));
-    if (!(amax > 0.f) || !std::isfinite(amax)) return 0;
-    int e;
-    std::frexp(amax, &e);                                          // amax = m * 2^e, m in [0.5, 1)
-    return std::min(24, std::max(-8, 14 - e));
+    return oww_scale_exponent_of_max(amax);
 }
 
 #define OWW_N_CONV 20
