@@ -363,6 +363,44 @@ int oww_detector_export(oww_ctx* ctx, const int32_t* h_stream_ids, int n, float*
 int oww_detector_import(oww_ctx* ctx, const int32_t* h_stream_ids, int n, const float* d_hist, const int32_t* d_counts,
                         void* stream);
 
+/* ---- stream audio on the device (openwakeword/utils.py:164,403-430: AudioFeatures.raw_data_buffer) ------------------
+ * With an audio history of H samples the handle keeps, per stream, the last H samples it stepped (int16 ring) and pos =
+ * the samples it has stepped since its reset; the ring holds samples [max(0, pos - H), pos).  Every step appends exactly
+ * the samples it steps, in stream order, in one launch per call before the frontend: oww_step, oww_step_host and
+ * oww_step_host_submit n_chunks*1280 per stream, the ragged calls cnt[b]*1280 for stream b (a held stream is untouched).
+ * Memory: 2*H + 8 bytes per stream (8192 streams x 10 s: 2.6 GB).  Samples a caller holds back (less than a chunk) are
+ * not in the ring until a step consumes them.
+ *   oww_set_audio_history - n_samples 0: off (frees); else a multiple of 1280, <= 960000 (60 s).  Synchronises the
+ *                       device; every stream starts with an empty history.  Before oww_set_streams the state is
+ *                       allocated by that call.  OWW_ENOMEM (or OWW_ECUDA) on a failed allocation, with history off.
+ *   oww_get_audio     - row i of d_out [n][n_samples] <- samples [e - n_samples, e) of stream h_stream_ids[i], e =
+ *                       h_end[i] (h_end NULL or h_end[i] < 0: the stream's pos).  An e beyond pos asks for audio after
+ *                       an event once the stream has advanced far enough (post-roll).  d_pos [n] (may be NULL) receives
+ *                       the stream's pos at that point in stream order.  Duplicate ids are allowed; 1 <= n_samples <= H.
+ *   oww_capture_events - for the event list of oww_detect, read from device memory (enqueue it right after oww_detect,
+ *                       before the host has read the count): row i < min(*d_n_events, max_events) of d_out
+ *                       [max_events][n_samples] <- the last n_samples samples of stream d_events[i].stream, ending at its
+ *                       pos; d_pos[i] (may be NULL) <- that pos.  Rows past the count are not written.  One CTA per
+ *                       possible event; those past the count exit at once.
+ *   oww_audio_export / _import - the history of streams h_stream_ids[i] <-> d_audio [n][H] oldest first (entry k is
+ *                       sample pos - H + k; zeros before sample 0) and d_pos [n].  Import takes records of the same H
+ *                       (a negative pos is taken as 0); duplicate ids fail with OWW_EINVAL.  Stream records
+ *                       (oww_export_streams) do not carry the audio: move it with these two calls.
+ * Samples outside [max(0, pos - H), pos) come out as zeros.  Every call is stream-ordered, ordered with the host-buffer
+ * steps of oww_step_host_submit (the handle's own stream), and allocates nothing after the first (oww_get_audio grows
+ * its id staging once when n exceeds the stream count).  OWW_EINVAL before anything is enqueued: no history, n_samples
+ * outside its range (or, for oww_set_audio_history, not a multiple of 1280), a stream id out of range, a NULL output.
+ * oww_reset / oww_reset_async empty the history of the streams they reset (one more launch), oww_set_streams that of
+ * all.  A handle without history launches nothing for it.                                                              */
+int oww_set_audio_history(oww_ctx* ctx, int n_samples);
+int oww_get_audio(oww_ctx* ctx, const int32_t* h_stream_ids, const int64_t* h_end, int n, int n_samples, int16_t* d_out,
+                  int64_t* d_pos, void* stream);
+int oww_capture_events(oww_ctx* ctx, const oww_event* d_events, const int32_t* d_n_events, int max_events, int n_samples,
+                       int16_t* d_out, int64_t* d_pos, void* stream);
+int oww_audio_export(oww_ctx* ctx, const int32_t* h_stream_ids, int n, int16_t* d_audio, int64_t* d_pos, void* stream);
+int oww_audio_import(oww_ctx* ctx, const int32_t* h_stream_ids, int n, const int16_t* d_audio, const int64_t* d_pos,
+                     void* stream);
+
 /* ---- batch paths --------------------------------------------------------------------------- */
 /* d_pcm [n_clips][n_samples] -> d_emb [n_clips][W][96], W = (T-76)/8+1 (utils.py:322).           */
 int oww_embed_clips(oww_ctx* ctx, const int16_t* d_pcm, int n_clips, int n_samples, float* d_emb, void* stream);

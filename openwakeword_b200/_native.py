@@ -91,6 +91,11 @@ _SIGNATURES = {
     "oww_detect": (C.c_int, [_P, _P, C.c_int, _P, _P, _P, C.c_int, _P, _P]),
     "oww_detector_export": (C.c_int, [_P, _P, C.c_int, _P, _P, _P]),
     "oww_detector_import": (C.c_int, [_P, _P, C.c_int, _P, _P, _P]),
+    "oww_set_audio_history": (C.c_int, [_P, C.c_int]),
+    "oww_get_audio": (C.c_int, [_P, _P, _P, C.c_int, C.c_int, _P, _P, _P]),
+    "oww_capture_events": (C.c_int, [_P, _P, _P, C.c_int, C.c_int, _P, _P, _P]),
+    "oww_audio_export": (C.c_int, [_P, _P, C.c_int, _P, _P, _P]),
+    "oww_audio_import": (C.c_int, [_P, _P, C.c_int, _P, _P, _P]),
     "oww_embed_clips": (C.c_int, [_P, _P, C.c_int, C.c_int, _P, _P]),
     "oww_predict_clips": (C.c_int, [_P, _P, C.c_int, C.c_int, C.c_int, _P, C.c_int, _P, _P]),
     "oww_clip_schedule": (C.c_int, [C.c_int, C.c_int64, _P, C.c_int]),
@@ -213,6 +218,7 @@ class Context:
         self._head_bank_n_in = []           # per head bank: n_in
         self.n_detect_labels = 0            # labels of the detector (set_detector)
         self._det_buf = None                # device event list and count of detect_events
+        self.audio_history = 0              # samples of audio history per stream (set_audio_history; 0 = off)
 
     def close(self):
         if getattr(self, "h", None):
@@ -665,6 +671,94 @@ class Context:
         h = torch.from_numpy(np.ascontiguousarray(hist, np.float32).reshape(ids.size, self.n_detect_labels, 30)).to(dev)
         c = torch.from_numpy(np.ascontiguousarray(counts, np.int32).reshape(ids.size)).to(dev)
         self.detector_import(ids, h, c, self._current_stream())
+
+    # ---- stream audio on the device (include/owwb200.h, oww_set_audio_history) ----
+    def set_audio_history(self, n_samples):
+        """n_samples: 0 (off) or a multiple of 1280 up to 960000.  Synchronises the device; every history starts empty."""
+        self.audio_history = 0
+        self._check(self.lib.oww_set_audio_history(self.h, int(n_samples)))
+        self.audio_history = int(n_samples)
+
+    def get_audio(self, stream_ids, ends, n_samples, d_out, d_pos, stream=None):
+        """oww_get_audio: ends None or host int64 [n] (< 0: the stream's pos)."""
+        ids = np.ascontiguousarray(stream_ids, np.int32).ravel()
+        e = None if ends is None else np.ascontiguousarray(ends, np.int64).ravel()
+        if e is not None and e.size != ids.size:
+            raise ValueError(f"{e.size} ends for {ids.size} streams")
+        self._check(self.lib.oww_get_audio(self.h, _ptr(ids), _ptr(e), ids.size, int(n_samples), _ptr(d_out), _ptr(d_pos),
+                                           stream))
+
+    def capture_events(self, d_events, d_n_events, max_events, n_samples, d_out, d_pos, stream=None):
+        self._check(self.lib.oww_capture_events(self.h, _ptr(d_events), _ptr(d_n_events), int(max_events), int(n_samples),
+                                                _ptr(d_out), _ptr(d_pos), stream))
+
+    def audio_export(self, stream_ids, d_audio, d_pos, stream=None):
+        ids = np.ascontiguousarray(stream_ids, np.int32).ravel()
+        self._check(self.lib.oww_audio_export(self.h, _ptr(ids), ids.size, _ptr(d_audio), _ptr(d_pos), stream))
+
+    def audio_import(self, stream_ids, d_audio, d_pos, stream=None):
+        ids = np.ascontiguousarray(stream_ids, np.int32).ravel()
+        self._check(self.lib.oww_audio_import(self.h, _ptr(ids), ids.size, _ptr(d_audio), _ptr(d_pos), stream))
+
+    def read_audio(self, stream_ids, n_samples, ends=None):
+        """oww_get_audio on the current CUDA stream into new tensors -> (int16 [n, n_samples] on the device, int64 [n]
+        pos on the device)"""
+        import torch
+        ids = np.ascontiguousarray(stream_ids, np.int32).ravel()
+        dev = torch.device("cuda", self.device)
+        out = torch.empty((ids.size, int(n_samples)), dtype=torch.int16, device=dev)
+        pos = torch.empty(ids.size, dtype=torch.int64, device=dev)
+        self.get_audio(ids, ends, n_samples, out, pos, self._current_stream())
+        return out, pos
+
+    def detect_capture(self, d_scores, prepared, n_samples, max_events=None):
+        """detect_events with oww_capture_events enqueued right after oww_detect -> (events, n, clips int16 [min(n,
+        max_events), n_samples] on the device, ends int64 [same] on the host).  max_events None: the clips are gathered
+        once the count is known (n_streams * n_labels rows of clips could be gigabytes), with nothing enqueued between."""
+        import torch
+        dev = torch.device("cuda", self.device)
+        if max_events is None:
+            events, n = self.detect_events(d_scores, prepared)
+            clips = torch.empty((n, int(n_samples)), dtype=torch.int16, device=dev)
+            ends = torch.empty(n, dtype=torch.int64, device=dev)
+            if n:
+                self.capture_events(self._det_buf[0], self._det_buf[1], n, n_samples, clips, ends, self._current_stream())
+            return events, n, clips, ends.cpu().numpy()
+        cap = int(max_events)
+        if self._det_buf is None or self._det_buf[0].shape[0] < cap:
+            self._det_buf = (torch.empty((cap, 4), dtype=torch.int32, device=dev),
+                             torch.zeros(1, dtype=torch.int32, device=dev))
+        ev, n_ev = self._det_buf
+        clips = torch.empty((cap, int(n_samples)), dtype=torch.int16, device=dev)
+        ends = torch.empty(cap, dtype=torch.int64, device=dev)
+        s = self._current_stream()
+        self.detect(d_scores, prepared, None, ev if cap else None, cap, n_ev, s)
+        self.capture_events(ev, n_ev, cap, n_samples, clips, ends, s)
+        n = int(n_ev.item())
+        k = min(n, cap)
+        return ev[:k].cpu().numpy().view(EVENT_DTYPE).reshape(-1), n, clips[:k], ends[:k].cpu().numpy()
+
+    def audio_state(self, stream_ids):
+        """-> (int16 [n, H] oldest first, int64 [n] pos) host arrays of the listed streams (synchronises)"""
+        import torch
+        ids = np.ascontiguousarray(stream_ids, np.int32).ravel()
+        dev = torch.device("cuda", self.device)
+        audio = torch.empty((ids.size, self.audio_history), dtype=torch.int16, device=dev)
+        pos = torch.empty(ids.size, dtype=torch.int64, device=dev)
+        self.audio_export(ids, audio, pos, self._current_stream())
+        return audio.cpu().numpy(), pos.cpu().numpy()
+
+    def set_audio_state(self, stream_ids, audio, pos):
+        """the reverse of audio_state (distinct ids, records of this handle's H), on the current CUDA stream"""
+        import torch
+        ids = np.ascontiguousarray(stream_ids, np.int32).ravel()
+        a = np.ascontiguousarray(audio, np.int16)
+        if a.shape != (ids.size, self.audio_history):
+            raise ValueError(f"audio has shape {a.shape}; this handle keeps [{ids.size}, {self.audio_history}]")
+        dev = torch.device("cuda", self.device)
+        d = torch.from_numpy(a).to(dev)
+        p = torch.from_numpy(np.ascontiguousarray(pos, np.int64).reshape(ids.size)).to(dev)
+        self.audio_import(ids, d, p, self._current_stream())
 
     # ---- batch ----
     def embed_clips(self, d_pcm, n_clips, n_samples, d_emb, stream=None):

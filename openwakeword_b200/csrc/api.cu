@@ -255,6 +255,7 @@ void free_streams(oww_ctx* c) {
     c->rag_streams = 0;
     oww_verifiers_free_streams(c);
     oww_detect_free_streams(c);
+    oww_audio_free_streams(c);
     oww_heads_grp_drop_mirror(c);
     for (auto& X : c->late_x) for (auto& b : X.buf) { cudaFree(b); b = nullptr; }
     cudaFree(c->d_late_tmp); c->d_late_tmp = nullptr;
@@ -420,15 +421,22 @@ int stride_check(oww_ctx* ctx, int64_t pcm_stride, int n_chunks) {
     return OWW_OK;
 }
 
-int step_core(oww_ctx* ctx, const int16_t* d_pcm, int64_t pcm_stride, int n_chunks, float* d_scores, int out_stride,
-              cudaStream_t s) {
-    const int B = ctx->n_streams;
+// what step_core refuses before it enqueues anything
+int step_core_check(oww_ctx* ctx, int64_t pcm_stride, int n_chunks) {
     int rc;
-    if (B <= 0) return oww_fail(ctx, OWW_EINVAL, "oww_set_streams has not been called");
+    if (ctx->n_streams <= 0) return oww_fail(ctx, OWW_EINVAL, "oww_set_streams has not been called");
     if (n_chunks < 1 || n_chunks > ctx->cfg.max_chunks)
         return oww_fail(ctx, OWW_EINVAL, "n_chunks=%d outside [1,%d]", n_chunks, ctx->cfg.max_chunks);
     if ((rc = stride_check(ctx, pcm_stride, n_chunks))) return rc;
     if (!ctx->mel_loaded || !ctx->emb_loaded) return oww_fail(ctx, OWW_EINVAL, "weights not loaded");
+    return OWW_OK;
+}
+
+int step_core(oww_ctx* ctx, const int16_t* d_pcm, int64_t pcm_stride, int n_chunks, float* d_scores, int out_stride,
+              cudaStream_t s) {
+    const int B = ctx->n_streams;
+    int rc;
+    if ((rc = step_core_check(ctx, pcm_stride, n_chunks))) return rc;
     const long slot = ctx->timing ? ctx->ev_steps % ctx->ev_slots : 0;
     cudaEvent_t* ev = ctx->timing ? &ctx->ev[4 * slot] : nullptr;
     const bool inc = ctx->cfg.cnn_mode == OWW_CNN_TC_INCREMENTAL;
@@ -526,32 +534,10 @@ int carry_launch(oww_ctx* ctx, const int* d_ids, int n, cudaStream_t s) {
     return OWW_OK;
 }
 
-// Ragged step (oww_step_ragged): stream b steps cnt[b] = h_chunks[b] chunks, the first cnt[b]*1280 samples of its row;
-// n = max cnt >= 1 and the counts are not all equal (the caller runs those as oww_step).  Streams that do not step in a
-// launch are dead slots there: no state, ring or score write; carry_kernel moves their rotating tails.  Multi-chunk
-// calls run right-aligned: CNN launch i steps the streams with cnt >= n - i, so its window offset 8*(n-1-i) is right
-// relative to each stream's own mel count.
-int step_ragged_core(oww_ctx* ctx, const int16_t* d_pcm, int64_t pcm_stride, const int32_t* h_chunks, int n, float* d_scores,
-                     int out_stride, cudaStream_t s) {
-    const int B = ctx->n_streams, n_out = ctx->n_out_total, mc = ctx->cfg.max_chunks;
-    int rc;
-    const bool inc = ctx->cfg.cnn_mode == OWW_CNN_TC_INCREMENTAL;
-    if (inc && n > 1 && oww_fused_heads_supported(ctx)) {
-        // oww_step(1) runs the heads inside the fused kernel (its own summation order): streams with one chunk take
-        // that launch as a ragged step of their own, the others the general path
-        std::vector<int32_t> one(B), more(B);
-        bool any_one = false;
-        for (int b = 0; b < B; ++b) {
-            one[b] = h_chunks[b] == 1;
-            more[b] = h_chunks[b] >= 2 ? h_chunks[b] : 0;
-            any_one = any_one || h_chunks[b] == 1;
-        }
-        if (any_one) {
-            if ((rc = step_ragged_core(ctx, d_pcm, pcm_stride, one.data(), 1, d_scores, out_stride, s))) return rc;
-            return step_ragged_core(ctx, d_pcm, pcm_stride, more.data(), n, d_scores, out_stride, s);
-        }
-    }
-    // staging: [B counts | B stream ids by ascending count]; below[c] = number of streams with fewer than c chunks
+// Staging of a ragged step's counts: [B counts | B stream ids by ascending count] in the next slot of the ring, copied on
+// `s` -> its device copy; below[c] = number of streams with fewer than c chunks.
+int stage_ragged(oww_ctx* ctx, const int32_t* h_chunks, cudaStream_t s, std::vector<int>& below, const int** d_staged) {
+    const int B = ctx->n_streams, mc = ctx->cfg.max_chunks;
     if (ctx->rag_streams != B) {
         for (int j = 0; j < oww_ctx::kRagSlots; ++j) {
             if (ctx->rag_ev[j]) OWW_CUDA(ctx, cudaEventSynchronize(ctx->rag_ev[j]));
@@ -565,17 +551,11 @@ int step_ragged_core(oww_ctx* ctx, const int16_t* d_pcm, int64_t pcm_stride, con
         }
         ctx->rag_streams = B;
     }
-    const size_t need = (size_t)mc * B * n_out;
-    if (ctx->rag_scores_floats < need) {
-        cudaFree(ctx->d_rag_scores); ctx->d_rag_scores = nullptr; ctx->rag_scores_floats = 0;
-        OWW_CUDA(ctx, cudaMalloc(&ctx->d_rag_scores, need * sizeof(float)));
-        ctx->rag_scores_floats = need;
-    }
     const int j = ctx->rag_next;
     ctx->rag_next = (j + 1) % oww_ctx::kRagSlots;
     OWW_CUDA(ctx, cudaEventSynchronize(ctx->rag_ev[j]));          // the copy of the call kRagSlots back has run
     int32_t* h = ctx->h_rag[j];
-    std::vector<int> below(mc + 2, 0);
+    below.assign(mc + 2, 0);
     for (int b = 0; b < B; ++b) below[h_chunks[b] + 1]++;
     for (int c = 1; c <= mc + 1; ++c) below[c] += below[c - 1];
     {
@@ -584,7 +564,50 @@ int step_ragged_core(oww_ctx* ctx, const int16_t* d_pcm, int64_t pcm_stride, con
     }
     OWW_CUDA(ctx, cudaMemcpyAsync(ctx->d_rag[j], h, (size_t)2 * B * sizeof(int32_t), cudaMemcpyHostToDevice, s));
     OWW_CUDA(ctx, cudaEventRecord(ctx->rag_ev[j], s));
-    const int* d_cnt = ctx->d_rag[j];
+    *d_staged = ctx->d_rag[j];
+    return OWW_OK;
+}
+
+// Ragged step (oww_step_ragged): stream b steps cnt[b] = h_chunks[b] chunks, the first cnt[b]*1280 samples of its row;
+// n = max cnt >= 1 and the counts are not all equal (the caller runs those as oww_step).  Streams that do not step in a
+// launch are dead slots there: no state, ring or score write; carry_kernel moves their rotating tails.  Multi-chunk
+// calls run right-aligned: CNN launch i steps the streams with cnt >= n - i, so its window offset 8*(n-1-i) is right
+// relative to each stream's own mel count.  audio: append the streams' samples to their audio history first (the
+// entry point's call; not the calls this one makes on split counts).
+int step_ragged_core(oww_ctx* ctx, const int16_t* d_pcm, int64_t pcm_stride, const int32_t* h_chunks, int n, float* d_scores,
+                     int out_stride, cudaStream_t s, bool audio) {
+    const int B = ctx->n_streams, n_out = ctx->n_out_total, mc = ctx->cfg.max_chunks;
+    int rc;
+    const bool inc = ctx->cfg.cnn_mode == OWW_CNN_TC_INCREMENTAL;
+    std::vector<int> below;
+    const int* d_cnt = nullptr;
+    if (inc && n > 1 && oww_fused_heads_supported(ctx)) {
+        // oww_step(1) runs the heads inside the fused kernel (its own summation order): streams with one chunk take
+        // that launch as a ragged step of their own, the others the general path
+        std::vector<int32_t> one(B), more(B);
+        bool any_one = false;
+        for (int b = 0; b < B; ++b) {
+            one[b] = h_chunks[b] == 1;
+            more[b] = h_chunks[b] >= 2 ? h_chunks[b] : 0;
+            any_one = any_one || h_chunks[b] == 1;
+        }
+        if (any_one) {
+            if (audio && ctx->audio) {                     // the whole call's counts, for its one append
+                if ((rc = stage_ragged(ctx, h_chunks, s, below, &d_cnt))) return rc;
+                if ((rc = oww_audio_append(ctx, d_pcm, pcm_stride, n, d_cnt, s))) return rc;
+            }
+            if ((rc = step_ragged_core(ctx, d_pcm, pcm_stride, one.data(), 1, d_scores, out_stride, s, false))) return rc;
+            return step_ragged_core(ctx, d_pcm, pcm_stride, more.data(), n, d_scores, out_stride, s, false);
+        }
+    }
+    const size_t need = (size_t)mc * B * n_out;
+    if (ctx->rag_scores_floats < need) {
+        cudaFree(ctx->d_rag_scores); ctx->d_rag_scores = nullptr; ctx->rag_scores_floats = 0;
+        OWW_CUDA(ctx, cudaMalloc(&ctx->d_rag_scores, need * sizeof(float)));
+        ctx->rag_scores_floats = need;
+    }
+    if ((rc = stage_ragged(ctx, h_chunks, s, below, &d_cnt))) return rc;
+    if (audio && (rc = oww_audio_append(ctx, d_pcm, pcm_stride, n, d_cnt, s))) return rc;
     const int* d_ord = d_cnt + B;
     const FeatSrc fs0{ctx->d_feat_ring, (int64_t)ctx->feat_rows * 96, ctx->d_feat_count, ctx->feat_rows - 1, 0};
     auto append = [&](int n_launch) {
@@ -711,6 +734,7 @@ int reset_enqueue(oww_ctx* ctx, const int32_t* h_stream_ids, int n, const float*
     OWW_LAUNCH_CHECK(ctx);
     int rc = oww_detect_reset(ctx, h_stream_ids ? ctx->d_reset_ids : nullptr, n, s);    // the detector's history of those streams
     if (rc) return rc;
+    if ((rc = oww_audio_reset(ctx, h_stream_ids ? ctx->d_reset_ids : nullptr, n, s))) return rc;     // ... and their audio
     return oww_feat16_resync(ctx, h_stream_ids ? ctx->d_reset_ids : nullptr, n, s);     // fp16 mirror of the rings (heads_grp.cu)
 }
 
@@ -854,6 +878,7 @@ void oww_destroy(oww_ctx* ctx) {
     oww_head_banks_free(ctx);
     oww_verifier_fit_free(ctx);
     oww_detect_free(ctx);
+    oww_audio_free(ctx);
     cudaFree(ctx->d_window); cudaFree(ctx->d_twiddle); cudaFree(ctx->d_mel_start); cudaFree(ctx->d_mel_len);
     cudaFree(ctx->d_mel_w); cudaFree(ctx->d_emb_blob); cudaFree(ctx->d_tc_w); cudaFree(ctx->d_tc_sb);
     cudaFree(ctx->d_tc_w3); cudaFree(ctx->d_tc_sb3);
@@ -1043,6 +1068,7 @@ int oww_set_streams(oww_ctx* ctx, int n_streams) {
     if ((rc = oww_verifiers_alloc_streams(ctx))) return rc;         // every stream starts without a verifier
     if ((rc = oww_head_banks_alloc_streams(ctx))) return rc;        // ... and without a bank head
     if ((rc = oww_detect_alloc_streams(ctx))) return rc;            // ... and with an empty detector history
+    if ((rc = oww_audio_alloc_streams(ctx))) return rc;             // ... and an empty audio history
     return oww_reset(ctx, nullptr, B, nullptr, OWW_INIT_FEATURE_ROWS);
 }
 
@@ -1097,6 +1123,9 @@ int oww_stream_state_status(oww_ctx* ctx, int* n_rejected) {
 int oww_step(oww_ctx* ctx, const int16_t* d_pcm, int64_t pcm_stride, int n_chunks, float* d_scores, void* stream) {
     if (!ctx || !d_pcm || !d_scores) return oww_fail(ctx, OWW_EINVAL, "null argument");
     OWW_CUDA(ctx, cudaSetDevice(ctx->device));
+    int rc = step_core_check(ctx, pcm_stride, n_chunks);
+    if (rc) return rc;
+    if ((rc = oww_audio_append(ctx, d_pcm, pcm_stride, n_chunks, nullptr, (cudaStream_t)stream))) return rc;
     return step_core(ctx, d_pcm, pcm_stride, n_chunks, d_scores, ctx->n_out_total, (cudaStream_t)stream);
 }
 
@@ -1121,8 +1150,11 @@ int oww_step_ragged(oww_ctx* ctx, const int16_t* d_pcm, int64_t pcm_stride, cons
     if (rc) return rc;
     if (n == 0) return OWW_OK;
     if (!d_pcm) return oww_fail(ctx, OWW_EINVAL, "null argument");
-    if (eq) return step_core(ctx, d_pcm, pcm_stride, n, d_scores, ctx->n_out_total, (cudaStream_t)stream);
-    return step_ragged_core(ctx, d_pcm, pcm_stride, h_chunks, n, d_scores, ctx->n_out_total, (cudaStream_t)stream);
+    if (eq) {
+        if ((rc = oww_audio_append(ctx, d_pcm, pcm_stride, n, nullptr, (cudaStream_t)stream))) return rc;
+        return step_core(ctx, d_pcm, pcm_stride, n, d_scores, ctx->n_out_total, (cudaStream_t)stream);
+    }
+    return step_ragged_core(ctx, d_pcm, pcm_stride, h_chunks, n, d_scores, ctx->n_out_total, (cudaStream_t)stream, true);
 }
 
 int oww_step_host_ragged_submit(oww_ctx* ctx, const int16_t* h_pcm, int64_t pcm_stride, const int32_t* h_chunks, int* ticket) {
@@ -1200,8 +1232,11 @@ int host_submit(oww_ctx* ctx, const int16_t* h_pcm, int64_t pcm_stride, int n_ch
         OWW_CUDA(ctx, cudaMemcpyAsync(S.d_pcm, src, pcm_bytes, cudaMemcpyHostToDevice, ctx->copy_stream));
         OWW_CUDA(ctx, cudaEventRecord(S.h2d_done, ctx->copy_stream));
         OWW_CUDA(ctx, cudaStreamWaitEvent(s, S.h2d_done, 0));
-        int rc = all_step ? step_core(ctx, S.d_pcm, (int64_t)row, n_chunks, S.d_scores, ctx->n_out_total, s)
-                          : step_ragged_core(ctx, S.d_pcm, (int64_t)row, h_chunks, n_chunks, S.d_scores, ctx->n_out_total, s);
+        int rc = all_step ? step_core_check(ctx, (int64_t)row, n_chunks) : OWW_OK;
+        if (!rc && all_step) rc = oww_audio_append(ctx, S.d_pcm, (int64_t)row, n_chunks, nullptr, s);
+        if (rc) return rc;
+        rc = all_step ? step_core(ctx, S.d_pcm, (int64_t)row, n_chunks, S.d_scores, ctx->n_out_total, s)
+                      : step_ragged_core(ctx, S.d_pcm, (int64_t)row, h_chunks, n_chunks, S.d_scores, ctx->n_out_total, s, true);
         if (rc) return rc;
         if (ctx->n_out_total > 0)
             OWW_CUDA(ctx, cudaMemcpyAsync(S.h_scores, S.d_scores, (size_t)B * ctx->n_out_total * sizeof(float),

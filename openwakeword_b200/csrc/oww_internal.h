@@ -324,6 +324,7 @@ struct oww_ctx {
     struct oww_heads_grp* heads_grp = nullptr;
     int tc_heads_terms = 3;          // 3 = hi*hi + lo*hi + hi*lo (fp32-grade), 1 = plain fp16 operands
     struct oww_detector* det = nullptr;   // detections on the device (detect.cu); nullptr: no detector configured
+    struct oww_audio* audio = nullptr;    // the streams' recent audio (audio.cu); nullptr: no history
 };
 
 int oww_fail(oww_ctx* ctx, int code, const char* fmt, ...);
@@ -535,6 +536,17 @@ void oww_detect_free_streams(oww_ctx* ctx);
 int oww_detect_alloc_streams(oww_ctx* ctx);      // for ctx->n_streams streams, every history empty; the device is idle
 // the listed streams (d_ids == nullptr: streams 0..n-1) start afresh: one launch on `s`
 int oww_detect_reset(oww_ctx* ctx, const int* d_ids, int n, cudaStream_t s);
+
+// ---- audio.cu: the streams' recent audio (nothing happens on a handle without history) ----
+void oww_audio_free(oww_ctx* ctx);
+void oww_audio_free_streams(oww_ctx* ctx);
+int oww_audio_alloc_streams(oww_ctx* ctx);       // for ctx->n_streams streams, every history empty; the device is idle
+// the listed streams (d_ids == nullptr: streams 0..n-1) start with an empty history: one launch on `s`
+int oww_audio_reset(oww_ctx* ctx, const int* d_ids, int n, cudaStream_t s);
+// one launch on `s`: stream b appends the first cnt * 1280 samples of its row, cnt = d_counts[b] (device; nullptr:
+// n_chunks for every stream)
+int oww_audio_append(oww_ctx* ctx, const int16_t* d_pcm, int64_t pcm_stride, int n_chunks, const int* d_counts,
+                     cudaStream_t s);
 
 // ---- verifier.cu: custom verifier banks ----
 // every bank of the handle on n rows of final scores (one launch; nothing when the handle has no bank).  The window of

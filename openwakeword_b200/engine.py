@@ -158,7 +158,7 @@ class StreamEngine:
             table.append((col, rep, thr, patience.get(j, 0)))
         self.ctx.set_detector(table, debounce_time)
 
-    def detect(self, scores, prepared=1280, final=None, max_events=None):
+    def detect(self, scores, prepared=1280, final=None, max_events=None, capture=None):
         """The detections of the step that wrote `scores` (float32 [n_streams, n_cols] on the engine's device).
         prepared: the samples every stream prepared in that step, or host ints [n_streams] (< 0: the stream is skipped,
         as for one held in step_ragged; 0..1279: it repeats its previous prediction).  final: float32 [n_streams, n_labels]
@@ -168,12 +168,40 @@ class StreamEngine:
         score, index = which prediction of the stream since its reset).  max_events None: n_streams * n_labels.
         Runs on the current CUDA stream and synchronises it to read the count; only the count and the events are copied.
         Typical loop:  scores = eng.step_ragged(pcm, chunks);
-                       ev, n = eng.detect(scores, np.where(chunks > 0, chunks * 1280, -1))"""
+                       ev, n = eng.detect(scores, np.where(chunks > 0, chunks * 1280, -1))
+        capture: a number of samples (needs set_audio_history): the last `capture` samples of each event's stream are
+        gathered on the device right after the detection, before the count is read, and the call returns (events, n,
+        clips, ends): clips int16 [min(n, max_events), capture] on the device, ends int64 (host) = each clip's end, the
+        stream's sample position.  `final` is not written then."""
         torch = _torch()
         self.ctx._cuda("scores", scores, torch.float32, (self.n_streams, self.n_cols))
+        if capture is not None:
+            return self.ctx.detect_capture(scores, prepared, int(capture), max_events)
         if final is not None:
             self.ctx._cuda("final", final, torch.float32, (self.n_streams, self.ctx.n_detect_labels))
         return self.ctx.detect_events(scores, prepared, final, max_events)
+
+    # ---- stream audio on the device (include/owwb200.h, oww_set_audio_history) ----
+    def set_audio_history(self, n_samples):
+        """Keep the last n_samples (a multiple of 1280, up to 960000; 0 = off) samples every stream steps on the device.
+        Synchronises the device; every stream starts with an empty history."""
+        self.ctx.set_audio_history(n_samples)
+
+    def get_audio(self, stream_ids, n_samples, end=None):
+        """-> (int16 [n, n_samples] on the device, int64 [n] on the device): row i = samples [e - n_samples, e) of stream
+        stream_ids[i] (ids may repeat), e = end[i] (None or < 0: the stream's position, the samples it has stepped since its
+        reset), and the stream's position.  Samples the history does not hold (before it, overwritten, or not stepped yet)
+        are zeros.  Enqueued on the current CUDA stream, after the steps enqueued there and the submitted host steps."""
+        return self.ctx.read_audio(stream_ids, n_samples, end)
+
+    def audio_history(self, stream_ids):
+        """-> (int16 [n, H] oldest first, int64 [n] positions) host arrays of the listed streams, for moving them"""
+        return self.ctx.audio_state(stream_ids)
+
+    def set_audio_history_state(self, stream_ids, audio, pos):
+        """Streams stream_ids (distinct) continue from the history `audio_history` returned, of this engine or another
+        with the same history length."""
+        self.ctx.set_audio_state(stream_ids, audio, pos)
 
     def detector_history(self, stream_ids):
         """-> (float32 [n, n_labels, 30] oldest first, int32 [n] predictions since the reset) of the listed streams"""

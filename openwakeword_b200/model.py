@@ -559,9 +559,12 @@ class Model:
         buf, lens = pre._ragged_pending()
         labels = self.labels()
         self._pull_history()
+        audio = None
+        if pre.audio_history_samples:
+            audio = pre.ctx.audio_state(ids) + (pre._held_in_raw[ids].copy(),)
         return StreamState(records, key, labels, [buf[b, :lens[b]].copy() for b in ids],
                            {lab: self._h(lab)[0][:, ids].copy() for lab in labels},
-                           {lab: self._h(lab)[1][ids].copy() for lab in labels})
+                           {lab: self._h(lab)[1][ids].copy() for lab in labels}, audio)
 
     def import_streams(self, stream_ids, state):
         """Streams stream_ids (distinct) become the streams `state` was exported from: device state, samples not yet
@@ -581,7 +584,14 @@ class Model:
             raise ValueError("the streams were exported under another configuration (cnn_mode, split_from or weights)")
         if list(state.labels) != self.labels():
             raise ValueError(f"the streams were exported with the labels {list(state.labels)}, this Model has {self.labels()}")
+        h_state = 0 if state.audio is None else state.audio[0].shape[1]
+        if h_state != pre.audio_history_samples:
+            raise ValueError(f"the streams were exported with an audio history of {h_state} samples, this Model keeps "
+                             f"{pre.audio_history_samples}")
         pre.ctx.import_records(ids, state.records)
+        if state.audio is not None:
+            pre.ctx.set_audio_state(ids, state.audio[0], state.audio[1])
+            pre._held_in_raw[ids] = state.audio[2]
         buf, lens = pre._ragged_pending()
         for i, b in enumerate(ids):
             p = state.pending[i]
@@ -688,7 +698,7 @@ class Model:
         return self._finish(n_prepared, split, patience, threshold, debounce_time, timing, t0, B == 1)
 
     # ---- detections on the device (include/owwb200.h, oww_set_detector / oww_detect) ----
-    def detect(self, x, threshold, patience={}, debounce_time=0.0):
+    def detect(self, x, threshold, patience={}, debounce_time=0.0, capture=None):
         """``predict(x, patience, threshold, debounce_time)`` that returns only the detections of this call: a list of
         (stream id, label, score) for every label whose prediction is >= the threshold of its model, ordered by stream,
         then by label in ``labels()`` order.  threshold: {model name: float} as in the reference (a model without one
@@ -704,15 +714,20 @@ class Model:
 
         One difference from ``predict``, only on models with device verifier banks: a stream that prepares fewer than
         1280 samples repeats its previous prediction as stored; ``predict`` passes the repeated value through the
-        verifier once more."""
+        verifier once more.
+
+        capture: seconds (needs ``audio_history``).  Each event then becomes (stream id, label, score, audio, end): audio
+        = the last ``capture`` seconds the stream stepped (int16; zeros for what its history does not hold), gathered on
+        the device right after the detection, and end = the stream's sample position at its last sample (what
+        ``get_audio(end=...)`` takes for audio after the event).  Without capture the return value is unchanged."""
         if not isinstance(x, np.ndarray):
             raise ValueError(f"The input audio data (x) must by a Numpy array, instead received an object of type {type(x)}.")
         self._detect_refusals()
         if self.speex_ns:
             x = self._suppress_noise_with_speex(x)
-        return self._detect(self.preprocessor._coerce(x), threshold, patience, debounce_time)
+        return self._detect(self.preprocessor._coerce(x), threshold, patience, debounce_time, capture)
 
-    def detect_ragged(self, x, threshold, patience={}, debounce_time=0.0):
+    def detect_ragged(self, x, threshold, patience={}, debounce_time=0.0, capture=None):
         """``detect`` with the inputs of ``predict_ragged``: one 1-D array of any length per stream."""
         B = self.n_streams
         try:
@@ -729,7 +744,7 @@ class Model:
         self._detect_refusals()
         if self.speex_ns:
             xs = [self._suppress_noise_with_speex(xs[0])]
-        return self._detect(xs, threshold, patience, debounce_time)
+        return self._detect(xs, threshold, patience, debounce_time, capture)
 
     def _detect_refusals(self):
         if self._host_verifiers:
@@ -761,13 +776,14 @@ class Model:
                 table.append((col, repeats, None if thr is None else float(thr), pat))
         return table
 
-    def _detect(self, xs, threshold, patience, debounce_time):
+    def _detect(self, xs, threshold, patience, debounce_time, capture=None):
         pre = self.preprocessor
         pre._ensure_streams()
         ctx = pre.ctx
         labels = self.labels()
         if not labels:
             raise ValueError("detect needs at least one model")
+        n_capture = None if capture is None else self._audio_samples(capture)
         table = self._detector_table(threshold, patience, debounce_time)
         lockstep = isinstance(xs, np.ndarray) and not pre.pending_ragged      # as predict: one length, one remainder
         if not lockstep:
@@ -791,8 +807,40 @@ class Model:
             n_prepared = pre._streaming_features(xs, self._d_scores, device=True)[0]
         else:
             n_prepared = pre._streaming_features_ragged(xs, self._d_scores, device=True)[0].astype(np.int32)
-        events, n = ctx.detect_events(self._d_scores, n_prepared)
-        return list(zip(events["stream"].tolist(), [labels[j] for j in events["label"].tolist()], events["score"].tolist()))
+        if n_capture is None:
+            events, n = ctx.detect_events(self._d_scores, n_prepared)
+            return list(zip(events["stream"].tolist(), [labels[j] for j in events["label"].tolist()],
+                            events["score"].tolist()))
+        events, n, clips, ends = ctx.detect_capture(self._d_scores, n_prepared, n_capture)
+        clips = clips.cpu().numpy()
+        return list(zip(events["stream"].tolist(), [labels[j] for j in events["label"].tolist()], events["score"].tolist(),
+                        list(clips), ends.tolist()))
+
+    # ---- stream audio on the device (include/owwb200.h, oww_set_audio_history) ----
+    def _audio_samples(self, seconds):
+        H = self.preprocessor.audio_history_samples
+        if not H:
+            raise ValueError("stream audio needs the audio history: construct the Model with audio_history=<seconds>")
+        n = int(round(float(seconds) * 16000))
+        if not 1 <= n <= H:
+            raise ValueError(f"{seconds} s is outside (0, {H / 16000}] s, the audio history")
+        return n
+
+    def get_audio(self, stream_ids, seconds, end=None):
+        """The audio the listed streams stepped (ids may repeat) -> (int16 [n, samples], int64 [n] ends): row i = the
+        ``seconds`` of stream stream_ids[i] that end at sample position end[i] (the samples the stream has stepped since
+        its reset; None or < 0: its current position, which ``ends`` then reports).  Samples the history does not hold -
+        before it, overwritten, or not stepped yet (an end past the position asks for audio after an event, to be read
+        once the stream has advanced) - are zeros.  Samples held back because they do not fill a chunk are not
+        included: only stepped audio is, addressed by stream sample position."""
+        pre = self.preprocessor
+        pre._ensure_streams()
+        n = self._audio_samples(seconds)
+        ids = self._ids(stream_ids)
+        e = None if end is None else np.broadcast_to(np.asarray(end, np.int64), ids.shape).copy()
+        clips, pos = pre.ctx.read_audio(ids, n, e)
+        pos = pos.cpu().numpy()
+        return clips.cpu().numpy(), pos if e is None else np.where(e >= 0, e, pos)
 
     def _finish(self, n_prepared, split, patience, threshold, debounce_time, timing, t0, single):
         """model.py:285-386 per stream after the device step(s): stream b prepared n_prepared[b] samples (its row of
@@ -1109,18 +1157,21 @@ class StreamState:
     """Streams exported by ``Model.export_streams``, in export order: ``records`` (torch.uint8 [n, record bytes], the
     device state of include/owwb200.h), ``key`` (the configuration the records are valid under), ``labels``, and per
     stream what the host keeps: ``pending`` (int16 samples not yet stepped), ``history`` / ``counts`` ({label: float32
-    [30, n] prediction ring, int64 [n] predictions appended}).  ``to(device)`` moves the records; on the CPU it
-    pickles."""
+    [30, n] prediction ring, int64 [n] predictions appended}), ``audio`` (None without an audio history, else the
+    history: int16 [n, H] oldest first, int64 [n] sample positions, bool [n] whether the samples held not yet stepped
+    count in ``raw_data_buffer``).  ``to(device)`` moves the records; on the CPU it pickles."""
 
-    def __init__(self, records, key, labels, pending, history, counts):
+    def __init__(self, records, key, labels, pending, history, counts, audio=None):
         self.records, self.key, self.labels = records, int(key), list(labels)
         self.pending, self.history, self.counts = pending, history, counts
+        self.audio = audio
 
     def __len__(self):
         return len(self.pending)
 
     def to(self, device):
-        return StreamState(self.records.to(device), self.key, self.labels, self.pending, self.history, self.counts)
+        return StreamState(self.records.to(device), self.key, self.labels, self.pending, self.history, self.counts,
+                           self.audio)
 
 
 def _concat_clips(clips):

@@ -10,6 +10,7 @@ errors; all arithmetic is in the CUDA library.
 import functools
 import os
 import wave
+from collections import deque
 
 import numpy as np
 
@@ -68,16 +69,20 @@ class AudioFeatures:
     axis; 1 behaves exactly like the reference object), ``feature_init`` ([rows,96] initial content
     of the embedding ring - the reference fills it from unseeded noise, SURVEY.md F6; default is
     the embeddings of ``np.random.randint(-1000,1000,64000)`` computed on the GPU, as the reference
-    does), ``max_chunks`` (largest multiple of 1280 samples one call may carry), ``cnn_mode``.
+    does), ``max_chunks`` (largest multiple of 1280 samples one call may carry), ``cnn_mode``, ``audio_history``
+    (seconds, a multiple of 0.08; 0 = off): the last samples every stream stepped are kept on the device
+    (include/owwb200.h, oww_set_audio_history) and ``raw_data_buffer`` reads them as the reference's deque.
     """
 
     def __init__(self, melspec_model_path="", embedding_model_path="", sr=16000, ncpu=1,
                  inference_framework="b200", device="gpu", n_streams=1, feature_init=None,
-                 max_chunks=8, cnn_mode=_native.CNN_TC_INCREMENTAL, window_batch=0, device_index=0, split_from=None):
+                 max_chunks=8, cnn_mode=_native.CNN_TC_INCREMENTAL, window_batch=0, device_index=0, split_from=None,
+                 audio_history=0.0):
         if inference_framework != "b200":
             raise ValueError(f"openwakeword_b200 only provides inference_framework='b200' (got '{inference_framework}')")
         if sr != 16000:
             raise ValueError("only 16 kHz audio is supported")
+        self.audio_history_samples = audio_history_samples(audio_history)
         self.ctx = _native.Context(device=device_index, max_chunks=max_chunks, cnn_mode=cnn_mode,
                                    window_batch=window_batch, split_from=split_from)
         if melspec_model_path.endswith(".npz"):
@@ -89,6 +94,8 @@ class AudioFeatures:
             self.ctx.load_mel()
         self.embedding_weights = load_embedding_weights(embedding_model_path)
         self.ctx.load_embedding(_weights.pack_embedding_blob(self.embedding_weights))
+        if self.audio_history_samples:
+            self.ctx.set_audio_history(self.audio_history_samples)
         self.n_streams = int(n_streams)
         self.cnn_mode = cnn_mode
         self.max_chunks = max_chunks
@@ -100,6 +107,9 @@ class AudioFeatures:
         self._streams_ready = False
         self._pending = np.zeros((self.n_streams, 0), np.int16)
         self._rpend = None
+        # per stream: the samples it holds not yet stepped are in the reference's raw_data_buffer (its last call stepped
+        # nothing, accumulated_samples > 0 there); a remainder left after a step is not
+        self._held_in_raw = np.zeros(self.n_streams, bool)
         self._verifier_banks = False    # set by Model once the handle has a verifier bank (split calls skip the banks)
         # the three session callables of the reference (utils.py:87,93), numpy in / numpy out
         self.melspec_model_predict = self._melspec_model_predict
@@ -126,10 +136,12 @@ class AudioFeatures:
             self._pending = np.zeros((self.n_streams, 0), np.int16)
             self._rpend = None
             self.accumulated_samples = 0
+            self._held_in_raw[:] = False
         else:
             buf, lens = self._ragged_pending()
             lens[np.asarray(stream_ids, np.int64)] = 0
             self._set_ragged_pending(buf, lens)
+            self._held_in_raw[np.asarray(stream_ids, np.int64)] = False
 
     # ---- per-stream remainders: `_pending` [B, L] while every stream holds the same number of samples, else
     #      `_rpend` = (int16 [B, 1279], lengths [B]) ----
@@ -273,6 +285,7 @@ class AudioFeatures:
         else:
             self._pending = buf.copy()
             self.accumulated_samples = total
+            self._held_in_raw[:] = True
             return total, 0
         n_chunks = ready.shape[1] // CHUNK
         if scores_out is None:
@@ -299,6 +312,7 @@ class AudioFeatures:
                 if self._verifier_banks:
                     self.ctx.enable_verifiers(True)
         self.accumulated_samples = 0
+        self._held_in_raw[:] = False
         self._last_scores = scores_out
         return ready.shape[1], n_chunks
 
@@ -343,6 +357,7 @@ class AudioFeatures:
             if split and self._verifier_banks:
                 self.ctx.enable_verifiers(True)
         self._set_ragged_pending(new_buf, new_lens)
+        self._held_in_raw = n_chunks == 0
         n_prepared = np.where(n_chunks > 0, n_chunks * CHUNK, tot)
         return n_prepared, n_chunks, split
 
@@ -376,6 +391,32 @@ class AudioFeatures:
     def melspectrogram_buffer(self):
         self._ensure_streams()
         return self.ctx.get_mel(0, 76)
+
+    @property
+    def raw_data_buffer(self):
+        """What the reference's ``raw_data_buffer`` holds for stream 0 (utils.py:164,403-430), as a
+        ``deque(maxlen=H)`` of ints, H = the audio history in samples: the samples the stream stepped, from the device,
+        followed by the samples it holds not yet stepped when its last call stepped nothing (the reference buffers
+        those at once, but not a remainder left over after a step).  Needs ``audio_history``; reads the device."""
+        H = self.audio_history_samples
+        if not H:
+            raise AttributeError("raw_data_buffer needs the audio history on the device: construct AudioFeatures (or "
+                                 "Model) with audio_history=<seconds>, e.g. audio_history=10 as the reference keeps")
+        self._ensure_streams()
+        audio, pos = self.ctx.audio_state([0])
+        x = audio[0, H - int(min(pos[0], H)):]
+        if self._held_in_raw[0]:
+            buf, lens = self._ragged_pending()
+            x = np.concatenate((x, buf[0, :lens[0]]))[-H:]
+        return deque(x.tolist(), maxlen=H)
+
+
+def audio_history_samples(seconds):
+    """audio_history in seconds -> samples (a multiple of 1280, up to 60 s); ValueError otherwise"""
+    n = int(round(float(seconds) * 16000))
+    if n < 0 or n % CHUNK or n > 60 * 16000 or abs(n - float(seconds) * 16000) > 1e-6 * max(n, 1):
+        raise ValueError(f"audio_history={seconds}: seconds in whole 80 ms chunks (a multiple of 0.08), at most 60")
+    return n
 
 
 def _take_rows(dst, src, rows, maximum):

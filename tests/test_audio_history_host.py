@@ -1,0 +1,269 @@
+"""Stream audio without a GPU: ``AudioFeatures.raw_data_buffer`` against the reference's own deque (the fixture
+tests/golden/raw_buffer.npz, recorded by make_raw_buffer_golden.py from the unmodified reference), on the lockstep and
+the ragged accumulation paths, and the host-side rules of the audio calls (ValueError / AttributeError), on a stand-in
+of the C ABI whose audio history is a NumPy ring with the semantics of include/owwb200.h (oww_set_audio_history)."""
+import os
+
+import numpy as np
+import pytest
+import torch
+
+import fake_backend
+from openwakeword_b200 import _native
+from openwakeword_b200.utils import AudioFeatures, audio_history_samples
+from test_detect_host import DetectFakeContext, _model
+from helpers import emb_weights
+
+GOLDEN = os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden", "raw_buffer.npz")
+
+
+class _AudioRing:
+    """The audio calls of _native.Context on a NumPy ring: ring [B, H], pos [B]; every step appends what it steps."""
+    audio_history = 0
+
+    def set_audio_history(self, n):
+        if n < 0 or n % 1280 or n > 960000:
+            raise _native.NativeError("n_samples")
+        self.audio_history = n
+        self._alloc_ring()
+
+    def _alloc_ring(self):
+        B = getattr(self, "_n", 0)
+        self.ring = np.zeros((B, self.audio_history), np.int16)
+        self.pos = np.zeros(B, np.int64)
+
+    def set_streams(self, n):
+        super().set_streams(n)
+        self._alloc_ring()
+
+    def reset(self, stream_ids=None, feature_init=None):
+        super().reset(stream_ids, feature_init)
+        if self.audio_history:
+            self.pos[slice(None) if stream_ids is None else np.asarray(stream_ids, np.int64)] = 0
+
+    def _append(self, b, x):
+        H = self.audio_history
+        if not H:
+            return
+        p = self.pos[b] + np.arange(x.size)
+        self.ring[b, p % H] = x
+        self.pos[b] += x.size
+
+    def _window(self, b, e, n):
+        H, p = self.audio_history, self.pos[b]
+        q = np.arange(e - n, e)
+        ok = (q >= max(p - H, 0)) & (q < p)
+        out = np.zeros(n, np.int16)
+        out[ok] = self.ring[b, q[ok] % H]
+        return out
+
+    def step_host(self, pcm, n_chunks, scores_out):
+        for b in range(self._n):
+            self._append(b, pcm[b, :n_chunks * 1280])
+        self._step_host(pcm, n_chunks, scores_out)
+
+    def step_host_ragged(self, pcm, chunks, scores_out):
+        for b in range(self._n):
+            self._append(b, pcm[b, :int(chunks[b]) * 1280])
+        self._step_host_ragged(pcm, chunks, scores_out)
+
+    def _need(self):
+        if not self.audio_history:
+            raise _native.NativeError("no audio history")
+
+    def audio_state(self, stream_ids):
+        self._need()
+        H = self.audio_history
+        ids = np.asarray(stream_ids, np.int64)
+        return np.stack([self._window(b, self.pos[b], H) for b in ids]).reshape(ids.size, H), self.pos[ids].copy()
+
+    def set_audio_state(self, stream_ids, audio, pos):
+        self._need()
+        ids = np.asarray(stream_ids, np.int64)
+        if len(set(ids.tolist())) != ids.size:
+            raise _native.NativeError("duplicate ids")
+        audio = np.asarray(audio, np.int16)
+        if audio.shape != (ids.size, self.audio_history):
+            raise ValueError("audio shape")
+        H = self.audio_history
+        for i, b in enumerate(ids):
+            p = max(int(pos[i]), 0)
+            self.ring[b, (p + np.arange(H)) % H] = audio[i]
+            self.pos[b] = p
+
+    def read_audio(self, stream_ids, n_samples, ends=None):
+        self._need()
+        ids = np.asarray(stream_ids, np.int64).ravel()
+        e = [self.pos[b] if ends is None or ends[i] < 0 else ends[i] for i, b in enumerate(ids)]
+        out = np.stack([self._window(b, e[i], n_samples) for i, b in enumerate(ids)]) if ids.size else \
+            np.zeros((0, n_samples), np.int16)
+        return torch.from_numpy(out), torch.from_numpy(self.pos[ids].copy())
+
+    def detect_capture(self, d_scores, prepared, n_samples, max_events=None):
+        self._need()
+        events, n = self.detect_events(d_scores, prepared, None, max_events)
+        clips = np.stack([self._window(b, self.pos[b], n_samples) for b in events["stream"]]) if len(events) else \
+            np.zeros((0, n_samples), np.int16)
+        return events, n, torch.from_numpy(clips), self.pos[events["stream"]].copy()
+
+
+class AudioOnlyContext(_AudioRing, fake_backend.FakeContext):
+    """Steps record the audio and nothing else (no features, no scores)."""
+
+    def _step_host(self, pcm, n_chunks, scores_out):
+        pass
+
+    def _step_host_ragged(self, pcm, chunks, scores_out):
+        pass
+
+
+class AudioDetectContext(_AudioRing, DetectFakeContext):
+    """DetectFakeContext (the oracle behind every step and detection) with the audio ring."""
+
+    def _step_host(self, pcm, n_chunks, scores_out):
+        DetectFakeContext.step_host(self, pcm, n_chunks, scores_out)
+
+    def _step_host_ragged(self, pcm, chunks, scores_out):
+        DetectFakeContext.step_host_ragged(self, pcm, chunks, scores_out)
+
+
+@pytest.fixture
+def audio_only(monkeypatch):
+    monkeypatch.setattr(_native, "Context", AudioOnlyContext)
+    yield
+
+
+@pytest.fixture
+def audio_detect(monkeypatch):
+    monkeypatch.setattr(_native, "Context", AudioDetectContext)
+    yield
+
+
+def _features(n_streams=1, seconds=10.0):
+    return AudioFeatures(embedding_model_path=emb_weights(), n_streams=n_streams,
+                         feature_init=np.zeros((41, 96), np.float32), audio_history=seconds)
+
+
+def _expected(z, k):
+    return z["signal"][z["raw_lo"][k]:z["raw_hi"][k]]
+
+
+def test_raw_data_buffer_matches_the_reference_lockstep(audio_only):
+    z = np.load(GOLDEN)
+    af = _features()
+    off = 0
+    for k, c in enumerate(z["calls"]):
+        if c < 0:
+            af.reset()
+        else:
+            assert af(z["signal"][off:off + c]) == z["ret"][k], k
+            off += c
+        buf = af.raw_data_buffer
+        assert buf.maxlen == 160000
+        assert np.array_equal(np.array(buf, np.int16), _expected(z, k)), k
+        assert all(type(v) is int for v in list(buf)[:3])
+
+
+def test_raw_data_buffer_matches_the_reference_ragged(audio_only):
+    """Stream 0 gets the fixture's calls while stream 1 gets other lengths, so the streams hold different remainders
+    and the per-stream accumulation (with its per-stream flag) runs throughout."""
+    z = np.load(GOLDEN)
+    af = _features(n_streams=2)
+    rng = np.random.default_rng(3)
+    scores = np.zeros((2, 1), np.float32)
+    off = 0
+    for k, c in enumerate(z["calls"]):
+        if c < 0:
+            af.reset(stream_ids=[0])
+        else:
+            other = rng.integers(-2000, 2000, int(rng.integers(0, 3000))).astype(np.int16)
+            n_prep = af._streaming_features_ragged([z["signal"][off:off + c], other], scores)[0]
+            assert n_prep[0] == z["ret"][k], k
+            off += c
+        assert np.array_equal(np.array(af.raw_data_buffer, np.int16), _expected(z, k)), k
+
+
+def test_raw_data_buffer_shorter_history_keeps_the_last_samples(audio_only):
+    af = _features(seconds=0.16)
+    x = np.arange(5000, dtype=np.int16)
+    af(x)                                       # steps 3840, holds 1160 (a remainder: not in the buffer)
+    assert np.array_equal(np.array(af.raw_data_buffer, np.int16), x[3840 - 2560:3840])
+    af(x[:100])                                 # steps nothing: 1260 held, all in the reference's buffer
+    assert np.array_equal(np.array(af.raw_data_buffer, np.int16), np.concatenate((x, x[:100]))[-2560:])
+
+
+def test_audio_history_rules(audio_only):
+    af = _features(seconds=0.0)
+    with pytest.raises(AttributeError, match="audio_history"):
+        af.raw_data_buffer
+    assert not hasattr(af, "raw_data_buffer")
+    for bad in (0.05, -0.08, 60.08, 1.0001):
+        with pytest.raises(ValueError, match="audio_history"):
+            _features(seconds=bad)
+    assert audio_history_samples(10) == 160000 and audio_history_samples(0.08) == 1280
+    assert audio_history_samples(60) == 960000
+
+
+def _mk(B, seconds, **kw):
+    m = _model(B, np.zeros((41, 96), np.float32), audio_history=seconds, **kw)
+    m.preprocessor._ensure_streams()
+    return m
+
+
+def _feed(m, host, xs, call):
+    """call(xs) on Model m; host[b] += the samples stream b stepped in it"""
+    held, lens0 = m.preprocessor._ragged_pending()
+    out = call(xs)
+    lens = m.preprocessor._ragged_pending()[1]
+    for b in range(len(host)):
+        allx = np.concatenate((held[b, :lens0[b]], xs[b]))
+        host[b] = np.concatenate((host[b], allx[:allx.size - lens[b]]))
+    return out
+
+
+def test_model_get_audio_and_capture_on_the_stand_in(audio_detect):
+    B = 3
+    m = _mk(B, 0.32)
+    rng = np.random.default_rng(5)
+    host = [np.zeros(0, np.int16) for _ in range(B)]
+    for _ in range(4):
+        xs = [rng.integers(-3000, 3000, int(rng.integers(0, 4000))).astype(np.int16) for _ in range(B)]
+        _feed(m, host, xs, m.predict_ragged)
+    clips, ends = m.get_audio([2, 0, 2], 0.08)
+    for i, b in enumerate([2, 0, 2]):
+        assert ends[i] == host[b].size
+        want = host[b][-1280:]
+        assert np.array_equal(clips[i, 1280 - want.size:], want)
+    clips, ends = m.get_audio([1], 0.16, end=host[1].size + 1280)        # post-roll not stepped yet: zeros
+    assert ends[0] == host[1].size + 1280 and not clips[0, 1280:].any()
+    assert np.array_equal(clips[0, :1280], host[1][-1280:])
+    xs = [rng.integers(-3000, 3000, 1280).astype(np.int16) for _ in range(B)]
+    ev = _feed(m, host, xs, lambda x: m.detect_ragged(x, threshold=0.0, capture=0.08))
+    assert ev and all(len(e) == 5 for e in ev)
+    for s, lab, sc, clip, end in ev:
+        assert end == host[s].size and clip.dtype == np.int16 and np.array_equal(clip, host[s][-1280:])
+    assert all(len(e) == 3 for e in m.detect(np.zeros((B, 1280), np.int16), threshold=0.0))
+
+
+def test_model_audio_refusals(audio_detect):
+    on, off, other = _mk(2, 0.16), _mk(2, 0.0), _mk(2, 0.32)
+    with pytest.raises(ValueError, match="audio_history"):
+        off.get_audio([0], 0.08)
+    with pytest.raises(ValueError, match="audio_history"):
+        off.detect(np.zeros((2, 1280), np.int16), threshold=0.5, capture=0.08)
+    with pytest.raises(ValueError, match="outside"):
+        on.get_audio([0], 0.32)                     # longer than the history
+    with pytest.raises(ValueError):
+        on.get_audio([2], 0.08)                     # no such stream
+    st_on, st_off = on.export_streams([0]), off.export_streams([0])
+    assert st_off.audio is None and st_on.audio[0].shape == (1, 2560)
+    for dst, st in ((off, st_on), (on, st_off), (other, st_on)):
+        with pytest.raises(ValueError, match="audio history"):
+            dst.import_streams([1], st)
+    on.predict(np.arange(2 * 2000, dtype=np.int16).reshape(2, 2000) % 700)
+    on2 = _mk(2, 0.16)
+    on2.import_streams([1], on.export_streams([0]))
+    assert np.array_equal(on2.get_audio([1], 0.16)[0], on.get_audio([0], 0.16)[0])
+    assert on2.get_audio([1], 0.16)[1][0] == 1280
+    on.reset_streams([0])
+    assert on.get_audio([0], 0.08)[1][0] == 0 and not on.get_audio([0], 0.08)[0].any()
