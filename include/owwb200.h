@@ -401,6 +401,72 @@ int oww_audio_export(oww_ctx* ctx, const int32_t* h_stream_ids, int n, int16_t* 
 int oww_audio_import(oww_ctx* ctx, const int32_t* h_stream_ids, int n, const int16_t* d_audio, const int64_t* d_pos,
                      void* stream);
 
+/* ---- ingest: every stream's packets at its own sample rate (the reference's server example resamples each packet on
+ *      the host before Model.predict, examples/web/streaming_server.py:54-60, and AudioFeatures keeps the remainder
+ *      below a chunk on the host, openwakeword/utils.py:409-430) -------------------------------------------------------
+ * Rates: r in {8000, 11025, 12000, 16000, 22050, 24000, 32000, 44100, 48000}; with g = gcd(16000, r), up = 16000/g and
+ * down = r/g.  16000 is the identity (a copy).  For the other rates the filter is scipy's resample_poly design: mr =
+ * max(up, down), half = 10*mr, N = 2*half + 1, h[k] = sinc((k - half)/mr) * kaiser(N, beta 5)[k] for k < N, normalised to
+ * sum 1 and multiplied by up; computed in double on the host and rounded once to fp32.  A phase has at most 61 taps.
+ * Stream b's 16 kHz output is y = upfirdn(h, x, up, down) of its input x since its restart (causal: 0.6 - 1.3 ms of
+ * delay).  After S input samples the first A(S) = ceil(S*up/down) outputs depend on no later input: those are final and
+ * are staged.  An 80 ms packet at any rate of the table therefore yields exactly 1280 samples.  Each output is one fp32
+ * sum over its phase's taps in a fixed order (newest input sample first), so the 16 kHz samples are the same bits whatever the
+ * packet split; it is converted to int16 by round-half-even with saturation (sum |h| of a phase reaches 2.24, so
+ * full-scale input can overshoot).
+ * Per stream the handle keeps the rate, the last 128 input samples (the filter history), and a staging row of the 16 kHz
+ * samples not yet stepped; its capacity is C = max_chunks*1280 + 1279 samples (8192 streams at max_chunks 2: 63 MB).
+ * The input count S, the staged count and the rate live on the host, so no call reads the device.  Nothing is allocated
+ * and nothing is launched for ingest until the first oww_set_input_rates.
+ *   oww_set_input_rates - stream h_stream_ids[i] (NULL: all streams, n = the stream count) takes input at h_rates[i]
+ *                       from the next oww_ingest on; its resampler restarts (history zero, S = 0), its staged samples are
+ *                       kept.  The first call allocates the state (every other stream at 16000) and synchronises the
+ *                       device; later calls enqueue nothing.  OWW_EINVAL: a rate outside the table, an id out of range.
+ *   oww_ingest        - stream b's new samples are d_in[h_offsets[b] .. h_offsets[b+1]) (int16 at its rate; host int64
+ *                       offsets, n_streams + 1 entries, non-decreasing, first >= 0; a stream may get none).  One launch
+ *                       resamples every stream and writes its new final samples behind its staged ones; then the
+ *                       staged samples step as oww_step_ragged steps them: stream b steps chunks[b] = floor(staged / 1280)
+ *                       chunks, d_scores rows as oww_step_ragged writes them (held rows are not written), with the audio
+ *                       history, detector inputs, verifiers and head banks of that call.  The rest (< 1280 samples) stays
+ *                       staged.  h_chunks_out[b] (may be NULL) <- chunks[b]; h_prepared_out[b] (may be NULL) <- what
+ *                       AudioFeatures.__call__ returns: chunks[b]*1280, or the staged count when the stream stepped
+ *                       nothing - oww_detect's h_prepared.  Both are filled on the host before the call returns, with no
+ *                       synchronisation.  The per-stream table is staged through a ring of four pinned buffers (a call
+ *                       waits, host side, for the copy of the call four back).  OWW_EINVAL before anything is enqueued:
+ *                       no ingest state, bad offsets, a NULL d_in with samples or a NULL d_scores, or a stream whose
+ *                       staged plus new samples would exceed C (oww_ingest_capacity gives the limit).
+ *   oww_ingest_capacity - pure host: h_max_in[b] (int64 [n_streams]) <- the most input samples stream b's next
+ *                       oww_ingest may take.  A caller splits longer packets with it.
+ *   oww_ingest_plan   - pure host, no handle or GPU: for a stream at `rate` on a handle of max_chunks, that has taken
+ *                       n_before input samples since its restart and holds `staged` samples, an oww_ingest of n_in more
+ *                       samples makes *n_out (may be NULL) new final samples, steps *chunks chunks and leaves *staged_after;
+ *                       *max_in (may be NULL) <- oww_ingest_capacity's limit.  OWW_EINVAL: a rate outside the table, or
+ *                       n_in over that limit (only *max_in is written then).
+ *   oww_resampler_taps - pure host, no handle or GPU: the fp32 taps h (N of them; the first min(N, max) go to h_taps, which
+ *                       may be NULL) and *up, *down the library uses for `rate`.  Returns N (0 at 16000), or OWW_EINVAL
+ *                       outside the table.
+ *   oww_ingest_export / _import - stream h_stream_ids[i] <-> h_rates[i], h_consumed[i] (S, int64), h_staged[i] (host), its
+ *                       staged samples in row i of d_staged [n][staged_stride] int16 (the rest of the row zero on export),
+ *                       and its history in d_hist [n][128] int16 (oldest first).  Export fills the host arrays before
+ *                       it returns; with d_staged and d_hist NULL it enqueues nothing (a query of the staged counts), else
+ *                       staged_stride must hold every exported row.  Import takes rates from the table, h_staged[i] in
+ *                       [0, C], distinct ids; a moved stream continues bit for bit.  Stream-ordered on `stream`.
+ * oww_reset / oww_reset_async clear the staged samples and the history of the streams they reset and keep their rates;
+ * oww_set_streams sets every stream to 16000 with nothing staged.  The steps of oww_step* do not touch the ingest state
+ * (a caller that mixes them on one stream feeds that stream at one place only).                                          */
+int oww_set_input_rates(oww_ctx* ctx, const int32_t* h_stream_ids, int n, const int32_t* h_rates, void* stream);
+int oww_ingest(oww_ctx* ctx, const int16_t* d_in, const int64_t* h_offsets, int32_t* h_chunks_out, int32_t* h_prepared_out,
+               float* d_scores, void* stream);
+int oww_ingest_capacity(oww_ctx* ctx, int64_t* h_max_in);
+int oww_ingest_plan(int rate, int max_chunks, int64_t n_before, int staged, int64_t n_in, int64_t* n_out, int32_t* chunks,
+                    int32_t* staged_after, int64_t* max_in);
+int oww_resampler_taps(int rate, float* h_taps, int max, int* up, int* down);
+int oww_ingest_export(oww_ctx* ctx, const int32_t* h_stream_ids, int n, int32_t* h_rates, int64_t* h_consumed,
+                      int32_t* h_staged, int16_t* d_staged, int64_t staged_stride, int16_t* d_hist, void* stream);
+int oww_ingest_import(oww_ctx* ctx, const int32_t* h_stream_ids, int n, const int32_t* h_rates, const int64_t* h_consumed,
+                      const int32_t* h_staged, const int16_t* d_staged, int64_t staged_stride, const int16_t* d_hist,
+                      void* stream);
+
 /* ---- batch paths --------------------------------------------------------------------------- */
 /* d_pcm [n_clips][n_samples] -> d_emb [n_clips][W][96], W = (T-76)/8+1 (utils.py:322).           */
 int oww_embed_clips(oww_ctx* ctx, const int16_t* d_pcm, int n_clips, int n_samples, float* d_emb, void* stream);

@@ -96,6 +96,14 @@ _SIGNATURES = {
     "oww_capture_events": (C.c_int, [_P, _P, _P, C.c_int, C.c_int, _P, _P, _P]),
     "oww_audio_export": (C.c_int, [_P, _P, C.c_int, _P, _P, _P]),
     "oww_audio_import": (C.c_int, [_P, _P, C.c_int, _P, _P, _P]),
+    "oww_set_input_rates": (C.c_int, [_P, _P, C.c_int, _P, _P]),
+    "oww_ingest": (C.c_int, [_P, _P, _P, _P, _P, _P, _P]),
+    "oww_ingest_capacity": (C.c_int, [_P, _P]),
+    "oww_ingest_plan": (C.c_int, [C.c_int, C.c_int, C.c_int64, C.c_int, C.c_int64, C.POINTER(C.c_int64),
+                                  C.POINTER(C.c_int32), C.POINTER(C.c_int32), C.POINTER(C.c_int64)]),
+    "oww_resampler_taps": (C.c_int, [C.c_int, _P, C.c_int, C.POINTER(C.c_int), C.POINTER(C.c_int)]),
+    "oww_ingest_export": (C.c_int, [_P, _P, C.c_int, _P, _P, _P, _P, C.c_int64, _P, _P]),
+    "oww_ingest_import": (C.c_int, [_P, _P, C.c_int, _P, _P, _P, _P, C.c_int64, _P, _P]),
     "oww_embed_clips": (C.c_int, [_P, _P, C.c_int, C.c_int, _P, _P]),
     "oww_predict_clips": (C.c_int, [_P, _P, C.c_int, C.c_int, C.c_int, _P, C.c_int, _P, _P]),
     "oww_clip_schedule": (C.c_int, [C.c_int, C.c_int64, _P, C.c_int]),
@@ -177,6 +185,35 @@ def clip_slab_plan(steps, ctx=None):
     if n < 0:
         raise NativeError(f"oww_clip_slab_plan failed ({n})")
     return n, done.value, need.value
+
+
+def resampler_taps(rate):
+    """-> (float32 taps, up, down) the library resamples input at `rate` Hz with (no taps at 16000: a copy); ValueError
+    for a rate outside its table (oww_resampler_taps: pure host code, no GPU needed)."""
+    lib = load_library()
+    up, down = C.c_int(0), C.c_int(0)
+    n = lib.oww_resampler_taps(int(rate), None, 0, C.byref(up), C.byref(down))
+    if n < 0:
+        raise ValueError(f"sample rate {rate} Hz is not supported: the input rates are 8000, 11025, 12000, 16000, 22050, "
+                         "24000, 32000, 44100 and 48000 Hz")
+    taps = np.zeros(n, np.float32)
+    if n:
+        lib.oww_resampler_taps(int(rate), _ptr(taps), n, None, None)
+    return taps, up.value, down.value
+
+
+def ingest_plan(rate, max_chunks, n_before, staged, n_in):
+    """What one oww_ingest call does to a stream (oww_ingest_plan: pure host, no GPU) -> (new final samples, chunks
+    stepped, samples left staged, capacity); the first three are None when n_in is over the capacity."""
+    lib = load_library()
+    n_out, chunks, after, max_in = C.c_int64(0), C.c_int32(0), C.c_int32(0), C.c_int64(0)
+    rc = lib.oww_ingest_plan(int(rate), int(max_chunks), int(n_before), int(staged), int(n_in), C.byref(n_out),
+                             C.byref(chunks), C.byref(after), C.byref(max_in))
+    if rc and n_in <= max_in.value:
+        raise ValueError(f"oww_ingest_plan refused rate {rate}")
+    if rc:
+        return None, None, None, max_in.value
+    return n_out.value, chunks.value, after.value, max_in.value
 
 
 def _ptr(a):
@@ -759,6 +796,76 @@ class Context:
         d = torch.from_numpy(a).to(dev)
         p = torch.from_numpy(np.ascontiguousarray(pos, np.int64).reshape(ids.size)).to(dev)
         self.audio_import(ids, d, p, self._current_stream())
+
+    # ---- ingest: packets at any rate (include/owwb200.h, oww_set_input_rates) ----
+    def set_input_rates(self, stream_ids, rates, stream=None):
+        """stream_ids None = all streams (rates then has one entry per stream); their resamplers restart."""
+        ids = None if stream_ids is None else np.ascontiguousarray(stream_ids, np.int32).ravel()
+        r = np.ascontiguousarray(rates, np.int32).ravel()
+        n = r.size if ids is None else ids.size
+        if r.size != n:
+            raise ValueError(f"{r.size} rates for {n} streams")
+        for v in np.unique(r):
+            resampler_taps(int(v))                        # ValueError outside the table
+        self._check(self.lib.oww_set_input_rates(self.h, _ptr(ids), n, _ptr(r), stream))
+
+    def ingest(self, d_in, offsets, d_scores, stream=None):
+        """oww_ingest: stream b's samples are d_in[offsets[b]:offsets[b+1]] (host int64 offsets) -> (chunks, prepared)
+        int32 [n_streams] host arrays."""
+        off = np.ascontiguousarray(offsets, np.int64).ravel()
+        if off.size != self.n_streams + 1:
+            raise ValueError(f"offsets has {off.size} entries, the handle takes {self.n_streams + 1}")
+        chunks = np.zeros(self.n_streams, np.int32)
+        prepared = np.zeros(self.n_streams, np.int32)
+        self._check(self.lib.oww_ingest(self.h, _ptr(d_in), _ptr(off), _ptr(chunks), _ptr(prepared), _ptr(d_scores),
+                                        stream))
+        return chunks, prepared
+
+    def ingest_pcm(self, pcm, offsets, d_scores):
+        """ingest on a host int16 array of packed packets, uploaded and ingested on the current CUDA stream"""
+        import torch
+        x = np.ascontiguousarray(pcm, np.int16).ravel()
+        d = torch.from_numpy(x if x.size else np.zeros(1, np.int16)).to(torch.device("cuda", self.device))
+        return self.ingest(d, offsets, d_scores, self._current_stream())
+
+    def ingest_capacity(self):
+        """-> int64 [n_streams]: the most input samples each stream's next ingest call may take"""
+        out = np.zeros(self.n_streams, np.int64)
+        self._check(self.lib.oww_ingest_capacity(self.h, _ptr(out)))
+        return out
+
+    def ingest_state(self, stream_ids, samples=True):
+        """-> (rates int32 [n], input counts int64 [n], staged counts int32 [n], staged int16 [n, max staged] or None,
+        history int16 [n, 128] or None) of the listed streams; host arrays (synchronises when samples)"""
+        import torch
+        ids = np.ascontiguousarray(stream_ids, np.int32).ravel()
+        rates, S, staged = np.zeros(ids.size, np.int32), np.zeros(ids.size, np.int64), np.zeros(ids.size, np.int32)
+        self._check(self.lib.oww_ingest_export(self.h, _ptr(ids), ids.size, _ptr(rates), _ptr(S), _ptr(staged), None, 0,
+                                               None, None))
+        if not samples:
+            return rates, S, staged, None, None
+        dev = torch.device("cuda", self.device)
+        width = max(int(staged.max(initial=0)), 1)
+        d = torch.empty((ids.size, width), dtype=torch.int16, device=dev)
+        hist = torch.empty((ids.size, 128), dtype=torch.int16, device=dev)
+        if ids.size:
+            self._check(self.lib.oww_ingest_export(self.h, _ptr(ids), ids.size, None, None, None, _ptr(d), width,
+                                                   _ptr(hist), self._current_stream()))
+        return rates, S, staged, d.cpu().numpy(), hist.cpu().numpy()
+
+    def set_ingest_state(self, stream_ids, rates, consumed, staged, samples, hist):
+        """the reverse of ingest_state (distinct ids), on the current CUDA stream"""
+        import torch
+        ids = np.ascontiguousarray(stream_ids, np.int32).ravel()
+        r = np.ascontiguousarray(rates, np.int32).ravel()
+        S = np.ascontiguousarray(consumed, np.int64).ravel()
+        st = np.ascontiguousarray(staged, np.int32).ravel()
+        x = np.ascontiguousarray(samples, np.int16).reshape(ids.size, -1)
+        dev = torch.device("cuda", self.device)
+        d = torch.from_numpy(x).to(dev)
+        h = torch.from_numpy(np.ascontiguousarray(hist, np.int16).reshape(ids.size, 128)).to(dev)
+        self._check(self.lib.oww_ingest_import(self.h, _ptr(ids), ids.size, _ptr(r), _ptr(S), _ptr(st), _ptr(d),
+                                               x.shape[1], _ptr(h), self._current_stream()))
 
     # ---- batch ----
     def embed_clips(self, d_pcm, n_clips, n_samples, d_emb, stream=None):

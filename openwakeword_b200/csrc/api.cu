@@ -256,6 +256,7 @@ void free_streams(oww_ctx* c) {
     oww_verifiers_free_streams(c);
     oww_detect_free_streams(c);
     oww_audio_free_streams(c);
+    oww_ingest_free_streams(c);
     oww_heads_grp_drop_mirror(c);
     for (auto& X : c->late_x) for (auto& b : X.buf) { cudaFree(b); b = nullptr; }
     cudaFree(c->d_late_tmp); c->d_late_tmp = nullptr;
@@ -735,6 +736,7 @@ int reset_enqueue(oww_ctx* ctx, const int32_t* h_stream_ids, int n, const float*
     int rc = oww_detect_reset(ctx, h_stream_ids ? ctx->d_reset_ids : nullptr, n, s);    // the detector's history of those streams
     if (rc) return rc;
     if ((rc = oww_audio_reset(ctx, h_stream_ids ? ctx->d_reset_ids : nullptr, n, s))) return rc;     // ... and their audio
+    oww_ingest_reset(ctx, h_stream_ids, n);               // ... and their staged samples (host counters only)
     return oww_feat16_resync(ctx, h_stream_ids ? ctx->d_reset_ids : nullptr, n, s);     // fp16 mirror of the rings (heads_grp.cu)
 }
 
@@ -879,6 +881,7 @@ void oww_destroy(oww_ctx* ctx) {
     oww_verifier_fit_free(ctx);
     oww_detect_free(ctx);
     oww_audio_free(ctx);
+    oww_ingest_free(ctx);
     cudaFree(ctx->d_window); cudaFree(ctx->d_twiddle); cudaFree(ctx->d_mel_start); cudaFree(ctx->d_mel_len);
     cudaFree(ctx->d_mel_w); cudaFree(ctx->d_emb_blob); cudaFree(ctx->d_tc_w); cudaFree(ctx->d_tc_sb);
     cudaFree(ctx->d_tc_w3); cudaFree(ctx->d_tc_sb3);
@@ -1069,6 +1072,7 @@ int oww_set_streams(oww_ctx* ctx, int n_streams) {
     if ((rc = oww_head_banks_alloc_streams(ctx))) return rc;        // ... and without a bank head
     if ((rc = oww_detect_alloc_streams(ctx))) return rc;            // ... and with an empty detector history
     if ((rc = oww_audio_alloc_streams(ctx))) return rc;             // ... and an empty audio history
+    if ((rc = oww_ingest_alloc_streams(ctx))) return rc;            // ... and at 16 kHz with nothing staged
     return oww_reset(ctx, nullptr, B, nullptr, OWW_INIT_FEATURE_ROWS);
 }
 

@@ -325,6 +325,7 @@ struct oww_ctx {
     int tc_heads_terms = 3;          // 3 = hi*hi + lo*hi + hi*lo (fp32-grade), 1 = plain fp16 operands
     struct oww_detector* det = nullptr;   // detections on the device (detect.cu); nullptr: no detector configured
     struct oww_audio* audio = nullptr;    // the streams' recent audio (audio.cu); nullptr: no history
+    struct oww_ingest_state* ingest = nullptr;  // resampling and staging of packets at any rate (ingest.cu); nullptr: off
 };
 
 int oww_fail(oww_ctx* ctx, int code, const char* fmt, ...);
@@ -547,6 +548,13 @@ int oww_audio_reset(oww_ctx* ctx, const int* d_ids, int n, cudaStream_t s);
 // n_chunks for every stream)
 int oww_audio_append(oww_ctx* ctx, const int16_t* d_pcm, int64_t pcm_stride, int n_chunks, const int* d_counts,
                      cudaStream_t s);
+
+// ---- ingest.cu: packets at any rate (nothing happens on a handle without ingest state) ----
+void oww_ingest_free(oww_ctx* ctx);
+void oww_ingest_free_streams(oww_ctx* ctx);
+int oww_ingest_alloc_streams(oww_ctx* ctx);      // for ctx->n_streams streams, every one at 16000, nothing staged
+// the listed streams (h_ids == nullptr: streams 0..n-1) drop their staged samples and history: host state only
+void oww_ingest_reset(oww_ctx* ctx, const int32_t* h_ids, int n);
 
 // ---- verifier.cu: custom verifier banks ----
 // every bank of the handle on n rows of final scores (one launch; nothing when the handle has no bank).  The window of

@@ -143,6 +143,51 @@ class StreamEngine:
         when `out` is None)."""
         return self.ctx.step_host_ragged_submit(pcm, chunks)
 
+    # ---- ingest: packets at any sample rate (include/owwb200.h, oww_set_input_rates / oww_ingest) ----
+    def set_input_rates(self, rates, stream_ids=None):
+        """Streams stream_ids (None = all; rates then has one entry per stream) take packets at rates[i] Hz (8000, 11025,
+        12000, 16000, 22050, 24000, 32000, 44100 or 48000) from the next ``ingest`` on; their resamplers restart and the
+        16 kHz samples they hold are kept.  The first call allocates the ingest state (every other stream at 16000)."""
+        if stream_ids is None and np.ndim(rates) == 0:
+            rates = np.full(self.n_streams, int(rates), np.int32)
+        elif stream_ids is not None:
+            rates = np.broadcast_to(np.asarray(rates, np.int64), np.shape(np.ravel(stream_ids)))
+        self.ctx.set_input_rates(stream_ids, rates, self._stream(None))
+
+    def ingest_capacity(self):
+        """-> int64 [n_streams]: the most input samples each stream's next ``ingest`` may take"""
+        return self.ctx.ingest_capacity()
+
+    def ingest(self, d_packets, offsets, out=None):
+        """Every stream's new packet, at its own rate, in one packed int16 tensor on the engine's device: stream b's
+        samples are d_packets[offsets[b]:offsets[b+1]] (host ints, n_streams + 1 of them; a stream may get none).  The
+        device resamples them to 16 kHz, steps every stream's whole chunks as ``step_ragged`` does and keeps the rest.
+        The scores go to out (float32 [n_streams, n_cols] on the device; None: ``self.ingest_scores``, a matrix the engine
+        keeps), rows of streams that stepped nothing are not written.  -> (chunks, prepared): int32 [n_streams] host arrays
+        filled without synchronisation; prepared is what ``detect`` takes (chunks*1280, or the samples staged when a
+        stream stepped nothing).  Enqueued on the current CUDA stream.  A packet longer than ``ingest_capacity`` raises
+        NativeError before anything is enqueued.
+        Typical loop:  chunks, prepared = eng.ingest(packets, offsets)
+                       ev, n = eng.detect(eng.ingest_scores, prepared)"""
+        torch = _torch()
+        dev = torch.device("cuda", self.device_index)
+        if not isinstance(d_packets, torch.Tensor) or d_packets.dtype != torch.int16 or d_packets.device != dev \
+                or d_packets.dim() != 1 or not d_packets.is_contiguous():
+            raise _native.ArgumentError(f"d_packets must be a contiguous 1-D int16 tensor on {dev}")
+        off = np.ascontiguousarray(offsets, np.int64).ravel()
+        if off.size != self.n_streams + 1 or (off.size and (off[0] < 0 or off[-1] > d_packets.numel())):
+            raise _native.ArgumentError(f"offsets must hold {self.n_streams + 1} sample offsets into d_packets "
+                                        f"({d_packets.numel()} samples)")
+        if out is None:
+            if getattr(self, "ingest_scores", None) is None or tuple(self.ingest_scores.shape) != (self.n_streams,
+                                                                                                 self.n_cols):
+                self.ingest_scores = torch.full((self.n_streams, self.n_cols), float("nan"), dtype=torch.float32,
+                                                device=dev)
+            out = self.ingest_scores
+        else:
+            self.ctx._cuda("out", out, torch.float32, (self.n_streams, self.n_cols))
+        return self.ctx.ingest(d_packets, off, out, torch.cuda.current_stream(dev).cuda_stream)
+
     # ---- detections on the device (include/owwb200.h, oww_set_detector) ----
     def set_detector(self, labels, threshold, patience={}, debounce_time=0.0):
         """Configure the detector.  labels: one (column, repeats) per label - the score column it reads (-1: always 0.0)

@@ -5,7 +5,9 @@ Same constructor keywords, ``predict`` / ``predict_clip`` / ``reset`` semantics,
 ``preprocessor``) and ``ValueError`` behaviour; the three inference sessions and the buffers between
 them are replaced by one libowwb200 step per call.  Additions: ``n_streams`` independent streams on
 the batch axis (``predict`` then takes ``[n_streams, samples]`` and returns arrays per label),
-``predict_clips`` / ``predict_clips_ragged`` (bulk path over clips of any lengths) and ``feature_init``.
+``predict_clips`` / ``predict_clips_ragged`` (bulk path over clips of any lengths) and ``feature_init``.  ``sr`` (passed
+to ``AudioFeatures``) other than 16000 makes ``predict*`` and ``detect*`` take each stream's audio at its own rate,
+resampled on the device (``set_sample_rates`` changes it); the clip and bulk paths then refuse with ValueError.
 """
 import os
 import time
@@ -89,6 +91,7 @@ class Model:
         # feature pipeline + device context (weights are registered on its handle)
         self.preprocessor = AudioFeatures(inference_framework=inference_framework, **kwargs)
         self.n_streams = self.preprocessor.n_streams
+        self._check_speex_rates()
         ctx = self.preprocessor.ctx
 
         self._columns = {}     # model name -> (col0, n_out)
@@ -562,9 +565,10 @@ class Model:
         audio = None
         if pre.audio_history_samples:
             audio = pre.ctx.audio_state(ids) + (pre._held_in_raw[ids].copy(),)
+        ingest = pre.ctx.ingest_state(ids) if pre.ingest else None
         return StreamState(records, key, labels, [buf[b, :lens[b]].copy() for b in ids],
                            {lab: self._h(lab)[0][:, ids].copy() for lab in labels},
-                           {lab: self._h(lab)[1][ids].copy() for lab in labels}, audio)
+                           {lab: self._h(lab)[1][ids].copy() for lab in labels}, audio, ingest)
 
     def import_streams(self, stream_ids, state):
         """Streams stream_ids (distinct) become the streams `state` was exported from: device state, samples not yet
@@ -588,7 +592,15 @@ class Model:
         if h_state != pre.audio_history_samples:
             raise ValueError(f"the streams were exported with an audio history of {h_state} samples, this Model keeps "
                              f"{pre.audio_history_samples}")
+        if (state.ingest is not None) != pre.ingest:
+            raise ValueError("the streams were exported from a Model " + ("with" if state.ingest is not None else "without")
+                             + " device ingest (sr=...), this Model " + ("has it" if pre.ingest else "has not"))
+        if self.speex_ns is not None and state.ingest is not None and (state.ingest[0] != 16000).any():
+            self._check_speex_rates(state.ingest[0])
         pre.ctx.import_records(ids, state.records)
+        if state.ingest is not None:
+            pre.ctx.set_ingest_state(ids, *state.ingest)
+            pre.sample_rates[ids] = state.ingest[0]
         if state.audio is not None:
             pre.ctx.set_audio_state(ids, state.audio[0], state.audio[1])
             pre._held_in_raw[ids] = state.audio[2]
@@ -640,6 +652,30 @@ class Model:
         p1 = self._head_predict(hid, n_in, 1, x)[0]
         p2 = self._head_predict(vid, n_in, 1, x)[0]
         return [np.where(p1 > np.float32(thr), p2, p1).astype(np.float32)]
+
+    # ---- audio at other sample rates (AudioFeatures(sr=...), include/owwb200.h, oww_ingest) ----
+    def set_sample_rates(self, stream_ids, rates):
+        """Streams stream_ids take audio at rates[i] (one int for all, or one per id; a rate of the library's table) from
+        the next call on; their resamplers restart, the 16 kHz samples they hold are kept.  ValueError on a Model built
+        without device ingest (sr=16000, the default)."""
+        if not self.preprocessor.ingest:
+            raise ValueError("set_sample_rates needs device ingest: construct the Model with sr=<rate> or "
+                             "sr=[one rate per stream]")
+        if self.speex_ns is not None and (np.asarray(rates) != 16000).any():
+            self._check_speex_rates(np.asarray(rates))
+        self.preprocessor.set_sample_rates(stream_ids, rates)
+
+    def _check_speex_rates(self, rates=None):
+        pre = self.preprocessor
+        rates = pre.sample_rates if rates is None else rates
+        if self.speex_ns is not None and pre.ingest and (rates != 16000).any():
+            raise ValueError("Speex noise suppression runs on 16 kHz audio only; it cannot be combined with streams at "
+                             "other sample rates")
+
+    def _no_ingest(self, what):
+        if self.preprocessor.ingest:
+            raise ValueError(f"{what} takes 16 kHz clips; this Model takes streams at other sample rates (sr=...), "
+                             "which the clip and bulk paths do not")
 
     def _suppress_noise_with_speex(self, x, frame_size=160):
         cleaned = [self.speex_ns.process(x[i:i + frame_size].tobytes()) for i in range(0, x.shape[0], frame_size)]
@@ -788,9 +824,13 @@ class Model:
         lockstep = isinstance(xs, np.ndarray) and not pre.pending_ragged      # as predict: one length, one remainder
         if not lockstep:
             xs = list(xs)
-        held = pre._pending.shape[1] if not pre.pending_ragged else pre._ragged_pending()[1]
-        if (self._vbanks or self._svbanks) and \
-                ((held + np.array([a.shape[0] for a in xs], np.int64)) // CHUNK > pre.max_chunks).any():
+        n_in = np.array([a.shape[0] for a in xs], np.int64)
+        if pre.ingest:                  # more than one ingest call
+            too_long = (self._vbanks or self._svbanks) and (n_in > ctx.ingest_capacity()).any()
+        else:
+            held = pre._pending.shape[1] if not pre.pending_ragged else pre._ragged_pending()[1]
+            too_long = (self._vbanks or self._svbanks) and ((held + n_in) // CHUNK > pre.max_chunks).any()
+        if too_long:
             raise ValueError(f"detect: a stream prepares more than max_chunks={pre.max_chunks} chunks in this call while "
                              "custom verifiers are loaded; construct the Model with a larger max_chunks, or use predict")
         config = (table, float(debounce_time))
@@ -931,6 +971,7 @@ class Model:
             raise ValueError("clip must be a WAV path or a numpy array")
         if self.n_streams != 1:
             raise ValueError("predict_clip is single-stream; use predict_clips for batches")
+        self._no_ingest("predict_clip")
         if padding:
             z = np.zeros(16000 * padding).astype(np.int16)
             data = np.concatenate((z, data, z))
@@ -945,6 +986,7 @@ class Model:
             raise ValueError("return_type must be 'features' or 'audio'")
         if self.n_streams != 1:
             raise ValueError("_get_positive_prediction_frames is single-stream")
+        self._no_ingest("_get_positive_prediction_frames")
         data = _read_wav(file)
         hits = defaultdict(list)
         for i in range(0, data.shape[0] - CHUNK, CHUNK):
@@ -966,6 +1008,7 @@ class Model:
         call) of {label: float}, i.e. what predict_clip(clip, padding, chunk_size) would return for each clip after
         reset(feature_init).  streams (N stream ids, or None: stream 0's models and verifiers): clip i is predicted as
         stream streams[i] would predict it, with its stream models and device verifiers."""
+        self._no_ingest("predict_clips")
         torch = _torch()
         if streams is None and chunk_size == CHUNK and (isinstance(clips, torch.Tensor)
                                                         or (isinstance(clips, np.ndarray) and clips.ndim == 2)):
@@ -988,6 +1031,7 @@ class Model:
         One oww_predict_clips_ragged call; the host fills the rows of calls that stepped no chunk as Model.predict does
         (the previous prediction of single-output heads, zeros for multi-class heads, re-verified), then zeroes each
         clip's first 5 calls (model.py:330-333).  Vectorised over rows."""
+        self._no_ingest("the bulk clip path (predict_clips_ragged, bulk_predict)")
         if self._host_verifiers:
             warnings.warn(f"custom verifiers of {sorted(self._host_verifiers)} are not device-runnable (only the linear "
                           "pipeline of train_verifier_model is): predict_clips returns their models' unverified scores",
@@ -1082,6 +1126,7 @@ class Model:
         {label: stacked array} of what produced a score >= threshold."""
         if return_type not in ("features", "audio"):
             raise ValueError("return_type must be 'features' or 'audio'")
+        self._no_ingest("_get_positive_prediction_frames")
         pcm, offsets = _concat_clips(pcms)
         scores, row_off, labels, emb, step_off, fi = self._predict_ragged(pcm, offsets, 0, CHUNK, None,
                                                                           want_features=return_type == "features")
@@ -1116,6 +1161,7 @@ class Model:
     def predict_clips_array(self, clips, padding=1, feature_init=None):
         """-> (float32 [N, steps, n_labels], labels) with the first-5-steps zeroing of model.py:330-333 applied.
         Device verifiers apply (stream 0's); host-only verifiers do not, and a warning says so."""
+        self._no_ingest("predict_clips_array")
         if self._host_verifiers:
             warnings.warn(f"custom verifiers of {sorted(self._host_verifiers)} are not device-runnable (only the linear "
                           "pipeline of train_verifier_model is): predict_clips returns their models' unverified scores",
@@ -1159,19 +1205,22 @@ class StreamState:
     stream what the host keeps: ``pending`` (int16 samples not yet stepped), ``history`` / ``counts`` ({label: float32
     [30, n] prediction ring, int64 [n] predictions appended}), ``audio`` (None without an audio history, else the
     history: int16 [n, H] oldest first, int64 [n] sample positions, bool [n] whether the samples held not yet stepped
-    count in ``raw_data_buffer``).  ``to(device)`` moves the records; on the CPU it pickles."""
+    count in ``raw_data_buffer``), ``ingest`` (None without device ingest, else the resampler state: int32 [n] rates, int64
+    [n] input samples since each resampler's restart, int32 [n] staged counts, int16 [n, max staged] staged 16 kHz samples,
+    int16 [n, 128] filter histories).  ``to(device)`` moves the records; on the CPU it pickles."""
 
-    def __init__(self, records, key, labels, pending, history, counts, audio=None):
+    def __init__(self, records, key, labels, pending, history, counts, audio=None, ingest=None):
         self.records, self.key, self.labels = records, int(key), list(labels)
         self.pending, self.history, self.counts = pending, history, counts
         self.audio = audio
+        self.ingest = ingest
 
     def __len__(self):
         return len(self.pending)
 
     def to(self, device):
         return StreamState(self.records.to(device), self.key, self.labels, self.pending, self.history, self.counts,
-                           self.audio)
+                           self.audio, self.ingest)
 
 
 def _concat_clips(clips):

@@ -72,6 +72,12 @@ class AudioFeatures:
     does), ``max_chunks`` (largest multiple of 1280 samples one call may carry), ``cnn_mode``, ``audio_history``
     (seconds, a multiple of 0.08; 0 = off): the last samples every stream stepped are kept on the device
     (include/owwb200.h, oww_set_audio_history) and ``raw_data_buffer`` reads them as the reference's deque.
+
+    ``sr``, the reference's keyword ("The sample rate of the audio"): 16000 (the default) keeps the host-side chunk
+    accumulation.  Any other rate of the library's table (8000, 11025, 12000, 22050, 24000, 32000, 44100, 48000), or a
+    sequence of n_streams rates, turns on device ingest for every stream of the handle (include/owwb200.h, oww_ingest):
+    calls take each stream's audio at its own rate, the device resamples it to 16 kHz and keeps the samples below a chunk
+    there.  Features, scores and the audio history are then those of the 16 kHz samples the resampler makes final.
     """
 
     def __init__(self, melspec_model_path="", embedding_model_path="", sr=16000, ncpu=1,
@@ -80,8 +86,9 @@ class AudioFeatures:
                  audio_history=0.0):
         if inference_framework != "b200":
             raise ValueError(f"openwakeword_b200 only provides inference_framework='b200' (got '{inference_framework}')")
-        if sr != 16000:
-            raise ValueError("only 16 kHz audio is supported")
+        self.n_streams = int(n_streams)
+        self.sample_rates = input_rates(sr, self.n_streams)    # None: 16 kHz on the host-side path
+        self.ingest = self.sample_rates is not None
         self.audio_history_samples = audio_history_samples(audio_history)
         self.ctx = _native.Context(device=device_index, max_chunks=max_chunks, cnn_mode=cnn_mode,
                                    window_batch=window_batch, split_from=split_from)
@@ -96,7 +103,6 @@ class AudioFeatures:
         self.ctx.load_embedding(_weights.pack_embedding_blob(self.embedding_weights))
         if self.audio_history_samples:
             self.ctx.set_audio_history(self.audio_history_samples)
-        self.n_streams = int(n_streams)
         self.cnn_mode = cnn_mode
         self.max_chunks = max_chunks
         self.device_index = device_index
@@ -118,15 +124,32 @@ class AudioFeatures:
     # ---- lazily allocate the stream state (heads must be registered on ctx first) ----
     def _ensure_streams(self):
         if not self._streams_ready:
-            self.ctx.set_streams(self.n_streams)
-            self._streams_ready = True
+            self._set_streams()
             self.reset()
+
+    def _set_streams(self):
+        self.ctx.set_streams(self.n_streams)
+        if self.ingest:
+            self.ctx.set_input_rates(None, self.sample_rates)
+        self._streams_ready = True
+
+    def set_sample_rates(self, stream_ids, rates):
+        """Streams stream_ids take audio at rates[i] (one int for all, or one per id) from the next call on; their
+        resamplers restart and the 16 kHz samples they hold are kept.  Needs device ingest (``sr`` other than 16000)."""
+        if not self.ingest:
+            raise ValueError("set_sample_rates needs device ingest: construct with sr=<rate> or sr=[one rate per stream]")
+        self._ensure_streams()
+        ids = np.asarray(stream_ids, np.int64).ravel()
+        if ids.size and (ids.min() < 0 or ids.max() >= self.n_streams):
+            raise ValueError(f"stream ids must lie in [0, {self.n_streams})")
+        r = np.broadcast_to(np.asarray(rates, np.int64), ids.shape).astype(np.int32)
+        self.ctx.set_input_rates(ids.astype(np.int32), r)
+        self.sample_rates[ids] = r
 
     def reset(self, feature_init=None, stream_ids=None):
         """Reset buffers (utils.py:172-178).  ``feature_init`` overrides the ring content."""
         if not self._streams_ready:
-            self.ctx.set_streams(self.n_streams)
-            self._streams_ready = True
+            self._set_streams()
         fi = feature_init if feature_init is not None else self._feature_init
         if fi is None:
             noise = np.random.randint(-1000, 1000, 16000 * 4).astype(np.int16)
@@ -163,8 +186,8 @@ class AudioFeatures:
     @property
     def pending_ragged(self):
         """True while the streams hold different numbers of not yet stepped samples (lockstep input then runs through
-        the ragged path)."""
-        return self._rpend is not None
+        the ragged path).  Always true with device ingest, whose calls are per stream."""
+        return self._rpend is not None or self.ingest
 
     # ---- session-shaped calls ----
     def _melspec_model_predict(self, x):
@@ -272,6 +295,10 @@ class AudioFeatures:
         step = self.ctx.step_pcm if device else self.ctx.step_host
         if scores_out is None:
             scores_out = np.empty((self.n_streams, max(self.ctx.n_outputs, 1)), np.float32)
+        if self.ingest:                     # device ingest: per stream, at its rate
+            n_prepared, n_chunks, _ = self._ingest_features(list(x), scores_out, device)
+            self._last_scores = scores_out
+            return n_prepared, n_chunks
         if self._rpend is not None:         # the streams hold different remainders: per-stream accumulation
             n_prepared, n_chunks, _ = self._streaming_features_ragged(list(x), scores_out, device)
             self._last_scores = scores_out
@@ -325,6 +352,8 @@ class AudioFeatures:
         the verifier banks (the caller verifies the max over all chunk windows).  device: scores_out is a device score
         matrix (Context.new_scores) and the steps run on the current CUDA stream without a copy back."""
         self._ensure_streams()
+        if self.ingest:
+            return self._ingest_features(xs, scores_out, device)
         B = self.n_streams
         step = self.ctx.step_ragged_pcm if device else self.ctx.step_host_ragged
         buf, lens = self._ragged_pending()
@@ -360,6 +389,58 @@ class AudioFeatures:
         self._held_in_raw = n_chunks == 0
         n_prepared = np.where(n_chunks > 0, n_chunks * CHUNK, tot)
         return n_prepared, n_chunks, split
+
+    def _ingest_features(self, xs, scores_out, device=False):
+        """_streaming_features_ragged with device ingest: stream b's xs[b] is audio at its own rate.  One oww_ingest call
+        when every stream's audio fits its capacity (oww_ingest_capacity), else as many as needed, each taking what fits;
+        then, as on the host path, per stream the max over the parts and the verifier banks off for all of them (split).
+        Returns (n_prepared [B], n_chunks [B], split) as _streaming_features_ragged does."""
+        B = self.n_streams
+        xs = [np.asarray(x).astype(np.int16, copy=False).ravel() for x in xs]
+        lens = np.array([x.size for x in xs], np.int64)
+        if getattr(self, "_d_ingest_scores", None) is None:
+            self._d_ingest_scores = self.ctx.new_scores()
+        d_scores = scores_out if device else self._d_ingest_scores
+        split = bool((lens > self.ctx.ingest_capacity()).any())
+        part = self.ctx.new_scores() if split else d_scores
+        done = np.zeros(B, np.int64)
+        prepared = np.zeros(B, np.int64)
+        pos = np.zeros(B, np.int64)
+        if split and self._verifier_banks:
+            self.ctx.enable_verifiers(False)
+        try:
+            while True:
+                take = np.minimum(lens - pos, self.ctx.ingest_capacity())
+                offsets = np.concatenate([[0], np.cumsum(take)]).astype(np.int64)
+                pcm = np.concatenate([xs[b][pos[b]:pos[b] + take[b]] for b in range(B)])
+                c, p = self.ctx.ingest_pcm(pcm, offsets, part)
+                if split:               # per stream the max over all its parts
+                    _take_rows(d_scores, part, (done == 0) & (c > 0), False)
+                    _take_rows(d_scores, part, (done > 0) & (c > 0), True)
+                done += c
+                prepared = p.astype(np.int64)
+                pos += take
+                if (pos >= lens).all():
+                    break
+        finally:
+            if split and self._verifier_banks:
+                self.ctx.enable_verifiers(True)
+        if not device:
+            stepped = done > 0
+            if stepped.any():
+                host = d_scores if isinstance(d_scores, np.ndarray) else d_scores.cpu().numpy()
+                scores_out[stepped] = host[stepped]
+        self._held_in_raw = done == 0
+        n_prepared = np.where(done > 0, done * CHUNK, prepared)
+        return n_prepared, done, split
+
+    def _held(self, b):
+        """int16 samples stream b holds not yet stepped (16 kHz)"""
+        if self.ingest:
+            _, _, staged, x, _ = self.ctx.ingest_state([b])
+            return x[0, :staged[0]]
+        buf, lens = self._ragged_pending()
+        return buf[b, :lens[b]]
 
     def __call__(self, x):
         return self._streaming_features(x)[0]
@@ -406,9 +487,25 @@ class AudioFeatures:
         audio, pos = self.ctx.audio_state([0])
         x = audio[0, H - int(min(pos[0], H)):]
         if self._held_in_raw[0]:
-            buf, lens = self._ragged_pending()
-            x = np.concatenate((x, buf[0, :lens[0]]))[-H:]
+            x = np.concatenate((x, self._held(0)))[-H:]
         return deque(x.tolist(), maxlen=H)
+
+
+def input_rates(sr, n_streams):
+    """sr (an int, or a sequence of n_streams ints) -> int32 [n_streams] input rates for device ingest, or None for the
+    default int 16000 (the host-side path).  ValueError for a rate the library does not take (oww_resampler_taps)."""
+    if np.ndim(sr) == 0:
+        if int(sr) == 16000:
+            return None
+        rates = np.full(n_streams, int(sr), np.int32)
+    else:
+        rates = np.asarray(sr, np.int64).ravel()
+        if rates.size != n_streams:
+            raise ValueError(f"sr has {rates.size} rates for {n_streams} streams")
+        rates = rates.astype(np.int32)
+    for r in np.unique(rates):
+        _native.resampler_taps(int(r))
+    return rates
 
 
 def audio_history_samples(seconds):
