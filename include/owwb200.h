@@ -509,6 +509,29 @@ int oww_predict_clips_streams(oww_ctx* ctx, const int16_t* d_pcm, const int64_t*
 /* The slabs oww_predict_clips_ragged would run for clips of h_steps[i] chunks each (ctx may be NULL: the default
  * configuration): returns the slab count, and the steps the slabs compute and the steps the clips need.  Pure host. */
 int oww_clip_slab_plan(oww_ctx* ctx, const int32_t* h_steps, int n_clips, int64_t* h_steps_computed, int64_t* h_steps_needed);
+/* Whole clips at any rate of the ingest table, resampled to 16 kHz without state (the reference converts a corpus to
+ * 16 kHz with ffmpeg / sox first, openwakeword/data.py:convert_clips).  A clip x of S samples at rate r, with pad_samples
+ * = pad 16 kHz samples of padding, becomes the first A(S) + 2*pad outputs of upfirdn(h, zeros(pad*down/up) ++ x ++
+ * zeros(pad*down/up), up, down), with h, up, down and A of the ingest section above and each output computed exactly as
+ * oww_ingest computes it (the same fp32 FMA chain and int16 rounding).  So the first pad outputs are 0, the next A(S) are
+ * the samples oww_ingest makes final for x on a fresh stream, bit for bit, and the last pad hold the filter's tail (at
+ * most 39 nonzero samples), then zeros: the whole is what a fresh stream makes of the padded clip.  At 16000 a clip is
+ * copied between pad zeros.
+ *   oww_resample_clip_plan - pure host, no handle or GPU: *n_out (may be NULL) <- A(n_in) + 2*pad_samples.  OWW_EINVAL:
+ *                       a rate outside the table, a negative n_in or pad_samples, or a pad_samples the rate's up factor
+ *                       does not divide (every up of the table divides 640, so whole seconds always work).
+ *   oww_resample_clips - clip i is d_in[h_in_offsets[i] .. h_in_offsets[i+1]) at h_rates[i] Hz (host arrays, n_clips + 1
+ *                       offsets, non-decreasing, first >= 0; rates may differ between clips; lengths 0 and 1 are legal);
+ *                       its outputs go to d_out[h_out_offsets[i] .. h_out_offsets[i+1]), pads included, and
+ *                       h_out_offsets[i+1] - h_out_offsets[i] must equal oww_resample_clip_plan's count.  One launch
+ *                       over tiles of 2048 outputs; the pads are never read from memory.  The first call uploads the
+ *                       filter tables (a synchronous copy); a call waits, host side, until the previous call's launch has
+ *                       read its tables.  The handle's streams and ingest state are not touched, and a handle that never
+ *                       calls it allocates nothing for it.  OWW_EINVAL before anything is enqueued: bad offsets or rates,
+ *                       a pad the up factor does not divide, output offsets that do not match the plan, NULL buffers. */
+int oww_resample_clip_plan(int rate, int64_t n_in, int pad_samples, int64_t* n_out);
+int oww_resample_clips(oww_ctx* ctx, const int16_t* d_in, const int64_t* h_in_offsets, const int32_t* h_rates, int n_clips,
+                       int pad_samples, int16_t* d_out, const int64_t* h_out_offsets, void* stream);
 
 /* ---- score metrics on the device (openwakeword/metrics.py:24-100) --------------------------------
  * d_scores holds n_series score sequences of n_frames float32 each, series i at d_scores + i*series_stride.

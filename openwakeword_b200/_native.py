@@ -110,6 +110,8 @@ _SIGNATURES = {
     "oww_predict_clips_ragged": (C.c_int, [_P, _P, _P, C.c_int, C.c_int, C.c_int, _P, C.c_int, _P, _P, _P, _P]),
     "oww_predict_clips_streams": (C.c_int, [_P, _P, _P, C.c_int, C.c_int, C.c_int, _P, C.c_int, _P, _P, _P, _P, _P]),
     "oww_clip_slab_plan": (C.c_int, [_P, _P, C.c_int, C.POINTER(C.c_int64), C.POINTER(C.c_int64)]),
+    "oww_resample_clip_plan": (C.c_int, [C.c_int, C.c_int64, C.c_int, C.POINTER(C.c_int64)]),
+    "oww_resample_clips": (C.c_int, [_P, _P, _P, _P, C.c_int, C.c_int, _P, _P, _P]),
     "oww_debug_layer": (C.c_int, [_P, _P, C.c_int, C.c_int, _P, _P]),
     "oww_debug_inc_plan": (C.c_int, [_P, C.c_int, C.c_int, _P, C.c_int]),
     "oww_debug_inc_cut_plan": (C.c_int, [_P, C.c_int, C.c_int, C.c_int, _P, C.c_int]),
@@ -214,6 +216,18 @@ def ingest_plan(rate, max_chunks, n_before, staged, n_in):
     if rc:
         return None, None, None, max_in.value
     return n_out.value, chunks.value, after.value, max_in.value
+
+
+def resample_clip_plan(rate, n_in, pad_samples):
+    """16 kHz samples a clip of n_in samples at `rate` becomes with pad_samples of padding each side (oww_resample_clip_plan:
+    pure host, no GPU); ValueError for a rate outside the table, negative arguments, or a pad the rate cannot take."""
+    lib = load_library()
+    n = C.c_int64(0)
+    if lib.oww_resample_clip_plan(int(rate), int(n_in), int(pad_samples), C.byref(n)):
+        raise ValueError(f"oww_resample_clip_plan refused rate {rate}, {n_in} samples, pad {pad_samples}: the rates are "
+                         "8000, 11025, 12000, 16000, 22050, 24000, 32000, 44100 and 48000 Hz, and the padding a multiple "
+                         "of 640 samples (40 ms)")
+    return n.value
 
 
 def _ptr(a):
@@ -892,6 +906,17 @@ class Context:
         if cs.size != off.size - 1:
             raise ValueError(f"{cs.size} clip streams for {off.size - 1} clips")
         self._check(self.lib.oww_predict_clips_streams(*args, _ptr(cs), stream))
+
+    def resample_clips(self, d_in, in_offsets, rates, pad_samples, d_out, out_offsets, stream=None):
+        """oww_resample_clips: clip i is d_in[in_offsets[i]:in_offsets[i+1]] at rates[i] Hz -> d_out[out_offsets[i]:
+        out_offsets[i+1]] at 16 kHz with pad_samples of padding each side (host int64 offsets, host int32 rates)."""
+        off = np.ascontiguousarray(in_offsets, np.int64).ravel()
+        out = np.ascontiguousarray(out_offsets, np.int64).ravel()
+        r = np.ascontiguousarray(rates, np.int32).ravel()
+        if r.size != off.size - 1 or out.size != off.size:
+            raise ValueError(f"{off.size} input offsets, {out.size} output offsets and {r.size} rates")
+        self._check(self.lib.oww_resample_clips(self.h, _ptr(d_in), _ptr(off), _ptr(r), r.size, int(pad_samples),
+                                                _ptr(d_out), _ptr(out), stream))
 
     def debug_layer(self, d_windows, n, layer, d_out, stream=None):
         self._check(self.lib.oww_debug_layer(self.h, _ptr(d_windows), n, layer, _ptr(d_out), stream))

@@ -120,6 +120,24 @@ struct oww_ingest_state {
     std::vector<int32_t> chunks;      // scratch of a call
 };
 
+// One 16 kHz output, the single definition both resamplers use: output index i0 + j of a rate whose output i0 reads input
+// q00 (r0 = i0 * down - q00 * up), with q00 at position `base` of the caller's input; load(k) returns the input at
+// position k.  One fp32 FMA chain over the phase's K taps (zero taps included), newest input first, from 0; then round
+// half to even and saturate.
+template <typename Load>
+__device__ __forceinline__ int16_t resample_output(const IngestRate& rt, const float* __restrict__ taps, int r0, int base,
+                                                   int j, Load load) {
+    const int frac = r0 + j * rt.down;
+    const int dq = frac / rt.up;
+    const int p = frac - dq * rt.up;
+    const int local = base + dq;                                // newest input sample the output reads
+    const float* h = taps + rt.off + p * rt.K;
+    float acc = 0.f;
+    for (int t = 0; t < rt.K; ++t) acc = fmaf(h[t], load(local - t), acc);
+    const int r = __float2int_rn(acc);                          // round half to even
+    return (int16_t)max(-32768, min(32767, r));
+}
+
 // The kernels stay outside the anonymous namespace: their names in a profile do not depend on the build.
 // CTA b: stream b of the call (rows[b]).
 __global__ void __launch_bounds__(ING_THREADS) resample_kernel(const int16_t* __restrict__ in,
@@ -153,26 +171,68 @@ __global__ void __launch_bounds__(ING_THREADS) resample_kernel(const int16_t* __
     const int64_t n0 = i0 * rt.down, q00 = n0 / rt.up;
     const int r0 = (int)(n0 - q00 * rt.up);
     const int base = (int)(q00 - R.s_prev);                    // >= 0: A(S) * down >= S * up
-    for (int j = threadIdx.x; j < R.n_out; j += ING_THREADS) {
-        const int frac = r0 + j * rt.down;
-        const int dq = frac / rt.up;
-        const int p = frac - dq * rt.up;
-        const int local = base + dq;                            // newest input sample the output reads
-        const float* h = taps + rt.off + p * rt.K;
-        float acc = 0.f;
-        for (int t = 0; t < rt.K; ++t) {
-            const int idx = local - t;
-            const int16_t v = idx >= 0 ? x[idx] : s_hist[ING_HIST + idx];
-            acc = fmaf(h[t], (float)v, acc);
-        }
-        const int r = __float2int_rn(acc);                      // round half to even
-        out[j] = (int16_t)max(-32768, min(32767, r));
-    }
+    const auto load = [&](int idx) { return (float)(idx >= 0 ? x[idx] : s_hist[ING_HIST + idx]); };
+    for (int j = threadIdx.x; j < R.n_out; j += ING_THREADS) out[j] = resample_output(rt, taps, r0, base, j, load);
     // the new history: the last 128 samples of [old history | new input]
     for (int k = threadIdx.x; k < ING_HIST; k += ING_THREADS) {
         const int idx = R.n_in - ING_HIST + k;
         hb[k] = idx >= 0 ? x[idx] : s_hist[ING_HIST + idx];
     }
+}
+
+// ---- oww_resample_clips: whole clips, no state ----
+// Clip c with n_in input samples and `pad` 16 kHz samples of padding has L = A(n_in) + 2*pad outputs: output i is output
+// j = i - pad of upfirdn(h, clip, up, down) (pad*down/up leading zeros in front of the clip shift it by exactly pad
+// outputs), and outputs with j < 0 read only those zeros, so they are 0.  The outputs are cut into tiles of CLIP_TILE; a
+// CTA stages its tile's input window (the K - 1 samples before it included, zeros outside the clip) as fp32 in shared
+// memory.  The window is at most (CLIP_TILE - 1) * down/up + 1 + (K - 1) samples; down/up <= 3 and K <= 61 in the table.
+#define CLIP_TILE 2048
+#define CLIP_WIN (3 * CLIP_TILE + 64)
+
+struct ClipRow {                      // per clip of a call
+    int64_t in_off, n_in;             // its input d_in[in_off, in_off + n_in)
+    int64_t out_off, n_out;           // its outputs d_out[out_off, out_off + n_out), pads included
+    int32_t rate;                     // index into the rate table
+    int32_t unused;
+};
+struct ClipTile { int32_t clip, tile; };    // outputs [tile * CLIP_TILE, (tile + 1) * CLIP_TILE) of clip `clip`
+
+__global__ void __launch_bounds__(ING_THREADS) resample_clips_kernel(const int16_t* __restrict__ in,
+                                                                     const ClipRow* __restrict__ clips,
+                                                                     const ClipTile* __restrict__ tiles,
+                                                                     const IngestRates rates, const float* __restrict__ taps,
+                                                                     int pad, int16_t* __restrict__ out) {
+    __shared__ float s_in[CLIP_WIN];
+    const ClipTile T = tiles[blockIdx.x];
+    const ClipRow C = clips[T.clip];
+    const IngestRate rt = rates.r[C.rate];
+    const int64_t i_first = (int64_t)T.tile * CLIP_TILE;
+    const int n = (int)min((int64_t)CLIP_TILE, C.n_out - i_first);
+    int16_t* y = out + C.out_off + i_first;
+    const int16_t* x = in + C.in_off;
+    const int64_t j_first = i_first - pad;
+    const int lead = (int)max((int64_t)0, min((int64_t)n, -j_first));   // outputs of the tile in the leading pad
+    for (int k = threadIdx.x; k < lead; k += ING_THREADS) y[k] = 0;
+    if (lead == n) return;
+    const int64_t j0 = j_first + lead;                                     // >= 0
+    const int m = n - lead;
+    y += lead;
+    if (rt.up == rt.down) {                                                // 16 kHz: a copy, zeros past the clip
+        for (int k = threadIdx.x; k < m; k += ING_THREADS) y[k] = j0 + k < C.n_in ? x[j0 + k] : (int16_t)0;
+        return;
+    }
+    // the 64-bit part split off once per tile: output j0 reads input q00, phase r0; the window starts K - 1 before it
+    const int64_t n0 = j0 * rt.down, q00 = n0 / rt.up;
+    const int r0 = (int)(n0 - q00 * rt.up);
+    const int64_t q_lo = q00 - (rt.K - 1);
+    const int w = (r0 + (m - 1) * rt.down) / rt.up + rt.K;
+    for (int k = threadIdx.x; k < w; k += ING_THREADS) {
+        const int64_t q = q_lo + k;
+        s_in[k] = q >= 0 && q < C.n_in ? (float)x[q] : 0.f;
+    }
+    __syncthreads();
+    const auto load = [&](int idx) { return s_in[idx]; };
+    for (int k = threadIdx.x; k < m; k += ING_THREADS) y[k] = resample_output(rt, taps, r0, rt.K - 1, k, load);
 }
 
 // record i <-> stream ids[i]: the staged samples [off, off + staged) of the row (export: row i of out, zeros after them)
@@ -246,12 +306,11 @@ int alloc_stream_state(oww_ctx* ctx) {
     return OWW_OK;
 }
 
-// the polyphase tables of every rate, once per handle
-int upload_taps(oww_ctx* ctx) {
-    oww_ingest_state* g = ctx->ingest;
+// the polyphase tables of every rate, uploaded to *d_taps
+int upload_taps(oww_ctx* ctx, IngestRates* rates, float** d_taps) {
     std::vector<float> all;
     for (int r = 0; r < kNRates; ++r) {
-        IngestRate& R = g->rates.r[r];
+        IngestRate& R = rates->r[r];
         R.off = (int)all.size();
         if (kRates[r] == 16000) { R.up = R.down = 1; R.K = 0; continue; }
         const std::vector<double> h = design(kRates[r], &R.up, &R.down);
@@ -262,9 +321,44 @@ int upload_taps(oww_ctx* ctx) {
             for (int t = 0; t < R.K; ++t)
                 if (p + R.up * t < N) all[R.off + (size_t)p * R.K + t] = (float)h[p + R.up * t];
     }
-    OWW_CUDA(ctx, cudaMalloc(&g->d_taps, all.size() * sizeof(float)));
-    OWW_CUDA(ctx, cudaMemcpy(g->d_taps, all.data(), all.size() * sizeof(float), cudaMemcpyHostToDevice));
+    OWW_CUDA(ctx, cudaMalloc(d_taps, all.size() * sizeof(float)));
+    OWW_CUDA(ctx, cudaMemcpy(*d_taps, all.data(), all.size() * sizeof(float), cudaMemcpyHostToDevice));
     return OWW_OK;
+}
+
+// n_in samples at `rate` with `pad` 16 kHz samples of padding -> outputs (A(n_in) + 2*pad); false for arguments
+// oww_resample_clip_plan refuses
+bool clip_plan(int rate, int64_t n_in, int pad, int64_t* n_out) {
+    if (rate_index(rate) < 0 || n_in < 0 || pad < 0) return false;
+    int up, down;
+    up_down(rate, &up, &down);
+    if (pad % up) return false;
+    *n_out = final_outputs(n_in, up, down) + 2 * (int64_t)pad;
+    return true;
+}
+
+}  // namespace
+
+// The clip resampler's own taps and tables: kept apart from oww_ingest_state, whose existence means "the handle's
+// streams take ingest" to oww_set_input_rates.
+struct oww_clip_resampler {
+    IngestRates rates;
+    float* d_taps = nullptr;
+    void* h_tab = nullptr;            // pinned: ClipRow [n_clips], then ClipTile [n_tiles]
+    void* d_tab = nullptr;
+    size_t tab_bytes = 0;
+    cudaEvent_t done = nullptr;       // after the last launch: the tables may be rewritten once it has completed
+};
+
+namespace {
+
+void clip_free(oww_ctx* ctx) {
+    oww_clip_resampler* c = ctx->clip_rs;
+    if (!c) return;
+    cudaFree(c->d_taps); cudaFreeHost(c->h_tab); cudaFree(c->d_tab);
+    if (c->done) cudaEventDestroy(c->done);
+    delete c;
+    ctx->clip_rs = nullptr;
 }
 
 int check_ids(oww_ctx* ctx, const int32_t* h_ids, int n, bool distinct) {
@@ -287,7 +381,7 @@ int need_state(oww_ctx* ctx) {
 
 }  // namespace
 
-void oww_ingest_free(oww_ctx* ctx) { ingest_free(ctx); }
+void oww_ingest_free(oww_ctx* ctx) { ingest_free(ctx); clip_free(ctx); }
 
 void oww_ingest_free_streams(oww_ctx* ctx) { if (ctx->ingest) free_stream_state(ctx->ingest); }
 
@@ -349,7 +443,8 @@ int oww_set_input_rates(oww_ctx* ctx, const int32_t* h_stream_ids, int n, const 
         OWW_CUDA(ctx, cudaDeviceSynchronize());
         ctx->ingest = new (std::nothrow) oww_ingest_state();
         if (!ctx->ingest) return oww_fail(ctx, OWW_ENOMEM, "out of host memory");
-        if ((rc = upload_taps(ctx)) || (rc = alloc_stream_state(ctx))) { ingest_free(ctx); return rc; }
+        oww_ingest_state* g = ctx->ingest;
+        if ((rc = upload_taps(ctx, &g->rates, &g->d_taps)) || (rc = alloc_stream_state(ctx))) { ingest_free(ctx); return rc; }
     }
     oww_ingest_state* g = ctx->ingest;
     for (int i = 0; i < n; ++i) {
@@ -487,6 +582,79 @@ int oww_ingest_import(oww_ctx* ctx, const int32_t* h_stream_ids, int n, const in
         const int b = h_stream_ids[i];
         g->rate[b] = h_rates[i]; g->S[b] = h_consumed[i]; g->staged[b] = h_staged[i]; g->staged_off[b] = 0;
     }
+    return OWW_OK;
+}
+
+int oww_resample_clip_plan(int rate, int64_t n_in, int pad_samples, int64_t* n_out) {
+    int64_t n = 0;
+    if (!clip_plan(rate, n_in, pad_samples, &n)) return OWW_EINVAL;
+    if (n_out) *n_out = n;
+    return OWW_OK;
+}
+
+int oww_resample_clips(oww_ctx* ctx, const int16_t* d_in, const int64_t* h_in_offsets, const int32_t* h_rates, int n_clips,
+                       int pad_samples, int16_t* d_out, const int64_t* h_out_offsets, void* stream) {
+    if (!ctx) return OWW_EINVAL;
+    if (n_clips < 0) return oww_fail(ctx, OWW_EINVAL, "n_clips=%d is negative", n_clips);
+    if (pad_samples < 0) return oww_fail(ctx, OWW_EINVAL, "pad_samples=%d is negative", pad_samples);
+    if (n_clips == 0) return OWW_OK;
+    if (!h_in_offsets || !h_rates || !h_out_offsets) return oww_fail(ctx, OWW_EINVAL, "null argument");
+    if (h_in_offsets[0] < 0 || h_out_offsets[0] < 0) return oww_fail(ctx, OWW_EINVAL, "negative first offset");
+    int64_t n_tiles = 0;
+    for (int i = 0; i < n_clips; ++i) {
+        const int64_t n_in = h_in_offsets[i + 1] - h_in_offsets[i];
+        if (n_in < 0) return oww_fail(ctx, OWW_EINVAL, "input offsets decrease at clip %d", i);
+        if (rate_index(h_rates[i]) < 0)
+            return oww_fail(ctx, OWW_EINVAL, "clip %d: rate %d is not in the rate table", i, h_rates[i]);
+        int64_t L;
+        if (!clip_plan(h_rates[i], n_in, pad_samples, &L))
+            return oww_fail(ctx, OWW_EINVAL, "clip %d: pad_samples=%d is not a multiple of %d Hz's up factor", i,
+                            pad_samples, h_rates[i]);
+        if (h_out_offsets[i + 1] - h_out_offsets[i] != L)
+            return oww_fail(ctx, OWW_EINVAL, "clip %d: output offsets give %lld samples, oww_resample_clip_plan %lld", i,
+                            (long long)(h_out_offsets[i + 1] - h_out_offsets[i]), (long long)L);
+        n_tiles += (L + CLIP_TILE - 1) / CLIP_TILE;
+    }
+    if (n_tiles > INT32_MAX) return oww_fail(ctx, OWW_EINVAL, "%lld tiles in one call", (long long)n_tiles);
+    if (h_in_offsets[n_clips] > h_in_offsets[0] && !d_in) return oww_fail(ctx, OWW_EINVAL, "null argument");
+    if (n_tiles == 0) return OWW_OK;
+    if (!d_out) return oww_fail(ctx, OWW_EINVAL, "null argument");
+    OWW_CUDA(ctx, cudaSetDevice(ctx->device));
+    if (!ctx->clip_rs) {
+        ctx->clip_rs = new (std::nothrow) oww_clip_resampler();
+        if (!ctx->clip_rs) return oww_fail(ctx, OWW_ENOMEM, "out of host memory");
+        int rc = upload_taps(ctx, &ctx->clip_rs->rates, &ctx->clip_rs->d_taps);
+        if (!rc && cudaEventCreateWithFlags(&ctx->clip_rs->done, cudaEventDisableTiming) != cudaSuccess)
+            rc = oww_fail(ctx, OWW_ECUDA, "cudaEventCreate failed");
+        if (rc) { clip_free(ctx); return rc; }
+    }
+    oww_clip_resampler* c = ctx->clip_rs;
+    OWW_CUDA(ctx, cudaEventSynchronize(c->done));              // the previous call's tables have been read
+    const size_t tile_off = (size_t)n_clips * sizeof(ClipRow);
+    const size_t bytes = tile_off + (size_t)n_tiles * sizeof(ClipTile);
+    if (bytes > c->tab_bytes) {
+        cudaFreeHost(c->h_tab); cudaFree(c->d_tab);
+        c->h_tab = nullptr; c->d_tab = nullptr; c->tab_bytes = 0;
+        const size_t want = std::max(bytes, 2 * c->tab_bytes);
+        OWW_CUDA(ctx, cudaMallocHost(&c->h_tab, want));
+        OWW_CUDA(ctx, cudaMalloc(&c->d_tab, want));
+        c->tab_bytes = want;
+    }
+    ClipRow* rows = (ClipRow*)c->h_tab;
+    ClipTile* tiles = (ClipTile*)((char*)c->h_tab + tile_off);
+    int64_t t = 0;
+    for (int i = 0; i < n_clips; ++i) {
+        const int64_t L = h_out_offsets[i + 1] - h_out_offsets[i];
+        rows[i] = ClipRow{h_in_offsets[i], h_in_offsets[i + 1] - h_in_offsets[i], h_out_offsets[i], L, rate_index(h_rates[i]), 0};
+        for (int64_t k = 0; k * CLIP_TILE < L; ++k) tiles[t++] = ClipTile{i, (int32_t)k};
+    }
+    cudaStream_t s = (cudaStream_t)stream;
+    OWW_CUDA(ctx, cudaMemcpyAsync(c->d_tab, c->h_tab, bytes, cudaMemcpyHostToDevice, s));
+    resample_clips_kernel<<<(unsigned)n_tiles, ING_THREADS, 0, s>>>(d_in, (const ClipRow*)c->d_tab,
+                                                                   (const ClipTile*)((char*)c->d_tab + tile_off), c->rates,
+                                                                   c->d_taps, pad_samples, d_out);
+    OWW_LAUNCH_CHECK(ctx);
+    OWW_CUDA(ctx, cudaEventRecord(c->done, s));
     return OWW_OK;
 }
 

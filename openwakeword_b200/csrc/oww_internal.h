@@ -326,6 +326,7 @@ struct oww_ctx {
     struct oww_detector* det = nullptr;   // detections on the device (detect.cu); nullptr: no detector configured
     struct oww_audio* audio = nullptr;    // the streams' recent audio (audio.cu); nullptr: no history
     struct oww_ingest_state* ingest = nullptr;  // resampling and staging of packets at any rate (ingest.cu); nullptr: off
+    struct oww_clip_resampler* clip_rs = nullptr;  // taps and tile tables of oww_resample_clips (ingest.cu); nullptr: unused
 };
 
 int oww_fail(oww_ctx* ctx, int code, const char* fmt, ...);
@@ -550,7 +551,7 @@ int oww_audio_append(oww_ctx* ctx, const int16_t* d_pcm, int64_t pcm_stride, int
                      cudaStream_t s);
 
 // ---- ingest.cu: packets at any rate (nothing happens on a handle without ingest state) ----
-void oww_ingest_free(oww_ctx* ctx);
+void oww_ingest_free(oww_ctx* ctx);              // the ingest state and the clip resampler's buffers
 void oww_ingest_free_streams(oww_ctx* ctx);
 int oww_ingest_alloc_streams(oww_ctx* ctx);      // for ctx->n_streams streams, every one at 16000, nothing staged
 // the listed streams (h_ids == nullptr: streams 0..n-1) drop their staged samples and history: host state only

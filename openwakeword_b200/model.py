@@ -7,7 +7,10 @@ them are replaced by one libowwb200 step per call.  Additions: ``n_streams`` ind
 the batch axis (``predict`` then takes ``[n_streams, samples]`` and returns arrays per label),
 ``predict_clips`` / ``predict_clips_ragged`` (bulk path over clips of any lengths) and ``feature_init``.  ``sr`` (passed
 to ``AudioFeatures``) other than 16000 makes ``predict*`` and ``detect*`` take each stream's audio at its own rate,
-resampled on the device (``set_sample_rates`` changes it); the clip and bulk paths then refuse with ValueError.
+resampled on the device (``set_sample_rates`` changes it); the clip and bulk paths then refuse clips without an ``sr``
+of their own.  Those paths take ``sr=`` (one rate or one per clip) on any Model, and WAV paths their header's rate:
+the clips are resampled to 16 kHz on the device with their padding (``AudioFeatures.resample_clips``) and run as
+16 kHz clips, which is what a fresh stream at that rate makes of the padded clip.
 """
 import os
 import time
@@ -19,7 +22,7 @@ import numpy as np
 
 from . import _native
 from . import weights as _weights
-from .utils import AudioFeatures, re_arg, _read_wav, CHUNK, _torch
+from .utils import AudioFeatures, re_arg, _read_wav, _read_wav_rate, CHUNK, _torch
 from . import registry as _registry
 from .custom_verifier_model import load_verifier, linear_verifier_params
 
@@ -672,10 +675,24 @@ class Model:
             raise ValueError("Speex noise suppression runs on 16 kHz audio only; it cannot be combined with streams at "
                              "other sample rates")
 
-    def _no_ingest(self, what):
+    def _no_ingest(self, what, hint=""):
         if self.preprocessor.ingest:
-            raise ValueError(f"{what} takes 16 kHz clips; this Model takes streams at other sample rates (sr=...), "
-                             "which the clip and bulk paths do not")
+            raise ValueError(f"{what} takes 16 kHz clips; this Model takes streams at other sample rates (sr=...)"
+                             + hint)
+
+    def _clip_rates(self, sr, n, what):
+        """sr of a clip call (None, one rate, or one per clip) -> int32 [n] rates, or None when the clips are 16 kHz
+        (no sr on a Model without device ingest, or every rate 16000).  No sr on a device-ingest Model raises."""
+        if sr is None:
+            self._no_ingest(what, "; pass the clips' rates as sr=")
+            return None
+        rates = np.asarray(sr, np.int64).ravel()
+        if rates.size not in (1, n):
+            raise ValueError(f"sr has {rates.size} rates for {n} clips")
+        for r in np.unique(rates):
+            _native.resampler_taps(int(r))                   # ValueError outside the table
+        rates = np.ascontiguousarray(np.broadcast_to(rates, (n,)), np.int32)
+        return None if (rates == 16000).all() else rates
 
     def _suppress_noise_with_speex(self, x, frame_size=160):
         cleaned = [self.speex_ns.process(x[i:i + frame_size].tobytes()) for i in range(0, x.shape[0], frame_size)]
@@ -961,18 +978,27 @@ class Model:
             return out, timing_dict
         return out
 
-    def predict_clip(self, clip, padding=1, chunk_size=1280, **kwargs):
-        """model.py:388-426: path or int16 array -> list of per-step dicts (no reset, like the reference)."""
+    def predict_clip(self, clip, padding=1, chunk_size=1280, sr=None, **kwargs):
+        """model.py:388-426: path or int16 array -> list of per-step dicts (no reset, like the reference).  A WAV is read
+        at its header's rate (an ``sr`` that disagrees raises ValueError), an array is at ``sr`` (default 16000).  At
+        another rate the clip is resampled to 16 kHz on the device with its padding, and ``chunk_size`` counts 16 kHz
+        samples.  A Model with device ingest refuses whatever ``sr``: its ``predict`` takes audio at the stream's rate."""
         if isinstance(clip, str):
-            data = _read_wav(clip)
+            data, rate = _read_wav_rate(clip)
+            if sr is not None and int(sr) != rate:
+                raise ValueError(f"{clip}: the header says {rate} Hz, sr={sr}")
         elif isinstance(clip, np.ndarray):
-            data = clip
+            data, rate = clip, 16000 if sr is None else int(sr)
         else:
             raise ValueError("clip must be a WAV path or a numpy array")
         if self.n_streams != 1:
             raise ValueError("predict_clip is single-stream; use predict_clips for batches")
         self._no_ingest("predict_clip")
-        if padding:
+        if rate != 16000:
+            x = np.asarray(data).astype(np.int16, copy=False).ravel()
+            d, _ = self.preprocessor.resample_clips(x, [0, x.size], rate, 16000 * int(padding))
+            data = d.cpu().numpy()
+        elif padding:
             z = np.zeros(16000 * padding).astype(np.int16)
             data = np.concatenate((z, data, z))
         return [self.predict(data[i:i + chunk_size], **kwargs) for i in range(0, data.shape[0] - chunk_size, chunk_size)]
@@ -981,13 +1007,17 @@ class Model:
         """model.py:428-478: run the WAV through ``predict`` in 1280-sample steps and collect, per label, what produced
         a score >= ``threshold``: the head's input features ``[n_in, 96]`` at that step (``return_type="features"``) or
         the 4 s of audio around it (``"audio"``: 3 s before, 1 s after; steps without a full 4 s are dropped).
-        Returns {label: stacked array}; labels without a hit are absent."""
+        Returns {label: stacked array}; labels without a hit are absent.  A WAV at another rate than 16 kHz is resampled
+        on the device first, and the audio context is cut from the 16 kHz samples."""
         if return_type not in ("features", "audio"):
             raise ValueError("return_type must be 'features' or 'audio'")
         if self.n_streams != 1:
             raise ValueError("_get_positive_prediction_frames is single-stream")
         self._no_ingest("_get_positive_prediction_frames")
-        data = _read_wav(file)
+        data, rate = _read_wav_rate(file)
+        if rate != 16000:
+            d, _ = self.preprocessor.resample_clips(data, [0, data.size], rate, 0)
+            data = d.cpu().numpy()
         hits = defaultdict(list)
         for i in range(0, data.shape[0] - CHUNK, CHUNK):
             for lbl, score in self.predict(data[i:i + CHUNK], **kwargs).items():
@@ -1002,36 +1032,50 @@ class Model:
                         hits[lbl].append(context)
         return {lbl: np.vstack(v) for lbl, v in hits.items() if v}
 
-    def predict_clips(self, clips, padding=1, feature_init=None, chunk_size=1280, streams=None):
+    def predict_clips(self, clips, padding=1, feature_init=None, chunk_size=1280, streams=None, sr=None):
         """Bulk path (extension; SURVEY.md F9): each clip from a fresh state, in one device call.  ``clips``: an int16
         [N,S] array or tensor, or a sequence of 1-D int16 arrays of any lengths.  Returns a list (per clip) of lists (per
         call) of {label: float}, i.e. what predict_clip(clip, padding, chunk_size) would return for each clip after
         reset(feature_init).  streams (N stream ids, or None: stream 0's models and verifiers): clip i is predicted as
-        stream streams[i] would predict it, with its stream models and device verifiers."""
-        self._no_ingest("predict_clips")
+        stream streams[i] would predict it, with its stream models and device verifiers.  sr: as in
+        predict_clips_ragged."""
+        rates = self._clip_rates(sr, len(clips), "predict_clips")
         torch = _torch()
-        if streams is None and chunk_size == CHUNK and (isinstance(clips, torch.Tensor)
-                                                        or (isinstance(clips, np.ndarray) and clips.ndim == 2)):
+        if rates is None and (sr is None or not self.preprocessor.ingest) and streams is None and chunk_size == CHUNK \
+                and (isinstance(clips, torch.Tensor) or (isinstance(clips, np.ndarray) and clips.ndim == 2)):
             scores, labels = self.predict_clips_array(clips, padding, feature_init)
             return [[{lab: float(scores[c, s, j]) for j, lab in enumerate(labels)} for s in range(scores.shape[1])]
                     for c in range(scores.shape[0])]
         pcm, offsets = _concat_clips(clips)
-        scores, row_off, labels = self.predict_clips_ragged(pcm, offsets, padding, chunk_size, feature_init, streams)
+        scores, row_off, labels = self.predict_clips_ragged(pcm, offsets, padding, chunk_size, feature_init, streams,
+                                                            sr=sr)
         return _rows_to_dicts(scores, row_off, labels)
 
-    def predict_clips_ragged(self, pcm, offsets, padding=1, chunk_size=1280, feature_init=None, streams=None):
+    def predict_clips_ragged(self, pcm, offsets, padding=1, chunk_size=1280, feature_init=None, streams=None, sr=None):
         """Array form of the bulk path over clips of any lengths: clip i is ``pcm[offsets[i]:offsets[i+1]]`` (int16 1-D
         array or tensor, int64 offsets).  Returns (float32 [rows, n_labels], int64 row_offsets [N+1], labels): clip i's
         rows ``row_offsets[i]:row_offsets[i+1]`` are the predictions predict_clip(clip, padding, chunk_size) returns after
-        reset(feature_init), one per call.  streams: as in predict_clips."""
-        return self._predict_ragged(pcm, offsets, padding, chunk_size, feature_init, streams=streams)[:3]
+        reset(feature_init), one per call.  streams: as in predict_clips.  sr: the clips' rate, one for all or one per
+        clip (None: 16 kHz).  Clips at other rates are resampled to 16 kHz with their padding in one device launch
+        (AudioFeatures.resample_clips) and then run as 16 kHz clips without padding: ``chunk_size`` counts 16 kHz samples
+        and a clip makes len(range(0, L - chunk_size, chunk_size)) calls over its L = A(S) + 2*16000*padding samples."""
+        offsets = np.ascontiguousarray(offsets, np.int64)
+        rates = self._clip_rates(sr, offsets.size - 1, "the bulk clip path (predict_clips_ragged, bulk_predict)")
+        if rates is None:
+            return self._predict_ragged(pcm, offsets, padding, chunk_size, feature_init, streams=streams,
+                                        check_ingest=sr is None)[:3]
+        d, off16 = self.preprocessor.resample_clips(pcm, offsets, rates, 16000 * int(padding))
+        return self._predict_ragged(d, off16, 0, chunk_size, feature_init, streams=streams, check_ingest=False)[:3]
 
-    def _predict_ragged(self, pcm, offsets, padding, chunk_size, feature_init, want_features=False, streams=None):
+    def _predict_ragged(self, pcm, offsets, padding, chunk_size, feature_init, want_features=False, streams=None,
+                        check_ingest=True):
         """-> (scores, row_offsets, labels, embeddings [steps, 96] or None, step_offsets [N+1], feature_init rows).
         One oww_predict_clips_ragged call; the host fills the rows of calls that stepped no chunk as Model.predict does
         (the previous prediction of single-output heads, zeros for multi-class heads, re-verified), then zeroes each
-        clip's first 5 calls (model.py:330-333).  Vectorised over rows."""
-        self._no_ingest("the bulk clip path (predict_clips_ragged, bulk_predict)")
+        clip's first 5 calls (model.py:330-333).  Vectorised over rows.  check_ingest=False: the caller gave the
+        clips' rate, so a device-ingest Model takes them too."""
+        if check_ingest:
+            self._no_ingest("the bulk clip path (predict_clips_ragged, bulk_predict)")
         if self._host_verifiers:
             warnings.warn(f"custom verifiers of {sorted(self._host_verifiers)} are not device-runnable (only the linear "
                           "pipeline of train_verifier_model is): predict_clips returns their models' unverified scores",
@@ -1121,15 +1165,22 @@ class Model:
                     sel = out[hit_rows, j] >= thr
                     out[hit_rows[sel], j] = p[sel]
 
-    def _positive_frames_bulk(self, pcms, threshold=0.5, return_type="features"):
+    def _positive_frames_bulk(self, pcms, threshold=0.5, return_type="features", sr=None):
         """_get_positive_prediction_frames over many clips in one device call (padding 0, 1280-sample calls): per clip
-        {label: stacked array} of what produced a score >= threshold."""
+        {label: stacked array} of what produced a score >= threshold.  sr: as in predict_clips_ragged; the audio context
+        of clips at other rates is cut from their 16 kHz samples."""
         if return_type not in ("features", "audio"):
             raise ValueError("return_type must be 'features' or 'audio'")
-        self._no_ingest("_get_positive_prediction_frames")
+        rates = self._clip_rates(sr, len(pcms), "_get_positive_prediction_frames")
         pcm, offsets = _concat_clips(pcms)
+        if rates is not None:
+            pcm, offsets = self.preprocessor.resample_clips(pcm, offsets, rates, 0)
+            if return_type == "audio":
+                host = pcm.cpu().numpy()
+                pcms = [host[offsets[c]:offsets[c + 1]] for c in range(offsets.size - 1)]
         scores, row_off, labels, emb, step_off, fi = self._predict_ragged(pcm, offsets, 0, CHUNK, None,
-                                                                          want_features=return_type == "features")
+                                                                          want_features=return_type == "features",
+                                                                          check_ingest=sr is None)
         n_in = {lab: self.model_inputs[self.get_parent_model_from_label(lab)] for lab in labels}
         res = []
         for c, data in enumerate(pcms):

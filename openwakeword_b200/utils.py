@@ -259,21 +259,49 @@ class AudioFeatures:
         wins = np.stack([x[:, 8 * i:8 * i + 76] for i in range(n_w)], axis=1).reshape(-1, 76, 32)
         return np.atleast_2d(self._embedding_model_predict(wins)).reshape(x.shape[0], n_w, 96)
 
-    def embed_clips(self, x, batch_size=128, ncpu=1):
-        """utils.py:358-385: int16 [N,samples] -> float32 [N,(T-76)//8+1,96]; one device call."""
+    def embed_clips(self, x, batch_size=128, ncpu=1, sr=16000):
+        """utils.py:358-385: int16 [N,samples] -> float32 [N,(T-76)//8+1,96]; one device call.  ``sr``: the clips' rate;
+        at another rate of the table they are resampled on the device first (resample_clips, no padding) and T counts
+        the A(samples) 16 kHz samples."""
         torch = _torch()
         x = np.ascontiguousarray(np.asarray(x))
         if x.dtype != np.int16:
             raise ValueError(f"Input data must be 16-bit integers. You provided {x.dtype} data.")
         n, s = x.shape
+        if int(sr) != 16000:
+            s = _native.resample_clip_plan(int(sr), s, 0)
         T = (s - 512) // 160 + 1 if s >= 512 else 0
         if T < 76:
             raise ValueError("Embedding model requires the input melspectrograms to have at least 76 frames")
         W = (T - 76) // 8 + 1
-        d = torch.from_numpy(x).to(f"cuda:{self.device_index}")
+        if int(sr) != 16000:
+            d, _ = self.resample_clips(x.reshape(-1), np.arange(n + 1, dtype=np.int64) * x.shape[1], int(sr), 0)
+        else:
+            d = torch.from_numpy(x).to(f"cuda:{self.device_index}")
         out = torch.empty((n, W, 96), dtype=torch.float32, device=d.device)
         self.ctx.embed_clips(d, n, s, out, torch.cuda.current_stream(d.device).cuda_stream)
         return out.cpu().numpy()
+
+    def resample_clips(self, pcm, offsets, rates, pad_samples=0):
+        """Clips at any rates of the table -> 16 kHz on the device in one launch (include/owwb200.h, oww_resample_clips):
+        clip i is ``pcm[offsets[i]:offsets[i+1]]`` (int16 host array or tensor) at ``rates[i]`` Hz (or one rate for all),
+        padded with ``pad_samples`` 16 kHz samples each side.  Returns (int16 CUDA tensor, int64 host offsets [N+1]) of the
+        resampled clips, pads included: what a fresh stream of that rate makes of the padded clip."""
+        torch = _torch()
+        offsets = np.ascontiguousarray(offsets, np.int64).ravel()
+        n = offsets.size - 1
+        rates = np.ascontiguousarray(np.broadcast_to(np.asarray(rates, np.int64).ravel(), (n,)), np.int32)
+        lengths = [_native.resample_clip_plan(int(r), int(k), int(pad_samples)) for r, k in zip(rates, np.diff(offsets))]
+        out_off = np.concatenate([[0], np.cumsum(lengths, dtype=np.int64)]).astype(np.int64)
+        dev = f"cuda:{self.device_index}"
+        if isinstance(pcm, torch.Tensor):
+            d_in = pcm.to(device=dev, dtype=torch.int16, non_blocking=True).contiguous()
+        else:
+            d_in = torch.from_numpy(np.ascontiguousarray(pcm, np.int16)).to(dev)
+        d_out = torch.empty(max(int(out_off[-1]), 1), dtype=torch.int16, device=dev)[:int(out_off[-1])]
+        self.ctx.resample_clips(d_in, offsets, rates, int(pad_samples), d_out, out_off,
+                                torch.cuda.current_stream(d_out.device).cuda_stream)
+        return d_out, out_off
 
     # ---- streaming ----
     def _coerce(self, x):
@@ -526,34 +554,51 @@ def _take_rows(dst, src, rows, maximum):
         dst[rows] = np.maximum(dst[rows], src[rows]) if maximum else src[rows]
 
 
-def _read_wav(path):
+def _read_wav_rate(path):
+    """16-bit single-channel WAV at any rate of the resampler's table -> (int16 samples, rate); ValueError naming the
+    file otherwise"""
     with wave.open(path, mode="rb") as f:
-        if f.getframerate() != 16000 or f.getnchannels() != 1 or f.getsampwidth() != 2:
-            raise ValueError(f"{path}: expected 16-bit, 16 khz, single-channel WAV")
-        return np.frombuffer(f.readframes(f.getnframes()), dtype=np.int16)
+        rate = f.getframerate()
+        if f.getnchannels() != 1 or f.getsampwidth() != 2:
+            raise ValueError(f"{path}: expected a 16-bit, single-channel WAV")
+        if rate != 16000:
+            try:
+                _native.resampler_taps(rate)
+            except ValueError as e:
+                raise ValueError(f"{path}: {e}") from None
+        return np.frombuffer(f.readframes(f.getnframes()), dtype=np.int16), rate
 
 
-def _read_wavs(paths, n_threads=1):
+def _read_wav(path):
+    pcm, rate = _read_wav_rate(path)
+    if rate != 16000:
+        raise ValueError(f"{path}: expected 16-bit, 16 khz, single-channel WAV")
+    return pcm
+
+
+def _read_wavs(paths, n_threads=1, reader=_read_wav):
     """RIFF parsing is I/O bound: read the files on ``n_threads`` host threads, keep the order."""
     if n_threads <= 1 or len(paths) < 2:
-        return [_read_wav(p) for p in paths]
+        return [reader(p) for p in paths]
     from concurrent.futures import ThreadPoolExecutor
     with ThreadPoolExecutor(max_workers=int(n_threads)) as pool:
-        return list(pool.map(_read_wav, paths))
+        return list(pool.map(reader, paths))
 
 
 def compute_features_from_generator(generator, n_total, clip_duration, output_file, device="gpu", ncpu=1,
-                                    audio_features=None):
+                                    audio_features=None, sr=16000):
     """Reference signature (utils.py:542-601): pull int16 batches ``[batch, clip_duration]`` from ``generator``,
     embed them (``AudioFeatures.embed_clips``, one device call per batch) and write float32
     ``[n, (T-76)//8+1, 96]`` to the ``.npy`` file ``output_file`` through a memmap, so the result may exceed host
     memory.  ``n_total`` may over-estimate the number of clips: the file is cut to the rows actually written (the
     reference trims trailing all-zero rows with ``data.trim_mmap`` - same result unless a clip embeds to exactly
     zero).  ``device``/``ncpu`` are accepted for signature compatibility; the work runs on the GPU.
-    ``audio_features`` lets a caller reuse an existing ``AudioFeatures`` (weights already on the device)."""
+    ``audio_features`` lets a caller reuse an existing ``AudioFeatures`` (weights already on the device).  ``sr``: the
+    generator's rate; ``clip_duration`` counts its samples, and T those of the clip resampled to 16 kHz on the device."""
     from numpy.lib.format import open_memmap
     F = audio_features if audio_features is not None else AudioFeatures(device=device)
-    n_windows, dim = F.get_embedding_shape(clip_duration / 16000)
+    n16 = clip_duration if int(sr) == 16000 else _native.resample_clip_plan(int(sr), int(clip_duration), 0)
+    n_windows, dim = F.get_embedding_shape(n16 / 16000)
     if n_windows < 1:
         raise ValueError("clip_duration is too short for one 76-frame embedding window")
     n_total = int(n_total)
@@ -568,7 +613,8 @@ def compute_features_from_generator(generator, n_total, clip_duration, output_fi
                              " Please increase 'n_total' to be >= batch size.")
         if rows >= n_total:
             break
-        feats = F.embed_clips(audio, batch_size=audio.shape[0], ncpu=ncpu)[: n_total - rows]
+        kw = {} if int(sr) == 16000 else {"sr": int(sr)}
+        feats = F.embed_clips(audio, batch_size=audio.shape[0], ncpu=ncpu, **kw)[: n_total - rows]
         fp[rows:rows + feats.shape[0]] = feats
         rows += feats.shape[0]
         fp.flush()
@@ -611,24 +657,35 @@ def bulk_predict(file_paths, wakeword_models, prediction_function="predict_clip"
     per batch of about BULK_STAGING_BYTES of audio (Model.predict_clips_ragged).  As in the reference, keyword arguments
     go to the Model constructor and to the prediction function where they name one of its parameters, and are dropped
     otherwise.  ``prediction_function``: "predict_clip" (``padding``, ``chunk_size``) or
-    "_get_positive_prediction_frames" (``threshold``, ``return_type``).  Returns {path: result of the function}."""
+    "_get_positive_prediction_frames" (``threshold``, ``return_type``).  Returns {path: result of the function}.
+    Files are 16-bit single-channel WAVs at any rate of the resampler's table, mixed freely; each is read at its
+    header's rate and resampled to 16 kHz on the device (one launch per batch; none for a batch of 16 kHz files).  An
+    ``sr`` keyword is checked against every header and is not passed to the Model."""
     from .model import Model, _rows_to_dicts
     if prediction_function not in ("predict_clip", "_get_positive_prediction_frames"):
         raise ValueError("the b200 bulk path implements prediction_function='predict_clip' and "
                          "'_get_positive_prediction_frames'")
     import inspect
     init_names = set(inspect.signature(Model.__init__).parameters) | set(inspect.signature(AudioFeatures.__init__).parameters)
-    init_kw = {k: v for k, v in kwargs.items() if k in init_names}
+    init_kw = {k: v for k, v in kwargs.items() if k in init_names and k != "sr"}
     fn_names = set(inspect.signature(getattr(Model, prediction_function)).parameters) - {"self", "kwargs"}
     fn_kw = {k: v for k, v in kwargs.items() if k in fn_names}
+    sr = kwargs.get("sr")
     mdl = Model(wakeword_models=wakeword_models, inference_framework=inference_framework, **init_kw)
     torch = _torch()
     out = {}
     for paths in _wav_batches(list(file_paths), BULK_STAGING_BYTES):
-        clips = _read_wavs(paths, ncpu)                        # RIFF parsing on ncpu host threads, order kept
+        read = _read_wavs(paths, ncpu, _read_wav_rate)        # RIFF parsing on ncpu host threads, order kept
+        clips = [c for c, _ in read]
+        rates = np.array([r for _, r in read], np.int32)
+        if sr is not None:
+            for p, r in zip(paths, rates):
+                if r != int(sr):
+                    raise ValueError(f"{p}: the header says {r} Hz, sr={sr}")
+        rates = None if (rates == 16000).all() else rates      # 16 kHz batches run exactly as before
         if prediction_function == "_get_positive_prediction_frames":
             res = mdl._positive_frames_bulk(clips, threshold=fn_kw.get("threshold", 0.5),
-                                            return_type=fn_kw.get("return_type", "features"))
+                                            return_type=fn_kw.get("return_type", "features"), sr=rates)
             out.update(zip(paths, res))
             continue
         # the batch is gathered in page-locked memory so the H2D copy is a single asynchronous DMA (the reference forks
@@ -639,6 +696,6 @@ def bulk_predict(file_paths, wakeword_models, prediction_function="predict_clip"
         for c, o in zip(clips, offsets):
             view[o:o + c.shape[0]] = c
         scores, row_off, labels = mdl.predict_clips_ragged(stage, offsets, padding=fn_kw.get("padding", 1),
-                                                           chunk_size=fn_kw.get("chunk_size", CHUNK))
+                                                           chunk_size=fn_kw.get("chunk_size", CHUNK), sr=rates)
         out.update(zip(paths, _rows_to_dicts(scores, row_off, labels)))
     return out
