@@ -323,6 +323,7 @@ struct TcBlkArgs {
     int n, W, rows_new;                     // streams, real width, output rows per stream
     int m_valid, tap;                       // accumulator rows that are positions of the block; unit distance of the taps
     int pool_f;                             // 2: (1,2) max-pool fused into the epilogue (columns f, f^1 sit in adjacent lanes); 0: none
+    int pool_t;                             // 2 (with pool_f 2): (2,2) max-pool; rows t = 0, 1 sit in the two warpgroups (S*W = 64)
     int cg_in, cg_out, apply_act, n_tiles;
     float* out_f32;                         // final layer: [n][rows_new][96]
     __half* out[3]; int out_toff[3];        // destination buffers (this step / later steps' tails) and their row offsets
@@ -342,6 +343,7 @@ __global__ void __launch_bounds__(kTcThreads, 1) tc_conv_blk_kernel(TcBlkArgs a)
     uint64_t* bars = reinterpret_cast<uint64_t*>(a_smem + 2 * half_bytes);
     // bars: full[2], empty[2], w_full
     float* s_sb = reinterpret_cast<float*>(bars + 6);
+    float* s_x = s_sb + 2 * NP;                                            // (2,2) pool: [NP/2][64] row-1 maxima
     for (int i = threadIdx.x; i < NP; i += kTcThreads) { s_sb[i] = a.scale[i]; s_sb[NP + i] = a.bias[i]; }
 
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
@@ -433,6 +435,63 @@ __global__ void __launch_bounds__(kTcThreads, 1) tc_conv_blk_kernel(TcBlkArgs a)
                 if (lane == 0) mbar_arrive(empty_bar(h));
             }
             phase ^= 1;
+
+            if (a.pool_t == 2) {
+                // (2,2) max-pool in the epilogue: columns f, f^1 are lanes 4 apart (shuffle), rows t = 0 and 1 are the
+                // same fragment position in warpgroups 0 and 1 (S*W = 64 accumulator rows apart).  Warpgroup 1 leaves
+                // its column maxima in shared memory; warpgroup 0 takes the maximum of the four fp32 values, splits it
+                // into hi / lo and stores pooled row 0.  That is the element the lexicographic (hi, lo) maximum of
+                // tc_pool_kernel picks.  Writers: the even columns, (lane >> 2) even (W is even).
+                const bool fw = ((lane >> 2) & 1) == 0;
+                const int ci = wq * 16 + (lane >> 3) * 4 + (lane & 3);
+#pragma unroll
+                for (int i = 0; i < 2; ++i)
+#pragma unroll
+                    for (int j = 0; j < NP / 8; ++j) {
+                        const int c = j * 8 + 2 * q;
+                        float y0 = fmaf(acc[4 * j + 2 * i], s_sb[c], s_sb[NP + c]);
+                        float y1 = fmaf(acc[4 * j + 2 * i + 1], s_sb[c + 1], s_sb[NP + c + 1]);
+                        if (a.apply_act) { y0 = act(y0); y1 = act(y1); }
+                        acc[4 * j + 2 * i] = fmaxf(y0, __shfl_xor_sync(0xffffffffu, y0, 4));
+                        acc[4 * j + 2 * i + 1] = fmaxf(y1, __shfl_xor_sync(0xffffffffu, y1, 4));
+                    }
+                if (wg == 1 && fw) {
+#pragma unroll
+                    for (int k = 0; k < NP / 2; ++k) s_x[k * 64 + ci] = acc[k];
+                }
+                named_bar_sync(1, 256);
+                if (wg == 0 && fw) {
+#pragma unroll
+                    for (int i = 0; i < 2; ++i) {
+                        const int sl = slr[i], fo = fr[i] >> 1;
+                        const int n = tile * a.lay.S + sl;
+                        if (!okr[i] || n >= a.n) continue;
+                        uint4* dst[3];
+#pragma unroll
+                        for (int kk = 0; kk < 3; ++kk)
+                            dst[kk] = a.out[kk] && a.out_toff[kk] >= 0
+                                          ? reinterpret_cast<uint4*>(a.out[kk]) + late_unit(a.out_lay, 0, n, a.out_toff[kk], fo) : nullptr;
+#pragma unroll
+                        for (int j = 0; j < NP / 8; ++j) {
+                            if (j >= a.cg_out) break;
+                            const float y0 = fmaxf(acc[4 * j + 2 * i], s_x[(4 * j + 2 * i) * 64 + ci]);
+                            const float y1 = fmaxf(acc[4 * j + 2 * i + 1], s_x[(4 * j + 2 * i + 1) * 64 + ci]);
+                            const __half h0 = __float2half_rn(y0), h1 = __float2half_rn(y1);
+                            const __half2 hh = __halves2half2(h0, h1);
+                            const __half2 ll = __floats2half2_rn(y0 - __half2float(h0), y1 - __half2float(h1));
+                            const uint32_t hw = *reinterpret_cast<const uint32_t*>(&hh), lw = *reinterpret_cast<const uint32_t*>(&ll);
+#pragma unroll
+                            for (int kk = 0; kk < 3; ++kk)
+                                if (dst[kk]) {
+                                    reinterpret_cast<uint32_t*>(dst[kk] + (int64_t)j * a.out_lay.units)[q] = hw;
+                                    reinterpret_cast<uint32_t*>(dst[kk] + (int64_t)(a.cg_out + j) * a.out_lay.units)[q] = lw;
+                                }
+                        }
+                    }
+                }
+                named_bar_sync(2, 256);                                 // s_x is free for the next tile
+                continue;
+            }
 
 #pragma unroll
             for (int i = 0; i < 2; ++i) {
@@ -596,7 +655,8 @@ int launch_tc(oww_ctx* ctx, const TcConvArgs& a, cudaStream_t s) {
 
 template <int CGP, int NP>
 int launch_tc_blk(oww_ctx* ctx, const TcBlkArgs& a, cudaStream_t s) {
-    const size_t smem = (size_t)2 * 3 * CGP * NP * 16 + (size_t)2 * CGP * a.lay.units * 16 + 8 * 6 + 2 * NP * sizeof(float);
+    const size_t smem = (size_t)2 * 3 * CGP * NP * 16 + (size_t)2 * CGP * a.lay.units * 16 + 8 * 6 + 2 * NP * sizeof(float) +
+                        (a.pool_t == 2 ? (size_t)NP / 2 * 64 * sizeof(float) : 0);
     if (smem > 227 * 1024) return oww_fail(ctx, OWW_EUNSUPPORTED, "blocked late conv tile does not fit shared memory (%zu bytes)", smem);
     const uint32_t bit = 1u << (CGP / 2 + NP / 16);                    // distinct for the instances in use
     if (!(ctx->tc_blk_attr_mask & bit)) {
@@ -813,6 +873,15 @@ int oww_cnn_tc_pyramid_impl(oww_ctx* ctx, const WindowSrc& src, int n, int T0, i
 // ================================================================================================
 namespace {
 
+// Is conv layer l's pool fused into its tc_conv_blk_kernel epilogue (no unpooled temp, no tc_pool_kernel launch)?
+// (1,2): columns f, f^1 are adjacent accumulator rows.  (2,2) with two output rows: additionally rows 0 and 1 are the
+// two warpgroups' halves of the 128 accumulator rows (S*W = 64) - layer 18 at split_from 11 / 15.
+int late_fused_pool_t(const ConvLayer& C, const LateLay& X, int rows, int W, bool last) {
+    if (last || !C.pool_t || C.pool_f != 2 || !X.kh3 || (W & 1)) return 0;
+    if (C.pool_t == 1) return 1;
+    return C.pool_t == 2 && rows == 2 && X.S * W == 64 ? 2 : 0;
+}
+
 __global__ void late_capture_kernel(const uint4* planes, int64_t plane_pitch, int T, int Wp, int n_planes, uint4* tmpl) {
     // last two rows of window 0 of every plane -> tmpl[plane][row][f]
     const int total = n_planes * 2 * Wp;
@@ -861,8 +930,10 @@ int oww_late_alloc(oww_ctx* ctx) {
             OWW_CUDA(ctx, cudaMemset(X.buf[k], 0, buf_units * 16));
         }
         if (C.pool_t) {
-            const size_t u = (size_t)2 * (C.cout / 8) * ((kGuard + (size_t)n * rows * (W + 1) + kGuardBack + 7) & ~(size_t)7);
-            if (u > tmp_units) tmp_units = u;
+            if (!late_fused_pool_t(C, Y, rows, W, l == OWW_N_CONV - 1)) {       // unpooled temp of a separate pool launch
+                const size_t u = (size_t)2 * (C.cout / 8) * ((kGuard + (size_t)n * rows * (W + 1) + kGuardBack + 7) & ~(size_t)7);
+                if (u > tmp_units) tmp_units = u;
+            }
             rows /= C.pool_t; W /= C.pool_f;
         }
     }
@@ -910,8 +981,9 @@ int oww_late_chain(oww_ctx* ctx, float* d_emb, cudaStream_t s) {
         b.tap = C.kh == 3 ? X.lay.S * W : 1;
         b.cg_in = cg; b.cg_out = C.cout / 8; b.apply_act = last ? 0 : 1;
         b.n_tiles = (n + X.lay.S - 1) / X.lay.S;
-        // (1,2) max-pool in the epilogue: straight into the next layer's tensor, no temp, no pool launch
-        const bool fuse_pool = !last && C.pool_t == 1 && C.pool_f == 2 && X.lay.kh3 && (W & 1) == 0;
+        // (1,2) / (2,2) max-pool in the epilogue: straight into the next layer's tensor, no temp, no pool launch
+        const int fused_pool_t = late_fused_pool_t(C, X.lay, T_out, W, last);
+        const bool fuse_pool = fused_pool_t != 0;
         if (last) {
             b.out_f32 = d_emb;
         } else if (C.pool_t && !fuse_pool) {
@@ -922,6 +994,7 @@ int oww_late_chain(oww_ctx* ctx, float* d_emb, cudaStream_t s) {
             route(Y, b.out, b.out_toff);
             b.out_lay = Y.lay;
             b.pool_f = fuse_pool ? 2 : 0;
+            b.pool_t = fused_pool_t == 2 ? 2 : 0;
         }
         int rc;
         if (cgp == 4 && np == 48) rc = launch_tc_blk<4, 48>(ctx, b, s);

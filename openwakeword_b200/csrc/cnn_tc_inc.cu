@@ -50,8 +50,8 @@ struct IncArgs {
     // does not is a dead slot (no state, ring or score write) and its tails are carried by the caller
     const int* live_chunks; int live_min;
     long long* dbg_clock;                                     // optional: 21 clock64 stamps of CTA 0's first group
-    // ---- fused step (fused != 0): the same launch also runs the log-mel frontend before layer 0, appends the embedding
-    //      to the feature ring and evaluates every head, i.e. PCM in -> scores out ----
+    // ---- fused step (fused != 0, full-depth instance only): the same launch also runs the log-mel frontend before
+    //      layer 0, appends the embedding to the feature ring and evaluates every head, i.e. PCM in -> scores out ----
     int fused;
     const int16_t* pcm; int64_t pcm_stride;                   // this step's 1280 samples per stream
     int16_t* tail; int* seen; float* mel_rw; int* mel_count_rw;
@@ -75,11 +75,14 @@ __device__ __forceinline__ int head_rows(int slot_bytes, int K, int D) {
 // kNL: number of conv layers the kernel runs, fixed at compile time (20 = whole CNN, 11 / 15 = cuts before the
 // split-operand layers) or 0 = read from the plan (any other cut).  With the count known the full-depth instance
 // carries none of the cut layer's code.
+// A cut instance (kNL != 20) has no frontend phase: its step launches the frontend kernel (mel.cu) first and layer 0
+// reads all ten input rows from the mel ring.
 template <int kNL>
 __global__ void __launch_bounds__(kIncThreads, 1) tc_inc_kernel(const __grid_constant__ IncArgs a) {
     extern __shared__ __align__(128) uint8_t smem[];
     const IncPlan& P = a.plan;
     const int NL = kNL ? kNL : P.n_layers;
+    const bool fused = kNL == OWW_N_CONV && a.fused;
     const int G = P.G;
     // [0, 2048): barriers, per-group stream state, layer-0 weights.  Activations grow from 2048 up; the per-layer weight
     // slots sit at the top of the arena (offsets in the plan, checked against the activation extents).
@@ -113,6 +116,9 @@ __global__ void __launch_bounds__(kIncThreads, 1) tc_inc_kernel(const __grid_con
         bulk_g2s(smem_u32(smem + P.L[l].w_smem), a.wblob + P.L[l].w_off, (uint32_t)P.L[l].w_bytes, wfull(l & 1));
     };
     if (threadIdx.x == 0 && (int)blockIdx.x < P.n_groups) { load_weights(1); load_weights(2); }
+    // dependent launch behind the frontend kernel: the prologue above (barriers, layer-0 weights, the bulk copies of
+    // layers 1 / 2) ran beside the frontend's tail; everything below reads or writes step state (no-op otherwise)
+    pdl_wait();
 
     // Heads ring: thread 0 streams every head's weights, in consumption order, through hns slots of hslot_bytes.  Cursor
     // of the next chunk to issue: head, layer, first row (a feature row of the first layer, a weight row of a later one).
@@ -159,7 +165,7 @@ __global__ void __launch_bounds__(kIncThreads, 1) tc_inc_kernel(const __grid_con
             s_live[et] = b < a.B && (!a.live_chunks || a.live_chunks[b] >= a.live_min);
         }
         named_bar_sync(2, kIncEpiWarps * 32);
-        if (a.fused) {
+        if (fused) {
             // ===== frontend: log-mel of this step's 8 frames per stream (K1 inside the step kernel) =====
             uint8_t* sc = smem + P.scratch_off;
             float2* s_tw = reinterpret_cast<float2*>(sc);
@@ -298,11 +304,11 @@ __global__ void __launch_bounds__(kIncThreads, 1) tc_inc_kernel(const __grid_con
                     }
                     const float* base = a.mel + (int64_t)b * a.mel_stride;
                     // rows 0..9 of the input = two rows from before this step + the eight new ones
-                    const int row0 = (a.fused ? s_cnt[g] - 2 : a.mel_count[b] - a.back - 10) + t;     // fused: the two rows before this step's
+                    const int row0 = (fused ? s_cnt[g] - 2 : a.mel_count[b] - a.back - 10) + t;     // fused: the two rows before this step's
                     float x[3][4];                               // mel rows t..t+2, columns f0-1..f0+2
 #pragma unroll
                     for (int dt = 0; dt < 3; ++dt) {
-                        const float* rp = (a.fused && t + dt >= 2) ? s_mel + (g * 8 + t + dt - 2) * 32
+                        const float* rp = (fused && t + dt >= 2) ? s_mel + (g * 8 + t + dt - 2) * 32
                                                                    : base + (int64_t)((row0 + dt) & a.mel_mask) * 32;
 #pragma unroll
                         for (int i = 0; i < 4; ++i) {
@@ -431,7 +437,7 @@ __global__ void __launch_bounds__(kIncThreads, 1) tc_inc_kernel(const __grid_con
                         const bool live = s_live[g] != 0;
                         if constexpr (kFinal) {
                             if (f != 0 || !live) continue;
-                            float* o = a.fused ? a.feat_ring + (int64_t)(grp * G + g) * a.feat_stride + (int64_t)(s_cnt[8 + g] & a.feat_mask) * 96
+                            float* o = fused ? a.feat_ring + (int64_t)(grp * G + g) * a.feat_stride + (int64_t)(s_cnt[8 + g] & a.feat_mask) * 96
                                                : a.emb + (int64_t)(grp * G + g) * 96;
 #pragma unroll
                             for (int j = 0; j < NP / 8; ++j) {
@@ -596,7 +602,7 @@ __global__ void __launch_bounds__(kIncThreads, 1) tc_inc_kernel(const __grid_con
             }
         }
         if (a.dbg_clock && blockIdx.x == 0 && grp == 0 && et == 0) a.dbg_clock[OWW_N_CONV] = clock64();
-        if (a.fused && NL == OWW_N_CONV) {
+        if (fused) {
             // ===== K3 inside the step kernel: every head on this group's streams, straight from the feature ring =====
             named_bar_sync(2, kIncEpiWarps * 32);              // the new embedding rows (written by this CTA) are visible
             if (a.n_heads > 0) {                               // n_heads == 0: the heads run as their own launch after this one
@@ -928,9 +934,10 @@ int oww_inc_build_plan(oww_ctx* ctx, int G, int n_streams, int n_layers, IncPlan
             return oww_fail(ctx, OWW_EUNSUPPORTED, "fused-CNN smem plan does not fit at layer %d (G=%d)", l, G);
         if (l >= 2 && wsz(l) < wsz(l - 1)) return oww_fail(ctx, OWW_EUNSUPPORTED, "weight sizes must not shrink with depth");
     }
-    // frontend of the fused step: FFT work buffers at the arena base (dead before layer 0 writes its output there);
-    // twiddles 4 KB | window 2 KB | G x 8 x 32 mel rows | G floors sit above both, below the weight slots of layers 1-2
-    {
+    // frontend of the fused step (full depth only; a cut plan's step runs the frontend kernel): FFT work buffers at the
+    // arena base (dead before layer 0 writes its output there); twiddles 4 KB | window 2 KB | G x 8 x 32 mel rows | G
+    // floors sit above both, below the weight slots of layers 1-2
+    if (NL == OWW_N_CONV) {
         int off = kActBase + r8(size_nx[0]) * 16;
         const int work_end = kActBase + kIncEpiWarps * kMelNF * kMelFrameScratch;
         if (work_end > off) off = (work_end + 127) & ~127;
@@ -1045,8 +1052,10 @@ int oww_heads_sync_devs(oww_ctx* ctx) {
 }
 
 // Can the frontend + CNN + ring append of a one-chunk step run as the fused launch?
+// (A cut plan always can: its frontend is a launch of its own.)
 bool oww_fused_frontend_supported(const oww_ctx* ctx) {
-    return ctx->fuse_step && ctx->cfg.cnn_mode == OWW_CNN_TC_INCREMENTAL && ctx->inc_plan.scratch_off != 0;
+    return ctx->fuse_step && ctx->cfg.cnn_mode == OWW_CNN_TC_INCREMENTAL &&
+           (ctx->inc_plan.n_layers < OWW_N_CONV || ctx->inc_plan.scratch_off != 0);
 }
 
 // Can the heads run inside that launch too?  (heads within the in-kernel limits; worthwhile only while re-streaming the
@@ -1071,11 +1080,12 @@ bool oww_fused_heads_supported(const oww_ctx* ctx) {
     return 2048 + floats * 4 + 128 + (size_t)96 * d1max * 4 <= (size_t)ctx->inc_plan.L[2].w_smem;
 }
 
-static void launch_inc(const IncArgs& a, int grid, cudaStream_t s) {
-    if (a.plan.n_layers == OWW_N_CONV) tc_inc_kernel<OWW_N_CONV><<<grid, kIncThreads, a.plan.smem_bytes, s>>>(a);
-    else if (a.plan.n_layers == 11) tc_inc_kernel<11><<<grid, kIncThreads, a.plan.smem_bytes, s>>>(a);
-    else if (a.plan.n_layers == 15) tc_inc_kernel<15><<<grid, kIncThreads, a.plan.smem_bytes, s>>>(a);
-    else tc_inc_kernel<0><<<grid, kIncThreads, a.plan.smem_bytes, s>>>(a);
+static cudaError_t launch_inc(const IncArgs& a, int grid, cudaStream_t s, bool pdl = false) {
+    void (*k)(IncArgs) = a.plan.n_layers == OWW_N_CONV ? tc_inc_kernel<OWW_N_CONV>
+                       : a.plan.n_layers == 11         ? tc_inc_kernel<11>
+                       : a.plan.n_layers == 15         ? tc_inc_kernel<15>
+                                                       : tc_inc_kernel<0>;
+    return oww_launch_pdl(pdl, k, dim3(grid), dim3(kIncThreads), (size_t)a.plan.smem_bytes, s, a);
 }
 
 static void fill_inc_args(oww_ctx* ctx, IncArgs& a) {
@@ -1095,13 +1105,28 @@ static void fill_inc_args(oww_ctx* ctx, IncArgs& a) {
     }
 }
 
-// One launch per step: frontend, 20-layer CNN and ring append for every stream, plus - with_heads - every head and
-// the verifier gates, i.e. PCM in -> scores out.
+// Full depth: one launch per step - frontend, 20-layer CNN and ring append for every stream, plus - with_heads - every
+// head and the verifier gates, i.e. PCM in -> scores out.
+// Cut plan (split_from < 20): the frontend kernel (mel.cu), then the kernel's layers 0 .. split_from-1 on the ring rows it
+// wrote, the second as a dependent launch of the first, and the first of the previous step's last launch; the late
+// chain follows (caller).
 int oww_fused_step(oww_ctx* ctx, const int16_t* d_pcm, int64_t pcm_stride, float* d_scores, int out_stride, bool with_heads,
                    cudaStream_t s, const int* d_chunks, int min_chunks) {
     IncArgs a;
     fill_inc_args(ctx, a);
     a.live_chunks = d_chunks; a.live_min = min_chunks;
+    const int grid = a.plan.n_groups < ctx->sm_count ? a.plan.n_groups : ctx->sm_count;
+    if (a.plan.n_layers < OWW_N_CONV) {
+        MelLaunch m{d_pcm, pcm_stride, OWW_SAMPLES_PER_CHUNK, ctx->d_tail, ctx->d_seen, ctx->d_mel_ring,
+                    (int64_t)ctx->mel_rows * 32, ctx->mel_rows - 1, ctx->d_mel_count, ctx->n_streams, 1, 1};
+        m.live = d_chunks; m.live_min = min_chunks; m.pdl = ctx->late_pdl;
+        int rc = oww_mel_launch(ctx, m, s);
+        if (rc) return rc;
+        OWW_CUDA(ctx, launch_inc(a, grid, s, ctx->late_pdl));
+        OWW_LAUNCH_CHECK(ctx);
+        ctx->inc_cur ^= 1;
+        return OWW_OK;
+    }
     a.fused = 1;
     a.pcm = d_pcm; a.pcm_stride = pcm_stride;
     a.tail = ctx->d_tail; a.seen = ctx->d_seen; a.mel_rw = ctx->d_mel_ring; a.mel_count_rw = ctx->d_mel_count;
@@ -1124,8 +1149,7 @@ int oww_fused_step(oww_ctx* ctx, const int16_t* d_pcm, int64_t pcm_stride, float
         if (a.hns > 4) a.hns = 4;
         if (a.hns < 1 && !ctx->heads.empty()) return oww_fail(ctx, OWW_EUNSUPPORTED, "no room for the fused heads weight ring");
     }
-    const int grid = a.plan.n_groups < ctx->sm_count ? a.plan.n_groups : ctx->sm_count;
-    launch_inc(a, grid, s);
+    OWW_CUDA(ctx, launch_inc(a, grid, s));
     OWW_LAUNCH_CHECK(ctx);
     ctx->inc_cur ^= 1;
     return OWW_OK;
@@ -1139,7 +1163,7 @@ int oww_cnn_inc_step(oww_ctx* ctx, int back, float* d_emb, cudaStream_t s, const
     a.back = back;
     a.emb = d_emb;
     const int grid = a.plan.n_groups < ctx->sm_count ? a.plan.n_groups : ctx->sm_count;
-    launch_inc(a, grid, s);
+    OWW_CUDA(ctx, launch_inc(a, grid, s));
     OWW_LAUNCH_CHECK(ctx);
     ctx->inc_cur ^= 1;
     if (ctx->late_active) return oww_late_chain(ctx, d_emb, s);

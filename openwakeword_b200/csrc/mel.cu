@@ -11,7 +11,17 @@
 // the bins the filterbank touches.  One CTA owns one call of one stream, so the per-call dB
 // maximum (SURVEY.md F7) is a block reduction; the CTA also advances the stream's PCM tail and mel
 // ring, so the whole frontend is one launch with no host round trip.
+//
+// The frame routine is mel_frames_db (mel_device.cuh), the one the full-depth fused step kernel runs, so rows are
+// bit-identical between the two.  A CTA takes 4 KB of work buffer per warp plus the 6 KB twiddle / window tables, so
+// five CTAs (40 warps) share an SM: the one-chunk step's frontend (8 frames per stream) runs as a single launch at
+// that occupancy instead of on the 16 warps of the step kernel.
+// Dependent launch (MelLaunch::pdl): every CTA lets its successor start at once, computes its frames, and only then
+// waits for the predecessor grid before its first store.  What it reads before that wait - PCM, PCM tail, `seen`,
+// the ring count - is written only by kernels that are complete by then: the previous frontend, reset and import
+// kernels all finish before the step kernel that follows them (launched without an early trigger) ends.
 #include "oww_internal.h"
+#include "tc_common.cuh"
 #include "mel_device.cuh"
 #include <climits>
 #include <cmath>
@@ -31,24 +41,31 @@ struct MelDev {
     int kmax;
 };
 
-__global__ void __launch_bounds__(kThreads) mel_kernel(MelLaunch p, MelDev c) {
-    __shared__ float2 s_buf[kWarps][2][256];
+__global__ void __launch_bounds__(kThreads, 5) mel_kernel(MelLaunch p, MelDev c) {
+    __shared__ __align__(16) uint8_t s_work[kWarps][kMelFrameScratch];
     __shared__ float2 s_tw[512];
     __shared__ float s_win[512];
-    __shared__ float s_pow[kWarps][264];
     __shared__ float s_red[kWarps];
 
+    pdl_trigger();
     const int clip = p.ids ? p.ids[blockIdx.x] : blockIdx.x;
     const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+    if (p.live && p.live[clip] < p.live_min) {       // dead slot of a ragged step: no trace
+        pdl_wait();
+        return;
+    }
 
     for (int i = tid; i < 512; i += kThreads) { s_tw[i] = c.twiddle[i]; s_win[i] = c.window[i]; }
 
     const bool streaming = p.tail != nullptr;
     const int prefix = streaming ? OWW_TAIL : 0;
-    const bool fresh = streaming && p.seen[clip] == 0;
+    const int seen0 = streaming ? p.seen[clip] : 0;
+    const bool fresh = streaming && seen0 == 0;
     const int total = prefix + p.n_body;
     const int T = (total - OWW_FFT_N) / OWW_HOP + 1;
     const int f0 = fresh ? 3 : 0;                 // frames 0..2 would read the (absent) prefix
+    const int nrows = T - f0;
+    const bool one_pass = nrows <= kWarps;        // every frame's row stays in a register until the clamp
     const int16_t* body = p.body + (int64_t)clip * p.body_stride;
     const int16_t* tail = streaming ? p.tail + (int64_t)clip * OWW_TAIL : nullptr;
     const int row0 = p.out_count ? p.out_count[clip] : 0;
@@ -58,42 +75,60 @@ __global__ void __launch_bounds__(kThreads) mel_kernel(MelLaunch p, MelDev c) {
     const int my_start = c.mel_start[lane];
     const int my_len = c.mel_len[lane];
     const float* my_w = c.mel_w + lane * OWW_MEL_MAXSUPPORT;
-    float vmax = -INFINITY;
+    float vmax = -INFINITY, kept = 0.f;
 
     for (int f = f0 + warp; f < T; f += kWarps) {
-        const float db = mel_frame_db(tail, prefix, body, f, s_buf[warp][0], s_buf[warp][1], s_pow[warp], s_tw, s_win, c.kmax,
-                                      my_start, my_len, my_w, lane);
+        float db;
+        mel_frames_db<1>(&tail, prefix, &body, &f, s_work[warp], s_tw, s_win, c.kmax, my_start, my_len, my_w, lane, &db);
         vmax = fmaxf(vmax, db);
+        if (one_pass) { kept = db; continue; }
+        pdl_wait();
         const int r = f - f0;
         const int slot = p.out_rows_mask >= 0 ? ((row0 + r) & p.out_rows_mask) : r;
         out[(int64_t)slot * OWW_MEL_BINS + lane] = db;
-        __syncwarp();
     }
     // per-call maximum -> clamp -> affine
 #pragma unroll
     for (int o = 16; o > 0; o >>= 1) vmax = fmaxf(vmax, __shfl_xor_sync(0xffffffffu, vmax, o));
     if (lane == 0) s_red[warp] = vmax;
-    __syncthreads();
+    __syncthreads();                              // also: every frame has read the old tail
     float m = s_red[0];
 #pragma unroll
     for (int w = 1; w < kWarps; ++w) m = fmaxf(m, s_red[w]);
     const float floor_db = m - 80.0f;
-    const int nrows = T - f0;
-    for (int i = tid; i < nrows * OWW_MEL_BINS; i += kThreads) {
-        const int r = i >> 5, col = i & 31;
-        const int slot = p.out_rows_mask >= 0 ? ((row0 + r) & p.out_rows_mask) : r;
-        float* q = out + (int64_t)slot * OWW_MEL_BINS + col;
-        float v = fmaxf(__ldcg(q), floor_db);
-        if (p.affine) v = v / 10.0f + 2.0f;
-        *q = v;
+    // the stream's new tail = the last 480 samples of this call: loaded now, stored behind the wait
+    int16_t tv[(OWW_TAIL + kThreads - 1) / kThreads];
+#pragma unroll
+    for (int u = 0; u < (OWW_TAIL + kThreads - 1) / kThreads; ++u) {
+        const int i = tid + u * kThreads;
+        tv[u] = streaming && i < OWW_TAIL ? __ldg(body + (p.n_body - OWW_TAIL + i)) : (int16_t)0;
+    }
+    pdl_wait();
+    if (one_pass) {
+        if (warp < nrows) {
+            float v = fmaxf(kept, floor_db);
+            if (p.affine) v = v / 10.0f + 2.0f;
+            const int slot = p.out_rows_mask >= 0 ? ((row0 + warp) & p.out_rows_mask) : warp;
+            out[(int64_t)slot * OWW_MEL_BINS + lane] = v;
+        }
+    } else {
+        for (int i = tid; i < nrows * OWW_MEL_BINS; i += kThreads) {
+            const int r = i >> 5, col = i & 31;
+            const int slot = p.out_rows_mask >= 0 ? ((row0 + r) & p.out_rows_mask) : r;
+            float* q = out + (int64_t)slot * OWW_MEL_BINS + col;
+            float v = fmaxf(__ldcg(q), floor_db);
+            if (p.affine) v = v / 10.0f + 2.0f;
+            *q = v;
+        }
     }
     if (streaming) {
-        __syncthreads();                       // every frame has read the old tail
         int16_t* tw = p.tail + (int64_t)clip * OWW_TAIL;
-        for (int i = tid; i < OWW_TAIL; i += kThreads) tw[i] = __ldg(body + (p.n_body - OWW_TAIL + i));
+#pragma unroll
+        for (int u = 0; u < (OWW_TAIL + kThreads - 1) / kThreads; ++u)
+            if (tid + u * kThreads < OWW_TAIL) tw[tid + u * kThreads] = tv[u];
         if (tid == 0) {
             p.out_count[clip] = oww_wrap_count(row0 + nrows);
-            const int sn = p.seen[clip] + p.n_chunks;
+            const int sn = seen0 + p.n_chunks;
             p.seen[clip] = sn > (1 << 30) ? (1 << 30) : sn;
         }
     }
@@ -188,7 +223,7 @@ int oww_mel_launch(oww_ctx* ctx, const MelLaunch& p, cudaStream_t s) {
     if (prefix + p.n_body < OWW_FFT_N) return oww_fail(ctx, OWW_EINVAL, "clip shorter than 512 samples");
     if (p.n_clips <= 0) return OWW_OK;
     MelDev c{ctx->d_window, ctx->d_twiddle, ctx->d_mel_start, ctx->d_mel_len, ctx->d_mel_w, ctx->mel_kmax};
-    mel_kernel<<<p.n_clips, kThreads, 0, s>>>(p, c);
+    OWW_CUDA(ctx, oww_launch_pdl(p.pdl, mel_kernel, dim3(p.n_clips), dim3(kThreads), 0, s, p, c));
     OWW_LAUNCH_CHECK(ctx);
     return OWW_OK;
 }

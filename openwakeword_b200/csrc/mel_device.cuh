@@ -89,7 +89,8 @@ __device__ __forceinline__ float mel_frame_db(const int16_t* tail, int prefix, c
 // Same arithmetic as mel_frame_db for NF frames at once: the NF instruction streams are interleaved stage by stage, so
 // a lone warp (the fused step kernel runs only 16 of them per SM) has NF independent dependency chains in flight.
 // Frame i: clip pointers tail[i]/body[i], frame index f[i], work buffers bufs + i*kMelFrameScratch bytes laid out as
-// a[256] float2 | b[256] float2 | pw[320] float.  db[i] receives this lane's dB value.
+// a[256] float2 | b[256] float2; the bin powers pw[<= 257] reuse b, which is free once the last FFT pass has read it.
+// db[i] receives this lane's dB value.
 // Index swizzle of the FFT work buffers in mel_frames_db: the radix-4 Stockham stores of the first two passes are strided by
 // 4 and 16 elements (8- and 4-way bank conflicts on 8-byte elements); XOR-ing bits 4..5 of the index into bits 0..1 and 2..3
 // makes every access pattern of the four passes conflict-free per half-warp.  Pure layout: the arithmetic is unchanged.
@@ -104,7 +105,7 @@ __device__ __forceinline__ int fswz(int e) {
 #endif
 }
 
-constexpr int kMelFrameScratch = 2048 + 2048 + 1280;
+constexpr int kMelFrameScratch = 2048 + 2048;
 template <int NF>
 __device__ __forceinline__ void mel_frames_db(const int16_t* const* tail, int prefix, const int16_t* const* body, const int* f,
                                               uint8_t* bufs, const float2* s_tw, const float* s_win, int kmax, int my_start,
@@ -115,7 +116,7 @@ __device__ __forceinline__ void mel_frames_db(const int16_t* const* tail, int pr
     for (int i = 0; i < NF; ++i) {
         a[i] = reinterpret_cast<float2*>(bufs + i * kMelFrameScratch);
         b[i] = a[i] + 256;
-        pw[i] = reinterpret_cast<float*>(b[i] + 256);
+        pw[i] = reinterpret_cast<float*>(b[i]);            // four passes (even): the spectrum ends in a, b is free
     }
     // sample pairs (x[2n], x[2n+1]) never straddle the tail / body boundary (s0 and prefix are even), so each pair is one
     // 32-bit load when the clip is 4-byte aligned (it is for every contiguous int16 batch); all 8 x NF loads are in flight

@@ -398,6 +398,9 @@ struct MelLaunch {
     int* out_count;                // ring row counters or nullptr
     int n_clips; int affine; int n_chunks;
     const int* ids = nullptr;      // streaming only: clip j is stream ids[j] (body / tail / seen / ring rows of that stream)
+    const int* live = nullptr;     // ragged step: stream b takes part iff live[b] >= live_min (otherwise no write at all)
+    int live_min = 0;
+    bool pdl = false;              // dependent launch: the kernel waits for its predecessor only before its first store
 };
 int oww_mel_launch(oww_ctx* ctx, const MelLaunch& p, cudaStream_t s);
 // bulk path: mel rows of whole padded clips, grouped and clamped per streaming call of `chunk` samples, behind 71 rows of
