@@ -362,6 +362,28 @@ int oww_detect(oww_ctx* ctx, const float* d_scores, int prepared_all, const int3
 int oww_detector_export(oww_ctx* ctx, const int32_t* h_stream_ids, int n, float* d_hist, int32_t* d_counts, void* stream);
 int oww_detector_import(oww_ctx* ctx, const int32_t* h_stream_ids, int n, const float* d_hist, const int32_t* d_counts,
                         void* stream);
+/* The same rules over the calls of the bulk clip path (oww_predict_clips_ragged / _streams, oww_predict_clips): what
+ * predict_clip(clip, padding, chunk_size, patience=..., threshold=..., debounce_time=...) returns after a reset, for
+ * every clip at once.  Stateless: it uses neither the handle's detector nor its streams.
+ *   h_labels, n_labels (1..256), debounce_time: as oww_set_detector, checked the same way.
+ *   d_scores [rows][oww_n_outputs]: the raw rows of the clip call; only rows of calls that step a chunk are read.
+ *   h_row_offsets (host int64 [n_clips + 1], 0 first, non-decreasing): clip i's calls are rows [off[i], off[i+1]), in call
+ *     order, each clip from an empty history.  chunk_size: samples per call (>= 1).  Call j of a clip steps k = floor((j+1)
+ *     c / 1280) - floor(j c / 1280) chunks (oww_clip_schedule; d_stepped of the clip call is 1 exactly there), has count
+ *     j and prepared 1280 k samples, or ((j+1) c) mod 1280 when k = 0 - what AudioFeatures._streaming_features returns.
+ *   d_verified (may be NULL) [rows][n_labels]: on a call with k = 0, a label whose entry is not NaN and whose prediction
+ *     (the repeat, or 0.0) is >= verifier_threshold takes that entry instead, before the zeroing of the first five -
+ *     Model.predict re-verifies a repeated prediction on the clip's newest window.
+ *   d_final [rows][n_labels] (may be NULL): the predictions.  d_n_events / d_events / max_events as oww_detect, with the
+ *     events in ascending (clip, label, call) order: `stream` = clip, `index` = call.
+ * Stream-ordered, no synchronisation; two launches, one without d_n_events, none for n_clips 0 (d_n_events is then
+ * set to 0).  The row offsets are staged before the call returns.  OWW_EINVAL before anything is enqueued: the
+ * label checks, null pointers, offsets that do not start at 0 or decrease, chunk_size < 1, and the output checks of
+ * oww_detect.                                                                                                       */
+int oww_detect_clips(oww_ctx* ctx, const oww_detect_label* h_labels, int n_labels, double debounce_time,
+                     const float* d_scores, const float* d_verified, float verifier_threshold, const int64_t* h_row_offsets,
+                     int n_clips, int chunk_size, float* d_final, oww_event* d_events, int max_events, int32_t* d_n_events,
+                     void* stream);
 
 /* ---- stream audio on the device (openwakeword/utils.py:164,403-430: AudioFeatures.raw_data_buffer) ------------------
  * With an audio history of H samples the handle keeps, per stream, the last H samples it stepped (int16 ring) and pos =

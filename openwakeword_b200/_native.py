@@ -89,6 +89,8 @@ _SIGNATURES = {
     "oww_stream_state_status": (C.c_int, [_P, C.POINTER(C.c_int)]),
     "oww_set_detector": (C.c_int, [_P, C.POINTER(DetectLabel), C.c_int, C.c_double]),
     "oww_detect": (C.c_int, [_P, _P, C.c_int, _P, _P, _P, C.c_int, _P, _P]),
+    "oww_detect_clips": (C.c_int, [_P, C.POINTER(DetectLabel), C.c_int, C.c_double, _P, _P, C.c_float, _P, C.c_int, C.c_int,
+                                   _P, _P, C.c_int, _P, _P]),
     "oww_detector_export": (C.c_int, [_P, _P, C.c_int, _P, _P, _P]),
     "oww_detector_import": (C.c_int, [_P, _P, C.c_int, _P, _P, _P]),
     "oww_set_audio_history": (C.c_int, [_P, C.c_int]),
@@ -634,13 +636,17 @@ class Context:
             d.record_stream(ext)
 
     # ---- detections on the device (include/owwb200.h, oww_set_detector) ----
-    def set_detector(self, labels, debounce_time=0.0):
-        """labels: [(column, repeats, threshold or None / NaN, patience)], one per label; [] removes the detector.
-        Synchronises the device.  The same columns and repeats as before keep the histories."""
+    @staticmethod
+    def _label_table(labels):
         arr = (DetectLabel * max(len(labels), 1))()
         for i, (col, rep, thr, pat) in enumerate(labels):
             arr[i] = DetectLabel(int(col), int(bool(rep)), float("nan") if thr is None else float(thr), int(pat))
-        self._check(self.lib.oww_set_detector(self.h, arr, len(labels), float(debounce_time)))
+        return arr
+
+    def set_detector(self, labels, debounce_time=0.0):
+        """labels: [(column, repeats, threshold or None / NaN, patience)], one per label; [] removes the detector.
+        Synchronises the device.  The same columns and repeats as before keep the histories."""
+        self._check(self.lib.oww_set_detector(self.h, self._label_table(labels), len(labels), float(debounce_time)))
         self.n_detect_labels = len(labels)
         self._det_buf = None
 
@@ -654,6 +660,16 @@ class Context:
                 raise ValueError(f"prepared has shape {per.shape}, the handle has {self.n_streams} streams")
         self._check(self.lib.oww_detect(self.h, _ptr(d_scores), all_, _ptr(per), _ptr(d_final), _ptr(d_events),
                                         int(max_events), _ptr(d_n_events), stream))
+
+    def detect_clips(self, labels, debounce_time, d_scores, d_verified, verifier_threshold, row_offsets, chunk_size,
+                     d_final, d_events, max_events, d_n_events, stream=None):
+        """oww_detect_clips: labels as set_detector; row_offsets host int64 [n_clips + 1]; d_verified [rows][n_labels]
+        or None."""
+        off = np.ascontiguousarray(row_offsets, np.int64).ravel()
+        self._check(self.lib.oww_detect_clips(self.h, self._label_table(labels), len(labels), float(debounce_time),
+                                              _ptr(d_scores), _ptr(d_verified), float(verifier_threshold), _ptr(off),
+                                              off.size - 1, int(chunk_size), _ptr(d_final), _ptr(d_events),
+                                              int(max_events), _ptr(d_n_events), stream))
 
     def detector_export(self, stream_ids, d_hist, d_counts, stream=None):
         ids = np.ascontiguousarray(stream_ids, np.int32).ravel()

@@ -44,6 +44,39 @@ static __device__ __forceinline__ int det_wrap(int c) { return c >= OWW_COUNT_WR
 // streams per CTA: whole streams only, so that the one count of a stream is read by all its threads before it is written
 static inline int det_streams_per_cta(int L) { return DET_THREADS / L; }
 
+// The rule of one prediction of one (stream or clip, label), model.py:303-363.  stepped: the call stepped at least one
+// chunk, and `score` is its score; prep: the samples it prepared; c: the predictions appended before it (only c > 0,
+// c < 5 and min(c, 30) matter); hist(i): the prediction appended i + 1 calls ago, i < min(c, 30).  p (NaN: none): a
+// verifier's p on the call's newest window, which a repeated prediction >= vthr becomes (Model.predict re-verifies it).
+template <class Hist>
+static __device__ __forceinline__ float det_rule(const oww_detect_label& lab, bool stepped, float score, float p, float vthr,
+                                                 int c, int prep, double debounce, Hist hist) {
+    const int n = min(c, DET_HIST);
+    float pred = 0.f;
+    if (stepped) pred = score;
+    else if (lab.repeats && c > 0) pred = hist(0);
+    if (!stepped && !isnan(p) && pred >= vthr) pred = p;
+    if (c < 5) pred = 0.f;
+    if (lab.patience > 0) {
+        if (pred != 0.f) {
+            const int k = min(lab.patience, n);
+            int ge = 0;
+            for (int i = 0; i < k; ++i) ge += hist(i) >= lab.threshold;
+            if (ge < lab.patience) pred = 0.f;
+        }
+    } else if (debounce > 0.0 && !isnan(lab.threshold) && pred != 0.f && pred >= lab.threshold) {
+        int k = n;
+        if (prep > 0) {
+            const double nf = ceil(debounce / ((double)prep / 16000.0));
+            if (nf < (double)k) k = (int)nf;
+        }
+        bool hit = false;
+        for (int i = 0; i < k; ++i) hit = hit || hist(i) >= lab.threshold;
+        if (hit) pred = 0.f;
+    }
+    return pred;
+}
+
 // The kernels stay outside the anonymous namespace: their names in a profile do not depend on the build.
 // One thread per (stream, label); CTA `blockIdx.x` owns streams [blockIdx.x * S, +S).
 __global__ void __launch_bounds__(DET_THREADS) detect_kernel(const float* __restrict__ scores, int n_out, int B, int L, int S,
@@ -65,29 +98,11 @@ __global__ void __launch_bounds__(DET_THREADS) detect_kernel(const float* __rest
     float pred = 0.f;
     if (prep >= 0) {
         const oww_detect_label lab = labels[j];
-        const int n = min(c, DET_HIST);
-        if (prep >= OWW_SAMPLES_PER_CHUNK) pred = lab.column >= 0 ? scores[(size_t)b * n_out + lab.column] : 0.f;
-        else if (lab.repeats && c > 0) pred = hist[(size_t)((c - 1) % DET_HIST) * P + p];
-        if (c < 5) pred = 0.f;
-        const bool has_thr = !isnan(lab.threshold);
-        if (lab.patience > 0) {
-            if (pred != 0.f) {
-                const int k = min(lab.patience, n);
-                int ge = 0;
-                for (int i = 0; i < k; ++i) ge += hist[(size_t)((c - 1 - i) % DET_HIST) * P + p] >= lab.threshold;
-                if (ge < lab.patience) pred = 0.f;
-            }
-        } else if (debounce > 0.0 && has_thr && pred != 0.f && pred >= lab.threshold) {
-            int k = n;
-            if (prep > 0) {
-                const double nf = ceil(debounce / ((double)prep / 16000.0));
-                if (nf < (double)k) k = (int)nf;
-            }
-            bool hit = false;
-            for (int i = 0; i < k; ++i) hit = hit || hist[(size_t)((c - 1 - i) % DET_HIST) * P + p] >= lab.threshold;
-            if (hit) pred = 0.f;
-        }
-        fired = has_thr && pred >= lab.threshold;
+        const bool stepped = prep >= OWW_SAMPLES_PER_CHUNK;
+        const float score = stepped && lab.column >= 0 ? scores[(size_t)b * n_out + lab.column] : 0.f;
+        pred = det_rule(lab, stepped, score, __int_as_float(0x7fc00000), 0.f, c, prep, debounce,
+                        [&](int i) { return hist[(size_t)((c - 1 - i) % DET_HIST) * P + p]; });
+        fired = !isnan(lab.threshold) && pred >= lab.threshold;
         hist[(size_t)(c % DET_HIST) * P + p] = pred;
         if (d_final) d_final[p] = pred;
     }
@@ -154,6 +169,103 @@ __global__ void detect_import_kernel(const int* ids, int B, int L, float* hist, 
         hist[(size_t)((c % DET_HIST + k) % DET_HIST) * P + (size_t)b * L + j] = in[(size_t)blockIdx.x * L * DET_HIST + i];
     }
     if (threadIdx.x == 0) count[b] = c;
+}
+
+// ---- the bulk clip path (oww_detect_clips) ----
+// One thread per (clip, label), CTA `blockIdx.x` owns clips [blockIdx.x * S, +S).  Each thread walks its clip's rows in
+// call order from an empty history, kept as a ring in shared memory (ring[slot][threadIdx.x]: no bank conflicts, no
+// local memory).  Two passes, as detect_kernel / detect_events_kernel: detect_clips_kernel writes the final rows and
+// counts each thread's events, detect_clips_events_kernel walks again and writes the events behind those of the threads
+// before it - ascending (clip, label, call) - so no CTA ever waits for another.
+struct DetClips {
+    const float* scores; int n_out;             // [rows][n_out]
+    const float* verified; float vthr;          // [rows][L] or nullptr
+    const int64_t* row_off; int n_clips;        // [n_clips + 1]
+    int chunk;
+    const oww_detect_label* labels; int L, S;
+    double debounce;
+    float* final;                               // [rows][L] or nullptr
+    int* thread_events;                         // [n_clips * L] or nullptr (no event list)
+    int* cta_events;                            // [CTAs]
+    oww_event* events; int max_events; int* n_events;
+};
+
+// emit(row, call, pred, fired) for every call of `clip`, in call order
+template <class F>
+static __device__ __forceinline__ void clip_walk(const DetClips& a, float (*ring)[DET_THREADS], int clip, int j, F emit) {
+    const oww_detect_label lab = a.labels[j];
+    const int64_t r0 = a.row_off[clip], n = a.row_off[clip + 1] - r0;
+    const int t = threadIdx.x;
+    int slot = 0;                                                  // c % 30
+    for (int64_t c = 0; c < n; ++c) {
+        const int64_t row = r0 + c;
+        const int64_t k = oww_call_first_step(c + 1, a.chunk) - oww_call_first_step(c, a.chunk);   // chunks stepped
+        const int prep = k > 0 ? (int)(k * OWW_SAMPLES_PER_CHUNK) : (int)((c + 1) * a.chunk % OWW_SAMPLES_PER_CHUNK);
+        const bool stepped = k > 0;
+        const float score = stepped && lab.column >= 0 ? a.scores[row * a.n_out + lab.column] : 0.f;
+        const float p = !stepped && a.verified ? a.verified[row * a.L + j] : __int_as_float(0x7fc00000);
+        const float pred = det_rule(lab, stepped, score, p, a.vthr, (int)min(c, (int64_t)DET_HIST), prep, a.debounce,
+                                    [&](int i) { return ring[(slot + DET_HIST - 1 - i) % DET_HIST][t]; });
+        ring[slot][t] = pred;
+        slot = slot == DET_HIST - 1 ? 0 : slot + 1;
+        emit(row, c, pred, !isnan(lab.threshold) && pred >= lab.threshold);
+    }
+}
+
+__global__ void __launch_bounds__(DET_THREADS) detect_clips_kernel(const DetClips a) {
+    __shared__ float ring[DET_HIST][DET_THREADS];
+    __shared__ int s_events;
+    const int sl = threadIdx.x / a.L, j = threadIdx.x - sl * a.L;
+    const int clip = blockIdx.x * a.S + sl;
+    const bool live = sl < a.S && clip < a.n_clips;
+    if (threadIdx.x == 0) s_events = 0;
+    __syncthreads();
+    int ev = 0;
+    if (live)
+        clip_walk(a, ring, clip, j, [&](int64_t row, int64_t, float pred, bool fired) {
+            if (a.final) a.final[row * a.L + j] = pred;
+            ev += fired;
+        });
+    if (!a.thread_events) return;
+    if (live) a.thread_events[(size_t)clip * a.L + j] = ev;
+    if (ev) atomicAdd(&s_events, ev);
+    __syncthreads();
+    if (threadIdx.x == 0) a.cta_events[blockIdx.x] = s_events;
+}
+
+// Same grid and thread mapping.  A thread's events start behind those of the CTAs and threads before it.
+__global__ void __launch_bounds__(DET_THREADS) detect_clips_events_kernel(const DetClips a) {
+    __shared__ float ring[DET_HIST][DET_THREADS];
+    __shared__ int s_sum[DET_THREADS / 32];
+    __shared__ int s_warp[DET_THREADS / 32];
+    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+    int part = 0;
+    for (int i = threadIdx.x; i < (int)blockIdx.x; i += DET_THREADS) part += a.cta_events[i];
+    for (int o = 16; o; o >>= 1) part += __shfl_xor_sync(0xffffffffu, part, o);
+    const int sl = threadIdx.x / a.L, j = threadIdx.x - sl * a.L;
+    const int clip = blockIdx.x * a.S + sl;
+    const bool live = sl < a.S && clip < a.n_clips;
+    const int mine = live ? a.thread_events[(size_t)clip * a.L + j] : 0;
+    int incl = mine;                                               // inclusive scan over the warp
+    for (int o = 1; o < 32; o <<= 1) {
+        const int v = __shfl_up_sync(0xffffffffu, incl, o);
+        if (lane >= o) incl += v;
+    }
+    if (lane == 31) s_warp[warp] = incl;
+    if (lane == 0) s_sum[warp] = part;
+    __syncthreads();
+    int base = 0, before = 0;
+    for (int w = 0; w < DET_THREADS / 32; ++w) {
+        base += s_sum[w];
+        if (w < warp) before += s_warp[w];
+    }
+    if (blockIdx.x == gridDim.x - 1 && threadIdx.x == 0) *a.n_events = base + a.cta_events[blockIdx.x];
+    int pos = base + before + incl - mine;
+    if (!mine || !a.events || pos >= a.max_events) return;
+    clip_walk(a, ring, clip, j, [&](int64_t, int64_t c, float pred, bool fired) {
+        if (fired && pos < a.max_events) a.events[pos] = oww_event{clip, j, pred, (int)c};
+        pos += fired;
+    });
 }
 
 namespace {
@@ -299,6 +411,68 @@ int oww_detect(oww_ctx* ctx, const float* d_scores, int prepared_all, const int3
         detect_events_kernel<<<ctas, DET_THREADS, 0, s>>>(d->d_fire, d->d_count, d->d_cta, B, L, S, d_events, max_events, d_n_events);
         OWW_LAUNCH_CHECK(ctx);
     }
+    return OWW_OK;
+}
+
+int oww_detect_clips(oww_ctx* ctx, const oww_detect_label* h_labels, int n_labels, double debounce_time,
+                     const float* d_scores, const float* d_verified, float verifier_threshold, const int64_t* h_row_offsets,
+                     int n_clips, int chunk_size, float* d_final, oww_event* d_events, int max_events, int32_t* d_n_events,
+                     void* stream) {
+    if (!ctx) return OWW_EINVAL;
+    if (n_labels < 1 || n_labels > DET_MAX_LABELS) return oww_fail(ctx, OWW_EINVAL, "n_labels=%d outside [1,%d]", n_labels, DET_MAX_LABELS);
+    if (!h_labels || !h_row_offsets) return oww_fail(ctx, OWW_EINVAL, "null argument");
+    if (!(debounce_time >= 0.0) || !std::isfinite(debounce_time)) return oww_fail(ctx, OWW_EINVAL, "debounce_time must be finite and >= 0");
+    for (int j = 0; j < n_labels; ++j) {
+        const oww_detect_label& l = h_labels[j];
+        if (l.column < -1 || l.column >= ctx->n_out_total)
+            return oww_fail(ctx, OWW_EINVAL, "label %d: column %d outside [-1,%d)", j, l.column, ctx->n_out_total);
+        if (l.patience < 0 || l.patience > DET_HIST) return oww_fail(ctx, OWW_EINVAL, "label %d: patience %d outside [0,%d]", j, l.patience, DET_HIST);
+        if (l.patience > 0 && std::isnan(l.threshold)) return oww_fail(ctx, OWW_EINVAL, "label %d: patience needs a threshold", j);
+        if (l.patience > 0 && debounce_time > 0.0) return oww_fail(ctx, OWW_EINVAL, "patience and debounce_time cannot be used together");
+    }
+    if (n_clips < 0) return oww_fail(ctx, OWW_EINVAL, "n_clips=%d is negative", n_clips);
+    if (chunk_size < 1) return oww_fail(ctx, OWW_EINVAL, "chunk_size=%d < 1", chunk_size);
+    if (h_row_offsets[0] != 0) return oww_fail(ctx, OWW_EINVAL, "row offsets must start at 0");
+    for (int i = 0; i < n_clips; ++i)
+        if (h_row_offsets[i + 1] < h_row_offsets[i]) return oww_fail(ctx, OWW_EINVAL, "row offsets decrease at clip %d", i);
+    const int64_t rows = h_row_offsets[n_clips];
+    if (rows > 0 && !d_scores) return oww_fail(ctx, OWW_EINVAL, "null argument");
+    if (max_events < 0) return oww_fail(ctx, OWW_EINVAL, "max_events=%d is negative", max_events);
+    if (!d_final && !d_n_events && !d_events) return oww_fail(ctx, OWW_EINVAL, "no output: d_final and the event list are both NULL");
+    if (max_events > 0 && !d_events) return oww_fail(ctx, OWW_EINVAL, "max_events=%d without d_events", max_events);
+    if (d_events && !d_n_events) return oww_fail(ctx, OWW_EINVAL, "d_events without d_n_events");
+    OWW_CUDA(ctx, cudaSetDevice(ctx->device));
+    cudaStream_t s = (cudaStream_t)stream;
+    if (n_clips == 0) {
+        if (d_n_events) OWW_CUDA(ctx, cudaMemsetAsync(d_n_events, 0, sizeof(int32_t), s));
+        return OWW_OK;
+    }
+    const int L = n_labels, S = det_streams_per_cta(L), ctas = (n_clips + S - 1) / S;
+    // one allocation: the row offsets and the labels (uploaded), then the event counts of the threads and the CTAs
+    const size_t off_bytes = (size_t)(n_clips + 1) * sizeof(int64_t), lab_bytes = (size_t)L * sizeof(oww_detect_label);
+    const size_t cnt_bytes = d_n_events ? ((size_t)n_clips * L + ctas) * sizeof(int) : 0;
+    std::vector<uint8_t> tab(off_bytes + lab_bytes);
+    std::memcpy(tab.data(), h_row_offsets, off_bytes);
+    std::memcpy(tab.data() + off_bytes, h_labels, lab_bytes);
+    uint8_t* d_tab = nullptr;
+    OWW_CUDA(ctx, cudaMallocAsync(&d_tab, tab.size() + cnt_bytes, s));
+    int* d_counts = d_n_events ? reinterpret_cast<int*>(d_tab + tab.size()) : nullptr;
+    cudaError_t e = cudaMemcpyAsync(d_tab, tab.data(), tab.size(), cudaMemcpyHostToDevice, s);   // pageable: staged before return
+    DetClips a{d_scores, ctx->n_out_total, d_verified, verifier_threshold, reinterpret_cast<const int64_t*>(d_tab), n_clips,
+               chunk_size, reinterpret_cast<const oww_detect_label*>(d_tab + off_bytes), L, S, debounce_time, d_final,
+               d_counts, d_counts ? d_counts + (size_t)n_clips * L : nullptr, d_events, max_events, d_n_events};
+    if (e == cudaSuccess) {
+        detect_clips_kernel<<<ctas, DET_THREADS, 0, s>>>(a);
+        ctx->launches++;
+        e = cudaGetLastError();
+    }
+    if (e == cudaSuccess && d_n_events) {
+        detect_clips_events_kernel<<<ctas, DET_THREADS, 0, s>>>(a);
+        ctx->launches++;
+        e = cudaGetLastError();
+    }
+    cudaFreeAsync(d_tab, s);
+    if (e != cudaSuccess) return oww_fail(ctx, OWW_ECUDA, "detect_clips: %s (%s:%d)", cudaGetErrorString(e), __FILE__, __LINE__);
     return OWW_OK;
 }
 

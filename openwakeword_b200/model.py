@@ -1032,48 +1032,123 @@ class Model:
                         hits[lbl].append(context)
         return {lbl: np.vstack(v) for lbl, v in hits.items() if v}
 
-    def predict_clips(self, clips, padding=1, feature_init=None, chunk_size=1280, streams=None, sr=None):
+    def predict_clips(self, clips, padding=1, feature_init=None, chunk_size=1280, streams=None, sr=None, patience={},
+                      threshold={}, debounce_time=0.0):
         """Bulk path (extension; SURVEY.md F9): each clip from a fresh state, in one device call.  ``clips``: an int16
         [N,S] array or tensor, or a sequence of 1-D int16 arrays of any lengths.  Returns a list (per clip) of lists (per
-        call) of {label: float}, i.e. what predict_clip(clip, padding, chunk_size) would return for each clip after
-        reset(feature_init).  streams (N stream ids, or None: stream 0's models and verifiers): clip i is predicted as
-        stream streams[i] would predict it, with its stream models and device verifiers.  sr: as in
-        predict_clips_ragged."""
+        call) of {label: float}, i.e. what predict_clip(clip, padding, chunk_size, patience=patience,
+        threshold=threshold, debounce_time=debounce_time) would return for each clip after reset(feature_init).  streams
+        (N stream ids, or None: stream 0's models and verifiers): clip i is predicted as stream streams[i] would predict
+        it, with its stream models and device verifiers.  sr: as in predict_clips_ragged.  patience, threshold,
+        debounce_time: as in ``predict``, with the same ValueErrors; the history, the first-5 zeroing, patience and
+        debounce run on the device (oww_detect_clips)."""
         rates = self._clip_rates(sr, len(clips), "predict_clips")
         torch = _torch()
         if rates is None and (sr is None or not self.preprocessor.ingest) and streams is None and chunk_size == CHUNK \
                 and (isinstance(clips, torch.Tensor) or (isinstance(clips, np.ndarray) and clips.ndim == 2)):
-            scores, labels = self.predict_clips_array(clips, padding, feature_init)
+            scores, labels = self.predict_clips_array(clips, padding, feature_init, patience, threshold, debounce_time)
             return [[{lab: float(scores[c, s, j]) for j, lab in enumerate(labels)} for s in range(scores.shape[1])]
                     for c in range(scores.shape[0])]
         pcm, offsets = _concat_clips(clips)
         scores, row_off, labels = self.predict_clips_ragged(pcm, offsets, padding, chunk_size, feature_init, streams,
-                                                            sr=sr)
+                                                            sr=sr, patience=patience, threshold=threshold,
+                                                            debounce_time=debounce_time)
         return _rows_to_dicts(scores, row_off, labels)
 
-    def predict_clips_ragged(self, pcm, offsets, padding=1, chunk_size=1280, feature_init=None, streams=None, sr=None):
+    def predict_clips_ragged(self, pcm, offsets, padding=1, chunk_size=1280, feature_init=None, streams=None, sr=None,
+                             patience={}, threshold={}, debounce_time=0.0):
         """Array form of the bulk path over clips of any lengths: clip i is ``pcm[offsets[i]:offsets[i+1]]`` (int16 1-D
         array or tensor, int64 offsets).  Returns (float32 [rows, n_labels], int64 row_offsets [N+1], labels): clip i's
-        rows ``row_offsets[i]:row_offsets[i+1]`` are the predictions predict_clip(clip, padding, chunk_size) returns after
-        reset(feature_init), one per call.  streams: as in predict_clips.  sr: the clips' rate, one for all or one per
-        clip (None: 16 kHz).  Clips at other rates are resampled to 16 kHz with their padding in one device launch
+        rows ``row_offsets[i]:row_offsets[i+1]`` are the predictions predict_clip(clip, padding, chunk_size, patience=...,
+        threshold=..., debounce_time=...) returns after reset(feature_init), one per call.  streams, patience,
+        threshold, debounce_time: as in predict_clips.  sr: the clips' rate, one for all or one per clip (None: 16 kHz).
+        Clips at other rates are resampled to 16 kHz with their padding in one device launch
         (AudioFeatures.resample_clips) and then run as 16 kHz clips without padding: ``chunk_size`` counts 16 kHz samples
         and a clip makes len(range(0, L - chunk_size, chunk_size)) calls over its L = A(S) + 2*16000*padding samples."""
+        table = self._clip_table(patience, threshold, debounce_time)
+        rules = dict(table=table, debounce_time=debounce_time) if patience or threshold or debounce_time > 0 else {}
+        pcm, offsets, padding, check = self._clips_16k(pcm, offsets, padding, sr)
+        return self._predict_ragged(pcm, offsets, padding, chunk_size, feature_init, streams=streams, check_ingest=check,
+                                    **rules)[:3]
+
+    def detect_clips(self, clips, threshold, patience={}, debounce_time=0.0, padding=1, chunk_size=1280,
+                     feature_init=None, streams=None, sr=None):
+        """The detections of ``predict_clips(clips, padding, feature_init, chunk_size, streams, sr, patience, threshold,
+        debounce_time)``: a list of (clip index, label, call index, score) for every call whose prediction is >= the
+        threshold of its model, ordered by clip, then label (``labels()`` order), then call.  threshold: {model name:
+        float} as in the reference (a model without one never fires), or one float for every model.  The scores stay
+        on the device; only the event count and the events come back."""
+        if not self.labels():
+            raise ValueError("detect_clips needs at least one model")
+        table = self._clip_table(patience, threshold, debounce_time)
+        pcm, offsets = _concat_clips(clips)
+        pcm, offsets, padding, check = self._clips_16k(pcm, offsets, padding, sr)
+        raw, row_off, verified, dev = self._clip_call(pcm, offsets, padding, chunk_size, feature_init, streams, check)[:4]
+        torch = _torch()
+        labels = self.labels()
+        ctx, stream = self.preprocessor.ctx, torch.cuda.current_stream(dev).cuda_stream
+        n_ev = torch.zeros(1, dtype=torch.int32, device=dev)
+        cap = min(int(row_off[-1]) * len(labels), 1 << 16)
+        while True:                     # stateless: a call that found more events than the buffer holds runs again
+            ev = torch.empty((max(cap, 1), 4), dtype=torch.int32, device=dev)
+            ctx.detect_clips(table, max(float(debounce_time), 0.0), raw, verified, self.custom_verifier_threshold,
+                             row_off, chunk_size, None, ev, cap, n_ev, stream)
+            n = int(n_ev.item())
+            if n <= cap:
+                break
+            cap = n
+        e = ev[:n].cpu().numpy().view(_native.EVENT_DTYPE).reshape(-1)
+        return list(zip(e["stream"].tolist(), [labels[j] for j in e["label"].tolist()], e["index"].tolist(),
+                        e["score"].tolist()))
+
+    def _clip_table(self, patience, threshold, debounce_time):
+        """the label table of oww_detect_clips for predict's arguments, refused as predict refuses them"""
+        if (patience != {} or debounce_time > 0) and threshold == {}:
+            raise ValueError("Error! When using the `patience` argument, threshold "
+                             "values must be provided via the `threshold` argument!")
+        return self._detector_table(threshold, patience, debounce_time)
+
+    def _clips_16k(self, pcm, offsets, padding, sr):
+        """-> (pcm, offsets, padding, check_ingest) of the clips at 16 kHz: clips at other rates are resampled with their
+        padding in one device launch"""
         offsets = np.ascontiguousarray(offsets, np.int64)
         rates = self._clip_rates(sr, offsets.size - 1, "the bulk clip path (predict_clips_ragged, bulk_predict)")
         if rates is None:
-            return self._predict_ragged(pcm, offsets, padding, chunk_size, feature_init, streams=streams,
-                                        check_ingest=sr is None)[:3]
+            return pcm, offsets, padding, sr is None
         d, off16 = self.preprocessor.resample_clips(pcm, offsets, rates, 16000 * int(padding))
-        return self._predict_ragged(d, off16, 0, chunk_size, feature_init, streams=streams, check_ingest=False)[:3]
+        return d, off16, 0, False
 
     def _predict_ragged(self, pcm, offsets, padding, chunk_size, feature_init, want_features=False, streams=None,
-                        check_ingest=True):
+                        check_ingest=True, table=None, debounce_time=0.0):
         """-> (scores, row_offsets, labels, embeddings [steps, 96] or None, step_offsets [N+1], feature_init rows).
-        One oww_predict_clips_ragged call; the host fills the rows of calls that stepped no chunk as Model.predict does
-        (the previous prediction of single-output heads, zeros for multi-class heads, re-verified), then zeroes each
-        clip's first 5 calls (model.py:330-333).  Vectorised over rows.  check_ingest=False: the caller gave the
-        clips' rate, so a device-ingest Model takes them too."""
+        One oww_predict_clips_ragged call, then oww_detect_clips fills the rows of calls that stepped no chunk as
+        Model.predict does (the previous prediction of single-output heads, zeros for multi-class heads, re-verified),
+        zeroes each clip's first 5 calls (model.py:330-333) and applies `table` (_clip_table; None: no thresholds) and
+        debounce_time.  check_ingest=False: the caller gave the clips' rate, so a device-ingest Model takes them too."""
+        labels = self.labels()
+        if table is None:
+            table = self._clip_table({}, {}, 0.0)
+        raw, row_off, verified, dev, emb, step_off, fi = self._clip_call(pcm, offsets, padding, chunk_size, feature_init,
+                                                                         streams, check_ingest, want_features)
+        out = self._clip_final(raw, row_off, chunk_size, table, debounce_time, verified, dev)
+        emb = emb.cpu().numpy() if emb is not None else None
+        return out, row_off, labels, emb, step_off, fi
+
+    def _clip_final(self, raw, row_off, chunk_size, table, debounce_time, verified, dev):
+        """oww_detect_clips over the raw rows -> host float32 [rows, n_labels]"""
+        torch = _torch()
+        rows = int(row_off[-1])
+        if not table or not rows:
+            return np.zeros((rows, len(table)), np.float32)
+        final = torch.empty((rows, len(table)), dtype=torch.float32, device=dev)
+        self.preprocessor.ctx.detect_clips(table, max(float(debounce_time), 0.0), raw, verified,
+                                           self.custom_verifier_threshold, row_off, chunk_size, final, None, 0, None,
+                                           torch.cuda.current_stream(dev).cuda_stream)
+        return final.cpu().numpy()
+
+    def _clip_call(self, pcm, offsets, padding, chunk_size, feature_init, streams, check_ingest, want_features=False):
+        """One oww_predict_clips_ragged / _streams call -> (device raw rows, row_offsets [N+1], device p rows of the
+        repeated calls' verifiers or None, device, device embeddings or None, step_offsets [N+1], feature_init rows)."""
         if check_ingest:
             self._no_ingest("the bulk clip path (predict_clips_ragged, bulk_predict)")
         if self._host_verifiers:
@@ -1106,64 +1181,62 @@ class Model:
         if fi is None:
             fi = self.preprocessor._get_embeddings(np.random.randint(-1000, 1000, 16000 * 4).astype(np.int16))
         fi = np.ascontiguousarray(fi, np.float32)
-        cols, labels, single = [], [], []
-        for mdl in self.models:
-            col0, n_out = self._columns[mdl]
-            if n_out == 1:
-                cols.append(col0); labels.append(mdl); single.append(True)
-            else:
-                for k, lab in self.class_mapping[mdl].items():
-                    cols.append(col0 + int(k)); labels.append(lab); single.append(False)
-        dev = f"cuda:{self.preprocessor.device_index}"
+        dev = torch.device("cuda", self.preprocessor.device_index)
         if isinstance(pcm, torch.Tensor):
             d = pcm.to(device=dev, dtype=torch.int16, non_blocking=True).contiguous()
         else:
             d = torch.from_numpy(np.ascontiguousarray(pcm, np.int16)).to(dev)
         raw = torch.zeros((rows, max(self._n_cols, 1)), dtype=torch.float32, device=dev)
-        stepped = torch.zeros(rows, dtype=torch.uint8, device=dev)
         need_emb = want_features or (chunk_size < CHUNK and bool(self._vbanks or self._svbanks))
         emb = torch.zeros((int(step_off[-1]), 96), dtype=torch.float32, device=dev) if need_emb else None
-        self.preprocessor.ctx.predict_clips_ragged(d, offsets, pad, chunk_size, fi, raw, stepped, emb,
-                                                   torch.cuda.current_stream(d.device).cuda_stream,
+        stream = torch.cuda.current_stream(dev).cuda_stream
+        self.preprocessor.ctx.predict_clips_ragged(d, offsets, pad, chunk_size, fi, raw, None, emb, stream,
                                                    clip_streams=streams)
-        out = raw.cpu().numpy()[:, cols]
-        stepped = stepped.cpu().numpy().astype(bool)
-        emb = emb.cpu().numpy() if emb is not None else None
-        if rows:
-            clip = np.repeat(np.arange(n), calls)
-            idx = np.arange(rows)
-            local = idx - row_off[clip]
-            first5 = local < 5
-            out[first5] = 0.0
-            # a row is its own source when it stepped or is zeroed; other rows repeat the final value of the source row
-            # before them (re-verification on an unchanged window is idempotent, so repeating a repeat is the same)
-            src = np.maximum.accumulate(np.where(stepped | first5, idx, -1))
-            rep = ~(stepped | first5)
-            single = np.asarray(single)
-            out[rep] = np.where(single[None, :], out[src[rep]], np.float32(0.0))
-            if rep.any():
-                self._reverify_rows(out, rep, local, clip, step_off, chunk_size, emb, fi, labels, streams)
-        return out, row_off, labels, emb, step_off, fi
+        verified = self._verified_rows(calls, chunk_size, step_off, emb, fi, streams, dev) \
+            if rows and chunk_size < CHUNK and (self._vbanks or self._svbanks) else None
+        return raw, row_off, verified, dev, emb, step_off, fi
 
-    def _reverify_rows(self, out, rep, local, clip, step_off, chunk_size, emb, fi, labels, streams=None):
-        """_reverify on the rows of calls that stepped no chunk: labels of a device-verified model >= the threshold take
-        the verifier's p on the clip's newest window ([feature_init rows | the clip's embeddings] up to the last step).
-        A row takes the slots of its clip's stream (streams[clip], or stream 0)."""
-        thr = np.float32(self.custom_verifier_threshold)
-        row_stream = np.zeros(out.shape[0], np.int64) if streams is None else streams[clip]
+    def _verified_rows(self, calls, chunk_size, step_off, emb, fi, streams, dev):
+        """_reverify on the rows of calls that step no chunk, on the device: -> float32 [rows, n_labels] (NaN where a
+        label's model has no device verifier on the clip's stream, or the call steps) of the verifier's p on the clip's
+        newest window ([feature_init rows | the clip's embeddings] up to its last step).  A row takes the slots of its
+        clip's stream (streams[clip], or stream 0).  Calls with the same window share one verifier row; oww_detect_clips
+        applies p to the predictions >= custom_verifier_threshold."""
+        torch = _torch()
+        labels = self.labels()
+        n = calls.size
+        rows = int(calls.sum())
+        clip = np.repeat(np.arange(n), calls)
+        local = np.arange(rows) - np.repeat(np.concatenate([[0], np.cumsum(calls)[:-1]]), calls)
+        done = (local + 1) * chunk_size // CHUNK                     # chunks stepped up to and including the call
+        rep = done == local * chunk_size // CHUNK
+        row_stream = np.zeros(rows, np.int64) if streams is None else streams[clip]
+        # [zero row | feature_init | every clip's embeddings]: a window's rows are gathered from it on the device
+        table = torch.cat([torch.zeros((1, 96), dtype=torch.float32, device=dev), torch.from_numpy(fi).to(dev), emb])
+        F = fi.shape[0]
+        out = torch.full((rows, len(labels)), float("nan"), dtype=torch.float32, device=dev)
+        stream = torch.cuda.current_stream(dev).cuda_stream
         for mdl, st in list(self._vbanks.items()) + list(self._svbanks.items()):
             slots = np.where(self._has_model(mdl, row_stream), st["slots"][row_stream], -1)
-            js = [j for j, lab in enumerate(labels) if self.get_parent_model_from_label(lab) == mdl]
-            hit = rep & (slots >= 0) & (out[:, js] >= thr).any(axis=1)
+            js = torch.tensor([j for j, lab in enumerate(labels) if self.get_parent_model_from_label(lab) == mdl],
+                              dtype=torch.int64, device=dev)
             n_in = self.model_inputs[mdl]
+            hit = rep & (slots >= 0)
             for slot in np.unique(slots[hit]):
                 hit_rows = np.nonzero(hit & (slots == slot))[0]
-                done = (local[hit_rows] + 1) * chunk_size // CHUNK       # chunks stepped up to and including the call
-                feats = np.stack([_window(fi, emb, step_off[clip[r]], int(k), n_in) for r, k in zip(hit_rows, done)])
-                p = self.preprocessor.ctx.verifier_predict_host(st["bank"], int(slot), feats)
-                for j in js:
-                    sel = out[hit_rows, j] >= thr
-                    out[hit_rows[sel], j] = p[sel]
+                key = step_off[clip[hit_rows]] + clip[hit_rows] + done[hit_rows]    # one per (clip, window)
+                _, first, inv = np.unique(key, return_index=True, return_inverse=True)
+                r = hit_rows[first]
+                q = F + done[r][:, None] - n_in + np.arange(n_in)[None, :]          # row of [fi | clip's embeddings]
+                src = np.where(q < 0, 0, np.where(q < F, 1 + q, 1 + F + step_off[clip[r]][:, None] + q - F))
+                p = torch.empty(r.size, dtype=torch.float32, device=dev)
+                for a in range(0, r.size, 1 << 16):
+                    b = min(r.size, a + (1 << 16))
+                    feats = table[torch.from_numpy(src[a:b]).to(dev)].contiguous()
+                    self.preprocessor.ctx.verifier_predict(st["bank"], int(slot), feats, b - a, p[a:b], stream)
+                rt = torch.from_numpy(hit_rows).to(dev)
+                out[rt[:, None], js[None, :]] = p[torch.from_numpy(inv.ravel()).to(dev)][:, None].expand(-1, js.numel())
+        return out
 
     def _positive_frames_bulk(self, pcms, threshold=0.5, return_type="features", sr=None):
         """_get_positive_prediction_frames over many clips in one device call (padding 0, 1280-sample calls): per clip
@@ -1209,10 +1282,12 @@ class Model:
                 labs += list(self.class_mapping[mdl].values())
         return labs
 
-    def predict_clips_array(self, clips, padding=1, feature_init=None):
-        """-> (float32 [N, steps, n_labels], labels) with the first-5-steps zeroing of model.py:330-333 applied.
-        Device verifiers apply (stream 0's); host-only verifiers do not, and a warning says so."""
+    def predict_clips_array(self, clips, padding=1, feature_init=None, patience={}, threshold={}, debounce_time=0.0):
+        """-> (float32 [N, steps, n_labels], labels) with the first-5-steps zeroing of model.py:330-333 applied, and
+        patience, threshold and debounce_time as in ``predict`` (oww_detect_clips on the device).  Device verifiers
+        apply (stream 0's); host-only verifiers do not, and a warning says so."""
         self._no_ingest("predict_clips_array")
+        table = self._clip_table(patience, threshold, debounce_time)
         if self._host_verifiers:
             warnings.warn(f"custom verifiers of {sorted(self._host_verifiers)} are not device-runnable (only the linear "
                           "pipeline of train_verifier_model is): predict_clips returns their models' unverified scores",
@@ -1232,22 +1307,13 @@ class Model:
         fi = feature_init if feature_init is not None else self.preprocessor._feature_init
         if fi is None:
             fi = self.preprocessor._get_embeddings(np.random.randint(-1000, 1000, 16000 * 4).astype(np.int16))
-        dev = f"cuda:{self.preprocessor.device_index}"
+        dev = torch.device("cuda", self.preprocessor.device_index)
         d = clips.to(dev, non_blocking=True) if isinstance(clips, torch.Tensor) else torch.from_numpy(clips).to(dev)
         raw = torch.zeros((N, steps, max(self._n_cols, 1)), dtype=torch.float32, device=dev)
         self.preprocessor.ctx.predict_clips(d, N, S, 16000 * padding, fi, raw, torch.cuda.current_stream(d.device).cuda_stream)
-        raw = raw.cpu().numpy()
-        cols, labels = [], []
-        for mdl in self.models:
-            col0, n_out = self._columns[mdl]
-            if n_out == 1:
-                cols.append(col0); labels.append(mdl)
-            else:
-                for k, lab in self.class_mapping[mdl].items():
-                    cols.append(col0 + int(k)); labels.append(lab)
-        out = raw[:, :, cols]
-        out[:, :5, :] = 0.0
-        return out, labels
+        row_off = np.arange(N + 1, dtype=np.int64) * steps
+        out = self._clip_final(raw, row_off, CHUNK, table, debounce_time, None, dev)
+        return out.reshape(N, steps, len(table)), self.labels()
 
 
 class StreamState:
