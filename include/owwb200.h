@@ -556,16 +556,26 @@ int oww_resample_clips(oww_ctx* ctx, const int16_t* d_in, const int64_t* h_in_of
                        int pad_samples, int16_t* d_out, const int64_t* h_out_offsets, void* stream);
 
 /* ---- score metrics on the device (openwakeword/metrics.py:24-100) --------------------------------
- * d_scores holds n_series score sequences of n_frames float32 each, series i at d_scores + i*series_stride.
+ * d_scores holds n_series score sequences of n_frames float32 (or float64) each, series i at d_scores + i*series_stride.
  * oww_metrics_false_positives: h_counts[i][j] = get_false_positives(series i, h_thresholds[j], grouping_window)
  * with the reference's grouping rule (restated in oracle/metrics.py); generate_roc_curve_fprs is this count at
  * np.linspace(0.01, 0.99, n_points) divided by the hours the series spans.
  * oww_metrics_count_ge: h_counts[j] = number of the n scores >= h_thresholds[j] (generate_roc_curve_tprs * len).
- * Comparisons are done in double, as NumPy does for float32 scores against np.float64 thresholds.  Both synchronise. */
+ * The _f64 forms take float64 scores and are otherwise the same.
+ * Every comparison is (double)score >= h_thresholds[j].  To reproduce NumPy's `scores >= threshold` in the dtype D it
+ * promotes to, round the threshold to D before passing it (openwakeword_b200.metrics does): widening the scores and
+ * a D-rounded threshold to double is exact, so the double comparison is exactly the comparison in D.
+ * 1..4096 thresholds per false-positive call, 1..64 per count call, n_series >= 1, n_frames >= 0, n >= 0; anything
+ * else, or a NULL pointer, is OWW_EINVAL with nothing launched.  Both synchronise. */
 int oww_metrics_false_positives(oww_ctx* ctx, const float* d_scores, int64_t series_stride, int n_series, int n_frames,
                                 const double* h_thresholds, int n_thresholds, int grouping_window, int32_t* h_counts, void* stream);
+int oww_metrics_false_positives_f64(oww_ctx* ctx, const double* d_scores, int64_t series_stride, int n_series, int n_frames,
+                                    const double* h_thresholds, int n_thresholds, int grouping_window, int32_t* h_counts,
+                                    void* stream);
 int oww_metrics_count_ge(oww_ctx* ctx, const float* d_scores, int64_t n, const double* h_thresholds, int n_thresholds,
                          uint64_t* h_counts, void* stream);
+int oww_metrics_count_ge_f64(oww_ctx* ctx, const double* d_scores, int64_t n, const double* h_thresholds, int n_thresholds,
+                             uint64_t* h_counts, void* stream);
 
 /* ---- parity instrumentation --------------------------------------------------------------- */
 /* Runs the embedding CNN on d_windows [n][76][32] (n <= window_batch) up to and including conv

@@ -129,7 +129,9 @@ _SIGNATURES = {
     "oww_peer_wait": (C.c_int, [_P, _P, C.c_int, C.c_int, C.c_uint64, C.c_double, _P]),
     "oww_peer_status": (C.c_int, [_P, C.POINTER(C.c_int)]),
     "oww_metrics_false_positives": (C.c_int, [_P, _P, C.c_int64, C.c_int, C.c_int, _P, C.c_int, C.c_int, _P, _P]),
+    "oww_metrics_false_positives_f64": (C.c_int, [_P, _P, C.c_int64, C.c_int, C.c_int, _P, C.c_int, C.c_int, _P, _P]),
     "oww_metrics_count_ge": (C.c_int, [_P, _P, C.c_int64, _P, C.c_int, _P, _P]),
+    "oww_metrics_count_ge_f64": (C.c_int, [_P, _P, C.c_int64, _P, C.c_int, _P, _P]),
     "oww_launch_count": (C.c_uint64, [_P]),
     "oww_enable_stage_timing": (C.c_int, [_P, C.c_int]),
     "oww_stage_ms": (C.c_int, [_P, _P]),
@@ -989,20 +991,31 @@ class Context:
         return bool(v.value)
 
     # ---- metrics (device-resident scores) ----
+    @staticmethod
+    def _metrics_f64(d_scores):
+        """True for float64 scores (the _f64 entry points), False for float32; any other dtype is refused."""
+        name = str(d_scores.dtype)
+        if name not in ("torch.float32", "torch.float64"):
+            raise ValueError(f"metrics take float32 or float64 scores, got {name}")
+        return name == "torch.float64"
+
     def metrics_false_positives(self, d_scores, series_stride, n_series, n_frames, thresholds, grouping_window=50, stream=None):
+        """Thresholds are compared as the float64 values given (round them to the comparison dtype first: metrics.py)."""
+        fn = self.lib.oww_metrics_false_positives_f64 if self._metrics_f64(d_scores) else self.lib.oww_metrics_false_positives
         thr = np.ascontiguousarray(thresholds, np.float64)
         out = np.zeros((n_series, thr.size), np.int32)
-        self._check(self.lib.oww_metrics_false_positives(self.h, _ptr(d_scores), int(series_stride), int(n_series), int(n_frames),
-                                                         _ptr(thr), thr.size, int(grouping_window), _ptr(out), stream))
+        self._check(fn(self.h, _ptr(d_scores), int(series_stride), int(n_series), int(n_frames), _ptr(thr), thr.size,
+                       int(grouping_window), _ptr(out), stream))
         return out
 
     def metrics_count_ge(self, d_scores, n, thresholds, stream=None):
+        fn = self.lib.oww_metrics_count_ge_f64 if self._metrics_f64(d_scores) else self.lib.oww_metrics_count_ge
         thr = np.ascontiguousarray(thresholds, np.float64)
         out = np.zeros(thr.size, np.uint64)
         for j0 in range(0, thr.size, 64):
             t = np.ascontiguousarray(thr[j0:j0 + 64])
             o = np.zeros(t.size, np.uint64)
-            self._check(self.lib.oww_metrics_count_ge(self.h, _ptr(d_scores), int(n), _ptr(t), t.size, _ptr(o), stream))
+            self._check(fn(self.h, _ptr(d_scores), int(n), _ptr(t), t.size, _ptr(o), stream))
             out[j0:j0 + 64] = o
         return out
 

@@ -6,18 +6,24 @@
 // (generate_roc_curve_fprs: the same count at 25 thresholds) and :81-100 (generate_roc_curve_tprs: count of scores >= t).
 // The reference walks one Python list per threshold; here one thread owns one (series, threshold) pair and the 32 lanes
 // of a warp share a series, so every score load is a broadcast and the whole ROC of a series costs two passes over it.
-// HBM bound: 4 B per score per pass.
+// HBM bound: 4 B (float32) or 8 B (float64) per score per pass.
+//
+// Every comparison is (double)score >= threshold.  The host rounds each threshold to the dtype in which NumPy would
+// compare it with the scores (openwakeword_b200/metrics.py comparison_dtype) and passes that as a double; widening a
+// float32 score, or a threshold already rounded to float16/32/64, to double is exact, so the double comparison is
+// exactly NumPy's comparison in that dtype.
 #include "oww_internal.h"
 
 namespace {
 
-__global__ void __launch_bounds__(128) false_positives_kernel(const float* scores, int64_t series_stride, int n_series, int n_frames,
+template <typename T>
+__global__ void __launch_bounds__(128) false_positives_kernel(const T* scores, int64_t series_stride, int n_series, int n_frames,
                                                              const double* thr, int n_thr, int window, int* out) {
     const int64_t gid = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
     const int per = (n_thr + 31) & ~31;                       // a warp never straddles two series
     const int sidx = (int)(gid / per), ti = (int)(gid % per);
     if (sidx >= n_series || ti >= n_thr) return;
-    const float* s = scores + (int64_t)sidx * series_stride;
+    const T* s = scores + (int64_t)sidx * series_stride;
     const double t = thr[ti];
     // pass 1: ones and 0->1 transitions of the original sequence
     int ones = 0, n_tr = 0;
@@ -50,7 +56,8 @@ __global__ void __launch_bounds__(128) false_positives_kernel(const float* score
     out[(int64_t)sidx * n_thr + ti] = ones - removed;
 }
 
-__global__ void __launch_bounds__(256) count_ge_kernel(const float* scores, int64_t n, const double* thr, int n_thr, unsigned long long* out) {
+template <typename T>
+__global__ void __launch_bounds__(256) count_ge_kernel(const T* scores, int64_t n, const double* thr, int n_thr, unsigned long long* out) {
     // grid-stride over the scores; per-thread counters for every threshold (n_thr <= 64), block reduction, one atomic each
     __shared__ unsigned int s_cnt[64];
     if (threadIdx.x < 64) s_cnt[threadIdx.x] = 0;
@@ -68,12 +75,9 @@ __global__ void __launch_bounds__(256) count_ge_kernel(const float* scores, int6
     if (threadIdx.x < n_thr && s_cnt[threadIdx.x]) atomicAdd(out + threadIdx.x, (unsigned long long)s_cnt[threadIdx.x]);
 }
 
-}  // namespace
-
-extern "C" {
-
-int oww_metrics_false_positives(oww_ctx* ctx, const float* d_scores, int64_t series_stride, int n_series, int n_frames,
-                                const double* h_thresholds, int n_thresholds, int grouping_window, int32_t* h_counts, void* stream) {
+template <typename T>
+int false_positives(oww_ctx* ctx, const T* d_scores, int64_t series_stride, int n_series, int n_frames,
+                    const double* h_thresholds, int n_thresholds, int grouping_window, int32_t* h_counts, void* stream) {
     if (!ctx || !d_scores || !h_thresholds || !h_counts) return oww_fail(ctx, OWW_EINVAL, "null argument");
     if (n_series < 1 || n_frames < 0 || n_thresholds < 1 || n_thresholds > 4096) return oww_fail(ctx, OWW_EINVAL, "bad sizes");
     OWW_CUDA(ctx, cudaSetDevice(ctx->device));
@@ -96,8 +100,9 @@ int oww_metrics_false_positives(oww_ctx* ctx, const float* d_scores, int64_t ser
     return OWW_OK;
 }
 
-int oww_metrics_count_ge(oww_ctx* ctx, const float* d_scores, int64_t n, const double* h_thresholds, int n_thresholds,
-                         uint64_t* h_counts, void* stream) {
+template <typename T>
+int count_ge(oww_ctx* ctx, const T* d_scores, int64_t n, const double* h_thresholds, int n_thresholds,
+             uint64_t* h_counts, void* stream) {
     if (!ctx || !d_scores || !h_thresholds || !h_counts) return oww_fail(ctx, OWW_EINVAL, "null argument");
     if (n < 0 || n_thresholds < 1 || n_thresholds > 64) return oww_fail(ctx, OWW_EINVAL, "1..64 thresholds per call");
     OWW_CUDA(ctx, cudaSetDevice(ctx->device));
@@ -118,6 +123,31 @@ int oww_metrics_count_ge(oww_ctx* ctx, const float* d_scores, int64_t n, const d
     cudaFreeAsync(d_thr, s); cudaFreeAsync(d_out, s);
     if (e != cudaSuccess) return oww_fail(ctx, OWW_ECUDA, "threshold count failed: %s", cudaGetErrorString(e));
     return OWW_OK;
+}
+
+}  // namespace
+
+extern "C" {
+
+int oww_metrics_false_positives(oww_ctx* ctx, const float* d_scores, int64_t series_stride, int n_series, int n_frames,
+                                const double* h_thresholds, int n_thresholds, int grouping_window, int32_t* h_counts, void* stream) {
+    return false_positives(ctx, d_scores, series_stride, n_series, n_frames, h_thresholds, n_thresholds, grouping_window, h_counts, stream);
+}
+
+int oww_metrics_false_positives_f64(oww_ctx* ctx, const double* d_scores, int64_t series_stride, int n_series, int n_frames,
+                                    const double* h_thresholds, int n_thresholds, int grouping_window, int32_t* h_counts,
+                                    void* stream) {
+    return false_positives(ctx, d_scores, series_stride, n_series, n_frames, h_thresholds, n_thresholds, grouping_window, h_counts, stream);
+}
+
+int oww_metrics_count_ge(oww_ctx* ctx, const float* d_scores, int64_t n, const double* h_thresholds, int n_thresholds,
+                         uint64_t* h_counts, void* stream) {
+    return count_ge(ctx, d_scores, n, h_thresholds, n_thresholds, h_counts, stream);
+}
+
+int oww_metrics_count_ge_f64(oww_ctx* ctx, const double* d_scores, int64_t n, const double* h_thresholds, int n_thresholds,
+                             uint64_t* h_counts, void* stream) {
+    return count_ge(ctx, d_scores, n, h_thresholds, n_thresholds, h_counts, stream);
 }
 
 }  // extern "C"
