@@ -555,6 +555,47 @@ int oww_resample_clip_plan(int rate, int64_t n_in, int pad_samples, int64_t* n_o
 int oww_resample_clips(oww_ctx* ctx, const int16_t* d_in, const int64_t* h_in_offsets, const int32_t* h_rates, int n_clips,
                        int pad_samples, int16_t* d_out, const int64_t* h_out_offsets, void* stream);
 
+/* ---- mixing clips with background noise and room impulse responses (openwakeword/data.py:294-527: mix_clips_batch,
+ * mix_clip, truncate_clip and speechbrain's reverberate), the test clips of a false-reject evaluation ----------------
+ * Foreground and background clips are packed int16 (clip i is d_x[h_x_off[i] .. h_x_off[i+1]), host int64 offsets,
+ * non-decreasing, first >= 0), RIRs packed float32 the same way.  A sample s is read as s / 32768.  Mixture i, with the
+ * record p = h_params[i] and N = n_samples for every mixture of the call, is computed as (real arithmetic):
+ *   1. f[k] = fg clip p.fg at p.fg_start + k, k < p.fg_len (the window is the host's truncation of the clip)
+ *   2. b[n] = bg clip p.bg at (p.bg_offset + n) mod len_bg, n < N (tiling of a short background, crop of a long one)
+ *   3. g = 10^(p.snr_db / 20) * |b|_2 / |f|_2;  m = b;  m[p.start + k] += g f[k];  m /= 2        (data.py:491-496)
+ *   4. p.rir >= 0, h the RIR of L taps: d = first index of max |h[k]|, a0 = mean |m|,
+ *      y[n] = sum_{k<L} h[k] m[(n - k + d) mod N]  (circular, aligned on the direct path), y *= a0 / (mean |y| + 1e-14)
+ *      (speechbrain's reverberate(x, h, rescale_amp="avg") as its published source reads; not compared against it);
+ *      p.rir < 0: y = m
+ *   5. p.volume >= 0: y *= p.volume / max_n y[n] (the signed maximum, data.py:454); else y /= max(max_n |y[n]|, 1)
+ *   6. out[i][n] = clamp(trunc(32767 y[n]), -32768, 32767).  The reference's astype(int16) wraps instead; saturation
+ *      is deliberate (a negative peak can exceed full scale under the signed-maximum rule).
+ * d_valid[i] = 0 when |f|_2 = 0, |b|_2 = 0 or (with a volume) max y <= 0: such a row is written as zeros; and when the
+ * row's largest int16 sample is 0 (what data.py:466 means to drop).  Otherwise 1.
+ * Device arithmetic: norms and the mixture in float64, m stored as float32; the reverb as a banded circulant GEMM on the
+ * tensor cores with fp16 hi/lo split operands (three products) and fp32 accumulation, the taps scaled by a power of two
+ * so that the largest is in [0.5, 1); the rescale and level in float64.  Launches per call: two without any reverb, three
+ * with, whatever n_mix.  Stream-ordered: the call returns once its tables are enqueued; it waits, host side,
+ * until the previous call's launches have read their tables, and it may (re)allocate its scratch (n_mix * N floats,
+ * plus as many for the reverberated rows) with cudaMalloc, which synchronises the device.
+ *   OWW_EINVAL before anything is enqueued: N <= 0, negative counts, bad offsets, an index out of range, a foreground
+ *   window outside its clip, an empty background, bg_offset outside [0, len_bg), start < 0 or start + fg_len > N,
+ *   an empty RIR or one longer than N, a non-finite snr_db or volume, NULL buffers.  n_mix = 0 enqueues nothing. */
+typedef struct oww_mix_params {
+    int32_t fg, bg, rir;       /* clip indices; rir = -1: no reverb */
+    int32_t reserved;          /* 0 */
+    int64_t fg_start, fg_len;  /* foreground window */
+    int64_t bg_offset;         /* background sample at output 0, in [0, len_bg) */
+    int64_t start;             /* output sample of the foreground's first sample */
+    double snr_db;
+    double volume;             /* < 0: no volume, normalise to [-1, 1] only where needed */
+} oww_mix_params;
+int oww_mix_clips(oww_ctx* ctx, const int16_t* d_fg, const int64_t* h_fg_off, int n_fg,
+                  const int16_t* d_bg, const int64_t* h_bg_off, int n_bg,
+                  const float* d_rir, const int64_t* h_rir_off, int n_rir,
+                  const oww_mix_params* h_params, int n_mix, int64_t n_samples,
+                  int16_t* d_out, uint8_t* d_valid, void* stream);
+
 /* ---- score metrics on the device (openwakeword/metrics.py:24-100) --------------------------------
  * d_scores holds n_series score sequences of n_frames float32 (or float64) each, series i at d_scores + i*series_stride.
  * oww_metrics_false_positives: h_counts[i][j] = get_false_positives(series i, h_thresholds[j], grouping_window)

@@ -36,6 +36,10 @@ class DetectLabel(C.Structure):
 # one record of oww_detect's event list (oww_event): 16 bytes
 EVENT_DTYPE = np.dtype([("stream", "<i4"), ("label", "<i4"), ("score", "<f4"), ("index", "<i4")])
 
+# one mixture of oww_mix_clips (oww_mix_params): 64 bytes.  rir = -1: no reverb; volume < 0: no volume
+MIX_DTYPE = np.dtype([("fg", "<i4"), ("bg", "<i4"), ("rir", "<i4"), ("reserved", "<i4"), ("fg_start", "<i8"),
+                      ("fg_len", "<i8"), ("bg_offset", "<i8"), ("start", "<i8"), ("snr_db", "<f8"), ("volume", "<f8")])
+
 
 # name -> (restype, argtypes): every symbol include/owwb200.h declares
 _P = C.c_void_p
@@ -114,6 +118,7 @@ _SIGNATURES = {
     "oww_clip_slab_plan": (C.c_int, [_P, _P, C.c_int, C.POINTER(C.c_int64), C.POINTER(C.c_int64)]),
     "oww_resample_clip_plan": (C.c_int, [C.c_int, C.c_int64, C.c_int, C.POINTER(C.c_int64)]),
     "oww_resample_clips": (C.c_int, [_P, _P, _P, _P, C.c_int, C.c_int, _P, _P, _P]),
+    "oww_mix_clips": (C.c_int, [_P, _P, _P, C.c_int, _P, _P, C.c_int, _P, _P, C.c_int, _P, C.c_int, C.c_int64, _P, _P, _P]),
     "oww_debug_layer": (C.c_int, [_P, _P, C.c_int, C.c_int, _P, _P]),
     "oww_debug_inc_plan": (C.c_int, [_P, C.c_int, C.c_int, _P, C.c_int]),
     "oww_debug_inc_cut_plan": (C.c_int, [_P, C.c_int, C.c_int, C.c_int, _P, C.c_int]),
@@ -935,6 +940,17 @@ class Context:
             raise ValueError(f"{off.size} input offsets, {out.size} output offsets and {r.size} rates")
         self._check(self.lib.oww_resample_clips(self.h, _ptr(d_in), _ptr(off), _ptr(r), r.size, int(pad_samples),
                                                 _ptr(d_out), _ptr(out), stream))
+
+    def mix_clips(self, d_fg, fg_offsets, d_bg, bg_offsets, d_rir, rir_offsets, params, n_samples, d_out, d_valid,
+                  stream=None):
+        """oww_mix_clips: mixture i of the MIX_DTYPE records `params` -> d_out[i] (int16 [n_mix][n_samples]) and d_valid[i]
+        (uint8); clips packed on the device with host int64 offsets (int16 foregrounds and backgrounds, float32 RIRs)."""
+        p = np.ascontiguousarray(params, MIX_DTYPE).ravel()
+        offs = [np.ascontiguousarray(o if len(o) else [0], np.int64).ravel() for o in (fg_offsets, bg_offsets, rir_offsets)]
+        n = [o.size - 1 for o in offs]
+        self._check(self.lib.oww_mix_clips(self.h, _ptr(d_fg), _ptr(offs[0]), n[0], _ptr(d_bg), _ptr(offs[1]), n[1],
+                                           _ptr(d_rir), _ptr(offs[2]), n[2], _ptr(p), p.size,
+                                           int(n_samples), _ptr(d_out), _ptr(d_valid), stream))
 
     def debug_layer(self, d_windows, n, layer, d_out, stream=None):
         self._check(self.lib.oww_debug_layer(self.h, _ptr(d_windows), n, layer, _ptr(d_out), stream))

@@ -882,6 +882,7 @@ void oww_destroy(oww_ctx* ctx) {
     oww_detect_free(ctx);
     oww_audio_free(ctx);
     oww_ingest_free(ctx);
+    oww_mix_free(ctx);
     cudaFree(ctx->d_window); cudaFree(ctx->d_twiddle); cudaFree(ctx->d_mel_start); cudaFree(ctx->d_mel_len);
     cudaFree(ctx->d_mel_w); cudaFree(ctx->d_emb_blob); cudaFree(ctx->d_tc_w); cudaFree(ctx->d_tc_sb);
     cudaFree(ctx->d_tc_w3); cudaFree(ctx->d_tc_sb3);

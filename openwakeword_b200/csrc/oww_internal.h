@@ -327,10 +327,12 @@ struct oww_ctx {
     struct oww_audio* audio = nullptr;    // the streams' recent audio (audio.cu); nullptr: no history
     struct oww_ingest_state* ingest = nullptr;  // resampling and staging of packets at any rate (ingest.cu); nullptr: off
     struct oww_clip_resampler* clip_rs = nullptr;  // taps and tile tables of oww_resample_clips (ingest.cu); nullptr: unused
+    struct oww_mixer* mixer = nullptr;    // tables and scratch of oww_mix_clips (mix.cu); nullptr: unused
 };
 
 int oww_fail(oww_ctx* ctx, int code, const char* fmt, ...);
 void oww_verifier_fit_free(oww_ctx* ctx);          // verifier_fit.cu: the training scratch
+void oww_mix_free(oww_ctx* ctx);                   // mix.cu: the mixer's tables and scratch
 // 64-bit FNV-1a of `bytes` bytes, continuing from h (the stream record's configuration key)
 inline uint64_t oww_fnv1a(const void* p, size_t bytes, uint64_t h = 14695981039346656037ull) {
     const unsigned char* c = static_cast<const unsigned char*>(p);

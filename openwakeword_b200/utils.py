@@ -303,6 +303,15 @@ class AudioFeatures:
                                 torch.cuda.current_stream(d_out.device).cuda_stream)
         return d_out, out_off
 
+    def mix_clips(self, fg, bg, n_samples, params, rirs=None):
+        """Foreground clips mixed with background clips at an SNR, reverberated with room impulse responses and levelled,
+        on the device in one call (include/owwb200.h, oww_mix_clips): the noisy, reverberant positives of a false-reject
+        evaluation (the reference's mix_clips_batch).  ``fg`` and ``bg`` are int16 clips, ``rirs`` float32 ones, each a
+        sequence of 1-D arrays or a ``(pcm, offsets)`` pair; ``params`` holds one ``_native.MIX_DTYPE`` record per
+        mixture.  Returns (int16 CUDA tensor [n_mix, n_samples], bool CUDA tensor [n_mix] valid); the tensor goes to
+        ``predict_clips_array`` / ``predict_clips_ragged`` / ``detect_clips`` as it is."""
+        return _mix_clips_on(self.ctx, self.device_index, fg, bg, n_samples, params, rirs)
+
     # ---- streaming ----
     def _coerce(self, x):
         x = np.asarray(x)
@@ -542,6 +551,45 @@ def audio_history_samples(seconds):
     if n < 0 or n % CHUNK or n > 60 * 16000 or abs(n - float(seconds) * 16000) > 1e-6 * max(n, 1):
         raise ValueError(f"audio_history={seconds}: seconds in whole 80 ms chunks (a multiple of 0.08), at most 60")
     return n
+
+
+def _packed_clips(clips, dtype, dev):
+    """A sequence of 1-D arrays or a (pcm, offsets) pair, told apart by the int64 offsets -> (CUDA tensor of `dtype`,
+    int64 host offsets)"""
+    torch = _torch()
+    if isinstance(clips, tuple) and len(clips) == 2 and np.asarray(clips[1]).dtype == np.int64:
+        pcm, off = clips
+        off = np.ascontiguousarray(off, np.int64).ravel()
+    else:
+        parts = [np.asarray(c).ravel() for c in clips]
+        off = np.concatenate([[0], np.cumsum([p.size for p in parts], dtype=np.int64)]).astype(np.int64)
+        pcm = np.concatenate(parts) if parts else np.zeros(0, dtype)
+    if isinstance(pcm, torch.Tensor):
+        if pcm.dtype != getattr(torch, np.dtype(dtype).name):
+            raise ValueError(f"clips must be {np.dtype(dtype).name}, got {pcm.dtype}")
+        d = pcm.to(dev).contiguous().reshape(-1)
+    else:
+        pcm = np.asarray(pcm)
+        if pcm.dtype != dtype:
+            raise ValueError(f"clips must be {np.dtype(dtype).name}, got {pcm.dtype}")
+        d = torch.from_numpy(np.ascontiguousarray(pcm).reshape(-1)).to(dev)
+    return d, off
+
+
+def _mix_clips_on(ctx, device_index, fg, bg, n_samples, params, rirs=None):
+    """AudioFeatures.mix_clips on a bare Context (data.mix_clips_batch needs no model weights)"""
+    torch = _torch()
+    dev = f"cuda:{device_index}"
+    params = np.ascontiguousarray(params, _native.MIX_DTYPE).ravel()
+    d_fg, fg_off = _packed_clips(fg, np.int16, dev)
+    d_bg, bg_off = _packed_clips(bg, np.int16, dev)
+    d_rir, rir_off = _packed_clips([] if rirs is None else rirs, np.float32, dev)
+    n = params.size
+    out = torch.empty((n, int(n_samples)), dtype=torch.int16, device=dev)
+    valid = torch.empty(n, dtype=torch.uint8, device=dev)
+    ctx.mix_clips(d_fg, fg_off, d_bg, bg_off, d_rir, rir_off, params, int(n_samples), out, valid,
+                  torch.cuda.current_stream(out.device).cuda_stream)
+    return out, valid.bool()
 
 
 def _take_rows(dst, src, rows, maximum):
