@@ -1,12 +1,17 @@
-"""Shared test helpers: golden-case loading and the synthetic weight set the goldens were made with."""
+"""Shared test helpers: golden-case loading, the synthetic weight set the goldens were made with, the Models the host
+tests build, and the verifier arithmetic of verifier.cu in NumPy."""
 import glob
 import os
 
 import numpy as np
 
+import openwakeword_b200 as owb
 from openwakeword_b200 import weights as W
+from openwakeword_b200.custom_verifier_model import load_verifier
 
 GOLDEN = os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden")
+NAMES = ["alexa_v0.1", "timer_v0.1", "hey_jarvis_v0.1"]
+VERIFIER_CASES = ["verifier_alexa_c1280", "verifier_alexa_c2560", "verifier_timer_c1280", "verifier_timer_c2560"]
 
 HEAD_SPECS = {   # must match tests/golden/make_golden.py
     "alexa_v0.1": dict(n_in=16, hidden=64, n_blocks=1, n_out=1, layernorm=True, final="sigmoid", seed=1),
@@ -65,3 +70,41 @@ def load_case(tag):
         if k in c:
             c[k] = [str(s) for s in c[k]]
     return c
+
+
+def case_model(c, **kw):
+    """the Model of golden case c: its models, embedding seed and feature_init, max_chunks 8"""
+    specs = [{"name": n, "head": head(n), "class_mapping": class_mapping([n]).get(n)} for n in c["names"]]
+    return owb.Model(wakeword_models=specs, embedding_model_path=emb_weights(int(c["emb_seed"])),
+                     feature_init=c["feature_init"], max_chunks=8, **kw)
+
+
+def streams_model(B, fi, names=NAMES, max_chunks=2, **kw):
+    """a Model of B streams on the models `names`"""
+    specs = [{"name": n, "head": head(n), "class_mapping": class_mapping([n]).get(n)} for n in names]
+    return owb.Model(wakeword_models=specs, embedding_model_path=emb_weights(), feature_init=fi, n_streams=B,
+                     max_chunks=max_chunks, **kw)
+
+
+def verifier_pipeline(tag):
+    return load_verifier(os.path.join(GOLDEN, f"verifier_{tag}.pkl"))
+
+
+def kernel_order_proba(mean, weight, bias, feats):
+    """verifier.cu in NumPy fp32: lane l accumulates float4 l, l+32, ... with fmaf (x - mu) * w in x, y, z, w order,
+    then the xor-shuffle tree; p = 1 / (1 + exp(-(bias + acc))).  feats [n, n_in, 96] -> float32 [n]."""
+    x = np.asarray(feats, np.float32).reshape(len(feats), -1)
+    d = (x - mean[None]).astype(np.float32)
+    n, D = x.shape
+    lanes = np.zeros((n, 32), np.float32)
+    for j in range(D // 4):
+        for e in range(4):
+            k = 4 * j + e
+            # fmaf: the fp32 product is exact in float64, one rounding of the sum
+            lanes[:, j % 32] = (d[:, k].astype(np.float64) * np.float64(weight[k]) + lanes[:, j % 32]).astype(np.float32)
+    off = 16
+    while off:
+        lanes = (lanes + lanes[:, np.arange(32) ^ off]).astype(np.float32)
+        off >>= 1
+    z = (np.float32(bias) + lanes[:, 0]).astype(np.float32)
+    return (np.float32(1) / (np.float32(1) + np.exp(-z))).astype(np.float32)

@@ -11,7 +11,7 @@ import pytest
 import openwakeword_b200 as owb
 from openwakeword_b200 import _native, weights as W, registry
 from openwakeword_b200.utils import re_arg
-from helpers import emb_weights, head, class_mapping, golden_cases, load_case, TIMER_MAP
+from helpers import case_model as _model, emb_weights, head, class_mapping, golden_cases, load_case, TIMER_MAP
 import fake_backend
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
@@ -84,13 +84,6 @@ def test_re_arg():
 @pytest.fixture
 def fake_ctx(monkeypatch):
     monkeypatch.setattr(_native, "Context", fake_backend.FakeContext)
-    yield
-
-
-def _model(c, **kw):
-    specs = [{"name": n, "head": head(n), "class_mapping": class_mapping([n]).get(n)} for n in c["names"]]
-    return owb.Model(wakeword_models=specs, embedding_model_path=emb_weights(int(c["emb_seed"])),
-                     feature_init=c["feature_init"], max_chunks=8, **kw)
 
 
 @pytest.mark.parametrize("tag", golden_cases("predict_clip"))

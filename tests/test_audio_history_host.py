@@ -6,137 +6,25 @@ import os
 
 import numpy as np
 import pytest
-import torch
 
 import fake_backend
 from openwakeword_b200 import _native
 from openwakeword_b200.utils import AudioFeatures, audio_history_samples
-from test_detect_host import DetectFakeContext, _model
-from helpers import emb_weights
+from helpers import emb_weights, streams_model as _model
 
 GOLDEN = os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden", "raw_buffer.npz")
 
 
-class _AudioRing:
-    """The audio calls of _native.Context on a NumPy ring: ring [B, H], pos [B]; every step appends what it steps."""
-    audio_history = 0
-
-    def set_audio_history(self, n):
-        if n < 0 or n % 1280 or n > 960000:
-            raise _native.NativeError("n_samples")
-        self.audio_history = n
-        self._alloc_ring()
-
-    def _alloc_ring(self):
-        B = getattr(self, "_n", 0)
-        self.ring = np.zeros((B, self.audio_history), np.int16)
-        self.pos = np.zeros(B, np.int64)
-
-    def set_streams(self, n):
-        super().set_streams(n)
-        self._alloc_ring()
-
-    def reset(self, stream_ids=None, feature_init=None):
-        super().reset(stream_ids, feature_init)
-        if self.audio_history:
-            self.pos[slice(None) if stream_ids is None else np.asarray(stream_ids, np.int64)] = 0
-
-    def _append(self, b, x):
-        H = self.audio_history
-        if not H:
-            return
-        p = self.pos[b] + np.arange(x.size)
-        self.ring[b, p % H] = x
-        self.pos[b] += x.size
-
-    def _window(self, b, e, n):
-        H, p = self.audio_history, self.pos[b]
-        q = np.arange(e - n, e)
-        ok = (q >= max(p - H, 0)) & (q < p)
-        out = np.zeros(n, np.int16)
-        out[ok] = self.ring[b, q[ok] % H]
-        return out
-
-    def step_host(self, pcm, n_chunks, scores_out):
-        for b in range(self._n):
-            self._append(b, pcm[b, :n_chunks * 1280])
-        self._step_host(pcm, n_chunks, scores_out)
-
-    def step_host_ragged(self, pcm, chunks, scores_out):
-        for b in range(self._n):
-            self._append(b, pcm[b, :int(chunks[b]) * 1280])
-        self._step_host_ragged(pcm, chunks, scores_out)
-
-    def _need(self):
-        if not self.audio_history:
-            raise _native.NativeError("no audio history")
-
-    def audio_state(self, stream_ids):
-        self._need()
-        H = self.audio_history
-        ids = np.asarray(stream_ids, np.int64)
-        return np.stack([self._window(b, self.pos[b], H) for b in ids]).reshape(ids.size, H), self.pos[ids].copy()
-
-    def set_audio_state(self, stream_ids, audio, pos):
-        self._need()
-        ids = np.asarray(stream_ids, np.int64)
-        if len(set(ids.tolist())) != ids.size:
-            raise _native.NativeError("duplicate ids")
-        audio = np.asarray(audio, np.int16)
-        if audio.shape != (ids.size, self.audio_history):
-            raise ValueError("audio shape")
-        H = self.audio_history
-        for i, b in enumerate(ids):
-            p = max(int(pos[i]), 0)
-            self.ring[b, (p + np.arange(H)) % H] = audio[i]
-            self.pos[b] = p
-
-    def read_audio(self, stream_ids, n_samples, ends=None):
-        self._need()
-        ids = np.asarray(stream_ids, np.int64).ravel()
-        e = [self.pos[b] if ends is None or ends[i] < 0 else ends[i] for i, b in enumerate(ids)]
-        out = np.stack([self._window(b, e[i], n_samples) for i, b in enumerate(ids)]) if ids.size else \
-            np.zeros((0, n_samples), np.int16)
-        return torch.from_numpy(out), torch.from_numpy(self.pos[ids].copy())
-
-    def detect_capture(self, d_scores, prepared, n_samples, max_events=None):
-        self._need()
-        events, n = self.detect_events(d_scores, prepared, None, max_events)
-        clips = np.stack([self._window(b, self.pos[b], n_samples) for b in events["stream"]]) if len(events) else \
-            np.zeros((0, n_samples), np.int16)
-        return events, n, torch.from_numpy(clips), self.pos[events["stream"]].copy()
-
-
-class AudioOnlyContext(_AudioRing, fake_backend.FakeContext):
-    """Steps record the audio and nothing else (no features, no scores)."""
-
-    def _step_host(self, pcm, n_chunks, scores_out):
-        pass
-
-    def _step_host_ragged(self, pcm, chunks, scores_out):
-        pass
-
-
-class AudioDetectContext(_AudioRing, DetectFakeContext):
-    """DetectFakeContext (the oracle behind every step and detection) with the audio ring."""
-
-    def _step_host(self, pcm, n_chunks, scores_out):
-        DetectFakeContext.step_host(self, pcm, n_chunks, scores_out)
-
-    def _step_host_ragged(self, pcm, chunks, scores_out):
-        DetectFakeContext.step_host_ragged(self, pcm, chunks, scores_out)
-
-
 @pytest.fixture
 def audio_only(monkeypatch):
-    monkeypatch.setattr(_native, "Context", AudioOnlyContext)
-    yield
+    """steps record the audio and nothing else (no features, no scores)"""
+    monkeypatch.setattr(_native, "Context", fake_backend.FakeContext)
+    monkeypatch.setattr(fake_backend.FakeContext, "features", False)
 
 
 @pytest.fixture
 def audio_detect(monkeypatch):
-    monkeypatch.setattr(_native, "Context", AudioDetectContext)
-    yield
+    monkeypatch.setattr(_native, "Context", fake_backend.FakeContext)
 
 
 def _features(n_streams=1, seconds=10.0):

@@ -6,27 +6,21 @@ refusals of the bulk entry points, which come before any device work."""
 import numpy as np
 import pytest
 
+import fake_backend
 import openwakeword_b200 as owb
 from clip_detect_ref import ClipDetector, chunks_of_call, detect_clips, prepared_of_call
-from helpers import TIMER_MAP, emb_weights, head, load_case
+from helpers import NAMES, TIMER_MAP, emb_weights, head, load_case
 from openwakeword_b200 import _native
 from oracle import detect as odet
-from test_detect_host import DetectFakeContext
 
 f32 = np.float32
-NAMES = ["alexa_v0.1", "timer_v0.1", "hey_jarvis_v0.1"]
 # class 7 lies past the timer head's 7 outputs: a label whose column is -1
 TIMER_PAST = dict(TIMER_MAP, **{"7": "2_hour_timer"})
 
 
-class ClipHostContext(DetectFakeContext):
-    """DetectFakeContext; the bulk entry points are not run here (they need the device), only their refusals."""
-
-
 @pytest.fixture
 def fake_ctx(monkeypatch):
-    monkeypatch.setattr(_native, "Context", ClipHostContext)
-    yield
+    monkeypatch.setattr(_native, "Context", fake_backend.FakeContext)
 
 
 def _model(fi, names=NAMES, max_chunks=3):

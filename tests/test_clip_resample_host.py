@@ -14,10 +14,10 @@ import pytest
 import scipy.signal as ss
 
 import clip_resample_ref as cref
+import fake_backend
 from helpers import emb_weights, head
 from openwakeword_b200 import _native
 from oracle import resample as ores
-from test_ingest_host import IngestFakeContext
 
 CHUNK = 1280
 FI = np.zeros((41, 96), np.float32)
@@ -107,23 +107,12 @@ def test_wav_reader(built_library, tmp_path):
 
 
 # ---- routing on the stand-in ----
-class ClipFakeContext(IngestFakeContext):
-    """IngestFakeContext with oww_resample_clips through the float64 reference on the library's fp32 taps"""
-
-    def resample_clips(self, d_in, in_offsets, rates, pad_samples, d_out, out_offsets, stream=None):
-        for i, r in enumerate(rates):
-            h, _, _ = _native.resampler_taps(int(r))
-            x = d_in[in_offsets[i]:in_offsets[i + 1]]
-            y = cref.resample_clip(x, int(r), pad_samples, h=h.astype(np.float64) if h.size else None)
-            d_out[out_offsets[i]:out_offsets[i + 1]] = ores.to_int16(y)
-
-
 @pytest.fixture
 def routed(monkeypatch):
     """the stand-in, the resampler's calls recorded, and _predict_ragged replaced by a recorder (the bulk path needs a
     GPU): it returns one zero row per call of each clip"""
     from openwakeword_b200 import Model, utils
-    monkeypatch.setattr(_native, "Context", ClipFakeContext)
+    monkeypatch.setattr(_native, "Context", fake_backend.FakeContext)
     log = {"resample": [], "ragged": [], "init": []}
 
     def resample(self, pcm, offsets, rates, pad_samples=0):

@@ -5,82 +5,18 @@ on a twin Model, the hand-over of the history between the two, and the refusals.
 import numpy as np
 import pytest
 
+import fake_backend
 import openwakeword_b200 as owb
-from helpers import class_mapping, emb_weights, head, load_case
+from helpers import NAMES, emb_weights, head, load_case, streams_model as _model
 from openwakeword_b200 import _native
 from oracle import detect as odet
-from test_model_stream_state import StateFakeContext
 
-EVENT_DTYPE = _native.EVENT_DTYPE
 f32 = np.float32
-
-
-class DetectFakeContext(StateFakeContext):
-    """StateFakeContext with the detector calls of _native.Context, one oracle StreamDetector per stream; "device"
-    buffers are NumPy arrays."""
-
-    def set_streams(self, n):
-        super().set_streams(n)
-        self._new_detectors()
-
-    def _new_detectors(self):
-        self.det = [odet.StreamDetector(self._labels, self._debounce) for _ in range(self._n)] if getattr(self, "_labels", None) else None
-
-    def reset(self, stream_ids=None, feature_init=None):
-        super().reset(stream_ids, feature_init)
-        if getattr(self, "det", None):
-            for b in (range(self._n) if stream_ids is None else stream_ids):
-                self.det[b].reset()
-
-    def set_detector(self, table, debounce_time=0.0):
-        labels = [odet.Label(*row) for row in table]
-        odet.check(labels, debounce_time)
-        old = getattr(self, "_labels", None)
-        self._labels, self._debounce = labels, debounce_time
-        self.n_detect_labels = len(labels)
-        if old and [(a.column, a.repeats) for a in old] == [(a.column, a.repeats) for a in labels] and getattr(self, "det", None):
-            for d in self.det:
-                d.configure(labels, debounce_time)
-        else:
-            self._new_detectors()
-
-    def new_scores(self):
-        return np.zeros((self._n, self.n_outputs), np.float32)
-
-    def step_pcm(self, pcm, n_chunks, d_scores):
-        self.step_host(pcm, n_chunks, d_scores)
-
-    def step_ragged_pcm(self, pcm, chunks, d_scores):
-        self.step_host_ragged(pcm, chunks, d_scores)
-
-    def detect_events(self, d_scores, prepared, d_final=None, max_events=None):
-        prepared = np.broadcast_to(np.asarray(prepared, np.int32), (self._n,))
-        ev = []
-        for b in range(self._n):
-            r = self.det[b].detect(d_scores[b], int(prepared[b]))
-            if r is None:
-                continue
-            if d_final is not None:
-                d_final[b] = r[0]
-            ev += [(b, j, s, i) for j, s, i in r[1]]
-        cap = self._n * self.n_detect_labels if max_events is None else max_events
-        return np.array(ev[:cap], EVENT_DTYPE), len(ev)
-
-    def detector_history(self, stream_ids):
-        out = [self.det[b].export() for b in stream_ids]
-        return (np.stack([h for h, _ in out]).reshape(len(out), self.n_detect_labels, 30),
-                np.array([c for _, c in out], np.int32))
-
-    def set_detector_history(self, stream_ids, hist, counts):
-        assert len(set(int(b) for b in stream_ids)) == len(stream_ids)
-        for i, b in enumerate(stream_ids):
-            self.det[b].load(hist[i], counts[i])
 
 
 @pytest.fixture
 def fake_ctx(monkeypatch):
-    monkeypatch.setattr(_native, "Context", DetectFakeContext)
-    yield
+    monkeypatch.setattr(_native, "Context", fake_backend.FakeContext)
 
 
 # ---- the oracle, branch by branch ----
@@ -183,15 +119,6 @@ def test_oracle_export_load_round_trip():
 
 
 # ---- Model.detect on the stand-in ----
-NAMES = ["alexa_v0.1", "timer_v0.1", "hey_jarvis_v0.1"]
-
-
-def _model(B, fi, names=NAMES, max_chunks=2, **kw):
-    specs = [{"name": n, "head": head(n), "class_mapping": class_mapping([n]).get(n)} for n in names]
-    return owb.Model(wakeword_models=specs, embedding_model_path=emb_weights(), feature_init=fi, n_streams=B,
-                     max_chunks=max_chunks, **kw)
-
-
 @pytest.mark.parametrize("tag", ["jane_debounce", "jane_patience"])
 def test_detect_fires_where_the_golden_scores_reach_the_threshold(fake_ctx, tag):
     c = load_case(tag)

@@ -14,9 +14,9 @@ import wave
 import numpy as np
 import pytest
 
-from helpers import GOLDEN, class_mapping, emb_weights, golden_cases, head, load_case
+from helpers import (GOLDEN, VERIFIER_CASES, case_model as _model, class_mapping, emb_weights, golden_cases, head,
+                     load_case)
 from test_gpu_parity import SCORE_TOL, _gated_error
-from test_verifier_host import VERIFIER_CASES, _model
 
 pytestmark = pytest.mark.gpu
 

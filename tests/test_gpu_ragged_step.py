@@ -303,14 +303,14 @@ def test_model_predict_ragged_gpu_equals_cpu_fake(torch_cuda, built_library, mon
     reset_streams: every label within 1e-3."""
     import openwakeword_b200 as owb
     from openwakeword_b200 import _native
-    from helpers import class_mapping
-    from test_model_ragged import NAMES, RaggedFakeContext
+    import fake_backend
+    from helpers import NAMES, class_mapping
     rng = np.random.default_rng(21)
     B, mc = 7, 2
     fi = rng.normal(0, 1, (41, 96)).astype(np.float32)
     specs = [{"name": n, "head": head(n), "class_mapping": class_mapping([n]).get(n)} for n in NAMES]
     kw = dict(wakeword_models=specs, embedding_model_path=emb_weights(), feature_init=fi, n_streams=B, max_chunks=mc)
-    monkeypatch.setattr(_native, "Context", RaggedFakeContext)
+    monkeypatch.setattr(_native, "Context", fake_backend.FakeContext)
     cpu = owb.Model(**kw)
     monkeypatch.undo()
     gpu = owb.Model(**kw)
@@ -340,8 +340,7 @@ def test_model_predict_ragged_custom_verifiers(torch_cuda, built_library):
     streams whose call exceeds max_chunks verify the max, on the host, as predict does."""
     from openwakeword_b200 import Model
     from oracle.verifier import VerifiedOracleModel
-    from helpers import load_case
-    from test_verifier_host import _pipeline
+    from helpers import load_case, verifier_pipeline as _pipeline
     c = load_case("verifier_alexa_c1280")
     name = c["names"][0]
     rng = np.random.default_rng(17)

@@ -5,8 +5,8 @@ import os
 import numpy as np
 import pytest
 
-from helpers import GOLDEN, emb_weights, head, class_mapping, load_case
-from test_verifier_host import VERIFIER_CASES, FakeVerifierContext, _pipeline, _model
+import fake_backend
+from helpers import GOLDEN, VERIFIER_CASES, case_model as _model, emb_weights, head, load_case, verifier_pipeline as _pipeline
 
 pytestmark = pytest.mark.gpu
 
@@ -183,7 +183,7 @@ def test_151_streams_vs_oracle_and_host_path(torch_cuda, built_library, mode, sp
     # oracle: the fake context (NumPy graphs + the kernel's verifier arithmetic) on sampled streams
     if "oracle" not in _oracle_cache:
         sample = sorted({0, 1, 2, 3, 75, 76, 150} | set(swap_ids[:3].tolist()))
-        fake = FakeVerifierContext()
+        fake = fake_backend.FakeContext()
         fake.rows = np.array(sample)
         fake.load_embedding(W.pack_embedding_blob(emb_weights()))
         for h in (head("alexa_v0.1"), head("timer_v0.1")):

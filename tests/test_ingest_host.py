@@ -5,16 +5,16 @@
 * the float64 streaming oracle (oracle/resample.py) against scipy.signal.upfirdn over random packet splits, with empty,
   1-sample and prime-length packets, and its final-output count against A(S) = ceil(S*up/down);
 * the library's pure-host arithmetic (oww_ingest_plan, which oww_ingest and oww_ingest_capacity run) against the oracle;
-* Model routing, splitting of long calls, refusals and export / import of the ingest state, on a stand-in of the C ABI
-  (the detector stand-in of test_detect_host.py plus ingest through the oracle)."""
+* Model routing, splitting of long calls, refusals and export / import of the ingest state, on the stand-in of the C
+  ABI (ingest through the oracle)."""
 import numpy as np
 import pytest
 import scipy.signal as ss
 
+import fake_backend
 from helpers import emb_weights, head
 from openwakeword_b200 import _native
 from oracle import resample as ores
-from test_detect_host import DetectFakeContext
 
 CHUNK = 1280
 FI = np.zeros((41, 96), np.float32)
@@ -90,94 +90,9 @@ def test_library_plan_matches_the_oracle(built_library, rate):
         assert n_out == CHUNK and chunks == 1
 
 
-class IngestFakeContext(DetectFakeContext):
-    """DetectFakeContext with the ingest calls: resampling by the oracle (the library's fp32 taps in float64, rounded
-    half to even), the capacity from the library's own host arithmetic, steps through step_host_ragged."""
-    _ing = None
-
-    def _new_ing(self):
-        n = self._n
-        self._ing = dict(rate=np.full(n, 16000, np.int32), S=np.zeros(n, np.int64),
-                         staged=[np.zeros(0, np.int16) for _ in range(n)], res=[None] * n)
-
-    def set_streams(self, n):
-        super().set_streams(n)
-        if self._ing is not None:
-            self._new_ing()
-
-    def reset(self, stream_ids=None, feature_init=None):
-        super().reset(stream_ids, feature_init)
-        if self._ing is not None:
-            for b in (range(self._n) if stream_ids is None else stream_ids):
-                self._ing["S"][b], self._ing["staged"][b], self._ing["res"][b] = 0, np.zeros(0, np.int16), None
-
-    def set_input_rates(self, stream_ids, rates, stream=None):
-        for r in np.unique(rates):
-            _native.resampler_taps(int(r))
-        if self._ing is None:
-            self._new_ing()
-        ids = range(self._n) if stream_ids is None else stream_ids
-        for b, r in zip(ids, rates):
-            self._ing["rate"][b], self._ing["S"][b], self._ing["res"][b] = r, 0, None
-
-    def _res(self, b):
-        g = self._ing
-        if g["res"][b] is None:
-            h, _, _ = _native.resampler_taps(int(g["rate"][b]))
-            g["res"][b] = ores.StreamResampler(int(g["rate"][b]), h=h.astype(np.float64) if h.size else None)
-            g["res"][b].S = int(g["S"][b])
-        return g["res"][b]
-
-    def ingest_capacity(self):
-        g = self._ing
-        return np.array([_native.ingest_plan(int(g["rate"][b]), self.max_chunks, int(g["S"][b]), g["staged"][b].size, 0)[3]
-                         for b in range(self._n)], np.int64)
-
-    def ingest_pcm(self, pcm, offsets, d_scores):
-        g, B = self._ing, self._n
-        n = np.diff(offsets)
-        if (n > self.ingest_capacity()).any():
-            raise _native.NativeError("over capacity")
-        tot = []
-        for b in range(B):
-            y = self._res(b).feed(pcm[offsets[b]:offsets[b + 1]])
-            tot.append(np.concatenate((g["staged"][b], ores.to_int16(y))))
-            g["S"][b] += n[b]
-        chunks = np.array([t.size // CHUNK for t in tot], np.int32)
-        if chunks.max() > 0:
-            x = np.zeros((B, int(chunks.max()) * CHUNK), np.int16)
-            for b in range(B):
-                x[b, :chunks[b] * CHUNK] = tot[b][:chunks[b] * CHUNK]
-            self.step_host_ragged(x, chunks, d_scores)
-        g["staged"] = [t[c * CHUNK:] for t, c in zip(tot, chunks)]
-        return chunks, np.where(chunks > 0, chunks * CHUNK, [t.size for t in tot]).astype(np.int32)
-
-    def ingest_state(self, stream_ids, samples=True):
-        g = self._ing
-        ids = list(stream_ids)
-        staged = np.array([g["staged"][b].size for b in ids], np.int32)
-        x = np.zeros((len(ids), max(int(staged.max(initial=0)), 1)), np.int16)
-        hist = np.zeros((len(ids), 128), np.int16)
-        for i, b in enumerate(ids):
-            x[i, :staged[i]] = g["staged"][b]
-            if g["rate"][b] != 16000 and g["S"][b]:
-                hist[i] = np.asarray(self._res(b).hist[-128:], np.int16)
-        return g["rate"][ids].copy(), g["S"][ids].copy(), staged, x, hist
-
-    def set_ingest_state(self, stream_ids, rates, consumed, staged, samples, hist):
-        g = self._ing
-        assert len(set(int(b) for b in stream_ids)) == len(stream_ids)
-        for i, b in enumerate(stream_ids):
-            g["rate"][b], g["S"][b], g["res"][b] = rates[i], consumed[i], None
-            g["staged"][b] = np.asarray(samples[i, :staged[i]], np.int16).copy()
-            if rates[i] != 16000:
-                self._res(b).hist[-128:] = hist[i]
-
-
 @pytest.fixture
 def ingest_ctx(monkeypatch):
-    monkeypatch.setattr(_native, "Context", IngestFakeContext)
-    yield
+    monkeypatch.setattr(_native, "Context", fake_backend.FakeContext)
 
 
 def _model(B, sr, **kw):

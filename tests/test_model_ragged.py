@@ -7,39 +7,16 @@ import pytest
 
 import fake_backend
 import openwakeword_b200 as owb
-from helpers import class_mapping, emb_weights, head
+from helpers import NAMES, class_mapping, emb_weights, head
 from openwakeword_b200 import _native
-from oracle import heads as oheads, streaming
+from oracle import streaming
 
-NAMES = ["alexa_v0.1", "timer_v0.1", "hey_jarvis_v0.1"]
 MAX_CHUNKS = 2
-
-
-class RaggedFakeContext(fake_backend.FakeContext):
-    """FakeContext with the ragged host step: stream b steps chunks[b] chunks of its row, held streams are skipped."""
-
-    def step_host_ragged(self, pcm, chunks, scores_out):
-        for b in range(self._n):
-            c = int(chunks[b])
-            if c == 0:
-                continue
-            assert self.af[b](pcm[b, :c * 1280]) == c * 1280
-            per_head = []
-            for h in self.heads:
-                n_in = h["n_in"]
-                per_head.append(np.stack([oheads.forward(h, self.af[b].get_features(n_in, -n_in - i))[0]
-                                          for i in range(c - 1, -1, -1)]))
-            raw = np.concatenate(per_head, axis=1)
-            for m, v, thr in self.gates:
-                cm, cv = self._col0(m), self._col0(v)
-                raw[:, cm] = np.where(raw[:, cm] > np.float32(thr), raw[:, cv], raw[:, cm])
-            scores_out[b, :raw.shape[1]] = raw.max(axis=0)
 
 
 @pytest.fixture
 def fake_ctx(monkeypatch):
-    monkeypatch.setattr(_native, "Context", RaggedFakeContext)
-    yield
+    monkeypatch.setattr(_native, "Context", fake_backend.FakeContext)
 
 
 def _models(B, fi):

@@ -5,68 +5,13 @@ import pytest
 
 import fake_backend
 from helpers import emb_weights, head
-from oracle import heads as oheads
 from openwakeword_b200 import _native, weights as W
 import openwakeword_b200 as owb
 
 
-class FakeBankContext(fake_backend.FakeContext):
-    """FakeContext plus head banks with the semantics of include/owwb200.h: the bank's columns follow the heads', a
-    stream on slot k gets head k's max over its chunk windows, a stream on slot -1 gets 0."""
-
-    def __init__(self, *a, **kw):
-        super().__init__(*a, **kw)
-        self.hbanks = []
-
-    @property
-    def n_outputs(self):
-        return super().n_outputs + sum(b["n_out"] for b in self.hbanks)
-
-    def add_head_bank(self, n_in, dims, layernorm, final_act, capacity):
-        self.hbanks.append({"shape": (n_in, list(dims), layernorm, final_act), "n_out": dims[-1], "capacity": capacity,
-                            "heads": [None] * capacity, "assign": None, "clip": -1})
-        return len(self.hbanks) - 1
-
-    def load_bank_head(self, bank, slot, blob):
-        b = self.hbanks[bank]
-        assert 0 <= slot < b["capacity"]
-        b["heads"][slot] = fake_backend.unpack_head_blob(*b["shape"], np.asarray(blob, np.float32))
-
-    def set_streams(self, n):
-        super().set_streams(n)
-        for b in self.hbanks:
-            b["assign"] = np.full(n, -1, np.int32)
-
-    def assign_bank_head(self, bank, stream_ids, slots, stream=None):
-        b = self.hbanks[bank]
-        ids = np.arange(self._n) if stream_ids is None else np.asarray(stream_ids)
-        for i, s in zip(ids, np.asarray(slots)):
-            assert s == -1 or b["heads"][s] is not None
-            b["assign"][i] = s
-
-    def set_head_bank_clip_slot(self, bank, slot):
-        self.hbanks[bank]["clip"] = slot
-
-    def step_host(self, pcm, n_chunks, scores_out):
-        super().step_host(pcm, n_chunks, scores_out)
-        col = super().n_outputs
-        for b in self.hbanks:
-            for s in range(self._n):
-                k = b["assign"][s]
-                if k < 0:
-                    scores_out[s, col:col + b["n_out"]] = 0.0
-                    continue
-                h = b["heads"][k]
-                g = [oheads.forward(h, self.af[s].get_features(h["n_in"], -h["n_in"] - i))[0]
-                     for i in range(n_chunks - 1, -1, -1)]
-                scores_out[s, col:col + b["n_out"]] = np.stack(g).max(axis=0)
-            col += b["n_out"]
-
-
 @pytest.fixture
 def fake_bctx(monkeypatch):
-    monkeypatch.setattr(_native, "Context", FakeBankContext)
-    yield
+    monkeypatch.setattr(_native, "Context", fake_backend.FakeContext)
 
 
 FI = np.random.default_rng(0).normal(0, 1, (41, 96)).astype(np.float32)

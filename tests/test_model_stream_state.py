@@ -1,8 +1,7 @@
-"""Model.export_streams / Model.import_streams on the CPU (no GPU), with a stand-in of the C ABI defined here: a stream
+"""Model.export_streams / Model.import_streams on the CPU (no GPU), on the CPU stand-in of the C ABI: a stream
 moved to another Model of the same configuration returns, call for call, what the unmoved stream returns - through
 lockstep ``predict`` and ``predict_ragged``, remainders below 1280 samples, the first-5 zeroing, patience and debounce
 history - also after a pickle round trip of the CPU StreamState.  The refusals raise ValueError."""
-import hashlib
 import pickle
 
 import numpy as np
@@ -10,74 +9,15 @@ import pytest
 
 import fake_backend
 import openwakeword_b200 as owb
-from helpers import class_mapping, emb_weights, head
+from helpers import NAMES, class_mapping, emb_weights, head
 from openwakeword_b200 import _native
-from oracle import heads as oheads
 
-NAMES = ["alexa_v0.1", "timer_v0.1", "hey_jarvis_v0.1"]
 MAX_CHUNKS = 2
-_FIELDS = ("raw", "melspectrogram_buffer", "accumulated_samples", "remainder", "feature_buffer")
-
-
-class StateFakeContext(fake_backend.FakeContext):
-    """FakeContext with the ragged host step and stream records: a record is [payload bytes, configuration key, the
-    pickled oracle state of the stream], the key at bytes 8..16 as in the library's records."""
-    RECORD_BYTES = 1 << 20
-
-    def __init__(self, *args, cnn_mode=0, split_from=None, **kw):
-        super().__init__(*args, cnn_mode=cnn_mode, split_from=split_from, **kw)
-        self._config = (cnn_mode, split_from)
-
-    def step_host_ragged(self, pcm, chunks, scores_out):
-        for b in range(self._n):
-            c = int(chunks[b])
-            if c == 0:
-                continue
-            assert self.af[b](pcm[b, :c * 1280]) == c * 1280
-            per_head = []
-            for h in self.heads:
-                n_in = h["n_in"]
-                per_head.append(np.stack([oheads.forward(h, self.af[b].get_features(n_in, -n_in - i))[0]
-                                          for i in range(c - 1, -1, -1)]))
-            raw = np.concatenate(per_head, axis=1)
-            for m, v, thr in self.gates:
-                cm, cv = self._col0(m), self._col0(v)
-                raw[:, cm] = np.where(raw[:, cm] > np.float32(thr), raw[:, cv], raw[:, cm])
-            scores_out[b, :raw.shape[1]] = raw.max(axis=0)
-
-    def stream_state_info(self):
-        h = hashlib.sha256(repr(self._config).encode())
-        for c in self.emb["conv"]:
-            h.update(np.ascontiguousarray(c).tobytes())
-        return self.RECORD_BYTES, int.from_bytes(h.digest()[:8], "little")
-
-    def export_records(self, stream_ids, stream=None):
-        import torch
-        _, key = self.stream_state_info()
-        out = np.zeros((len(stream_ids), self.RECORD_BYTES), np.uint8)
-        for i, b in enumerate(stream_ids):
-            blob = pickle.dumps({k: getattr(self.af[b], k) for k in _FIELDS})
-            assert 16 + len(blob) <= self.RECORD_BYTES
-            out[i, :16] = np.frombuffer(np.array([len(blob), key], np.uint64).tobytes(), np.uint8)
-            out[i, 16:16 + len(blob)] = np.frombuffer(blob, np.uint8)
-        return torch.from_numpy(out)
-
-    def import_records(self, stream_ids, records, stream=None):
-        _, key = self.stream_state_info()
-        rec = records.cpu().numpy()
-        assert len(set(int(b) for b in stream_ids)) == len(stream_ids)
-        for i, b in enumerate(stream_ids):
-            n, k = np.frombuffer(rec[i, :16].tobytes(), np.uint64)
-            if int(k) != key:
-                raise ValueError("records of another configuration")
-            for f, v in pickle.loads(rec[i, 16:16 + int(n)].tobytes()).items():
-                setattr(self.af[b], f, v)
 
 
 @pytest.fixture
 def fake_ctx(monkeypatch):
-    monkeypatch.setattr(_native, "Context", StateFakeContext)
-    yield
+    monkeypatch.setattr(_native, "Context", fake_backend.FakeContext)
 
 
 def _model(B, fi, names=NAMES, **kw):

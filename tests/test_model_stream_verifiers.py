@@ -8,39 +8,13 @@ import pytest
 import openwakeword_b200 as owb
 from openwakeword_b200 import _native
 from openwakeword_b200 import weights as W
-from helpers import emb_weights
+from helpers import emb_weights, verifier_pipeline as _pipeline
 import fake_backend
-from test_model_stream_models import FakeBankContext
-from test_verifier_host import FakeVerifierContext, _pipeline
-
-
-class FakeStreamVerifierContext(FakeVerifierContext, FakeBankContext):
-    """FakeVerifierContext's banks plus verifier banks of head banks: a stream on head-bank slot -1 is never verified."""
-
-    def add_bank_verifier_bank(self, head_bank, capacity, threshold):
-        hb = self.hbanks[head_bank]
-        col0 = fake_backend.FakeContext.n_outputs.fget(self) + sum(b["n_out"] for b in self.hbanks[:head_bank])
-        self.banks.append(dict(col0=col0, n_cols=hb["n_out"], n_in=hb["shape"][0], thr=np.float32(threshold), slots={},
-                               assign=np.full(self._n, -1, np.int32), own=np.full(self._n, -1, np.int32), clip=-1,
-                               capacity=capacity, hbank=head_bank))
-        return len(self.banks) - 1
-
-    def assign_verifier(self, bank, stream_ids, slots, stream=None):
-        ids = np.arange(self._n) if stream_ids is None else np.asarray(stream_ids)
-        bk = self.banks[bank]
-        bk["own" if "hbank" in bk else "assign"][ids] = slots
-
-    def step_host(self, pcm, n_chunks, scores_out):
-        for bk in self.banks:
-            if "hbank" in bk:
-                bk["assign"] = np.where(self.hbanks[bk["hbank"]]["assign"] >= 0, bk["own"], -1).astype(np.int32)
-        super().step_host(pcm, n_chunks, scores_out)
 
 
 @pytest.fixture
 def fake_svctx(monkeypatch):
-    monkeypatch.setattr(_native, "Context", FakeStreamVerifierContext)
-    yield
+    monkeypatch.setattr(_native, "Context", fake_backend.FakeContext)
 
 
 FI = np.random.default_rng(0).normal(0, 1, (41, 96)).astype(np.float32)

@@ -11,106 +11,17 @@ import pytest
 
 import openwakeword_b200 as owb
 from openwakeword_b200 import _native
-from openwakeword_b200.custom_verifier_model import load_verifier, linear_verifier_params, flatten_features
-from helpers import GOLDEN, emb_weights, head, class_mapping, load_case
+from openwakeword_b200.custom_verifier_model import linear_verifier_params, flatten_features
+from helpers import (GOLDEN, VERIFIER_CASES, case_model as _model, emb_weights, head, class_mapping, kernel_order_proba,
+                     load_case, verifier_pipeline as _pipeline)
 import fake_backend
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-VERIFIER_CASES = ["verifier_alexa_c1280", "verifier_alexa_c2560", "verifier_timer_c1280", "verifier_timer_c2560"]
-
-
-def kernel_order_proba(mean, weight, bias, feats):
-    """verifier.cu in NumPy fp32: lane l accumulates float4 l, l+32, ... with fmaf (x - mu) * w in x, y, z, w order,
-    then the xor-shuffle tree; p = 1 / (1 + exp(-(bias + acc))).  feats [n, n_in, 96] -> float32 [n]."""
-    x = np.asarray(feats, np.float32).reshape(len(feats), -1)
-    d = (x - mean[None]).astype(np.float32)
-    n, D = x.shape
-    lanes = np.zeros((n, 32), np.float32)
-    for j in range(D // 4):
-        for e in range(4):
-            k = 4 * j + e
-            # fmaf: the fp32 product is exact in float64, one rounding of the sum
-            lanes[:, j % 32] = (d[:, k].astype(np.float64) * np.float64(weight[k]) + lanes[:, j % 32]).astype(np.float32)
-    off = 16
-    while off:
-        lanes = (lanes + lanes[:, np.arange(32) ^ off]).astype(np.float32)
-        off >>= 1
-    z = (np.float32(bias) + lanes[:, 0]).astype(np.float32)
-    return (np.float32(1) / (np.float32(1) + np.exp(-z))).astype(np.float32)
-
-
-class FakeVerifierContext(fake_backend.FakeContext):
-    """FakeContext plus verifier banks with the semantics of include/owwb200.h: after a step's scores (max over the
-    chunk windows), columns of the bank's head >= threshold (fp32) are replaced by p of the stream's slot."""
-
-    def __init__(self, *a, **kw):
-        super().__init__(*a, **kw)
-        self.banks = []
-        self.feature_reads = 0
-        self.verifiers_on = True
-
-    def set_streams(self, n):
-        super().set_streams(n)
-        for b in self.banks:
-            b["assign"] = np.full(n, -1, np.int32)
-
-    def add_verifier_bank(self, head_id, capacity, threshold):
-        h = self.heads[head_id]
-        self.banks.append(dict(col0=self._col0(head_id), n_cols=h["layers"][-1]["W"].shape[1], n_in=h["n_in"],
-                               thr=np.float32(threshold), slots={}, assign=np.full(self._n, -1, np.int32), clip=-1,
-                               capacity=capacity))
-        return len(self.banks) - 1
-
-    def load_verifier(self, bank, slot, mean, weight, bias):
-        assert 0 <= slot < self.banks[bank]["capacity"]
-        self.banks[bank]["slots"][slot] = (np.asarray(mean, np.float32), np.asarray(weight, np.float32), np.float32(bias))
-
-    def assign_verifier(self, bank, stream_ids, slots, stream=None):
-        ids = np.arange(self._n) if stream_ids is None else np.asarray(stream_ids)
-        self.banks[bank]["assign"][ids] = slots
-
-    def set_verifier_clip_slot(self, bank, slot):
-        self.banks[bank]["clip"] = slot
-
-    def set_verifier_threshold(self, bank, threshold):
-        self.banks[bank]["thr"] = np.float32(threshold)
-
-    def enable_verifiers(self, enabled):
-        self.verifiers_on = bool(enabled)
-
-    def verifier_predict_host(self, bank, slot, feats):
-        return kernel_order_proba(*self.banks[bank]["slots"][slot], feats)
-
-    def step_host(self, pcm, n_chunks, scores_out):
-        super().step_host(pcm, n_chunks, scores_out)
-        for bk in (self.banks if self.verifiers_on else []):
-            for b in range(self._n):
-                slot = bk["assign"][b]
-                cols = scores_out[b, bk["col0"]:bk["col0"] + bk["n_cols"]]
-                if slot < 0 or not (cols >= bk["thr"]).any():
-                    continue
-                p = kernel_order_proba(*bk["slots"][slot], fake_backend.FakeContext.get_features(self, b, bk["n_in"])[None])[0]
-                cols[cols >= bk["thr"]] = p
-
-    def get_features(self, stream_id, n, back=0):
-        self.feature_reads += 1
-        return super().get_features(stream_id, n, back)
 
 
 @pytest.fixture
 def fake_vctx(monkeypatch):
-    monkeypatch.setattr(_native, "Context", FakeVerifierContext)
-    yield
-
-
-def _pipeline(tag):
-    return load_verifier(os.path.join(GOLDEN, f"verifier_{tag}.pkl"))
-
-
-def _model(c, **kw):
-    specs = [{"name": n, "head": head(n), "class_mapping": class_mapping([n]).get(n)} for n in c["names"]]
-    return owb.Model(wakeword_models=specs, embedding_model_path=emb_weights(int(c["emb_seed"])),
-                     feature_init=c["feature_init"], max_chunks=8, **kw)
+    monkeypatch.setattr(_native, "Context", fake_backend.FakeContext)
 
 
 def test_golden_pickle_loads_without_the_reference_package():
