@@ -1,11 +1,11 @@
-"""-m gpu: the fused step kernel (tc_inc_kernel) at every group size G = 1..7 and at split_from 11, 15 and 20.
+"""-m gpu: the fused step kernel (tc_inc_kernel) at every group size G = 1..7 and at every split_from (3, 7, 11, 15, 20).
 
 The kernel runs each layer as 64-position items spread over four warpgroups, with weight copies issued by one thread
 of the CTA; how many items a warpgroup takes (none, one or many), whether the last 64-row tile is partial and whether
 the last group of streams is ragged all depend on G.  The stream count of each case is chosen so that the library picks
 that G on this device, with a ragged last group; the handle's plan is read back to confirm it.  The padded clips are
 streamed one chunk per call and compared with oww_predict_clips_ragged on the same clips, whose CNN runs in
-tc_conv_kernel (same per-element arithmetic): feature rows bit for bit at every split; scores bit for bit at 11 and 15,
+tc_conv_kernel (same per-element arithmetic): feature rows bit for bit at every split; scores bit for bit below 20,
 where the heads run as their own launch, and within 2e-5 at 20, where they run inside the fused kernel (the bound of
 test_bulk_clips_equal_streaming_at_every_split)."""
 import ctypes as C
@@ -38,7 +38,7 @@ def _plan_g(built_library, h, G=0, n=0, split=20):
     return int(buf[0])
 
 
-@pytest.mark.parametrize("split", [11, 15, 20])
+@pytest.mark.parametrize("split", [3, 7, 11, 15, 20])
 @pytest.mark.parametrize("G", list(range(1, 8)))
 def test_fused_items_every_group_size(torch_cuda, built_library, G, split):
     torch = torch_cuda
