@@ -469,9 +469,10 @@ int oww_audio_import(oww_ctx* ctx, const int32_t* h_stream_ids, int n, const int
  *                       outside the table.
  *   oww_ingest_export / _import - stream h_stream_ids[i] <-> h_rates[i], h_consumed[i] (S, int64), h_staged[i] (host), its
  *                       staged samples in row i of d_staged [n][staged_stride] int16 (the rest of the row zero on export),
- *                       and its history in d_hist [n][128] int16 (oldest first).  Export fills the host arrays before
- *                       it returns; with d_staged and d_hist NULL it enqueues nothing (a query of the staged counts), else
- *                       staged_stride must hold every exported row.  Import takes rates from the table, h_staged[i] in
+ *                       and its history in d_hist [n][128] int16 (oldest first; zeros at 16000 Hz, which keeps none, and
+ *                       before the first input).  Export fills the host arrays before it returns; with d_staged and d_hist
+ *                       NULL it enqueues nothing (a query of the staged counts), else staged_stride must hold every
+ *                       exported row.  Import takes rates from the table, h_staged[i] in
  *                       [0, C], distinct ids; a moved stream continues bit for bit.  Stream-ordered on `stream`.
  * oww_reset / oww_reset_async clear the staged samples and the history of the streams they reset and keep their rates;
  * oww_set_streams sets every stream to 16000 with nothing staged.  The steps of oww_step* do not touch the ingest state

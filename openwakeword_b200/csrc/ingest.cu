@@ -533,7 +533,8 @@ int oww_ingest_export(oww_ctx* ctx, const int32_t* h_stream_ids, int n, int32_t*
         if (device && g->staged[b] > staged_stride)
             return oww_fail(ctx, OWW_EINVAL, "stream %d holds %d staged samples, staged_stride is %lld", b, g->staged[b],
                             (long long)staged_stride);
-        info[3 * i] = g->staged_off[b]; info[3 * i + 1] = g->staged[b]; info[3 * i + 2] = g->S[b] == 0;
+        // no history before the first input, and none at 16 kHz (the kernel keeps no filter state for a copy): zeros
+        info[3 * i] = g->staged_off[b]; info[3 * i + 1] = g->staged[b]; info[3 * i + 2] = g->S[b] == 0 || g->rate[b] == 16000;
     }
     for (int i = 0; i < n; ++i) {
         const int b = h_stream_ids[i];

@@ -60,6 +60,7 @@ class FakeContext:
         self.banks = []             # verifier banks, of ordinary heads and of head banks
         self.verifiers_on = True
         self.feature_reads = 0      # the host's get_features calls
+        self.unverified = {}        # stream -> its score row of its last step before the verifier banks
         self._n = 0
         self.det = self._labels = self._ing = None
 
@@ -89,6 +90,8 @@ class FakeContext:
 
     # ---- head banks: a stream on slot k gets head k's max over its chunk windows, a stream on slot -1 gets 0 ----
     def add_head_bank(self, n_in, dims, layernorm, final_act, capacity):
+        if self._config[0] == _native.CNN_FP32_WINDOW:
+            raise _native.NativeError("head banks run on the tensor cores: not in cnn_mode 0")
         self.hbanks.append({"shape": (n_in, list(dims), layernorm, final_act), "n_out": dims[-1], "capacity": capacity,
                             "heads": [None] * capacity, "assign": np.full(self._n, -1, np.int32), "clip": -1})
         return len(self.hbanks) - 1
@@ -187,9 +190,25 @@ class FakeContext:
 
     # ---- steps ----
     def _windows(self, b, h, chunks):
-        """head h on stream b's feature window of each of its last `chunks` chunks, oldest first -> [chunks, n_out]"""
-        return np.stack([oheads.forward(h, self.af[b].get_features(h["n_in"], -h["n_in"] - i))[0]
-                         for i in range(chunks - 1, -1, -1)])
+        """head h on stream b's feature window of each of its last `chunks` chunks, oldest first -> [chunks, n_out]; rows
+        older than the stream has (a reset with fewer feature rows than n_in) are zeros, as on the handle's ring"""
+        return np.stack([oheads.forward(h, self._features(b, h["n_in"], i)[None])[0] for i in range(chunks - 1, -1, -1)])
+
+    def _gated(self, raw):
+        """the gates on the heads' [chunks, columns] window scores: per chunk, before the max over chunks (as the gated
+        graph would)"""
+        for m, v, thr in self.gates:
+            cm, cv = self._col0(m), self._col0(v)
+            raw[:, cm] = np.where(raw[:, cm] > np.float32(thr), raw[:, cv], raw[:, cm])
+        return raw
+
+    def _bank_scores(self, b, hb, chunks):
+        k = hb["assign"][b]
+        return np.zeros(hb["n_out"], np.float32) if k < 0 else self._windows(b, hb["heads"][k], chunks).max(axis=0)
+
+    @staticmethod
+    def _verified(cols, thr):
+        return cols >= thr
 
     def _step(self, b, pcm, chunks, scores):
         """stream b steps the first `chunks` chunks of its samples pcm into its score row"""
@@ -198,23 +217,20 @@ class FakeContext:
         if not self.features:
             return
         assert self.af[b](x) == chunks * CHUNK
-        raw = np.concatenate([self._windows(b, h, chunks) for h in self.heads], axis=1)   # [chunks, head columns]
-        for m, v, thr in self.gates:                 # per chunk, before the max over chunks (as the gated graph would)
-            cm, cv = self._col0(m), self._col0(v)
-            raw[:, cm] = np.where(raw[:, cm] > np.float32(thr), raw[:, cv], raw[:, cm])
+        raw = self._gated(np.concatenate([self._windows(b, h, chunks) for h in self.heads], axis=1))
         scores[:raw.shape[1]] = raw.max(axis=0)
         col = raw.shape[1]
         for hb in self.hbanks:
-            k = hb["assign"][b]
-            scores[col:col + hb["n_out"]] = 0.0 if k < 0 else self._windows(b, hb["heads"][k], chunks).max(axis=0)
+            scores[col:col + hb["n_out"]] = self._bank_scores(b, hb, chunks)
             col += hb["n_out"]
+        self.unverified[b] = scores.copy()          # the row before the verifier banks, for tests that judge them
         for bk in self.banks if self.verifiers_on else []:
             slot = bk["assign"][b] if bk["hbank"] is None or self.hbanks[bk["hbank"]]["assign"][b] >= 0 else -1
             cols = scores[bk["col0"]:bk["col0"] + bk["n_cols"]]
-            if slot < 0 or not (cols >= bk["thr"]).any():
+            if slot < 0 or not self._verified(cols, bk["thr"]).any():
                 continue
             p = kernel_order_proba(*bk["slots"][slot], self._features(b, bk["n_in"])[None])[0]
-            cols[cols >= bk["thr"]] = p
+            cols[self._verified(cols, bk["thr"])] = p
 
     def step_host(self, pcm, n_chunks, scores_out):
         for b in range(self._n):
@@ -236,7 +252,8 @@ class FakeContext:
         self.step_host_ragged(pcm, chunks, d_scores)
 
     # ---- stream records: [payload bytes, configuration key, the pickled oracle state of the stream], the key at bytes
-    #      8..16 as in the library's records ----
+    #      8..16 as in the library's records; the rest of the library's byte layout is deliberately not modelled (only
+    #      the key is read across), so a record moves between handles of one kind only ----
     def stream_state_info(self):
         h = hashlib.sha256(repr(self._config).encode())
         for c in self.emb["conv"]:
