@@ -61,9 +61,14 @@ extern "C" {
 
 typedef struct oww_ctx oww_ctx;
 
+/* Largest max_chunks oww_create accepts (a larger one fails with OWW_EINVAL before anything is allocated): the mel ring
+ * of next_pow2(76 + 8 * max_chunks) rows stays within 2^20 rows, which the rebase of the row counts past 2^30 needs
+ * (oww_get_counts). */
+#define OWW_MAX_CHUNKS 131062
+
 typedef struct oww_config {
     int32_t device;        /* CUDA device ordinal                                               */
-    int32_t max_chunks;    /* largest n_chunks a single oww_step may carry (>=1)                */
+    int32_t max_chunks;    /* largest n_chunks a single oww_step may carry (1..OWW_MAX_CHUNKS)  */
     int32_t cnn_mode;      /* OWW_CNN_*                                                         */
     int32_t window_batch;  /* windows per CNN sub-batch in the window modes (0 = default)       */
     int32_t reserved[4];   /* reserved[0] bit 0: 1 = keep mode 3's steady-state step as separate launches
@@ -279,7 +284,9 @@ int oww_get_features(oww_ctx* ctx, int stream_id, int n, int back, float* h_out)
 int oww_get_mel(oww_ctx* ctx, int stream_id, int n_rows, float* h_out);   /* last n_rows<=76 mel rows */
 /* rows written to the stream's mel / feature buffer since its last reset, initial rows included (76 ones / the
  * feature_init rows) - len(melspectrogram_buffer) / len(feature_buffer) of the reference before its 970 / 120 caps
- * (utils.py:400-401,449-450).  Either pointer may be NULL.  Synchronises.                                     */
+ * (utils.py:400-401,449-450).  A count that reaches 2^30 is lowered by 2^30 - 2^20 (a multiple of every ring size) by
+ * the step that reaches it, so past 2^30 rows it is that number minus a multiple of 2^30 - 2^20, never below 2^20;
+ * it always exceeds 120 there.  Either pointer may be NULL.  Synchronises.                                     */
 int oww_get_counts(oww_ctx* ctx, int stream_id, int* mel_rows, int* feature_rows);
 
 /* ---- moving live streams: stream records ----------------------------------------------------------------------------
@@ -296,7 +303,8 @@ int oww_get_counts(oww_ctx* ctx, int stream_id, int* mel_rows, int* feature_rows
  *                             stream the record was taken from: its next steps of any kind give the same scores and leave
  *                             the same rings and counts, bit for bit wherever both handles run the same arithmetic.  The
  *                             fp16 feature mirror of the targets is resynced as after a reset.  No other stream changes,
- *                             and no stream's verifier or head-bank assignment changes (targets included).
+ *                             and no stream's verifier or head-bank assignment changes (targets included).  A row
+ *                             count at or past 2^30 in a record is rebased as a step rebases it (oww_get_counts).
  *   oww_stream_state_status - records the imports since the last call skipped (*n_rejected); synchronises; clears.
  * Export and import are stream-ordered and allocation-free after the first call, like oww_reset_async, and ordered
  * against oww_step_host / oww_step_host_submit on the handle's own stream: an export enqueued between two steps
@@ -341,8 +349,9 @@ int oww_stream_state_status(oww_ctx* ctx, int* n_rejected);
  *                       then so is d_events) receives the number of (stream, label) pairs whose label has a threshold and
  *                       whose prediction is >= it; d_events (may be NULL with max_events 0) receives the first
  *                       min(that number, max_events) of them in ascending (stream, label) order - the order never
- *                       depends on scheduling - with `index` = the stream's count before the append.  Memory past those
- *                       is not written.  Stream-ordered, no allocation, no synchronisation: one launch, two with
+ *                       depends on scheduling - with `index` = the stream's count before the append, in the count's
+ *                       frame after this call's rebase (the count after the call minus 1: 63, not 2^30 - 1, on the call
+ *                       that reaches 2^30).  Memory past those is not written.  Stream-ordered, no allocation, no synchronisation: one launch, two with
  *                       d_n_events.  h_prepared is staged through a ring of four pinned buffers: a call waits (host
  *                       side) for the copy of the call four staging uses back.  OWW_EINVAL before anything is enqueued:
  *                       no detector (or no streams), d_scores NULL, max_events < 0 or > 0 without d_events, d_events

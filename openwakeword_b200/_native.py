@@ -12,6 +12,7 @@ import numpy as np
 _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.path.join(_HERE, "csrc", "libowwb200.so")
 MAX_HEAD_LAYERS = 8
+MAX_CHUNKS = 131062          # OWW_MAX_CHUNKS: the largest max_chunks a handle takes
 
 CNN_FP32_WINDOW = 0
 CNN_FP32_INCREMENTAL = 1

@@ -165,12 +165,14 @@ __global__ void __launch_bounds__(256) stream_export_kernel(const int* ids, Stre
 }
 
 // one CTA per record: record j -> stream ids[j] (reset_kernel's scatter with the record as the source).  A record whose
-// header does not match the handle (or whose counts are impossible) is skipped and counted.
+// header does not match the handle (or whose counts are impossible) is skipped and counted.  Counts at or past 2^30,
+// which no step leaves behind, are rebased as a step would rebase them: a step adds at most 8 * OWW_MAX_CHUNKS rows,
+// which then cannot overflow int.
 __global__ void __launch_bounds__(256) stream_import_kernel(const int* ids, StreamState a, ResetTails rt, const uint4* rec) {
     const int b = ids[blockIdx.x];
     const uint4* r = rec + (int64_t)blockIdx.x * a.rec_units;
     const uint4 h0 = r[0], h1 = r[1];
-    const int seen = (int)h1.x, mc = (int)h1.y, fc = (int)h1.z;
+    const int seen = (int)h1.x, mc = oww_wrap_count((int)h1.y), fc = oww_wrap_count((int)h1.z);
     if (h0.x != kRecVersion || h0.y != a.bytes || h0.z != (uint32_t)a.key || h0.w != (uint32_t)(a.key >> 32) ||
         seen < 0 || mc < kRecMelRows || fc < 0) {
         if (threadIdx.x == 0) atomicAdd(a.rejected, 1);
@@ -835,6 +837,8 @@ const char* oww_last_error(const oww_ctx* ctx) { return ctx ? ctx->err.c_str() :
 int oww_create(const oww_config* cfg, oww_ctx** out) {
     if (!cfg || !out) return oww_fail(nullptr, OWW_EINVAL, "null argument");
     *out = nullptr;
+    if (cfg->max_chunks > OWW_MAX_CHUNKS)      // a larger mel ring breaks the count rebase (oww_internal.h)
+        return oww_fail(nullptr, OWW_EINVAL, "max_chunks %d above %d", cfg->max_chunks, OWW_MAX_CHUNKS);
     int ndev = 0;
     cudaError_t e = cudaGetDeviceCount(&ndev);
     if (e != cudaSuccess || ndev == 0)

@@ -135,7 +135,7 @@ struct HeadBank {
 
 // Ring row counters (rows ever written; ring slot = count & (rows-1)) would overflow int32 after ~248 days of
 // continuous streaming at 100 mel rows/s.  Past 2^30 they are rebased by a multiple of every ring size (rings are
-// powers of two <= 2^20 rows), which keeps the slot and leaves the count >= the ring size, so "row not yet written"
+// powers of two <= 2^20 rows: oww_create refuses max_chunks above OWW_MAX_CHUNKS), which keeps the slot and leaves the count >= the ring size, so "row not yet written"
 // tests (count - k >= 0) stay true.
 #define OWW_COUNT_WRAP (1 << 30)
 #define OWW_COUNT_REBASE ((1 << 30) - (1 << 20))

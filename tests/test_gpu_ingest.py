@@ -17,7 +17,7 @@ import os
 import numpy as np
 import pytest
 
-from helpers import GOLDEN, emb_weights, head
+from helpers import GOLDEN, emb_weights, head, judge_resampled
 from oracle import resample as ores
 
 pytestmark = pytest.mark.gpu
@@ -87,17 +87,7 @@ def _judge(got, x, rate):
         return 1.0
     y64, s = ores.StreamResampler(rate, h=h32.astype(np.float64)).feed(x, abs_sum=True)
     assert got.size == y64.size == ores.final_outputs(x.size, up, down)
-    K = -(-h32.size // up)
-    u = 2.0 ** -24
-    band = K * u / (1 - K * u) * s
-    ref = ores.to_int16(y64)
-    frac = y64 - np.floor(y64)
-    near = np.abs(frac - 0.5) <= band
-    sat = (y64 > 32767 + band) | (y64 < -32768 - band)
-    judged = ~near | sat
-    assert np.array_equal(got[judged], ref[judged]), (rate, np.nonzero(got[judged] != ref[judged])[0][:5])
-    assert (np.abs(got.astype(np.int32) - ref) <= 1).all()
-    return judged.mean()
+    return judge_resampled(got, y64, s, up, down, h32.size)
 
 
 def test_samples_against_the_float64_oracle(torch_cuda):
