@@ -323,7 +323,8 @@ int oww_stream_state_status(oww_ctx* ctx, int* n_rejected);
  * n_labels labels (<= 256); label j reads score column `column` (-1: always 0.0, a class mapped past its head's outputs)
  * and has `repeats` (1: a label of a single-output head, which repeats its previous prediction when fewer than 1280
  * samples were prepared; 0: a class of a multi-output head, which reads 0.0 then), `threshold` (NaN = none) and `patience`
- * (0 = none, else 1..30); debounce_time (seconds, 0 = off) is one per handle.  Per stream the handle keeps the last 30
+ * (0 = none, else 1..30); debounce_time (seconds, 0 = off) is one per handle (oww_set_stream_detection, below, gives
+ * streams their own).  Per stream the handle keeps the last 30
  * final predictions of every label and one count of predictions appended since the stream's reset (11 labels: 1324 B).
  *   oww_set_detector  - configure, reconfigure or (n_labels 0) remove the detector.  Synchronises the device.  The same
  *                       columns and repeats as before keep the histories (the reference takes thresholds, patience and
@@ -371,6 +372,42 @@ int oww_detect(oww_ctx* ctx, const float* d_scores, int prepared_all, const int3
 int oww_detector_export(oww_ctx* ctx, const int32_t* h_stream_ids, int n, float* d_hist, int32_t* d_counts, void* stream);
 int oww_detector_import(oww_ctx* ctx, const int32_t* h_stream_ids, int n, const float* d_hist, const int32_t* d_counts,
                         void* stream);
+/* ---- per-stream detection settings: every stream at its own sensitivity ----------------------------------------------
+ * A stream may override, per label, the threshold and patience of oww_set_detector, and the debounce_time.  oww_detect
+ * applies its rules, unchanged, with the stream's values; a stream without an override detects with the handle's values,
+ * bit for bit as without this call.  One record per (stream, label), oww_stream_detect:
+ *   threshold - NaN: the handle's threshold of the label; else this stream's;
+ *   patience  - -1: the handle's patience of the label; else this stream's, 0..30;
+ *   flags     - OWW_DETECT_NO_THRESHOLD: the label has no threshold on this stream (it never fires there and is not
+ *               debounced; `threshold` is ignored).  Other bits must be 0.
+ * and one debounce per stream (seconds; NaN: the handle's debounce_time).
+ *   oww_set_stream_detection - streams h_stream_ids[i] (NULL: every stream, n = the stream count) take the records
+ *                       h_overrides [n][n_labels] and the debounce h_debounce [n] (NULL: the handle's for all of them);
+ *                       h_overrides NULL returns the streams to the handle's settings (h_debounce is then ignored).  A
+ *                       record set equal to "the handle's values" (NaN, -1, 0 and NaN) is no override.  Each stream's
+ *                       resulting values are checked as oww_set_detector checks the handle's: patience 0..30, a debounce
+ *                       finite and >= 0, a patience needs a threshold and excludes a debounce.  Stream-ordered: oww_detect
+ *                       calls enqueued on `stream` afterwards use the new settings.  The host keeps the whole table and
+ *                       uploads it ([n_streams][n_labels] records and [n_streams] doubles, pageable: staged before the
+ *                       call returns) while any stream has an override; no device allocation.
+ *   oww_get_stream_detection - the settings of streams h_stream_ids[i] -> h_overrides [n][n_labels] and h_debounce [n]
+ *                       (either may be NULL); a stream without an override reads NaN, -1, 0 and NaN.  Host only.
+ * Both fail with OWW_EINVAL before anything changes for no detector (or no streams), an id out of range or a duplicate id,
+ * n outside [0, n_streams], a record or debounce the checks refuse (a getter may repeat ids).  oww_set_detector clears every override (the checks
+ * were made against the values it replaces); oww_set_streams keeps those of the streams below the new count and gives
+ * the new streams none; oww_reset / oww_reset_async keep them.  oww_detector_export / _import move histories only:
+ * move the settings with these two calls.  While no stream has an override oww_detect reads no record.                */
+typedef struct oww_stream_detect { float threshold; int32_t patience; int32_t flags; } oww_stream_detect;
+#define OWW_DETECT_NO_THRESHOLD 1
+#ifdef __cplusplus
+static_assert(sizeof(oww_stream_detect) == 12, "oww_stream_detect is 12 bytes");
+#else
+_Static_assert(sizeof(oww_stream_detect) == 12, "oww_stream_detect is 12 bytes");
+#endif
+int oww_set_stream_detection(oww_ctx* ctx, const int32_t* h_stream_ids, int n, const oww_stream_detect* h_overrides,
+                             const double* h_debounce, void* stream);
+int oww_get_stream_detection(oww_ctx* ctx, const int32_t* h_stream_ids, int n, oww_stream_detect* h_overrides,
+                             double* h_debounce);
 /* The same rules over the calls of the bulk clip path (oww_predict_clips_ragged / _streams, oww_predict_clips): what
  * predict_clip(clip, padding, chunk_size, patience=..., threshold=..., debounce_time=...) returns after a reset, for
  * every clip at once.  Stateless: it uses neither the handle's detector nor its streams.

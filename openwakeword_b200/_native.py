@@ -37,6 +37,11 @@ class DetectLabel(C.Structure):
 # one record of oww_detect's event list (oww_event): 16 bytes
 EVENT_DTYPE = np.dtype([("stream", "<i4"), ("label", "<i4"), ("score", "<f4"), ("index", "<i4")])
 
+# one (stream, label) record of oww_set_stream_detection (oww_stream_detect): 12 bytes.  threshold NaN: the handle's;
+# patience -1: the handle's; flags DETECT_NO_THRESHOLD: the label has no threshold on the stream
+STREAM_DETECT_DTYPE = np.dtype([("threshold", "<f4"), ("patience", "<i4"), ("flags", "<i4")])
+DETECT_NO_THRESHOLD = 1
+
 # one mixture of oww_mix_clips (oww_mix_params): 64 bytes.  rir = -1: no reverb; volume < 0: no volume
 MIX_DTYPE = np.dtype([("fg", "<i4"), ("bg", "<i4"), ("rir", "<i4"), ("reserved", "<i4"), ("fg_start", "<i8"),
                       ("fg_len", "<i8"), ("bg_offset", "<i8"), ("start", "<i8"), ("snr_db", "<f8"), ("volume", "<f8")])
@@ -98,6 +103,8 @@ _SIGNATURES = {
                                    _P, _P, C.c_int, _P, _P]),
     "oww_detector_export": (C.c_int, [_P, _P, C.c_int, _P, _P, _P]),
     "oww_detector_import": (C.c_int, [_P, _P, C.c_int, _P, _P, _P]),
+    "oww_set_stream_detection": (C.c_int, [_P, _P, C.c_int, _P, _P, _P]),
+    "oww_get_stream_detection": (C.c_int, [_P, _P, C.c_int, _P, _P]),
     "oww_set_audio_history": (C.c_int, [_P, C.c_int]),
     "oww_get_audio": (C.c_int, [_P, _P, _P, C.c_int, C.c_int, _P, _P, _P]),
     "oww_capture_events": (C.c_int, [_P, _P, _P, C.c_int, C.c_int, _P, _P, _P]),
@@ -686,6 +693,32 @@ class Context:
     def detector_import(self, stream_ids, d_hist, d_counts, stream=None):
         ids = np.ascontiguousarray(stream_ids, np.int32).ravel()
         self._check(self.lib.oww_detector_import(self.h, _ptr(ids), ids.size, _ptr(d_hist), _ptr(d_counts), stream))
+
+    def set_stream_detection(self, stream_ids, records, debounce=None, stream=None):
+        """oww_set_stream_detection: streams stream_ids (distinct; None = all) take records (STREAM_DETECT_DTYPE [n,
+        n_labels]; None: back to the handle's settings) and debounce (float64 [n], NaN: the handle's; None: all NaN), on
+        the current CUDA stream (or `stream`)."""
+        ids = None if stream_ids is None else np.ascontiguousarray(stream_ids, np.int32).ravel()
+        n = self.n_streams if ids is None else ids.size
+        rec = deb = None
+        if records is not None:
+            rec = np.ascontiguousarray(records, STREAM_DETECT_DTYPE)
+            if rec.shape != (n, self.n_detect_labels):
+                raise ValueError(f"records have shape {rec.shape}, expected {(n, self.n_detect_labels)}")
+            if debounce is not None:
+                deb = np.ascontiguousarray(np.broadcast_to(np.asarray(debounce, np.float64), (n,)))
+        if stream is None:
+            stream = self._current_stream()
+        self._check(self.lib.oww_set_stream_detection(self.h, _ptr(ids), n, _ptr(rec), _ptr(deb), stream))
+
+    def stream_detection(self, stream_ids=None):
+        """-> (STREAM_DETECT_DTYPE [n, n_labels], float64 [n] debounce) of streams stream_ids (None = all); host only"""
+        ids = None if stream_ids is None else np.ascontiguousarray(stream_ids, np.int32).ravel()
+        n = self.n_streams if ids is None else ids.size
+        rec = np.zeros((n, self.n_detect_labels), STREAM_DETECT_DTYPE)
+        deb = np.zeros(n, np.float64)
+        self._check(self.lib.oww_get_stream_detection(self.h, _ptr(ids), n, _ptr(rec), _ptr(deb)))
+        return rec, deb
 
     def _current_stream(self):
         import torch

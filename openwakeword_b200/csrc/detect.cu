@@ -6,12 +6,15 @@
 //
 // State: hist [30][B * n_labels] fp32 (ring slot s of pair p = stream * n_labels + label at hist[s * P + p]: the threads of
 // a warp read one slot of neighbouring pairs, so every history pass is coalesced) and count [B] int32 (predictions
-// appended since the stream's reset; ring slot = count % 30).
+// appended since the stream's reset; ring slot = count % 30).  Per-stream settings (oww_set_stream_detection): ovr
+// [B * n_labels] records at pair p and ovr_deb [B] doubles, read only while some stream has an override; the host keeps
+// the table and uploads it whole, so the device copy never needs a scatter or a clear.
 //
 // Event compaction is two launches rather than one pass with decoupled look-back: detect_kernel leaves each CTA's event
 // count and each pair's fired score, detect_events_kernel sums the counts of the CTAs before it (a few hundred ints at
 // 8192 streams) and writes its events behind them.  No CTA ever waits for another, so nothing can spin on a device that
 // is shared, and the order - ascending (stream, label) - follows from the thread mapping alone.
+#include <cmath>
 #include <cstring>
 #include "oww_internal.h"
 
@@ -31,6 +34,11 @@ struct oww_detector {
     float* d_fire = nullptr;           // [B * L] final score of the pairs that fired in the last call, NaN elsewhere
     int* d_cta = nullptr;              // [CTAs] events per CTA of the last call
     int* d_ids = nullptr;              // [B] staging of export / import ids
+    std::vector<oww_stream_detect> ovr;   // [B * L] per-stream settings (host copy of d_ovr); kNoOverride: the handle's
+    std::vector<double> ovr_deb;          // [B] per-stream debounce, NaN: the handle's
+    int n_ovr = 0;                        // streams with an override; 0: oww_detect passes no table
+    oww_stream_detect* d_ovr = nullptr;
+    double* d_ovr_deb = nullptr;
     // per-stream `prepared` of a call, staged like the counts of oww_step_ragged
     static constexpr int kSlots = 4;
     int32_t* h_prep[kSlots] = {nullptr, nullptr, nullptr, nullptr};
@@ -38,6 +46,8 @@ struct oww_detector {
     cudaEvent_t ev[kSlots] = {nullptr, nullptr, nullptr, nullptr};
     int next = 0;
 };
+
+static const oww_stream_detect kNoOverride = {NAN, -1, 0};
 
 static __device__ __forceinline__ int det_wrap(int c) { return c >= OWW_COUNT_WRAP ? c - DET_COUNT_REBASE : c; }
 
@@ -81,7 +91,8 @@ static __device__ __forceinline__ float det_rule(const oww_detect_label& lab, bo
 // One thread per (stream, label); CTA `blockIdx.x` owns streams [blockIdx.x * S, +S).
 __global__ void __launch_bounds__(DET_THREADS) detect_kernel(const float* __restrict__ scores, int n_out, int B, int L, int S,
                                                              const oww_detect_label* __restrict__ labels, double debounce,
-                                                             int prepared_all, const int* __restrict__ prepared,
+                                                             const oww_stream_detect* __restrict__ ovr,
+                                                             const double* __restrict__ ovr_deb, int prepared_all, const int* __restrict__ prepared,
                                                              float* __restrict__ hist, int* __restrict__ count,
                                                              float* __restrict__ d_final, float* __restrict__ fire,
                                                              int* __restrict__ cta_events) {
@@ -97,7 +108,14 @@ __global__ void __launch_bounds__(DET_THREADS) detect_kernel(const float* __rest
     bool fired = false;
     float pred = 0.f;
     if (prep >= 0) {
-        const oww_detect_label lab = labels[j];
+        oww_detect_label lab = labels[j];
+        if (ovr) {                                           // this stream's settings (oww_set_stream_detection)
+            const oww_stream_detect o = ovr[p];
+            if (o.flags & OWW_DETECT_NO_THRESHOLD) lab.threshold = __int_as_float(0x7fc00000);
+            else if (!isnan(o.threshold)) lab.threshold = o.threshold;
+            if (o.patience >= 0) lab.patience = o.patience;
+            if (!isnan(ovr_deb[b])) debounce = ovr_deb[b];
+        }
         const bool stepped = prep >= OWW_SAMPLES_PER_CHUNK;
         const float score = stepped && lab.column >= 0 ? scores[(size_t)b * n_out + lab.column] : 0.f;
         pred = det_rule(lab, stepped, score, __int_as_float(0x7fc00000), 0.f, c, prep, debounce,
@@ -272,8 +290,11 @@ namespace {
 
 void free_stream_state(oww_detector* d) {
     cudaFree(d->d_hist); cudaFree(d->d_count); cudaFree(d->d_fire); cudaFree(d->d_cta); cudaFree(d->d_ids);
+    cudaFree(d->d_ovr); cudaFree(d->d_ovr_deb);
     d->d_hist = d->d_fire = nullptr;
     d->d_count = d->d_cta = d->d_ids = nullptr;
+    d->d_ovr = nullptr;
+    d->d_ovr_deb = nullptr;
     for (int j = 0; j < oww_detector::kSlots; ++j) {
         cudaFreeHost(d->h_prep[j]); cudaFree(d->d_prep[j]);
         d->h_prep[j] = d->d_prep[j] = nullptr;
@@ -281,12 +302,36 @@ void free_stream_state(oww_detector* d) {
     d->n_streams = 0;
 }
 
-// the detector's per-stream state for ctx->n_streams streams, every history empty; the device is idle
+bool is_override(const oww_stream_detect& o) { return !std::isnan(o.threshold) || o.patience != -1 || o.flags != 0; }
+
+// n_ovr from the host table, and the table to the device on `s` while some stream has an override
+int sync_overrides(oww_ctx* ctx, cudaStream_t s) {
+    oww_detector* d = ctx->det;
+    const size_t L = d->labels.size();
+    d->n_ovr = 0;
+    for (size_t b = 0; b < d->ovr_deb.size(); ++b) {
+        bool any = !std::isnan(d->ovr_deb[b]);
+        for (size_t j = 0; j < L && !any; ++j) any = is_override(d->ovr[b * L + j]);
+        d->n_ovr += any;
+    }
+    if (d->n_ovr && d->d_ovr) {                          // pageable sources: staged by the driver before the call returns
+        OWW_CUDA(ctx, cudaMemcpyAsync(d->d_ovr, d->ovr.data(), d->ovr.size() * sizeof(oww_stream_detect),
+                                      cudaMemcpyHostToDevice, s));
+        OWW_CUDA(ctx, cudaMemcpyAsync(d->d_ovr_deb, d->ovr_deb.data(), d->ovr_deb.size() * sizeof(double),
+                                      cudaMemcpyHostToDevice, s));
+    }
+    return OWW_OK;
+}
+
+// the detector's per-stream state for ctx->n_streams streams, every history empty, the settings of the streams below
+// that count kept; the device is idle
 int alloc_stream_state(oww_ctx* ctx) {
     oww_detector* d = ctx->det;
     free_stream_state(d);
-    const int B = ctx->n_streams, L = (int)d->labels.size();
-    if (B <= 0) return OWW_OK;
+    const int B = std::max(ctx->n_streams, 0), L = (int)d->labels.size();
+    d->ovr.resize((size_t)B * L, kNoOverride);          // stream-major: the first streams keep their rows
+    d->ovr_deb.resize((size_t)B, NAN);
+    if (B == 0) { d->n_ovr = 0; return OWW_OK; }
     const size_t P = (size_t)B * L;
     const int ctas = (B + det_streams_per_cta(L) - 1) / det_streams_per_cta(L);
     OWW_CUDA(ctx, cudaMalloc(&d->d_hist, DET_HIST * P * sizeof(float)));
@@ -294,6 +339,8 @@ int alloc_stream_state(oww_ctx* ctx) {
     OWW_CUDA(ctx, cudaMalloc(&d->d_fire, P * sizeof(float)));
     OWW_CUDA(ctx, cudaMalloc(&d->d_cta, (size_t)ctas * sizeof(int)));
     OWW_CUDA(ctx, cudaMalloc(&d->d_ids, (size_t)B * sizeof(int)));
+    OWW_CUDA(ctx, cudaMalloc(&d->d_ovr, P * sizeof(oww_stream_detect)));
+    OWW_CUDA(ctx, cudaMalloc(&d->d_ovr_deb, (size_t)B * sizeof(double)));
     OWW_CUDA(ctx, cudaMemset(d->d_hist, 0, DET_HIST * P * sizeof(float)));
     OWW_CUDA(ctx, cudaMemset(d->d_count, 0, (size_t)B * sizeof(int)));
     for (int j = 0; j < oww_detector::kSlots; ++j) {
@@ -302,7 +349,7 @@ int alloc_stream_state(oww_ctx* ctx) {
         if (!d->ev[j]) OWW_CUDA(ctx, cudaEventCreateWithFlags(&d->ev[j], cudaEventDisableTiming));
     }
     d->n_streams = B;
-    return OWW_OK;
+    return sync_overrides(ctx, nullptr);
 }
 
 // checks shared by export and import; stages the ids on `s`
@@ -319,6 +366,20 @@ int stage_ids(oww_ctx* ctx, const int32_t* h_ids, int n, bool distinct, cudaStre
     }
     // pageable source: staged by the driver before the call returns; stream-ordered on the device
     if (n) OWW_CUDA(ctx, cudaMemcpyAsync(d->d_ids, h_ids, (size_t)n * sizeof(int), cudaMemcpyHostToDevice, s));
+    return OWW_OK;
+}
+
+// checks of the settings calls: a detector with streams, ids in range (NULL: every stream), distinct if asked
+int check_settings_ids(oww_ctx* ctx, const int32_t* h_ids, int n, bool distinct) {
+    const oww_detector* d = ctx->det;
+    if (!d || !d->d_hist) return oww_fail(ctx, OWW_EINVAL, "no detector configured (oww_set_detector, oww_set_streams)");
+    const int B = ctx->n_streams;
+    if (n < 0 || n > B || (!h_ids && n != B)) return oww_fail(ctx, OWW_EINVAL, "n=%d outside [0,%d] (or not %d without ids)", n, B, B);
+    std::vector<uint8_t> hit(h_ids && distinct ? B : 0, 0);
+    for (int i = 0; h_ids && i < n; ++i) {
+        if (h_ids[i] < 0 || h_ids[i] >= B) return oww_fail(ctx, OWW_EINVAL, "stream id %d out of range", h_ids[i]);
+        if (distinct && hit[h_ids[i]]++) return oww_fail(ctx, OWW_EINVAL, "stream id %d given twice", h_ids[i]);
+    }
     return OWW_OK;
 }
 
@@ -376,6 +437,9 @@ int oww_set_detector(oww_ctx* ctx, const oww_detect_label* h_labels, int n_label
     }
     d->labels.assign(h_labels, h_labels + n_labels);
     d->debounce = debounce_time;
+    d->ovr.assign(d->ovr.size(), kNoOverride);           // every stream back to the handle's settings
+    d->ovr_deb.assign(d->ovr_deb.size(), NAN);
+    d->n_ovr = 0;
     OWW_CUDA(ctx, cudaMemcpy(d->d_labels, h_labels, (size_t)n_labels * sizeof(oww_detect_label), cudaMemcpyHostToDevice));
     return same ? OWW_OK : alloc_stream_state(ctx);
 }
@@ -404,8 +468,8 @@ int oww_detect(oww_ctx* ctx, const float* d_scores, int prepared_all, const int3
         OWW_CUDA(ctx, cudaEventRecord(d->ev[j], s));
         d_prep = d->d_prep[j];
     }
-    detect_kernel<<<ctas, DET_THREADS, 0, s>>>(d_scores, ctx->n_out_total, B, L, S, d->d_labels, d->debounce, prepared_all,
-                                               d_prep, d->d_hist, d->d_count, d_final, d->d_fire, d->d_cta);
+    detect_kernel<<<ctas, DET_THREADS, 0, s>>>(d_scores, ctx->n_out_total, B, L, S, d->d_labels, d->debounce,
+                                               d->n_ovr ? d->d_ovr : nullptr, d->d_ovr_deb, prepared_all, d_prep, d->d_hist, d->d_count, d_final, d->d_fire, d->d_cta);
     OWW_LAUNCH_CHECK(ctx);
     if (d_n_events) {
         detect_events_kernel<<<ctas, DET_THREADS, 0, s>>>(d->d_fire, d->d_count, d->d_cta, B, L, S, d_events, max_events, d_n_events);
@@ -499,6 +563,55 @@ int oww_detector_import(oww_ctx* ctx, const int32_t* h_stream_ids, int n, const 
     detect_import_kernel<<<n, DET_THREADS, 0, (cudaStream_t)stream>>>(d->d_ids, ctx->n_streams, (int)d->labels.size(), d->d_hist,
                                                                       d->d_count, d_hist, d_counts);
     OWW_LAUNCH_CHECK(ctx);
+    return OWW_OK;
+}
+
+int oww_set_stream_detection(oww_ctx* ctx, const int32_t* h_stream_ids, int n, const oww_stream_detect* h_overrides,
+                             const double* h_debounce, void* stream) {
+    if (!ctx) return OWW_EINVAL;
+    int rc = check_settings_ids(ctx, h_stream_ids, n, true);
+    if (rc) return rc;
+    oww_detector* d = ctx->det;
+    const int L = (int)d->labels.size();
+    for (int i = 0; h_overrides && i < n; ++i) {         // every stream's resulting values, before anything changes
+        const int b = h_stream_ids ? h_stream_ids[i] : i;
+        const double deb = h_debounce ? h_debounce[i] : NAN;
+        if (!std::isnan(deb) && !(deb >= 0.0 && std::isfinite(deb)))
+            return oww_fail(ctx, OWW_EINVAL, "stream %d: debounce_time must be finite and >= 0 (NaN: the handle's)", b);
+        const double eff_deb = std::isnan(deb) ? d->debounce : deb;
+        for (int j = 0; j < L; ++j) {
+            const oww_stream_detect& o = h_overrides[(size_t)i * L + j];
+            if (o.flags & ~OWW_DETECT_NO_THRESHOLD) return oww_fail(ctx, OWW_EINVAL, "stream %d label %d: flags 0x%x", b, j, o.flags);
+            if (o.patience < -1 || o.patience > DET_HIST)
+                return oww_fail(ctx, OWW_EINVAL, "stream %d label %d: patience %d outside [-1,%d]", b, j, o.patience, DET_HIST);
+            const bool thr = !(o.flags & OWW_DETECT_NO_THRESHOLD) && !std::isnan(std::isnan(o.threshold) ? d->labels[j].threshold : o.threshold);
+            const int pat = o.patience >= 0 ? o.patience : d->labels[j].patience;
+            if (pat > 0 && !thr) return oww_fail(ctx, OWW_EINVAL, "stream %d label %d: patience needs a threshold", b, j);
+            if (pat > 0 && eff_deb > 0.0)
+                return oww_fail(ctx, OWW_EINVAL, "stream %d: patience and debounce_time cannot be used together", b);
+        }
+    }
+    OWW_CUDA(ctx, cudaSetDevice(ctx->device));
+    for (int i = 0; i < n; ++i) {
+        const int b = h_stream_ids ? h_stream_ids[i] : i;
+        for (int j = 0; j < L; ++j) d->ovr[(size_t)b * L + j] = h_overrides ? h_overrides[(size_t)i * L + j] : kNoOverride;
+        d->ovr_deb[b] = h_overrides && h_debounce ? h_debounce[i] : NAN;
+    }
+    return sync_overrides(ctx, (cudaStream_t)stream);
+}
+
+int oww_get_stream_detection(oww_ctx* ctx, const int32_t* h_stream_ids, int n, oww_stream_detect* h_overrides,
+                             double* h_debounce) {
+    if (!ctx) return OWW_EINVAL;
+    int rc = check_settings_ids(ctx, h_stream_ids, n, false);
+    if (rc) return rc;
+    const oww_detector* d = ctx->det;
+    const size_t L = d->labels.size();
+    for (int i = 0; i < n; ++i) {
+        const size_t b = h_stream_ids ? h_stream_ids[i] : i;
+        if (h_overrides) std::memcpy(h_overrides + i * L, d->ovr.data() + b * L, L * sizeof(oww_stream_detect));
+        if (h_debounce) h_debounce[i] = d->ovr_deb[b];
+    }
     return OWW_OK;
 }
 

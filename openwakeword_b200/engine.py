@@ -226,6 +226,47 @@ class StreamEngine:
             self.ctx._cuda("final", final, torch.float32, (self.n_streams, self.ctx.n_detect_labels))
         return self.ctx.detect_events(scores, prepared, final, max_events)
 
+    # ---- per-stream detection settings (include/owwb200.h, oww_set_stream_detection) ----
+    def set_stream_detection(self, stream_ids, threshold=None, patience=None, debounce_time=None, stream=None):
+        """Streams stream_ids (distinct; None = all) detect at their own sensitivity from the next ``detect`` enqueued on
+        the current CUDA stream (or `stream`) on.  threshold: one float for every label, or {label index: float, or None
+        for no threshold on these streams (the label never fires there)}; patience: one int for every label, or {label
+        index: 0..30}; debounce_time: seconds.  What is not given (None, a label missing from a dict, a NaN threshold)
+        stays the handle's (set_detector).  The call replaces the streams' earlier settings.  Each stream's resulting
+        values are checked as set_detector checks the handle's (NativeError: a patience without a threshold, patience
+        together with a debounce_time).  set_detector clears every stream's settings; reset keeps them; set_streams keeps
+        those of the streams below the new count."""
+        n = self.n_streams if stream_ids is None else np.size(stream_ids)
+        L = self.ctx.n_detect_labels
+        rec = np.zeros((n, L), _native.STREAM_DETECT_DTYPE)
+        rec["threshold"], rec["patience"] = np.nan, -1
+        for field, val in (("threshold", threshold), ("patience", patience)):
+            if val is None:
+                continue
+            for j, v in (val.items() if isinstance(val, dict) else ((j, val) for j in range(L))):
+                if not isinstance(j, (int, np.integer)) or not 0 <= j < L:
+                    raise ValueError(f"no label {j!r}: the detector has {L} labels")
+                if field == "threshold" and v is None:
+                    rec["flags"][:, j] = _native.DETECT_NO_THRESHOLD
+                elif v is not None:
+                    rec[field][:, j] = v
+        deb = np.nan if debounce_time is None else float(debounce_time)
+        self.ctx.set_stream_detection(stream_ids, rec, deb, self._stream(stream))
+
+    def clear_stream_detection(self, stream_ids=None, stream=None):
+        """Streams stream_ids (None = all) detect with the handle's settings again."""
+        self.ctx.set_stream_detection(stream_ids, None, None, self._stream(stream))
+
+    def stream_detection(self, stream_ids=None):
+        """-> (records _native.STREAM_DETECT_DTYPE [n, n_labels], float64 [n] debounce) of streams stream_ids (None = all):
+        threshold NaN / patience -1 / debounce NaN = the handle's, flags _native.DETECT_NO_THRESHOLD = no threshold.  What
+        ``set_stream_detection_records`` takes, on this engine or another with the same labels, to move the settings."""
+        return self.ctx.stream_detection(stream_ids)
+
+    def set_stream_detection_records(self, stream_ids, records, debounce):
+        """Streams stream_ids (distinct) take the settings ``stream_detection`` returned for other streams."""
+        self.ctx.set_stream_detection(stream_ids, records, debounce, self._stream(None))
+
     # ---- stream audio on the device (include/owwb200.h, oww_set_audio_history) ----
     def set_audio_history(self, n_samples):
         """Keep the last n_samples (a multiple of 1280, up to 960000; 0 = off) samples every stream steps on the device.

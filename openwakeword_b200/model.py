@@ -184,6 +184,9 @@ class Model:
         self._n_cols = col
         self._scores = np.zeros((self.n_streams, max(col, 1)), np.float32)
         self._reset_history()
+        self._stream_det = {}          # stream id -> (threshold, patience, debounce_time) of set_stream_detection
+        self._stream_det_pushed = None  # the detect call settings the device's stream settings were resolved under
+        self._stream_det_on_device = False
         for name, per_stream in device_verifiers.items():
             for b, v in per_stream.items():
                 self.set_custom_verifier(name, v, None if b is None else [b])
@@ -571,11 +574,13 @@ class Model:
         ingest = pre.ctx.ingest_state(ids) if pre.ingest else None
         return StreamState(records, key, labels, [buf[b, :lens[b]].copy() for b in ids],
                            {lab: self._h(lab)[0][:, ids].copy() for lab in labels},
-                           {lab: self._h(lab)[1][ids].copy() for lab in labels}, audio, ingest)
+                           {lab: self._h(lab)[1][ids].copy() for lab in labels}, audio, ingest,
+                           [self._stream_det.get(b) for b in ids.tolist()])
 
     def import_streams(self, stream_ids, state):
         """Streams stream_ids (distinct) become the streams `state` was exported from: device state, samples not yet
-        stepped and prediction history (first-5 zeroing, patience, debounce).  Their stream models and verifiers stay as
+        stepped, prediction history (first-5 zeroing, patience, debounce) and detection settings (set_stream_detection;
+        none when the state has none).  Their stream models and verifiers stay as
         they are here.  ValueError: another configuration (cnn_mode, split_from, weights), another label set, or Speex
         noise suppression on (its state cannot be exported)."""
         ids = self._ids(stream_ids)
@@ -620,6 +625,12 @@ class Model:
             cnt[ids] = state.counts[lab]
         if self._hist_on_device and ids.size:
             self._push_history(ids)
+        for i, b in enumerate(ids.tolist()):
+            if state.detection is None or state.detection[i] is None:
+                self._stream_det.pop(b, None)
+            else:
+                self._stream_det[b] = state.detection[i]
+        self._stream_det_pushed = False
 
     def _ids(self, stream_ids):
         ids = np.asarray(stream_ids, np.int64).ravel()
@@ -760,6 +771,7 @@ class Model:
         the event count and the events are copied back.  ``predict*`` and ``detect*`` may be mixed freely: the history
         moves between host and device at each switch (one copy of [n_streams, labels, 30] floats), and
         ``prediction_buffer``, ``reset``, ``reset_streams``, ``export_streams`` and ``import_streams`` see it wherever it is.
+        Streams given settings of their own (``set_stream_detection``) detect with those in place of the call's.
 
         ValueError, so that no call needs per-stream host work: a custom verifier that only runs on the host; Speex noise
         suppression with more than one stream; a stream that prepares more than ``max_chunks`` chunks in one call while
@@ -829,6 +841,77 @@ class Model:
                 table.append((col, repeats, None if thr is None else float(thr), pat))
         return table
 
+    # ---- per-stream detection settings (include/owwb200.h, oww_set_stream_detection) ----
+    def set_stream_detection(self, stream_ids, threshold=None, patience=None, debounce_time=None):
+        """Streams stream_ids detect at their own sensitivity in ``detect`` / ``detect_ragged``: threshold - one float for
+        every model, or {model name: float, or None for no threshold on these streams}; patience - {model name: 0..30};
+        debounce_time - seconds.  Each given value replaces, on these streams, the one the ``detect*`` call passes; what
+        is not given (None, a model missing from a dict) stays the call's.  Names resolve as in ``predict`` (a multi-class
+        model's labels take its values; stream models by their name).  The call replaces the streams' earlier settings.
+        ``predict*`` keep taking their per-call arguments only.  Each stream's resulting settings are checked at the next
+        ``detect*`` as ``predict`` checks its arguments (ValueError before anything runs).  ``reset*`` keep the settings;
+        ``export_streams`` / ``import_streams`` move them with the streams."""
+        ids = self._ids(stream_ids)
+        if isinstance(threshold, dict):
+            threshold = {k: None if v is None else float(v) for k, v in threshold.items()}
+        elif threshold is not None:
+            threshold = float(threshold)
+        patience = {k: int(v) for k, v in (patience or {}).items()}
+        for name in list(threshold if isinstance(threshold, dict) else []) + list(patience):
+            if name not in self.models:
+                raise ValueError(f"no model named '{name}'; the models are {list(self.models)}")
+        for name, pat in patience.items():
+            if not 0 <= pat <= 30:
+                raise ValueError(f"patience of '{name}' must lie in 0..30 (the history holds 30 predictions)")
+        if debounce_time is not None:
+            debounce_time = float(debounce_time)
+            if not debounce_time >= 0 or not np.isfinite(debounce_time):
+                raise ValueError("debounce_time must be finite and >= 0")
+            if patience and debounce_time > 0:
+                raise ValueError("Error! The `patience` and `debounce_time` arguments cannot be used together!")
+        for b in ids.tolist():
+            self._stream_det[b] = (threshold, patience, debounce_time)
+        self._stream_det_pushed = False
+
+    def clear_stream_detection(self, stream_ids=None):
+        """Streams stream_ids (None = all) detect with the settings of each ``detect*`` call again."""
+        for b in (range(self.n_streams) if stream_ids is None else self._ids(stream_ids).tolist()):
+            self._stream_det.pop(b, None)
+        self._stream_det_pushed = False
+
+    def stream_detection(self, stream_id):
+        """-> {"threshold", "patience", "debounce_time"} as set_stream_detection took them for the stream, or None"""
+        s = self._stream_det.get(int(stream_id))
+        return None if s is None else dict(threshold=s[0], patience=dict(s[1]), debounce_time=s[2])
+
+    def _stream_detection_table(self, threshold, patience, debounce_time):
+        """-> None when no stream has settings of its own, else (STREAM_DETECT_DTYPE [n_streams, labels], float64
+        [n_streams] debounce): each such stream's settings over the call's, resolved by _detector_table (and checked
+        there), the others the handle's.  Streams with the same settings are resolved once."""
+        if not self._stream_det:
+            return None
+        rec = np.zeros((self.n_streams, len(self.labels())), _native.STREAM_DETECT_DTYPE)
+        rec["threshold"], rec["patience"] = np.nan, -1
+        deb = np.full(self.n_streams, np.nan)
+        groups = {}
+        for b, (thr, pat, dt) in self._stream_det.items():
+            key = (tuple(sorted(thr.items())) if isinstance(thr, dict) else thr, tuple(sorted(pat.items())), dt)
+            groups.setdefault(key, ([], (thr, pat, dt)))[0].append(b)
+        for ids, (thr, pat, dt) in groups.values():
+            if thr is None:
+                thr = threshold
+            elif isinstance(thr, dict):
+                thr = {**(threshold if isinstance(threshold, dict) else {m: threshold for m in self.models}), **thr}
+            dt = debounce_time if dt is None else dt
+            rows = self._detector_table(thr, {**patience, **pat}, dt)
+            ids = np.asarray(ids)
+            for j, (_, _, t, p) in enumerate(rows):
+                rec["threshold"][ids, j] = np.nan if t is None else t
+                rec["flags"][ids, j] = _native.DETECT_NO_THRESHOLD if t is None else 0
+                rec["patience"][ids, j] = p
+            deb[ids] = dt
+        return rec, deb
+
     def _detect(self, xs, threshold, patience, debounce_time, capture=None):
         pre = self.preprocessor
         pre._ensure_streams()
@@ -851,9 +934,18 @@ class Model:
             raise ValueError(f"detect: a stream prepares more than max_chunks={pre.max_chunks} chunks in this call while "
                              "custom verifiers are loaded; construct the Model with a larger max_chunks, or use predict")
         config = (table, float(debounce_time))
+        call = (repr(threshold), repr(patience), float(debounce_time))
+        if self._stream_det_pushed != call:                        # checks every stream's settings before any change
+            stream_table = self._stream_detection_table(threshold, patience, debounce_time)
         if getattr(self, "_detector_config", None) != config:      # oww_set_detector synchronises: only on a change
-            ctx.set_detector(table, debounce_time)
+            ctx.set_detector(table, debounce_time)                  # ... and clears every stream's settings
             self._detector_config = config
+            self._stream_det_on_device = False
+        if self._stream_det_pushed != call:
+            if stream_table is not None or self._stream_det_on_device:
+                ctx.set_stream_detection(None, *(stream_table or (None, None)))
+            self._stream_det_on_device = stream_table is not None
+            self._stream_det_pushed = call
         if not self._hist_on_device:
             if self._hist:
                 self._push_history(np.arange(self.n_streams))
@@ -1324,20 +1416,22 @@ class StreamState:
     history: int16 [n, H] oldest first, int64 [n] sample positions, bool [n] whether the samples held not yet stepped
     count in ``raw_data_buffer``), ``ingest`` (None without device ingest, else the resampler state: int32 [n] rates, int64
     [n] input samples since each resampler's restart, int32 [n] staged counts, int16 [n, max staged] staged 16 kHz samples,
-    int16 [n, 128] filter histories).  ``to(device)`` moves the records; on the CPU it pickles."""
+    int16 [n, 128] filter histories), ``detection`` (None, or per stream None or the (threshold, patience, debounce_time)
+    of ``Model.set_stream_detection``).  ``to(device)`` moves the records; on the CPU it pickles."""
 
-    def __init__(self, records, key, labels, pending, history, counts, audio=None, ingest=None):
+    def __init__(self, records, key, labels, pending, history, counts, audio=None, ingest=None, detection=None):
         self.records, self.key, self.labels = records, int(key), list(labels)
         self.pending, self.history, self.counts = pending, history, counts
         self.audio = audio
         self.ingest = ingest
+        self.detection = detection
 
     def __len__(self):
         return len(self.pending)
 
     def to(self, device):
         return StreamState(self.records.to(device), self.key, self.labels, self.pending, self.history, self.counts,
-                           self.audio, self.ingest)
+                           self.audio, self.ingest, self.detection)
 
 
 def _concat_clips(clips):
