@@ -536,6 +536,45 @@ int oww_ingest_import(oww_ctx* ctx, const int32_t* h_stream_ids, int n, const in
                       const int32_t* h_staged, const int16_t* d_staged, int64_t staged_stride, const int16_t* d_hist,
                       void* stream);
 
+/* ---- pipelined detection from host audio: a serving loop's whole call (the reference's server example runs it per
+ *      packet on the host, examples/web/streaming_server.py:40-68; examples/capture_activations.py keeps the audio of
+ *      each activation) with nothing in between that waits for the device ------------------------------------------------
+ *   oww_detect_host_submit - exactly oww_ingest(packets, h_offsets) followed by oww_detect(h_prepared = what that ingest
+ *                       returned) and, with capture_samples > 0, oww_capture_events(capture_samples): stream b's packet is
+ *                       h_packets[h_offsets[b] .. h_offsets[b+1]) (host int16 at the stream's rate; host int64 offsets,
+ *                       n_streams + 1 entries, as oww_ingest).  Returns a ticket (0/1) without waiting; at most two are in
+ *                       flight.  The packets [h_offsets[0], h_offsets[n_streams]) are staged through one of two pinned
+ *                       slots of the handle, or, when that span is page-locked (cudaMallocHost, cudaHostRegister, torch
+ *                       pin_memory), DMA'd straight from it: then it must stay untouched until the ticket is collected.
+ *                       The copy runs on a copy stream, the work on the handle's own stream behind an event, so the copy
+ *                       of one call overlaps the kernels of the other.  After the detect a delivery kernel reads the event
+ *                       count on the device and writes it, the first min(count, max_events) events and with capture their
+ *                       clip rows and ends into the slot's mapped host buffer: only the events found cross PCIe.  With
+ *                       want_final the final predictions [n_streams][n_labels] follow as one copy.  No device allocation
+ *                       once the slots have grown to the largest call (samples, max_events, capture_samples) so far.
+ *   oww_detect_host_collect - waits for the ticket and copies its results out of the slot: *h_n_events <- the event count;
+ *                       h_events <- the first min(count, max_events) events in oww_detect's (stream, label) order; with
+ *                       capture, h_clips [that many][capture_samples] and h_ends (each clip's end, its stream's position);
+ *                       h_chunks / h_prepared [n_streams] <- what oww_ingest returned; with want_final h_final [n_streams]
+ *                       [n_labels].  Every output may be NULL (not delivered).  These are what the synchronous sequence
+ *                       gives, bit for bit.  A ticket that is not in flight, or one collected before an older ticket, fails
+ *                       with OWW_EINVAL.
+ * Preconditions: ingest state (oww_set_input_rates; a 16 kHz stream takes the identity rate) and a detector; with capture
+ * an audio history.  OWW_EINVAL before anything is enqueued, every stream unchanged: a third ticket while two are in
+ * flight, no ingest state or weights, no detector, capture_samples < 0 or above the history (or any without one),
+ * max_events < 0, offsets that are negative or decrease, a packet over its stream's capacity.  The host keeps each
+ * stream's input and staged counts at submit time, so oww_ingest_capacity stays exact while calls are in flight and the
+ * capacity check counts what earlier submits staged.
+ * Ordering: a call made between two submits applies to the later one and not to the earlier one, as in the synchronous
+ * loop - oww_reset / oww_reset_async, oww_set_stream_detection, oww_set_input_rates, oww_assign_*, and the export and
+ * import of streams, detector histories, ingest state and audio are ordered against the handle's own stream, on
+ * whichever stream they are enqueued.  Steps of oww_step_host_submit may be pending beside detect tickets: all their work
+ * is ordered on the handle's own stream.  A stream must still be fed at one place only (ingest, above).               */
+int oww_detect_host_submit(oww_ctx* ctx, const int16_t* h_packets, const int64_t* h_offsets, int max_events,
+                           int capture_samples, int want_final, int* ticket);
+int oww_detect_host_collect(oww_ctx* ctx, int ticket, oww_event* h_events, int32_t* h_n_events, int16_t* h_clips,
+                            int64_t* h_ends, int32_t* h_chunks, int32_t* h_prepared, float* h_final);
+
 /* ---- batch paths --------------------------------------------------------------------------- */
 /* d_pcm [n_clips][n_samples] -> d_emb [n_clips][W][96], W = (T-76)/8+1 (utils.py:322).           */
 int oww_embed_clips(oww_ctx* ctx, const int16_t* d_pcm, int n_clips, int n_samples, float* d_emb, void* stream);

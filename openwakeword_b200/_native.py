@@ -118,6 +118,8 @@ _SIGNATURES = {
     "oww_resampler_taps": (C.c_int, [C.c_int, _P, C.c_int, C.POINTER(C.c_int), C.POINTER(C.c_int)]),
     "oww_ingest_export": (C.c_int, [_P, _P, C.c_int, _P, _P, _P, _P, C.c_int64, _P, _P]),
     "oww_ingest_import": (C.c_int, [_P, _P, C.c_int, _P, _P, _P, _P, C.c_int64, _P, _P]),
+    "oww_detect_host_submit": (C.c_int, [_P, _P, _P, C.c_int, C.c_int, C.c_int, C.POINTER(C.c_int)]),
+    "oww_detect_host_collect": (C.c_int, [_P, C.c_int, _P, _P, _P, _P, _P, _P, _P]),
     "oww_embed_clips": (C.c_int, [_P, _P, C.c_int, C.c_int, _P, _P]),
     "oww_predict_clips": (C.c_int, [_P, _P, C.c_int, C.c_int, C.c_int, _P, C.c_int, _P, _P]),
     "oww_clip_schedule": (C.c_int, [C.c_int, C.c_int64, _P, C.c_int]),
@@ -287,6 +289,7 @@ class Context:
         self.n_detect_labels = 0            # labels of the detector (set_detector)
         self._det_buf = None                # device event list and count of detect_events
         self.audio_history = 0              # samples of audio history per stream (set_audio_history; 0 = off)
+        self._det_tickets = {}              # detect ticket -> (packets kept alive, the output arrays of its collect)
 
     def close(self):
         if getattr(self, "h", None):
@@ -937,6 +940,42 @@ class Context:
         h = torch.from_numpy(np.ascontiguousarray(hist, np.int16).reshape(ids.size, 128)).to(dev)
         self._check(self.lib.oww_ingest_import(self.h, _ptr(ids), ids.size, _ptr(r), _ptr(S), _ptr(st), _ptr(d),
                                                x.shape[1], _ptr(h), self._current_stream()))
+
+    # ---- pipelined detection from host audio (include/owwb200.h, oww_detect_host_submit) ----
+    def detect_host_submit(self, packets, offsets, max_events, capture=None, final=False):
+        """oww_detect_host_submit: ingest + detect (+ capture of `capture` samples per event) of host int16 packets
+        (stream b's: packets[offsets[b]:offsets[b+1]]) -> ticket.  The output arrays of the ticket are allocated here; the
+        packets array is kept until the collect (a page-locked one is read by the copy engine until then)."""
+        if not isinstance(packets, np.ndarray) or packets.dtype != np.int16 or packets.ndim != 1 \
+                or not packets.flags.c_contiguous:
+            raise ArgumentError("packets must be a contiguous 1-D int16 numpy array")
+        off = np.ascontiguousarray(offsets, np.int64).ravel()
+        B, L = self.n_streams, self.n_detect_labels
+        if off.size != B + 1 or off[0] < 0 or off[-1] > packets.size:
+            raise ArgumentError(f"offsets must hold {B + 1} sample offsets into packets ({packets.size} samples)")
+        m, cs = int(max_events), 0 if capture is None else int(capture)
+        rows = max(m, 0) if cs > 0 else 0
+        out = (np.empty(max(m, 0), EVENT_DTYPE), np.zeros(1, np.int32), np.empty((rows, max(cs, 0)), np.int16),
+               np.empty(rows, np.int64), np.zeros(B, np.int32), np.zeros(B, np.int32),
+               np.empty((B, L), np.float32) if final else None)
+        t = C.c_int(-1)
+        self._check(self.lib.oww_detect_host_submit(self.h, _ptr(packets), _ptr(off), m, cs, int(bool(final)), C.byref(t)))
+        self._det_tickets[t.value] = (packets, cs, out)
+        return t.value
+
+    def detect_host_collect(self, ticket):
+        """oww_detect_host_collect -> (events EVENT_DTYPE [k], n, chunks int32 [B], prepared int32 [B], clips int16 [k,
+        capture] or None, ends int64 [k] or None, final float32 [B, n_labels] or None), k = min(n, max_events)."""
+        entry = self._det_tickets.get(ticket)
+        if entry is None:                                  # the library's refusal (not in flight)
+            self._check(self.lib.oww_detect_host_collect(self.h, int(ticket), None, None, None, None, None, None, None))
+            raise NativeError(f"detect ticket {ticket} is not in flight")
+        _, cs, (ev, n, clips, ends, chunks, prepared, fin) = entry
+        self._check(self.lib.oww_detect_host_collect(self.h, int(ticket), _ptr(ev), _ptr(n), _ptr(clips), _ptr(ends),
+                                                     _ptr(chunks), _ptr(prepared), _ptr(fin)))
+        del self._det_tickets[ticket]
+        k = min(int(n[0]), ev.size)
+        return (ev[:k], int(n[0]), chunks, prepared, clips[:k] if cs > 0 else None, ends[:k] if cs > 0 else None, fin)
 
     # ---- batch ----
     def embed_clips(self, d_pcm, n_clips, n_samples, d_emb, stream=None):

@@ -21,6 +21,20 @@ int oww_fail(oww_ctx* ctx, int code, const char* fmt, ...) {
     return code;
 }
 
+int oww_order_begin(oww_ctx* ctx, cudaStream_t s) {
+    if (s == ctx->own_stream) return OWW_OK;
+    OWW_CUDA(ctx, cudaEventRecord(ctx->order_ev[0], ctx->own_stream));
+    OWW_CUDA(ctx, cudaStreamWaitEvent(s, ctx->order_ev[0], 0));
+    return OWW_OK;
+}
+
+int oww_order_end(oww_ctx* ctx, cudaStream_t s) {
+    if (s == ctx->own_stream) return OWW_OK;
+    OWW_CUDA(ctx, cudaEventRecord(ctx->order_ev[1], s));
+    OWW_CUDA(ctx, cudaStreamWaitEvent(ctx->own_stream, ctx->order_ev[1], 0));
+    return OWW_OK;
+}
+
 namespace {
 
 const int kLayerTable[OWW_N_CONV][6] = {   // kh kw cin cout pool_t pool_f  (SURVEY.md Appendix B)
@@ -721,10 +735,13 @@ int reset_enqueue(oww_ctx* ctx, const int32_t* h_stream_ids, int n, const float*
     const bool have_init = h_feature_init && n_rows > 0;
     if (have_init)
         OWW_CUDA(ctx, cudaMemcpyAsync(ctx->d_reset_init, h_feature_init, (size_t)n_rows * 96 * sizeof(float), cudaMemcpyHostToDevice, s));
+    // after the host-buffer calls submitted so far, before the later ones (their host counters already see the reset)
+    int rc = oww_order_begin(ctx, s);
+    if (rc) return rc;
     ResetTails rt;
     std::memset(&rt, 0, sizeof(rt));
     if (ctx->cfg.cnn_mode == OWW_CNN_TC_INCREMENTAL) {
-        int rc = next_step_tables(ctx, rt);
+        rc = next_step_tables(ctx, rt);
         if (rc) return rc;
         rt.tmpl = reinterpret_cast<const uint4*>(ctx->d_tails_template);
         for (int i = 0, l = ctx->split_from; i < rt.n_late; ++l)
@@ -735,11 +752,12 @@ int reset_enqueue(oww_ctx* ctx, const int32_t* h_stream_ids, int n, const float*
                                    ctx->d_mel_count, ctx->d_feat_count, ctx->d_mel_ring, ctx->mel_rows, ctx->d_feat_ring,
                                    ctx->feat_rows, have_init ? ctx->d_reset_init : nullptr, n_rows, rt);
     OWW_LAUNCH_CHECK(ctx);
-    int rc = oww_detect_reset(ctx, h_stream_ids ? ctx->d_reset_ids : nullptr, n, s);    // the detector's history of those streams
+    rc = oww_detect_reset(ctx, h_stream_ids ? ctx->d_reset_ids : nullptr, n, s);        // the detector's history of those streams
     if (rc) return rc;
     if ((rc = oww_audio_reset(ctx, h_stream_ids ? ctx->d_reset_ids : nullptr, n, s))) return rc;     // ... and their audio
     oww_ingest_reset(ctx, h_stream_ids, n);               // ... and their staged samples (host counters only)
-    return oww_feat16_resync(ctx, h_stream_ids ? ctx->d_reset_ids : nullptr, n, s);     // fp16 mirror of the rings (heads_grp.cu)
+    if ((rc = oww_feat16_resync(ctx, h_stream_ids ? ctx->d_reset_ids : nullptr, n, s))) return rc;  // fp16 mirror (heads_grp.cu)
+    return oww_order_end(ctx, s);
 }
 
 // Units of a stream record's two conv tails sections (0 outside mode 3).  tail_tab is filled by the reset that
@@ -871,6 +889,7 @@ int oww_create(const oww_config* cfg, oww_ctx** out) {
     ctx->late_pdl = (cfg->reserved[0] & 32) == 0;
     cudaStreamCreateWithFlags(&ctx->own_stream, cudaStreamNonBlocking);
     cudaStreamCreateWithFlags(&ctx->copy_stream, cudaStreamNonBlocking);
+    for (auto& ev : ctx->order_ev) cudaEventCreateWithFlags(&ev, cudaEventDisableTiming);
     fill_layer_table(ctx);
     *out = ctx;
     return OWW_OK;
@@ -902,6 +921,13 @@ void oww_destroy(oww_ctx* ctx) {
         if (S.done) cudaEventDestroy(S.done);
         if (S.h2d_done) cudaEventDestroy(S.h2d_done);
     }
+    for (auto& S : ctx->det_slot) {
+        cudaFreeHost(S.h_pkt); cudaFree(S.d_pkt); cudaFree(S.d_scores); cudaFree(S.d_final); cudaFree(S.d_out);
+        cudaFreeHost(S.h_out);
+        if (S.done) cudaEventDestroy(S.done);
+        if (S.h2d_done) cudaEventDestroy(S.h2d_done);
+    }
+    for (auto e : ctx->order_ev) if (e) cudaEventDestroy(e);
     if (ctx->copy_stream) cudaStreamDestroy(ctx->copy_stream);
     for (auto e : ctx->ev) cudaEventDestroy(e);
     cudaStreamDestroy(ctx->own_stream);
@@ -1289,6 +1315,144 @@ int oww_step_host(oww_ctx* ctx, const int16_t* h_pcm, int64_t pcm_stride, int n_
     int rc = oww_step_host_submit(ctx, h_pcm, pcm_stride, n_chunks, &ticket);
     if (rc) return rc;
     return oww_step_host_collect(ctx, ticket, h_scores);
+}
+
+}  // extern "C"
+
+namespace {
+
+// a slot's buffers for a call of B streams, `samples` packet samples, max_events events of `capture` samples, L labels:
+// each grows (and only grows) when a call needs more than any before it
+int detect_slot_grow(oww_ctx* ctx, oww_ctx::DetectSlot& S, int B, size_t samples, int max_events, int capture, int L) {
+    const size_t scores = (size_t)B * std::max(ctx->n_out_total, 1), fin = (size_t)B * L;
+    const DetectLayout lay = oww_detect_layout(max_events, capture, B, L);
+    if (!S.done) {
+        OWW_CUDA(ctx, cudaEventCreateWithFlags(&S.done, cudaEventDisableTiming));
+        OWW_CUDA(ctx, cudaEventCreateWithFlags(&S.h2d_done, cudaEventDisableTiming));
+    }
+    if (S.pkt_samples < samples) {
+        cudaFreeHost(S.h_pkt); cudaFree(S.d_pkt); S.h_pkt = nullptr; S.d_pkt = nullptr; S.pkt_samples = 0;
+        OWW_CUDA(ctx, cudaMallocHost(&S.h_pkt, samples * sizeof(int16_t)));
+        OWW_CUDA(ctx, cudaMalloc(&S.d_pkt, samples * sizeof(int16_t)));
+        S.pkt_samples = samples;
+    }
+    if (S.scores_floats < scores) {
+        cudaFree(S.d_scores); S.d_scores = nullptr; S.scores_floats = 0;
+        OWW_CUDA(ctx, cudaMalloc(&S.d_scores, scores * sizeof(float)));
+        S.scores_floats = scores;
+    }
+    if (S.final_floats < fin) {
+        cudaFree(S.d_final); S.d_final = nullptr; S.final_floats = 0;
+        OWW_CUDA(ctx, cudaMalloc(&S.d_final, fin * sizeof(float)));
+        S.final_floats = fin;
+    }
+    if (S.d_out_bytes < lay.final) {
+        cudaFree(S.d_out); S.d_out = nullptr; S.d_out_bytes = 0;
+        OWW_CUDA(ctx, cudaMalloc(&S.d_out, lay.final));
+        S.d_out_bytes = lay.final;
+    }
+    if (S.h_out_bytes < lay.bytes) {
+        cudaFreeHost(S.h_out); S.h_out = nullptr; S.h_out_dev = nullptr; S.h_out_bytes = 0;
+        OWW_CUDA(ctx, cudaHostAlloc(&S.h_out, lay.bytes, cudaHostAllocMapped));
+        OWW_CUDA(ctx, cudaHostGetDevicePointer(reinterpret_cast<void**>(&S.h_out_dev), S.h_out, 0));
+        S.h_out_bytes = lay.bytes;
+    }
+    return OWW_OK;
+}
+
+}  // namespace
+
+extern "C" {
+
+int oww_detect_host_submit(oww_ctx* ctx, const int16_t* h_packets, const int64_t* h_offsets, int max_events,
+                           int capture_samples, int want_final, int* ticket) {
+    if (!ctx) return OWW_EINVAL;
+    if (!h_offsets || !ticket) return oww_fail(ctx, OWW_EINVAL, "null argument");
+    OWW_CUDA(ctx, cudaSetDevice(ctx->device));
+    const int si = ctx->det_next;
+    oww_ctx::DetectSlot& S = ctx->det_slot[si];
+    if (S.busy) return oww_fail(ctx, OWW_EINVAL, "two detect tickets are in flight: collect one first");
+    // every refusal before anything is enqueued; the capacities count what earlier submits staged (host counters)
+    int rc = oww_ingest_check(ctx, h_offsets);
+    if (rc) return rc;
+    const int L = oww_detect_n_labels(ctx);
+    if (L == 0) return oww_fail(ctx, OWW_EINVAL, "no detector configured (oww_set_detector, oww_set_streams)");
+    if (max_events < 0) return oww_fail(ctx, OWW_EINVAL, "max_events=%d is negative", max_events);
+    const int H = oww_audio_history_samples(ctx);
+    if (capture_samples < 0 || (capture_samples > 0 && capture_samples > H))
+        return oww_fail(ctx, OWW_EINVAL, H ? "capture_samples=%d outside [0,%d]" : "capture_samples=%d without an audio "
+                        "history (oww_set_audio_history)", capture_samples, H);
+    const int B = ctx->n_streams;
+    const int64_t off0 = h_offsets[0], total = h_offsets[B] - off0;
+    if (total > 0 && !h_packets) return oww_fail(ctx, OWW_EINVAL, "null argument");
+    if ((rc = detect_slot_grow(ctx, S, B, (size_t)std::max<int64_t>(total, 1), max_events, capture_samples, L))) return rc;
+    S.offsets.resize((size_t)B + 1);
+    for (int b = 0; b <= B; ++b) S.offsets[b] = h_offsets[b] - off0;
+    S.chunks.resize(B);
+    S.prepared.resize(B);
+    cudaStream_t s = ctx->own_stream;
+    if (total > 0) {
+        // A dense page-locked span (cudaMallocHost / cudaHostRegister / torch pin_memory) is DMA'd straight from the
+        // caller's buffer, which must stay untouched until the ticket is collected; otherwise it is staged
+        const int16_t* src = h_packets + off0;
+        cudaPointerAttributes a0, a1;
+        const bool pinned = cudaPointerGetAttributes(&a0, src) == cudaSuccess && a0.type == cudaMemoryTypeHost &&
+                            cudaPointerGetAttributes(&a1, src + total - 1) == cudaSuccess && a1.type == cudaMemoryTypeHost;
+        cudaGetLastError();                                 // unregistered host memory reports an error on older drivers
+        if (!pinned) {
+            std::memcpy(S.h_pkt, src, (size_t)total * sizeof(int16_t));
+            src = S.h_pkt;
+        }
+        OWW_CUDA(ctx, cudaMemcpyAsync(S.d_pkt, src, (size_t)total * sizeof(int16_t), cudaMemcpyHostToDevice, ctx->copy_stream));
+        OWW_CUDA(ctx, cudaEventRecord(S.h2d_done, ctx->copy_stream));
+        OWW_CUDA(ctx, cudaStreamWaitEvent(s, S.h2d_done, 0));
+    }
+    uint8_t* d_out = S.d_out;
+    const DetectLayout lay = oww_detect_layout(max_events, capture_samples, B, L);
+    oww_event* d_events = max_events > 0 ? reinterpret_cast<oww_event*>(d_out + lay.events) : nullptr;
+    int32_t* d_n = reinterpret_cast<int32_t*>(d_out);
+    if ((rc = oww_ingest(ctx, S.d_pkt, S.offsets.data(), S.chunks.data(), S.prepared.data(), S.d_scores, s))) return rc;
+    if ((rc = oww_detect(ctx, S.d_scores, 0, S.prepared.data(), want_final ? S.d_final : nullptr, d_events, max_events, d_n, s)))
+        return rc;
+    if (capture_samples > 0 &&
+        (rc = oww_capture_events(ctx, d_events, d_n, max_events, capture_samples, reinterpret_cast<int16_t*>(d_out + lay.clips),
+                                 reinterpret_cast<int64_t*>(d_out + lay.ends), s)))
+        return rc;
+    if ((rc = oww_detect_deliver(ctx, d_out, S.h_out_dev, max_events, capture_samples, s))) return rc;
+    if (want_final)
+        OWW_CUDA(ctx, cudaMemcpyAsync(S.h_out + lay.final, S.d_final, (size_t)B * L * sizeof(float), cudaMemcpyDeviceToHost, s));
+    OWW_CUDA(ctx, cudaEventRecord(S.done, s));
+    S.n_streams = B; S.n_labels = L; S.max_events = max_events; S.capture = capture_samples; S.want_final = want_final != 0;
+    S.seq = ++ctx->det_seq;
+    S.busy = true;
+    ctx->det_next = si ^ 1;
+    *ticket = si;
+    return OWW_OK;
+}
+
+int oww_detect_host_collect(oww_ctx* ctx, int ticket, oww_event* h_events, int32_t* h_n_events, int16_t* h_clips,
+                            int64_t* h_ends, int32_t* h_chunks, int32_t* h_prepared, float* h_final) {
+    if (!ctx) return OWW_EINVAL;
+    if (ticket < 0 || ticket > 1 || !ctx->det_slot[ticket].busy)
+        return oww_fail(ctx, OWW_EINVAL, "detect ticket %d is not in flight", ticket);
+    oww_ctx::DetectSlot& S = ctx->det_slot[ticket];
+    const oww_ctx::DetectSlot& other = ctx->det_slot[ticket ^ 1];
+    if (other.busy && other.seq < S.seq)
+        return oww_fail(ctx, OWW_EINVAL, "detect ticket %d was submitted before ticket %d: collect it first", ticket ^ 1, ticket);
+    OWW_CUDA(ctx, cudaSetDevice(ctx->device));
+    OWW_CUDA(ctx, cudaEventSynchronize(S.done));
+    const DetectLayout lay = oww_detect_layout(S.max_events, S.capture, S.n_streams, S.n_labels);
+    const int n = *reinterpret_cast<const int32_t*>(S.h_out);
+    const size_t k = (size_t)std::min(n, S.max_events);
+    if (h_n_events) *h_n_events = n;
+    if (h_events && k) std::memcpy(h_events, S.h_out + lay.events, k * sizeof(oww_event));
+    if (h_ends && S.capture && k) std::memcpy(h_ends, S.h_out + lay.ends, k * sizeof(int64_t));
+    if (h_clips && S.capture && k) std::memcpy(h_clips, S.h_out + lay.clips, k * S.capture * sizeof(int16_t));
+    if (h_chunks) std::memcpy(h_chunks, S.chunks.data(), (size_t)S.n_streams * sizeof(int32_t));
+    if (h_prepared) std::memcpy(h_prepared, S.prepared.data(), (size_t)S.n_streams * sizeof(int32_t));
+    if (h_final && S.want_final) std::memcpy(h_final, S.h_out + lay.final, (size_t)S.n_streams * S.n_labels * sizeof(float));
+    S.busy = false;
+    return OWW_OK;
 }
 
 int oww_get_features(oww_ctx* ctx, int stream_id, int n, int back, float* h_out) {

@@ -233,6 +233,8 @@ void oww_audio_free_streams(oww_ctx* ctx) { if (ctx->audio) free_stream_state(ct
 
 int oww_audio_alloc_streams(oww_ctx* ctx) { return ctx->audio ? alloc_stream_state(ctx) : OWW_OK; }
 
+int oww_audio_history_samples(const oww_ctx* ctx) { return ctx->audio && ctx->audio->d_audio ? ctx->audio->H : 0; }
+
 int oww_audio_reset(oww_ctx* ctx, const int* d_ids, int n, cudaStream_t s) {
     const oww_audio* a = ctx->audio;
     if (!a || !a->d_audio || n <= 0) return OWW_OK;

@@ -159,6 +159,40 @@ __global__ void __launch_bounds__(DET_THREADS) detect_events_kernel(const float*
     if (f && events && pos < max_events) events[pos] = oww_event{b, j, sc, count[b] - 1};
 }
 
+// The delivery of oww_detect_host_submit: the count, the first k = min(count, max_events) events and, with capture > 0,
+// their ends and clip rows, from the device buffers of the call (oww_detect_layout) into its mapped host buffer, so that
+// PCIe carries only what was found.  CTA 0 writes the count.  Without capture thread t of the grid writes event t; with
+// capture CTA i writes event i, its end and its clip row.  CTAs past the count exit at once, as in audio_capture_kernel.
+__global__ void __launch_bounds__(DET_THREADS) detect_deliver_kernel(const uint8_t* __restrict__ src, uint8_t* __restrict__ dst,
+                                                                     DetectLayout lay, int max_events, int capture) {
+    const int n = *reinterpret_cast<const int*>(src);
+    const int k = min(n, max_events);
+    if (blockIdx.x == 0 && threadIdx.x == 0) *reinterpret_cast<int*>(dst) = n;
+    const uint4* ev = reinterpret_cast<const uint4*>(src + lay.events);     // oww_event: 16 bytes
+    uint4* ev_out = reinterpret_cast<uint4*>(dst + lay.events);
+    if (capture == 0) {
+        const int i = blockIdx.x * DET_THREADS + threadIdx.x;
+        if (i < k) ev_out[i] = ev[i];
+        return;
+    }
+    const int i = blockIdx.x;
+    if (i >= k) return;
+    if (threadIdx.x == 0) {
+        ev_out[i] = ev[i];
+        reinterpret_cast<int64_t*>(dst + lay.ends)[i] = reinterpret_cast<const int64_t*>(src + lay.ends)[i];
+    }
+    const int16_t* row = reinterpret_cast<const int16_t*>(src + lay.clips) + (size_t)i * capture;
+    int16_t* out = reinterpret_cast<int16_t*>(dst + lay.clips) + (size_t)i * capture;
+    int j0 = 0;
+    if (((reinterpret_cast<uintptr_t>(row) | reinterpret_cast<uintptr_t>(out)) & 15) == 0) {   // 8 samples per store
+        const int nv = capture / 8;
+        for (int j = threadIdx.x; j < nv; j += DET_THREADS)
+            reinterpret_cast<uint4*>(out)[j] = reinterpret_cast<const uint4*>(row)[j];
+        j0 = nv * 8;
+    }
+    for (int j = j0 + threadIdx.x; j < capture; j += DET_THREADS) out[j] = row[j];
+}
+
 // streams ids[0..n) (nullptr: stream blockIdx.x) start afresh: an empty history
 __global__ void detect_clear_kernel(const int* ids, int B, int L, float* hist, int* count) {
     const int b = ids ? ids[blockIdx.x] : blockIdx.x;
@@ -407,6 +441,28 @@ int oww_detect_reset(oww_ctx* ctx, const int* d_ids, int n, cudaStream_t s) {
     return OWW_OK;
 }
 
+int oww_detect_n_labels(const oww_ctx* ctx) { return ctx->det && ctx->det->d_hist ? (int)ctx->det->labels.size() : 0; }
+
+DetectLayout oww_detect_layout(int max_events, int capture, int n_streams, int n_labels) {
+    const auto up16 = [](size_t x) { return (x + 15) & ~(size_t)15; };
+    DetectLayout l;
+    const size_t m = (size_t)std::max(max_events, 0);
+    l.events = 16;
+    l.ends = up16(l.events + m * sizeof(oww_event));
+    l.clips = up16(l.ends + (capture > 0 ? m * sizeof(int64_t) : 0));
+    l.final = up16(l.clips + (capture > 0 ? m * (size_t)capture * sizeof(int16_t) : 0));
+    l.bytes = l.final + (size_t)n_streams * n_labels * sizeof(float);
+    return l;
+}
+
+int oww_detect_deliver(oww_ctx* ctx, const uint8_t* d_out, uint8_t* h_out, int max_events, int capture, cudaStream_t s) {
+    const DetectLayout lay = oww_detect_layout(max_events, capture, 0, 0);
+    const int ctas = capture > 0 ? std::max(max_events, 1) : std::max((max_events + DET_THREADS - 1) / DET_THREADS, 1);
+    detect_deliver_kernel<<<ctas, DET_THREADS, 0, s>>>(d_out, h_out, lay, max_events, capture);
+    OWW_LAUNCH_CHECK(ctx);
+    return OWW_OK;
+}
+
 extern "C" {
 
 int oww_set_detector(oww_ctx* ctx, const oww_detect_label* h_labels, int n_labels, double debounce_time) {
@@ -547,10 +603,11 @@ int oww_detector_export(oww_ctx* ctx, const int32_t* h_stream_ids, int n, float*
     int rc = stage_ids(ctx, h_stream_ids, n, false, (cudaStream_t)stream);
     if (rc || n == 0) return rc;
     const oww_detector* d = ctx->det;
+    if ((rc = oww_order_begin(ctx, (cudaStream_t)stream))) return rc;     // between the detect calls submitted around it
     detect_export_kernel<<<n, DET_THREADS, 0, (cudaStream_t)stream>>>(d->d_ids, ctx->n_streams, (int)d->labels.size(), d->d_hist,
                                                                       d->d_count, d_hist, d_counts);
     OWW_LAUNCH_CHECK(ctx);
-    return OWW_OK;
+    return oww_order_end(ctx, (cudaStream_t)stream);
 }
 
 int oww_detector_import(oww_ctx* ctx, const int32_t* h_stream_ids, int n, const float* d_hist, const int32_t* d_counts, void* stream) {
@@ -560,10 +617,11 @@ int oww_detector_import(oww_ctx* ctx, const int32_t* h_stream_ids, int n, const 
     int rc = stage_ids(ctx, h_stream_ids, n, true, (cudaStream_t)stream);
     if (rc || n == 0) return rc;
     const oww_detector* d = ctx->det;
+    if ((rc = oww_order_begin(ctx, (cudaStream_t)stream))) return rc;
     detect_import_kernel<<<n, DET_THREADS, 0, (cudaStream_t)stream>>>(d->d_ids, ctx->n_streams, (int)d->labels.size(), d->d_hist,
                                                                       d->d_count, d_hist, d_counts);
     OWW_LAUNCH_CHECK(ctx);
-    return OWW_OK;
+    return oww_order_end(ctx, (cudaStream_t)stream);
 }
 
 int oww_set_stream_detection(oww_ctx* ctx, const int32_t* h_stream_ids, int n, const oww_stream_detect* h_overrides,
@@ -597,7 +655,10 @@ int oww_set_stream_detection(oww_ctx* ctx, const int32_t* h_stream_ids, int n, c
         for (int j = 0; j < L; ++j) d->ovr[(size_t)b * L + j] = h_overrides ? h_overrides[(size_t)i * L + j] : kNoOverride;
         d->ovr_deb[b] = h_overrides && h_debounce ? h_debounce[i] : NAN;
     }
-    return sync_overrides(ctx, (cudaStream_t)stream);
+    // the table is one device buffer: the upload waits for the detect calls submitted so far, which read the old one,
+    // and those submitted later wait for it
+    if ((rc = oww_order_begin(ctx, (cudaStream_t)stream)) || (rc = sync_overrides(ctx, (cudaStream_t)stream))) return rc;
+    return oww_order_end(ctx, (cudaStream_t)stream);
 }
 
 int oww_get_stream_detection(oww_ctx* ctx, const int32_t* h_stream_ids, int n, oww_stream_detect* h_overrides,

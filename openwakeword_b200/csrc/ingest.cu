@@ -396,6 +396,25 @@ void oww_ingest_reset(oww_ctx* ctx, const int32_t* h_ids, int n) {
     }
 }
 
+int oww_ingest_check(oww_ctx* ctx, const int64_t* h_offsets) {
+    int rc = need_state(ctx);
+    if (rc) return rc;
+    const oww_ingest_state* g = ctx->ingest;
+    if (!h_offsets) return oww_fail(ctx, OWW_EINVAL, "null argument");
+    if (!ctx->mel_loaded || !ctx->emb_loaded) return oww_fail(ctx, OWW_EINVAL, "weights not loaded");
+    if (h_offsets[0] < 0) return oww_fail(ctx, OWW_EINVAL, "offsets[0]=%lld is negative", (long long)h_offsets[0]);
+    for (int b = 0; b < g->n_streams; ++b) {
+        const int64_t n = h_offsets[b + 1] - h_offsets[b];
+        if (n < 0) return oww_fail(ctx, OWW_EINVAL, "offsets decrease at stream %d", b);
+        int64_t n_out, max_in;
+        int c, after;
+        if (!plan(g->rate[b], ctx->cfg.max_chunks, g->S[b], g->staged[b], n, &n_out, &c, &after, &max_in))
+            return oww_fail(ctx, OWW_EINVAL, "stream %d: %lld input samples, its capacity is %lld (oww_ingest_capacity)", b,
+                            (long long)n, (long long)max_in);
+    }
+    return OWW_OK;
+}
+
 extern "C" {
 
 int oww_resampler_taps(int rate, float* h_taps, int max, int* up, int* down) {
@@ -548,10 +567,12 @@ int oww_ingest_export(oww_ctx* ctx, const int32_t* h_stream_ids, int n, int32_t*
     // pageable sources: staged by the driver before the call returns; stream-ordered on the device
     OWW_CUDA(ctx, cudaMemcpyAsync(g->d_ids, h_stream_ids, (size_t)n * sizeof(int), cudaMemcpyHostToDevice, s));
     OWW_CUDA(ctx, cudaMemcpyAsync(g->d_ids + g->n_streams, info.data(), info.size() * sizeof(int), cudaMemcpyHostToDevice, s));
+    // the staged rows as the host counters describe them: after the detect calls submitted so far
+    if ((rc = oww_order_begin(ctx, s))) return rc;
     ingest_export_kernel<<<n, ING_THREADS, 0, s>>>(g->d_ids, g->d_ids + g->n_streams, g->d_stage, g->cap, g->d_hist, d_staged,
                                                    staged_stride, d_hist);
     OWW_LAUNCH_CHECK(ctx);
-    return OWW_OK;
+    return oww_order_end(ctx, s);
 }
 
 int oww_ingest_import(oww_ctx* ctx, const int32_t* h_stream_ids, int n, const int32_t* h_rates, const int64_t* h_consumed,
@@ -576,9 +597,11 @@ int oww_ingest_import(oww_ctx* ctx, const int32_t* h_stream_ids, int n, const in
     cudaStream_t s = (cudaStream_t)stream;
     OWW_CUDA(ctx, cudaMemcpyAsync(g->d_ids, h_stream_ids, (size_t)n * sizeof(int), cudaMemcpyHostToDevice, s));
     OWW_CUDA(ctx, cudaMemcpyAsync(g->d_ids + g->n_streams, info.data(), info.size() * sizeof(int), cudaMemcpyHostToDevice, s));
+    if ((rc = oww_order_begin(ctx, s))) return rc;
     ingest_import_kernel<<<n, ING_THREADS, 0, s>>>(g->d_ids, g->d_ids + g->n_streams, g->d_stage, g->cap, g->d_hist, d_staged,
                                                    staged_stride, d_hist);
     OWW_LAUNCH_CHECK(ctx);
+    if ((rc = oww_order_end(ctx, s))) return rc;
     for (int i = 0; i < n; ++i) {
         const int b = h_stream_ids[i];
         g->rate[b] = h_rates[i]; g->S[b] = h_consumed[i]; g->staged[b] = h_staged[i]; g->staged_off[b] = 0;

@@ -294,6 +294,26 @@ struct oww_ctx {
     } slot[2];
     int next_slot = 0;
     std::vector<int32_t> slot_chunks[2];   // per host slot: the ragged counts of its step (empty: every row stepped)
+    // orders a call enqueued on the caller's stream with the host-buffer calls on own_stream (oww_order_begin / _end)
+    cudaEvent_t order_ev[2] = {nullptr, nullptr};
+
+    // host staging of oww_detect_host_submit / _collect: two slots, like the step's.  Each keeps its ticket's device
+    // buffers, the delivery buffer the device writes through a mapped pointer, and what the collect hands out.
+    struct DetectSlot {
+        int16_t* h_pkt = nullptr; int16_t* d_pkt = nullptr; size_t pkt_samples = 0;   // pinned staging | device packets
+        float* d_scores = nullptr; size_t scores_floats = 0;                           // [B][n_out]
+        float* d_final = nullptr; size_t final_floats = 0;                             // [B][n_labels]
+        uint8_t* d_out = nullptr; size_t d_out_bytes = 0;            // count | events | ends | clips (oww_detect_layout)
+        uint8_t* h_out = nullptr; uint8_t* h_out_dev = nullptr; size_t h_out_bytes = 0;   // mapped: the same | final
+        std::vector<int64_t> offsets;                                // the call's offsets, rebased to the staged span
+        std::vector<int32_t> chunks, prepared;                       // oww_ingest's, filled at submit
+        int n_streams = 0, n_labels = 0, max_events = 0, capture = 0, want_final = 0;
+        uint64_t seq = 0;                                            // submission order
+        cudaEvent_t h2d_done = nullptr, done = nullptr;
+        bool busy = false;
+    } det_slot[2];
+    int det_next = 0;
+    uint64_t det_seq = 0;
 
     // ragged steps (oww_step_ragged): per call [B counts | B stream ids ordered by count], staged through a ring of
     // pinned buffers (a slot is reused once the copy of the call kRagSlots calls back has run)
@@ -331,6 +351,11 @@ struct oww_ctx {
 };
 
 int oww_fail(oww_ctx* ctx, int code, const char* fmt, ...);
+// api.cu: a call enqueued on `s` that reads or writes state the host-buffer calls use on the handle's own stream runs
+// after everything submitted there so far (begin, before its first device work) and before everything submitted later
+// (end, after its last).  Both do nothing when s is the own stream.
+int oww_order_begin(oww_ctx* ctx, cudaStream_t s);
+int oww_order_end(oww_ctx* ctx, cudaStream_t s);
 void oww_verifier_fit_free(oww_ctx* ctx);          // verifier_fit.cu: the training scratch
 void oww_mix_free(oww_ctx* ctx);                   // mix.cu: the mixer's tables and scratch
 // 64-bit FNV-1a of `bytes` bytes, continuing from h (the stream record's configuration key)
@@ -543,6 +568,15 @@ void oww_detect_free_streams(oww_ctx* ctx);
 int oww_detect_alloc_streams(oww_ctx* ctx);      // for ctx->n_streams streams, every history empty; the device is idle
 // the listed streams (d_ids == nullptr: streams 0..n-1) start afresh: one launch on `s`
 int oww_detect_reset(oww_ctx* ctx, const int* d_ids, int n, cudaStream_t s);
+int oww_detect_n_labels(const oww_ctx* ctx);      // labels of the detector; 0 without one (or without streams)
+// Byte offsets of one delivery buffer of oww_detect_host_submit for max_events events of `capture` samples: the count
+// (int32) at 0, then events, ends and clip rows, each on a 16-byte boundary; `final` is where a host buffer keeps the
+// final predictions, `bytes` its size.  A device buffer ends at `final`.
+struct DetectLayout { size_t events, ends, clips, final, bytes; };
+DetectLayout oww_detect_layout(int max_events, int capture, int n_streams, int n_labels);
+// one launch on `s`: the count d_out (layout above) holds, the first min(count, max_events) events and with capture > 0
+// their ends and clip rows -> the same places of h_out (a device pointer to mapped host memory)
+int oww_detect_deliver(oww_ctx* ctx, const uint8_t* d_out, uint8_t* h_out, int max_events, int capture, cudaStream_t s);
 
 // ---- audio.cu: the streams' recent audio (nothing happens on a handle without history) ----
 void oww_audio_free(oww_ctx* ctx);
@@ -550,6 +584,7 @@ void oww_audio_free_streams(oww_ctx* ctx);
 int oww_audio_alloc_streams(oww_ctx* ctx);       // for ctx->n_streams streams, every history empty; the device is idle
 // the listed streams (d_ids == nullptr: streams 0..n-1) start with an empty history: one launch on `s`
 int oww_audio_reset(oww_ctx* ctx, const int* d_ids, int n, cudaStream_t s);
+int oww_audio_history_samples(const oww_ctx* ctx);   // H; 0 without history (or without streams)
 // one launch on `s`: stream b appends the first cnt * 1280 samples of its row, cnt = d_counts[b] (device; nullptr:
 // n_chunks for every stream)
 int oww_audio_append(oww_ctx* ctx, const int16_t* d_pcm, int64_t pcm_stride, int n_chunks, const int* d_counts,
@@ -561,6 +596,9 @@ void oww_ingest_free_streams(oww_ctx* ctx);
 int oww_ingest_alloc_streams(oww_ctx* ctx);      // for ctx->n_streams streams, every one at 16000, nothing staged
 // the listed streams (h_ids == nullptr: streams 0..n-1) drop their staged samples and history: host state only
 void oww_ingest_reset(oww_ctx* ctx, const int32_t* h_ids, int n);
+// what oww_ingest refuses before it enqueues anything (no ingest state, weights, offsets, a packet over its stream's
+// capacity), checked without enqueueing
+int oww_ingest_check(oww_ctx* ctx, const int64_t* h_offsets);
 
 // ---- verifier.cu: custom verifier banks ----
 // every bank of the handle on n rows of final scores (one launch; nothing when the handle has no bank).  The window of

@@ -188,6 +188,44 @@ class StreamEngine:
             self.ctx._cuda("out", out, torch.float32, (self.n_streams, self.n_cols))
         return self.ctx.ingest(d_packets, off, out, torch.cuda.current_stream(dev).cuda_stream)
 
+    # ---- pipelined detection from host audio (include/owwb200.h, oww_detect_host_submit) ----
+    def submit_detect(self, packets, offsets, max_events=None, capture=None, final=False):
+        """Every stream's new packet from host memory, ingested and detected on the device without waiting for it: what
+        ``ingest`` then ``detect`` (with ``capture``: the last `capture` samples of each event's stream, as
+        ``detect(capture=...)``) give, delivered to host memory.  packets: a contiguous 1-D int16 NumPy array, stream b's
+        packet packets[offsets[b]:offsets[b+1]] at its own rate (set_input_rates; needs a detector, and with capture an
+        audio history).  A page-locked array (e.g. torch.empty(n, dtype=torch.int16).pin_memory().numpy()) is copied
+        straight from, so it must not change before the collect; any other is staged before the call returns.
+        max_events None: n_streams * n_labels, which never truncates (with capture it must be given: the clips are
+        buffered for max_events events).  -> a ticket; at most two are in flight.  Calls made between two submits
+        (settings, resets, exports, imports) apply to the later one.
+        Typical serving loop, the next call's copy overlapping the device work of the one before:
+            pending = []
+            for packets, offsets in source:
+                pending.append(eng.submit_detect(packets, offsets, max_events=64, capture=16000))
+                if len(pending) == 2:
+                    events, n, chunks, prepared, clips, ends = eng.collect_detect(pending.pop(0))
+            while pending:
+                events, n, chunks, prepared, clips, ends = eng.collect_detect(pending.pop(0))"""
+        if max_events is None:
+            if capture:
+                raise ValueError("submit_detect with capture needs max_events (the clip buffers hold that many events)")
+            max_events = self.n_streams * self.ctx.n_detect_labels
+        return self.ctx.detect_host_submit(packets, offsets, int(max_events), capture, bool(final))
+
+    def collect_detect(self, ticket):
+        """Waits for a ticket of ``submit_detect`` (collect them in submission order) -> (events, n, chunks, prepared):
+        the first min(n, max_events) of the n events (_native.EVENT_DTYPE, ascending by stream then label), and the chunks
+        and prepared samples of the ingest, int32 [n_streams]; with capture + (clips int16 [events, capture], ends int64
+        [events]: each clip's end, its stream's position); with final + (float32 [n_streams, n_labels] predictions,)."""
+        events, n, chunks, prepared, clips, ends, fin = self.ctx.detect_host_collect(ticket)
+        out = (events, n, chunks, prepared)
+        if clips is not None:
+            out += (clips, ends)
+        if fin is not None:
+            out += (fin,)
+        return out
+
     # ---- detections on the device (include/owwb200.h, oww_set_detector) ----
     def set_detector(self, labels, threshold, patience={}, debounce_time=0.0):
         """Configure the detector.  labels: one (column, repeats) per label - the score column it reads (-1: always 0.0)
